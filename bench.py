@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """bench.py -- MPFA + MPSA interaction-region assembly throughput (3-D cells/s) and SpMV GB/s.
 
-    python bench.py --gpus N --steps K --warmup W [--impl reference] [--workload NAME]
+    python bench.py --gpus N --steps K --warmup W [--impl reference] [--workload NAME] [--dump-outputs DIR]
 
 One "step" = one full MPFA assembly (all six matrices) + one full MPSA assembly (all four matrices) of the
 workload grid, inputs resident in HBM.  ``value`` = cells of the WHOLE mesh / device time (CUDA events on the
@@ -21,8 +21,14 @@ discretization matrices and the two system matrices stay in HBM behind scipy-com
 (``porepy_b200.sparse.LazyCsr``); ``e2e.variants`` also reports the same call with the two system matrices, and
 with all ten matrices, fetched to the host.
 
-``--impl reference`` times the UNMODIFIED reference (``pp.Mpfa.discretize`` + ``pp.Mpsa.discretize``, loaded from
-/root/reference or oracle/_ref) on the host cores, on a bounded sample of the same kind of mesh.
+``--impl reference`` times the UNMODIFIED reference (``pp.Mpfa.discretize`` + ``pp.Mpsa.discretize``, loaded by
+oracle/ref_loader.py) on the host cores, on a bounded sample of the same kind of mesh.
+
+``--dump-outputs DIR`` (one GPU) writes, after the timed steps, what the last timed step assembled: for each of the ten
+discretization matrices ``DIR/<name>.npy``, float64 of shape (k, 3) -- (row, column, value) of every entry of DUMP_ROWS
+rows drawn with a fixed seed from the matrix's row count, sorted by row and column, so the dump does not depend on how a
+build orders its value arrays -- and ``DIR/<name>_sum_sumsq.npy`` (sum and sum of squares of all its values).  The
+inputs depend only on the arguments, so two builds can be compared output for output.
 """
 from __future__ import annotations
 
@@ -54,6 +60,14 @@ WORKLOADS = {
     "cart512": ("cart", (8, 8, 8), "tooling: 512 hexes (compute-sanitizer runs)"),
 }
 CPU_SAMPLE = {"tet": (8, 8, 8), "cart": (20, 20, 20)}   # 3,072 tets / 8,000 hexes: 10-20 s of reference time
+DUMP_ROWS = 2000          # rows per matrix in --dump-outputs
+DUMP_MAX_ENTRIES = 250_000   # entries per matrix (24 B each): 10 x 6 MB, under 64 MB in all
+# the MPFA and MPSA matrices one step assembles: plan output key (PB_OUT_*, include/poreb200.h), pattern, block rows,
+# block columns (as DevicePlan.mpfa_lazy / mpsa_lazy; nd = 3)
+OUTPUTS = {"flux": (0, 0, 1, 1), "bound_flux": (1, 1, 1, 1), "bound_pressure_cell": (2, 0, 1, 1),
+           "bound_pressure_face": (3, 1, 1, 1), "vector_source": (4, 0, 1, 3), "bound_pressure_vector_source": (5, 0, 1, 3),
+           "stress": (6, 0, 3, 3), "bound_stress": (7, 1, 3, 3), "bound_displacement_cell": (8, 0, 3, 3),
+           "bound_displacement_face": (9, 1, 3, 3)}
 
 
 def make_grid(kind, dims, seed=0):
@@ -127,7 +141,7 @@ def measured_peak_hbm():
     try:
         return float(json.load(open(p))["hbm_gbs"]), "measured (MEASURED_PEAKS.json)"
     except Exception:
-        return 6650.0, "fallback (B200_PROFILING.md)"
+        return 3350.0, "H100 SXM data sheet (HBM3), not measured"
 
 
 def gj_flops(nsf_unknowns, nrhs):
@@ -376,6 +390,27 @@ def md_network_block(kind, dims, solve=True, newton=True):
     return out
 
 
+def dump_outputs(plan, out_dir, seed=0):
+    """The ten matrices of the plan's last assembly step (see ``--dump-outputs``); moves them out of the plan."""
+    os.makedirs(out_dir, exist_ok=True)
+    for name, (key, which, br, bc) in OUTPUTS.items():
+        vals = plan.take(key)
+        np.save(os.path.join(out_dir, f"{name}_sum_sumsq.npy"), np.array(vals.checksum(), dtype=np.float64))
+        data = vals.download()
+        ip, ix = plan.pattern(which, br, bc)
+        nrows = ip.size - 1
+        rows = np.sort(np.random.default_rng(seed + key).choice(nrows, size=min(nrows, DUMP_ROWS), replace=False))
+        lens = (ip[rows + 1] - ip[rows]).astype(np.int64)
+        keep = int(np.searchsorted(np.cumsum(lens), DUMP_MAX_ENTRIES, side="right"))
+        rows, lens = rows[:keep], lens[:keep]
+        pos = np.repeat(ip[rows].astype(np.int64) - np.cumsum(lens) + lens, lens) + np.arange(int(lens.sum()))
+        r, c = np.repeat(rows, lens), np.asarray(ix[pos], dtype=np.int64)
+        order = np.lexsort((c, r))
+        out = np.stack([r[order], c[order], np.asarray(data[pos])[order]], axis=1).astype(np.float64)
+        np.save(os.path.join(out_dir, f"{name}.npy"), out)
+        del vals, data
+
+
 def pinned_copy(a):
     """Page-locked copy of a host array (the e2e inputs are read by H2D copies at full PCIe rate)."""
     from porepy_b200 import _lib
@@ -414,7 +449,15 @@ def main():
     ap.add_argument("--no-krylov", action="store_true")
     ap.add_argument("--no-mech-solve", action="store_true", help="skip the block-Jacobi solve of the mechanics system")
     ap.add_argument("--no-md-network", action="store_true", help="skip the mixed-dimensional fracture-network extra (N = 1)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write what the last timed step assembled to DIR/<name>.npy (one GPU)")
     args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be at least 1")
+    if args.dump_outputs and args.impl == "reference":
+        ap.error("--dump-outputs dumps the GPU path's matrices; --impl reference has none")
+    if args.dump_outputs and (args.gpus > 1 or int(os.environ.get("WORLD_SIZE", "1")) > 1):
+        ap.error("--dump-outputs needs one GPU (a shard's matrices are in the shard's own numbering)")
     rank = int(os.environ.get("RANK", "0"))
     world = int(os.environ.get("WORLD_SIZE", "1"))
     local = int(os.environ.get("LOCAL_RANK", "0"))
@@ -528,6 +571,8 @@ def main():
     ms_per_step = dev_ms / args.steps
     value = nc_global / (ms_per_step * 1e-3)
     sz = plan.sizes()
+    if args.dump_outputs:
+        dump_outputs(plan, args.dump_outputs)
     regions_all = allsum([float((shard.own_node.sum() if shard is not None else g.num_nodes))])[0]
     cells_all = allsum([float(nc)])[0]
     del plan
@@ -767,14 +812,17 @@ def main():
     fl_dom = fl_mpsa if dom == "mpsa" else fl_mpfa
     import ctypes
     fp64_peak = {}
-    for kind_id, nm in ((0, "dmma_tflops"), (1, "dfma_tflops")):
+    for kind_id, nm in ((0, "dmma_m8n8k4_tflops"), (1, "dfma_tflops"), (2, "dmma_m16n8k4_tflops"),
+                        (3, "dmma_m16n8k8_tflops"), (4, "dmma_m16n8k16_tflops")):
         v = ctypes.c_double()
         _lib.check(lib.pb_fp64_peak(kind_id, ctypes.byref(v)))
         fp64_peak[nm] = v.value
-    fp64_peak["how"] = "dependency-free register loops, 148 SMs x 8 CTAs x 256 threads, best of 5 (csrc/peaks.cu)"
-    traffic = None
+    fp64_peak["dmma_tflops"] = max(v for k, v in fp64_peak.items() if k.startswith("dmma_"))
+    fp64_peak["how"] = (f"dependency-free register loops, {torch.cuda.get_device_properties(local).multi_processor_count} "
+                        "SMs x 8 CTAs x 256 threads, best of 5 (csrc/peaks.cu); dmma_tflops: the best mma.sync .f64 shape")
+    traffic = None     # DRAM bytes of one launch of the dominant kernel from an ncu capture (tools/traffic_json.py)
     try:
-        tj = json.load(open(os.path.join(ROOT, "profiles", "r02_traffic.json"))).get(args.workload)
+        tj = json.load(open(os.path.join(ROOT, "profiles", "traffic.json"))).get(args.workload)
         if tj and dom in tj["kernel"] and world == 1:
             traffic = int(tj["dram_bytes_read"] + tj["dram_bytes_write"])
     except Exception:
@@ -791,7 +839,8 @@ def main():
         "fp64_frac_of_measured_dmma": (fl_dom / (dom_ms * 1e-3) / 1e12 / fp64_peak["dmma_tflops"])
         if fp64_peak.get("dmma_tflops") else None,
         "fp64_note": "Gauss-Jordan flops of the reduced local systems (from the plan's per-node sizes) over the "
-                     "kernel time, against the DMMA / DFMA register-loop peaks measured in this run (pb_fp64_peak)",
+                     "kernel time, against the best FP64 tensor-core (DMMA) shape's register-loop peak measured in this "
+                     "run (pb_fp64_peak)",
         "fp64_flops_per_launch_gauss_jordan": fl_dom,
     }
     # ---- SpMV on the assembled Jacobians (HBM-bound): flow (scalar) and mechanics (3 x 3 blocks)
@@ -823,7 +872,7 @@ def main():
         "higher_is_better": True, "scaling": "strong", "vs_baseline": None, "dtype": "f64",
         "data": "synthetic",
         "config": {"workload": desc, "cells": int(nc_global), "outputs": "all six MPFA + all four MPSA matrices",
-                   "l2": "inputs+outputs per step exceed the 126 MB L2 (no explicit flush)" if nc > 200000
+                   "l2": "inputs+outputs per step exceed the 50 MB L2 (no explicit flush)" if nc > 200000
                    else "small shard/workload: outputs of one step may fit L2",
                    "parallelism": ("single GPU" if world == 1 else
                                    f"one mesh, recursive coordinate bisection into {world} shards, node ownership + "

@@ -1,4 +1,4 @@
-/* poreb200.h -- C ABI of libporeb200.so: B200 (sm_100a) MPFA / MPSA / Biot
+/* poreb200.h -- C ABI of libporeb200.so: H100 (sm_90a) MPFA / MPSA / Biot
  * interaction-region assembly and CSR SpMV behind PorePy's discretization API.
  *
  * Plain pointers and sizes only; no torch / numpy types.  The Python host side
@@ -68,8 +68,9 @@ int64_t pb_launch_count(void);
 /* Return the device blocks cached by the library's size-keyed pool (see csrc/plan.hpp: DevPool) to the driver. */
 void pb_device_pool_trim(void);
 
-/* FP64 peak of this device, measured by a dependency-free register loop: kind 0 = DMMA (mma.sync.m8n8k4.f64, the
- * pipe of the block Gauss-Jordan), kind 1 = scalar DFMA.  TFLOP/s, best of 5 launches (roofline denominator). */
+/* FP64 peak of this device, measured by a dependency-free register loop: kind 0 = DMMA mma.sync.m8n8k4.f64,
+ * 1 = scalar DFMA, 2 / 3 / 4 = DMMA mma.sync.m16n8k4 / m16n8k8 / m16n8k16 .f64.  TFLOP/s, best of 5 launches
+ * (roofline denominator). */
 int pb_fp64_peak(int kind, double *tflops);
 
 /* Page-locked host buffers for the CSR value arrays the *_download calls fill (full PCIe rate;

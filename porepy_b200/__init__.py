@@ -1,4 +1,4 @@
-"""porepy_b200 -- B200 (sm_100a) MPFA / MPSA / Biot interaction-region assembly and CSR
+"""porepy_b200 -- H100 (sm_90a) MPFA / MPSA / Biot interaction-region assembly and CSR
 SpMV behind PorePy's ``Discretization.discretize() / assemble_matrix_rhs()`` operator API.
 
 The CUDA library (``libporeb200.so``, built in-tree by ``porepy_b200.build``) is loaded on

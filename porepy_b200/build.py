@@ -1,4 +1,4 @@
-"""Build libporeb200.so in-tree with nvcc for sm_100a (cross-compiles without a GPU)."""
+"""Build libporeb200.so in-tree with nvcc for sm_90a (H100; cross-compiles without a GPU)."""
 from __future__ import annotations
 
 import os
@@ -9,7 +9,8 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libporeb200.so")
 SOURCES = ["api.cu", "spmv.cu", "mpfa_launch.cu", "mpsa2d.cu", "mpsa3d.cu", "face.cu", "peaks.cu", "krylov.cu", "sparse_ops.cu", "plan_device.cu", "shard.cu", "geometry.cu"]
-NVCC_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17",
+GENCODE = ["-gencode", "arch=compute_90a,code=sm_90a"]
+NVCC_FLAGS = [*GENCODE, "-lineinfo", "-O3", "-std=c++17",
               "-Xcompiler", "-fPIC", "-Xcompiler", "-O3", "-Xcompiler", "-fopenmp"]
 
 
@@ -26,6 +27,7 @@ def needs_build() -> bool:
     t = os.path.getmtime(LIB)
     deps = [os.path.join(CSRC, f) for f in os.listdir(CSRC)]
     deps.append(os.path.join(os.path.dirname(HERE), "include", "poreb200.h"))
+    deps.append(os.path.abspath(__file__))   # compiler flags and target architecture
     return any(os.path.getmtime(d) > t for d in deps)
 
 
@@ -53,8 +55,8 @@ def build(force: bool = False, verbose: bool = False, extra_flags=(), lib: str =
         if proc.returncode:
             raise subprocess.CalledProcessError(proc.returncode, cmd)
         objs.append(obj)
-    subprocess.check_call([_nvcc(), "-shared", "-o", lib, *objs, "-gencode",
-                           "arch=compute_100a,code=sm_100a", "-Xcompiler", "-fopenmp", "-lgomp"])
+    subprocess.check_call([_nvcc(), "-shared", "-o", lib, *objs, *GENCODE,
+                           "-Xcompiler", "-fopenmp", "-lgomp"])
     return lib
 
 

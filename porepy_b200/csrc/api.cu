@@ -1,5 +1,5 @@
 // api.cu -- C ABI of libporeb200.so (see include/poreb200.h), device memory management and
-// kernel launches.  sm_100a only; there is no CPU path in this library: every compute entry
+// kernel launches.  sm_90a (H100) only; there is no CPU path in this library: every compute entry
 // point needs a CUDA device and fails with PB_ECUDA otherwise.
 #include <cuda_runtime.h>
 
@@ -150,7 +150,8 @@ static int build_classes(pb_plan *p, std::vector<NodeClass> &out, F size_of) {
         // Launch order = a space-filling (Morton) order of the node coordinates when the geometry is known: the <= m_f
         // nodes of a face are then processed close in time, so the scatter-adds into one face row meet in L2 instead
         // of each paying a DRAM read-modify-write (index order puts the neighbours in the 2nd / 3rd grid direction
-        // thousands of regions apart; ncu: 2.9x the algorithmic DRAM traffic).  POREB200_NODE_ORDER=index disables it.
+        // thousands of regions apart, so that the DRAM traffic grows well above the algorithmic bytes).
+        // POREB200_NODE_ORDER=index disables it.
         if (!p->node_key.empty()) {
             const std::vector<uint32_t> &nk = p->node_key;
             std::stable_sort(lists[key].begin(), lists[key].end(), [&](int32_t x, int32_t y) { return nk[x] < nk[y]; });
@@ -371,7 +372,7 @@ extern "C" int pb_plan_create(int nd, int64_t nc, int64_t nf, int64_t nn, const 
             if ((e = counts.ensure((size_t)(j.nrows + 1) * sizeof(int32_t))) != cudaSuccess) return bail("counts", e);
             if ((e = j.ip->ensure((size_t)(j.nrows + 1) * sizeof(int32_t))) != cudaSuccess) return bail("indptr", e);
             const int block = 256;
-            int grid = (int)std::max<int64_t>(1, std::min<int64_t>((j.nrows + 7) / 8, (int64_t)kSMs * 8));
+            int grid = (int)std::max<int64_t>(1, std::min<int64_t>((j.nrows + 7) / 8, (int64_t)pb_sm_count() * 8));
             pattern_kernel<256><<<grid, block, 0, st>>>(j.nrows, j.rnp->as<int32_t>(), j.rn->as<int32_t>(),
                                                         j.cp->as<int32_t>(), j.ci->as<int32_t>(),
                                                         counts.as<int32_t>(), nullptr, nullptr, 0, flag.as<int>());
@@ -429,7 +430,7 @@ extern "C" int pb_plan_create(int nd, int64_t nc, int64_t nf, int64_t nn, const 
                 return bail("pos map", e);
             const int block = 256;
             int64_t need = (nn * 32 + block - 1) / block;
-            int grid = (int)std::max<int64_t>(1, std::min<int64_t>(need, (int64_t)kSMs * 16));
+            int grid = (int)std::max<int64_t>(1, std::min<int64_t>(need, (int64_t)pb_sm_count() * 16));
             posmap_kernel<<<grid, block, 0, st>>>(nn, j.rp->as<int32_t>(), j.re->as<int32_t>(),
                                                   j.cp->as<int32_t>(), j.ce->as<int32_t>(),
                                                   j.ip->as<int32_t>(), p->pat_idx[j.pat].as<int32_t>(),
@@ -556,7 +557,7 @@ extern "C" int pb_plan_pattern_expanded(pb_plan *p, int which, int br, int bc, i
     CUDA_TRY(nix.ensure((nnz ? nnz : 1) * sizeof(int32_t)));
     const int block = 256;
     int64_t need = (c.nrows * 32 + block - 1) / block;
-    int grid = (int)std::max<int64_t>(1, std::min<int64_t>(need, (int64_t)kSMs * 16));
+    int grid = (int)std::max<int64_t>(1, std::min<int64_t>(need, (int64_t)pb_sm_count() * 16));
     expand_pattern_kernel<<<grid, block, 0, st>>>(c.nrows, bip->as<int32_t>(), dix.as<int32_t>(), br, bc,
                                                   nip.as<int32_t>(), nix.as<int32_t>());
     g_launches++;
@@ -582,7 +583,7 @@ int pb_upload_repacked_(cudaStream_t st, DevBuf &tmp, DevBuf &dst, const double 
     CUDA_TRY(tmp.upload(host, (size_t)ncomp * n, st));
     CUDA_TRY(dst.ensure((size_t)ncomp * n * sizeof(double)));
     const int64_t total = (int64_t)ncomp * n;
-    int grid = (int)std::max<int64_t>(1, std::min<int64_t>((total + 255) / 256, (int64_t)kSMs * 32));
+    int grid = (int)std::max<int64_t>(1, std::min<int64_t>((total + 255) / 256, (int64_t)pb_sm_count() * 32));
     repack_kernel<<<grid, 256, 0, st>>>(tmp.as<double>(), dst.as<double>(), ncomp, n);
     g_launches++;
     CUDA_TRY(cudaGetLastError());
@@ -614,7 +615,7 @@ static int upload_cell_tensor(pb_plan *p, DevBuf &dst, const double *host, int n
     CUDA_TRY(p->repack_tmp.upload(host, (size_t)ncomp * p->cell_map_src, st));
     CUDA_TRY(dst.ensure((size_t)ncomp * n * sizeof(double)));
     const int64_t total = (int64_t)ncomp * n;
-    int grid = (int)std::max<int64_t>(1, std::min<int64_t>((total + 255) / 256, (int64_t)kSMs * 32));
+    int grid = (int)std::max<int64_t>(1, std::min<int64_t>((total + 255) / 256, (int64_t)pb_sm_count() * 32));
     repack_gather_kernel<<<grid, 256, 0, st>>>(p->repack_tmp.as<double>(), dst.as<double>(), ncomp, n, p->cell_map_src,
                                                p->cell_map.as<int64_t>());
     g_launches++;
@@ -858,7 +859,7 @@ int pb_checksum_dev_(const double *v, int64_t n, double *sum, double *sumsq) {
     DevBuf o;
     CUDA_TRY(o.ensure(16));
     CUDA_TRY(cudaMemset(o.p, 0, 16));
-    const int grid = (int)std::max<int64_t>(1, std::min<int64_t>((n + 255) / 256, (int64_t)kSMs * 8));
+    const int grid = (int)std::max<int64_t>(1, std::min<int64_t>((n + 255) / 256, (int64_t)pb_sm_count() * 8));
     values_checksum_kernel<<<grid, 256>>>(n, v, o.as<double>());
     g_launches++;
     double h[2];
@@ -962,7 +963,7 @@ extern "C" int pb_plan_output_csr(pb_plan *p, const pb_values *v, int which, int
     if (rc) return rc;
     DevBuf *bip = which == 0 ? &p->fc_indptr : which == 1 ? &p->fb_indptr : which == 2 ? &p->cc_indptr : &p->cb_indptr;
     const int block = 256;
-    int grid = (int)std::max<int64_t>(1, std::min<int64_t>((nrows * 32 + block - 1) / block, (int64_t)kSMs * 16));
+    int grid = (int)std::max<int64_t>(1, std::min<int64_t>((nrows * 32 + block - 1) / block, (int64_t)pb_sm_count() * 16));
     expand_pattern_kernel<<<grid, block, 0, p->stream>>>(nrows, bip->as<int32_t>(), p->pat_idx[which].as<int32_t>(), br, bc,
                                                          pb_csr_indptr_(a), pb_csr_indices_(a));
     g_launches++;
@@ -988,7 +989,7 @@ extern "C" int pb_mpfa_system(pb_plan *p, const pb_values *flux, pb_csr **out) {
                                      p->pat_idx[2].as<int32_t>(), &a);
     if (rc) return rc;
     const int block = 256;
-    int grid = (int)std::max<int64_t>(1, std::min<int64_t>((H.nf * 32 + block - 1) / block, (int64_t)kSMs * 16));
+    int grid = (int)std::max<int64_t>(1, std::min<int64_t>((H.nf * 32 + block - 1) / block, (int64_t)pb_sm_count() * 16));
     div_flux_kernel<<<grid, block, 0, p->stream>>>(H.nf, p->fc_indptr.as<int32_t>(), p->pat_idx[0].as<int32_t>(),
                                                    flux_dev, p->face_cells.as<int32_t>(),
                                                    p->cc_indptr.as<int32_t>(), p->pat_idx[2].as<int32_t>(),
@@ -1022,7 +1023,7 @@ extern "C" int pb_mpfa_rhs(pb_plan *p, const pb_values *bound_flux, const pb_val
     CUDA_TRY(cudaMemsetAsync(w.p, 0, (size_t)H.nf * sizeof(double), st));
     CUDA_TRY(cudaMemsetAsync(r.p, 0, (size_t)H.nc * sizeof(double), st));
     const int block = 256;
-    int grid = (int)std::max<int64_t>(1, std::min<int64_t>((H.nf * 32 + block - 1) / block, (int64_t)kSMs * 16));
+    int grid = (int)std::max<int64_t>(1, std::min<int64_t>((H.nf * 32 + block - 1) / block, (int64_t)pb_sm_count() * 16));
     face_row_dot_kernel<<<grid, block, 0, st>>>(H.nf, p->fb_indptr.as<int32_t>(), p->pat_idx[1].as<int32_t>(),
                                                 bflux_dev, 1, bc.as<double>(), w.as<double>());
     g_launches++;
@@ -1032,7 +1033,7 @@ extern "C" int pb_mpfa_rhs(pb_plan *p, const pb_values *bound_flux, const pb_val
                                                     vs_dev, H.nd, vs.as<double>(), w.as<double>());
         g_launches++;
     }
-    int grid2 = (int)std::max<int64_t>(1, std::min<int64_t>((H.nf + block - 1) / block, (int64_t)kSMs * 16));
+    int grid2 = (int)std::max<int64_t>(1, std::min<int64_t>((H.nf + block - 1) / block, (int64_t)pb_sm_count() * 16));
     neg_div_kernel<<<grid2, block, 0, st>>>(H.nf, p->face_cells.as<int32_t>(), w.as<double>(), r.as<double>());
     g_launches++;
     CUDA_TRY(cudaGetLastError());
@@ -1177,7 +1178,7 @@ extern "C" int pb_mpsa_system(pb_plan *p, const pb_values *stress, pb_csr **out)
     CUDA_TRY(nip.ensure((size_t)(H.nc * nd + 1) * sizeof(int32_t)));
     CUDA_TRY(nix.ensure((size_t)std::max<int64_t>(1, p->pat_nnz[2] * nd2) * sizeof(int32_t)));
     const int block = 256;
-    int grid = (int)std::max<int64_t>(1, std::min<int64_t>((H.nc * 32 + block - 1) / block, (int64_t)kSMs * 16));
+    int grid = (int)std::max<int64_t>(1, std::min<int64_t>((H.nc * 32 + block - 1) / block, (int64_t)pb_sm_count() * 16));
     expand_pattern_kernel<<<grid, block, 0, st>>>(H.nc, p->cc_indptr.as<int32_t>(), p->pat_idx[2].as<int32_t>(), nd, nd,
                                                   nip.as<int32_t>(), nix.as<int32_t>());
     g_launches++;
@@ -1188,13 +1189,13 @@ extern "C" int pb_mpsa_system(pb_plan *p, const pb_values *stress, pb_csr **out)
     if (rc) return rc;
     if (p->cf_ip.p && !getenv("POREB200_DIV_SCATTER")) {
         constexpr int kWarps = 4, kCap = 128;           // 4 x 128 x 9 doubles = 36 KB of shared memory per block
-        int gridg = (int)std::max<int64_t>(1, std::min<int64_t>((H.nc + kWarps - 1) / kWarps, (int64_t)kSMs * 24));
+        int gridg = (int)std::max<int64_t>(1, std::min<int64_t>((H.nc + kWarps - 1) / kWarps, (int64_t)pb_sm_count() * 24));
         div_stress_gather_kernel<kWarps><<<gridg, kWarps * 32, (size_t)kWarps * kCap * nd2 * sizeof(double), st>>>(
             H.nc, nd, p->cf_ip.as<int32_t>(), p->cf_ix.as<int32_t>(), p->cf_sg.as<int8_t>(), p->fc_indptr.as<int32_t>(),
             p->pat_idx[0].as<int32_t>(), stress_dev, p->cc_indptr.as<int32_t>(), p->pat_idx[2].as<int32_t>(),
             pb_csr_data_(a), kCap);
     } else {
-        int grid2 = (int)std::max<int64_t>(1, std::min<int64_t>((H.nf * 32 + block - 1) / block, (int64_t)kSMs * 16));
+        int grid2 = (int)std::max<int64_t>(1, std::min<int64_t>((H.nf * 32 + block - 1) / block, (int64_t)pb_sm_count() * 16));
         div_stress_kernel<<<grid2, block, 0, st>>>(H.nf, nd, p->fc_indptr.as<int32_t>(), p->pat_idx[0].as<int32_t>(),
                                                    stress_dev, p->face_cells.as<int32_t>(),
                                                    p->cc_indptr.as<int32_t>(), p->pat_idx[2].as<int32_t>(), pb_csr_data_(a));
@@ -1226,10 +1227,10 @@ extern "C" int pb_mpsa_rhs(pb_plan *p, const pb_values *bound_stress, const doub
     if (source) CUDA_TRY(cudaMemcpyAsync(r.p, source, (size_t)H.nc * nd * sizeof(double), cudaMemcpyHostToDevice, st));
     else CUDA_TRY(cudaMemsetAsync(r.p, 0, (size_t)H.nc * nd * sizeof(double), st));
     const int block = 256;
-    int grid = (int)std::max<int64_t>(1, std::min<int64_t>((H.nf * nd * 32 + block - 1) / block, (int64_t)kSMs * 16));
+    int grid = (int)std::max<int64_t>(1, std::min<int64_t>((H.nf * nd * 32 + block - 1) / block, (int64_t)pb_sm_count() * 16));
     bound_stress_dot_kernel<<<grid, block, 0, st>>>(H.nf, nd, p->fb_indptr.as<int32_t>(), p->pat_idx[1].as<int32_t>(),
                                                     bstress_dev, bc.as<double>(), w.as<double>());
-    int grid2 = (int)std::max<int64_t>(1, std::min<int64_t>((H.nf * nd + block - 1) / block, (int64_t)kSMs * 16));
+    int grid2 = (int)std::max<int64_t>(1, std::min<int64_t>((H.nf * nd + block - 1) / block, (int64_t)pb_sm_count() * 16));
     neg_div_nd_kernel<<<grid2, block, 0, st>>>(H.nf, nd, p->face_cells.as<int32_t>(), w.as<double>(), r.as<double>());
     g_launches += 2;
     CUDA_TRY(cudaGetLastError());

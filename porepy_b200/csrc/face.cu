@@ -57,10 +57,10 @@ extern "C" int pb_facegrid_create(int64_t nc, int64_t nf, const int32_t *cf_indp
     FG_TRY(g->face_cells.ensure((size_t)2 * nf * sizeof(int32_t)));
     FG_TRY(cudaMemsetAsync(g->face_cells.p, 0xFF, (size_t)2 * nf * sizeof(int32_t), st));
     const int block = 256;
-    int grid = (int)std::max<int64_t>(1, std::min<int64_t>((nc + block - 1) / block, (int64_t)kSMs * 16));
+    int grid = (int)std::max<int64_t>(1, std::min<int64_t>((nc + block - 1) / block, (int64_t)pb_sm_count() * 16));
     face_cells_kernel<<<grid, block, 0, st>>>(nc, ip.as<int32_t>(), ix.as<int32_t>(), da.as<int8_t>(),
                                               g->face_cells.as<int32_t>(), bad.as<int>());
-    grid = (int)std::max<int64_t>(1, std::min<int64_t>((nf + block - 1) / block, (int64_t)kSMs * 16));
+    grid = (int)std::max<int64_t>(1, std::min<int64_t>((nf + block - 1) / block, (int64_t)pb_sm_count() * 16));
     face_cells_order_kernel<<<grid, block, 0, st>>>(nf, g->face_cells.as<int32_t>());
     pb_count_launch_(); pb_count_launch_();
     FG_TRY(cudaGetLastError());
@@ -122,7 +122,7 @@ extern "C" int pb_tpfa(pb_facegrid *g, const double *permeability, const uint8_t
     TpfaOut o{o_flux.as<double>(), o_bpc.as<double>(), o_vs.as<double>(), o_bpvs.as<double>(),
               o_bf.as<double>(), o_bpf.as<double>()};
     const int block = 256;
-    const int grid = (int)std::max<int64_t>(1, std::min<int64_t>((nf + block - 1) / block, (int64_t)kSMs * 16));
+    const int grid = (int)std::max<int64_t>(1, std::min<int64_t>((nf + block - 1) / block, (int64_t)pb_sm_count() * 16));
     tpfa_kernel<<<grid, block, 0, st>>>(nf, g->geo, perm.as<double>(), 1, 9, bc.as<uint8_t>(),
                                         g->face_cells.as<int32_t>(), ip.as<int32_t>(), vdim, o);
     pb_count_launch_();
@@ -162,7 +162,7 @@ extern "C" int pb_tpfa_diff(pb_facegrid *g, const double *k, const int32_t *fc_i
     CUDA_TRY(o_T.ensure((size_t)nf * sizeof(double)));
     CUDA_TRY(o_d.ensure(nhf * 9 * sizeof(double)));
     const int block = 256;
-    const int grid = (int)std::max<int64_t>(1, std::min<int64_t>((nf + block - 1) / block, (int64_t)kSMs * 16));
+    const int grid = (int)std::max<int64_t>(1, std::min<int64_t>((nf + block - 1) / block, (int64_t)pb_sm_count() * 16));
     tpfa_diff_kernel<<<grid, block, 0, st>>>(nf, g->geo, dk.as<double>(), g->face_cells.as<int32_t>(), ip.as<int32_t>(),
                                              o_t.as<double>(), o_T.as<double>(), o_d.as<double>());
     pb_count_launch_();
@@ -187,7 +187,7 @@ extern "C" int pb_upwind(pb_facegrid *g, const double *darcy_flux, const uint8_t
     CUDA_TRY(neu.ensure((size_t)nf * sizeof(double)));
     CUDA_TRY(dir.ensure((size_t)nf * sizeof(double)));
     const int block = 256;
-    const int grid = (int)std::max<int64_t>(1, std::min<int64_t>((nf + block - 1) / block, (int64_t)kSMs * 16));
+    const int grid = (int)std::max<int64_t>(1, std::min<int64_t>((nf + block - 1) / block, (int64_t)pb_sm_count() * 16));
     upwind_kernel<<<grid, block, 0, st>>>(nf, q.as<double>(), bc.as<uint8_t>(), g->face_cells.as<int32_t>(),
                                           up.as<int32_t>(), neu.as<double>(), dir.as<double>());
     pb_count_launch_();
@@ -224,7 +224,7 @@ extern "C" int pb_upwind_coupling(int64_t n, const double *interface_flux, doubl
     CUDA_TRY(in.upload(interface_flux, (size_t)n, 0));
     CUDA_TRY(o0.ensure((size_t)n * 8)); CUDA_TRY(o1.ensure((size_t)n * 8)); CUDA_TRY(o2.ensure((size_t)n * 8));
     const int block = 256;
-    const int grid = (int)std::max<int64_t>(1, std::min<int64_t>((n + block - 1) / block, (int64_t)kSMs * 16));
+    const int grid = (int)std::max<int64_t>(1, std::min<int64_t>((n + block - 1) / block, (int64_t)pb_sm_count() * 16));
     upwind_coupling_kernel<<<grid, block>>>(n, in.as<double>(), o0.as<double>(), o1.as<double>(), o2.as<double>());
     pb_count_launch_();
     CUDA_TRY(cudaGetLastError());

@@ -72,7 +72,7 @@ extern "C" int pb_compute_geometry_3d(int64_t nc, int64_t nf, int64_t nn, const 
     G_TRY(cudaMemcpyAsync(d_bad.p, &init, sizeof(int), cudaMemcpyHostToDevice, st));
     // outputs straight in the reference's (3, n) row-major layout: component stride n, entity stride 1
     GeomOut o{d_fn.as<double>(), d_fc.as<double>(), d_fa.as<double>(), d_cc.as<double>(), d_cv.as<double>(), nf, 1, nc, 1};
-    auto grid = [](int64_t n) { return (int)std::max<int64_t>(1, std::min<int64_t>((n + 127) / 128, (int64_t)kSMs * 16)); };
+    auto grid = [](int64_t n) { return (int)std::max<int64_t>(1, std::min<int64_t>((n + 127) / 128, (int64_t)pb_sm_count() * 16)); };
     G_TRY(cudaEventRecord(e0, st));
     geom_face_kernel<<<grid(nf), 128, 0, st>>>(nf, d_fn_ip.as<int32_t>(), d_fn_ix.as<int32_t>(), d_nodes.as<double>(), o);
     pb_count_launch_();

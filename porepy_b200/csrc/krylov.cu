@@ -156,7 +156,7 @@ __global__ void kry_xr_kernel(int64_t n, double *__restrict__ x, const double *_
     block_add(rho, gn + KS_RHO);
 }
 
-static int kgrid(int64_t n) { return (int)std::max<int64_t>(1, std::min<int64_t>((n + 255) / 256, (int64_t)kSMs * 8)); }
+static int kgrid(int64_t n) { return (int)std::max<int64_t>(1, std::min<int64_t>((n + 255) / 256, (int64_t)pb_sm_count() * 8)); }
 
 extern "C" int pb_kry_init(int64_t n, const double *b, double *x, double *r, double *rhat, double *p, double *v,
                            double *scal, double tol, uint64_t stream) {

@@ -48,12 +48,12 @@ PB_HD int64_t mpsa_rest_doubles(int nd, int nsf, int nsc, int nb, int nalpha) {
 }
 
 #if defined(PB_EXP_TMA) && defined(__CUDACC__)
-// Build variant -DPB_EXP_TMA -DPB_TMA_STAGE_DOUBLES=768 (A/B of round 2, profiles/r02_ab_tma.log; NOT the default build):
+// Build variant -DPB_EXP_TMA -DPB_TMA_STAGE_DOUBLES=768 (an A/B experiment; NOT the default build):
 // the NEXT region's face x cell position map (nsf * nsc int32, contiguous) is fetched by the TMA engine (cp.async.bulk ->
 // UBLKCP.S.G, completion on an mbarrier) into a shared-memory stage while the region's phases 1-6 run, instead of being
 // read from L2 inside the output phase.  One stage per CTA; the source range is widened to 16-byte boundaries (the plan
-// pads pos_fc), `off` ints are skipped on the shared side.  Measured on B200: 111.0 ms against 108.9 ms (tetrahedra) --
-// the L2 prefetch already hides these loads, the extra barrier and the 6 KB of shared memory cost more than they save.
+// pads pos_fc), `off` ints are skipped on the shared side.  The L2 prefetch of the default build already hides these
+// loads; whether the extra barrier and the 6 KB of shared memory pay off on H100 is not measured.
 struct TmaStage {
     int32_t *stage;      // 16-byte aligned, PB_TMA_STAGE_DOUBLES * 8 bytes
     uint64_t *mbar;
@@ -475,25 +475,32 @@ PB_HD void mpsa_node(Team &t, const PlanView &P, const GeoView &G, const MpsaPar
 #endif
     // ---- phase 6: Z[p][c] = SigmaA[p] applied to the solution (+ direct cell-displacement term)
 #if defined(__CUDA_ARCH__)
-    // (ND2 x n) * (n x nrhs) on the FP64 tensor cores: one 8x8 tile of Z per warp iteration
+    // (ND2 x n) * (n x nrhs) on the FP64 tensor cores: one 16x8 tile of Z per warp iteration (m16n8k4)
     {
         const int l = t.lane();
-        const int ntr = (ND2 + 7) / 8, ntc = (nrhs + 7) / 8;
+        const int ntr = (ND2 + 15) / 16, ntc = (nrhs + 7) / 8;
         for (int tile = t.warp(); tile < ntr * ntc; tile += t.nwarps()) {
             const int tr = tile / ntc, tc = tile - tr * ntc;
-            const int row = 8 * tr + (l >> 2);
+            const int row0 = 16 * tr + (l >> 2), row1 = row0 + 8;
             const int colb = 8 * tc + (l >> 2);
-            double acc[2] = {0.0, 0.0};
+            double acc0[2] = {0.0, 0.0}, acc1[2] = {0.0, 0.0};
             for (int k0 = 0; k0 < n; k0 += 4) {
                 const int k = k0 + (l & 3);
-                const double a = (row < ND2 && k < n) ? SA[row * n + k] : 0.0;
+                const double a0 = (row0 < ND2 && k < n) ? SA[row0 * n + k] : 0.0;
+                const double a1 = (row1 < ND2 && k < n) ? SA[row1 * n + k] : 0.0;
                 const double b = (k < n && colb < nrhs) ? A[(int64_t)rowidx[k] * W + n + colb] : 0.0;
-                pb_dmma(acc, a, b);
+                pb_dmma2(acc0, acc1, a0, a1, b);
             }
             const int c0 = 8 * tc + 2 * (l & 3);
-            if (row < ND2) {
-                if (c0 < nrhs) Z[row * nrhs + c0] = acc[0] + (c0 < ncc ? SAc[row * ncc + c0] : 0.0);
-                if (c0 + 1 < nrhs) Z[row * nrhs + c0 + 1] = acc[1] + (c0 + 1 < ncc ? SAc[row * ncc + c0 + 1] : 0.0);
+            const int rows[2] = {row0, row1};
+            const double *accs[2] = {acc0, acc1};
+            for (int h = 0; h < 2; ++h) {
+                const int row = rows[h];
+                if (row < ND2) {
+                    if (c0 < nrhs) Z[row * nrhs + c0] = accs[h][0] + (c0 < ncc ? SAc[row * ncc + c0] : 0.0);
+                    if (c0 + 1 < nrhs)
+                        Z[row * nrhs + c0 + 1] = accs[h][1] + (c0 + 1 < ncc ? SAc[row * ncc + c0 + 1] : 0.0);
+                }
             }
         }
     }

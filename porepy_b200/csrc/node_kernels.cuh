@@ -321,8 +321,8 @@ struct RegGJ {
 #endif
 
 #if defined(__CUDACC__)
-// Blocked Gauss-Jordan on FP64 tensor cores (DMMA, mma.sync.m8n8k4.f64 -- tcgen05 has no FP64
-// kind).  The augmented matrix lives in registers as 8x8 accumulator tiles: warp w owns row
+// Blocked Gauss-Jordan on FP64 tensor cores (DMMA: mma.sync.m16n8k4.f64 on pairs of row tiles, m8n8k4 on an
+// odd one; wgmma has no FP64 type).  The augmented matrix lives in registers as 8x8 accumulator tiles: warp w owns row
 // tile w (8 rows) and all NCT column tiles (2 doubles per lane and tile).  Pivots are taken four
 // at a time (a panel = half a column tile):
 //   S1  every warp dumps its 8x4 slice of the panel to shared memory;            -- barrier --
@@ -340,12 +340,21 @@ __device__ __forceinline__ void pb_dmma(double (&c)[2], double a, double b) {
                  : "+d"(c[0]), "+d"(c[1])
                  : "d"(a), "d"(b));
 }
+// Two 8-row tiles that share the B fragment in ONE instruction: m16n8k4 rows 0-7 are tile (c0, a0), rows 8-15 tile
+// (c1, a1); per lane the fragments are those of two m8n8k4 (A: row lane/4 [+8], column lane%4; C: row lane/4 [+8],
+// columns 2*(lane%4) + {0,1}).  On H100 m8n8k4 runs at half the FP64 tensor rate of the m16n8 shapes (register loops
+// of csrc/peaks.cu: 33 against 65 TFLOP/s), and the assembly step of 10^6 tetrahedra is 6 % faster with this pairing.
+__device__ __forceinline__ void pb_dmma2(double (&c0)[2], double (&c1)[2], double a0, double a1, double b) {
+    asm volatile("mma.sync.aligned.m16n8k4.row.col.f64.f64.f64.f64 {%0,%1,%2,%3}, {%4,%5}, {%6}, {%0,%1,%2,%3};"
+                 : "+d"(c0[0]), "+d"(c0[1]), "+d"(c1[0]), "+d"(c1[1])
+                 : "d"(a0), "d"(a1), "d"(b));
+}
 
 template <int NW, int RT, int NCT, int MINB>
 struct TileGJ {
     // NW warps; warp w owns the row tiles {w + NW*rt, rt < RT} (8 rows each) and all NCT column
     // tiles.  (A variant with a dedicated panel warp factorizing panel q+1 during the block update
-    // of panel q was measured no faster on B200 and is not kept: profiles/r01_notes.md.)
+    // of panel q was measured no faster and is not kept.)
     static_assert(NCT % 2 == 0, "padded row stride must be 4 mod 16");
     static constexpr int team = NW * 32;
     static constexpr int min_blocks = MINB;
@@ -642,7 +651,8 @@ struct TileGJ {
                     for (int tc = tcp; tc < NCT; ++tc) {
                         const double bf = rb[8 * tc];
 #pragma unroll
-                        for (int rt = 0; rt < RT; ++rt) pb_dmma(c[rt][tc], af[rt], bf);
+                        for (int rt = 0; rt + 1 < RT; rt += 2) pb_dmma2(c[rt][tc], c[rt + 1][tc], af[rt], af[rt + 1], bf);
+                        if (RT & 1) pb_dmma(c[RT - 1][tc], af[RT - 1], bf);
                     }
 #pragma unroll
                     for (int rt = 0; rt < RT; ++rt)

@@ -205,7 +205,18 @@ struct pb_plan {
 
 
 static const size_t kMaxSmem = 227 * 1024;
-static const int kSMs = 148;
+// SMs of the current device: the cap of every grid-stride launch (H100 SXM 132, H100 PCIe 114)
+inline int pb_sm_count() {
+    static int cache[64] = {0};
+    int dev = 0;
+    if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) dev = 0;
+    if (!cache[dev]) {
+        int n = 0;
+        if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n < 1) n = 1;
+        cache[dev] = n;
+    }
+    return cache[dev];
+}
 
 
 // launch one class with kernel template KERNEL<ND, Solver>
@@ -235,7 +246,7 @@ static int launch_one(K kernel, const NodeClass &c, pb_plan *p, const Prm &prm, 
     CUDA_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, blk, smem));
     if (per_sm < 1) per_sm = 1;
     int64_t need = ((int64_t)c.n + tpb - 1) / tpb;
-    int grid = (int)std::max<int64_t>(1, std::min<int64_t>(need, (int64_t)kSMs * per_sm));
+    int grid = (int)std::max<int64_t>(1, std::min<int64_t>(need, (int64_t)pb_sm_count() * per_sm));
     double *ws = nullptr;
     if (c.a_global) {
         CUDA_TRY(p->a_ws.ensure((size_t)grid * tpb * c.a_doubles * sizeof(double)));

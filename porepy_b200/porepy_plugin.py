@@ -79,7 +79,7 @@ def plugin(pp, allow_reference_fallback: bool = False) -> SimpleNamespace:
             except NotImplementedError as e:
                 if not allow_reference_fallback:
                     raise
-                logger.warning("B200 %s: %s -> reference path (allow_reference_fallback)", name, e)
+                logger.warning("porepy_b200 %s: %s -> reference path (allow_reference_fallback)", name, e)
                 _count(fallback_calls, f"{name}: {e}")
             ref_cls.discretize(self, sd, data)
 
@@ -118,7 +118,7 @@ def plugin(pp, allow_reference_fallback: bool = False) -> SimpleNamespace:
             except NotImplementedError as e:
                 if not allow_reference_fallback:
                     raise
-                logger.warning("B200 Upwind: %s -> reference path (allow_reference_fallback)", e)
+                logger.warning("porepy_b200 Upwind: %s -> reference path (allow_reference_fallback)", e)
                 _count(fallback_calls, f"Upwind: {e}")
             RefUpwind.discretize(self, sd, data)
 

@@ -86,14 +86,15 @@ def digest_params(g, seed=0):
     return k, bc, C, vbc, alpha
 
 
-def digest_of(m, seed=0, nvec=2, nrows=200, max_strided=20000, nbil=8):
-    """What is stored per output matrix: M @ x_k and |M| @ 1 on a strided subset of the rows (<= ``max_strided``),
-    ``nbil`` bilinear forms y^T M x over ALL entries, and ``nrows`` sampled rows entrywise (a CSR sub-matrix)."""
+def digest_of(m, seed=0, nvec=2, nrows=200, max_strided=20000, nbil=8, stride=None):
+    """What is stored per output matrix: M @ x_k and |M| @ 1 on every ``stride``-th row (default: <= ``max_strided``
+    rows; the row stride is stored with the digest), ``nbil`` bilinear forms y^T M x over ALL entries, and ``nrows``
+    sampled rows entrywise (a CSR sub-matrix)."""
     import scipy.sparse as sps
     m = sps.csr_matrix(m)
     rng = np.random.default_rng(seed)
     x = rng.standard_normal((m.shape[1], nvec))
-    stride = max(1, -(-m.shape[0] // max_strided))
+    stride = int(stride) if stride else max(1, -(-m.shape[0] // max_strided))
     mx = (m @ x)
     y = rng.standard_normal((m.shape[0], nbil))
     xb = rng.standard_normal((m.shape[1], nbil))
@@ -106,7 +107,7 @@ def digest_of(m, seed=0, nvec=2, nrows=200, max_strided=20000, nbil=8):
     return {"mx": mx[::stride], "abs1": np.asarray(abs(m).sum(axis=1)).ravel()[::stride], "bil": bil,
             "bil_scale": bil_scale, "rows": rows.astype(np.int64), "sub_data": sub.data,
             "sub_indices": sub.indices.astype(np.int32), "sub_indptr": sub.indptr.astype(np.int64),
-            "shape": np.array(m.shape, dtype=np.int64)}
+            "shape": np.array(m.shape, dtype=np.int64), "stride": np.int64(stride)}
 
 
 def digest_errors(dig: dict, m, seed=0):
@@ -116,7 +117,8 @@ def digest_errors(dig: dict, m, seed=0):
     import scipy.sparse as sps
     m = sps.csr_matrix(m)
     assert tuple(dig["shape"]) == m.shape, (tuple(dig["shape"]), m.shape)
-    mine = digest_of(m, seed, nvec=dig["mx"].shape[1], nrows=dig["rows"].size, nbil=dig["bil"].size)
+    mine = digest_of(m, seed, nvec=dig["mx"].shape[1], nrows=dig["rows"].size, nbil=dig["bil"].size,
+                     stride=int(dig["stride"]))
     assert np.array_equal(mine["rows"], dig["rows"]) and mine["mx"].shape == dig["mx"].shape
     e_mx = np.abs(mine["mx"] - dig["mx"]).max() / max(np.abs(dig["mx"]).max(), 1e-300)
     e_abs = np.abs(mine["abs1"] - dig["abs1"]).max() / max(np.abs(dig["abs1"]).max(), 1e-300)

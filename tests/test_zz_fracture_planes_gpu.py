@@ -1,6 +1,6 @@
 """GPU leg of tests/test_embedded_planes.py: flux discretization of fracture planes (2-D grids
 embedded in 3-D, ``ambient_dimension = 3``; reference mpfa.py:733-754 / 423-466) through the real
-device plan, against golden fixtures written by the reference (3 passed on B200 at the end of round 1)."""
+device plan, against golden fixtures written by the reference."""
 import pytest
 
 import porepy_b200 as pb

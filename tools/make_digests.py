@@ -4,7 +4,7 @@ The golden cases of tools/make_golden.py are 36-48 cells.  This script runs ``pp
 pp.Biot.discretize`` of the read-only reference on the sizes the benchmark configurations are built from
 (Cartesian 32^3 = BASELINE config[0], structured tetrahedra 12^3 x 6 and 16^3 x 6, Biot 16^3) and stores a
 DIGEST of every output matrix (tests/cases.py: ``digest_of``): M @ x and |M| @ 1 on a strided subset of the rows,
-8 bilinear forms over all entries, 200 sampled rows entrywise -- a few MB instead of GB.  Grid and parameters are regenerated from the seed on both sides
+8 bilinear forms over all entries, 200 sampled rows entrywise -- under 1 MB per case instead of GB (ROW_THINNING).  Grid and parameters are regenerated from the seed on both sides
 (tests/cases.py: ``digest_grid``, ``digest_params``); the reference is handed the very same arrays.
 
     python tools/make_digests.py [case ...]
@@ -31,6 +31,10 @@ import cases  # noqa: E402
 
 OUT = os.path.join(ROOT, "tests", "golden")
 
+
+# every k-th of (at most 20,000 strided) rows in M @ x and |M| @ 1: the finest thinning that keeps each case under 1 MB
+ROW_THINNING = {"digest_biot_cart16": 4, "digest_mpfa_cart32": 3, "digest_mpfa_tet12": 5, "digest_mpfa_tet16": 8,
+                "digest_mpsa_cart32": 2, "digest_mpsa_tet12": 3, "digest_mpsa_tet16": 3}
 
 def run(name):
     kind, dims, what = cases.DIGEST_CASES[name]
@@ -71,7 +75,8 @@ def run(name):
     secs = time.perf_counter() - t0
     d = {"seconds_reference": np.float64(secs), "num_cells": np.int64(g.num_cells)}
     for key, m in mats.items():
-        for kk, v in cases.digest_of(m).items():
+        stride = max(1, -(-m.shape[0] // 20000)) * ROW_THINNING[name]
+        for kk, v in cases.digest_of(m, stride=stride).items():
             d[f"D__{key}__{kk}"] = v
     np.savez_compressed(os.path.join(OUT, name + ".npz"), **d)
     print(f"{name}: {g.num_cells} cells, reference discretize {secs:.1f} s "

@@ -71,8 +71,9 @@ def make_grid(kind, rng):
         return g
     elif kind == "tet3d":
         g = pp.StructuredTetrahedralGrid([2, 2, 2], [1.0, 1.0, 1.0])
-    elif kind == "tet3d_delaunay":
-        pts = rng.random((3, 22))
+    elif kind in ("tet3d_delaunay", "tet3d_delaunay_small"):
+        # the small mesh keeps the MPSA fixture (nearly dense 3 x 3 blocks) under 1 MB
+        pts = rng.random((3, 22 if kind == "tet3d_delaunay" else 12))
         corners = np.array([[0, 0, 0], [1, 0, 0], [0, 1, 0], [1, 1, 0], [0, 0, 1], [1, 0, 1],
                             [0, 1, 1], [1, 1, 1]], float).T
         g = pp.TetrahedralGrid(np.hstack((corners, pts)))
@@ -497,7 +498,7 @@ def main():
         (case_mpsa, ("mpsa_cart3d_robin", "cart3d", True, 12), {}),
         (case_mpsa, ("mpsa_cart3d_pert", "cart3d_pert", False, 13), {}),
         (case_mpsa, ("mpsa_tet3d", "tet3d", False, 14), {}),
-        (case_mpsa, ("mpsa_tet3d_delaunay", "tet3d_delaunay", False, 15), {}),
+        (case_mpsa, ("mpsa_tet3d_delaunay", "tet3d_delaunay_small", False, 15), {}),
         (case_mpsa, ("mpsa_cart2d_robin", "cart2d", True, 16), {}),
         (case_mpsa, ("mpsa_tri2d", "tri2d", False, 17), {}),
         (case_mpsa, ("biot_cart3d", "cart3d", False, 21), {"biot": True}),

@@ -96,6 +96,10 @@ void pb_plan_destroy(pb_plan *p);
 int pb_plan_sizes(const pb_plan *p, int64_t *num_subcells, int64_t *num_subfaces,
                   int64_t *num_subhalffaces, int32_t *max_subfaces_per_node,
                   int32_t *max_subcells_per_node);
+/* Nodes per local-solver class of the classes last built for kind 0 (MPFA, at pb_mpfa_upload) or 1 (MPSA / Biot, at
+ * pb_mpsa_upload): counts[2 * cfg + g] for solver configuration cfg (0-7, see csrc/plan.hpp) with the local matrix
+ * in shared memory (g = 0) or in a global-memory workspace (g = 1).  counts has 16 entries.  Read-only. */
+int pb_plan_class_counts(const pb_plan *p, int kind, int64_t *counts);
 /* Shards: cell e of this plan is cell cells[e] of a larger (global) grid of n_source_cells cells.  The cell tensors of
  * the following pb_mpfa_upload / pb_mpsa_upload (permeability, stiffness, coupling tensors) are then the GLOBAL arrays
  * ((3,3,n_source), (9,9,n_source)) and are restricted on the device; NULL removes the map. */

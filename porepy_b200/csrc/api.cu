@@ -491,6 +491,14 @@ extern "C" int pb_plan_sizes(const pb_plan *p, int64_t *num_subcells, int64_t *n
     return PB_OK;
 }
 
+extern "C" int pb_plan_class_counts(const pb_plan *p, int kind, int64_t *counts) {
+    if (!p || !counts) return fail(PB_EINVAL, "null pointer");
+    if (kind != 0 && kind != 1) return fail(PB_EINVAL, "kind must be 0 (MPFA) or 1 (MPSA)");
+    for (int k = 0; k < 2 * kNumCfg; ++k) counts[k] = 0;
+    for (const NodeClass &c : kind == 0 ? p->mpfa_cls : p->mpsa_cls) counts[2 * c.cfg + (c.a_global ? 1 : 0)] += c.n;
+    return PB_OK;
+}
+
 extern "C" int pb_plan_set_active_nodes(pb_plan *p, const uint8_t *mask) {
     if (!p) return pb_fail_(PB_EINVAL, "null plan");
     if (mask) p->active.assign(mask, mask + p->H.nn); else p->active.clear();

@@ -243,7 +243,8 @@ struct RegGJ {
                     const unsigned long long k2 = __shfl_xor_sync(0xffffffffu, key, o);
                     key = k2 > key ? k2 : key;
                 }
-                if ((key >> 8) == 0ull) { ok = false; break; }  // zero column: uniform over the team
+                // zero column, or a NaN / inf pivot magnitude (exponent field all ones): uniform over the team
+                if ((key >> 8) == 0ull || (key >> 52) == 0x7FFull) { ok = false; break; }
                 const int pr = (int)(key & 0xFFull);
                 const int xpiv = (ti == pr % TR) ? pr / TR : -1;
                 if (xpiv >= 0) {
@@ -485,18 +486,20 @@ struct TileGJ {
 #pragma unroll
                         for (int jj = 0; jj < 4; ++jj) prow[jj] = __shfl_sync(0xffffffffu, x[jj], ol);
                     }
-                    // fraction-free elimination: the panel copy is only used to CHOOSE the pivots
-                    // (A11^-1 is formed from the original entries below), and scaling every row by
-                    // the same pivot does not change the arg-max -> no reciprocal on the critical path
-                    const double piv = prow[j];
+                    // the panel copy is only used to CHOOSE the pivots (A11^-1 is formed from the original
+                    // entries below).  It is eliminated at the scale of its entries: a fraction-free update
+                    // (v*piv - f*prow) squares that scale per column, so that entries of 1e-6 leave the
+                    // float range of the keys by column 3 (every key 0: a false "singular") and entries of
+                    // 1e5 overflow them (every key inf: the tie goes to the highest row).
+                    const double rpiv = __drcp_rn(prow[j]);
 #pragma unroll
                     for (int i = 0; i < NI; ++i) {
                         const bool me = (l == ol) && (i == os);
                         if (me) us[i] = true;
                         else {
-                            const double f = v[i][j];
+                            const double f = v[i][j] * rpiv;
 #pragma unroll
-                            for (int jj = j + 1; jj < 4; ++jj) v[i][jj] = v[i][jj] * piv - f * prow[jj];
+                            for (int jj = j + 1; jj < 4; ++jj) v[i][jj] -= f * prow[jj];
                         }
                     }
                 }

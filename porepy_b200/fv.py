@@ -344,6 +344,13 @@ class DevicePlan:
         return dict(subcells=a.value, subfaces=b.value, subhalffaces=c.value,
                     max_subfaces_per_node=d.value, max_subcells_per_node=e.value)
 
+    def class_counts(self, kind: str) -> dict:
+        """Nodes per local-solver class of the classes last built for ``kind`` ("mpfa" or "mpsa"):
+        {(cfg, a_in_global_memory): count} over the non-empty classes (solver configurations: csrc/plan.hpp)."""
+        counts = np.zeros(16, np.int64)
+        _lib.check(self.lib.pb_plan_class_counts(self.h, {"mpfa": 0, "mpsa": 1}[kind], _lib.ptr(counts, _lib._i64p)))
+        return {(k // 2, bool(k & 1)): int(v) for k, v in enumerate(counts) if v}
+
     # ---- MPFA
     def mpfa_upload(self, perm, codes, robw, eta) -> None:
         perm = _lib.f64(perm)

@@ -256,6 +256,58 @@ int pb_tpfa_diff(pb_facegrid *g, const double *k, const int32_t *fc_indptr, doub
 int pb_upwind(pb_facegrid *g, const double *darcy_flux, const uint8_t *bc_bits, int32_t *upstream_cell,
               double *neumann_diag, double *dirichlet_diag);
 
+/* ---- two-point stress approximation (csrc/tpsa_face.cuh; reference numerics/fv/tpsa.py:376-1430) ------------------
+ * One thread per face writes every value of the 14 TPSA matrices in that face's rows.  nr = nd in 3-D (the rotation
+ * is a 3-vector) and nr = 1 in 2-D (a scalar).  Shapes (rows x columns) and the block of one (face, cell) entry or of
+ * one face:
+ *   PB_TPSA_STRESS                          nd nf x nd nc   kron(., I_nd): nd diagonal values per (face, cell)
+ *   PB_TPSA_STRESS_ROTATION                 nd nf x nr nc   nd x nr
+ *   PB_TPSA_STRESS_TOTAL_PRESSURE           nd nf x nc      nd x 1
+ *   PB_TPSA_ROTATION_DISPLACEMENT           nr nf x nd nc   nr x nd
+ *   PB_TPSA_ROTATION_ROTATION               nr nf x nr nc   nr x nr
+ *   PB_TPSA_SOLID_MASS_DISPLACEMENT         nf x nd nc      1 x nd
+ *   PB_TPSA_SOLID_MASS_TOTAL_PRESSURE       nf x nc         1 x 1
+ *   PB_TPSA_BOUND_DISPLACEMENT_CELL         nd nf x nd nc   kron(., I_nd): nd diagonal values per (face, cell)
+ *   PB_TPSA_BOUND_DISPLACEMENT_ROTATION_CELL       nd nf x nr nc  nd x nr
+ *   PB_TPSA_BOUND_DISPLACEMENT_SOLID_PRESSURE_CELL nd nf x nc     nd x 1
+ *   PB_TPSA_BOUND_STRESS                    nd nf x nd nf   kron(., I_nd): nd diagonal values per face
+ *   PB_TPSA_BOUND_ROTATION_DISPLACEMENT     nr nf x nd nf   nr x nd per face
+ *   PB_TPSA_BOUND_MASS_DISPLACEMENT         nf x nd nf      1 x nd per face
+ *   PB_TPSA_BOUND_DISPLACEMENT_FACE         nd nf x nd nf   kron(., I_nd): nd diagonal values per face
+ * Cell terms follow the pattern of cell_faces in CSR-by-face form with ascending columns (fc_indptr, as for
+ * pb_tpfa), block-expanded: their value arrays are the CSR data of the expanded matrices (row f*br + i holds the
+ * blocks of the face's cells one after the other; kron(., I_nd) terms are nd x 1 blocks in column c*nd + i).  Face
+ * terms are the br x bc blocks row-major, face after face.
+ *   mu:         FourthOrderTensor.mu (nc), finite and > 0
+ *   codes:      nd * nf PB_BC_* codes, at f*nd + i (is_dir / is_neu / is_rob raveled in "F" order); PB_BC_INTERIOR
+ *               where no flag is set (interior and internal faces)
+ *   robin_diag: nd * nf diagonal Robin weights at f*nd + i, or NULL when no component is Robin
+ *   face_flags: nf bytes, non-zero for the faces of sd.get_all_boundary_faces(); such a face has exactly one cell
+ *   out:        PB_TPSA_NTERMS host pointers, each may be NULL
+ *   kernel_ms:  device time of the kernel (may be NULL)
+ * The face areas must have been set with pb_facegrid_set_face_areas. */
+enum {
+    PB_TPSA_STRESS = 0,
+    PB_TPSA_STRESS_ROTATION = 1,
+    PB_TPSA_STRESS_TOTAL_PRESSURE = 2,
+    PB_TPSA_ROTATION_DISPLACEMENT = 3,
+    PB_TPSA_ROTATION_ROTATION = 4,
+    PB_TPSA_SOLID_MASS_DISPLACEMENT = 5,
+    PB_TPSA_SOLID_MASS_TOTAL_PRESSURE = 6,
+    PB_TPSA_BOUND_DISPLACEMENT_CELL = 7,
+    PB_TPSA_BOUND_DISPLACEMENT_ROTATION_CELL = 8,
+    PB_TPSA_BOUND_DISPLACEMENT_SOLID_PRESSURE_CELL = 9,
+    PB_TPSA_BOUND_STRESS = 10,
+    PB_TPSA_BOUND_ROTATION_DISPLACEMENT = 11,
+    PB_TPSA_BOUND_MASS_DISPLACEMENT = 12,
+    PB_TPSA_BOUND_DISPLACEMENT_FACE = 13,
+    PB_TPSA_NTERMS = 14
+};
+/* face areas (nf, host pointer) of a pb_facegrid, read by pb_tpsa */
+int pb_facegrid_set_face_areas(pb_facegrid *g, const double *face_areas);
+int pb_tpsa(pb_facegrid *g, int nd, const double *mu, const uint8_t *codes, const double *robin_diag,
+            const uint8_t *face_flags, const int32_t *fc_indptr, double **out, float *kernel_ms);
+
 /* Interface upwinding (UpwindCoupling.discretize, numerics/fv/upwind.py:427-528): per mortar cell the sign of the
  * interface flux and the masks "upstream is the higher-dimensional side" / "... the lower-dimensional side".
  * Host pointers, n doubles each. */

@@ -7,7 +7,7 @@ first use; there is no CPU fallback.
 from .contact import FractureContact, FracturedMomentumBalance  # noqa: F401
 from .fractured_poromech import FractureCoupling, FracturedPoromechanics  # noqa: F401
 from .fractured_thm import FracturedThermoporomechanics  # noqa: F401
-from .fv import (Biot, DevicePlan, FaceGrid, Mpfa, Mpsa, Tpfa, Upwind, UpwindCoupling,  # noqa: F401
+from .fv import (Biot, DevicePlan, FaceGrid, Mpfa, Mpsa, Tpfa, Tpsa, Upwind, UpwindCoupling,  # noqa: F401
                  determine_eta)
 from .geometry import compute_geometry  # noqa: F401
 from .grid import Grid, cart_grid_2d, cart_grid_3d, structured_tet_grid, tet_grid_from_cells  # noqa: F401
@@ -22,7 +22,7 @@ from .sparse import DeviceCsr  # noqa: F401
 from .thermoporomech import Thermoporomechanics  # noqa: F401
 from .tpfa_ad import DifferentiableTpfa  # noqa: F401
 
-__all__ = ["Mpfa", "Mpsa", "Biot", "Tpfa", "Upwind", "UpwindCoupling", "DevicePlan", "FaceGrid", "DeviceCsr", "Grid", "cart_grid_2d", "cart_grid_3d",
+__all__ = ["Mpfa", "Mpsa", "Biot", "Tpfa", "Tpsa", "Upwind", "UpwindCoupling", "DevicePlan", "FaceGrid", "DeviceCsr", "Grid", "cart_grid_2d", "cart_grid_3d",
            "structured_tet_grid", "tet_grid_from_cells", "SecondOrderTensor", "FourthOrderTensor",
            "BoundaryCondition", "BoundaryConditionVectorial", "initialize_data", "PARAMETERS",
            "DISCRETIZATION_MATRICES", "determine_eta", "compute_geometry", "DifferentiableTpfa",

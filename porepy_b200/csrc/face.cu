@@ -4,11 +4,12 @@
 // 690-712, mpsa.py:666-697); no interaction-region plan is built.
 #include "plan.hpp"
 #include "tpfa_diff.cuh"
+#include "tpsa_face.cuh"
 
 struct pb_facegrid {
     int64_t nc = 0, nf = 0;
     cudaStream_t stream = nullptr;
-    DevBuf face_cells, fnorm, fcent, ccent, tmp;
+    DevBuf face_cells, fnorm, fcent, ccent, farea, tmp;   // farea: set by pb_facegrid_set_face_areas
     GeoView geo{};
 };
 
@@ -91,6 +92,14 @@ __global__ void tpfa_kernel(int64_t nf, GeoView G, const double *__restrict__ pe
                             int vdim, TpfaOut o) {
     for (int64_t f = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; f < nf; f += (int64_t)gridDim.x * blockDim.x)
         tpfa_face(f, G, perm, perm_cs, perm_es, bc, face_cells, fc_ptr, vdim, o);
+}
+
+template <int ND>
+__global__ void tpsa_kernel(int64_t nf, GeoView G, const double *__restrict__ mu, const uint8_t *__restrict__ codes,
+                            const double *__restrict__ robw, const uint8_t *__restrict__ flags,
+                            const int32_t *__restrict__ face_cells, const int32_t *__restrict__ fc_ptr, TpsaOut o) {
+    for (int64_t f = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; f < nf; f += (int64_t)gridDim.x * blockDim.x)
+        tpsa_face<ND>(f, G, mu, codes, robw, flags, face_cells, fc_ptr, o);
 }
 
 __global__ void upwind_kernel(int64_t nf, const double *__restrict__ q, const uint8_t *__restrict__ bc,
@@ -231,5 +240,81 @@ extern "C" int pb_upwind_coupling(int64_t n, const double *interface_flux, doubl
     CUDA_TRY(cudaMemcpy(sign, o0.p, (size_t)n * 8, cudaMemcpyDeviceToHost));
     CUDA_TRY(cudaMemcpy(from_primary, o1.p, (size_t)n * 8, cudaMemcpyDeviceToHost));
     CUDA_TRY(cudaMemcpy(from_secondary, o2.p, (size_t)n * 8, cudaMemcpyDeviceToHost));
+    return PB_OK;
+}
+
+extern "C" int pb_facegrid_set_face_areas(pb_facegrid *g, const double *face_areas) {
+    if (!g || !face_areas) return pb_fail_(PB_EINVAL, "null pointer");
+    CUDA_TRY(g->farea.upload(face_areas, (size_t)g->nf, g->stream));
+    CUDA_TRY(cudaStreamSynchronize(g->stream));
+    g->geo.farea = g->farea.as<double>();
+    return PB_OK;
+}
+
+// Two-point stress approximation (tpsa_face.cuh): value arrays of the 14 terms, layouts in include/poreb200.h.
+extern "C" int pb_tpsa(pb_facegrid *g, int nd, const double *mu, const uint8_t *codes, const double *robin_diag,
+                       const uint8_t *face_flags, const int32_t *fc_indptr, double **out, float *kernel_ms) {
+    if (!g || !mu || !codes || !face_flags || !fc_indptr || !out) return pb_fail_(PB_EINVAL, "null pointer");
+    if (nd != 2 && nd != 3) return pb_fail_(PB_EINVAL, "Tpsa is only implemented for 2d and 3d grids.");
+    if (!g->geo.farea) return pb_fail_(PB_EINVAL, "face areas not set (pb_facegrid_set_face_areas)");
+    const int64_t nf = g->nf, nc = g->nc;
+    for (int64_t c = 0; c < nc; ++c)   // the scheme divides by mu and by mu / distance
+        if (!(mu[c] > 0.0) || !std::isfinite(mu[c])) return pb_fail_(PB_EINVAL, "shear modulus must be finite and > 0");
+    bool any_rob = false;
+    for (int64_t q = 0; q < nd * nf; ++q) {
+        if (codes[q] > PB_BC_ROB) return pb_fail_(PB_EINVAL, "boundary code out of range");
+        any_rob |= codes[q] == PB_BC_ROB;
+    }
+    if (any_rob && !robin_diag) return pb_fail_(PB_EINVAL, "Robin faces need robin_diag");
+    for (int64_t f = 0; f < nf; ++f) {
+        const int32_t len = fc_indptr[f + 1] - fc_indptr[f];
+        if (len < 1 || len > 2) return pb_fail_(PB_EINVAL, "fc_indptr: a face has one or two cells");
+        if (face_flags[f] && len != 1) return pb_fail_(PB_EINVAL, "sign of internal faces does not make sense");
+    }
+    cudaStream_t st = g->stream;
+    const size_t nnz = (size_t)fc_indptr[nf];
+    const size_t nr = nd == 3 ? 3 : 1;
+    // values per (face, cell) entry or per face, in PB_TPSA_* order
+    const size_t per[PB_TPSA_NTERMS] = {(size_t)nd, nd * nr, (size_t)nd, nr * nd, nr * nr, (size_t)nd, 1, (size_t)nd,
+                                        nd * nr, (size_t)nd, (size_t)nd, nr * nd, (size_t)nd, (size_t)nd};
+    DevBuf dmu, dcodes, drob, dflags, dip, o_buf[PB_TPSA_NTERMS];
+    CUDA_TRY(dmu.upload(mu, (size_t)nc, st));
+    CUDA_TRY(dcodes.upload(codes, (size_t)nd * nf, st));
+    if (any_rob) CUDA_TRY(drob.upload(robin_diag, (size_t)nd * nf, st));
+    CUDA_TRY(dflags.upload(face_flags, (size_t)nf, st));
+    CUDA_TRY(dip.upload(fc_indptr, (size_t)nf + 1, st));
+    TpsaOut o{};
+    size_t count[PB_TPSA_NTERMS];
+    for (int k = 0; k < PB_TPSA_NTERMS; ++k) {
+        count[k] = per[k] * (k < PB_TPSA_BOUND_STRESS ? nnz : (size_t)nf);
+        if (!out[k]) continue;
+        CUDA_TRY(o_buf[k].ensure(count[k] * sizeof(double)));
+        o.t[k] = o_buf[k].as<double>();
+    }
+    struct Events {
+        cudaEvent_t e0 = nullptr, e1 = nullptr;
+        ~Events() { if (e0) cudaEventDestroy(e0); if (e1) cudaEventDestroy(e1); }
+    } ev;
+    if (kernel_ms) {
+        CUDA_TRY(cudaEventCreate(&ev.e0));
+        CUDA_TRY(cudaEventCreate(&ev.e1));
+        CUDA_TRY(cudaEventRecord(ev.e0, st));
+    }
+    const int block = 256;
+    const int grid = (int)std::max<int64_t>(1, std::min<int64_t>((nf + block - 1) / block, (int64_t)pb_sm_count() * 16));
+    const double *rw = any_rob ? drob.as<double>() : nullptr;
+    if (nd == 3)
+        tpsa_kernel<3><<<grid, block, 0, st>>>(nf, g->geo, dmu.as<double>(), dcodes.as<uint8_t>(), rw,
+                                              dflags.as<uint8_t>(), g->face_cells.as<int32_t>(), dip.as<int32_t>(), o);
+    else
+        tpsa_kernel<2><<<grid, block, 0, st>>>(nf, g->geo, dmu.as<double>(), dcodes.as<uint8_t>(), rw,
+                                              dflags.as<uint8_t>(), g->face_cells.as<int32_t>(), dip.as<int32_t>(), o);
+    pb_count_launch_();
+    CUDA_TRY(cudaGetLastError());
+    if (kernel_ms) CUDA_TRY(cudaEventRecord(ev.e1, st));
+    for (int k = 0; k < PB_TPSA_NTERMS; ++k)
+        if (out[k]) CUDA_TRY(cudaMemcpyAsync(out[k], o_buf[k].p, count[k] * sizeof(double), cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(cudaStreamSynchronize(st));
+    if (kernel_ms) CUDA_TRY(cudaEventElapsedTime(kernel_ms, ev.e0, ev.e1));
     return PB_OK;
 }

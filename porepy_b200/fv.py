@@ -616,6 +616,52 @@ class FaceGrid:
                                       _lib.ptr(up, _lib._i32p), _lib.ptr(neu, _lib._f64p), _lib.ptr(dr, _lib._f64p)))
         return up, neu, dr
 
+    def tpsa(self, nd: int, mu, codes, robin_diag, face_flags, fc_indptr, face_areas) -> tuple:
+        """Value arrays of the 14 TPSA terms in ``PB_TPSA_*`` order (layouts in include/poreb200.h; sizes from
+        ``tpsa_value_counts``) and the kernel time in ms.  ``codes`` / ``robin_diag``: (nf, nd), ``face_flags``: nf."""
+        mu = _lib.f64(mu)
+        if mu.shape != (self.nc,):
+            raise ValueError("fourth_order_tensor.mu must have one value per cell")
+        cod = np.ascontiguousarray(codes, dtype=np.uint8)
+        rob = None if robin_diag is None else _lib.f64(robin_diag)
+        flags = np.ascontiguousarray(face_flags, dtype=np.uint8)
+        ip = np.ascontiguousarray(fc_indptr, dtype=np.int32)
+        _lib.check(self.lib.pb_facegrid_set_face_areas(self.h, _lib.ptr(_lib.f64(face_areas), _lib._f64p)))
+        out = [_lib.pinned_empty(n) for n in tpsa_value_counts(nd, self.nf, int(ip[-1]))]
+        ptrs = (_lib._f64p * len(out))(*[_lib.ptr(a, _lib._f64p) for a in out])
+        ms = C.c_float(0.0)
+        _lib.check(self.lib.pb_tpsa(self.h, int(nd), _lib.ptr(mu, _lib._f64p), _lib.ptr(cod, _lib._u8p),
+                                    _lib.ptr(rob, _lib._f64p), _lib.ptr(flags, _lib._u8p), _lib.ptr(ip, _lib._i32p),
+                                    ptrs, C.byref(ms)))
+        return out, float(ms.value)
+
+
+# (rows per face, columns per cell or face) of the 14 TPSA terms in PB_TPSA_* order; "k" marks kron(., I_nd), "r" the
+# rotation dimension (nd in 3-D, 1 in 2-D), "d" the dimension.  The first ten terms have cell columns.
+_TPSA_BLOCKS = (("d", "k"), ("d", "r"), ("d", 1), ("r", "d"), ("r", "r"), (1, "d"), (1, 1), ("d", "k"), ("d", "r"),
+                ("d", 1), ("d", "k"), ("r", "d"), (1, "d"), ("d", "k"))
+_TPSA_NCELLTERMS = 10
+
+
+def _tpsa_block(nd: int, k: int):
+    """(rows, columns, kron) of one block of TPSA term k."""
+    nr = 3 if nd == 3 else 1
+    size = {"d": nd, "r": nr, 1: 1}
+    br, bc = _TPSA_BLOCKS[k]
+    if bc == "k":
+        return nd, nd, True
+    return size[br], size[bc], False
+
+
+def tpsa_value_counts(nd: int, nf: int, nnz: int) -> list:
+    """Number of values of each TPSA term (``nnz`` = entries of cell_faces)."""
+    counts = []
+    for k in range(len(_TPSA_BLOCKS)):
+        br, bc, kron = _tpsa_block(nd, k)
+        per = br if kron else br * bc
+        counts.append(per * (nnz if k < _TPSA_NCELLTERMS else nf))
+    return counts
+
 
 
 # ------------------------------------------------------------------------------------------
@@ -1108,6 +1154,153 @@ class Tpfa(Mpfa):
             self.bound_pressure_vector_source_matrix_key: sps.csr_matrix((vals[3], cols_v, ipv),
                                                                          shape=(nf, nc * vdim)),
         }
+
+
+def _tpsa_patterns(nd: int, nc: int, nf: int, ip: np.ndarray, ix: np.ndarray) -> list:
+    """(indptr, indices, shape) of the 14 TPSA terms in the value layouts of ``pb_tpsa`` (include/poreb200.h).  Cell
+    terms expand the face x cell pattern with ``block_expand``; kron(., I_nd) terms keep column c*nd + i in row
+    f*nd + i; face terms are block diagonal."""
+    out, cache = [], {}
+    for k in range(len(_TPSA_BLOCKS)):
+        br, bc, kron = _tpsa_block(nd, k)
+        key = (k < _TPSA_NCELLTERMS, br, bc, kron)
+        if key not in cache:
+            if k < _TPSA_NCELLTERMS:
+                nip, cols = block_expand(ip, ix, br, 1 if kron else bc)
+                if kron:
+                    rows = np.repeat(np.arange(nf * br, dtype=np.int64), np.diff(nip))
+                    cols = cols * nd + rows % nd
+                shape = (nf * br, nc * bc)
+            else:
+                per = 1 if kron else bc
+                nip = np.arange(0, nf * br * per + 1, per, dtype=np.int64)
+                if kron:
+                    cols = np.arange(nf * br, dtype=np.int64)
+                else:
+                    cols = ((np.arange(nf * br, dtype=np.int64) // br) * bc)[:, None] + np.arange(bc, dtype=np.int64)
+                shape = (nf * br, nf * bc)
+            dt = _index_dtype(int(nip[-1]), shape[1])
+            cache[key] = (nip.astype(dt), cols.reshape(-1).astype(dt), shape)
+        out.append(cache[key])
+    return out
+
+
+def tpsa_bc_arrays(bc, nd: int, nf: int):
+    """Per-(face, component) codes (nf, nd) and diagonal Robin weights (nf, nd) or None, after the refusals of
+    tpsa.py:572-618 (same exceptions and messages)."""
+    basis = np.asarray(bc.basis)
+    if np.logical_or.reduce((np.any(basis[0, 1:, :] > 0), np.any(basis[1, 0, :] > 0), np.any(basis[1, 2:, :] > 0),
+                             np.any(basis[2:, :2, :] > 0), np.any(basis[0, 0, :] != 1),
+                             np.any(basis[1, 1, :] != 1))):
+        raise NotImplementedError("Have not implemented Robin conditions with a non-trivial basis.")
+    if nd == 3 and np.any(basis[2, 2] != 1):
+        raise NotImplementedError("Have not implemented Robin conditions with a non-trivial basis.")
+    rw = np.asarray(bc.robin_weight)
+    if np.logical_or.reduce((np.any(rw[0, 1:, :] > 0), np.any(rw[1, 0, :] > 0), np.any(rw[1, 2:, :] > 0),
+                             np.any(rw[2:, :2, :] > 0))):
+        raise NotImplementedError("Non-diagonal Robin weights have not been implemnted.")
+    is_rob = np.asarray(bc.is_rob, bool)[:nd]
+    if not all(np.logical_xor(np.any(is_rob, axis=0), np.logical_not(np.all(is_rob, axis=0)))):
+        raise NotImplementedError("Mixing Robin with Dirichlet or Neumann conditions is not implemneted.")
+    codes = np.zeros((nf, nd), np.uint8)
+    codes[np.asarray(bc.is_neu, bool)[:nd].T] = _lib.BC_NEU
+    codes[np.asarray(bc.is_dir, bool)[:nd].T] = _lib.BC_DIR
+    codes[is_rob.T] = _lib.BC_ROB
+    robin = None
+    if is_rob.any():
+        robin = np.ascontiguousarray(np.stack([rw[i, i] for i in range(nd)], axis=1), dtype=np.float64)
+    return codes, robin
+
+
+class Tpsa(_Base):
+    """Two-point stress approximation (numerics/fv/tpsa.py:136, Nordbotten & Keilegavlen): the same constructor,
+    matrix keys (:265-331), ``ndof`` and ``discretize`` outputs as the reference, computed by one thread per face on a
+    ``FaceGrid`` (csrc/tpsa_face.cuh).  The matrices are scipy CSR with the fixed block pattern of each term; values
+    equal the reference's (its explicit zeros are not reproduced).  Always the whole grid: the reference has no
+    partial mode."""
+
+    def __init__(self, keyword: str) -> None:
+        super().__init__(keyword)
+        self.stress_displacement_matrix_key = "stress"
+        self.stress_rotation_matrix_key = "stress_rotation"
+        self.stress_total_pressure_matrix_key = "stress_total_pressure"
+        self.rotation_displacement_matrix_key = "rotation_displacement"
+        self.rotation_rotation_matrix_key = "rotation_rotation"
+        self.mass_total_pressure_matrix_key = "solid_mass_total_pressure"
+        self.mass_displacement_matrix_key = "solid_mass_displacement"
+        self.bound_stress_matrix_key = "bound_stress"
+        self.bound_rotation_displacement_matrix_key = "bound_rotation_displacement"
+        self.bound_mass_displacement_matrix_key = "bound_mass_displacement"
+        self.bound_displacement_cell_matrix_key = "bound_displacement_cell"
+        self.bound_displacement_face_matrix_key = "bound_displacement_face"
+        self.bound_displacement_rotation_cell_matrix_key = "bound_displacement_rotation_cell"
+        self.bound_displacement_solid_pressure_cell_matrix_key = "bound_displacement_solid_pressure_cell"
+
+    def _term_keys(self) -> list:
+        """Matrix keys in PB_TPSA_* order."""
+        return [self.stress_displacement_matrix_key, self.stress_rotation_matrix_key,
+                self.stress_total_pressure_matrix_key, self.rotation_displacement_matrix_key,
+                self.rotation_rotation_matrix_key, self.mass_displacement_matrix_key,
+                self.mass_total_pressure_matrix_key, self.bound_displacement_cell_matrix_key,
+                self.bound_displacement_rotation_cell_matrix_key,
+                self.bound_displacement_solid_pressure_cell_matrix_key, self.bound_stress_matrix_key,
+                self.bound_rotation_displacement_matrix_key, self.bound_mass_displacement_matrix_key,
+                self.bound_displacement_face_matrix_key]
+
+    def ndof(self, sd) -> int:
+        """tpsa.py:333-348."""
+        if sd.dim == 2:
+            return sd.num_cells * (2 + sd.dim)
+        elif sd.dim == 3:
+            return sd.num_cells * (1 + 2 * sd.dim)
+        raise NotImplementedError("Tpsa is only implemented for 2d and 3d grids.")
+
+    def assemble_matrix_rhs(self, sd, sd_data: dict):
+        """tpsa.py:350-374: assembly belongs to the multiphysics models."""
+        raise NotImplementedError(
+            """This class cannot be used for assembly.
+            Use a multiphysics model class instead."""
+        )
+
+    def discretize(self, sd, data: dict) -> None:
+        params = data[PARAMETERS][self.keyword]
+        mats = data.setdefault(DISCRETIZATION_MATRICES, {}).setdefault(self.keyword, {})
+        mats.update(self._discretize_grid(sd, params))
+
+    def _discretize_grid(self, sd, params: dict) -> dict:
+        nd, nc, nf = sd.dim, sd.num_cells, sd.num_faces
+        if nd not in (2, 3):
+            raise NotImplementedError("Tpsa is only implemented for 2d and 3d grids.")
+        self._check_unsupported(params, sd)
+        mu = params["fourth_order_tensor"].mu
+        codes, robin = tpsa_bc_arrays(params["bc"], nd, nf)
+        if nd == 2 and np.any(np.abs(sd.face_normals[2]) > np.maximum(np.abs(sd.face_normals[0]),
+                                                                       np.abs(sd.face_normals[1]))):
+            # tpsa.py:1053-1054 indexes is_dir (2 rows) with the argmax over all three rows of the normals
+            raise IndexError("Tpsa: a face normal of a 2d grid points mostly out of the xy-plane")
+        t0 = time.perf_counter()
+        fg = FaceGrid.for_grid(sd)
+        fc = sps.csr_matrix(sd.cell_faces)
+        fc.sort_indices()
+        ip, ix = fc.indptr, fc.indices
+        flags = np.zeros(nf, np.uint8)
+        flags[np.asarray(sd.get_all_boundary_faces(), dtype=np.int64)] = 1
+        vals, kernel_ms = fg.tpsa(nd, mu, codes, robin, flags, ip, sd.face_areas)
+        t1 = time.perf_counter()
+        # the index arrays depend on the topology only: built once per grid, copied per matrix (scipy may edit a
+        # matrix's index arrays in place, e.g. eliminate_zeros)
+        cached = getattr(sd, "_b200_tpsa_patterns", None)
+        if (cached is None or cached[0] != nd or not np.array_equal(cached[1], ip)
+                or not np.array_equal(cached[2], ix)):
+            cached = (nd, ip.copy(), ix.copy(), _tpsa_patterns(nd, nc, nf, ip, ix))
+            try:
+                sd._b200_tpsa_patterns = cached
+            except AttributeError:
+                pass
+        mats = {key: sps.csr_matrix((v, pat[1].copy(), pat[0].copy()), shape=pat[2])
+                for key, v, pat in zip(self._term_keys(), vals, cached[3])}
+        self.last_timing = dict(kernel_ms=kernel_ms, device_s=t1 - t0, total_s=time.perf_counter() - t0)
+        return mats
 
 
 class Upwind(_Base):

@@ -1,5 +1,5 @@
-"""Drop-in plugin for an installed PorePy: subclasses of ``pp.Mpfa / pp.Mpsa / pp.Biot`` and of
-the AD wrappers ``pp.ad.MpfaAd / MpsaAd / BiotAd`` whose ``discretize`` runs on the GPU.
+"""Drop-in plugin for an installed PorePy: subclasses of ``pp.Mpfa / pp.Mpsa / pp.Biot / pp.Tpsa`` and of
+the AD wrappers ``pp.ad.MpfaAd / MpsaAd / BiotAd / TpsaAd`` whose ``discretize`` runs on the GPU.
 
 Why subclasses: ``MpfaAd.__init__`` hard-codes ``pp.Mpfa(keyword)`` (reference
 src/porepy/numerics/ad/discretizations.py:192-206) and the model mixins test
@@ -54,6 +54,7 @@ def plugin(pp, allow_reference_fallback: bool = False) -> SimpleNamespace:
     # pp.Mpfa etc. to the plugin classes (e.g. to run the reference's own tests on them)
     RefMpfa, RefMpsa, RefBiot = pp.Mpfa, pp.Mpsa, pp.Biot
     RefTpfa, RefUpwind = pp.Tpfa, pp.Upwind
+    RefTpsa, RefTpsaAd = pp.Tpsa, pp.ad.TpsaAd
     RefUpwindCoupling = pp.UpwindCoupling
     RefMpfaAd, RefMpsaAd, RefBiotAd = pp.ad.MpfaAd, pp.ad.MpsaAd, pp.ad.BiotAd
 
@@ -102,6 +103,7 @@ def plugin(pp, allow_reference_fallback: bool = False) -> SimpleNamespace:
     Tpfa = _core("Tpfa", fv.Tpfa, RefTpfa, False)
     Mpsa = _core("Mpsa", fv.Mpsa, RefMpsa, False)
     Biot = _core("Biot", fv.Biot, RefBiot, False)
+    Tpsa = _core("Tpsa", fv.Tpsa, RefTpsa, False)
 
     class Upwind(fv.Upwind, RefUpwind):
         """pp.Upwind with the per-face GPU kernel (grids of any dimension)."""
@@ -161,6 +163,11 @@ def plugin(pp, allow_reference_fallback: bool = False) -> SimpleNamespace:
                     ["displacement_divergence", "bound_displacement_divergence", "scalar_gradient",
                      "bound_pressure", "consistency"])
 
+    class TpsaAd(RefTpsaAd):
+        def __init__(self, keyword, subdomains):
+            super().__init__(keyword, subdomains)
+            _rewrap(self, Tpsa(keyword), subdomains)
+
     class ModelMixin:
         """Put FIRST among the bases of a PorePy model class to route its flux / stress
         discretizations through the GPU classes::
@@ -180,6 +187,8 @@ def plugin(pp, allow_reference_fallback: bool = False) -> SimpleNamespace:
 
         def stress_discretization(self, subdomains):
             stock = super().stress_discretization(subdomains)
+            if isinstance(stock, RefTpsaAd):   # the TPSA models (models/momentum_balance.py:998)
+                return TpsaAd(self.stress_keyword, subdomains)
             cls = BiotAd if isinstance(stock, RefBiotAd) else MpsaAd
             return cls(self.stress_keyword, subdomains)
 
@@ -190,7 +199,8 @@ def plugin(pp, allow_reference_fallback: bool = False) -> SimpleNamespace:
                 self._nonlinear_diffusive_flux_discretizations.append(discretization)
 
     def install() -> None:
-        """Rebind ``pp.Mpfa / pp.Mpsa / pp.Biot`` to the plugin classes for the whole process.  The AD
+        """Rebind ``pp.Mpfa / pp.Mpsa / pp.Biot`` (and ``pp.Tpfa / pp.Upwind / pp.UpwindCoupling / pp.Tpsa``) to
+        the plugin classes for the whole process.  The AD
         wrappers look the cores up at construction time (``pp.Mpfa(keyword)``,
         numerics/ad/discretizations.py:192-206) and the models' exact-type checks compare with
         ``pp.Mpfa``, so every stock model then discretizes through porepy_b200 without any change to
@@ -198,11 +208,13 @@ def plugin(pp, allow_reference_fallback: bool = False) -> SimpleNamespace:
         pp.Mpfa, pp.Mpsa, pp.Biot = Mpfa, Mpsa, Biot
         pp.Tpfa, pp.Upwind = Tpfa, Upwind
         pp.UpwindCoupling = UpwindCoupling
+        pp.Tpsa = Tpsa
 
     def uninstall() -> None:
         pp.Mpfa, pp.Mpsa, pp.Biot = RefMpfa, RefMpsa, RefBiot
         pp.Tpfa, pp.Upwind = RefTpfa, RefUpwind
         pp.UpwindCoupling = RefUpwindCoupling
+        pp.Tpsa = RefTpsa
 
     def md_flow_from_model(model, keyword=None):
         """The mixed-dimensional Darcy problem of a prepared single-phase flow model (``pp.SinglePhaseFlow`` after
@@ -235,7 +247,8 @@ def plugin(pp, allow_reference_fallback: bool = False) -> SimpleNamespace:
             specific_volume=lambda it: evaluated(model.specific_volume([it]), it.num_cells))
 
     from . import model_bridge as bridge
-    return SimpleNamespace(Mpfa=Mpfa, Mpsa=Mpsa, Biot=Biot, Tpfa=Tpfa, Upwind=Upwind, UpwindCoupling=UpwindCoupling, MpfaAd=MpfaAd, MpsaAd=MpsaAd, BiotAd=BiotAd,
+    return SimpleNamespace(Mpfa=Mpfa, Mpsa=Mpsa, Biot=Biot, Tpfa=Tpfa, Tpsa=Tpsa, Upwind=Upwind, UpwindCoupling=UpwindCoupling,
+                           MpfaAd=MpfaAd, MpsaAd=MpsaAd, BiotAd=BiotAd, TpsaAd=TpsaAd,
                            ModelMixin=ModelMixin, install=install, uninstall=uninstall, md_flow_from_model=md_flow_from_model,
                            # nonlinear model problems on the device AD chain (porepy_b200/model_bridge.py)
                            compressible_flow_from_model=bridge.compressible_flow_from_model,

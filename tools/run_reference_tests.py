@@ -1,5 +1,6 @@
-"""Run the REFERENCE's own finite-volume unit tests (tests/numerics/fv/test_{mpfa,mpsa,biot}.py of the
-read-only tree) with pp.Mpfa / pp.Mpsa / pp.Biot rebound to the porepy_b200 plugin classes.
+"""Run the REFERENCE's own finite-volume unit tests (tests/numerics/fv/test_{mpfa,mpsa,biot,tpsa}.py of the
+read-only tree) with pp.Mpfa / pp.Mpsa / pp.Biot / pp.Tpsa (and pp.Tpfa / pp.Upwind) rebound to the porepy_b200
+plugin classes.
 
     python tools/run_reference_tests.py            # build container or any box with /root/reference
     python tools/run_reference_tests.py functional/test_terzaghi.py [--stock] [pytest options]
@@ -34,13 +35,14 @@ class Rebind:
         except Exception:
             gpu = False
         if not gpu:
-            from emu_binding import EmuBackedFaceGrid, EmuBackedPlan
+            from emu_binding import EmuBackedPlan
+            from emu_tpsa import EmuTpsaFaceGrid   # the host build of the per-face routines, TPSA included
             fv.DevicePlan = EmuBackedPlan
-            fv.FaceGrid = EmuBackedFaceGrid
+            fv.FaceGrid = EmuTpsaFaceGrid
             import emu_binding
             fv.interface_upwind_masks = emu_binding.emu_interface_upwind_masks
         COUNTS["backend: " + ("cuda" if gpu else "host build of the node routines")] = 1
-        for name in ("Mpfa", "Mpsa", "Biot", "Tpfa", "Upwind"):
+        for name in ("Mpfa", "Mpsa", "Biot", "Tpfa", "Upwind", "Tpsa"):
             for owner, tag in ((getattr(fv, name), "porepy_b200"), (getattr(pp, name), "reference")):
                 stock = owner.discretize
 
@@ -75,7 +77,7 @@ if __name__ == "__main__":
     if extra:
         files = [os.path.join("/root/reference/tests", a) for a in extra]
     else:
-        files = [os.path.join(REF_TESTS, f) for f in ("test_mpfa.py", "test_mpsa.py", "test_biot.py")]
+        files = [os.path.join(REF_TESTS, f) for f in ("test_mpfa.py", "test_mpsa.py", "test_biot.py", "test_tpsa.py")]
     os.chdir("/tmp")
     sys.exit(pytest.main(files + ["-p", "no:cacheprovider", "-o", "addopts=", "-q", "--rootdir", "/tmp", *opts],
                          plugins=[Rebind()]))

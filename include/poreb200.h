@@ -97,8 +97,8 @@ int pb_plan_sizes(const pb_plan *p, int64_t *num_subcells, int64_t *num_subfaces
                   int64_t *num_subhalffaces, int32_t *max_subfaces_per_node,
                   int32_t *max_subcells_per_node);
 /* Nodes per local-solver class of the classes last built for kind 0 (MPFA, at pb_mpfa_upload) or 1 (MPSA / Biot, at
- * pb_mpsa_upload): counts[2 * cfg + g] for solver configuration cfg (0-7, see csrc/plan.hpp) with the local matrix
- * in shared memory (g = 0) or in a global-memory workspace (g = 1).  counts has 16 entries.  Read-only. */
+ * pb_mpsa_upload): counts[2 * cfg + g] for solver configuration cfg (0-6, see csrc/plan.hpp) with the local matrix
+ * in shared memory (g = 0) or in a global-memory workspace (g = 1).  counts has 14 entries.  Read-only. */
 int pb_plan_class_counts(const pb_plan *p, int kind, int64_t *counts);
 /* Shards: cell e of this plan is cell cells[e] of a larger (global) grid of n_source_cells cells.  The cell tensors of
  * the following pb_mpfa_upload / pb_mpsa_upload (permeability, stiffness, coupling tensors) are then the GLOBAL arrays
@@ -354,7 +354,7 @@ int pb_csr_create(int64_t nrows, int64_t ncols, int64_t nnz, const int32_t *indp
 void pb_csr_destroy(pb_csr *a);
 /* Keep the first nrows rows (a row-partitioned system: the rows of a rank's own cells come first). */
 int pb_csr_truncate_rows(pb_csr *a, int64_t nrows);
-/* lanes per row the SpMV of this matrix runs with (autotuned at creation; POREB200_SPMV_TPR overrides) */
+/* lanes per row the SpMV of this matrix runs with (autotuned at creation) */
 int pb_csr_lanes_per_row(const pb_csr *a);
 /* diagonal (min(nrows, ncols) doubles, host) -- the Jacobi preconditioner of the Krylov solve */
 int pb_csr_diagonal(pb_csr *a, double *diag);

@@ -8,8 +8,7 @@ import os
 import numpy as np
 
 HERE = os.path.dirname(os.path.abspath(__file__))
-# POREB200_LIB: developer knob, path of an alternative build of the same library (A/B timing)
-LIB_PATH = os.environ.get("POREB200_LIB") or os.path.join(HERE, "libporeb200.so")
+LIB_PATH = os.path.join(HERE, "libporeb200.so")
 
 PB_OK, PB_EINVAL, PB_ESINGULAR, PB_ECELLTYPE, PB_ECUDA, PB_ENOTIMPL = range(6)
 BC_INTERIOR, BC_DIR, BC_NEU, BC_ROB = 0, 1, 2, 3

@@ -31,18 +31,16 @@ def needs_build() -> bool:
     return any(os.path.getmtime(d) > t for d in deps)
 
 
-def build(force: bool = False, verbose: bool = False, extra_flags=(), lib: str = LIB) -> str:
-    """``extra_flags`` / ``lib``: developer knobs for A/B variants (e.g. ``-DPB_EXP_ONEBAR`` into
-    ``libporeb200_onebar.so``, selected at run time with ``POREB200_LIB``)."""
-    if not force and not needs_build() and lib == LIB:
+def build(force: bool = False, verbose: bool = False) -> str:
+    if not force and not needs_build():
         return LIB
     # one nvcc process per translation unit, in parallel (the kernel instantiations dominate)
     jobs = []
-    objdir = os.path.join(HERE, "_obj", os.path.basename(lib))
+    objdir = os.path.join(HERE, "_obj", os.path.basename(LIB))
     os.makedirs(objdir, exist_ok=True)
     for src in SOURCES:
         obj = os.path.join(objdir, src.replace(".cu", ".o"))
-        cmd = [_nvcc(), *NVCC_FLAGS, *extra_flags, "-c", os.path.join(CSRC, src), "-o", obj]
+        cmd = [_nvcc(), *NVCC_FLAGS, "-c", os.path.join(CSRC, src), "-o", obj]
         if verbose:
             cmd.insert(1, "-Xptxas=-v")
             print(" ".join(cmd), file=sys.stderr)
@@ -55,9 +53,9 @@ def build(force: bool = False, verbose: bool = False, extra_flags=(), lib: str =
         if proc.returncode:
             raise subprocess.CalledProcessError(proc.returncode, cmd)
         objs.append(obj)
-    subprocess.check_call([_nvcc(), "-shared", "-o", lib, *objs, *GENCODE,
+    subprocess.check_call([_nvcc(), "-shared", "-o", LIB, *objs, *GENCODE,
                            "-Xcompiler", "-fopenmp", "-lgomp"])
-    return lib
+    return LIB
 
 
 if __name__ == "__main__":

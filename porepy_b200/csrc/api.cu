@@ -92,7 +92,6 @@ static int64_t cfg_scratch(int cfg, int n) {
         case 3: return Cfg3::scratch_doubles_c();
         case 4: return Cfg4::scratch_doubles_c();
         case 5: return Cfg5::scratch_doubles_c();
-        case 7: return Cfg7::scratch_doubles_c();
         default: return n;
     }
 }
@@ -101,8 +100,6 @@ static int64_t cfg_scratch(int cfg, int n) {
 template <class F>
 static int build_classes(pb_plan *p, std::vector<NodeClass> &out, F size_of) {
     const HostPlan &H = p->H;
-    const char *alt = getenv("POREB200_CFG4");
-    const bool use7 = alt && strcmp(alt, "reg") == 0;
     // key: cfg*2 + a_global
     std::vector<int32_t> lists[2 * kNumCfg];
     int64_t amax[2 * kNumCfg] = {0}, rmax[2 * kNumCfg] = {0}, smax[2 * kNumCfg] = {0};
@@ -116,7 +113,6 @@ static int build_classes(pb_plan *p, std::vector<NodeClass> &out, F size_of) {
         size_of(nsf, nsc, H.node_nb[s], &n, &w, &a, &r);
         int cfg = 0;
         while (cfg < kCatchAll && (n > kCfg[cfg].max_n || w > kCfg[cfg].max_w)) ++cfg;
-        if (cfg == 4 && use7 && n <= kCfg[7].max_n && w <= kCfg[7].max_w) cfg = 7;
         const int64_t scr = cfg_scratch(cfg, n);
         const int tpb = kCfg[cfg].team == 32 ? 4 : 1;
         bool glob = (size_t)(a + r + scr) * 8 * tpb > kMaxSmem;
@@ -151,7 +147,6 @@ static int build_classes(pb_plan *p, std::vector<NodeClass> &out, F size_of) {
         // nodes of a face are then processed close in time, so the scatter-adds into one face row meet in L2 instead
         // of each paying a DRAM read-modify-write (index order puts the neighbours in the 2nd / 3rd grid direction
         // thousands of regions apart, so that the DRAM traffic grows well above the algorithmic bytes).
-        // POREB200_NODE_ORDER=index disables it.
         if (!p->node_key.empty()) {
             const std::vector<uint32_t> &nk = p->node_key;
             std::stable_sort(lists[key].begin(), lists[key].end(), [&](int32_t x, int32_t y) { return nk[x] < nk[y]; });
@@ -355,6 +350,9 @@ extern "C" int pb_plan_create(int nd, int64_t nc, int64_t nf, int64_t nn, const 
         UP(cn_idx, H.cn_idx) UP(face_cells, H.face_cells)
 #undef UP
         if ((e = fn_idx_dev.upload(fn_indices, (size_t)fn_indptr[nf], st)) != cudaSuccess) return bail("fn_indices", e);
+        if ((e = p->cf_ip.upload(cf_indptr, (size_t)nc + 1, st)) != cudaSuccess) return bail("cf_indptr", e);
+        if ((e = p->cf_ix.upload(cf_indices, (size_t)cf_indptr[nc], st)) != cudaSuccess) return bail("cf_indices", e);
+        if ((e = p->cf_sg.upload(cf_data, (size_t)cf_indptr[nc], st)) != cudaSuccess) return bail("cf_data", e);
     }
     {
         // ---- structural patterns on the device (host fallback when a row has > 256 candidates)
@@ -425,8 +423,7 @@ extern "C" int pb_plan_create(int nd, int64_t nc, int64_t nf, int64_t nn, const 
             {&p->pos_cb, &H.poscb_ptr, &p->poscb_ptr, 3, &p->node_sc_ptr, &p->sc_cell, &p->nbf_ptr, &p->nbf_idx, &p->cb_indptr},
         };
         for (auto &j : jobs) {
-            // + 32 bytes: a 16-byte widened bulk copy of the last node's block may read past the end (PB_EXP_TMA)
-            if ((e = j.pos->ensure((size_t)std::max<int64_t>(1, j.ptr->back()) * sizeof(int32_t) + 32)) != cudaSuccess)
+            if ((e = j.pos->ensure((size_t)std::max<int64_t>(1, j.ptr->back()) * sizeof(int32_t))) != cudaSuccess)
                 return bail("pos map", e);
             const int block = 256;
             int64_t need = (nn * 32 + block - 1) / block;
@@ -653,15 +650,11 @@ extern "C" int pb_plan_set_geometry(pb_plan *p, const double *nodes, const doubl
     cudaStream_t st = p->stream;
     int rc;
     {   // Morton keys of the nodes (10 bits per axis over the bounding box) and re-ordered class lists
-        const char *ord = getenv("POREB200_NODE_ORDER");
-        const bool morton = !(ord && strcmp(ord, "index") == 0);
-        const bool had = !p->node_key.empty();
         double sig = 0.0;   // cheap signature of the coordinates: unchanged geometry keeps the keys and the lists
         for (int64_t i = 0; i < 3 * H.nn; i += 7) sig += nodes[i] * (double)((i % 13) + 1);
-        const bool same = had && morton && sig == p->node_key_sig;
+        const bool same = !p->node_key.empty() && sig == p->node_key_sig;
         p->node_key_sig = sig;
-        if (!same) p->node_key.clear();
-        if (morton && !same) {
+        if (!same) {
             double lo[3], hi[3];
             for (int d = 0; d < 3; ++d) {
                 lo[d] = 1e300; hi[d] = -1e300;
@@ -682,8 +675,6 @@ extern "C" int pb_plan_set_geometry(pb_plan *p, const double *nodes, const doubl
                 }
                 p->node_key[s] = spread(q[0]) | (spread(q[1]) << 1) | (spread(q[2]) << 2);
             }
-        }
-        if (!same && (morton || had)) {
             if ((rc = build_mpfa_classes(p))) return rc;
             p->mpsa_cls_nalpha = -1;   // MPSA / Biot classes are rebuilt (and ordered) at the next upload
         }
@@ -1053,44 +1044,10 @@ extern "C" int pb_mpfa_rhs(pb_plan *p, const pb_values *bound_flux, const pb_val
 // ------------------------------------------------------------------------------------
 // device-side mechanics system  A = div_nd @ stress,  b = -div_nd @ (bound_stress @ bc) + source
 // ------------------------------------------------------------------------------------
-// one warp per face; block layouts as documented at pb_plan_pattern_expanded
-__global__ void div_stress_kernel(int64_t nf, int nd, const int32_t *__restrict__ fc_ip,
-                                  const int32_t *__restrict__ fc_ix, const double *__restrict__ stress,
-                                  const int32_t *__restrict__ face_cells, const int32_t *__restrict__ cc_ip,
-                                  const int32_t *__restrict__ cc_ix, double *__restrict__ a) {
-    const int lane = threadIdx.x & 31;
-    const int64_t warp = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
-    const int64_t nwarps = ((int64_t)gridDim.x * blockDim.x) >> 5;
-    const int nd2 = nd * nd;
-    for (int64_t f = warp; f < nf; f += nwarps) {
-        const int64_t fb = fc_ip[f], flen = fc_ip[f + 1] - fb;
-        for (int sd = 0; sd < 2; ++sd) {
-            const int32_t enc = face_cells[2 * f + sd];
-            if (enc < 0) continue;
-            const int c = enc >> 1;
-            const double sg = (enc & 1) ? -1.0 : 1.0;
-            const int64_t cb = cc_ip[c], clen = cc_ip[c + 1] - cb;
-            for (int64_t t = lane; t < flen * nd2; t += 32) {
-                const int64_t q = t / nd2;
-                const int ij = (int)(t - q * nd2);
-                const int i = ij / nd, j = ij - i * nd;
-                const int k = fc_ix[fb + q];
-                int64_t lo = cb, hi = cb + clen;
-                while (lo < hi) {
-                    const int64_t mid = (lo + hi) >> 1;
-                    if (cc_ix[mid] < k) lo = mid + 1; else hi = mid;
-                }
-                const double v = stress[nd2 * fb + (int64_t)i * nd * flen + q * nd + j];
-                atomicAdd(a + nd2 * cb + (int64_t)i * nd * clen + (lo - cb) * nd + j, sg * v);
-            }
-        }
-    }
-}
-
-// Gather form of the same product, used when the plan holds the cell -> faces lists (device topology build): one warp per
-// cell sums the rows of its faces into the cell's block row in shared memory -- no atomics, one coalesced store of the
-// nd*nd*clen values (the scatter form above issues nd*nd atomics and binary searches per stress entry and side: 20 ms at
-// 10^6 tetrahedra against ~13 GB = 2 ms of compulsory traffic).  Rows longer than `cap` block columns accumulate in place.
+// One warp per cell sums the stress rows of its faces, signed by div[c, f] = cell_faces[f, c], into the cell's block
+// row (layout as documented at pb_plan_pattern_expanded).  Each output row has a single writer, so it is accumulated
+// in shared memory without atomics and stored once, coalesced; the product stays close to its compulsory traffic
+// (~13 GB at 10^6 tetrahedra).  Rows longer than `cap` block columns accumulate in place in global memory.
 template <int WARPS>
 __global__ void __launch_bounds__(WARPS * 32)
     div_stress_gather_kernel(int64_t nc, int nd, const int32_t *__restrict__ cf_ip, const int32_t *__restrict__ cf_ix,
@@ -1178,8 +1135,6 @@ extern "C" int pb_mpsa_system(pb_plan *p, const pb_values *stress, pb_csr **out)
     const HostPlan &H = p->H;
     const int nd = H.nd, nd2 = nd * nd;
     if ((int64_t)p->pat_nnz[2] * nd2 >= 0x7FFFFFFFll) return fail(PB_ENOTIMPL, "system matrix does not fit int32 indices");
-    int rc = ensure_face_cells(p);
-    if (rc) return rc;
     cudaStream_t st = p->stream;
     // block-expanded CELL_CELL pattern on the device
     DevBuf nip, nix;
@@ -1193,21 +1148,14 @@ extern "C" int pb_mpsa_system(pb_plan *p, const pb_values *stress, pb_csr **out)
     CUDA_TRY(cudaGetLastError());
     CUDA_TRY(cudaStreamSynchronize(st));
     pb_csr *a = nullptr;
-    rc = pb_csr_from_device_pattern_(H.nc * nd, H.nc * nd, p->pat_nnz[2] * nd2, nip.as<int32_t>(), nix.as<int32_t>(), &a);
+    int rc = pb_csr_from_device_pattern_(H.nc * nd, H.nc * nd, p->pat_nnz[2] * nd2, nip.as<int32_t>(), nix.as<int32_t>(), &a);
     if (rc) return rc;
-    if (p->cf_ip.p && !getenv("POREB200_DIV_SCATTER")) {
-        constexpr int kWarps = 4, kCap = 128;           // 4 x 128 x 9 doubles = 36 KB of shared memory per block
-        int gridg = (int)std::max<int64_t>(1, std::min<int64_t>((H.nc + kWarps - 1) / kWarps, (int64_t)pb_sm_count() * 24));
-        div_stress_gather_kernel<kWarps><<<gridg, kWarps * 32, (size_t)kWarps * kCap * nd2 * sizeof(double), st>>>(
-            H.nc, nd, p->cf_ip.as<int32_t>(), p->cf_ix.as<int32_t>(), p->cf_sg.as<int8_t>(), p->fc_indptr.as<int32_t>(),
-            p->pat_idx[0].as<int32_t>(), stress_dev, p->cc_indptr.as<int32_t>(), p->pat_idx[2].as<int32_t>(),
-            pb_csr_data_(a), kCap);
-    } else {
-        int grid2 = (int)std::max<int64_t>(1, std::min<int64_t>((H.nf * 32 + block - 1) / block, (int64_t)pb_sm_count() * 16));
-        div_stress_kernel<<<grid2, block, 0, st>>>(H.nf, nd, p->fc_indptr.as<int32_t>(), p->pat_idx[0].as<int32_t>(),
-                                                   stress_dev, p->face_cells.as<int32_t>(),
-                                                   p->cc_indptr.as<int32_t>(), p->pat_idx[2].as<int32_t>(), pb_csr_data_(a));
-    }
+    constexpr int kWarps = 4, kCap = 128;           // 4 x 128 x 9 doubles = 36 KB of shared memory per block
+    int gridg = (int)std::max<int64_t>(1, std::min<int64_t>((H.nc + kWarps - 1) / kWarps, (int64_t)pb_sm_count() * 24));
+    div_stress_gather_kernel<kWarps><<<gridg, kWarps * 32, (size_t)kWarps * kCap * nd2 * sizeof(double), st>>>(
+        H.nc, nd, p->cf_ip.as<int32_t>(), p->cf_ix.as<int32_t>(), p->cf_sg.as<int8_t>(), p->fc_indptr.as<int32_t>(),
+        p->pat_idx[0].as<int32_t>(), stress_dev, p->cc_indptr.as<int32_t>(), p->pat_idx[2].as<int32_t>(),
+        pb_csr_data_(a), kCap);
     g_launches++;
     CUDA_TRY(cudaGetLastError());
     CUDA_TRY(cudaStreamSynchronize(st));

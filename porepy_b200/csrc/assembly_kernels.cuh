@@ -40,57 +40,11 @@ __global__ void __launch_bounds__(Solver::team == 32 ? 128 : Solver::team, Solve
     double *rest = scratch + scr_doubles;
     double *A = a_ws ? a_ws + ((size_t)blockIdx.x * teams_per_block + team_in_block) * a_doubles
                      : rest + rest_doubles;
-#if defined(PB_EXP_TMA)
-    pb::TmaStage ts{};
-    void *tma = nullptr;
-    if (TEAM >= 160 && a_ws == nullptr) {     // one team per CTA with the matrix in shared memory: cfg 3-5
-        double *tail = rest + rest_doubles - (PB_TMA_STAGE_DOUBLES + 4);
-        ts.stage = (int32_t *)(((uintptr_t)tail + 15) & ~(uintptr_t)15);
-        ts.mbar = (uint64_t *)((char *)ts.stage + PB_TMA_STAGE_DOUBLES * 8);
-        ts.parity = 0; ts.off = -1; ts.next_off = -1; ts.dead = false;
-        if (threadIdx.x == 0) {
-            asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" ::"r"(pb::pb_smem_u32(ts.mbar)) : "memory");
-            asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-        }
-        __syncthreads();
-        const int i0 = blockIdx.x * teams_per_block + team_in_block;
-        if (i0 < n_nodes) {
-            const int64_t s0 = nodes[i0];
-            const int nsc0 = P.node_sc_ptr[s0 + 1] - P.node_sc_ptr[s0], nsf0 = P.node_sf_ptr[s0 + 1] - P.node_sf_ptr[s0];
-            pb::pb_tma_issue(ts, P.pos_fc + P.posfc_ptr[s0], nsf0 * nsc0, threadIdx.x == 0);
-            ts.off = ts.next_off;
-        }
-        tma = &ts;
-    }
-#else
-    void *tma = nullptr;
-#endif
     for (int i = blockIdx.x * teams_per_block + team_in_block; i < n_nodes;
-         i += gridDim.x * teams_per_block)
-    {
+         i += gridDim.x * teams_per_block) {
         const int inext = i + gridDim.x * teams_per_block;  // prefetched into L2 during this region's output phase
         const int64_t s_next = inext < n_nodes ? (int64_t)nodes[inext] : -1;
-        mpsa_node<ND, Solver>(t, P, G, prm, o, (int64_t)nodes[i], A, rest, scratch, err, s_next, tma);
-#if defined(PB_EXP_TMA)
-        if (tma) {
-            // the region may have returned early (no sub-faces, singular system): make sure its copy has landed, then
-            // flip the phase parity and launch the copy for the next region (every thread is past its reads of the stage)
-            __syncthreads();
-            if (ts.off >= 0 && !ts.dead) {
-                (void)pb::pb_tma_wait(ts, nullptr);
-                ts.parity ^= 1u;
-            }
-            // every thread must be past its wait on the finished phase before the next copy may complete the FOLLOWING
-            // phase: a warp arriving late would otherwise find the parity it waits for to be the running phase again
-            __syncthreads();
-            if (s_next >= 0) {
-                const int nsc2 = P.node_sc_ptr[s_next + 1] - P.node_sc_ptr[s_next];
-                const int nsf2 = P.node_sf_ptr[s_next + 1] - P.node_sf_ptr[s_next];
-                pb::pb_tma_issue(ts, P.pos_fc + P.posfc_ptr[s_next], nsf2 * nsc2, threadIdx.x == 0);
-            } else ts.next_off = -1;
-            ts.off = ts.next_off;
-        }
-#endif
+        mpsa_node<ND, Solver>(t, P, G, prm, o, (int64_t)nodes[i], A, rest, scratch, err, s_next);
     }
 }
 

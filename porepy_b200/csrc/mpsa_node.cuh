@@ -40,57 +40,8 @@ PB_HD int64_t mpsa_rest_doubles(int nd, int nsf, int nsc, int nb, int nalpha) {
     d += (int64_t)nsc;                          // volk
     d += (int64_t)nalpha * nsc * nd2 * 2;       // NA, AE
     int64_t ints = nsc + 4 * (int64_t)nsf + (int64_t)nsf * nd + n + (int64_t)nsc * nd + 2 * nd;
-#if defined(PB_EXP_TMA)
-    return d + (ints + 1) / 2 + 2 + PB_TMA_STAGE_DOUBLES + 4;   // + bulk-copy stage, mbarrier, alignment slack
-#else
     return d + (ints + 1) / 2 + 2;
-#endif
 }
-
-#if defined(PB_EXP_TMA) && defined(__CUDACC__)
-// Build variant -DPB_EXP_TMA -DPB_TMA_STAGE_DOUBLES=768 (an A/B experiment; NOT the default build):
-// the NEXT region's face x cell position map (nsf * nsc int32, contiguous) is fetched by the TMA engine (cp.async.bulk ->
-// UBLKCP.S.G, completion on an mbarrier) into a shared-memory stage while the region's phases 1-6 run, instead of being
-// read from L2 inside the output phase.  One stage per CTA; the source range is widened to 16-byte boundaries (the plan
-// pads pos_fc), `off` ints are skipped on the shared side.  The L2 prefetch of the default build already hides these
-// loads; whether the extra barrier and the 6 KB of shared memory pay off on H100 is not measured.
-struct TmaStage {
-    int32_t *stage;      // 16-byte aligned, PB_TMA_STAGE_DOUBLES * 8 bytes
-    uint64_t *mbar;
-    uint32_t parity;
-    int off;             // ints to skip in the stage for the region being assembled, -1: not staged
-    int next_off;        // the same for the copy in flight
-    bool dead;
-};
-__device__ __forceinline__ uint32_t pb_smem_u32(const void *p) { return (uint32_t)__cvta_generic_to_shared(p); }
-__device__ __forceinline__ void pb_tma_issue(TmaStage &ts, const int32_t *src, int count, bool leader) {
-    // every thread computes the bookkeeping; the leader issues
-    ts.next_off = -1;
-    if (ts.dead || count <= 0) return;
-    const uintptr_t a = (uintptr_t)src;
-    const uintptr_t a0 = a & ~(uintptr_t)15;
-    const int off = (int)((a - a0) >> 2);
-    const uint32_t bytes = (uint32_t)((((size_t)(off + count) * 4) + 15) & ~(size_t)15);
-    if (bytes > (uint32_t)PB_TMA_STAGE_DOUBLES * 8u) return;
-    ts.next_off = off;
-    if (leader) {
-        asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-        asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(pb_smem_u32(ts.mbar)), "r"(bytes) : "memory");
-        asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
-                     ::"r"(pb_smem_u32(ts.stage)), "l"((const void *)a0), "r"(bytes), "r"(pb_smem_u32(ts.mbar)) : "memory");
-    }
-}
-// wait for the copy of THIS region (bounded: a missed completion falls back to the global loads for good)
-__device__ __forceinline__ const int32_t *pb_tma_wait(TmaStage &ts, const int32_t *fallback) {
-    if (ts.off < 0 || ts.dead) return fallback;
-    uint32_t ok = 0;
-    for (int spin = 0; spin < (1 << 20) && !ok; ++spin)
-        asm volatile("{ .reg .pred p; mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2; selp.u32 %0, 1, 0, p; }"
-                     : "=r"(ok) : "r"(pb_smem_u32(ts.mbar)), "r"(ts.parity) : "memory");
-    if (!ok) { ts.dead = true; return fallback; }
-    return ts.stage + ts.off;
-}
-#endif
 
 // 9-index of the stored (9,9,nc) stiffness for the local (i,r) pair (2-D: rows/cols
 // 2,5,6,7,8 deleted, mpsa.py:1475-1480)
@@ -108,7 +59,7 @@ PB_HD bool sym_mask(int p, int q) {
 template <int ND, class Solver, class Team>
 PB_HD void mpsa_node(Team &t, const PlanView &P, const GeoView &G, const MpsaParams &prm,
                      const MpsaOut &o, int64_t s, double *A, double *smd, double *scratch, int *err,
-                     int64_t s_next = -1, void *tma = nullptr) {
+                     int64_t s_next = -1) {
     constexpr int ND2 = ND * ND;
     const int sc0 = P.node_sc_ptr[s], nsc = P.node_sc_ptr[s + 1] - sc0;
     const int sf0 = P.node_sf_ptr[s], nsf = P.node_sf_ptr[s + 1] - sf0;
@@ -531,9 +482,6 @@ PB_HD void mpsa_node(Team &t, const PlanView &P, const GeoView &G, const MpsaPar
     // ---- phase 7: face rows (traction from the unique side, displacement trace)
     const int32_t *pfc = P.pos_fc + P.posfc_ptr[s];
     const int32_t *pfb = P.pos_fb + P.posfb_ptr[s];
-#if defined(PB_EXP_TMA) && defined(__CUDA_ARCH__)
-    if (tma) pfc = pb_tma_wait(*(TmaStage *)tma, pfc);
-#endif
     // one warp per sub-face, lanes over the right-hand-side columns, the nd components of the
     // row inside: the 9 solution rows of the selected sub-cell and the CSR position are loaded
     // once per (sub-face, column) instead of once per component

@@ -156,172 +156,6 @@ struct SmemGJ {
 };
 
 #if defined(__CUDACC__)
-// Register-tiled Gauss-Jordan.  The team is TR warps; warp w owns the rows {w + TR*x}, lane l
-// the columns {l + 32*y}: every thread keeps an RL x CL tile of the augmented matrix in
-// registers for the whole elimination (cyclic ownership keeps all threads busy while the
-// active part shrinks).  Per pivot step p:
-//   A  the lane that owns column p dumps it (RL values per warp) to shared memory, together
-//      with |value| of the rows that have not been pivots yet;            -- barrier --
-//   B  every warp finds the pivot row from the dumped column (<= 4 shared loads per lane and
-//      one packed-key warp arg-max); the owner warp scales the pivot row and posts it (one
-//      value per owned column);                                            -- barrier --
-//   C  rank-1 update of the tile: the row factors are broadcast shared loads of the dumped
-//      column, RL*CL FMAs against RL + CL shared loads.
-// The column dump is double-buffered (step p+1's dump may overtake slow readers of step p).
-// The loop over 32-column blocks is unrolled so that all register indices are compile-time.
-// Requires n <= TR*RL <= 255 and n + nrhs <= 32*CL.
-#define PB_GJ_CASE(X)                                                  \
-    case X:                                                            \
-        if constexpr (X < RL) {                                        \
-            _Pragma("unroll") for (int y = py; y < CL; ++y) {          \
-                a[X][y] *= inv;                                        \
-                pw[tj + 32 * y] = a[X][y];                             \
-            }                                                          \
-        }                                                              \
-        break;
-
-template <int TR, int RL, int CL, int MINB>
-struct RegGJ {
-    static_assert(RL <= 18, "extend the PB_GJ_CASE list");
-    static_assert(TR * RL <= 255, "row index must fit the 8-bit key field");
-    static constexpr int team = TR * 32;
-    static constexpr int min_blocks = MINB;
-    static constexpr int max_n = TR * RL;
-    static constexpr int max_w = 32 * CL;
-    static constexpr int NP = ((max_n + 31) / 32) * 32;  // padded column length
-    static __host__ __device__ constexpr int64_t scratch_doubles_c() { return 32 * CL + 4 * NP + 2; }
-    static PB_HD int64_t scratch_doubles(int) { return scratch_doubles_c(); }
-
-    template <class Team>
-    static __device__ __forceinline__ bool solve(Team &t, double *A, int n, int W, int nrhs,
-                                                 int *rowidx, double *scratch) {
-        const int ti = t.warp(), tj = t.lane();
-        const int wend = n + nrhs;
-        double a[RL][CL];
-#pragma unroll
-        for (int x = 0; x < RL; ++x)
-#pragma unroll
-            for (int y = 0; y < CL; ++y) {
-                const int r = ti + TR * x, c = tj + 32 * y;
-                a[x][y] = (r < n && c < wend) ? A[r * W + c] : 0.0;
-            }
-        double *pw = scratch;             // [32*CL]  scaled pivot row
-        double *col = pw + 32 * CL;       // [2][NP]  pivot column (factors), by physical row
-        double *cab = col + 2 * NP;       // [2][NP]  |pivot column| of rows still unused, else 0
-        for (int i = t.tid(); i < 4 * NP; i += t.size()) col[i] = 0.0;
-        t.sync();
-        unsigned used = 0;  // bit x: my row x has been a pivot row
-        bool ok = true;
-        // dump of column 0 (step 0's phase A); later dumps are issued as look-ahead inside phase C
-        if (tj == 0) {
-#pragma unroll
-            for (int x = 0; x < RL; ++x) {
-                col[ti + TR * x] = a[x][0];
-                cab[ti + TR * x] = fabs(a[x][0]);
-            }
-        }
-#pragma unroll
-        for (int py = 0; py < CL; ++py) {
-            if (py * 32 >= n) break;
-            for (int pl = 0; pl < 32; ++pl) {
-                const int p = py * 32 + pl;
-                if (p >= n) break;
-                const int buf = p & 1;
-                double *fc = col + buf * NP;
-                double *ca = cab + buf * NP;
-                t.sync();
-                // B: pivot = arg max |column| over unused rows (every warp redundantly)
-                unsigned long long key = 0ull;
-#pragma unroll
-                for (int q = 0; q < NP / 32; ++q) {
-                    unsigned long long k = (unsigned long long)__double_as_longlong(ca[tj + 32 * q]);
-                    k = (k & ~0xFFull) | (unsigned)(tj + 32 * q);
-                    key = k > key ? k : key;
-                }
-#pragma unroll
-                for (int o = 16; o > 0; o >>= 1) {
-                    const unsigned long long k2 = __shfl_xor_sync(0xffffffffu, key, o);
-                    key = k2 > key ? k2 : key;
-                }
-                // zero column, or a NaN / inf pivot magnitude (exponent field all ones): uniform over the team
-                if ((key >> 8) == 0ull || (key >> 52) == 0x7FFull) { ok = false; break; }
-                const int pr = (int)(key & 0xFFull);
-                const int xpiv = (ti == pr % TR) ? pr / TR : -1;
-                if (xpiv >= 0) {
-                    const double inv = 1.0 / fc[pr];
-                    switch (xpiv) {
-                        PB_GJ_CASE(0) PB_GJ_CASE(1) PB_GJ_CASE(2) PB_GJ_CASE(3) PB_GJ_CASE(4)
-                        PB_GJ_CASE(5) PB_GJ_CASE(6) PB_GJ_CASE(7) PB_GJ_CASE(8) PB_GJ_CASE(9)
-                        PB_GJ_CASE(10) PB_GJ_CASE(11) PB_GJ_CASE(12) PB_GJ_CASE(13) PB_GJ_CASE(14)
-                        PB_GJ_CASE(15) PB_GJ_CASE(16) PB_GJ_CASE(17)
-                        default: break;
-                    }
-                    used |= 1u << xpiv;
-                    if (tj == 0) rowidx[p] = pr;
-                }
-                t.sync();
-                // C1: rank-1 update of the pivot's own 32-column block (holds column p+1 as well)
-                double pv[CL];
-#pragma unroll
-                for (int y = py; y < CL; ++y) pv[y] = pw[tj + 32 * y];
-                double fx[RL];
-#pragma unroll
-                for (int x = 0; x < RL; ++x) {
-                    fx[x] = (x != xpiv) ? fc[ti + TR * x] : 0.0;
-                    if (tj > pl) a[x][py] -= fx[x] * pv[py];
-                }
-                // A' (look-ahead): dump column p+1 for the next step when it is in this block
-                const bool la = (pl < 31) && (p + 1 < n);
-                double *fc2 = col + (buf ^ 1) * NP;
-                double *ca2 = cab + (buf ^ 1) * NP;
-                if (la && tj == pl + 1) {
-#pragma unroll
-                    for (int x = 0; x < RL; ++x) {
-                        const double v = a[x][py];
-                        fc2[ti + TR * x] = v;
-                        ca2[ti + TR * x] = ((used >> x) & 1u) ? 0.0 : fabs(v);
-                    }
-                }
-                // C2: the remaining column blocks
-#pragma unroll
-                for (int x = 0; x < RL; ++x) {
-                    if (fx[x] != 0.0) {
-#pragma unroll
-                        for (int y = py + 1; y < CL; ++y) a[x][y] -= fx[x] * pv[y];
-                    }
-                }
-                if (!la && p + 1 < n && tj == 0) {  // first column of the next block
-#pragma unroll
-                    for (int x = 0; x < RL; ++x) {
-                        const double v = a[x][py + 1 < CL ? py + 1 : py];
-                        fc2[ti + TR * x] = v;
-                        ca2[ti + TR * x] = ((used >> x) & 1u) ? 0.0 : fabs(v);
-                    }
-                }
-                if (TR == 1) t.sync();
-            }
-            if (!ok) break;
-        }
-        t.sync();
-        if (!ok) return false;
-#pragma unroll
-        for (int x = 0; x < RL; ++x) {
-            const int r = ti + TR * x;
-            if (r < n) {
-#pragma unroll
-                for (int y = 0; y < CL; ++y) {
-                    const int c = tj + 32 * y;
-                    if (c >= n && c < wend) A[r * W + c] = a[x][y];
-                }
-            }
-        }
-        t.sync();
-        return true;
-    }
-};
-#endif
-
-#if defined(__CUDACC__)
 // Blocked Gauss-Jordan on FP64 tensor cores (DMMA: mma.sync.m16n8k4.f64 on pairs of row tiles, m8n8k4 on an
 // odd one; wgmma has no FP64 type).  The augmented matrix lives in registers as 8x8 accumulator tiles: warp w owns row
 // tile w (8 rows) and all NCT column tiles (2 doubles per lane and tile).  Pivots are taken four

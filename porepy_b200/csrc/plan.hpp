@@ -140,15 +140,14 @@ using Cfg4 = TileGJ<7, 2, 24, 1>;  // team 224 : MPSA tetrahedral nodes (108 x 1
                                    // (TileGJ<14,1,24>: 448 threads, half the tile registers -- measured 7 % slower)
 using Cfg5 = TileGJ<14, 1, 32, 1>; // team 448 : Biot tetrahedral nodes (108 x 205+), DMMA
 using Cfg6 = SmemGJ;               // team 256 : anything else (in-memory Gauss-Jordan)
-using Cfg7 = RegGJ<8, 14, 6, 1>;   // team 256 : scalar register-tiled alternative for cfg 4 (POREB200_CFG4=reg)
 struct SolverCfg { int team, max_n, max_w; };
 static const SolverCfg kCfg[] = {
     {Cfg0::team, Cfg0::max_n, Cfg0::max_w}, {Cfg1::team, Cfg1::max_n, Cfg1::max_w},
     {Cfg2::team, Cfg2::max_n, Cfg2::max_w}, {Cfg3::team, Cfg3::max_n, Cfg3::max_w},
     {Cfg4::team, Cfg4::max_n, Cfg4::max_w}, {Cfg5::team, Cfg5::max_n, Cfg5::max_w},
-    {Cfg6::team, 1 << 30, 1 << 30},         {Cfg7::team, Cfg7::max_n, Cfg7::max_w},
+    {Cfg6::team, 1 << 30, 1 << 30},
 };
-static const int kNumCfg = 8;      // cfg 6 is the catch-all; 7 only by request
+static const int kNumCfg = 7;      // class key cfg * 2 + a_global: pb_plan_class_counts has 2 * kNumCfg entries
 static const int kCatchAll = 6;
 
 struct NodeClass {
@@ -170,7 +169,7 @@ struct pb_plan {
     DevBuf fn_indptr, node_sc_ptr, sc_cell, node_sf_ptr, sf_face, sf_sides, sf_bloc, slot_sf, node_nb,
         sc_ncn, posfc_ptr, posfb_ptr, poscc_ptr, poscb_ptr, pos_fc, pos_fb, pos_cc, pos_cb, fc_indptr,
         fb_indptr, cc_indptr, cb_indptr, pat_idx[4], nbf_ptr, nbf_idx, cn_ptr, cn_idx, face_cells;
-    DevBuf cf_ip, cf_ix, cf_sg;    // cell -> faces (CSC of cell_faces) kept from the device topology build: gather form of div
+    DevBuf cf_ip, cf_ix, cf_sg;    // cell -> faces (CSC of cell_faces): the gather form of div_nd @ stress
     int64_t pat_rows[4] = {0, 0, 0, 0}, pat_cols[4] = {0, 0, 0, 0}, pat_nnz[4] = {0, 0, 0, 0};
     // geometry
     DevBuf nodes, fnorm, fcent, farea, ccent, cvol;
@@ -228,7 +227,6 @@ inline int pb_sm_count() {
         case 3: rc = launch_one(KERNEL<ND, Cfg3>, c, p, __VA_ARGS__); break;        \
         case 4: rc = launch_one(KERNEL<ND, Cfg4>, c, p, __VA_ARGS__); break;        \
         case 5: rc = launch_one(KERNEL<ND, Cfg5>, c, p, __VA_ARGS__); break;        \
-        case 7: rc = launch_one(KERNEL<ND, Cfg7>, c, p, __VA_ARGS__); break;        \
         default: rc = launch_one(KERNEL<ND, Cfg6>, c, p, __VA_ARGS__); break;       \
     }
 

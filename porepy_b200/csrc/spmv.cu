@@ -160,10 +160,6 @@ static int launch_spmv(pb_csr *a, const double *x, double *y, cudaStream_t st) {
 static void autotune_tpr(pb_csr *a) {
     const double mean = a->nrows ? (double)a->nnz / (double)a->nrows : 0.0;
     a->tpr = mean <= 3 ? 2 : mean <= 6 ? 4 : mean <= 24 ? 8 : mean <= 48 ? 16 : 32;
-    if (const char *forced = getenv("POREB200_SPMV_TPR")) {   // developer knob: lanes per row (2, 4, 8, 16, 32)
-        const int t = atoi(forced);
-        if (t == 2 || t == 4 || t == 8 || t == 16 || t == 32) { a->tpr = t; return; }
-    }
     if (a->nnz <= (1 << 20) || mean > 96.0) return;   // long rows: a full warp per row
     // A re-discretization of the same grid (every Newton iteration, every e2e step) recreates a matrix of the same shape:
     // reuse the choice instead of timing 30-40 launches again (6.6 ms per flow system at 10^6 tetrahedra)

@@ -347,7 +347,7 @@ class DevicePlan:
     def class_counts(self, kind: str) -> dict:
         """Nodes per local-solver class of the classes last built for ``kind`` ("mpfa" or "mpsa"):
         {(cfg, a_in_global_memory): count} over the non-empty classes (solver configurations: csrc/plan.hpp)."""
-        counts = np.zeros(16, np.int64)
+        counts = np.zeros(14, np.int64)
         _lib.check(self.lib.pb_plan_class_counts(self.h, {"mpfa": 0, "mpsa": 1}[kind], _lib.ptr(counts, _lib._i64p)))
         return {(k // 2, bool(k & 1)): int(v) for k, v in enumerate(counts) if v}
 

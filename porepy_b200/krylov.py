@@ -331,25 +331,11 @@ def _bicgstab_fused(op: DistributedOperator, b_own, tol, maxiter, diag_own, chec
     carry = 1 if op.loc.rank == 0 else 0
     nred = [0]
 
-    dbg_reduce = os.environ.get("POREB200_KRY_REDUCE", "")
-    dbg_exch = os.environ.get("POREB200_KRY_EXCH", "")
-
     def reduce(lo, hi):
         if world > 1:
             import torch.distributed as dist
-            if dbg_reduce == "clone":
-                tmp = scal[lo:hi].clone()
-                dist.all_reduce(tmp, group=op.group)
-                scal[lo:hi].copy_(tmp)
-            else:
-                dist.all_reduce(scal[lo:hi], group=op.group)
+            dist.all_reduce(scal[lo:hi], group=op.group)
             nred[0] += 1
-
-    def exch(buf):
-        if dbg_exch == "copy" and world > 1:
-            buf.copy_(op.exchange(buf[:n].clone()))
-        else:
-            op.exchange_into(buf)
 
     def iterations(count, it0):
         stream = torch.cuda.current_stream().cuda_stream
@@ -357,11 +343,11 @@ def _bicgstab_fused(op: DistributedOperator, b_own, tol, maxiter, diag_own, chec
             cur = it & 1
             g = 5 * cur
             _lib.check(lib.pb_kry_p(n, P(r), P(p), P(v), P(minv), P(ph), P(scal), cur, bs, stream))
-            exch(xb_p)
+            op.exchange_into(xb_p)
             _lib.check(lib.pb_csr_spmv_dots_dev(csr.h, P(xb_p), P(v), P(rhat), S(g + 0), None, None, stream))
             reduce(g + 0, g + 1)
             _lib.check(lib.pb_kry_s(n, P(r), P(v), P(minv), P(s), P(sh), P(scal), cur, bs, stream))
-            exch(xb_s)
+            op.exchange_into(xb_s)
             _lib.check(lib.pb_csr_spmv_dots_dev(csr.h, P(xb_s), P(t), P(s), S(g + 1), None, S(g + 2), stream))
             reduce(g + 1, g + 3)
             _lib.check(lib.pb_kry_xr(n, P(x), P(ph), P(sh), P(s), P(t), P(r), P(rhat), P(scal), cur, carry, stream))

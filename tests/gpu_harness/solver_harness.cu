@@ -1,6 +1,6 @@
 // solver_harness.cu -- TEST INFRASTRUCTURE ONLY (never loaded by the product).  Runs the dense local solvers of
 // porepy_b200/csrc/node_kernels.cuh on caller-supplied augmented matrices, one kernel per solver configuration
-// Cfg0..Cfg7 of plan.hpp, so that tests/test_zz_local_solvers_gpu.py checks exactly the types the library compiles.
+// Cfg0..Cfg6 of plan.hpp, so that tests/test_zz_local_solvers_gpu.py checks exactly the types the library compiles.
 //
 // The launch mirrors launch_one (plan.hpp) and the assembly kernels (assembly_kernels.cuh): 32-thread teams run four
 // to a 128-thread CTA at per-team offsets of the dynamic shared memory, larger teams one per CTA; the grid is capped
@@ -158,7 +158,6 @@ int sh_fits_shared(int cfg, int max_n, int64_t span) {
         case 4: scr = Cfg4::scratch_doubles_c(); break;
         case 5: scr = Cfg5::scratch_doubles_c(); break;
         case 6: scr = Cfg6::scratch_doubles(max_n); break;
-        case 7: scr = Cfg7::scratch_doubles_c(); break;
         default: return 0;
     }
     const int tpb = kCfg[cfg].team == 32 ? 4 : 1;
@@ -181,7 +180,6 @@ int sh_solve(int cfg, int a_global, int nsys, const int *n, const int *nrhs, con
         case 4: return run<Cfg4>(a_global, nsys, n, nrhs, W, a_off, A, rowidx, ok);
         case 5: return run<Cfg5>(a_global, nsys, n, nrhs, W, a_off, A, rowidx, ok);
         case 6: return run<Cfg6>(a_global, nsys, n, nrhs, W, a_off, A, rowidx, ok);
-        case 7: return run<Cfg7>(a_global, nsys, n, nrhs, W, a_off, A, rowidx, ok);
         default: g_err = "no such configuration"; return 1;
     }
 }

@@ -1,5 +1,5 @@
 """ctypes binding of tests/gpu_harness/_solver_harness.so -- the dense local solvers of the node routines
-(Cfg0..Cfg7 of porepy_b200/csrc/plan.hpp) on caller-supplied systems.  TEST INFRASTRUCTURE ONLY (see
+(Cfg0..Cfg6 of porepy_b200/csrc/plan.hpp) on caller-supplied systems.  TEST INFRASTRUCTURE ONLY (see
 tests/gpu_harness/solver_harness.cu); the product never loads it."""
 from __future__ import annotations
 
@@ -14,7 +14,7 @@ SRC = os.path.join(HERE, "gpu_harness", "solver_harness.cu")
 LIB = os.path.join(HERE, "gpu_harness", "_solver_harness.so")
 ROOT = os.path.dirname(HERE)
 CSRC = os.path.join(ROOT, "porepy_b200", "csrc")
-NUM_CFG = 8
+NUM_CFG = 7
 
 
 def _deps():

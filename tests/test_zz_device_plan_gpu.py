@@ -1,10 +1,12 @@
 """The sub-cell topology plan built on the device (csrc/plan_device.cu) against the host construction
 (csrc/plan_host.hpp, forced with POREB200_HOST_PLAN=1): same patterns and the same discretization matrices on
-hexahedra, tetrahedra (structured and Delaunay), 2-D grids and a grid with boundary-heavy nodes."""
+hexahedra, tetrahedra (structured and Delaunay), 2-D grids and a grid with boundary-heavy nodes, and the same
+mechanics system A = div_nd @ stress assembled on the device from either plan."""
 import os
 
 import numpy as np
 import pytest
+import scipy.sparse as sps
 
 import porepy_b200 as pb
 from cases import flatten, load_case
@@ -66,3 +68,31 @@ def test_device_plan_equals_host_plan_biot(make):
     for key in m_h:
         assert m_d[key].shape == m_h[key].shape
         assert rel_err(m_h[key], m_d[key]) < 1e-12, key
+
+
+@pytest.mark.parametrize("make", [lambda: pb.cart_grid_3d([6, 5, 4], perturb=0.3, seed=2),
+                                  lambda: pb.structured_tet_grid([4, 4, 3])])
+def test_device_mechanics_system_from_host_and_device_plan(make):
+    """pb_mpsa_system gathers each cell's faces through the plan's cell -> face lists, which the host-topology plan
+    uploads itself: the same matrix and pattern from both plans, and the scipy product g.divergence(dim=3) @ stress."""
+    g = make()
+    rng = np.random.default_rng(11)
+    nc = g.num_cells
+    C = pb.FourthOrderTensor(np.exp(0.4 * rng.standard_normal(nc)), np.exp(0.4 * rng.standard_normal(nc)))
+    bf = g.get_all_boundary_faces()
+    vbc = pb.BoundaryConditionVectorial(g, bf[g.face_centers[2, bf] < 1e-10], "dir")
+
+    def run():
+        data = pb.initialize_data({}, "mech", {"fourth_order_tensor": C, "bc": vbc,
+                                               "bc_values": np.zeros(3 * g.num_faces), "source": np.zeros(3 * nc)})
+        d = pb.Mpsa("mech")
+        d.discretize(g, data)
+        a_dev, _ = d.assemble_matrix_rhs_device(g, data)
+        stress = sps.csr_matrix(data[pb.DISCRETIZATION_MATRICES]["mech"]["stress"])
+        return a_dev.to_scipy(), (g.divergence(dim=3) @ stress).tocsr()
+    (a_d, ref_d), (a_h, ref_h) = _both_plans(g, run)
+    assert a_d.shape == a_h.shape == (3 * nc, 3 * nc)
+    assert np.array_equal(a_d.indptr, a_h.indptr) and np.array_equal(a_d.indices, a_h.indices)
+    assert rel_err(a_d, a_h) < 1e-13
+    assert rel_err(ref_d, a_d) < 1e-13
+    assert rel_err(ref_h, a_h) < 1e-13

@@ -1,5 +1,5 @@
-"""The dense local solvers of the node routines (TileGJ / SmemGJ / RegGJ, porepy_b200/csrc/node_kernels.cuh), run
-on their own through tests/gpu_harness for every solver configuration Cfg0..Cfg7 of porepy_b200/csrc/plan.hpp, and
+"""The dense local solvers of the node routines (TileGJ / SmemGJ, porepy_b200/csrc/node_kernels.cuh), run
+on their own through tests/gpu_harness for every solver configuration Cfg0..Cfg6 of porepy_b200/csrc/plan.hpp, and
 compared with an extended-precision reference.
 
 Shapes are those the dispatcher can send a configuration: every (n, nrhs) with n <= max_n and
@@ -384,7 +384,7 @@ def test_team_reuse_across_systems_is_bitwise_stable(cfg):
                    "condition ~1/delta and R, and the update A22 -= A21 R, lose accuracy like 1/delta^2")
 @pytest.mark.parametrize("cfg", TILE_CFGS)
 def test_tilegj_ill_conditioned_schur_complement(cfg):
-    """F4 with a trailing Schur complement delta * C (kappa ~ 1/delta): SmemGJ and RegGJ meet the forward-error bound
+    """F4 with a trailing Schur complement delta * C (kappa ~ 1/delta): SmemGJ meets the forward-error bound
     (test above); the tensor-core configurations do not, by orders of magnitude at delta = 1e-6 and 1e-8."""
     rng = np.random.default_rng(2000 + cfg)
     batch = Batch()

@@ -3,8 +3,8 @@ through a whole discretization and compared with the oracle at the 1e-10 bar of 
 each node is read back with DevicePlan.class_counts: {(solver configuration, A in global memory): nodes}.
 
 On structured tetrahedra an interior MPSA node has 36 sub-faces (n = 108) and 24 sub-cells, so its row width is
-W = (108 + 72 + 24 * n_alpha) | 1: 181 (MPSA, cfg 4, or cfg 7 with POREB200_CFG4=reg), 253 with 3 coupling
-tensors (cfg 5 at the top of its width range) and 277 with 4 (cfg 6; 108 x 277 doubles do not fit shared memory)."""
+W = (108 + 72 + 24 * n_alpha) | 1: 181 (MPSA, cfg 4), 253 with 3 coupling tensors (cfg 5 at the top of its width
+range) and 277 with 4 (cfg 6; 108 x 277 doubles do not fit shared memory)."""
 import numpy as np
 import pytest
 
@@ -82,23 +82,6 @@ def test_five_coupling_tensors_raise():
         pb.Biot("mech").discretize(g, data)
 
 
-def test_mpsa_tet_register_solver_cfg7(monkeypatch):
-    from oracle import fv_oracle as fo
-    monkeypatch.setenv("POREB200_CFG4", "reg")
-    g = pb.structured_tet_grid([3, 3, 3])     # a fresh grid: classes are built once per plan and n_alpha
-    rng = np.random.default_rng(23)
-    nc = g.num_cells
-    C = pb.FourthOrderTensor(np.exp(0.5 * rng.standard_normal(nc)), np.exp(0.5 * rng.standard_normal(nc)))
-    bc = _mixed_vector_bc(g)
-    data = pb.initialize_data({}, "mech", {"fourth_order_tensor": C, "bc": bc})
-    pb.Mpsa("mech").discretize(g, data)
-    ref = fo.mpsa(g, C.values, bc, pb.determine_eta(g))
-    err, key = max_rel_err(ref, data[pb.DISCRETIZATION_MATRICES]["mech"])
-    assert err < TOL, (key, err)
-    counts = _record(g, "mpsa")
-    assert counts.get((7, False), 0) > 0 and (4, False) not in counts, counts
-
-
 def test_mpsa_delaunay_fixture():
     from oracle import fv_oracle as fo
     c = load_case("mpsa_tet3d_delaunay")
@@ -144,10 +127,10 @@ def test_mpfa_and_mpsa_small_meshes():
 # node with n = 3 * nsf > 112 (nsf >= 38 sub-faces) whose A, solver scratch and the rest fit 227 KB, e.g. nsf = 38,
 # nsc = 26 on tetrahedra: 114 x 193 doubles of A plus ~4.9k of the rest, ~27k of 29k doubles.  Such nodes occur on
 # unstructured tetrahedral meshes, but not on the structured meshes here or the 70-cell Delaunay fixture.
-EXPECTED = {(0, False), (1, False), (2, False), (3, False), (4, False), (5, True), (6, True), (7, False)}
+EXPECTED = {(0, False), (1, False), (2, False), (3, False), (4, False), (5, True), (6, True)}
 
 
-def test_every_class_is_reached():
+def test_every_solver_class_is_reached():
     got = set(REACHED["mpfa"]) | set(REACHED["mpsa"])
     print(f"\nreached: mpfa {sorted(REACHED['mpfa'].items())}  mpsa {sorted(REACHED['mpsa'].items())}")
     assert EXPECTED <= got, sorted(EXPECTED - got)

@@ -1,5 +1,5 @@
-"""Where a fused BiCGStab iteration spends its time (one GPU, bench-size flow system): SpMV per lanes-per-row setting,
-the three vector kernels, the SpMV with dot-product epilogue, one graph-replayed block.   python tools/krylov_micro.py"""
+"""Where a fused BiCGStab iteration spends its time (one GPU, bench-size flow system): the SpMV at its
+autotuned lanes per row, the three vector kernels, the SpMV with dot-product epilogue, one graph-replayed block.   python tools/krylov_micro.py"""
 import ctypes as C
 import os
 import sys
@@ -31,14 +31,6 @@ A, b = m.assemble_matrix_rhs(g, d)
 a_dev = A.device_csr
 host = a_dev.to_scipy()
 print("rows", host.shape[0], "nnz", host.nnz, "autotuned lanes per row", lib.pb_csr_lanes_per_row(a_dev.h), flush=True)
-for tpr in (8, 16, 32):
-    os.environ["POREB200_SPMV_TPR"] = str(tpr)
-    a2 = pb.DeviceCsr(host)
-    ms = C.c_float()
-    _lib.check(lib.pb_csr_spmv_bench(a2.h, 50, C.byref(ms)))
-    gbs = (12 * host.nnz + 20 * host.shape[0]) / (ms.value * 1e-3) / 1e9
-    print(f"lanes per row {tpr:2d}: {ms.value:.4f} ms  {gbs:.0f} GB/s algorithmic", flush=True)
-del os.environ["POREB200_SPMV_TPR"]
 
 n = host.shape[0]
 dev = torch.device("cuda")

@@ -308,6 +308,32 @@ int pb_facegrid_set_face_areas(pb_facegrid *g, const double *face_areas);
 int pb_tpsa(pb_facegrid *g, int nd, const double *mu, const uint8_t *codes, const double *robin_diag,
             const uint8_t *face_flags, const int32_t *fc_indptr, double **out, float *kernel_ms);
 
+/* The linear system of the TPSA three-field elasticity model (csrc/tpsa_system.cuh; reference
+ * models/momentum_balance.py:82-106, 250-280, 344-368 and models/constitutive_laws.py:3064-3296) on one grid without
+ * fractures, assembled on the device:
+ *   momentum     -div_nd (S_u u + S_r r + S_p p + B_s g)               - f   = 0
+ *   angular      -vol/mu r + div_nr (R_u u + R_r r + B_r g)            - s_r = 0
+ *   solid mass   -vol/lambda p + div (M_u u + M_p p + B_m g)           - s_p = 0
+ * with the PB_TPSA_* terms above (S_u = STRESS, S_r = STRESS_ROTATION, S_p = STRESS_TOTAL_PRESSURE, R_u =
+ * ROTATION_DISPLACEMENT, R_r = ROTATION_ROTATION, M_u = SOLID_MASS_DISPLACEMENT, M_p = SOLID_MASS_TOTAL_PRESSURE, B_s =
+ * BOUND_STRESS, B_r = BOUND_ROTATION_DISPLACEMENT, B_m = BOUND_MASS_DISPLACEMENT) and div = cell_faces^T.  Unknowns and
+ * equations are numbered cell by cell, [u_c (nd), r_c (nr), p_c]: row / column c*(nd+nr+1) + l, so the diagonal
+ * (nd+nr+1)^2 blocks are the cell blocks.  Only the structurally non-zero entries are stored (u-u diagonal, r-p and p-r
+ * zero: 37 of 49 entries per block in 3-D, 12 of 16 in 2-D); rows are sorted.
+ * pb_tpsa_system: A as a new device CSR.  mu, codes, robin_diag, face_flags as for pb_tpsa; lambda (nc): the first
+ * Lame parameter, finite and > 0; cell_volumes (nc).  Host pointers.  The face areas must have been set.  The row
+ * pattern is built on the device at the first call for a dimension and kept on the handle; the face values of the
+ * last call stay on the handle for pb_tpsa_rhs.  No atomics: two calls give bit-identical values.  stage_ms (may be
+ * NULL): device times of the face kernel and of the row gather, 2 floats.
+ * pb_tpsa_rhs: b = -R(0) of the system last assembled on g, written to the DEVICE array rhs_dev (nc*(nd+nr+1)).
+ * bc_values: nd*nf face-major (the model's combined mechanical boundary operator); body_force (nd*nc), angular_source
+ * (nr*nc), mass_source (nc): cell-major host arrays, each may be NULL (zero). */
+int pb_tpsa_system(pb_facegrid *g, int nd, const double *mu, const double *lambda, const double *cell_volumes,
+                   const uint8_t *codes, const double *robin_diag, const uint8_t *face_flags, struct pb_csr **out,
+                   float *stage_ms);
+int pb_tpsa_rhs(pb_facegrid *g, const double *bc_values, const double *body_force, const double *angular_source,
+                const double *mass_source, double *rhs_dev);
+
 /* Interface upwinding (UpwindCoupling.discretize, numerics/fv/upwind.py:427-528): per mortar cell the sign of the
  * interface flux and the masks "upstream is the higher-dimensional side" / "... the lower-dimensional side".
  * Host pointers, n doubles each. */
@@ -390,13 +416,15 @@ int pb_csr_spmv_dots_dev(pb_csr *a, const double *x_dev, double *y_dev, const do
 int pb_kry_init(int64_t n, const double *b, double *x, double *r, double *rhat, double *p, double *v, double *scal,
                 double tol, uint64_t stream);
 int pb_kry_seed(double *scal, uint64_t stream);
-/* minv / bs: the preconditioner M^-1 -- bs = 1: inverse diagonal (n doubles, Jacobi); bs = 2, 3: inverted bs x bs
- * diagonal blocks, row-major (n/bs blocks; block Jacobi over the displacement components of a cell); NULL: none */
+/* minv / bs: the preconditioner M^-1 -- bs = 1: inverse diagonal (n doubles, Jacobi); bs = 2, 3, 4, 7: inverted bs x bs
+ * diagonal blocks, row-major (n/bs blocks; block Jacobi over the unknowns of a cell: the displacement components of
+ * the MPSA system (2, 3) or [u, r, p] of the TPSA system (4 in 2-D, 7 in 3-D)); NULL: none */
 int pb_kry_p(int64_t n, const double *r, double *p, const double *v, const double *minv, double *ph, double *scal,
              int cur, int bs, uint64_t stream);
 int pb_kry_s(int64_t n, const double *r, const double *v, const double *minv, double *s, double *sh, double *scal,
              int cur, int bs, uint64_t stream);
-/* inverses of the first nblocks bs x bs diagonal blocks of a device CSR, to a DEVICE array (nblocks*bs*bs doubles) */
+/* inverses of the first nblocks bs x bs diagonal blocks of a device CSR, to a DEVICE array (nblocks*bs*bs doubles);
+ * bs in {1, 2, 3, 4, 7}.  A singular block is replaced by the inverse of its diagonal (1 where that entry is 0). */
 int pb_csr_block_diag_inv_dev(const pb_csr *a, int bs, int64_t nblocks, double *out_dev, uint64_t stream);
 int pb_kry_xr(int64_t n, double *x, const double *ph, const double *sh, const double *s, const double *t, double *r,
               const double *rhat, double *scal, int cur, int carry /* 1 on exactly one rank */, uint64_t stream);

@@ -69,6 +69,9 @@ _SIGNATURES = {
     "pb_upwind": (C.c_int, [C.c_void_p, _f64p, _u8p, _i32p, _f64p, _f64p]),
     "pb_facegrid_set_face_areas": (C.c_int, [C.c_void_p, _f64p]),
     "pb_tpsa": (C.c_int, [C.c_void_p, C.c_int, _f64p, _u8p, _f64p, _u8p, _i32p, C.POINTER(_f64p), _f32p]),
+    "pb_tpsa_system": (C.c_int, [C.c_void_p, C.c_int, _f64p, _f64p, _f64p, _u8p, _f64p, _u8p, C.POINTER(C.c_void_p),
+                                 _f32p]),
+    "pb_tpsa_rhs": (C.c_int, [C.c_void_p, _f64p, _f64p, _f64p, _f64p, C.c_void_p]),
     "pb_upwind_coupling": (C.c_int, [C.c_int64, _f64p, _f64p, _f64p, _f64p]),
     "pb_compute_geometry_3d": (C.c_int, [C.c_int64, C.c_int64, C.c_int64, _i32p, _i32p, _i8p, _i32p, _i32p] + [_f64p] * 6
                                + [_f32p]),

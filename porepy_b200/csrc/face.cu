@@ -5,12 +5,22 @@
 #include "plan.hpp"
 #include "tpfa_diff.cuh"
 #include "tpsa_face.cuh"
+#include "tpsa_system.cuh"
+
+#include <cub/device/device_scan.cuh>
 
 struct pb_facegrid {
     int64_t nc = 0, nf = 0;
     cudaStream_t stream = nullptr;
     DevBuf face_cells, fnorm, fcent, ccent, farea, tmp;   // farea: set by pb_facegrid_set_face_areas
+    DevBuf cf_ip, cf_ix;                                  // cell -> face lists (cell_faces, CSC)
+    std::vector<uint8_t> face_ncell;                      // host: cells per face
     GeoView geo{};
+    // TPSA system (pb_tpsa_system): the row pattern, built once per topology and dimension, and the face values of
+    // the last assembly (read again by pb_tpsa_rhs)
+    int sys_nd = 0, terms_nd = 0;
+    int64_t sys_nnz = 0, sys_npairs = 0;
+    DevBuf fc_ptr, cc_ptr, cc_ix, cc_cell, sys_ip, sys_ix, terms[PB_TPSA_NTERMS];
 };
 
 // one thread per cell: claim the first free slot of each of its faces
@@ -41,15 +51,19 @@ extern "C" int pb_facegrid_create(int64_t nc, int64_t nf, const int32_t *cf_indp
     int ndev = 0;
     if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev < 1)
         return pb_fail_(PB_ECUDA, "no CUDA device: libporeb200 has no CPU path");
-    for (int64_t q = 0; q < cf_indptr[nc]; ++q)
+    std::vector<uint8_t> ncell((size_t)nf, 0);
+    for (int64_t q = 0; q < cf_indptr[nc]; ++q) {
         if (cf_indices[q] < 0 || cf_indices[q] >= nf) return pb_fail_(PB_EINVAL, "cell_faces index out of range");
+        if (ncell[cf_indices[q]] < 255) ++ncell[cf_indices[q]];
+    }
     pb_facegrid *g = new pb_facegrid;
     g->nc = nc; g->nf = nf;
+    g->face_ncell.swap(ncell);
     auto bail = [&](int rc) { pb_facegrid_destroy(g); return rc; };
 #define FG_TRY(x) do { cudaError_t e_ = (x); if (e_ != cudaSuccess) return bail(pb_fail_(PB_ECUDA, std::string(#x) + ": " + cudaGetErrorString(e_))); } while (0)
     FG_TRY(cudaStreamCreateWithFlags(&g->stream, cudaStreamNonBlocking));
     cudaStream_t st = g->stream;
-    DevBuf ip, ix, da, bad;
+    DevBuf &ip = g->cf_ip, &ix = g->cf_ix, da, bad;
     FG_TRY(ip.upload(cf_indptr, (size_t)nc + 1, st));
     FG_TRY(ix.upload(cf_indices, (size_t)cf_indptr[nc], st));
     FG_TRY(da.upload(cf_data, (size_t)cf_indptr[nc], st));
@@ -316,5 +330,257 @@ extern "C" int pb_tpsa(pb_facegrid *g, int nd, const double *mu, const uint8_t *
         if (out[k]) CUDA_TRY(cudaMemcpyAsync(out[k], o_buf[k].p, count[k] * sizeof(double), cudaMemcpyDeviceToHost, st));
     CUDA_TRY(cudaStreamSynchronize(st));
     if (kernel_ms) CUDA_TRY(cudaEventElapsedTime(kernel_ms, ev.e0, ev.e1));
+    return PB_OK;
+}
+
+// ---- TPSA three-field system (tpsa_system.cuh) -----------------------------------------------------------------
+struct pb_csr;
+int pb_csr_from_device_pattern_(int64_t nrows, int64_t ncols, int64_t nnz, const int32_t *indptr_dev,
+                                const int32_t *indices_dev, pb_csr **out);   // spmv.cu
+double *pb_csr_data_(pb_csr *a);                                              // spmv.cu
+
+__global__ void tpsa_nb_count_kernel(TpsaTopo t, int32_t *__restrict__ count, int *bad) {
+    for (int64_t c = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; c < t.nc; c += (int64_t)gridDim.x * blockDim.x) {
+        int32_t nb[kTpsaMaxNb];
+        int n = tpsa_cell_neighbours(c, t, nb);
+        if (n < 0) { atomicExch(bad, 1); n = 0; }
+        count[c] = n;
+    }
+}
+
+template <int ND>
+__global__ void tpsa_pattern_kernel(TpsaTopo t, const int32_t *__restrict__ cc_ptr, int32_t *__restrict__ cc_ix,
+                                    int32_t *__restrict__ cc_cell, int32_t *__restrict__ ip, int32_t *__restrict__ ix) {
+    for (int64_t c = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; c < t.nc; c += (int64_t)gridDim.x * blockDim.x) {
+        int32_t nb[kTpsaMaxNb];
+        const int n = tpsa_cell_neighbours(c, t, nb);
+        for (int j = 0; j < n; ++j) { cc_ix[cc_ptr[c] + j] = nb[j]; cc_cell[cc_ptr[c] + j] = (int32_t)c; }
+        tpsa_pattern_rows<ND>(c, n, nb, cc_ptr[c], ip, ix);
+    }
+}
+
+// one thread per block (c, k) of A, i.e. per entry of the neighbour lists: consecutive threads write consecutive
+// segments of the same rows
+template <int ND>
+__global__ void tpsa_system_kernel(int64_t npairs, TpsaTopo t, const int32_t *__restrict__ cc_ptr,
+                                   const int32_t *__restrict__ cc_ix, const int32_t *__restrict__ cc_cell, TpsaTerms T,
+                                   const double *__restrict__ mu, const double *__restrict__ lam,
+                                   const double *__restrict__ vol, double *__restrict__ a) {
+    for (int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; e < npairs; e += (int64_t)gridDim.x * blockDim.x) {
+        const int64_t c = cc_cell[e];
+        tpsa_system_block<ND>(c, (int)(e - cc_ptr[c]), t, cc_ptr, cc_ix, T, mu, lam, vol, a);
+    }
+}
+
+template <int ND>
+__global__ void tpsa_rhs_kernel(TpsaTopo t, TpsaTerms T, const double *__restrict__ g, const double *__restrict__ f,
+                                const double *__restrict__ sr, const double *__restrict__ sp, double *__restrict__ b) {
+    constexpr int NR = TpsaDims<ND>::NR, B = TpsaDims<ND>::B;
+    for (int64_t q = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; q < t.nc * B; q += (int64_t)gridDim.x * blockDim.x) {
+        const int64_t c = q / B;
+        const int l = (int)(q - c * B);
+        const double src = l < ND ? (f ? f[c * ND + l] : 0.0)
+                                   : (l < ND + NR ? (sr ? sr[c * NR + l - ND] : 0.0) : (sp ? sp[c] : 0.0));
+        b[q] = tpsa_rhs_row<ND>(c, l, t, T, g, src);
+    }
+}
+
+static int fg_grid(int64_t n) {
+    return (int)std::max<int64_t>(1, std::min<int64_t>((n + 255) / 256, (int64_t)pb_sm_count() * 16));
+}
+
+static TpsaTopo tpsa_topo(pb_facegrid *g) {
+    return TpsaTopo{g->nc, g->cf_ip.as<int32_t>(), g->cf_ix.as<int32_t>(), g->face_cells.as<int32_t>(),
+                    g->fc_ptr.as<int32_t>()};
+}
+
+// Row pattern of the system for dimension nd: neighbour lists, block-row offsets and the CSR arrays of A.
+static int tpsa_build_pattern(pb_facegrid *g, int nd) {
+    cudaStream_t st = g->stream;
+    const int64_t nc = g->nc;
+    const int B = nd == 3 ? 7 : 4, NZ = nd == 3 ? 37 : 12;
+    const TpsaTopo t = tpsa_topo(g);
+    DevBuf count, bad, scratch;
+    CUDA_TRY(count.ensure((size_t)(nc + 1) * sizeof(int32_t)));
+    CUDA_TRY(bad.ensure(sizeof(int)));
+    CUDA_TRY(cudaMemsetAsync(bad.p, 0, sizeof(int), st));
+    CUDA_TRY(cudaMemsetAsync(count.as<int32_t>() + nc, 0, sizeof(int32_t), st));
+    tpsa_nb_count_kernel<<<fg_grid(nc), 256, 0, st>>>(t, count.as<int32_t>(), bad.as<int>());
+    pb_count_launch_();
+    CUDA_TRY(cudaGetLastError());
+    CUDA_TRY(g->cc_ptr.ensure((size_t)(nc + 1) * sizeof(int32_t)));
+    size_t tmp_bytes = 0;
+    CUDA_TRY(cub::DeviceScan::ExclusiveSum(nullptr, tmp_bytes, count.as<int32_t>(), g->cc_ptr.as<int32_t>(),
+                                           (int)(nc + 1), st));
+    CUDA_TRY(scratch.ensure(tmp_bytes));
+    CUDA_TRY(cub::DeviceScan::ExclusiveSum(scratch.p, tmp_bytes, count.as<int32_t>(), g->cc_ptr.as<int32_t>(),
+                                           (int)(nc + 1), st));
+    int hbad = 0;
+    int32_t total = 0;
+    CUDA_TRY(cudaMemcpyAsync(&hbad, bad.p, sizeof(int), cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(cudaMemcpyAsync(&total, g->cc_ptr.as<int32_t>() + nc, sizeof(int32_t), cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(cudaStreamSynchronize(st));
+    if (hbad) return pb_fail_(PB_ENOTIMPL, "Tpsa system: a cell has more than 31 face neighbours");
+    const int64_t nnz = (int64_t)NZ * total;
+    if (nnz >= 0x7FFFFFFFll) return pb_fail_(PB_ENOTIMPL, "Tpsa system: the matrix does not fit int32 indices");
+    CUDA_TRY(g->cc_ix.ensure((size_t)std::max<int64_t>(1, total) * sizeof(int32_t)));
+    CUDA_TRY(g->cc_cell.ensure((size_t)std::max<int64_t>(1, total) * sizeof(int32_t)));
+    CUDA_TRY(g->sys_ip.ensure((size_t)(nc * B + 1) * sizeof(int32_t)));
+    CUDA_TRY(g->sys_ix.ensure((size_t)std::max<int64_t>(1, nnz) * sizeof(int32_t)));
+    const int32_t last = (int32_t)nnz;
+    CUDA_TRY(cudaMemcpyAsync(g->sys_ip.as<int32_t>() + nc * B, &last, sizeof(int32_t), cudaMemcpyHostToDevice, st));
+    if (nd == 3)
+        tpsa_pattern_kernel<3><<<fg_grid(nc), 256, 0, st>>>(t, g->cc_ptr.as<int32_t>(), g->cc_ix.as<int32_t>(),
+                                                             g->cc_cell.as<int32_t>(), g->sys_ip.as<int32_t>(),
+                                                             g->sys_ix.as<int32_t>());
+    else
+        tpsa_pattern_kernel<2><<<fg_grid(nc), 256, 0, st>>>(t, g->cc_ptr.as<int32_t>(), g->cc_ix.as<int32_t>(),
+                                                             g->cc_cell.as<int32_t>(), g->sys_ip.as<int32_t>(),
+                                                             g->sys_ix.as<int32_t>());
+    pb_count_launch_();
+    CUDA_TRY(cudaGetLastError());
+    CUDA_TRY(cudaStreamSynchronize(st));
+    g->sys_nd = nd;
+    g->sys_nnz = nnz;
+    g->sys_npairs = total;
+    return PB_OK;
+}
+
+struct FgEvents {
+    cudaEvent_t e[3] = {nullptr, nullptr, nullptr};
+    ~FgEvents() { for (auto x : e) if (x) cudaEventDestroy(x); }
+};
+
+extern "C" int pb_tpsa_system(pb_facegrid *g, int nd, const double *mu, const double *lambda,
+                              const double *cell_volumes, const uint8_t *codes, const double *robin_diag,
+                              const uint8_t *face_flags, pb_csr **out, float *stage_ms) {
+    if (!g || !mu || !lambda || !cell_volumes || !codes || !face_flags || !out)
+        return pb_fail_(PB_EINVAL, "null pointer");
+    if (nd != 2 && nd != 3) return pb_fail_(PB_EINVAL, "Tpsa is only implemented for 2d and 3d grids.");
+    if (!g->geo.farea) return pb_fail_(PB_EINVAL, "face areas not set (pb_facegrid_set_face_areas)");
+    const int64_t nf = g->nf, nc = g->nc;
+    for (int64_t c = 0; c < nc; ++c) {
+        if (!(mu[c] > 0.0) || !std::isfinite(mu[c])) return pb_fail_(PB_EINVAL, "shear modulus must be finite and > 0");
+        if (!(lambda[c] > 0.0) || !std::isfinite(lambda[c]))
+            return pb_fail_(PB_EINVAL, "first Lame parameter lambda must be finite and > 0");
+    }
+    bool any_rob = false;
+    for (int64_t q = 0; q < nd * nf; ++q) {
+        if (codes[q] > PB_BC_ROB) return pb_fail_(PB_EINVAL, "boundary code out of range");
+        any_rob |= codes[q] == PB_BC_ROB;
+    }
+    if (any_rob && !robin_diag) return pb_fail_(PB_EINVAL, "Robin faces need robin_diag");
+    for (int64_t f = 0; f < nf; ++f) {
+        const int len = g->face_ncell[f];
+        if (len < 1 || len > 2) return pb_fail_(PB_EINVAL, "fc_indptr: a face has one or two cells");
+        if (face_flags[f] && len != 1) return pb_fail_(PB_EINVAL, "sign of internal faces does not make sense");
+    }
+    cudaStream_t st = g->stream;
+    if (!g->fc_ptr.p) {   // CSR-by-face row pointer of cell_faces: where each face's (face, cell) values start
+        std::vector<int32_t> fp((size_t)nf + 1, 0);
+        for (int64_t f = 0; f < nf; ++f) fp[f + 1] = fp[f] + g->face_ncell[f];
+        CUDA_TRY(g->fc_ptr.upload(fp, st));
+        CUDA_TRY(cudaStreamSynchronize(st));
+    }
+    if (g->sys_nd != nd) {
+        g->sys_nd = 0;
+        int rc = tpsa_build_pattern(g, nd);
+        if (rc) return rc;
+    }
+    // stage 1: the ten face terms the system reads, kept on the handle
+    int64_t nfc = 0;   // (face, cell) entries
+    for (int64_t f = 0; f < nf; ++f) nfc += g->face_ncell[f];
+    const size_t nr = nd == 3 ? 3 : 1;
+    const size_t per[PB_TPSA_NTERMS] = {(size_t)nd, nd * nr, (size_t)nd, nr * nd, nr * nr, (size_t)nd, 1, (size_t)nd,
+                                        nd * nr, (size_t)nd, (size_t)nd, nr * nd, (size_t)nd, (size_t)nd};
+    const bool used[PB_TPSA_NTERMS] = {true, true, true, true, true, true, true, false, false, false, true, true, true,
+                                       false};
+    TpsaOut o{};
+    TpsaTerms T{};
+    for (int k = 0; k < PB_TPSA_NTERMS; ++k) {
+        if (!used[k]) continue;
+        CUDA_TRY(g->terms[k].ensure(per[k] * (k < PB_TPSA_BOUND_STRESS ? (size_t)nfc : (size_t)nf) * sizeof(double)));
+        o.t[k] = g->terms[k].as<double>();
+        T.t[k] = o.t[k];
+    }
+    DevBuf dmu, dlam, dvol, dcodes, drob, dflags;
+    CUDA_TRY(dmu.upload(mu, (size_t)nc, st));
+    CUDA_TRY(dlam.upload(lambda, (size_t)nc, st));
+    CUDA_TRY(dvol.upload(cell_volumes, (size_t)nc, st));
+    CUDA_TRY(dcodes.upload(codes, (size_t)nd * nf, st));
+    if (any_rob) CUDA_TRY(drob.upload(robin_diag, (size_t)nd * nf, st));
+    CUDA_TRY(dflags.upload(face_flags, (size_t)nf, st));
+    pb_csr *a = nullptr;
+    int rc = pb_csr_from_device_pattern_(nc * (nd == 3 ? 7 : 4), nc * (nd == 3 ? 7 : 4), g->sys_nnz,
+                                         g->sys_ip.as<int32_t>(), g->sys_ix.as<int32_t>(), &a);
+    if (rc) return rc;
+    FgEvents ev;
+    auto fail_cuda = [&](cudaError_t e, const char *what) {
+        pb_csr_destroy(a);
+        return pb_fail_(PB_ECUDA, std::string(what) + ": " + cudaGetErrorString(e));
+    };
+#define SYS_TRY(x) do { cudaError_t e_ = (x); if (e_ != cudaSuccess) return fail_cuda(e_, #x); } while (0)
+    if (stage_ms)
+        for (auto &x : ev.e) SYS_TRY(cudaEventCreate(&x));
+    if (stage_ms) SYS_TRY(cudaEventRecord(ev.e[0], st));
+    const double *rw = any_rob ? drob.as<double>() : nullptr;
+    const TpsaTopo t = tpsa_topo(g);
+    if (nd == 3)
+        tpsa_kernel<3><<<fg_grid(nf), 256, 0, st>>>(nf, g->geo, dmu.as<double>(), dcodes.as<uint8_t>(), rw,
+                                                     dflags.as<uint8_t>(), g->face_cells.as<int32_t>(), t.fc_ptr, o);
+    else
+        tpsa_kernel<2><<<fg_grid(nf), 256, 0, st>>>(nf, g->geo, dmu.as<double>(), dcodes.as<uint8_t>(), rw,
+                                                     dflags.as<uint8_t>(), g->face_cells.as<int32_t>(), t.fc_ptr, o);
+    pb_count_launch_();
+    SYS_TRY(cudaGetLastError());
+    if (stage_ms) SYS_TRY(cudaEventRecord(ev.e[1], st));
+    // stage 2: every block of A gathered from the faces of its cell
+    const int64_t np = g->sys_npairs;
+    if (nd == 3)
+        tpsa_system_kernel<3><<<fg_grid(np), 256, 0, st>>>(np, t, g->cc_ptr.as<int32_t>(), g->cc_ix.as<int32_t>(),
+                                                            g->cc_cell.as<int32_t>(), T, dmu.as<double>(),
+                                                            dlam.as<double>(), dvol.as<double>(), pb_csr_data_(a));
+    else
+        tpsa_system_kernel<2><<<fg_grid(np), 256, 0, st>>>(np, t, g->cc_ptr.as<int32_t>(), g->cc_ix.as<int32_t>(),
+                                                            g->cc_cell.as<int32_t>(), T, dmu.as<double>(),
+                                                            dlam.as<double>(), dvol.as<double>(), pb_csr_data_(a));
+    pb_count_launch_();
+    SYS_TRY(cudaGetLastError());
+    if (stage_ms) SYS_TRY(cudaEventRecord(ev.e[2], st));
+    SYS_TRY(cudaStreamSynchronize(st));
+    if (stage_ms) {
+        SYS_TRY(cudaEventElapsedTime(stage_ms, ev.e[0], ev.e[1]));
+        SYS_TRY(cudaEventElapsedTime(stage_ms + 1, ev.e[1], ev.e[2]));
+    }
+#undef SYS_TRY
+    g->terms_nd = nd;
+    *out = a;
+    return PB_OK;
+}
+
+extern "C" int pb_tpsa_rhs(pb_facegrid *g, const double *bc_values, const double *body_force,
+                           const double *angular_source, const double *mass_source, double *rhs_dev) {
+    if (!g || !bc_values || !rhs_dev) return pb_fail_(PB_EINVAL, "null pointer");
+    const int nd = g->terms_nd;
+    if (nd != 2 && nd != 3) return pb_fail_(PB_EINVAL, "pb_tpsa_system has not been called");
+    const int64_t nf = g->nf, nc = g->nc;
+    const int nr = nd == 3 ? 3 : 1;
+    cudaStream_t st = g->stream;
+    DevBuf dg, df, dsr, dsp;
+    CUDA_TRY(dg.upload(bc_values, (size_t)nd * nf, st));
+    if (body_force) CUDA_TRY(df.upload(body_force, (size_t)nd * nc, st));
+    if (angular_source) CUDA_TRY(dsr.upload(angular_source, (size_t)nr * nc, st));
+    if (mass_source) CUDA_TRY(dsp.upload(mass_source, (size_t)nc, st));
+    TpsaTerms T{};
+    for (int k = PB_TPSA_BOUND_STRESS; k <= PB_TPSA_BOUND_MASS_DISPLACEMENT; ++k) T.t[k] = g->terms[k].as<double>();
+    const TpsaTopo t = tpsa_topo(g);
+    const int64_t rows = nc * (nd + nr + 1);
+    const double *pf = body_force ? df.as<double>() : nullptr, *psr = angular_source ? dsr.as<double>() : nullptr,
+                 *psp = mass_source ? dsp.as<double>() : nullptr;
+    if (nd == 3) tpsa_rhs_kernel<3><<<fg_grid(rows), 256, 0, st>>>(t, T, dg.as<double>(), pf, psr, psp, rhs_dev);
+    else tpsa_rhs_kernel<2><<<fg_grid(rows), 256, 0, st>>>(t, T, dg.as<double>(), pf, psr, psp, rhs_dev);
+    pb_count_launch_();
+    CUDA_TRY(cudaGetLastError());
+    CUDA_TRY(cudaStreamSynchronize(st));
     return PB_OK;
 }

@@ -57,7 +57,8 @@ __global__ void kry_init_kernel(int64_t n, const double *__restrict__ b, double 
 
 // Preconditioner application z = M^-1 y on one block of BS consecutive entries: BS == 1 -- minv holds the inverse
 // diagonal (Jacobi); BS > 1 -- minv holds the inverted BS x BS diagonal blocks, row-major (block Jacobi: the nd
-// displacement components of a cell in the mechanics system A = div_nd @ stress).
+// displacement components of a cell in the mechanics system A = div_nd @ stress, or the nd + nr + 1 unknowns [u, r, p]
+// of a cell in the TPSA system, BS = 4 in 2-D and 7 in 3-D).
 template <int BS>
 __device__ __forceinline__ void apply_minv(const double *__restrict__ minv, int64_t b, const double (&y)[BS], double (&z)[BS]) {
     if (!minv) {
@@ -179,32 +180,40 @@ extern "C" int pb_kry_seed(double *scal, uint64_t stream) {
     CUDA_TRY(cudaGetLastError());
     return PB_OK;
 }
-// bs: size of the diagonal blocks of the preconditioner (1 = Jacobi, 2 / 3 = block Jacobi; n must be a multiple)
+static bool kry_block_size_ok(int bs) { return bs == 1 || bs == 2 || bs == 3 || bs == 4 || bs == 7; }
+
+// bs: size of the diagonal blocks of the preconditioner (1 = Jacobi, 2 / 3 / 4 / 7 = block Jacobi; n must be a multiple)
 extern "C" int pb_kry_p(int64_t n, const double *r, double *p, const double *v, const double *minv, double *ph,
                         double *scal, int cur, int bs, uint64_t stream) {
-    if (bs < 1 || bs > 3 || n % bs) return pb_fail_(PB_EINVAL, "pb_kry_p: block size must be 1, 2 or 3 and divide n");
+    if (!kry_block_size_ok(bs) || n % bs)
+        return pb_fail_(PB_EINVAL, "pb_kry_p: block size must be 1, 2, 3, 4 or 7 and divide n");
     cudaStream_t st = (cudaStream_t)stream;
     if (bs == 1) kry_p_kernel<1><<<kgrid(n), 256, 0, st>>>(n, r, p, v, minv, ph, scal, cur & 1);
     else if (bs == 2) kry_p_kernel<2><<<kgrid(n / 2), 256, 0, st>>>(n, r, p, v, minv, ph, scal, cur & 1);
-    else kry_p_kernel<3><<<kgrid(n / 3), 256, 0, st>>>(n, r, p, v, minv, ph, scal, cur & 1);
+    else if (bs == 3) kry_p_kernel<3><<<kgrid(n / 3), 256, 0, st>>>(n, r, p, v, minv, ph, scal, cur & 1);
+    else if (bs == 4) kry_p_kernel<4><<<kgrid(n / 4), 256, 0, st>>>(n, r, p, v, minv, ph, scal, cur & 1);
+    else kry_p_kernel<7><<<kgrid(n / 7), 256, 0, st>>>(n, r, p, v, minv, ph, scal, cur & 1);
     pb_count_launch_();
     CUDA_TRY(cudaGetLastError());
     return PB_OK;
 }
 extern "C" int pb_kry_s(int64_t n, const double *r, const double *v, const double *minv, double *s, double *sh,
                         double *scal, int cur, int bs, uint64_t stream) {
-    if (bs < 1 || bs > 3 || n % bs) return pb_fail_(PB_EINVAL, "pb_kry_s: block size must be 1, 2 or 3 and divide n");
+    if (!kry_block_size_ok(bs) || n % bs)
+        return pb_fail_(PB_EINVAL, "pb_kry_s: block size must be 1, 2, 3, 4 or 7 and divide n");
     cudaStream_t st = (cudaStream_t)stream;
     if (bs == 1) kry_s_kernel<1><<<kgrid(n), 256, 0, st>>>(n, r, v, minv, s, sh, scal, cur & 1);
     else if (bs == 2) kry_s_kernel<2><<<kgrid(n / 2), 256, 0, st>>>(n, r, v, minv, s, sh, scal, cur & 1);
-    else kry_s_kernel<3><<<kgrid(n / 3), 256, 0, st>>>(n, r, v, minv, s, sh, scal, cur & 1);
+    else if (bs == 3) kry_s_kernel<3><<<kgrid(n / 3), 256, 0, st>>>(n, r, v, minv, s, sh, scal, cur & 1);
+    else if (bs == 4) kry_s_kernel<4><<<kgrid(n / 4), 256, 0, st>>>(n, r, v, minv, s, sh, scal, cur & 1);
+    else kry_s_kernel<7><<<kgrid(n / 7), 256, 0, st>>>(n, r, v, minv, s, sh, scal, cur & 1);
     pb_count_launch_();
     CUDA_TRY(cudaGetLastError());
     return PB_OK;
 }
 
 // Inverses of the bs x bs diagonal blocks of a CSR matrix (rows / columns bs*b .. bs*b+bs-1), row-major, to a DEVICE
-// array of nblocks*bs*bs doubles: the block-Jacobi preconditioner of the mechanics system (one block per cell).
+// array of nblocks*bs*bs doubles: the block-Jacobi preconditioner of the mechanics systems (one block per cell).
 // A singular block is replaced by the inverse of its diagonal (identity where that is zero, too).
 template <int BS>
 __global__ void block_diag_inv_kernel(int64_t nb, const int32_t *__restrict__ ip, const int32_t *__restrict__ ix,
@@ -229,7 +238,7 @@ __global__ void block_diag_inv_kernel(int64_t nb, const int32_t *__restrict__ ip
         for (int i = 0; i < BS; ++i) dg[i] = D[i][i];
         bool ok = true;
 #pragma unroll
-        for (int k = 0; k < BS; ++k) {   // Gauss-Jordan with partial pivoting, fully unrolled (BS <= 3)
+        for (int k = 0; k < BS; ++k) {   // Gauss-Jordan with partial pivoting, fully unrolled (BS <= 7)
             int piv = k;
             double best = fabs(D[k][k]);
 #pragma unroll
@@ -268,12 +277,15 @@ CsrView pb_csr_view_(const pb_csr *a);   // spmv.cu
 extern "C" int pb_csr_block_diag_inv_dev(const pb_csr *a, int bs, int64_t nblocks, double *out_dev, uint64_t stream) {
     if (!a || !out_dev) return pb_fail_(PB_EINVAL, "null pointer");
     const CsrView v = pb_csr_view_(a);
-    if (bs < 1 || bs > 3 || nblocks < 0 || nblocks * bs > v.nrows) return pb_fail_(PB_EINVAL, "pb_csr_block_diag_inv_dev: bad block size / count");
+    if (!kry_block_size_ok(bs) || nblocks < 0 || nblocks * bs > v.nrows)
+        return pb_fail_(PB_EINVAL, "pb_csr_block_diag_inv_dev: bad block size / count");
     cudaStream_t st = (cudaStream_t)stream;
     const int grid = kgrid(nblocks);
     if (bs == 1) block_diag_inv_kernel<1><<<grid, 256, 0, st>>>(nblocks, v.indptr, v.indices, v.data, out_dev);
     else if (bs == 2) block_diag_inv_kernel<2><<<grid, 256, 0, st>>>(nblocks, v.indptr, v.indices, v.data, out_dev);
-    else block_diag_inv_kernel<3><<<grid, 256, 0, st>>>(nblocks, v.indptr, v.indices, v.data, out_dev);
+    else if (bs == 3) block_diag_inv_kernel<3><<<grid, 256, 0, st>>>(nblocks, v.indptr, v.indices, v.data, out_dev);
+    else if (bs == 4) block_diag_inv_kernel<4><<<grid, 256, 0, st>>>(nblocks, v.indptr, v.indices, v.data, out_dev);
+    else block_diag_inv_kernel<7><<<grid, 256, 0, st>>>(nblocks, v.indptr, v.indices, v.data, out_dev);
     pb_count_launch_();
     CUDA_TRY(cudaGetLastError());
     return PB_OK;

@@ -1,0 +1,177 @@
+// tpsa_system.cuh -- the linear system of the TPSA three-field elasticity model (reference models/momentum_balance.py:
+// 82-106, 250-280, 344-368 with the fluxes of models/constitutive_laws.py:3064-3296), gathered per cell from the face
+// values of tpsa_face.cuh:
+//   momentum     -div_nd (S_u u + S_r r + S_p p + B_s g)               - f   = 0
+//   angular      -vol/mu r + div_nr (R_u u + R_r r + B_r g)            - s_r = 0
+//   solid mass   -vol/lambda p + div (M_u u + M_p p + B_m g)           - s_p = 0
+// Unknowns and equations are numbered cell by cell, [u_c (nd), r_c (nr), p_c (1)], so the diagonal blocks of A are the
+// cell blocks.  Block (c, k) exists for k = c and every face neighbour k of c; of its (nd+nr+1)^2 entries only the
+// structurally non-zero ones are stored (u-u is diagonal, r-p and p-r are zero): 37 of 49 in 3-D, 12 of 16 in 2-D.
+// Each block (c, k) is written by one thread (or one host loop step) that walks the faces of c, so there are no atomics
+// and two assemblies are bit-identical.  The CUDA kernels are in face.cu; the test-only host build in tests/emu.
+#pragma once
+#include <cstdint>
+
+#include "views.hpp"
+
+namespace pb {
+
+// neighbours per cell (the cell itself included) the pattern supports
+constexpr int kTpsaMaxNb = 32;
+
+// Layout of one block row.  Row l of a cell: l < ND displacement component l, then NR rotation rows, then the total
+// pressure row.  Per neighbour a row holds len(l) entries, neighbours in ascending cell order; inside one neighbour k
+// the columns are ascending: u row i -> [u_i, r_0 .. r_NR-1, p], r row -> [u_0 .. u_ND-1, r_0 .. r_NR-1],
+// p row -> [u_0 .. u_ND-1, p].  Block row c starts at NZ * cc_ptr[c]; row l at NZ * cc_ptr[c] + off(l) * n_c.
+template <int ND>
+struct TpsaDims {
+    static constexpr int NR = ND == 3 ? 3 : 1, B = ND + NR + 1;
+    static constexpr int LU = NR + 2, LR = ND + NR, LP = ND + 1;
+    static constexpr int NZ = ND * LU + NR * LR + LP;
+    PB_HD static int len(int l) { return l < ND ? LU : (l < ND + NR ? LR : LP); }
+    PB_HD static int off(int l) { return l < ND ? l * LU : (l < ND + NR ? ND * LU + (l - ND) * LR : ND * LU + NR * LR); }
+    // column, relative to k * B, of entry t of row l
+    PB_HD static int col(int l, int t) {
+        if (l < ND) return t == 0 ? l : (t <= NR ? ND + t - 1 : ND + NR);
+        if (l < ND + NR) return t;
+        return t < ND ? t : ND + NR;
+    }
+};
+
+// cell -> face lists (cell_faces in CSC form) and the face -> cell table of face.cu: 2 per face, (cell << 1) | (sign <
+// 0), -1 = none; fc_ptr[f] = first (face, cell) entry of face f in the value layouts of tpsa_face.cuh
+struct TpsaTopo {
+    int64_t nc;
+    const int32_t *cf_ip, *cf_ix;
+    const int32_t *face_cells;
+    const int32_t *fc_ptr;
+};
+
+// The distinct cells sharing a face with c, c included, ascending, into nb; returns their number, or -1 when there
+// are more than kTpsaMaxNb.
+PB_HD int tpsa_cell_neighbours(int64_t c, const TpsaTopo &t, int32_t *nb) {
+    int n = 1;
+    nb[0] = (int32_t)c;
+    for (int q = t.cf_ip[c]; q < t.cf_ip[c + 1]; ++q) {
+        const int64_t f = t.cf_ix[q];
+        for (int sd = 0; sd < 2; ++sd) {
+            const int32_t e = t.face_cells[2 * f + sd];
+            if (e < 0) continue;
+            const int32_t k = e >> 1;
+            int pos = 0;
+            while (pos < n && nb[pos] < k) ++pos;
+            if (pos < n && nb[pos] == k) continue;
+            if (n == kTpsaMaxNb) return -1;
+            for (int i = n; i > pos; --i) nb[i] = nb[i - 1];
+            nb[pos] = k;
+            ++n;
+        }
+    }
+    return n;
+}
+
+// Row pointers and column indices of block row c (n = its neighbour count, nb = its neighbours).
+template <int ND>
+PB_HD void tpsa_pattern_rows(int64_t c, int n, const int32_t *nb, int64_t cc0, int32_t *ip, int32_t *ix) {
+    using D = TpsaDims<ND>;
+    const int64_t base = (int64_t)D::NZ * cc0;
+    for (int l = 0; l < D::B; ++l) {
+        const int len = D::len(l);
+        const int64_t r0 = base + (int64_t)D::off(l) * n;
+        ip[c * D::B + l] = (int32_t)r0;
+        for (int j = 0; j < n; ++j)
+            for (int t = 0; t < len; ++t) ix[r0 + j * len + t] = nb[j] * D::B + D::col(l, t);
+    }
+}
+
+// face values the system reads (PB_TPSA_* order of include/poreb200.h: 0-6 cell terms, 10-12 boundary terms)
+struct TpsaTerms {
+    const double *t[14];
+};
+
+// Entries of row l of block row c in block (c, k), k a neighbour of c (or c itself): the len(l) values at dst.  Every entry sums the faces of c in the order of its cell -> face list, so the values do not depend on how the
+// work is split.
+template <int ND>
+PB_HD void tpsa_system_segment(int64_t c, int l, int64_t k, const TpsaTopo &t, const TpsaTerms &T, const double *mu,
+                               const double *lam, const double *vol, double *dst) {
+    using D = TpsaDims<ND>;
+    constexpr int NR = D::NR, LMAX = D::LR > D::LU ? D::LR : D::LU;
+    double acc[LMAX];
+#pragma unroll
+    for (int q = 0; q < LMAX; ++q) acc[q] = 0.0;
+    for (int q = t.cf_ip[c]; q < t.cf_ip[c + 1]; ++q) {
+        const int64_t f = t.cf_ix[q];
+        const int32_t e0 = t.face_cells[2 * f], e1 = t.face_cells[2 * f + 1];
+        const int L = e1 >= 0 ? 2 : 1;
+        const int64_t c0 = e0 >> 1, c1 = e1 >= 0 ? (int64_t)(e1 >> 1) : -1;
+        if (c0 != k && c1 != k) continue;
+        const double s = (((c0 == c) ? e0 : e1) & 1) ? -1.0 : 1.0;   // cell_faces[f, c]: div = cell_faces^T
+        const int r = (L == 2 && (c0 == k ? c1 : c0) < k) ? 1 : 0;    // rank of k among the face's cells
+        const int64_t p0 = t.fc_ptr[f];
+        if (l < ND) {
+            const int i = l;
+            acc[0] -= s * T.t[0][ND * p0 + i * L + r];
+#pragma unroll
+            for (int m = 0; m < NR; ++m) acc[1 + m] -= s * T.t[1][ND * NR * p0 + i * NR * L + r * NR + m];
+            acc[1 + NR] -= s * T.t[2][ND * p0 + i * L + r];
+        } else if (l < ND + NR) {
+            const int i = l - ND;
+#pragma unroll
+            for (int m = 0; m < ND; ++m) acc[m] += s * T.t[3][NR * ND * p0 + i * ND * L + r * ND + m];
+#pragma unroll
+            for (int m = 0; m < NR; ++m) acc[ND + m] += s * T.t[4][NR * NR * p0 + i * NR * L + r * NR + m];
+        } else {
+#pragma unroll
+            for (int m = 0; m < ND; ++m) acc[m] += s * T.t[5][ND * p0 + r * ND + m];
+            acc[ND] += s * T.t[6][p0 + r];
+        }
+    }
+    if (k == c && l >= ND) {
+        if (l < ND + NR) acc[l] -= vol[c] / mu[c];    // r row i: column r_i is entry ND + i == l
+        else acc[ND] -= vol[c] / lam[c];
+    }
+    const int len = D::len(l);
+#pragma unroll
+    for (int q = 0; q < LMAX; ++q)
+        if (q < len) dst[q] = acc[q];
+}
+
+// Block (c, cc_ix[j0 + j]) of A, all rows, into the CSR values a (j0 = cc_ptr[c], n neighbours).
+template <int ND>
+PB_HD void tpsa_system_block(int64_t c, int j, const TpsaTopo &t, const int32_t *cc_ptr, const int32_t *cc_ix,
+                             const TpsaTerms &T, const double *mu, const double *lam, const double *vol, double *a) {
+    using D = TpsaDims<ND>;
+    const int64_t j0 = cc_ptr[c];
+    const int n = (int)(cc_ptr[c + 1] - j0);
+    const int64_t k = cc_ix[j0 + j];
+#pragma unroll
+    for (int l = 0; l < D::B; ++l)
+        tpsa_system_segment<ND>(c, l, k, t, T, mu, lam, vol,
+                                a + (int64_t)D::NZ * j0 + (int64_t)D::off(l) * n + (int64_t)j * D::len(l));
+}
+
+// Entry l of block c of b = -R(0):  div_nd B_s g + f,  -div_nr B_r g + s_r,  -div B_m g + s_p.  g: nd values per face
+// at f*nd + i; src: the f / s_r / s_p entry of this row (0 when not given).
+template <int ND>
+PB_HD double tpsa_rhs_row(int64_t c, int l, const TpsaTopo &t, const TpsaTerms &T, const double *g, double src) {
+    constexpr int NR = TpsaDims<ND>::NR;
+    double acc = 0.0;
+    for (int q = t.cf_ip[c]; q < t.cf_ip[c + 1]; ++q) {
+        const int64_t f = t.cf_ix[q];
+        const int32_t e0 = t.face_cells[2 * f], e1 = t.face_cells[2 * f + 1];
+        const double s = ((((int64_t)(e0 >> 1) == c) ? e0 : e1) & 1) ? -1.0 : 1.0;
+        const double *gf = g + f * ND;
+        if (l < ND) {
+            acc += s * (T.t[10][f * ND + l] * gf[l]);
+        } else {
+            const double *w = l < ND + NR ? T.t[11] + f * NR * ND + (l - ND) * ND : T.t[12] + f * ND;
+            double v = 0.0;
+#pragma unroll
+            for (int m = 0; m < ND; ++m) v += w[m] * gf[m];
+            acc -= s * v;
+        }
+    }
+    return acc + src;
+}
+
+}  // namespace pb

@@ -635,6 +635,36 @@ class FaceGrid:
                                     ptrs, C.byref(ms)))
         return out, float(ms.value)
 
+    def tpsa_system(self, nd: int, mu, lmbda, cell_volumes, codes, robin_diag, face_flags, face_areas) -> tuple:
+        """The TPSA three-field system matrix (``pb_tpsa_system``, layout in include/poreb200.h) as a ``DeviceCsr`` and
+        the device times of its two stages in ms.  ``codes`` / ``robin_diag``: (nf, nd), ``face_flags``: nf."""
+        from .sparse import DeviceCsr
+        mu, lam, vol = _lib.f64(mu), _lib.f64(lmbda), _lib.f64(cell_volumes)
+        if mu.shape != (self.nc,) or lam.shape != (self.nc,):
+            raise ValueError("fourth_order_tensor.mu and .lmbda must have one value per cell")
+        if vol.shape != (self.nc,):
+            raise ValueError("cell_volumes must have one value per cell")
+        cod = np.ascontiguousarray(codes, dtype=np.uint8)
+        rob = None if robin_diag is None else _lib.f64(robin_diag)
+        flags = np.ascontiguousarray(face_flags, dtype=np.uint8)
+        _lib.check(self.lib.pb_facegrid_set_face_areas(self.h, _lib.ptr(_lib.f64(face_areas), _lib._f64p)))
+        h = C.c_void_p()
+        ms = (C.c_float * 2)()
+        _lib.check(self.lib.pb_tpsa_system(self.h, int(nd), _lib.ptr(mu, _lib._f64p), _lib.ptr(lam, _lib._f64p),
+                                           _lib.ptr(vol, _lib._f64p), _lib.ptr(cod, _lib._u8p),
+                                           _lib.ptr(rob, _lib._f64p), _lib.ptr(flags, _lib._u8p), C.byref(h),
+                                           C.cast(ms, _lib._f32p)))
+        return DeviceCsr.from_handle(h), [float(ms[0]), float(ms[1])]
+
+    def tpsa_rhs(self, n: int, bc_values, body_force=None, angular_source=None, mass_source=None):
+        """b = -R(0) of the TPSA system last assembled on this grid (``pb_tpsa_rhs``) as a CUDA tensor of ``n``
+        doubles."""
+        import torch
+        arrs = [None if a is None else _lib.f64(a) for a in (bc_values, body_force, angular_source, mass_source)]
+        b = torch.empty(int(n), dtype=torch.float64, device="cuda")
+        _lib.check(self.lib.pb_tpsa_rhs(self.h, *[_lib.ptr(a, _lib._f64p) for a in arrs], C.c_void_p(b.data_ptr())))
+        return b
+
 
 # (rows per face, columns per cell or face) of the 14 TPSA terms in PB_TPSA_* order; "k" marks kron(., I_nd), "r" the
 # rotation dimension (nd in 3-D, 1 in 2-D), "d" the dimension.  The first ten terms have cell columns.

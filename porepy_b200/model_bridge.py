@@ -400,3 +400,42 @@ def fractured_thermoporomechanics_from_model(model):
              ("normal_fracture_deformation_equation", [(f, 1) for f in fracs]),
              ("tangential_fracture_deformation_equation", [(f, 2) for f in fracs])]
     return prob, np.concatenate(cols), _row_map(model, order)
+
+
+def tpsa_momentum_from_model(model):
+    """A prepared ``pp.MomentumBalance`` with ``TpsaMomentumBalanceMixin`` on one 2-D or 3-D grid without fractures ->
+    (``TpsaElasticity``, column_map, row_map): unknown k of the problem (cell-interleaved [u_c, r_c, p_c]) is dof
+    ``column_map[k]`` of the model's ``EquationSystem``, equation k its row ``row_map[k]``.  The boundary operator g is
+    the model's own ``combine_boundary_operators_mechanical_stress``, evaluated; f is its ``body_force``, s_r / s_p its
+    ``source_angular_momentum`` / ``solid_mass_source``."""
+    from .tpsa_elasticity import TpsaElasticity, interleave
+    mdg, es = model.mdg, model.equation_system
+    sds = list(mdg.subdomains())
+    if any(sd.dim < model.nd for sd in sds) or any(True for _ in mdg.interfaces()):
+        raise NotImplementedError("TpsaElasticity: fractures are not supported")
+    if len(sds) != 1:
+        raise NotImplementedError("TpsaElasticity: one subdomain is expected")
+    if "mass_balance_equation" in es.equations:
+        raise NotImplementedError("TpsaElasticity: the TPSA poromechanics model (four fields) is not supported")
+    sd = sds[0]
+    nd, nc = sd.dim, sd.num_cells
+    if nd not in (2, 3):
+        raise NotImplementedError("Tpsa is only implemented for 2d and 3d grids.")
+    nr = model.rotation_dimension()
+    mk = model.stress_keyword
+    data = _own_data(mdg.subdomain_data(sd), [mk])
+    prob = TpsaElasticity(sd, data, mk,
+                          _evaluated(model, model.combine_boundary_operators_mechanical_stress([sd]), nd * sd.num_faces),
+                          body_force=_evaluated(model, model.body_force([sd]), nd * nc),
+                          angular_source=_evaluated(model, model.source_angular_momentum([sd]), nr * nc),
+                          mass_source=_evaluated(model, model.solid_mass_source([sd]), nc))
+
+    def dofs(name):
+        return es.dofs_of([v for v in es.variables if v.name == name and v.domain is sd])
+    cols = [dofs(model.displacement_variable), dofs(model.rotation_stress_variable), dofs(model.total_pressure_variable)]
+    order = [("momentum_balance_equation", [(sd, nd)]), ("angular_momentum_balance_equation", [(sd, nr)]),
+             ("solid_mass_equation", [(sd, 1)])]
+    rows = _row_map(model, order)
+    prob.column_map = interleave(cols, nd, nr, nc)
+    prob.row_map = interleave([rows[:nd * nc], rows[nd * nc:(nd + nr) * nc], rows[(nd + nr) * nc:]], nd, nr, nc)
+    return prob, prob.column_map, prob.row_map

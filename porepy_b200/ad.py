@@ -37,9 +37,12 @@ def as_device_csr(m) -> DeviceCsr:
 
 
 def device_vector(v, device=None):
+    """``v`` as a contiguous float64 CUDA tensor (the kernels read it through its data pointer): views, other dtypes
+    and host tensors are copied."""
     import torch
     if torch.is_tensor(v):
-        return v.to(dtype=torch.float64)
+        dev = device or (v.device if v.is_cuda else torch.device("cuda", torch.cuda.current_device()))
+        return v.to(device=dev, dtype=torch.float64).contiguous()
     dev = device or torch.device("cuda", torch.cuda.current_device())
     return torch.as_tensor(np.ascontiguousarray(v, dtype=np.float64), device=dev)
 
@@ -120,7 +123,9 @@ def _plain(other, like):
     import torch
     if isinstance(other, (int, float, np.floating, np.integer)):
         return float(other)
-    return torch.as_tensor(np.asarray(other, dtype=np.float64), device=like.device) if not torch.is_tensor(other) else other
+    if torch.is_tensor(other):          # views and other dtypes: ``scaled`` reads a contiguous float64 buffer
+        return other.to(device=like.device, dtype=torch.float64).contiguous()
+    return torch.as_tensor(np.asarray(other, dtype=np.float64), device=like.device)
 
 
 def variables(values) -> list:

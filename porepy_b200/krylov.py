@@ -314,19 +314,26 @@ def _bicgstab_fused(op: DistributedOperator, b_own, tol, maxiter, diag_own, chec
     dev = b_own.device
     world = op.loc.world
     vec = lambda m=n: torch.zeros(m, dtype=torch.float64, device=dev)  # noqa: E731
+
+    def on_device(a, what):          # the kernels read these through data_ptr(): float64 on the solver's device only
+        if not (torch.is_tensor(a) and a.dtype == torch.float64 and a.device == dev):
+            raise TypeError(f"{what}: a float64 tensor on {dev} is required")
+        return a.contiguous()
+    if dev.type != "cuda":
+        raise TypeError("b_own: a CUDA tensor is required")
+    b_own = on_device(b_own, "b_own")
     x, r, rhat, p, v, s, t = (vec() for _ in range(7))
     xb_p, xb_s = vec(n + ng), vec(n + ng)            # SpMV inputs [own | ghost]; ph / sh are their own parts
     ph, sh = xb_p[:n], xb_s[:n]
-    minv = None if diag_own is None else (1.0 / diag_own).contiguous()
+    minv = None if diag_own is None else (1.0 / on_device(diag_own, "diag_own")).contiguous()
     bs = 1
     if block_inv is not None:
-        minv, bs = block_inv[0].contiguous(), int(block_inv[1])
+        minv, bs = on_device(block_inv[0], "block_inv[0]"), int(block_inv[1])
         if n % bs or minv.numel() != n * bs:
             raise ValueError("block_inv: expected (n / bs) inverted bs x bs blocks of the own rows")
     scal = torch.zeros(14, dtype=torch.float64, device=dev)
     P = lambda a: C.c_void_p(a.data_ptr()) if a is not None else None  # noqa: E731
     S = lambda i: C.c_void_p(scal.data_ptr() + 8 * i)  # noqa: E731
-    b_own = b_own.contiguous()
     csr = op.dev_csr
     carry = 1 if op.loc.rank == 0 else 0
     nred = [0]

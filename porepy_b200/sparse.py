@@ -12,6 +12,17 @@ import scipy.sparse as sps
 from . import _lib
 
 
+def device_operand(t, n: int, what: str):
+    """``t`` if the library may read it through ``t.data_ptr()``: a contiguous float64 CUDA tensor of ``n`` elements.
+    A view (strided, expanded), another dtype or a host tensor would be read as if it were that, so it is refused."""
+    import torch
+    if not (torch.is_tensor(t) and t.is_cuda and t.dtype == torch.float64 and t.is_contiguous()):
+        raise TypeError(f"{what}: a contiguous float64 CUDA tensor is required")
+    if t.numel() != n:
+        raise ValueError("dimension mismatch")
+    return t
+
+
 class DeviceCsr:
     def __init__(self, a):
         lib = _lib.load()
@@ -104,9 +115,9 @@ class DeviceCsr:
         return DeviceCsr.from_handle(h)
 
     def scaled(self, d, by_cols: bool = False) -> "DeviceCsr":
-        """diag(d) @ self (``_diagvec_mul_jac``, forward_mode.py:613-616) or self @ diag(d); ``d``: CUDA tensor."""
-        if d.numel() != self.shape[1 if by_cols else 0]:
-            raise ValueError("dimension mismatch")
+        """diag(d) @ self (``_diagvec_mul_jac``, forward_mode.py:613-616) or self @ diag(d); ``d``: contiguous float64
+        CUDA tensor."""
+        d = device_operand(d, self.shape[1 if by_cols else 0], "DeviceCsr.scaled")
         h = C.c_void_p()
         _lib.check(self.lib.pb_csr_scale_dev(self.h, C.c_void_p(d.data_ptr()), int(by_cols), C.byref(h)))
         return DeviceCsr.from_handle(h)
@@ -175,12 +186,13 @@ class DeviceCsr:
             return self.matmul(x)
         if hasattr(x, "__rmatmul__") and type(x).__name__ == "DeviceAdArray":
             return x.__rmatmul__(self)
-        if hasattr(x, "data_ptr"):       # CUDA tensor: y = A x on the device
+        if hasattr(x, "data_ptr"):       # CUDA tensor: y = A x on the device (a strided view is copied first)
             import torch
-            if x.numel() != self.shape[1]:
-                raise ValueError("dimension mismatch")
+            x = device_operand(x.contiguous() if torch.is_tensor(x) else x, self.shape[1], "DeviceCsr @ tensor")
+            if self.shape[0] == 0 or self.shape[1] == 0:
+                return torch.zeros(self.shape[0], dtype=torch.float64, device=x.device)
             y = torch.empty(self.shape[0], dtype=torch.float64, device=x.device)
-            self.spmv_device(x.contiguous().data_ptr(), y.data_ptr(), torch.cuda.current_stream().cuda_stream)
+            self.spmv_device(x.data_ptr(), y.data_ptr(), torch.cuda.current_stream().cuda_stream)
             return y
         x = _lib.f64(x)
         if x.shape != (self.shape[1],):

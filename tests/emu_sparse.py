@@ -100,7 +100,10 @@ class HostCsr:
         if type(x).__name__ == "DeviceAdArray":
             return x.__rmatmul__(self)
         if torch.is_tensor(x):
-            if x.numel() != self.shape[1] or x.dtype != torch.float64:
+            # DeviceCsr @ tensor copies a strided view, but refuses what the kernel cannot read as float64
+            if x.dtype != torch.float64:
+                raise TypeError("a float64 tensor is required")
+            if x.numel() != self.shape[1]:
                 raise ValueError("dimension mismatch")
             return torch.as_tensor(self.m @ x.cpu().numpy())
         x = np.asarray(x, float)

@@ -334,6 +334,30 @@ int pb_tpsa_system(pb_facegrid *g, int nd, const double *mu, const double *lambd
 int pb_tpsa_rhs(pb_facegrid *g, const double *bc_values, const double *body_force, const double *angular_source,
                 const double *mass_source, double *rhs_dev);
 
+/* The Jacobian of the TPSA poromechanics model (pp.Poromechanics + TpsaPoromechanicsMixin; reference
+ * models/poromechanics.py:92-136, 177-213, models/constitutive_laws.py:3299-3374) on one grid without fractures:
+ * four fields per cell, [u_c (nd), r_c (nr), p_t_c, p_c], B = nd + nr + 2 (5 in 2-D, 8 in 3-D), row / column c*B + l.
+ * The mechanics rows are those of pb_tpsa_system, the solid-mass row extended by -vol alpha/lambda p (its p entry is
+ * stored for every face neighbour, 0 off the cell's own block).  The fluid-mass row of c holds the p column of every
+ * cell of row c of flux_pattern (div @ flux of the MPFA discretization, nc x nc, sorted rows) and the whole own block.
+ * pb_tpsa_poro_system: the matrix with its mechanics rows, fluid rows 0, as a new device CSR.  Arguments as for
+ * pb_tpsa_system; alpha (nc, host): the Biot coefficient, finite.  The row pattern is built on the device at the first
+ * call for a dimension and flux pattern and kept on the handle.  No atomics: two calls give bit-identical values.
+ * pb_tpsa_poro_rhs: -R(0) of the mechanics rows (the right-hand side of pb_tpsa_rhs), 0 in the fluid rows, to the DEVICE
+ * array rhs_dev (nc*B).
+ * pb_tpsa_poro_fluid_rows: the fluid rows at one Newton step, on `stream`, nothing copied to the host: row c of jf
+ * (nc x 2 nc device CSR, columns [p_t | p], the field-ordered Jacobian of the fluid mass balance) into the fixed
+ * pattern of a (the matrix of pb_tpsa_poro_system on g), and neg_res_dev[c] (-R of the fluid mass balance, device) into
+ * rhs_dev[c*B + B-1].  Entries of jf outside the pattern are counted into *missing_dev (device int, may be NULL). */
+int pb_tpsa_poro_system(pb_facegrid *g, int nd, const double *mu, const double *lambda, const double *alpha,
+                        const double *cell_volumes, const uint8_t *codes, const double *robin_diag,
+                        const uint8_t *face_flags, const struct pb_csr *flux_pattern, struct pb_csr **out,
+                        float *stage_ms);
+int pb_tpsa_poro_rhs(pb_facegrid *g, const double *bc_values, const double *body_force, const double *angular_source,
+                     const double *mass_source, double *rhs_dev);
+int pb_tpsa_poro_fluid_rows(pb_facegrid *g, struct pb_csr *a, const struct pb_csr *jf, const double *neg_res_dev,
+                            double *rhs_dev, int *missing_dev, uint64_t stream);
+
 /* Interface upwinding (UpwindCoupling.discretize, numerics/fv/upwind.py:427-528): per mortar cell the sign of the
  * interface flux and the masks "upstream is the higher-dimensional side" / "... the lower-dimensional side".
  * Host pointers, n doubles each. */
@@ -416,15 +440,16 @@ int pb_csr_spmv_dots_dev(pb_csr *a, const double *x_dev, double *y_dev, const do
 int pb_kry_init(int64_t n, const double *b, double *x, double *r, double *rhat, double *p, double *v, double *scal,
                 double tol, uint64_t stream);
 int pb_kry_seed(double *scal, uint64_t stream);
-/* minv / bs: the preconditioner M^-1 -- bs = 1: inverse diagonal (n doubles, Jacobi); bs = 2, 3, 4, 7: inverted bs x bs
- * diagonal blocks, row-major (n/bs blocks; block Jacobi over the unknowns of a cell: the displacement components of
- * the MPSA system (2, 3) or [u, r, p] of the TPSA system (4 in 2-D, 7 in 3-D)); NULL: none */
+/* minv / bs: the preconditioner M^-1 -- bs = 1: inverse diagonal (n doubles, Jacobi); bs = 2, 3, 4, 5, 7, 8: inverted
+ * bs x bs diagonal blocks, row-major (n/bs blocks; block Jacobi over the unknowns of a cell: the displacement components
+ * of the MPSA system (2, 3), [u, r, p] of the TPSA system (4 in 2-D, 7 in 3-D) or [u, r, p_t, p] of the TPSA
+ * poromechanics system (5, 8)); NULL: none */
 int pb_kry_p(int64_t n, const double *r, double *p, const double *v, const double *minv, double *ph, double *scal,
              int cur, int bs, uint64_t stream);
 int pb_kry_s(int64_t n, const double *r, const double *v, const double *minv, double *s, double *sh, double *scal,
              int cur, int bs, uint64_t stream);
 /* inverses of the first nblocks bs x bs diagonal blocks of a device CSR, to a DEVICE array (nblocks*bs*bs doubles);
- * bs in {1, 2, 3, 4, 7}.  A singular block is replaced by the inverse of its diagonal (1 where that entry is 0). */
+ * bs in {1, 2, 3, 4, 5, 7, 8}.  A singular block is replaced by the inverse of its diagonal (1 where that entry is 0). */
 int pb_csr_block_diag_inv_dev(const pb_csr *a, int bs, int64_t nblocks, double *out_dev, uint64_t stream);
 int pb_kry_xr(int64_t n, double *x, const double *ph, const double *sh, const double *s, const double *t, double *r,
               const double *rhat, double *scal, int cur, int carry /* 1 on exactly one rank */, uint64_t stream);

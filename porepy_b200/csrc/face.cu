@@ -21,6 +21,11 @@ struct pb_facegrid {
     int sys_nd = 0, terms_nd = 0;
     int64_t sys_nnz = 0, sys_npairs = 0;
     DevBuf fc_ptr, cc_ptr, cc_ix, cc_cell, sys_ip, sys_ix, terms[PB_TPSA_NTERMS];
+    // TPSA poromechanics system (pb_tpsa_poro_system): its row pattern, built once per dimension and flux pattern
+    bool nb_ready = false;
+    int poro_nd = 0;
+    int64_t poro_nnz = 0, poro_fp_nnz = -1;
+    DevBuf blk_ptr, poro_ip, poro_ix;
 };
 
 // one thread per cell: claim the first free slot of each of its faces
@@ -394,11 +399,11 @@ static TpsaTopo tpsa_topo(pb_facegrid *g) {
                     g->fc_ptr.as<int32_t>()};
 }
 
-// Row pattern of the system for dimension nd: neighbour lists, block-row offsets and the CSR arrays of A.
-static int tpsa_build_pattern(pb_facegrid *g, int nd) {
+// Neighbour counts of every cell, scanned into cc_ptr; *total = number of (cell, neighbour) pairs.  cc_ix / cc_cell are
+// sized for them.
+static int tpsa_neighbour_counts(pb_facegrid *g, int32_t *total_out) {
     cudaStream_t st = g->stream;
     const int64_t nc = g->nc;
-    const int B = nd == 3 ? 7 : 4, NZ = nd == 3 ? 37 : 12;
     const TpsaTopo t = tpsa_topo(g);
     DevBuf count, bad, scratch;
     CUDA_TRY(count.ensure((size_t)(nc + 1) * sizeof(int32_t)));
@@ -421,10 +426,23 @@ static int tpsa_build_pattern(pb_facegrid *g, int nd) {
     CUDA_TRY(cudaMemcpyAsync(&total, g->cc_ptr.as<int32_t>() + nc, sizeof(int32_t), cudaMemcpyDeviceToHost, st));
     CUDA_TRY(cudaStreamSynchronize(st));
     if (hbad) return pb_fail_(PB_ENOTIMPL, "Tpsa system: a cell has more than 31 face neighbours");
-    const int64_t nnz = (int64_t)NZ * total;
-    if (nnz >= 0x7FFFFFFFll) return pb_fail_(PB_ENOTIMPL, "Tpsa system: the matrix does not fit int32 indices");
     CUDA_TRY(g->cc_ix.ensure((size_t)std::max<int64_t>(1, total) * sizeof(int32_t)));
     CUDA_TRY(g->cc_cell.ensure((size_t)std::max<int64_t>(1, total) * sizeof(int32_t)));
+    *total_out = total;
+    return PB_OK;
+}
+
+// Row pattern of the system for dimension nd: neighbour lists, block-row offsets and the CSR arrays of A.
+static int tpsa_build_pattern(pb_facegrid *g, int nd) {
+    cudaStream_t st = g->stream;
+    const int64_t nc = g->nc;
+    const int B = nd == 3 ? 7 : 4, NZ = nd == 3 ? 37 : 12;
+    const TpsaTopo t = tpsa_topo(g);
+    int32_t total = 0;
+    int rc0 = tpsa_neighbour_counts(g, &total);
+    if (rc0) return rc0;
+    const int64_t nnz = (int64_t)NZ * total;
+    if (nnz >= 0x7FFFFFFFll) return pb_fail_(PB_ENOTIMPL, "Tpsa system: the matrix does not fit int32 indices");
     CUDA_TRY(g->sys_ip.ensure((size_t)(nc * B + 1) * sizeof(int32_t)));
     CUDA_TRY(g->sys_ix.ensure((size_t)std::max<int64_t>(1, nnz) * sizeof(int32_t)));
     const int32_t last = (int32_t)nnz;
@@ -443,6 +461,7 @@ static int tpsa_build_pattern(pb_facegrid *g, int nd) {
     g->sys_nd = nd;
     g->sys_nnz = nnz;
     g->sys_npairs = total;
+    g->nb_ready = true;
     return PB_OK;
 }
 
@@ -451,11 +470,14 @@ struct FgEvents {
     ~FgEvents() { for (auto x : e) if (x) cudaEventDestroy(x); }
 };
 
-extern "C" int pb_tpsa_system(pb_facegrid *g, int nd, const double *mu, const double *lambda,
-                              const double *cell_volumes, const uint8_t *codes, const double *robin_diag,
-                              const uint8_t *face_flags, pb_csr **out, float *stage_ms) {
-    if (!g || !mu || !lambda || !cell_volumes || !codes || !face_flags || !out)
-        return pb_fail_(PB_EINVAL, "null pointer");
+// Inputs of both TPSA systems on the device, checked as pb_tpsa checks them (lambda also finite and > 0).
+struct TpsaInputs {
+    DevBuf mu, lam, vol, codes, rob, flags;
+    bool any_rob = false;
+};
+
+static int tpsa_prepare(pb_facegrid *g, int nd, const double *mu, const double *lambda, const double *cell_volumes,
+                        const uint8_t *codes, const double *robin_diag, const uint8_t *face_flags, TpsaInputs &in) {
     if (nd != 2 && nd != 3) return pb_fail_(PB_EINVAL, "Tpsa is only implemented for 2d and 3d grids.");
     if (!g->geo.farea) return pb_fail_(PB_EINVAL, "face areas not set (pb_facegrid_set_face_areas)");
     const int64_t nf = g->nf, nc = g->nc;
@@ -464,12 +486,11 @@ extern "C" int pb_tpsa_system(pb_facegrid *g, int nd, const double *mu, const do
         if (!(lambda[c] > 0.0) || !std::isfinite(lambda[c]))
             return pb_fail_(PB_EINVAL, "first Lame parameter lambda must be finite and > 0");
     }
-    bool any_rob = false;
     for (int64_t q = 0; q < nd * nf; ++q) {
         if (codes[q] > PB_BC_ROB) return pb_fail_(PB_EINVAL, "boundary code out of range");
-        any_rob |= codes[q] == PB_BC_ROB;
+        in.any_rob |= codes[q] == PB_BC_ROB;
     }
-    if (any_rob && !robin_diag) return pb_fail_(PB_EINVAL, "Robin faces need robin_diag");
+    if (in.any_rob && !robin_diag) return pb_fail_(PB_EINVAL, "Robin faces need robin_diag");
     for (int64_t f = 0; f < nf; ++f) {
         const int len = g->face_ncell[f];
         if (len < 1 || len > 2) return pb_fail_(PB_EINVAL, "fc_indptr: a face has one or two cells");
@@ -482,12 +503,18 @@ extern "C" int pb_tpsa_system(pb_facegrid *g, int nd, const double *mu, const do
         CUDA_TRY(g->fc_ptr.upload(fp, st));
         CUDA_TRY(cudaStreamSynchronize(st));
     }
-    if (g->sys_nd != nd) {
-        g->sys_nd = 0;
-        int rc = tpsa_build_pattern(g, nd);
-        if (rc) return rc;
-    }
-    // stage 1: the ten face terms the system reads, kept on the handle
+    CUDA_TRY(in.mu.upload(mu, (size_t)nc, st));
+    CUDA_TRY(in.lam.upload(lambda, (size_t)nc, st));
+    CUDA_TRY(in.vol.upload(cell_volumes, (size_t)nc, st));
+    CUDA_TRY(in.codes.upload(codes, (size_t)nd * nf, st));
+    if (in.any_rob) CUDA_TRY(in.rob.upload(robin_diag, (size_t)nd * nf, st));
+    CUDA_TRY(in.flags.upload(face_flags, (size_t)nf, st));
+    return PB_OK;
+}
+
+// Stage 1: the ten face terms the systems read, into buffers kept on the handle (T points at them).
+static int tpsa_face_terms(pb_facegrid *g, int nd, const TpsaInputs &in, TpsaTerms &T) {
+    const int64_t nf = g->nf;
     int64_t nfc = 0;   // (face, cell) entries
     for (int64_t f = 0; f < nf; ++f) nfc += g->face_ncell[f];
     const size_t nr = nd == 3 ? 3 : 1;
@@ -496,23 +523,44 @@ extern "C" int pb_tpsa_system(pb_facegrid *g, int nd, const double *mu, const do
     const bool used[PB_TPSA_NTERMS] = {true, true, true, true, true, true, true, false, false, false, true, true, true,
                                        false};
     TpsaOut o{};
-    TpsaTerms T{};
     for (int k = 0; k < PB_TPSA_NTERMS; ++k) {
         if (!used[k]) continue;
         CUDA_TRY(g->terms[k].ensure(per[k] * (k < PB_TPSA_BOUND_STRESS ? (size_t)nfc : (size_t)nf) * sizeof(double)));
         o.t[k] = g->terms[k].as<double>();
         T.t[k] = o.t[k];
     }
-    DevBuf dmu, dlam, dvol, dcodes, drob, dflags;
-    CUDA_TRY(dmu.upload(mu, (size_t)nc, st));
-    CUDA_TRY(dlam.upload(lambda, (size_t)nc, st));
-    CUDA_TRY(dvol.upload(cell_volumes, (size_t)nc, st));
-    CUDA_TRY(dcodes.upload(codes, (size_t)nd * nf, st));
-    if (any_rob) CUDA_TRY(drob.upload(robin_diag, (size_t)nd * nf, st));
-    CUDA_TRY(dflags.upload(face_flags, (size_t)nf, st));
+    cudaStream_t st = g->stream;
+    const double *rw = in.any_rob ? in.rob.as<double>() : nullptr;
+    const int32_t *fcp = g->fc_ptr.as<int32_t>();
+    if (nd == 3)
+        tpsa_kernel<3><<<fg_grid(nf), 256, 0, st>>>(nf, g->geo, in.mu.as<double>(), in.codes.as<uint8_t>(), rw,
+                                                     in.flags.as<uint8_t>(), g->face_cells.as<int32_t>(), fcp, o);
+    else
+        tpsa_kernel<2><<<fg_grid(nf), 256, 0, st>>>(nf, g->geo, in.mu.as<double>(), in.codes.as<uint8_t>(), rw,
+                                                     in.flags.as<uint8_t>(), g->face_cells.as<int32_t>(), fcp, o);
+    pb_count_launch_();
+    CUDA_TRY(cudaGetLastError());
+    return PB_OK;
+}
+
+extern "C" int pb_tpsa_system(pb_facegrid *g, int nd, const double *mu, const double *lambda,
+                              const double *cell_volumes, const uint8_t *codes, const double *robin_diag,
+                              const uint8_t *face_flags, pb_csr **out, float *stage_ms) {
+    if (!g || !mu || !lambda || !cell_volumes || !codes || !face_flags || !out)
+        return pb_fail_(PB_EINVAL, "null pointer");
+    TpsaInputs in;
+    int rc = tpsa_prepare(g, nd, mu, lambda, cell_volumes, codes, robin_diag, face_flags, in);
+    if (rc) return rc;
+    if (g->sys_nd != nd) {
+        g->sys_nd = 0;
+        rc = tpsa_build_pattern(g, nd);
+        if (rc) return rc;
+    }
+    cudaStream_t st = g->stream;
+    const int64_t nc = g->nc;
     pb_csr *a = nullptr;
-    int rc = pb_csr_from_device_pattern_(nc * (nd == 3 ? 7 : 4), nc * (nd == 3 ? 7 : 4), g->sys_nnz,
-                                         g->sys_ip.as<int32_t>(), g->sys_ix.as<int32_t>(), &a);
+    rc = pb_csr_from_device_pattern_(nc * (nd == 3 ? 7 : 4), nc * (nd == 3 ? 7 : 4), g->sys_nnz,
+                                     g->sys_ip.as<int32_t>(), g->sys_ix.as<int32_t>(), &a);
     if (rc) return rc;
     FgEvents ev;
     auto fail_cuda = [&](cudaError_t e, const char *what) {
@@ -523,27 +571,20 @@ extern "C" int pb_tpsa_system(pb_facegrid *g, int nd, const double *mu, const do
     if (stage_ms)
         for (auto &x : ev.e) SYS_TRY(cudaEventCreate(&x));
     if (stage_ms) SYS_TRY(cudaEventRecord(ev.e[0], st));
-    const double *rw = any_rob ? drob.as<double>() : nullptr;
-    const TpsaTopo t = tpsa_topo(g);
-    if (nd == 3)
-        tpsa_kernel<3><<<fg_grid(nf), 256, 0, st>>>(nf, g->geo, dmu.as<double>(), dcodes.as<uint8_t>(), rw,
-                                                     dflags.as<uint8_t>(), g->face_cells.as<int32_t>(), t.fc_ptr, o);
-    else
-        tpsa_kernel<2><<<fg_grid(nf), 256, 0, st>>>(nf, g->geo, dmu.as<double>(), dcodes.as<uint8_t>(), rw,
-                                                     dflags.as<uint8_t>(), g->face_cells.as<int32_t>(), t.fc_ptr, o);
-    pb_count_launch_();
-    SYS_TRY(cudaGetLastError());
+    TpsaTerms T{};
+    if ((rc = tpsa_face_terms(g, nd, in, T))) { pb_csr_destroy(a); return rc; }
     if (stage_ms) SYS_TRY(cudaEventRecord(ev.e[1], st));
     // stage 2: every block of A gathered from the faces of its cell
+    const TpsaTopo t = tpsa_topo(g);
     const int64_t np = g->sys_npairs;
     if (nd == 3)
         tpsa_system_kernel<3><<<fg_grid(np), 256, 0, st>>>(np, t, g->cc_ptr.as<int32_t>(), g->cc_ix.as<int32_t>(),
-                                                            g->cc_cell.as<int32_t>(), T, dmu.as<double>(),
-                                                            dlam.as<double>(), dvol.as<double>(), pb_csr_data_(a));
+                                                            g->cc_cell.as<int32_t>(), T, in.mu.as<double>(),
+                                                            in.lam.as<double>(), in.vol.as<double>(), pb_csr_data_(a));
     else
         tpsa_system_kernel<2><<<fg_grid(np), 256, 0, st>>>(np, t, g->cc_ptr.as<int32_t>(), g->cc_ix.as<int32_t>(),
-                                                            g->cc_cell.as<int32_t>(), T, dmu.as<double>(),
-                                                            dlam.as<double>(), dvol.as<double>(), pb_csr_data_(a));
+                                                            g->cc_cell.as<int32_t>(), T, in.mu.as<double>(),
+                                                            in.lam.as<double>(), in.vol.as<double>(), pb_csr_data_(a));
     pb_count_launch_();
     SYS_TRY(cudaGetLastError());
     if (stage_ms) SYS_TRY(cudaEventRecord(ev.e[2], st));
@@ -582,5 +623,248 @@ extern "C" int pb_tpsa_rhs(pb_facegrid *g, const double *bc_values, const double
     pb_count_launch_();
     CUDA_TRY(cudaGetLastError());
     CUDA_TRY(cudaStreamSynchronize(st));
+    return PB_OK;
+}
+
+// ---- TPSA poromechanics system (tpsa_system.cuh, four fields) ---------------------------------------------------
+struct CsrView { int64_t nrows, ncols, nnz; int32_t *indptr, *indices; double *data; };
+CsrView pb_csr_view_(const pb_csr *a);   // spmv.cu
+
+__global__ void tpsa_nb_list_kernel(TpsaTopo t, const int32_t *__restrict__ cc_ptr, int32_t *__restrict__ cc_ix,
+                                    int32_t *__restrict__ cc_cell) {
+    for (int64_t c = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; c < t.nc; c += (int64_t)gridDim.x * blockDim.x) {
+        int32_t nb[kTpsaMaxNb];
+        const int n = tpsa_cell_neighbours(c, t, nb);
+        for (int j = 0; j < n; ++j) { cc_ix[cc_ptr[c] + j] = nb[j]; cc_cell[cc_ptr[c] + j] = (int32_t)c; }
+    }
+}
+
+template <int ND>
+__global__ void tpsa_poro_count_kernel(int64_t nc, const int32_t *__restrict__ cc_ptr, const int32_t *__restrict__ fp_ip,
+                                       const int32_t *__restrict__ fp_ix, int64_t *__restrict__ count) {
+    for (int64_t c = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; c < nc; c += (int64_t)gridDim.x * blockDim.x)
+        count[c] = tpsa_poro_row_count<ND>(c, cc_ptr[c + 1] - cc_ptr[c], fp_ip, fp_ix);
+}
+
+template <int ND>
+__global__ void tpsa_poro_pattern_kernel(int64_t nc, const int32_t *__restrict__ cc_ptr,
+                                         const int32_t *__restrict__ cc_ix, const int64_t *__restrict__ blk_ptr,
+                                         const int32_t *__restrict__ fp_ip, const int32_t *__restrict__ fp_ix,
+                                         int32_t *__restrict__ ip, int32_t *__restrict__ ix) {
+    for (int64_t c = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; c < nc; c += (int64_t)gridDim.x * blockDim.x)
+        tpsa_poro_pattern_rows<ND>(c, cc_ptr[c + 1] - cc_ptr[c], cc_ix + cc_ptr[c], blk_ptr[c], fp_ip, fp_ix, ip, ix);
+}
+
+// one thread per block (c, k), as tpsa_system_kernel
+template <int ND>
+__global__ void tpsa_poro_system_kernel(int64_t npairs, TpsaTopo t, const int32_t *__restrict__ cc_ptr,
+                                        const int32_t *__restrict__ cc_ix, const int32_t *__restrict__ cc_cell,
+                                        const int64_t *__restrict__ blk_ptr, TpsaTerms T, const double *__restrict__ mu,
+                                        const double *__restrict__ lam, const double *__restrict__ alpha,
+                                        const double *__restrict__ vol, double *__restrict__ a) {
+    for (int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; e < npairs; e += (int64_t)gridDim.x * blockDim.x) {
+        const int64_t c = cc_cell[e];
+        tpsa_poro_block<ND>(c, (int)(e - cc_ptr[c]), t, cc_ptr, cc_ix, blk_ptr, T, mu, lam, alpha, vol, a);
+    }
+}
+
+template <int ND>
+__global__ void tpsa_poro_rhs_kernel(TpsaTopo t, TpsaTerms T, const double *__restrict__ g, const double *__restrict__ f,
+                                     const double *__restrict__ sr, const double *__restrict__ sp,
+                                     double *__restrict__ b) {
+    constexpr int NR = TpsaDims<ND>::NR, B = TpsaPoroDims<ND>::B;
+    for (int64_t q = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; q < t.nc * B; q += (int64_t)gridDim.x * blockDim.x) {
+        const int64_t c = q / B;
+        const int l = (int)(q - c * B);
+        if (l == B - 1) { b[q] = 0.0; continue; }   // the fluid rows are written at every linearization
+        const double src = l < ND ? (f ? f[c * ND + l] : 0.0)
+                                   : (l < ND + NR ? (sr ? sr[c * NR + l - ND] : 0.0) : (sp ? sp[c] : 0.0));
+        b[q] = tpsa_rhs_row<ND>(c, l, t, T, g, src);
+    }
+}
+
+// one thread per cell: its fluid row; the mechanics rows of the block row come first
+template <int ND>
+__global__ void tpsa_poro_fluid_kernel(int64_t nc, const int32_t *__restrict__ cc_ptr,
+                                       const int64_t *__restrict__ blk_ptr, const int32_t *__restrict__ ix,
+                                       const int32_t *__restrict__ jf_ip, const int32_t *__restrict__ jf_ix,
+                                       const double *__restrict__ jf_a, const double *__restrict__ neg_res,
+                                       double *__restrict__ a, double *__restrict__ b, int *__restrict__ missing) {
+    for (int64_t c = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; c < nc; c += (int64_t)gridDim.x * blockDim.x) {
+        const int64_t row0 = blk_ptr[c] + (int64_t)TpsaPoroDims<ND>::NZ * (cc_ptr[c + 1] - cc_ptr[c]);
+        const int m = tpsa_poro_fluid_row<ND>(c, nc, blk_ptr, row0, ix, jf_ip, jf_ix, jf_a, neg_res, a, b);
+        if (m && missing) atomicAdd(missing, m);
+    }
+}
+
+// Row pattern of the four-field system for dimension nd and the flux pattern fp (nc x nc, sorted rows).
+static int tpsa_poro_build_pattern(pb_facegrid *g, int nd, const CsrView &fp) {
+    cudaStream_t st = g->stream;
+    const int64_t nc = g->nc;
+    const int B = nd == 3 ? 8 : 5;
+    const TpsaTopo t = tpsa_topo(g);
+    if (!g->nb_ready) {
+        int32_t total = 0;
+        int rc = tpsa_neighbour_counts(g, &total);
+        if (rc) return rc;
+        tpsa_nb_list_kernel<<<fg_grid(nc), 256, 0, st>>>(t, g->cc_ptr.as<int32_t>(), g->cc_ix.as<int32_t>(),
+                                                          g->cc_cell.as<int32_t>());
+        pb_count_launch_();
+        CUDA_TRY(cudaGetLastError());
+        g->sys_npairs = total;
+        g->nb_ready = true;
+    }
+    DevBuf count, scratch;
+    CUDA_TRY(count.ensure((size_t)(nc + 1) * sizeof(int64_t)));
+    CUDA_TRY(cudaMemsetAsync(count.as<int64_t>() + nc, 0, sizeof(int64_t), st));
+    if (nd == 3) tpsa_poro_count_kernel<3><<<fg_grid(nc), 256, 0, st>>>(nc, g->cc_ptr.as<int32_t>(), fp.indptr, fp.indices, count.as<int64_t>());
+    else tpsa_poro_count_kernel<2><<<fg_grid(nc), 256, 0, st>>>(nc, g->cc_ptr.as<int32_t>(), fp.indptr, fp.indices, count.as<int64_t>());
+    pb_count_launch_();
+    CUDA_TRY(cudaGetLastError());
+    CUDA_TRY(g->blk_ptr.ensure((size_t)(nc + 1) * sizeof(int64_t)));
+    size_t tmp_bytes = 0;
+    CUDA_TRY(cub::DeviceScan::ExclusiveSum(nullptr, tmp_bytes, count.as<int64_t>(), g->blk_ptr.as<int64_t>(),
+                                           (int)(nc + 1), st));
+    CUDA_TRY(scratch.ensure(tmp_bytes));
+    CUDA_TRY(cub::DeviceScan::ExclusiveSum(scratch.p, tmp_bytes, count.as<int64_t>(), g->blk_ptr.as<int64_t>(),
+                                           (int)(nc + 1), st));
+    int64_t nnz = 0;
+    CUDA_TRY(cudaMemcpyAsync(&nnz, g->blk_ptr.as<int64_t>() + nc, sizeof(int64_t), cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(cudaStreamSynchronize(st));
+    if (nnz >= 0x7FFFFFFFll) return pb_fail_(PB_ENOTIMPL, "Tpsa system: the matrix does not fit int32 indices");
+    CUDA_TRY(g->poro_ip.ensure((size_t)(nc * B + 1) * sizeof(int32_t)));
+    CUDA_TRY(g->poro_ix.ensure((size_t)std::max<int64_t>(1, nnz) * sizeof(int32_t)));
+    const int32_t last = (int32_t)nnz;
+    CUDA_TRY(cudaMemcpyAsync(g->poro_ip.as<int32_t>() + nc * B, &last, sizeof(int32_t), cudaMemcpyHostToDevice, st));
+    if (nd == 3)
+        tpsa_poro_pattern_kernel<3><<<fg_grid(nc), 256, 0, st>>>(nc, g->cc_ptr.as<int32_t>(), g->cc_ix.as<int32_t>(),
+                                                                  g->blk_ptr.as<int64_t>(), fp.indptr, fp.indices,
+                                                                  g->poro_ip.as<int32_t>(), g->poro_ix.as<int32_t>());
+    else
+        tpsa_poro_pattern_kernel<2><<<fg_grid(nc), 256, 0, st>>>(nc, g->cc_ptr.as<int32_t>(), g->cc_ix.as<int32_t>(),
+                                                                  g->blk_ptr.as<int64_t>(), fp.indptr, fp.indices,
+                                                                  g->poro_ip.as<int32_t>(), g->poro_ix.as<int32_t>());
+    pb_count_launch_();
+    CUDA_TRY(cudaGetLastError());
+    CUDA_TRY(cudaStreamSynchronize(st));
+    g->poro_nd = nd;
+    g->poro_nnz = nnz;
+    g->poro_fp_nnz = fp.nnz;
+    return PB_OK;
+}
+
+extern "C" int pb_tpsa_poro_system(pb_facegrid *g, int nd, const double *mu, const double *lambda, const double *alpha,
+                                   const double *cell_volumes, const uint8_t *codes, const double *robin_diag,
+                                   const uint8_t *face_flags, const pb_csr *flux_pattern, pb_csr **out,
+                                   float *stage_ms) {
+    if (!g || !mu || !lambda || !alpha || !cell_volumes || !codes || !face_flags || !flux_pattern || !out)
+        return pb_fail_(PB_EINVAL, "null pointer");
+    const int64_t nc = g->nc;
+    for (int64_t c = 0; c < nc; ++c)
+        if (!std::isfinite(alpha[c])) return pb_fail_(PB_EINVAL, "Biot coefficient alpha must be finite");
+    const CsrView fp = pb_csr_view_(flux_pattern);
+    if (fp.nrows != nc || fp.ncols != nc) return pb_fail_(PB_EINVAL, "flux pattern must be num_cells x num_cells");
+    TpsaInputs in;
+    int rc = tpsa_prepare(g, nd, mu, lambda, cell_volumes, codes, robin_diag, face_flags, in);
+    if (rc) return rc;
+    if (g->poro_nd != nd || g->poro_fp_nnz != fp.nnz) {
+        g->poro_nd = 0;
+        if ((rc = tpsa_poro_build_pattern(g, nd, fp))) return rc;
+    }
+    cudaStream_t st = g->stream;
+    const int B = nd == 3 ? 8 : 5;
+    DevBuf dal;
+    CUDA_TRY(dal.upload(alpha, (size_t)nc, st));
+    pb_csr *a = nullptr;
+    rc = pb_csr_from_device_pattern_(nc * B, nc * B, g->poro_nnz, g->poro_ip.as<int32_t>(), g->poro_ix.as<int32_t>(), &a);
+    if (rc) return rc;
+    FgEvents ev;
+    auto fail_cuda = [&](cudaError_t e, const char *what) {
+        pb_csr_destroy(a);
+        return pb_fail_(PB_ECUDA, std::string(what) + ": " + cudaGetErrorString(e));
+    };
+#define SYS_TRY(x) do { cudaError_t e_ = (x); if (e_ != cudaSuccess) return fail_cuda(e_, #x); } while (0)
+    if (stage_ms)
+        for (auto &x : ev.e) SYS_TRY(cudaEventCreate(&x));
+    if (stage_ms) SYS_TRY(cudaEventRecord(ev.e[0], st));
+    TpsaTerms T{};
+    if ((rc = tpsa_face_terms(g, nd, in, T))) { pb_csr_destroy(a); return rc; }
+    if (stage_ms) SYS_TRY(cudaEventRecord(ev.e[1], st));
+    const TpsaTopo t = tpsa_topo(g);
+    const int64_t np = g->sys_npairs;
+    if (nd == 3)
+        tpsa_poro_system_kernel<3><<<fg_grid(np), 256, 0, st>>>(np, t, g->cc_ptr.as<int32_t>(), g->cc_ix.as<int32_t>(),
+                                                                 g->cc_cell.as<int32_t>(), g->blk_ptr.as<int64_t>(), T,
+                                                                 in.mu.as<double>(), in.lam.as<double>(),
+                                                                 dal.as<double>(), in.vol.as<double>(), pb_csr_data_(a));
+    else
+        tpsa_poro_system_kernel<2><<<fg_grid(np), 256, 0, st>>>(np, t, g->cc_ptr.as<int32_t>(), g->cc_ix.as<int32_t>(),
+                                                                 g->cc_cell.as<int32_t>(), g->blk_ptr.as<int64_t>(), T,
+                                                                 in.mu.as<double>(), in.lam.as<double>(),
+                                                                 dal.as<double>(), in.vol.as<double>(), pb_csr_data_(a));
+    pb_count_launch_();
+    SYS_TRY(cudaGetLastError());
+    if (stage_ms) SYS_TRY(cudaEventRecord(ev.e[2], st));
+    SYS_TRY(cudaStreamSynchronize(st));
+    if (stage_ms) {
+        SYS_TRY(cudaEventElapsedTime(stage_ms, ev.e[0], ev.e[1]));
+        SYS_TRY(cudaEventElapsedTime(stage_ms + 1, ev.e[1], ev.e[2]));
+    }
+#undef SYS_TRY
+    g->terms_nd = nd;
+    *out = a;
+    return PB_OK;
+}
+
+extern "C" int pb_tpsa_poro_rhs(pb_facegrid *g, const double *bc_values, const double *body_force,
+                                const double *angular_source, const double *mass_source, double *rhs_dev) {
+    if (!g || !bc_values || !rhs_dev) return pb_fail_(PB_EINVAL, "null pointer");
+    const int nd = g->poro_nd;
+    if ((nd != 2 && nd != 3) || g->terms_nd != nd) return pb_fail_(PB_EINVAL, "pb_tpsa_poro_system has not been called");
+    const int64_t nf = g->nf, nc = g->nc;
+    const int nr = nd == 3 ? 3 : 1;
+    cudaStream_t st = g->stream;
+    DevBuf dg, df, dsr, dsp;
+    CUDA_TRY(dg.upload(bc_values, (size_t)nd * nf, st));
+    if (body_force) CUDA_TRY(df.upload(body_force, (size_t)nd * nc, st));
+    if (angular_source) CUDA_TRY(dsr.upload(angular_source, (size_t)nr * nc, st));
+    if (mass_source) CUDA_TRY(dsp.upload(mass_source, (size_t)nc, st));
+    TpsaTerms T{};
+    for (int k = PB_TPSA_BOUND_STRESS; k <= PB_TPSA_BOUND_MASS_DISPLACEMENT; ++k) T.t[k] = g->terms[k].as<double>();
+    const TpsaTopo t = tpsa_topo(g);
+    const int64_t rows = nc * (nd + nr + 2);
+    const double *pf = body_force ? df.as<double>() : nullptr, *psr = angular_source ? dsr.as<double>() : nullptr,
+                 *psp = mass_source ? dsp.as<double>() : nullptr;
+    if (nd == 3) tpsa_poro_rhs_kernel<3><<<fg_grid(rows), 256, 0, st>>>(t, T, dg.as<double>(), pf, psr, psp, rhs_dev);
+    else tpsa_poro_rhs_kernel<2><<<fg_grid(rows), 256, 0, st>>>(t, T, dg.as<double>(), pf, psr, psp, rhs_dev);
+    pb_count_launch_();
+    CUDA_TRY(cudaGetLastError());
+    CUDA_TRY(cudaStreamSynchronize(st));
+    return PB_OK;
+}
+
+extern "C" int pb_tpsa_poro_fluid_rows(pb_facegrid *g, pb_csr *a, const pb_csr *jf, const double *neg_res_dev,
+                                       double *rhs_dev, int *missing_dev, uint64_t stream) {
+    if (!g || !a || !jf || !neg_res_dev || !rhs_dev) return pb_fail_(PB_EINVAL, "null pointer");
+    const int nd = g->poro_nd;
+    if (nd != 2 && nd != 3) return pb_fail_(PB_EINVAL, "pb_tpsa_poro_system has not been called");
+    const int64_t nc = g->nc;
+    const int B = nd == 3 ? 8 : 5;
+    const CsrView va = pb_csr_view_(a), vj = pb_csr_view_(jf);
+    if (va.nrows != nc * B || va.ncols != nc * B || va.nnz != g->poro_nnz)
+        return pb_fail_(PB_EINVAL, "the matrix is not the TPSA poromechanics system of this grid");
+    if (vj.nrows != nc || vj.ncols != 2 * nc)
+        return pb_fail_(PB_EINVAL, "fluid Jacobian must be num_cells x 2 num_cells ([p_t | p])");
+    cudaStream_t st = (cudaStream_t)stream;
+    if (nd == 3)
+        tpsa_poro_fluid_kernel<3><<<fg_grid(nc), 256, 0, st>>>(nc, g->cc_ptr.as<int32_t>(), g->blk_ptr.as<int64_t>(),
+                                                                va.indices, vj.indptr, vj.indices, vj.data, neg_res_dev,
+                                                                va.data, rhs_dev, missing_dev);
+    else
+        tpsa_poro_fluid_kernel<2><<<fg_grid(nc), 256, 0, st>>>(nc, g->cc_ptr.as<int32_t>(), g->blk_ptr.as<int64_t>(),
+                                                                va.indices, vj.indptr, vj.indices, vj.data, neg_res_dev,
+                                                                va.data, rhs_dev, missing_dev);
+    pb_count_launch_();
+    CUDA_TRY(cudaGetLastError());
     return PB_OK;
 }

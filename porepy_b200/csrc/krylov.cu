@@ -57,8 +57,9 @@ __global__ void kry_init_kernel(int64_t n, const double *__restrict__ b, double 
 
 // Preconditioner application z = M^-1 y on one block of BS consecutive entries: BS == 1 -- minv holds the inverse
 // diagonal (Jacobi); BS > 1 -- minv holds the inverted BS x BS diagonal blocks, row-major (block Jacobi: the nd
-// displacement components of a cell in the mechanics system A = div_nd @ stress, or the nd + nr + 1 unknowns [u, r, p]
-// of a cell in the TPSA system, BS = 4 in 2-D and 7 in 3-D).
+// displacement components of a cell in the mechanics system A = div_nd @ stress, the nd + nr + 1 unknowns [u, r, p]
+// of a cell in the TPSA system, BS = 4 in 2-D and 7 in 3-D, or the nd + nr + 2 unknowns [u, r, p_t, p] of a cell in the
+// TPSA poromechanics system, BS = 5 and 8).
 template <int BS>
 __device__ __forceinline__ void apply_minv(const double *__restrict__ minv, int64_t b, const double (&y)[BS], double (&z)[BS]) {
     if (!minv) {
@@ -180,19 +181,22 @@ extern "C" int pb_kry_seed(double *scal, uint64_t stream) {
     CUDA_TRY(cudaGetLastError());
     return PB_OK;
 }
-static bool kry_block_size_ok(int bs) { return bs == 1 || bs == 2 || bs == 3 || bs == 4 || bs == 7; }
+static bool kry_block_size_ok(int bs) { return (bs >= 1 && bs <= 5) || bs == 7 || bs == 8; }
 
-// bs: size of the diagonal blocks of the preconditioner (1 = Jacobi, 2 / 3 / 4 / 7 = block Jacobi; n must be a multiple)
+// bs: size of the diagonal blocks of the preconditioner (1 = Jacobi, 2 / 3 / 4 / 5 / 7 / 8 = block Jacobi; n must be a
+// multiple)
 extern "C" int pb_kry_p(int64_t n, const double *r, double *p, const double *v, const double *minv, double *ph,
                         double *scal, int cur, int bs, uint64_t stream) {
     if (!kry_block_size_ok(bs) || n % bs)
-        return pb_fail_(PB_EINVAL, "pb_kry_p: block size must be 1, 2, 3, 4 or 7 and divide n");
+        return pb_fail_(PB_EINVAL, "pb_kry_p: block size must be 1, 2, 3, 4, 5, 7 or 8 and divide n");
     cudaStream_t st = (cudaStream_t)stream;
     if (bs == 1) kry_p_kernel<1><<<kgrid(n), 256, 0, st>>>(n, r, p, v, minv, ph, scal, cur & 1);
     else if (bs == 2) kry_p_kernel<2><<<kgrid(n / 2), 256, 0, st>>>(n, r, p, v, minv, ph, scal, cur & 1);
     else if (bs == 3) kry_p_kernel<3><<<kgrid(n / 3), 256, 0, st>>>(n, r, p, v, minv, ph, scal, cur & 1);
     else if (bs == 4) kry_p_kernel<4><<<kgrid(n / 4), 256, 0, st>>>(n, r, p, v, minv, ph, scal, cur & 1);
-    else kry_p_kernel<7><<<kgrid(n / 7), 256, 0, st>>>(n, r, p, v, minv, ph, scal, cur & 1);
+    else if (bs == 5) kry_p_kernel<5><<<kgrid(n / 5), 256, 0, st>>>(n, r, p, v, minv, ph, scal, cur & 1);
+    else if (bs == 7) kry_p_kernel<7><<<kgrid(n / 7), 256, 0, st>>>(n, r, p, v, minv, ph, scal, cur & 1);
+    else kry_p_kernel<8><<<kgrid(n / 8), 256, 0, st>>>(n, r, p, v, minv, ph, scal, cur & 1);
     pb_count_launch_();
     CUDA_TRY(cudaGetLastError());
     return PB_OK;
@@ -200,13 +204,15 @@ extern "C" int pb_kry_p(int64_t n, const double *r, double *p, const double *v, 
 extern "C" int pb_kry_s(int64_t n, const double *r, const double *v, const double *minv, double *s, double *sh,
                         double *scal, int cur, int bs, uint64_t stream) {
     if (!kry_block_size_ok(bs) || n % bs)
-        return pb_fail_(PB_EINVAL, "pb_kry_s: block size must be 1, 2, 3, 4 or 7 and divide n");
+        return pb_fail_(PB_EINVAL, "pb_kry_s: block size must be 1, 2, 3, 4, 5, 7 or 8 and divide n");
     cudaStream_t st = (cudaStream_t)stream;
     if (bs == 1) kry_s_kernel<1><<<kgrid(n), 256, 0, st>>>(n, r, v, minv, s, sh, scal, cur & 1);
     else if (bs == 2) kry_s_kernel<2><<<kgrid(n / 2), 256, 0, st>>>(n, r, v, minv, s, sh, scal, cur & 1);
     else if (bs == 3) kry_s_kernel<3><<<kgrid(n / 3), 256, 0, st>>>(n, r, v, minv, s, sh, scal, cur & 1);
     else if (bs == 4) kry_s_kernel<4><<<kgrid(n / 4), 256, 0, st>>>(n, r, v, minv, s, sh, scal, cur & 1);
-    else kry_s_kernel<7><<<kgrid(n / 7), 256, 0, st>>>(n, r, v, minv, s, sh, scal, cur & 1);
+    else if (bs == 5) kry_s_kernel<5><<<kgrid(n / 5), 256, 0, st>>>(n, r, v, minv, s, sh, scal, cur & 1);
+    else if (bs == 7) kry_s_kernel<7><<<kgrid(n / 7), 256, 0, st>>>(n, r, v, minv, s, sh, scal, cur & 1);
+    else kry_s_kernel<8><<<kgrid(n / 8), 256, 0, st>>>(n, r, v, minv, s, sh, scal, cur & 1);
     pb_count_launch_();
     CUDA_TRY(cudaGetLastError());
     return PB_OK;
@@ -272,6 +278,78 @@ __global__ void block_diag_inv_kernel(int64_t nb, const int32_t *__restrict__ ip
     }
 }
 
+// BS = 8: the same inverse and fallback, Gauss-Jordan in place (the pivot rows are recorded and the columns of the
+// result swapped back at the end), so one 8 x 8 block instead of two stays in registers.
+template <int BS>
+__global__ void block_diag_inv_inplace_kernel(int64_t nb, const int32_t *__restrict__ ip, const int32_t *__restrict__ ix,
+                                              const double *__restrict__ data, double *__restrict__ out) {
+    for (int64_t b = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; b < nb; b += (int64_t)gridDim.x * blockDim.x) {
+        double D[BS][BS];
+#pragma unroll
+        for (int i = 0; i < BS; ++i) {
+#pragma unroll
+            for (int j = 0; j < BS; ++j) D[i][j] = 0.0;
+            const int64_t row = b * BS + i;
+            for (int q = ip[row]; q < ip[row + 1]; ++q) {
+                const int64_t c = (int64_t)ix[q] - b * BS;
+                if (c >= 0 && c < BS) {
+#pragma unroll
+                    for (int j = 0; j < BS; ++j) if (c == j) D[i][j] += data[q];
+                }
+            }
+        }
+        double dg[BS];
+        int perm[BS];
+#pragma unroll
+        for (int i = 0; i < BS; ++i) { dg[i] = D[i][i]; perm[i] = i; }
+        bool ok = true;
+#pragma unroll
+        for (int k = 0; k < BS; ++k) {
+            int piv = k;
+            double best = fabs(D[k][k]);
+#pragma unroll
+            for (int i = k + 1; i < BS; ++i) if (fabs(D[i][k]) > best) { best = fabs(D[i][k]); piv = i; }
+            ok = ok && best > 0.0;   // no early exit: the loop stays unrolled and D in registers
+            if (!ok) continue;
+            perm[k] = piv;
+#pragma unroll
+            for (int i = k + 1; i < BS; ++i)
+                if (i == piv) {
+#pragma unroll
+                    for (int j = 0; j < BS; ++j) { const double t = D[k][j]; D[k][j] = D[i][j]; D[i][j] = t; }
+                }
+            const double inv = 1.0 / D[k][k];
+            D[k][k] = 1.0;
+#pragma unroll
+            for (int j = 0; j < BS; ++j) D[k][j] *= inv;
+#pragma unroll
+            for (int i = 0; i < BS; ++i) {
+                if (i == k) continue;
+                const double f = D[i][k];
+                D[i][k] = 0.0;
+#pragma unroll
+                for (int j = 0; j < BS; ++j) D[i][j] -= f * D[k][j];
+            }
+        }
+        // row swap k <-> perm[k] of the block is column swap k <-> perm[k] of its inverse, undone in reverse order:
+        // column j of D goes to column pos[j] (a scattered store instead of register moves indexed by perm)
+        int pos[BS];
+#pragma unroll
+        for (int j = 0; j < BS; ++j) pos[j] = j;
+#pragma unroll
+        for (int k = BS - 1; k >= 0; --k)
+#pragma unroll
+            for (int j = 0; j < BS; ++j) pos[j] = pos[j] == k ? perm[k] : (pos[j] == perm[k] ? k : pos[j]);
+#pragma unroll
+        for (int i = 0; i < BS; ++i)
+#pragma unroll
+            for (int j = 0; j < BS; ++j) {
+                if (ok) out[(b * BS + i) * BS + pos[j]] = D[i][j];
+                else out[(b * BS + i) * BS + j] = i == j ? (dg[i] != 0.0 ? 1.0 / dg[i] : 1.0) : 0.0;
+            }
+    }
+}
+
 struct CsrView { int64_t nrows, ncols, nnz; int32_t *indptr, *indices; double *data; };
 CsrView pb_csr_view_(const pb_csr *a);   // spmv.cu
 extern "C" int pb_csr_block_diag_inv_dev(const pb_csr *a, int bs, int64_t nblocks, double *out_dev, uint64_t stream) {
@@ -285,7 +363,9 @@ extern "C" int pb_csr_block_diag_inv_dev(const pb_csr *a, int bs, int64_t nblock
     else if (bs == 2) block_diag_inv_kernel<2><<<grid, 256, 0, st>>>(nblocks, v.indptr, v.indices, v.data, out_dev);
     else if (bs == 3) block_diag_inv_kernel<3><<<grid, 256, 0, st>>>(nblocks, v.indptr, v.indices, v.data, out_dev);
     else if (bs == 4) block_diag_inv_kernel<4><<<grid, 256, 0, st>>>(nblocks, v.indptr, v.indices, v.data, out_dev);
-    else block_diag_inv_kernel<7><<<grid, 256, 0, st>>>(nblocks, v.indptr, v.indices, v.data, out_dev);
+    else if (bs == 5) block_diag_inv_kernel<5><<<grid, 256, 0, st>>>(nblocks, v.indptr, v.indices, v.data, out_dev);
+    else if (bs == 7) block_diag_inv_kernel<7><<<grid, 256, 0, st>>>(nblocks, v.indptr, v.indices, v.data, out_dev);
+    else block_diag_inv_inplace_kernel<8><<<grid, 256, 0, st>>>(nblocks, v.indptr, v.indices, v.data, out_dev);
     pb_count_launch_();
     CUDA_TRY(cudaGetLastError());
     return PB_OK;

@@ -416,7 +416,8 @@ def tpsa_momentum_from_model(model):
     if len(sds) != 1:
         raise NotImplementedError("TpsaElasticity: one subdomain is expected")
     if "mass_balance_equation" in es.equations:
-        raise NotImplementedError("TpsaElasticity: the TPSA poromechanics model (four fields) is not supported")
+        raise NotImplementedError("TpsaElasticity: the TPSA poromechanics model (four fields) is not supported; use "
+                                  "tpsa_poromechanics_from_model")
     sd = sds[0]
     nd, nc = sd.dim, sd.num_cells
     if nd not in (2, 3):
@@ -438,4 +439,54 @@ def tpsa_momentum_from_model(model):
     rows = _row_map(model, order)
     prob.column_map = interleave(cols, nd, nr, nc)
     prob.row_map = interleave([rows[:nd * nc], rows[nd * nc:(nd + nr) * nc], rows[(nd + nr) * nc:]], nd, nr, nc)
+    return prob, prob.column_map, prob.row_map
+
+
+def tpsa_poromechanics_from_model(model):
+    """A prepared ``pp.Poromechanics`` with ``TpsaPoromechanicsMixin`` on one 2-D or 3-D grid without fractures ->
+    (``TpsaPoromechanics``, column_map, row_map): unknown k of the problem (cell-interleaved [u_c, r_c, p_t_c, p_c]) is
+    dof ``column_map[k]`` of the model's ``EquationSystem``, equation k its row ``row_map[k]``.  The mechanical boundary
+    operator, body force, sources, Darcy and fluid-flux boundary data are the model's own operators, evaluated."""
+    from .tpsa_poromech import TpsaPoromechanics, interleave
+    mdg, es = model.mdg, model.equation_system
+    sds = list(mdg.subdomains())
+    if any(sd.dim < model.nd for sd in sds) or any(True for _ in mdg.interfaces()):
+        raise NotImplementedError("TpsaPoromechanics: fractures are not supported")
+    if len(sds) != 1:
+        raise NotImplementedError("TpsaPoromechanics: one subdomain is expected")
+    sd = sds[0]
+    nd, nc, nf = sd.dim, sd.num_cells, sd.num_faces
+    if nd not in (2, 3):
+        raise NotImplementedError("Tpsa is only implemented for 2d and 3d grids.")
+    nr = model.rotation_dimension()
+    fk, mk = model.darcy_keyword, model.stress_keyword
+    data = _own_data(mdg.subdomain_data(sd), [fk, mk])
+    fluid = _fluid(model, False)
+    w, _ = _boundary_weights(model, sd, fluid, False)
+    bc_ff = model.bc_type_fluid_flux(sd)
+    so = model.solid
+    solid = dict(reference_porosity=so.porosity, biot_coefficient=_evaluated(model, model.biot_coefficient([sd]), nc),
+                 bulk_modulus=float(np.atleast_1d(_evaluated(model, model.bulk_modulus([sd]), 1))[0]))
+    prob = TpsaPoromechanics(
+        sd, data, fluid, solid,
+        _face_values(model, sd, data[PARAMETERS][fk]["bc"], model.bc_values_pressure, model.bc_values_darcy_flux),
+        _evaluated(model, model.combine_boundary_operators_mechanical_stress([sd]), nd * nf), bc_ff,
+        _face_values(model, sd, bc_ff, w, model.bc_values_fluid_flux),
+        body_force=_evaluated(model, model.body_force([sd]), nd * nc),
+        angular_source=_evaluated(model, model.source_angular_momentum([sd]), nr * nc),
+        mass_source=_evaluated(model, model.solid_mass_source([sd]), nc),
+        fluid_source=_evaluated(model, model.fluid_source([sd]), nc), flow_keyword=fk, mechanics_keyword=mk)
+    prob.mobility_keyword = "b200_mobility"
+
+    def dofs(name):
+        return es.dofs_of([v for v in es.variables if v.name == name and v.domain is sd])
+    cols = [dofs(model.displacement_variable), dofs(model.rotation_stress_variable), dofs(model.total_pressure_variable),
+            dofs(model.pressure_variable)]
+    solid_mass = [eq for eq in es.equations if eq.lower().startswith("solid_mass_equation")][0]
+    order = [("momentum_balance_equation", [(sd, nd)]), ("angular_momentum_balance_equation", [(sd, nr)]),
+             (solid_mass, [(sd, 1)]), ("mass_balance_equation", [(sd, 1)])]
+    rows = _row_map(model, order)
+    prob.column_map = interleave(cols, nd, nr, nc)
+    o = np.cumsum([0, nd * nc, nr * nc, nc, nc])
+    prob.row_map = interleave([rows[o[i]:o[i + 1]] for i in range(4)], nd, nr, nc)
     return prob, prob.column_map, prob.row_map

@@ -185,7 +185,7 @@ def _prec_blocks(a, bs):
     return minv.ravel(), (lambda y: np.einsum("bij,bj->bi", minv, y.reshape(-1, bs)).ravel())
 
 
-PRECS = [None, 1, 2, 3, 4, 7]
+PRECS = [None, 1, 2, 3, 4, 5, 7, 8]
 
 
 # ---------------------------------------------------------------------------------------------------------------------
@@ -688,7 +688,7 @@ def test_bmat_many_block_rows_empty_blocks_and_none():
 # 4. block inverses
 # ---------------------------------------------------------------------------------------------------------------------
 @pytest.mark.gpu
-@pytest.mark.parametrize("bs", [1, 2, 3, 4, 7])
+@pytest.mark.parametrize("bs", [1, 2, 3, 4, 5, 7, 8])
 def test_block_inverse_partial_rectangular_duplicates(bs):
     """nblocks < nrows / bs on a rectangular matrix; entries outside the diagonal blocks (also beyond the square part)
     are ignored, duplicate in-block entries summed.  Residual |E D - I|_inf <= c bs u kappa_inf(D); a singular block
@@ -731,6 +731,79 @@ def test_block_inverse_partial_rectangular_duplicates(bs):
         res = np.abs(np.asarray(got[k], LD) @ np.asarray(dk, LD) - eye).sum(axis=1).max()
         kappa = np.abs(dk).sum(axis=1).max() * np.abs(np.linalg.inv(dk)).sum(axis=1).max()
         assert float(res) <= 8 * bs * U * kappa, (bs, k, float(res), kappa)
+
+
+def _gj_pivots(d):
+    """Row swaps and pivot magnitudes of Gauss-Jordan with partial pivoting in float64, as the block-inverse kernels
+    choose them (first row of the largest magnitude)."""
+    d = np.array(d, dtype=np.float64)
+    n = d.shape[0]
+    perm, best = [], []
+    for k in range(n):
+        piv = k + int(np.argmax(np.abs(d[k:, k])))
+        perm.append(piv), best.append(abs(d[piv, k]))
+        if not best[-1] > 0.0:
+            break
+        d[[k, piv]] = d[[piv, k]]
+        d[k] /= d[k, k]
+        for i in range(n):
+            if i != k:
+                d[i] -= d[i, k] * d[k]
+    return perm, best
+
+
+def _blocks8():
+    """Two 8 x 8 blocks for the in-place kernel's deferred column permutation:
+    cyclic -- a scaled cyclic shift plus a small perturbation: pivoting swaps at every step k < 7 and the swaps
+    compose to one 8-cycle;
+    last_singular -- small integers with power-of-two pivots, the last row the sum of rows 1 and 4: elimination is
+    exact and the pivot at k = 7 is exactly 0 after seven regular steps."""
+    rng = np.random.default_rng(47)
+    cyclic = np.zeros((8, 8))
+    cyclic[np.arange(8), (np.arange(8) + 1) % 8] = rng.uniform(2.0, 4.0, 8) * rng.choice([-1.0, 1.0], 8)
+    cyclic += 1e-2 * rng.uniform(-1.0, 1.0, (8, 8))
+    last = np.triu(rng.integers(-2, 3, (8, 8)).astype(np.float64), 1)
+    last[np.arange(7), np.arange(7)] = 8.0 * rng.choice([-1.0, 1.0], 7)
+    last[7] = last[1] + last[4]
+    return cyclic, last
+
+
+def test_block8_cases_pivot_as_intended():
+    cyclic, last = _blocks8()
+    perm, best = _gj_pivots(cyclic)
+    assert all(perm[k] != k for k in range(7)) and len(best) == 8 and min(best) > 0.5
+    order = np.arange(8)
+    for k, p in enumerate(perm):
+        order[[k, p]] = order[[p, k]]
+    seen, j = {0}, int(order[0])
+    while j != 0:
+        seen.add(j)
+        j = int(order[j])
+    assert len(seen) == 8, "the row swaps form a single cycle"
+    perm, best = _gj_pivots(last)
+    assert len(best) == 8 and min(best[:7]) > 0 and best[7] == 0.0
+
+
+@pytest.mark.gpu
+def test_block_inverse_8_cyclic_pivoting_and_last_pivot_singular():
+    """The in-place 8 x 8 Gauss-Jordan on a block that swaps rows at every step (its inverse needs the whole deferred
+    column permutation) and on one that is singular only at the last pivot (the diagonal fallback, with the ``ok``
+    flag carried through the unrolled loop)."""
+    cyclic, last = _blocks8()
+    rng = np.random.default_rng(48)
+    regular = rng.standard_normal((8, 8)) + 16 * np.eye(8)
+    blocks = [cyclic, last, regular, cyclic.T]
+    a = sps.csr_matrix(sps.block_diag([sps.csr_matrix(b) for b in blocks]))
+    got = _dev(a).block_diagonal_inverse(8).cpu().numpy().reshape(len(blocks), 8, 8)
+    eye = np.eye(8, dtype=LD)
+    for k, dk in enumerate(blocks):
+        if k == 1:
+            dg = np.diagonal(dk)
+            assert np.array_equal(got[k], np.diag(np.where(dg != 0, 1.0 / np.where(dg != 0, dg, 1.0), 1.0)))
+            continue
+        res = np.abs(np.asarray(got[k], LD) @ np.asarray(dk, LD) - eye).sum(axis=1).max()
+        kappa = np.abs(dk).sum(axis=1).max() * np.abs(np.linalg.inv(dk)).sum(axis=1).max()
+        assert float(res) <= 8 * 8 * U * kappa, (k, float(res), kappa)
 
 
 # ---------------------------------------------------------------------------------------------------------------------

@@ -96,9 +96,24 @@ static int64_t cfg_scratch(int cfg, int n) {
     }
 }
 
-// size_of(nsf, nsc, nb, &n, &w, &a_doubles, &rest_doubles)
+// doubles of the solver pool of a routine that hands its system to solve_rows (node_kernels.cuh)
+static int64_t cfg_pool(int cfg, int n, int w) {
+    switch (cfg) {
+        case 0: return Cfg0::pool_doubles(n, w);
+        case 1: return Cfg1::pool_doubles(n, w);
+        case 2: return Cfg2::pool_doubles(n, w);
+        case 3: return Cfg3::pool_doubles(n, w);
+        case 4: return Cfg4::pool_doubles(n, w);
+        case 5: return Cfg5::pool_doubles(n, w);
+        default: return Cfg6::pool_doubles(n, w);
+    }
+}
+
+// size_of(nsf, nsc, nb, &n, &w, &a_doubles, &rest_doubles).  With rows_to_solver the routine fills the solver's pool
+// row by row (solve_rows) and a_doubles is the size of that pool; otherwise it is the full augmented matrix A.  Either
+// way a node's class, including whether its A goes to a global-memory workspace, is decided on the full A.
 template <class F>
-static int build_classes(pb_plan *p, std::vector<NodeClass> &out, F size_of) {
+static int build_classes(pb_plan *p, std::vector<NodeClass> &out, bool rows_to_solver, F size_of) {
     const HostPlan &H = p->H;
     // key: cfg*2 + a_global
     std::vector<int32_t> lists[2 * kNumCfg];
@@ -122,7 +137,7 @@ static int build_classes(pb_plan *p, std::vector<NodeClass> &out, F size_of) {
                                          " sub-faces)");
         int key = cfg * 2 + (glob ? 1 : 0);
         lists[key].push_back((int32_t)s);
-        amax[key] = std::max(amax[key], a);
+        amax[key] = std::max(amax[key], rows_to_solver ? cfg_pool(cfg, n, w) : a);
         rmax[key] = std::max(rmax[key], r);
         smax[key] = std::max(smax[key], scr);
     }
@@ -158,7 +173,7 @@ static int build_classes(pb_plan *p, std::vector<NodeClass> &out, F size_of) {
 
 static int build_mpfa_classes(pb_plan *p) {
     const int nd = p->H.nd;
-    return build_classes(p, p->mpfa_cls, [&](int nsf, int nsc, int nb, int *n, int *w, int64_t *a, int64_t *r) {
+    return build_classes(p, p->mpfa_cls, false, [&](int nsf, int nsc, int nb, int *n, int *w, int64_t *a, int64_t *r) {
         *n = nsf;
         *w = mpfa_width(nd, nsf, nsc, nb);
         *a = mpfa_A_doubles(nd, nsf, nsc, nb);
@@ -1228,8 +1243,8 @@ extern "C" int pb_mpsa_upload(pb_plan *p, const double *stiffness, const uint8_t
     p->n_alpha = n_alpha;
     p->veta = eta;
     if (p->mpsa_cls_nalpha != n_alpha) {
-        int rc = build_classes(p, p->mpsa_cls, [&](int nsf, int nsc, int nb, int *n, int *w, int64_t *a,
-                                                   int64_t *r) {
+        int rc = build_classes(p, p->mpsa_cls, true, [&](int nsf, int nsc, int nb, int *n, int *w, int64_t *a,
+                                                         int64_t *r) {
             *n = nsf * nd;
             *w = mpsa_width(nd, nsf, nsc, nb, n_alpha);
             *a = mpsa_A_doubles(nd, nsf, nsc, nb, n_alpha);

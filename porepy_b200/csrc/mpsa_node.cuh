@@ -58,7 +58,7 @@ PB_HD bool sym_mask(int p, int q) {
 
 template <int ND, class Solver, class Team>
 PB_HD void mpsa_node(Team &t, const PlanView &P, const GeoView &G, const MpsaParams &prm,
-                     const MpsaOut &o, int64_t s, double *A, double *smd, double *scratch, int *err,
+                     const MpsaOut &o, int64_t s, double *pool, double *smd, double *scratch, int *err,
                      int64_t s_next = -1) {
     constexpr int ND2 = ND * ND;
     const int sc0 = P.node_sc_ptr[s], nsc = P.node_sc_ptr[s + 1] - sc0;
@@ -70,7 +70,6 @@ PB_HD void mpsa_node(Team &t, const PlanView &P, const GeoView &G, const MpsaPar
     const int ncc = nsc * ND;        // cell-displacement columns
     const int nbc = nb * ND;         // boundary-value columns
     const int nrhs = ncc + nbc + nal * nsc;
-    const int W = (n + nrhs) | 1;
     const int64_t nf = P.nf, nc = P.nc, nn = P.nn;
 
     double *PS = smd;                           // [k][p][a][m]
@@ -116,7 +115,6 @@ PB_HD void mpsa_node(Team &t, const PlanView &P, const GeoView &G, const MpsaPar
         }
     }
     for (int x = t.tid(); x < n; x += t.size()) rowidx[x] = x;
-    for (int i = t.tid(); i < n * W; i += t.size()) A[i] = 0.0;
     for (int i = t.tid(); i < ND2 * (n + ncc); i += t.size()) SA[i] = 0.0;
     t.sync();
 
@@ -260,15 +258,15 @@ PB_HD void mpsa_node(Team &t, const PlanView &P, const GeoView &G, const MpsaPar
     }
     t.sync();
 
-    // ---- phase 4: one row per (sub-face, component)
-    for (int x = t.tid(); x < n; x += t.size()) {
+    // ---- phase 4: row x = (sub-face, component) of the local system, handed to the solver row by row (the solver
+    // scales it to unit 1-norm, matrix_operations.py:1880-1906)
+    auto row_of = [&](int x, double *row) {
         const int u = x / ND, i = x - u * ND;
-        double *row = A + (int64_t)x * W;
         const int code = bcu[x];
         if (code == 1 && prm.basis == nullptr) {  // Dirichlet component: ubar_{u,i} = u_b
             row[x] = 1.0;
             row[n + ncc + bloc[u] * ND + i] = 1.0;
-            continue;
+            return;
         }
         const double *nu = nrm + u * ND;
         if (prm.basis != nullptr && bloc[u] >= 0) {
@@ -339,12 +337,7 @@ PB_HD void mpsa_node(Team &t, const PlanView &P, const GeoView &G, const MpsaPar
                     }
                 }
             }
-            double sum = 0.0;
-            for (int c = 0; c < n; ++c) sum += fabs(row[c]);
-            if (!(sum > 0.0)) { flag_singular(err, s); continue; }
-            const double is = 1.0 / sum;
-            for (int c = 0; c < n + nrhs; ++c) row[c] *= is;
-            continue;
+            return;
         }
         for (int sd = 0; sd < 2; ++sd) {
             const int side = sd == 0 ? (sides[u] & 0xFFFF) : ((sides[u] >> 16) & 0xFFFF);
@@ -396,16 +389,12 @@ PB_HD void mpsa_node(Team &t, const PlanView &P, const GeoView &G, const MpsaPar
                 row[u * ND + j] += as * w;
             }
         }
-        double sum = 0.0;
-        for (int c = 0; c < n; ++c) sum += fabs(row[c]);
-        if (!(sum > 0.0)) { flag_singular(err, s); continue; }
-        const double is = 1.0 / sum;
-        for (int c = 0; c < n + nrhs; ++c) row[c] *= is;
-    }
-    t.sync();
+    };
 
-    // ---- phase 5: solve
-    if (!Solver::solve(t, A, n, W, nrhs, rowidx, scratch)) {
+    // ---- phase 5: solve; X[rowidx[x]*ldx + c] is the solution
+    const double *X;
+    int ldx;
+    if (!Solver::solve_rows(t, row_of, n, nrhs, pool, rowidx, scratch, X, ldx)) {
         if (t.tid() == 0) flag_singular(err, s);
         t.sync();
         return;
@@ -439,7 +428,7 @@ PB_HD void mpsa_node(Team &t, const PlanView &P, const GeoView &G, const MpsaPar
                 const int k = k0 + (l & 3);
                 const double a0 = (row0 < ND2 && k < n) ? SA[row0 * n + k] : 0.0;
                 const double a1 = (row1 < ND2 && k < n) ? SA[row1 * n + k] : 0.0;
-                const double b = (k < n && colb < nrhs) ? A[(int64_t)rowidx[k] * W + n + colb] : 0.0;
+                const double b = (k < n && colb < nrhs) ? X[rowidx[k] * ldx + colb] : 0.0;
                 pb_dmma2(acc0, acc1, a0, a1, b);
             }
             const int c0 = 8 * tc + 2 * (l & 3);
@@ -459,7 +448,7 @@ PB_HD void mpsa_node(Team &t, const PlanView &P, const GeoView &G, const MpsaPar
     for (int it = t.tid(); it < ND2 * nrhs; it += t.size()) {
         const int p = it / nrhs, c = it - p * nrhs;
         double v = (c < ncc) ? SAc[p * ncc + c] : 0.0;
-        for (int x = 0; x < n; ++x) v += SA[p * n + x] * A[(int64_t)rowidx[x] * W + n + c];
+        for (int x = 0; x < n; ++x) v += SA[p * n + x] * X[(int64_t)rowidx[x] * ldx + c];
         Z[it] = v;
     }
 #endif
@@ -512,14 +501,14 @@ PB_HD void mpsa_node(Team &t, const PlanView &P, const GeoView &G, const MpsaPar
 #pragma unroll
         for (int a = 0; a < ND; ++a)
 #pragma unroll
-            for (int m = 0; m < ND; ++m) xo[a][m] = rowidx[(slot[k1 * ND + m] >> 1) * ND + a] * W + n;
+            for (int m = 0; m < ND; ++m) xo[a][m] = rowidx[(slot[k1 * ND + m] >> 1) * ND + a] * ldx;
         bool use_asym[ND];
         int uo[ND];
 #pragma unroll
         for (int i = 0; i < ND; ++i) {
             const int code = bcu[u * ND + i];
             use_asym[i] = !((code == 2 && elim[i]) || (code == 3 && elim[ND + i]));
-            uo[i] = rowidx[u * ND + i] * W + n;
+            uo[i] = rowidx[u * ND + i] * ldx;
         }
         const double im = invmf[u];
         const int64_t f = face[u];
@@ -533,7 +522,7 @@ PB_HD void mpsa_node(Team &t, const PlanView &P, const GeoView &G, const MpsaPar
             for (int a = 0; a < ND; ++a)
 #pragma unroll
                 for (int m = 0; m < ND; ++m) {
-                    const double xv = A[xo[a][m] + c];
+                    const double xv = X[xo[a][m] + c];
 #pragma unroll
                     for (int i = 0; i < ND; ++i) hk[i] += hs[i][a][m] * xv;
                 }
@@ -543,7 +532,7 @@ PB_HD void mpsa_node(Team &t, const PlanView &P, const GeoView &G, const MpsaPar
 #pragma unroll
                     for (int r = 0; r < ND; ++r) hk[i] += nu[r] * Z[(i * ND + r) * nrhs + c];
                 }
-                tr[i] = A[uo[i] + c] * im;
+                tr[i] = X[uo[i] + c] * im;
             }
             if (c < ncc) {
                 const int k = c / ND, j = c - k * ND;
@@ -624,7 +613,7 @@ PB_HD void mpsa_node(Team &t, const PlanView &P, const GeoView &G, const MpsaPar
             for (int a = 0; a < ND; ++a)
 #pragma unroll
                 for (int m = 0; m < ND; ++m)
-                    xr[a][m] = A + (int64_t)rowidx[(slot[k * ND + m] >> 1) * ND + a] * W + n;
+                    xr[a][m] = X + (int64_t)rowidx[(slot[k * ND + m] >> 1) * ND + a] * ldx;
             for (int c = t.lane(); c < nrhs; c += t.lanes()) {
                 double v = 0.0;
 #pragma unroll

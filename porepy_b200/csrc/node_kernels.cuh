@@ -142,16 +142,52 @@ PB_HD bool gauss_jordan(Team &t, double *A, int n, int W, int nrhs, int *rowidx,
     return ok;
 }
 
+// The augmented system assembled by the row routine `fill` (see solve_rows below) in A, one thread per row, each row
+// scaled to unit 1-norm of its n system columns
+template <class Team, class Fill>
+PB_HD void fill_system(Team &t, const Fill &fill, int n, int nrhs, double *A, int W) {
+    for (int i = t.tid(); i < n * W; i += t.size()) A[i] = 0.0;
+    t.sync();
+    for (int x = t.tid(); x < n; x += t.size()) {
+        double *row = A + (int64_t)x * W;
+        fill(x, row);
+        double sum = 0.0;
+        for (int c = 0; c < n; ++c) sum += fabs(row[c]);
+        if (sum > 0.0) {
+            const double is = 1.0 / sum;
+            for (int c = 0; c < n + nrhs; ++c) row[c] *= is;
+        }
+    }
+    t.sync();
+}
+
 // Solver policies.  `solve` leaves X(p, c) = A[rowidx[p]*W + n + c].
+//
+// `solve_rows` takes the system row by row from a routine instead of a whole A:
+//   void fill(int x, double *row)  writes row x of the augmented system (the n system columns, then the nrhs
+//                                  right-hand sides) into `row`, which is zeroed and at least n + nrhs wide.
+// Each row is scaled to unit 1-norm of its n system columns; a row without a positive norm is left as it is (it makes
+// the system singular).  `pool` holds pool_doubles(n, W) doubles, W = (n + nrhs) | 1.  On return
+// X[rowidx[p]*ldx + c] is the solution.
 struct SmemGJ {
     // Gauss-Jordan directly on the shared (or global) memory copy of A: works for any size
     // and on the host (kernel emulation); the slow path on the GPU.
     static constexpr int team = 256;
     static constexpr int min_blocks = 1;
     static PB_HD int64_t scratch_doubles(int n) { return n; }
+    static PB_HD int64_t pool_doubles(int n, int W) { return (int64_t)n * W; }
     template <class Team>
     static PB_HD bool solve(Team &t, double *A, int n, int W, int nrhs, int *rowidx, double *scratch) {
         return gauss_jordan(t, A, n, W, nrhs, rowidx, scratch);
+    }
+    template <class Team, class Fill>
+    static PB_HD bool solve_rows(Team &t, const Fill &fill, int n, int nrhs, double *pool, int *rowidx,
+                                 double *scratch, const double *&X, int &ldx) {
+        const int W = (n + nrhs) | 1;
+        fill_system(t, fill, n, nrhs, pool, W);
+        X = pool + n;
+        ldx = W;
+        return gauss_jordan(t, pool, n, W, nrhs, rowidx, scratch);
     }
 };
 
@@ -359,6 +395,21 @@ struct TileGJ {
     }
 
 
+    // Row stride of the compact solution block of solve_rows: 4 mod 16 doubles, so that the 4 rows x 4 columns
+    // that a half-warp reads in the m16n8k4 B fragments of phase 6 (mpsa_node.cuh) fall in distinct banks.
+    static PB_HD int x_stride(int nrhs) { return ((nrhs + 11) / 16) * 16 + 4; }
+    // Teams of one or two warps (the hexahedral configurations) assemble the whole A and solve it: filled one tile per
+    // warp at a time their rows would go through the row routine in 3 passes of 8 lanes instead of one pass of the
+    // team (Cartesian 64^3: MPSA 16 % slower), and their A is small (<= 48 x 96 doubles).
+    static constexpr bool kFillTiles = NW > 2;
+    // the solution block, or the per-warp fill buffers (one row tile of the augmented system each) before it is written
+    static PB_HD int64_t pool_doubles(int n, int W) {
+        if (!kFillTiles) return (int64_t)n * W;
+        const int64_t x = (int64_t)n * x_stride(W - n), f = (int64_t)NW * 8 * W;
+        return x > f ? x : f;
+    }
+
+    // the same elimination on a full A: X(p, c) = A[rowidx[p]*W + n + c]
     template <class Team>
     static __device__ __forceinline__ bool solve(Team &t, double *A, int n, int W, int nrhs,
                                                  int *rowidx, double *scratch) {
@@ -376,6 +427,97 @@ struct TileGJ {
                 c[rt][tc][1] = (myrow < n && col + 1 < wend) ? A[myrow * W + col + 1] : 0.0;
             }
         }
+        if (!eliminate(t, c, n, rowidx, scratch)) return false;
+        store(t, c, n, nrhs, A + n, W);
+        return true;
+    }
+
+    // The augmented system goes from the row routine straight into the tiles: each warp fills the rows of its row
+    // tiles, one tile (8 rows, lanes 0-7) at a time, in a private buffer of the pool, takes their 1-norms with 4
+    // lanes per row and its fragments from there; only the columns >= n of the result are written, to a compact block at the
+    // start of the pool.
+    template <class Team, class Fill>
+    static __device__ __forceinline__ bool solve_rows(Team &t, const Fill &fill, int n, int nrhs, double *pool,
+                                                      int *rowidx, double *scratch, const double *&X, int &ldx) {
+        const int ti = t.warp(), l = t.lane();
+        const int gr = l >> 2, gc = (l & 3) * 2;
+        const int wend = n + nrhs;
+        const int W = wend | 1;
+        if constexpr (!kFillTiles) {
+            fill_system(t, fill, n, nrhs, pool, W);
+            X = pool + n;
+            ldx = W;
+            return solve(t, pool, n, W, nrhs, rowidx, scratch);
+        }
+        double *buf = pool + (int64_t)ti * 8 * W;
+        double c[RT][NCT][2];
+#pragma unroll
+        for (int rt = 0; rt < RT; ++rt)
+#pragma unroll
+            for (int tc = 0; tc < NCT; ++tc) c[rt][tc][0] = c[rt][tc][1] = 0.0;
+        // one pass per row tile, not unrolled: the row routine is inlined once
+#pragma unroll 1
+        for (int ps = 0; ps < RT; ++ps) {
+            const int r0 = 8 * (ti + NW * ps);
+            if (r0 >= n) break;
+            for (int i = l; i < 8 * W; i += 32) buf[i] = 0.0;
+            __syncwarp();
+            if (l < 8 && r0 + l < n) fill(r0 + l, buf + l * W);
+            __syncwarp();
+            const double *row = buf + gr * W;
+            double sum = 0.0;
+            for (int cc = l & 3; cc < n; cc += 4) sum += fabs(row[cc]);
+            sum += __shfl_xor_sync(0xffffffffu, sum, 1);
+            sum += __shfl_xor_sync(0xffffffffu, sum, 2);
+            const double is = sum > 0.0 ? 1.0 / sum : 1.0;
+            const int myrow = r0 + gr;
+#pragma unroll
+            for (int rt = 0; rt < RT; ++rt) {
+                if (rt == ps && myrow < n) {
+#pragma unroll
+                    for (int tc = 0; tc < NCT; ++tc) {
+                        const int col = 8 * tc + gc;
+                        if (col < wend) c[rt][tc][0] = row[col] * is;
+                        if (col + 1 < wend) c[rt][tc][1] = row[col + 1] * is;
+                    }
+                }
+            }
+            __syncwarp();
+        }
+        if (!eliminate(t, c, n, rowidx, scratch)) return false;
+        ldx = x_stride(nrhs);
+        store(t, c, n, nrhs, pool, ldx);
+        X = pool;
+        return true;
+    }
+
+    // the solution columns of the tiles: X[row*ldx + c] for c < nrhs
+    template <class Team>
+    static __device__ __forceinline__ void store(Team &t, const double (&c)[RT][NCT][2], int n, int nrhs,
+                                                 double *X, int ldx) {
+        const int ti = t.warp(), l = t.lane();
+        const int gr = l >> 2, gc = (l & 3) * 2;
+#pragma unroll
+        for (int rt = 0; rt < RT; ++rt) {
+            const int myrow = 8 * (ti + NW * rt) + gr;
+#pragma unroll
+            for (int tc = 0; tc < NCT; ++tc) {
+                const int col = 8 * tc + gc - n;
+                if (myrow < n) {
+                    if (col >= 0 && col < nrhs) X[myrow * ldx + col] = c[rt][tc][0];
+                    if (col + 1 >= 0 && col + 1 < nrhs) X[myrow * ldx + col + 1] = c[rt][tc][1];
+                }
+            }
+        }
+        t.sync();
+    }
+
+    // Gauss-Jordan on the tiles; false (uniform over the team) when the system is singular
+    template <class Team>
+    static __device__ __forceinline__ bool eliminate(Team &t, double (&c)[RT][NCT][2], int n, int *rowidx,
+                                                     double *scratch) {
+        const int ti = t.warp(), l = t.lane();
+        const int gr = l >> 2, gc = (l & 3) * 2;
         double *P0 = scratch;              // [NP][4]  panel columns
         double *Raw = P0 + NP * 4;         // [4][WP]  raw pivot rows
         double *R = Raw + 4 * WP;          // [4][WP]  A11^-1 * pivot rows
@@ -504,21 +646,7 @@ struct TileGJ {
             }
         }
         t.sync();
-        if (!ok) return false;
-#pragma unroll
-        for (int rt = 0; rt < RT; ++rt) {
-            const int myrow = 8 * (ti + NW * rt) + gr;
-#pragma unroll
-            for (int tc = 0; tc < NCT; ++tc) {
-                const int col = 8 * tc + gc;
-                if (myrow < n) {
-                    if (col >= n && col < wend) A[myrow * W + col] = c[rt][tc][0];
-                    if (col + 1 >= n && col + 1 < wend) A[myrow * W + col + 1] = c[rt][tc][1];
-                }
-            }
-        }
-        t.sync();
-        return true;
+        return ok;
     }
 };
 #endif

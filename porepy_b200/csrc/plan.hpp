@@ -240,9 +240,22 @@ static int launch_one(K kernel, const NodeClass &c, pb_plan *p, const Prm &prm, 
         return pb_fail_(PB_ENOTIMPL, "interaction region needs " + std::to_string(smem) +
                                      " B of shared memory (> 227 KB)");
     CUDA_TRY(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    // occupancy with the whole carve-out available (the preference set below stays with the kernel)
+    CUDA_TRY(cudaFuncSetAttribute(kernel, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutDefault));
     int per_sm = 1;
     CUDA_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, blk, smem));
     if (per_sm < 1) per_sm = 1;
+    // The part of the SM's 256 KB of unified memory that is not shared memory is L1, which holds the register
+    // spills and the gathers of the node routines: ask for the smallest H100 shared-memory carve-out (KB) that keeps
+    // per_sm CTAs, each with its 1 KB system reserve.  The percentage is rounded up to a carve-out by the driver.
+    {
+        static const int kCarveKB[] = {0, 8, 16, 32, 64, 100, 132, 164, 196, 228};
+        const size_t need = (smem + 1024) * (size_t)per_sm;
+        int pct = 100;
+        for (int kb : kCarveKB)
+            if ((size_t)kb * 1024 >= need) { pct = kb * 100 / 228; break; }
+        CUDA_TRY(cudaFuncSetAttribute(kernel, cudaFuncAttributePreferredSharedMemoryCarveout, pct));
+    }
     int64_t need = ((int64_t)c.n + tpb - 1) / tpb;
     int grid = (int)std::max<int64_t>(1, std::min<int64_t>(need, (int64_t)pb_sm_count() * per_sm));
     double *ws = nullptr;

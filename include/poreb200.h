@@ -454,6 +454,35 @@ int pb_csr_block_diag_inv_dev(const pb_csr *a, int bs, int64_t nblocks, double *
 int pb_kry_xr(int64_t n, double *x, const double *ph, const double *sh, const double *s, const double *t, double *r,
               const double *rhat, double *scal, int cur, int carry /* 1 on exactly one rank */, uint64_t stream);
 
+/* ---- restarted GMRES(m) with a grouped block-Jacobi preconditioner (csrc/gmres.cu): the device solve of the Newton
+ * updates of the fractured contact models.  All pointers except `a` are DEVICE pointers.
+ * Groups: gptr (ngroups + 1, int64) into grows / gcols (int32): group g is rows grows[gptr[g] .. gptr[g+1]) and columns
+ * gcols[same range], of equal size <= 32; the groups partition all rows and all columns (checked by the caller).
+ * inv_off (int64, ngroups): offset of the row-major inverse of group g in `inv` (prefix sum of the squared sizes);
+ * grp_of (int32, n): the group of every position of the grouped order. */
+/* inverses of the blocks J[R_g, C_g] by Gauss-Jordan with partial pivoting; synchronises `stream`.  A zero or non-finite
+ * pivot returns PB_ESINGULAR naming the lowest failing group; status_dev: one int32 of device scratch. */
+int pb_group_inv_dev(const pb_csr *a, int64_t ngroups, const int64_t *gptr, const int32_t *grows, const int32_t *gcols,
+                     const int64_t *inv_off, int smax, double *inv_out, int32_t *status_dev, uint64_t stream);
+/* z[C_g] = inv_g y[R_g] for every group (accumulate != 0: z[C_g] +=) */
+int pb_group_apply_dev(int64_t n, const int32_t *grp_of, const int64_t *gptr, const int32_t *grows, const int32_t *gcols,
+                       const int64_t *inv_off, const double *inv, const double *y, double *z, int accumulate,
+                       uint64_t stream);
+/* doubles of the GMRES scalar buffer for restart length m (1 <= m <= 128), -1 otherwise */
+int64_t pb_gmres_scal_size(int m);
+/* V: (m + 1) n basis, z: n, partial: nblk (m + 2) per-block partial sums, scal: pb_gmres_scal_size(m).  init: x = 0,
+ * V_0 = b, |b| and the tolerance tol |b|.  step j (0 <= j < m): one Arnoldi step with CGS2 and the Givens update, a
+ * no-op once the cycle's DONE flag is set.  cycle_end: x += M^-1 V y, V_0 = b - A x and its norm (the next cycle's
+ * start).  inv == NULL: no preconditioner (the group arrays are not read). */
+int pb_gmres_init(int64_t n, int m, const double *b, double *x, double *V, double *partial, int nblk, double *scal,
+                  double tol, uint64_t stream);
+int pb_gmres_step(pb_csr *a, int64_t n, int m, int j, double *V, double *z, double *partial, int nblk, double *scal,
+                  const int32_t *grp_of, const int64_t *gptr, const int32_t *grows, const int32_t *gcols,
+                  const int64_t *inv_off, const double *inv, uint64_t stream);
+int pb_gmres_cycle_end(pb_csr *a, int64_t n, int m, const double *b, double *x, double *V, double *z, double *partial,
+                       int nblk, double *scal, const int32_t *grp_of, const int64_t *gptr, const int32_t *grows,
+                       const int32_t *gcols, const int64_t *inv_off, const double *inv, uint64_t stream);
+
 /* time `reps` device SpMVs with CUDA events on the launching stream; returns mean ms */
 int pb_csr_spmv_bench(pb_csr *a, int reps, float *mean_ms);
 

@@ -108,6 +108,15 @@ _SIGNATURES = {
     "pb_kry_s": (C.c_int, [C.c_int64] + [C.c_void_p] * 6 + [C.c_int, C.c_int, C.c_uint64]),
     "pb_csr_block_diag_inv_dev": (C.c_int, [C.c_void_p, C.c_int, C.c_int64, C.c_void_p, C.c_uint64]),
     "pb_kry_xr": (C.c_int, [C.c_int64] + [C.c_void_p] * 8 + [C.c_int, C.c_int, C.c_uint64]),
+    "pb_group_inv_dev": (C.c_int, [C.c_void_p, C.c_int64] + [C.c_void_p] * 4 + [C.c_int] + [C.c_void_p] * 2
+                         + [C.c_uint64]),
+    "pb_group_apply_dev": (C.c_int, [C.c_int64] + [C.c_void_p] * 8 + [C.c_int, C.c_uint64]),
+    "pb_gmres_scal_size": (C.c_int64, [C.c_int]),
+    "pb_gmres_init": (C.c_int, [C.c_int64, C.c_int] + [C.c_void_p] * 4 + [C.c_int, C.c_void_p, C.c_double, C.c_uint64]),
+    "pb_gmres_step": (C.c_int, [C.c_void_p, C.c_int64, C.c_int, C.c_int] + [C.c_void_p] * 3 + [C.c_int]
+                      + [C.c_void_p] * 7 + [C.c_uint64]),
+    "pb_gmres_cycle_end": (C.c_int, [C.c_void_p, C.c_int64, C.c_int] + [C.c_void_p] * 5 + [C.c_int]
+                           + [C.c_void_p] * 7 + [C.c_uint64]),
     "pb_csr_spmv_bench": (C.c_int, [C.c_void_p, C.c_int, _f32p]),
 }
 

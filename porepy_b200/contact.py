@@ -21,7 +21,8 @@ coordinates; constitutive_laws.py ``displacement_jump``).  ``maximum`` / ``l2_no
 ``porepy_b200.ad_functions`` with the reference's tie rules, so the Jacobian of the semismooth laws is the reference's.  The
 elastic fracture-deformation laws (Barton-Bandis closure, tangential stiffness) are off in the reference's defaults and not
 stated here.  The Jacobian has zeros on the diagonal of the complementarity rows: ``time_step`` takes the linear solver from
-the caller (the tests use a direct solve); a device Krylov method for this saddle-point system is future work.
+the caller.  ``krylov.gmres_solver(prob.preconditioner_groups())`` solves the updates on the device: restarted GMRES with a
+block-Jacobi over one group per matrix cell and one per fracture cell with its two mortar cells.
 ``tests/golden/contact_model.npz`` pins Jacobian, residual, residual history and the converged sliding state.
 """
 from __future__ import annotations
@@ -54,6 +55,32 @@ class FractureContact:
         self.rotation = sps.csr_matrix(local_coordinates)
         self.num_mortar = int(np.asarray(mortar_sign).size)
         self.num_cells = int(self.rotation.shape[0] // 3)
+        self.mortar_to_secondary = sps.csr_matrix(mortar_to_secondary_avg)
+
+
+def mortar_pairs(mortar_to_secondary) -> np.ndarray:
+    """(nfc, 2): the two mortar cells of every fracture cell, from the scalar ``mortar_to_secondary_avg``; a fracture cell
+    with another number of mortar cells raises ``ValueError``."""
+    m = sps.csr_matrix(mortar_to_secondary)
+    m.sort_indices()
+    count = np.diff(m.indptr)
+    if (count != 2).any():
+        k = int(np.flatnonzero(count != 2)[0])
+        raise ValueError(f"fracture cell {k} has {int(count[k])} mortar cells; the preconditioner groups need two")
+    return m.indices.reshape(-1, 2).astype(np.int64)
+
+
+def span(offset, index, width: int) -> np.ndarray:
+    """(len(index), width): the unknowns or equations ``offset + width * index + 0 .. width - 1``."""
+    return int(offset) + width * np.asarray(index, np.int64)[:, None] + np.arange(width)
+
+
+def block_groups(blocks):
+    """``krylov.BlockGroups`` from a list of (rows, cols) pairs of (number of groups, group size) arrays."""
+    from .krylov import BlockGroups
+    sizes = np.concatenate([np.full(r.shape[0], r.shape[1], np.int64) for r, _ in blocks])
+    return BlockGroups(np.concatenate(([0], np.cumsum(sizes))), np.concatenate([r.ravel() for r, _ in blocks]),
+                       np.concatenate([c.ravel() for _, c in blocks]))
 
 
 class FracturedMomentumBalance:
@@ -141,6 +168,25 @@ class FracturedMomentumBalance:
             tangential.append(((q.s2t @ b_p) * s - (q.s2t @ fn.maximum(b_p, fn.l2_norm(2, s))) * t_t) * (1.0 - chi)
                               + t_t * chi)
         return [momentum] + force + normal + tangential
+
+    def preconditioner_groups(self):
+        """Groups of the grouped block-Jacobi preconditioner of ``krylov.gmres`` in this problem's ordering: per matrix
+        cell c, momentum_c <-> u_c (3); per fracture cell k with mortar cells m1, m2, the normal and tangential laws of k
+        and the force balances of m1, m2 <-> t_k, u_j of m1, m2 (9)."""
+        nfr, nc = len(self.fractures), self.nc
+        eq = np.concatenate(([0], np.cumsum([3 * nc] + [3 * f.num_mortar for f in self.fractures]
+                                            + [f.num_cells for f in self.fractures]
+                                            + [2 * f.num_cells for f in self.fractures])))
+        cells = np.arange(nc)
+        blocks = [(span(eq[0], cells, 3), span(self.offsets[0], cells, 3))]
+        for j, fc in enumerate(self.fractures):
+            pair, k = mortar_pairs(fc.mortar_to_secondary), np.arange(fc.num_cells)
+            frc, jmp = eq[1 + j], self.offsets[1 + nfr + j]
+            rows = [span(eq[1 + nfr + j], k, 1), span(eq[1 + 2 * nfr + j], k, 2), span(frc, pair[:, 0], 3),
+                    span(frc, pair[:, 1], 3)]
+            cols = [span(self.offsets[1 + j], k, 3), span(jmp, pair[:, 0], 3), span(jmp, pair[:, 1], 3)]
+            blocks.append((np.hstack(rows), np.hstack(cols)))
+        return block_groups(blocks)
 
     def linearize(self, x, x_prev):
         """(J as ``DeviceCsr``, -R as a CUDA tensor) at the iterate ``x`` (previous time step ``x_prev``)."""

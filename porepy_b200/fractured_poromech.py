@@ -20,7 +20,7 @@ aperture (``operator_to_SecondOrderTensor``: the specific volume of the iterate;
 upwinding.  Unknowns: [p matrix | p fractures | u | contact tractions | lambda | u_j]; equations:
 [mass matrix | mass fractures | momentum | Darcy laws | force balances | normal laws | tangential laws] (the fixtures carry
 the maps to the reference's numbering).  One matrix subdomain, fractures without intersections; saddle-point Jacobian: the
-linear solver of ``time_step`` is the caller's.  ``tests/golden/contact_poromech*.npz`` pin Jacobian, residual, the residual
+linear solver of ``time_step`` is the caller's; ``krylov.gmres_solver(prob.preconditioner_groups())`` is the device one.  ``tests/golden/contact_poromech*.npz`` pin Jacobian, residual, the residual
 history of the semismooth Newton loop and the converged state.
 """
 from __future__ import annotations
@@ -31,6 +31,7 @@ import numpy as np
 import scipy.sparse as sps
 
 from . import ad, ad_functions as fn
+from .contact import block_groups, mortar_pairs, span
 from .fv import Biot, Mpfa, Upwind, UpwindCoupling
 from .params import DISCRETIZATION_MATRICES, PARAMETERS
 
@@ -266,6 +267,32 @@ class FracturedPoromechanics:
             tangential.append(((q.s2t @ b_p) * s - (q.s2t @ fn.maximum(b_p, fn.l2_norm(2, s))) * t_t) * (1.0 - chi)
                               + t_t * chi)
         return [mass3] + mass_f + [momentum] + darcy + force + normal + tangential
+
+    def _equation_offsets(self) -> np.ndarray:
+        nc, nfc, nm = self.nc, [f.num_cells for f in self.fractures], [f.num_mortar for f in self.fractures]
+        sizes = [nc] + nfc + [3 * nc] + nm + [3 * n for n in nm] + nfc + [2 * n for n in nfc]
+        return np.concatenate(([0], np.cumsum(sizes))).astype(np.int64)
+
+    def preconditioner_groups(self):
+        """Groups of the grouped block-Jacobi preconditioner of ``krylov.gmres`` in this problem's ordering: per matrix
+        cell c, mass_c and momentum_c <-> p_c, u_c (4); per fracture cell k with mortar cells m1, m2, the contact laws of
+        k, the force balances of m1, m2, the fracture mass balance of k and the Darcy laws of m1, m2 <-> t_k, u_j of
+        m1, m2, p_f of k, lambda of m1, m2 (12)."""
+        nfr, eq, var = len(self.fractures), self._equation_offsets(), self.offsets
+        cells = np.arange(self.nc)
+        blocks = [(np.hstack([span(eq[0], cells, 1), span(eq[1 + nfr], cells, 3)]),
+                   np.hstack([span(var[0], cells, 1), span(var[1 + nfr], cells, 3)]))]
+        for j, fc in enumerate(self.fractures):
+            pair, k = mortar_pairs(fc.p["mortar_to_secondary_avg"]), np.arange(fc.num_cells)
+            m1, m2 = pair[:, 0], pair[:, 1]
+            frc, darcy = eq[2 + 2 * nfr + j], eq[2 + nfr + j]
+            rows = [span(eq[2 + 3 * nfr + j], k, 1), span(eq[2 + 4 * nfr + j], k, 2), span(frc, m1, 3), span(frc, m2, 3),
+                    span(eq[1 + j], k, 1), span(darcy, m1, 1), span(darcy, m2, 1)]
+            jmp, lam = var[2 + 3 * nfr + j], var[2 + 2 * nfr + j]
+            cols = [span(var[2 + nfr + j], k, 3), span(jmp, m1, 3), span(jmp, m2, 3), span(var[1 + j], k, 1),
+                    span(lam, m1, 1), span(lam, m2, 1)]
+            blocks.append((np.hstack(rows), np.hstack(cols)))
+        return block_groups(blocks)
 
     def linearize(self, x, x_prev, dt: float):
         self.update_discretizations(x)

@@ -16,7 +16,8 @@ fracture's internal energy and in the interface Fourier law:
 Unknowns: [p matrix | p fractures | T matrix | T fractures | u | contact tractions | lambda | eta | eps | u_j]; equations:
 [mass matrix | mass fractures | energy matrix | energy fractures | momentum | Darcy laws | Fourier laws | enthalpy laws |
 force balances | normal laws | tangential laws].  ``tests/golden/contact_thm*.npz`` pin the Jacobian at the zero state and at
-the fourth Newton iterate, the residual history of the semismooth Newton loop and the converged state.
+the fourth Newton iterate, the residual history of the semismooth Newton loop and the converged state.  The Newton updates
+are solved on the device by ``krylov.gmres_solver(prob.preconditioner_groups())`` (17 unknowns per fracture-cell group).
 """
 from __future__ import annotations
 
@@ -25,6 +26,7 @@ from types import SimpleNamespace
 import numpy as np
 
 from . import ad, ad_functions as fn
+from .contact import block_groups, mortar_pairs, span
 from .fractured_poromech import FracturedPoromechanics
 from .fv import Mpfa, Upwind, UpwindCoupling
 from .params import DISCRETIZATION_MATRICES, PARAMETERS, SecondOrderTensor
@@ -50,6 +52,37 @@ class FracturedThermoporomechanics(FracturedPoromechanics):
         nm = [f.num_mortar for f in self.fractures]
         self.sizes = [self.nc] + nfc + [self.nc] + nfc + [3 * self.nc] + [3 * n for n in nfc] + nm + nm + nm + [3 * n for n in nm]
         self.offsets = np.concatenate(([0], np.cumsum(self.sizes))).astype(np.int64)
+
+    def preconditioner_groups(self):
+        """Groups of the grouped block-Jacobi preconditioner of ``krylov.gmres`` in this problem's ordering: per matrix
+        cell c, mass_c, energy_c and momentum_c <-> p_c, T_c, u_c (5); per fracture cell k with mortar cells m1, m2, the
+        twelve rows and columns of ``FracturedPoromechanics.preconditioner_groups`` plus the fracture energy balance of k
+        and the Fourier and enthalpy laws of m1, m2 <-> T_f of k, eta and eps of m1, m2 (17)."""
+        n, var = len(self.fractures), self.offsets
+        nc, nfc, nm = self.nc, [f.num_cells for f in self.fractures], [f.num_mortar for f in self.fractures]
+        sizes = [nc] + nfc + [nc] + nfc + [3 * nc] + nm + nm + nm + [3 * m for m in nm] + nfc + [2 * f for f in nfc]
+        eq = np.concatenate(([0], np.cumsum(sizes))).astype(np.int64)
+        # equation groups: mass | mass_f | energy | energy_f | momentum | darcy | fourier | enthalpy | force | normal |
+        # tangential; variable groups: p | p_f | T | T_f | u | t | lambda | eta | eps | u_j
+        e_mass, e_massf, e_en, e_enf, e_mom = 0, 1, 1 + n, 2 + n, 2 + 2 * n
+        e_darcy, e_four, e_enth, e_force, e_nrm, e_tan = (3 + 2 * n + q * n for q in range(6))
+        v_p, v_pf, v_t, v_tf, v_u = 0, 1, 1 + n, 2 + n, 2 + 2 * n
+        v_trac, v_lam, v_eta, v_eps, v_jmp = (3 + 2 * n + q * n for q in range(5))
+        cells = np.arange(nc)
+        blocks = [(np.hstack([span(eq[e_mass], cells, 1), span(eq[e_en], cells, 1), span(eq[e_mom], cells, 3)]),
+                   np.hstack([span(var[v_p], cells, 1), span(var[v_t], cells, 1), span(var[v_u], cells, 3)]))]
+        for j, fc in enumerate(self.fractures):
+            pair, k = mortar_pairs(fc.p["mortar_to_secondary_avg"]), np.arange(fc.num_cells)
+            m1, m2 = pair[:, 0], pair[:, 1]
+            pair_rows = lambda off, w: [span(off, m1, w), span(off, m2, w)]  # noqa: E731
+            rows = [span(eq[e_nrm + j], k, 1), span(eq[e_tan + j], k, 2), *pair_rows(eq[e_force + j], 3),
+                    span(eq[e_massf + j], k, 1), *pair_rows(eq[e_darcy + j], 1),
+                    span(eq[e_enf + j], k, 1), *pair_rows(eq[e_four + j], 1), *pair_rows(eq[e_enth + j], 1)]
+            cols = [span(var[v_trac + j], k, 3), *pair_rows(var[v_jmp + j], 3),
+                    span(var[v_pf + j], k, 1), *pair_rows(var[v_lam + j], 1),
+                    span(var[v_tf + j], k, 1), *pair_rows(var[v_eta + j], 1), *pair_rows(var[v_eps + j], 1)]
+            blocks.append((np.hstack(rows), np.hstack(cols)))
+        return block_groups(blocks)
 
     # ---- discretizations
     def _matrix_conductivity(self):

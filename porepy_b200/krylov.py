@@ -473,3 +473,194 @@ def solve_local(loc: LocalSystem, b_own, diag_own=None, tol: float = 1e-10, maxi
     x, info = bicgstab(op, b, tol=tol, maxiter=maxiter, diag_own=dg, block_inv=block_inv)
     info["halo_bytes_per_spmv"] = op.halo_bytes
     return x, info
+
+
+# ------------------------------------------------------------------------------------------
+# restarted GMRES with a grouped block-Jacobi preconditioner (csrc/gmres.cu): the Newton updates of the fractured contact
+# models, whose Jacobians have zero diagonals in the complementarity and force-balance rows
+# ------------------------------------------------------------------------------------------
+MAX_GROUP = 32
+MAX_RESTART = 128
+
+
+class BlockGroups:
+    """Groups of rows and columns of a square matrix: group g is rows ``rows[ptr[g]:ptr[g+1]]`` and columns
+    ``cols[ptr[g]:ptr[g+1]]``, at most 32 of each.  The groups must partition all rows and all columns; that is checked
+    here, on the host, and a violation raises ``ValueError``."""
+
+    def __init__(self, ptr, rows, cols):
+        ptr = np.asarray(ptr, dtype=np.int64).ravel()
+        rows = np.asarray(rows, dtype=np.int64).ravel()
+        cols = np.asarray(cols, dtype=np.int64).ravel()
+        if rows.size != cols.size:
+            raise ValueError(f"BlockGroups: {rows.size} rows but {cols.size} columns")
+        if ptr.size < 1 or ptr[0] != 0 or ptr[-1] != rows.size:
+            raise ValueError("BlockGroups: ptr must start at 0 and end at the number of rows")
+        sizes = np.diff(ptr)
+        if (sizes < 1).any():
+            raise ValueError(f"BlockGroups: group {int(np.flatnonzero(sizes < 1)[0])} is empty or ptr decreases")
+        if (sizes > MAX_GROUP).any():
+            g = int(np.flatnonzero(sizes > MAX_GROUP)[0])
+            raise ValueError(f"BlockGroups: group {g} has {int(sizes[g])} rows, more than {MAX_GROUP}")
+        n = rows.size
+        for what, ix in (("row", rows), ("column", cols)):
+            if n and (ix.min() < 0 or ix.max() >= n):
+                raise ValueError(f"BlockGroups: {what} index out of range 0 .. {n - 1}")
+            count = np.bincount(ix, minlength=n)
+            if (count > 1).any():
+                raise ValueError(f"BlockGroups: {what} {int(np.flatnonzero(count > 1)[0])} is in more than one group")
+            if (count == 0).any():
+                raise ValueError(f"BlockGroups: {what} {int(np.flatnonzero(count == 0)[0])} is in no group")
+        self.ptr, self.rows, self.cols, self.sizes = ptr, rows, cols, sizes
+        self.n, self.num_groups = int(n), int(sizes.size)
+        self.inv_offsets = np.concatenate(([0], np.cumsum(sizes * sizes))).astype(np.int64)
+        self._dev = None
+
+    def device_arrays(self):
+        """(ptr, rows, cols, group of every grouped position, inverse offsets) as CUDA tensors, uploaded once."""
+        if self._dev is None:
+            import torch
+            t = lambda a, dt: torch.as_tensor(np.ascontiguousarray(a), dtype=dt, device="cuda")  # noqa: E731
+            grp_of = np.repeat(np.arange(self.num_groups, dtype=np.int32), self.sizes)
+            self._dev = (t(self.ptr, torch.int64), t(self.rows, torch.int32), t(self.cols, torch.int32),
+                         t(grp_of, torch.int32), t(self.inv_offsets[:-1], torch.int64))
+        return self._dev
+
+
+class GroupedBlockJacobi:
+    """``M^-1 y``: ``z[C_g] = J[R_g, C_g]^-1 y[R_g]`` for every group of ``groups`` (``BlockGroups``), the inverses computed
+    on the device from ``A`` (``DeviceCsr``).  A block with a zero or non-finite pivot raises ``ValueError`` naming the
+    group."""
+
+    def __init__(self, A, groups: BlockGroups, stream: int = 0):
+        import ctypes as C
+        import torch
+        from . import _lib
+        if A.shape != (groups.n, groups.n):
+            raise ValueError(f"GroupedBlockJacobi: a {groups.n} x {groups.n} matrix is expected, got {A.shape}")
+        self.groups, self.lib = groups, _lib.load()
+        self.inv = torch.empty(int(groups.inv_offsets[-1]), dtype=torch.float64, device="cuda")
+        ptr, rows, cols, _, off = groups.device_arrays()
+        status = torch.empty(1, dtype=torch.int32, device="cuda")
+        P = lambda a: C.c_void_p(a.data_ptr())  # noqa: E731
+        _lib.check(self.lib.pb_group_inv_dev(A.h, groups.num_groups, P(ptr), P(rows), P(cols), P(off),
+                                             int(groups.sizes.max(initial=1)), P(self.inv), P(status),
+                                             stream or torch.cuda.current_stream().cuda_stream))
+
+    def block(self, g: int):
+        """The inverse of group ``g`` as an s x s CUDA tensor."""
+        o, s = self.groups.inv_offsets[g], int(self.groups.sizes[g])
+        return self.inv[o:o + s * s].reshape(s, s)
+
+    def pointers(self):
+        """Device addresses (group of every position, ptr, rows, cols, inverse offsets, inverses) in the order of the
+        GMRES entry points."""
+        ptr, rows, cols, grp_of, off = self.groups.device_arrays()
+        return [a.data_ptr() for a in (grp_of, ptr, rows, cols, off, self.inv)]
+
+    def apply(self, y, out=None):
+        import ctypes as C
+        import torch
+        from . import _lib
+        from .sparse import device_operand
+        y = device_operand(y, self.groups.n, "GroupedBlockJacobi.apply")
+        z = torch.empty_like(y) if out is None else device_operand(out, self.groups.n, "GroupedBlockJacobi.apply out")
+        _lib.check(self.lib.pb_group_apply_dev(self.groups.n, *[C.c_void_p(p) for p in self.pointers()],
+                                               C.c_void_p(y.data_ptr()), C.c_void_p(z.data_ptr()), 0,
+                                               torch.cuda.current_stream().cuda_stream))
+        return z
+
+
+def gmres(A, b, precond: GroupedBlockJacobi | None = None, tol: float = 1e-12, restart: int = 30,
+          maxiter: int = 1000):
+    """GMRES(restart) on the device for ``A x = b`` from x = 0, right-preconditioned by ``precond`` (or none): the
+    minimised residual is the true one.  ``A``: ``DeviceCsr``; ``b``: float64 CUDA tensor.  Arnoldi with classical
+    Gram-Schmidt and one re-orthogonalisation; every reduction is in a fixed order, so repeated solves are
+    bit-identical.  One cycle of ``restart`` steps is captured once as a CUDA graph and replayed; the host reads the
+    scalar buffer once per cycle and stops when the recomputed true residual ``|b - A x| / |b|`` is below ``tol``.
+    Returns (x, info) with ``iterations`` (Arnoldi steps), ``relres`` (true), ``converged``, ``breakdown``,
+    ``lucky_breakdown``, ``restarts`` (cycles), ``cuda_graph``, ``host_syncs``."""
+    import ctypes as C
+    import torch
+    from . import _lib
+    from .sparse import device_operand
+    if _dist_initialized():
+        import torch.distributed as dist
+        if dist.get_world_size() > 1:
+            raise NotImplementedError("krylov.gmres runs on one device; it has no distributed form")
+    n = int(A.shape[0])
+    if A.shape[1] != n:
+        raise ValueError(f"gmres: a square matrix is expected, got {A.shape}")
+    b = device_operand(b.contiguous() if torch.is_tensor(b) else b, n, "gmres: b")
+    if precond is not None and precond.groups.n != n:
+        raise ValueError("gmres: the preconditioner's groups do not match the matrix")
+    if restart < 1 or maxiter < 1:
+        raise ValueError("gmres: restart and maxiter must be positive")
+    m = min(int(restart), n, int(maxiter))
+    if m > MAX_RESTART:
+        raise ValueError(f"gmres: restart is limited to {MAX_RESTART}")
+    lib = _lib.load()
+    dev = b.device
+    nblk = int(max(1, min((n + 255) // 256, 4 * torch.cuda.get_device_properties(dev).multi_processor_count)))
+    x = torch.zeros(n, dtype=torch.float64, device=dev)
+    V = torch.empty((m + 1) * n, dtype=torch.float64, device=dev)
+    z = torch.empty(n, dtype=torch.float64, device=dev)
+    partial = torch.zeros(nblk * (m + 2), dtype=torch.float64, device=dev)
+    scal = torch.zeros(int(lib.pb_gmres_scal_size(m)), dtype=torch.float64, device=dev)
+    P = lambda a: C.c_void_p(a.data_ptr())  # noqa: E731
+    prec = [C.c_void_p(p) for p in precond.pointers()] if precond is not None else [None] * 6
+
+    def cycle(count):
+        stream = torch.cuda.current_stream().cuda_stream
+        for j in range(count):
+            _lib.check(lib.pb_gmres_step(A.h, n, m, j, P(V), P(z), P(partial), nblk, P(scal), *prec, stream))
+        _lib.check(lib.pb_gmres_cycle_end(A.h, n, m, P(b), P(x), P(V), P(z), P(partial), nblk, P(scal), *prec, stream))
+
+    _lib.check(lib.pb_gmres_init(n, m, P(b), P(x), P(V), P(partial), nblk, P(scal), float(tol),
+                                 torch.cuda.current_stream().cuda_stream))
+    h = scal[:16].cpu().numpy()
+    syncs = 1
+    if h[0] == 0.0:
+        return x, {"iterations": 0, "relres": 0.0, "converged": True, "breakdown": False, "lucky_breakdown": False,
+                   "restarts": 0, "cuda_graph": False, "host_syncs": syncs}
+    torch.cuda.synchronize()
+    graph = torch.cuda.CUDAGraph()                 # one whole cycle (m <= maxiter), replayed
+    with torch.cuda.graph(graph, stream=torch.cuda.Stream(device=dev)):
+        cycle(m)
+    it, restarts = 0, 0
+    relres, converged = float(np.sqrt(h[4] / h[0])), False
+    while it < maxiter:
+        count = min(m, maxiter - it)
+        if count == m:
+            graph.replay()
+        else:
+            cycle(count)
+        restarts += 1
+        h = scal[:16].cpu().numpy()         # the only host synchronisation: once per cycle
+        syncs += 1
+        steps, it = int(h[9]) - it, int(h[9])
+        relres = float(np.sqrt(h[4] / h[0])) if np.isfinite(h[4]) else float("inf")
+        if relres <= tol:
+            converged = True
+            break
+        if h[7] != 0.0 or steps == 0:       # breakdown, or a cycle that could not take a step
+            break
+    return x, {"iterations": it, "relres": relres, "converged": converged, "breakdown": bool(h[7] != 0.0),
+               "lucky_breakdown": bool(h[6] != 0.0), "restarts": restarts, "cuda_graph": True,
+               "host_syncs": syncs}
+
+
+def gmres_solver(groups: BlockGroups, tol: float = 1e-12, restart: int = 30, maxiter: int = 1000):
+    """A ``linear_solver(J, rhs) -> dx`` for the ``time_step`` of the fractured contact models (``groups``: their
+    ``preconditioner_groups()``): rebuilds the grouped block-Jacobi from every new ``J`` and solves with ``gmres``.  An
+    update that does not reach ``tol`` raises ``RuntimeError`` carrying the solver info; nothing inaccurate is
+    returned.  The info of the last solve is kept in ``solve.last_info``."""
+
+    def solve(J, rhs):
+        x, info = gmres(J, rhs, GroupedBlockJacobi(J, groups), tol=tol, restart=restart, maxiter=maxiter)
+        solve.last_info = info
+        if not info["converged"]:
+            raise RuntimeError(f"krylov.gmres did not converge: {info}")
+        return x
+    solve.last_info = None
+    return solve

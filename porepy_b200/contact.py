@@ -34,6 +34,7 @@ import scipy.sparse as sps
 
 from . import ad, ad_functions as fn
 from .fv import Mpsa
+from .newton import newton_loop
 from .params import DISCRETIZATION_MATRICES
 
 
@@ -83,6 +84,39 @@ def block_groups(blocks):
                        np.concatenate([c.ravel() for _, c in blocks]))
 
 
+def contact_operators(rotation, mortar_to_secondary, sign, secondary_to_mortar, volumes, characteristic_traction: float):
+    """Device operators of the contact laws of one fracture with n cells: ``sel_n`` / ``sel_t`` (normal / tangential
+    components of a local 3-vector per cell), ``s2t`` (one value per cell to its two tangential components), ``jump``
+    (u_j -> local displacement jump) and ``traction`` (contact traction -> force on the mortar cells).  ``rotation``:
+    ``local_coordinates``; ``mortar_to_secondary``, ``sign``, ``secondary_to_mortar``: the 3-component projections and
+    side signs; ``volumes``: mortar volumes, 3 per mortar cell."""
+    csr = ad.as_device_csr
+    n = rotation.shape[0] // 3
+    sel_n = sps.csr_matrix((np.ones(n), (np.arange(n), 3 * np.arange(n) + 2)), shape=(n, 3 * n))
+    sel_t = sps.csr_matrix((np.ones(2 * n), (np.arange(2 * n), 3 * np.repeat(np.arange(n), 2)
+                                             + np.tile([0, 1], n))), shape=(2 * n, 3 * n))
+    s2t = sps.csr_matrix((np.ones(2 * n), (np.arange(2 * n), np.repeat(np.arange(n), 2))), shape=(2 * n, n))
+    jump = rotation @ mortar_to_secondary @ sign
+    traction = sps.diags(volumes * characteristic_traction) @ sign @ secondary_to_mortar @ rotation.T
+    return dict(sel_n=csr(sel_n), sel_t=csr(sel_t), s2t=csr(s2t), jump=csr(jump), traction=csr(traction))
+
+
+def contact_laws(q, t, u_j, u_j_prev, c):
+    """(normal, tangential) complementarity laws of one fracture: ``q`` holds the ``contact_operators``, ``t`` and
+    ``u_j`` are the contact traction and the mortar displacement of the iterate, ``u_j_prev`` that of the previous time
+    step, ``c`` the contact constants."""
+    jump, jump_n = q.jump @ u_j, q.jump @ u_j_prev
+    t_n, u_n = q.sel_n @ t, q.sel_n @ jump
+    t_t, u_t, u_t_prev = q.sel_t @ t, q.sel_t @ jump, q.sel_t @ jump_n
+    gap = fn.l2_norm(2, u_t) * float(np.tan(c.dilation_angle)) + c.reference_gap
+    normal = t_n + fn.maximum(-t_n - (u_n - gap) * c.numerical_constant, 0.0)
+    s = t_t + (u_t - u_t_prev) * c.numerical_constant
+    b_p = fn.maximum(t_n * (-c.friction_coefficient), 0.0)
+    chi = q.s2t @ fn.characteristic_function(c.open_state_tolerance, b_p).val
+    tangential = ((q.s2t @ b_p) * s - (q.s2t @ fn.maximum(b_p, fn.l2_norm(2, s))) * t_t) * (1.0 - chi) + t_t * chi
+    return normal, tangential
+
+
 class FracturedMomentumBalance:
     """``sd``: the 3-D matrix grid (faces split along the fractures, ``fracture_faces`` tag), ``data``:
     ``parameters[keyword]`` with ``fourth_order_tensor`` and the vectorial ``bc`` (fracture faces Dirichlet,
@@ -126,15 +160,8 @@ class FracturedMomentumBalance:
                 outward=dev(np.repeat(out, 3)), f=dev(self.body_force), fr=[])
             k.stress_b = k.bound @ dev(self.bc_values)
             for fc in self.fractures:
-                n = fc.num_cells
-                sel_n = sps.csr_matrix((np.ones(n), (np.arange(n), 3 * np.arange(n) + 2)), shape=(n, 3 * n))
-                sel_t = sps.csr_matrix((np.ones(2 * n), (np.arange(2 * n), 3 * np.repeat(np.arange(n), 2)
-                                                         + np.tile([0, 1], n))), shape=(2 * n, 3 * n))
-                s2t = sps.csr_matrix((np.ones(2 * n), (np.arange(2 * n), np.repeat(np.arange(n), 2))), shape=(2 * n, n))
-                jump = fc.rotation @ fc.m2s @ fc.sign                            # u_j -> local displacement jump
-                trac = sps.diags(fc.volumes * self.k.characteristic_traction) @ fc.sign @ fc.s2m @ fc.rotation.T
-                k.fr.append(SimpleNamespace(m2p=csr(fc.m2p), p2m=csr(fc.p2m), jump=csr(jump), traction=csr(trac),
-                                            sel_n=csr(sel_n), sel_t=csr(sel_t), s2t=csr(s2t)))
+                k.fr.append(SimpleNamespace(m2p=csr(fc.m2p), p2m=csr(fc.p2m), **contact_operators(
+                    fc.rotation, fc.m2s, fc.sign, fc.s2m, fc.volumes, self.k.characteristic_traction)))
             self._const = k
         return self._const
 
@@ -157,16 +184,9 @@ class FracturedMomentumBalance:
         for j in range(nfr):
             q = k.fr[j]
             force.append((q.p2m @ (stress * k.outward)) + (q.traction @ t[j]))
-            jump, jump_n = q.jump @ uj[j], q.jump @ ujn[j]
-            t_n, u_n = q.sel_n @ t[j], q.sel_n @ jump
-            t_t, u_t, u_t_prev = q.sel_t @ t[j], q.sel_t @ jump, q.sel_t @ jump_n
-            gap = fn.l2_norm(2, u_t) * float(np.tan(c.dilation_angle)) + c.reference_gap
-            normal.append(t_n + fn.maximum(-t_n - (u_n - gap) * c.numerical_constant, 0.0))
-            s = t_t + (u_t - u_t_prev) * c.numerical_constant
-            b_p = fn.maximum(t_n * (-c.friction_coefficient), 0.0)
-            chi = q.s2t @ fn.characteristic_function(c.open_state_tolerance, b_p).val
-            tangential.append(((q.s2t @ b_p) * s - (q.s2t @ fn.maximum(b_p, fn.l2_norm(2, s))) * t_t) * (1.0 - chi)
-                              + t_t * chi)
+            nrm, tan = contact_laws(q, t[j], uj[j], ujn[j], c)
+            normal.append(nrm)
+            tangential.append(tan)
         return [momentum] + force + normal + tangential
 
     def preconditioner_groups(self):
@@ -194,18 +214,6 @@ class FracturedMomentumBalance:
 
     def time_step(self, x_prev, linear_solver, x0=None, tol: float = 1e-10, max_iterations: int = 30, verbose: bool = False):
         """Semismooth Newton from ``x0`` (default: the previous state); ``linear_solver(J, rhs) -> dx``."""
-        import torch
         x_prev = ad.device_vector(x_prev)
-        x = x_prev.clone() if x0 is None else ad.device_vector(x0).clone()
-        hist, r0 = [], None
-        for it in range(max_iterations + 1):
-            J, rhs = self.linearize(x, x_prev)
-            rn = float(torch.linalg.vector_norm(rhs))
-            r0 = rn if r0 is None else r0
-            hist.append({"iteration": it, "residual": rn})
-            if verbose:
-                print(hist[-1], flush=True)
-            if rn <= tol * max(r0, 1e-300) or it == max_iterations:
-                break
-            x = x + linear_solver(J, rhs)
-        return x, hist
+        x0 = x_prev if x0 is None else ad.device_vector(x0)
+        return newton_loop(lambda x: self.linearize(x, x_prev), x0, linear_solver, tol, max_iterations, verbose)

@@ -31,8 +31,10 @@ import numpy as np
 import scipy.sparse as sps
 
 from . import ad, ad_functions as fn
-from .contact import block_groups, mortar_pairs, span
-from .fv import Biot, Mpfa, Upwind, UpwindCoupling
+from .advection import advective_flux, rediscretize_upwind, rediscretize_upwind_coupling
+from .contact import block_groups, contact_laws, contact_operators, mortar_pairs, span
+from .fv import Biot, Mpfa
+from .newton import newton_loop
 from .params import DISCRETIZATION_MATRICES, PARAMETERS
 
 
@@ -124,15 +126,7 @@ class FracturedPoromechanics:
                 cons=csr(M["mpsa_consistency"][self.fk]), outward=dev(np.repeat(out, 3)),
                 bcq=dev(self.bc["flow"]), ubc=dev(self.bc["mechanics"]), bcw=dev(self.bc["fluid_flux"]), fr=[])
             for fc in self.fractures:
-                n, p = fc.num_cells, fc.p
-                sel_n = sps.csr_matrix((np.ones(n), (np.arange(n), 3 * np.arange(n) + 2)), shape=(n, 3 * n))
-                sel_t = sps.csr_matrix((np.ones(2 * n), (np.arange(2 * n), 3 * np.repeat(np.arange(n), 2)
-                                                         + np.tile([0, 1], n))), shape=(2 * n, 3 * n))
-                s2t = sps.csr_matrix((np.ones(2 * n), (np.arange(2 * n), np.repeat(np.arange(n), 2))), shape=(2 * n, n))
-                sign3 = sps.diags(np.repeat(fc.sign, 3))
-                jump = fc.rotation @ sps.kron(p["mortar_to_secondary_avg"], i3) @ sign3
-                trac = sps.diags(np.repeat(fc.volumes, 3) * self.ct.characteristic_traction) @ sign3 \
-                    @ sps.kron(p["secondary_to_mortar_int"], i3) @ fc.rotation.T
+                p = fc.p
                 # unit normal of the primary face of every mortar cell, pointing out of the matrix, times the mortar volume
                 pf = p["primary_to_mortar_avg"].tocsr().indices
                 n_out = np.asarray(self.sd.face_normals)[:, pf] / np.asarray(self.sd.face_areas)[pf] * out[pf]
@@ -144,10 +138,12 @@ class FracturedPoromechanics:
                     m2s=csr(p["mortar_to_secondary_int"]), s2m=csr(p["secondary_to_mortar_avg"]),
                     m2p3=csr(sps.kron(p["mortar_to_primary_avg"], i3).tocsr()),
                     p2m3=csr(sps.kron(p["primary_to_mortar_int"], i3).tocsr()),
-                    jump=csr(jump), traction=csr(trac), pressure_load=csr(pressure_load),
-                    sel_n=csr(sel_n), sel_t=csr(sel_t), s2t=csr(s2t), coef=dev(fc.volumes * fc.kappa * 2.0),
+                    pressure_load=csr(pressure_load), coef=dev(fc.volumes * fc.kappa * 2.0),
                     div=csr(sps.csr_matrix(fc.sd.cell_faces.T)), vol=dev(np.asarray(fc.sd.cell_volumes, float)),
-                    bc=None if fc.bc is None else {key: dev(v) for key, v in fc.bc.items() if not key.endswith("_type")}))
+                    bc=None if fc.bc is None else {key: dev(v) for key, v in fc.bc.items() if not key.endswith("_type")},
+                    **contact_operators(fc.rotation, sps.kron(p["mortar_to_secondary_avg"], i3),
+                                        sps.diags(np.repeat(fc.sign, 3)), sps.kron(p["secondary_to_mortar_int"], i3),
+                                        np.repeat(fc.volumes, 3), self.ct.characteristic_traction)))
             self._const = k
         return self._const
 
@@ -161,21 +157,23 @@ class FracturedPoromechanics:
             b = (k.fr[j].m2p3 @ uj[j]) + b
         return ((k.div_u @ u) + (k.div_u_b @ b) + (k.cons @ dp)) * k.inv_vol + dp * self.so.n_inv + self.so.reference_porosity
 
-    def _fracture_flux(self, fc, q, p):
-        """Darcy flux of a fracture: flux p (+ bound_flux p_b when the fracture carries boundary data)."""
-        F = fc.data[DISCRETIZATION_MATRICES][self.fk]
+    def _fracture_flux(self, fc, q, p, keyword=None, bc_key="flow"):
+        """Diffusive flux of a fracture (Darcy by default): flux p (+ bound_flux p_b when the fracture carries boundary
+        data)."""
+        F = fc.data[DISCRETIZATION_MATRICES][keyword or self.fk]
         flux = ad.as_device_csr(F["flux"]) @ p
         if q.bc is not None:
-            flux = flux + (ad.as_device_csr(F["bound_flux"]) @ q.bc["flow"])
+            flux = flux + (ad.as_device_csr(F["bound_flux"]) @ q.bc[bc_key])
         return flux
 
-    def _advective(self, T, flux, weight, q, key):
-        """Upwinded advective flux of a fracture (constitutive_laws.py:2555-2560) with its own boundary data, if any."""
-        csr = ad.as_device_csr
-        out = flux * (csr(T["transport"]) @ weight)
-        if q.bc is not None:
-            out = out + (csr(T["rhs_dir"]) @ (flux * q.bc[key])) + (csr(T["rhs_neu"]) @ q.bc[key])
-        return out
+    @staticmethod
+    def _fracture_bc(q, key):
+        """Boundary values ``key`` of a fracture, None for a fracture without boundary data."""
+        return None if q.bc is None else q.bc[key]
+
+    def _upwind_keywords(self):
+        """(upwind keyword, key of its boundary-condition object in ``bc``) of every advected quantity."""
+        return [(self.mobility_keyword, "fluid_flux_type")]
 
     def _aperture(self, uj_j, q):
         return fn.maximum((q.sel_n @ (q.jump @ uj_j)) + self.so.residual_aperture, self.so.residual_aperture)
@@ -187,29 +185,31 @@ class FracturedPoromechanics:
     def _parts(self, x):
         return self._group([x[self.offsets[q]:self.offsets[q + 1]] for q in range(len(self.sizes))])
 
+    def _flow_parts(self, x):
+        """(p matrix, p fractures, lambda, u_j) of ``x``: what the discretizations follow."""
+        p3, pf, _, _, lam, uj = self._parts(x)
+        return p3, pf, lam, uj
+
     def update_discretizations(self, x) -> None:
         """What follows the iterate: the fracture flux discretization (aperture) and every upwind direction."""
         x = ad.device_vector(x)
         k = self._operands()
-        p3, pf, _, _, lam, uj = self._parts(x)
+        p3, pf, lam, uj = self._flow_parts(x)
         for j, fc in enumerate(self.fractures):
             self._discretize_fracture(fc, self._aperture(uj[j], k.fr[j]).cpu().numpy())
-        mk = self.mobility_keyword
         b = k.bcq
         for j in range(len(self.fractures)):
             b = (k.fr[j].m2p @ lam[j]) + b
         q3 = ((k.F["flux"] @ p3) + (k.F["bound_flux"] @ b)).cpu().numpy()
-        prm = self.data.setdefault(PARAMETERS, {}).setdefault(mk, {})
-        prm["darcy_flux"], prm["bc"] = q3, self.bc["fluid_flux_type"]
-        Upwind(mk).discretize(self.sd, self.data)
+        for kw, key in self._upwind_keywords():
+            rediscretize_upwind(self.sd, self.data, kw, q3, self.bc[key])
         for j, fc in enumerate(self.fractures):
-            prm = fc.data.setdefault(PARAMETERS, {}).setdefault(mk, {})
-            prm["darcy_flux"] = self._fracture_flux(fc, k.fr[j], pf[j]).cpu().numpy()
-            prm["bc"] = fc.data[PARAMETERS][self.fk]["bc"] if fc.bc is None else fc.bc["fluid_flux_type"]
-            Upwind(mk).discretize(fc.sd, fc.data)
-            d = self._intf_data[j]
-            d.setdefault(PARAMETERS, {}).setdefault(mk, {})["darcy_flux"] = lam[j].cpu().numpy()
-            UpwindCoupling(mk).discretize(self.sd, fc.sd, SimpleNamespace(num_cells=fc.num_mortar), self.data, fc.data, d)
+            qf = self._fracture_flux(fc, k.fr[j], pf[j]).cpu().numpy()
+            for kw, key in self._upwind_keywords():
+                bc = fc.data[PARAMETERS][self.fk]["bc"] if fc.bc is None else fc.bc[key]
+                rediscretize_upwind(fc.sd, fc.data, kw, qf, bc)
+            rediscretize_upwind_coupling(self.sd, fc.sd, fc.num_mortar, self.data, fc.data, self._intf_data[j],
+                                         self.mobility_keyword, lam[j].cpu().numpy())
 
     def equations(self, x, x_prev, dt: float) -> list:
         k, ct, fl = self._operands(), self.ct, self.fl
@@ -237,7 +237,7 @@ class FracturedPoromechanics:
         neu = k.bcw
         for j in range(nfr):
             neu = (k.fr[j].m2p @ ifl[j]) + neu
-        ff3 = q3 * (csr(Tm["transport"]) @ w3) + (csr(Tm["rhs_dir"]) @ (q3 * k.bcw)) + (csr(Tm["rhs_neu"]) @ neu)
+        ff3 = advective_flux(Tm, q3, w3, k.bcw, neu)
         mass3 = (self._density(p3) * self._porosity(p3, u, uj, k) - self._density(p3n) * self._porosity(p3n, un, ujn, k)) \
             * (k.vol * (1.0 / dt)) + (k.div @ ff3)
         stress = (k.stress @ u) + (k.bound @ b_mech) + (k.grad_p @ (p3 - fl.reference_pressure))
@@ -250,22 +250,15 @@ class FracturedPoromechanics:
             # ---- fracture: mass balance
             Tf = fc.data[DISCRETIZATION_MATRICES][mk]
             qf = self._fracture_flux(fc, q, pf[j])
+            bw = self._fracture_bc(q, "fluid_flux")
             mass_f.append((a * self._density(pf[j]) - a_n * self._density(pfn[j])) * (q.vol * (1.0 / dt))
-                          + (q.div @ self._advective(Tf, qf, wf[j], q, "fluid_flux")) - (q.m2s @ ifl[j]))
+                          + (q.div @ advective_flux(Tf, qf, wf[j], bw, bw)) - (q.m2s @ ifl[j]))
             # ---- interface: Darcy law with the current aperture; force balance with the fluid pressure on the walls
             darcy.append(lam[j] - ((q.p2m @ trace_p) - (q.s2m @ pf[j])) * (q.s2m @ a.reciprocal()) * q.coef)
             force.append((q.p2m3 @ (stress * k.outward)) + (q.traction @ t[j]) + (q.pressure_load @ pf[j]))
-            # ---- contact laws (porepy_b200.contact)
-            jump, jump_n = q.jump @ uj[j], q.jump @ ujn[j]
-            t_n, u_n = q.sel_n @ t[j], q.sel_n @ jump
-            t_t, u_t, u_t_prev = q.sel_t @ t[j], q.sel_t @ jump, q.sel_t @ jump_n
-            gap = fn.l2_norm(2, u_t) * float(np.tan(ct.dilation_angle)) + ct.reference_gap
-            normal.append(t_n + fn.maximum(-t_n - (u_n - gap) * ct.numerical_constant, 0.0))
-            s = t_t + (u_t - u_t_prev) * ct.numerical_constant
-            b_p = fn.maximum(t_n * (-ct.friction_coefficient), 0.0)
-            chi = q.s2t @ fn.characteristic_function(ct.open_state_tolerance, b_p).val
-            tangential.append(((q.s2t @ b_p) * s - (q.s2t @ fn.maximum(b_p, fn.l2_norm(2, s))) * t_t) * (1.0 - chi)
-                              + t_t * chi)
+            nrm, tan = contact_laws(q, t[j], uj[j], ujn[j], ct)
+            normal.append(nrm)
+            tangential.append(tan)
         return [mass3] + mass_f + [momentum] + darcy + force + normal + tangential
 
     def _equation_offsets(self) -> np.ndarray:
@@ -300,18 +293,5 @@ class FracturedPoromechanics:
 
     def time_step(self, x_prev, dt: float, linear_solver, tol: float = 1e-10, max_iterations: int = 30, verbose: bool = False):
         """Semismooth Newton; ``linear_solver(J, rhs) -> dx``.  Returns (x, history)."""
-        import torch
         x_prev = ad.device_vector(x_prev)
-        x = x_prev.clone()
-        hist, r0 = [], None
-        for it in range(max_iterations + 1):
-            J, rhs = self.linearize(x, x_prev, dt)
-            rn = float(torch.linalg.vector_norm(rhs))
-            r0 = rn if r0 is None else r0
-            hist.append({"iteration": it, "residual": rn})
-            if verbose:
-                print(hist[-1], flush=True)
-            if rn <= tol * max(r0, 1e-300) or it == max_iterations:
-                break
-            x = x + linear_solver(J, rhs)
-        return x, hist
+        return newton_loop(lambda x: self.linearize(x, x_prev, dt), x_prev, linear_solver, tol, max_iterations, verbose)

@@ -21,14 +21,13 @@ are solved on the device by ``krylov.gmres_solver(prob.preconditioner_groups())`
 """
 from __future__ import annotations
 
-from types import SimpleNamespace
-
 import numpy as np
 
-from . import ad, ad_functions as fn
-from .contact import block_groups, mortar_pairs, span
+from . import ad
+from .advection import advective_flux
+from .contact import block_groups, contact_laws, mortar_pairs, span
 from .fractured_poromech import FracturedPoromechanics
-from .fv import Mpfa, Upwind, UpwindCoupling
+from .fv import Mpfa
 from .params import DISCRETIZATION_MATRICES, PARAMETERS, SecondOrderTensor
 
 
@@ -138,35 +137,15 @@ class FracturedThermoporomechanics(FracturedPoromechanics):
         p3, pf, t3, tf, u, t, lam, eta, eps, uj = out
         return p3[0], pf, t3[0], tf, u[0], t, lam, eta, eps, uj
 
-    def update_discretizations(self, x) -> None:
-        x = ad.device_vector(x)
-        k = self._operands()
+    def _flow_parts(self, x):
         p3, pf, _, _, _, _, lam, _, _, uj = self._parts(x)
-        for j, fc in enumerate(self.fractures):
-            self._discretize_fracture(fc, self._aperture(uj[j], k.fr[j]).cpu().numpy())
-        b = k.bcq
-        for j in range(len(self.fractures)):
-            b = (k.fr[j].m2p @ lam[j]) + b
-        q3 = ((k.F["flux"] @ p3) + (k.F["bound_flux"] @ b)).cpu().numpy()
-        for kw, bc in ((self.mobility_keyword, self.bc["fluid_flux_type"]),
-                       (self.enthalpy_upwind_keyword, self.bc["enthalpy_flux_type"])):
-            prm = self.data.setdefault(PARAMETERS, {}).setdefault(kw, {})
-            prm["darcy_flux"], prm["bc"] = q3, bc
-            Upwind(kw).discretize(self.sd, self.data)
-        for j, fc in enumerate(self.fractures):
-            qf = self._fracture_flux(fc, k.fr[j], pf[j]).cpu().numpy()
-            for kw, key in ((self.mobility_keyword, "fluid_flux_type"), (self.enthalpy_upwind_keyword, "enthalpy_flux_type")):
-                prm = fc.data.setdefault(PARAMETERS, {}).setdefault(kw, {})
-                prm["darcy_flux"] = qf
-                prm["bc"] = fc.data[PARAMETERS][self.fk]["bc"] if fc.bc is None else fc.bc[key]
-                Upwind(kw).discretize(fc.sd, fc.data)
-            d = self._intf_data[j]
-            d.setdefault(PARAMETERS, {}).setdefault(self.mobility_keyword, {})["darcy_flux"] = lam[j].cpu().numpy()
-            UpwindCoupling(self.mobility_keyword).discretize(self.sd, fc.sd, SimpleNamespace(num_cells=fc.num_mortar),
-                                                             self.data, fc.data, d)
+        return p3, pf, lam, uj
+
+    def _upwind_keywords(self):
+        return super()._upwind_keywords() + [(self.enthalpy_upwind_keyword, "enthalpy_flux_type")]
 
     def equations(self, x, x_prev, dt: float) -> list:
-        k, ct, fl, so = self._operands(), self.ct, self.fl, self.so
+        k, fl, so = self._operands(), self.fl, self.so
         csr = ad.as_device_csr
         nfr = len(self.fractures)
         mk, ek = self.mobility_keyword, self.enthalpy_upwind_keyword
@@ -201,8 +180,8 @@ class FracturedThermoporomechanics(FracturedPoromechanics):
         for j in range(nfr):
             neu_m = (k.fr[j].m2p @ ifl[j]) + neu_m
             neu_e = (k.fr[j].m2p @ eps[j]) + neu_e
-        ff3 = q3 * (csr(Tm["transport"]) @ w3) + (csr(Tm["rhs_dir"]) @ (q3 * k.bcw)) + (csr(Tm["rhs_neu"]) @ neu_m)
-        fe3 = q3 * (csr(Te["transport"]) @ we3) + (csr(Te["rhs_dir"]) @ (q3 * k.bce)) + (csr(Te["rhs_neu"]) @ neu_e)
+        ff3 = advective_flux(Tm, q3, w3, k.bcw, neu_m)
+        fe3 = advective_flux(Te, q3, we3, k.bce, neu_e)
         fo3 = (k.Fo["flux"] @ t3) + (k.Fo["bound_flux"] @ b_heat)
         phi, phi_n = self._porosity(p3, t3, u, uj, k), self._porosity(p3n, t3n, un, ujn, k)
         rho3, rho3n = self._density(p3, t3), self._density(p3n, t3n)
@@ -222,30 +201,21 @@ class FracturedThermoporomechanics(FracturedPoromechanics):
             a, a_n = self._aperture(uj[j], q), self._aperture(ujn[j], q)
             Tf, Tef = fc.data[DISCRETIZATION_MATRICES][mk], fc.data[DISCRETIZATION_MATRICES][ek]
             qf = self._fracture_flux(fc, q, pf[j])
-            Fof = fc.data[DISCRETIZATION_MATRICES][self.tk]
-            fof = csr(Fof["flux"]) @ tf[j]
-            if q.bc is not None:
-                fof = fof + (csr(Fof["bound_flux"]) @ q.bc["fourier"])
+            fof = self._fracture_flux(fc, q, tf[j], self.tk, "fourier")
+            bw, be = self._fracture_bc(q, "fluid_flux"), self._fracture_bc(q, "enthalpy_flux")
             rhof, rhofn = self._density(pf[j], tf[j]), self._density(pfn[j], tfn[j])
             mass_f.append((a * rhof - a_n * rhofn) * (q.vol * (1.0 / dt))
-                          + (q.div @ self._advective(Tf, qf, wf[j], q, "fluid_flux")) - (q.m2s @ ifl[j]))
+                          + (q.div @ advective_flux(Tf, qf, wf[j], bw, bw)) - (q.m2s @ ifl[j]))
             ef = rhof * (tf[j] - t0) * fl.heat_capacity - pf[j]                  # porosity 1: no solid part
             efn = rhofn * (tfn[j] - t0) * fl.heat_capacity - pfn[j]
             energy_f.append((a * ef - a_n * efn) * (q.vol * (1.0 / dt))
-                            + (q.div @ (self._advective(Tef, qf, wef[j], q, "enthalpy_flux") + fof))
+                            + (q.div @ (advective_flux(Tef, qf, wef[j], be, be) + fof))
                             - (q.m2s @ (eta[j] + eps[j])))
             inv_a = q.s2m @ a.reciprocal()
             darcy.append(lam[j] - ((q.p2m @ trace_p) - (q.s2m @ pf[j])) * inv_a * q.coef)
             fourier.append(eta[j] - ((q.p2m @ trace_t) - (q.s2m @ tf[j])) * inv_a * q.coef_t)
             force.append((q.p2m3 @ (stress * k.outward)) + (q.traction @ t[j]) + (q.pressure_load @ pf[j]))
-            jump, jump_n = q.jump @ uj[j], q.jump @ ujn[j]
-            t_n, u_n = q.sel_n @ t[j], q.sel_n @ jump
-            t_t, u_t, u_t_prev = q.sel_t @ t[j], q.sel_t @ jump, q.sel_t @ jump_n
-            gap = fn.l2_norm(2, u_t) * float(np.tan(ct.dilation_angle)) + ct.reference_gap
-            normal.append(t_n + fn.maximum(-t_n - (u_n - gap) * ct.numerical_constant, 0.0))
-            s = t_t + (u_t - u_t_prev) * ct.numerical_constant
-            b_p = fn.maximum(t_n * (-ct.friction_coefficient), 0.0)
-            chi = q.s2t @ fn.characteristic_function(ct.open_state_tolerance, b_p).val
-            tangential.append(((q.s2t @ b_p) * s - (q.s2t @ fn.maximum(b_p, fn.l2_norm(2, s))) * t_t) * (1.0 - chi)
-                              + t_t * chi)
+            nrm, tan = contact_laws(q, t[j], uj[j], ujn[j], self.ct)
+            normal.append(nrm)
+            tangential.append(tan)
         return [mass3] + mass_f + [energy3] + energy_f + [momentum] + darcy + fourier + enthalpy + force + normal + tangential

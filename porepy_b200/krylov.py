@@ -475,6 +475,26 @@ def solve_local(loc: LocalSystem, b_own, diag_own=None, tol: float = 1e-10, maxi
     return x, info
 
 
+def bicgstab_solver(tol: float = 1e-10, maxiter: int = 5000, block_size: int | None = None):
+    """A ``linear_solver(J, rhs) -> dx`` for one device: the fused BiCGStab on ``J`` (``DeviceCsr``), preconditioned by
+    Jacobi on ``J.diagonal()`` or, with ``block_size``, by the inverted ``block_size`` x ``block_size`` diagonal blocks.
+    An update that does not reach ``tol`` is returned as it is; the info of the last solve is kept in
+    ``solve.last_info``."""
+
+    def solve(J, rhs):
+        n = J.shape[0]
+        loc = LocalSystem(0, 1, np.arange(n), np.zeros(0, np.int64), J, [0], [np.zeros(0, np.int64)])
+        if block_size is None:
+            x, info = solve_local(loc, rhs, diag_own=J.diagonal(), tol=tol, maxiter=maxiter)
+        else:
+            x, info = solve_local(loc, rhs, tol=tol, maxiter=maxiter,
+                                  block_inv=(J.block_diagonal_inverse(block_size), block_size))
+        solve.last_info = info
+        return x
+    solve.last_info = None
+    return solve
+
+
 # ------------------------------------------------------------------------------------------
 # restarted GMRES with a grouped block-Jacobi preconditioner (csrc/gmres.cu): the Newton updates of the fractured contact
 # models, whose Jacobians have zero diagonals in the complementarity and force-balance rows

@@ -26,9 +26,10 @@ import numpy as np
 import scipy.sparse as sps
 
 from . import ad
-from .fv import Upwind, UpwindCoupling
+from .advection import advective_flux, rediscretize_upwind, rediscretize_upwind_coupling
 from .mdflow import MixedDimensionalFlow, schur_solve
-from .params import DISCRETIZATION_MATRICES, PARAMETERS
+from .newton import newton_loop
+from .params import DISCRETIZATION_MATRICES
 
 
 class CompressibleMixedDimensionalFlow(MixedDimensionalFlow):
@@ -94,15 +95,11 @@ class CompressibleMixedDimensionalFlow(MixedDimensionalFlow):
                     b = b + (k.m2p[j] @ parts[nsd + j])
             M = self._matrices(i)
             q = (ad.as_device_csr(M["flux"]) @ parts[i]) + (ad.as_device_csr(M["bound_flux"]) @ b)
-            prm = s.data.setdefault(PARAMETERS, {}).setdefault(mk, {})
-            prm["darcy_flux"] = q.cpu().numpy()          # nf doubles: what ``Upwind.discretize`` reads
-            prm["bc"] = self.bc_fluid_flux[i]
-            Upwind(mk).discretize(s.sd, s.data)
+            rediscretize_upwind(s.sd, s.data, mk, q.cpu().numpy(), self.bc_fluid_flux[i])
         for j, it in enumerate(self.interfaces):
-            d = self._intf_data[j]
-            d.setdefault(PARAMETERS, {}).setdefault(mk, {})["darcy_flux"] = parts[nsd + j].cpu().numpy()
             h, l = self.subdomains[it.primary], self.subdomains[it.secondary]
-            UpwindCoupling(mk).discretize(h.sd, l.sd, SimpleNamespace(num_cells=it.num_cells), h.data, l.data, d)
+            rediscretize_upwind_coupling(h.sd, l.sd, it.num_cells, h.data, l.data, self._intf_data[j], mk,
+                                         parts[nsd + j].cpu().numpy())
 
     # ---- value and Jacobian of every equation at x (previous time step: x_prev)
     def equations(self, x, x_prev=None, dt: float = 1.0) -> list:
@@ -141,7 +138,7 @@ class CompressibleMixedDimensionalFlow(MixedDimensionalFlow):
                 T = s.data[DISCRETIZATION_MATRICES][mk]
                 q = (csr(M["flux"]) @ p[i]) + (csr(M["bound_flux"]) @ b)
                 neu = k.bcw[i] if mass_in is None else mass_in + k.bcw[i]
-                ff = q * (csr(T["transport"]) @ w[i]) + (csr(T["rhs_dir"]) @ (q * k.bcw[i])) + (csr(T["rhs_neu"]) @ neu)
+                ff = advective_flux(T, q, w[i], k.bcw[i], neu)
                 eq = eq + (k.div[i] @ ff)
             for j, it in enumerate(self.interfaces):
                 if it.secondary == i:
@@ -165,42 +162,34 @@ class CompressibleMixedDimensionalFlow(MixedDimensionalFlow):
         nsd = len(self.subdomains)
         x_prev = ad.device_vector(x_prev)
 
-        def equations(x):
+        def linearize(x):
             self.update_upwind(x)
-            return self.equations(x, x_prev, dt)
-        return newton_schur(equations, x_prev, nsd, int(self.offsets[nsd]), self.num_dofs, tol, max_iterations,
-                            linear_tol, verbose)
+            return equation_system(self.equations(x, x_prev, dt))
+        solver = schur_solver(nsd, int(self.offsets[nsd]), self.num_dofs, linear_tol)
+        return newton_loop(linearize, x_prev, solver, tol, max_iterations, verbose)
 
 
-def newton_schur(equations, x0, n_primary_equations: int, n_primary_unknowns: int, n: int, tol: float = 1e-10,
-                 max_iterations: int = 15, linear_tol: float = 1e-10, verbose: bool = False):
-    """Newton's method on ``equations(x) -> [DeviceAdArray, ...]`` whose first ``n_primary_equations`` entries are the
-    subdomain balances and whose unknown vector starts with the ``n_primary_unknowns`` subdomain unknowns; the interface
-    unknowns behind them are eliminated in every step (``mdflow.schur_solve``).  Rows are split by equation group, columns
-    by two selection matrices (SpGEMM).  Returns (x, history)."""
+def equation_system(eqs):
+    """(the equations as the ``J`` of ``schur_solver``, -R): the full Jacobian is never assembled."""
     import torch
+    return eqs, -torch.cat([e.val for e in eqs])
+
+
+def schur_solver(n_primary_equations: int, n_primary_unknowns: int, n: int, tol: float = 1e-10):
+    """A ``linear_solver(eqs, rhs) -> dx`` for equation lists whose first ``n_primary_equations`` entries are the
+    subdomain balances and whose unknown vector starts with the ``n_primary_unknowns`` subdomain unknowns: the interface
+    unknowns behind them are eliminated (``mdflow.schur_solve``).  Rows are split by equation group, columns by two
+    selection matrices (SpGEMM).  The info of the last solve is kept in ``solve.last_info``."""
     D_ = ad.DeviceCsr
     npd, nq = int(n_primary_unknowns), int(n_primary_equations)
     sel_p = D_(sps.csr_matrix((np.ones(npd), (np.arange(npd), np.arange(npd))), shape=(n, npd)))
     sel_l = D_(sps.csr_matrix((np.ones(n - npd), (np.arange(npd, n), np.arange(n - npd))), shape=(n, n - npd)))
-    x = ad.device_vector(x0).clone()
-    hist, r0 = [], None
-    for it in range(max_iterations + 1):
-        eqs = equations(x)
-        rn = float(torch.sqrt(sum((e.val * e.val).sum() for e in eqs)))
-        r0 = rn if r0 is None else r0
-        rec = {"iteration": it, "residual": rn}
-        hist.append(rec)
-        if verbose:
-            print(rec, flush=True)
-        if rn <= tol * max(r0, 1e-300) or it == max_iterations:
-            break
+
+    def solve(eqs, rhs):
         Jp = eqs[0].jac if nq == 1 else D_.vstack([e.jac for e in eqs[:nq]])
         Jl = eqs[nq].jac if len(eqs) == nq + 1 else D_.vstack([e.jac for e in eqs[nq:]])
-        bp = -torch.cat([e.val for e in eqs[:nq]])
-        bl = -torch.cat([e.val for e in eqs[nq:]])
-        dx, info = schur_solve(Jp @ sel_p, Jp @ sel_l, Jl @ sel_p, Jl @ sel_l, bp, bl, tol=linear_tol)
-        rec.update(linear_iterations=int(info["iterations"]), linear_converged=bool(info["converged"]),
-                   linear_true_relres=info["true_relres"])
-        x = x + dx
-    return x, hist
+        m = Jp.shape[0]
+        dx, solve.last_info = schur_solve(Jp @ sel_p, Jp @ sel_l, Jl @ sel_p, Jl @ sel_l, rhs[:m], rhs[m:], tol=tol)
+        return dx
+    solve.last_info = None
+    return solve

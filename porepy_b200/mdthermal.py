@@ -18,7 +18,7 @@ Unknowns: [p per subdomain | T per subdomain | lambda | eta | eps per interface]
 Fourier law | enthalpy law] (the reference interleaves both per grid; ``tests/golden/mdthermal_*.npz`` carry the index
 maps).  Upwinding (``porepy_b200.Upwind`` / ``UpwindCoupling``, shared by the mass and the enthalpy flux: same Darcy flux)
 is re-discretized from the iterate in front of every linearization.  Every Newton step eliminates the three interface
-unknown sets (``mdflow_nl.newton_schur``).
+unknown sets (``mdflow_nl.schur_solver``).
 """
 from __future__ import annotations
 
@@ -28,9 +28,11 @@ import numpy as np
 import scipy.sparse as sps
 
 from . import ad
-from .fv import Mpfa, Upwind, UpwindCoupling
-from .mdflow_nl import newton_schur
-from .params import DISCRETIZATION_MATRICES, PARAMETERS
+from .advection import advective_flux, rediscretize_upwind, rediscretize_upwind_coupling
+from .fv import Mpfa
+from .mdflow_nl import equation_system, schur_solver
+from .newton import newton_loop
+from .params import DISCRETIZATION_MATRICES
 
 
 class MixedDimensionalMassEnergy:
@@ -142,15 +144,11 @@ class MixedDimensionalMassEnergy:
                 continue
             q = ((k.F[i]["flux"] @ p[i]) + (k.F[i]["bound_flux"] @ self._boundary(i, "flow", lam, k))).cpu().numpy()
             for kw, key in ((self.mobility_keyword, "fluid_flux"), (self.enthalpy_upwind_keyword, "enthalpy_flux")):
-                prm = s.data.setdefault(PARAMETERS, {}).setdefault(kw, {})
-                prm["darcy_flux"], prm["bc"] = q, self.bc_types[i][key]
-                Upwind(kw).discretize(s.sd, s.data)
+                rediscretize_upwind(s.sd, s.data, kw, q, self.bc_types[i][key])
         for j, it in enumerate(self.interfaces):
-            d = self._intf_data[j]
-            d.setdefault(PARAMETERS, {}).setdefault(self.mobility_keyword, {})["darcy_flux"] = lam[j].cpu().numpy()
             h, l = self.subdomains[it.primary], self.subdomains[it.secondary]
-            UpwindCoupling(self.mobility_keyword).discretize(h.sd, l.sd, SimpleNamespace(num_cells=it.num_cells), h.data,
-                                                             l.data, d)
+            rediscretize_upwind_coupling(h.sd, l.sd, it.num_cells, h.data, l.data, self._intf_data[j],
+                                         self.mobility_keyword, lam[j].cpu().numpy())
 
     def equations(self, x, x_prev, dt: float) -> list:
         k = self._operands()
@@ -183,10 +181,8 @@ class MixedDimensionalMassEnergy:
                 Tm = s.data[DISCRETIZATION_MATRICES][self.mobility_keyword]
                 Te = s.data[DISCRETIZATION_MATRICES][self.enthalpy_upwind_keyword]
                 q = (k.F[i]["flux"] @ p[i]) + (k.F[i]["bound_flux"] @ bq[i])
-                ff = q * (csr(Tm["transport"]) @ w[i]) + (csr(Tm["rhs_dir"]) @ (q * k.bc[i]["fluid_flux"])) \
-                    + (csr(Tm["rhs_neu"]) @ self._boundary(i, "fluid_flux", ifl, k))
-                fe = q * (csr(Te["transport"]) @ we[i]) + (csr(Te["rhs_dir"]) @ (q * k.bc[i]["enthalpy_flux"])) \
-                    + (csr(Te["rhs_neu"]) @ self._boundary(i, "enthalpy_flux", eps, k))
+                ff = advective_flux(Tm, q, w[i], k.bc[i]["fluid_flux"], self._boundary(i, "fluid_flux", ifl, k))
+                fe = advective_flux(Te, q, we[i], k.bc[i]["enthalpy_flux"], self._boundary(i, "enthalpy_flux", eps, k))
                 fo = (k.Fo[i]["flux"] @ t[i]) + (k.Fo[i]["bound_flux"] @ bt[i])
                 m_eq = m_eq + (k.div[i] @ ff)
                 e_eq = e_eq + (k.div[i] @ (fe + fo))
@@ -214,8 +210,8 @@ class MixedDimensionalMassEnergy:
         """One implicit time step by Newton's method; every step on the Schur complement of the subdomain unknowns."""
         x_prev = ad.device_vector(x_prev)
 
-        def equations(x):
+        def linearize(x):
             self.update_upwind(x)
-            return self.equations(x, x_prev, dt)
-        return newton_schur(equations, x_prev, 2 * len(self.subdomains), self.n_primary, self.num_dofs, tol,
-                            max_iterations, linear_tol, verbose)
+            return equation_system(self.equations(x, x_prev, dt))
+        solver = schur_solver(2 * len(self.subdomains), self.n_primary, self.num_dofs, linear_tol)
+        return newton_loop(linearize, x_prev, solver, tol, max_iterations, verbose)

@@ -97,35 +97,65 @@ class NonlinearTpfaFlow:
         return self.div_host @ flux - self.q_host, J.tocsr()
 
 
-def solve(problem: NonlinearTpfaFlow, p0=None, tol: float = 1e-10, max_iterations: int = 20, linear_tol: float = 1e-10,
-          verbose: bool = False):
-    """Newton's method on the device.  Returns (p as a CUDA tensor, history): one dict per iteration with the residual
-    norm, the linear iterations and the seconds spent assembling and solving."""
+def newton_loop(linearize, x0, linear_solver, tol: float = 1e-10, max_iterations: int = 20, verbose: bool = False):
+    """Newton's method shared by every model class: ``linearize(x) -> (J, rhs)`` with ``rhs`` = -R as a tensor and
+    ``J`` whatever ``linear_solver(J, rhs) -> dx`` accepts.  Stops when ||rhs|| <= ``tol`` x the first norm, or after
+    ``max_iterations`` steps (no solve after the last linearization); the tensor ``x0`` is not modified.  Returns
+    (x, history): one record per linearization with ``iteration``, ``residual``, ``jacobian_nnz`` when ``J`` has an
+    ``nnz``, and, when the linear solver keeps a non-empty ``last_info``, ``linear_iterations``, ``linear_converged``
+    (and ``linear_true_relres`` when the info has ``true_relres``)."""
     import torch
-    n = problem.g.num_cells
-    p = torch.zeros(n, dtype=torch.float64, device="cuda") if p0 is None else ad.device_vector(p0).clone()
-    hist = []
-    r0 = None
+    x = x0.clone()
+    hist, r0 = [], None
     for it in range(max_iterations + 1):
-        torch.cuda.synchronize()
-        t0 = time.perf_counter()
-        R = problem.residual(p)
-        J, rhs = ad.assemble([R])
+        J, rhs = linearize(x)
         rn = float(torch.linalg.vector_norm(rhs))
-        torch.cuda.synchronize()
-        t1 = time.perf_counter()
         r0 = rn if r0 is None else r0
-        rec = {"iteration": it, "residual": rn, "assemble_s": t1 - t0, "jacobian_nnz": int(J.nnz)}
+        rec = {"iteration": it, "residual": rn}
+        if hasattr(J, "nnz"):
+            rec["jacobian_nnz"] = int(J.nnz)
         hist.append(rec)
         if verbose:
             print(rec, flush=True)
         if rn <= tol * max(r0, 1e-300) or it == max_iterations:
             break
-        diag = J.diagonal()
-        loc = krylov.LocalSystem(0, 1, np.arange(n), np.zeros(0, np.int64), J, [0], [np.zeros(0, np.int64)])
-        dp, info = krylov.solve_local(loc, rhs, diag_own=diag, tol=linear_tol, maxiter=5000)
+        dx = linear_solver(J, rhs)
+        info = getattr(linear_solver, "last_info", None)
+        if info:
+            rec.update(linear_iterations=int(info["iterations"]), linear_converged=bool(info["converged"]))
+            if "true_relres" in info:
+                rec["linear_true_relres"] = info["true_relres"]
+        x = x + dx
+    return x, hist
+
+
+def solve(problem: NonlinearTpfaFlow, p0=None, tol: float = 1e-10, max_iterations: int = 20, linear_tol: float = 1e-10,
+          verbose: bool = False):
+    """Newton's method on the device.  Returns (p as a CUDA tensor, history): one dict per iteration with the residual
+    norm, the linear iterations and the seconds spent assembling and solving."""
+    import torch
+    p0 = torch.zeros(problem.g.num_cells, dtype=torch.float64, device="cuda") if p0 is None else ad.device_vector(p0)
+    bicgstab = krylov.bicgstab_solver(linear_tol)
+    assemble_s, solve_s = [], []
+
+    def linearize(p):
         torch.cuda.synchronize()
-        rec.update(linear_iterations=info["iterations"], linear_converged=bool(info["converged"]),
-                   solve_s=time.perf_counter() - t1)
-        p = p + dp
+        t0 = time.perf_counter()
+        J, rhs = ad.assemble([problem.residual(p)])
+        torch.cuda.synchronize()
+        assemble_s.append(time.perf_counter() - t0)
+        return J, rhs
+
+    def linear_solver(J, rhs):
+        t0 = time.perf_counter()
+        dp = bicgstab(J, rhs)
+        torch.cuda.synchronize()
+        solve_s.append(time.perf_counter() - t0)
+        linear_solver.last_info = bicgstab.last_info
+        return dp
+    p, hist = newton_loop(linearize, p0, linear_solver, tol, max_iterations, verbose)
+    for rec, a in zip(hist, assemble_s):
+        rec["assemble_s"] = a
+    for rec, s in zip(hist, solve_s):
+        rec["solve_s"] = s
     return p, hist

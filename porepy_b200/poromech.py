@@ -22,9 +22,11 @@ from __future__ import annotations
 import numpy as np
 import scipy.sparse as sps
 
-from . import ad
-from .fv import Biot, Mpfa, Upwind
-from .params import DISCRETIZATION_MATRICES, PARAMETERS
+from . import ad, krylov
+from .advection import advective_flux, rediscretize_upwind
+from .fv import Biot, Mpfa
+from .newton import newton_loop
+from .params import DISCRETIZATION_MATRICES
 
 
 class Poromechanics:
@@ -101,15 +103,11 @@ class Poromechanics:
         x = ad.device_vector(x)
         k = self._operands()
         q = (k.flux @ x[:self.nc]) + k.q_b
-        prm = self.data.setdefault(PARAMETERS, {}).setdefault(self.mobility_keyword, {})
-        prm["darcy_flux"] = q.cpu().numpy()
-        prm["bc"] = self.bc_fluid_flux
-        Upwind(self.mobility_keyword).discretize(self.sd, self.data)
+        rediscretize_upwind(self.sd, self.data, self.mobility_keyword, q.cpu().numpy(), self.bc_fluid_flux)
 
     def equations(self, x, x_prev, dt: float) -> list:
         """[mass balance, momentum balance] as ``DeviceAdArray`` at the iterate ``x``."""
         k = self._operands()
-        csr = ad.as_device_csr
         x, x_prev = ad.device_vector(x), ad.device_vector(x_prev)
         nc = self.nc
         p, u = ad.variables([x[:nc], x[nc:]])
@@ -119,7 +117,7 @@ class Poromechanics:
         mass_n = self._density(pn) * self._porosity(pn, un, k) * k.vol
         q = (k.flux @ p) + k.q_b
         w = self._density(p) * (1.0 / self.mu)
-        ff = q * (csr(T["transport"]) @ w) + (csr(T["rhs_dir"]) @ (q * k.bcw)) + (csr(T["rhs_neu"]) @ k.bcw)
+        ff = advective_flux(T, q, w, k.bcw, k.bcw)
         mass_eq = (mass - mass_n) * (1.0 / dt) + (k.div @ ff) - k.src
         stress = (k.stress @ u) + (k.grad_p @ (p - self.p_ref)) + k.stress_b
         momentum_eq = -(k.div3 @ stress) - k.f
@@ -134,27 +132,6 @@ class Poromechanics:
                   linear_solver=None, verbose: bool = False):
         """One implicit time step by Newton's method.  ``linear_solver(J, rhs) -> dx`` overrides the device Krylov solve
         (the CPU tests pass a direct solve for the scipy stand-in).  Returns (x, history)."""
-        import torch
         x_prev = ad.device_vector(x_prev)
-        x = x_prev.clone()
-        hist, r0 = [], None
-        for it in range(max_iterations + 1):
-            J, rhs = self.linearize(x, x_prev, dt)
-            rn = float(torch.linalg.vector_norm(rhs))
-            r0 = rn if r0 is None else r0
-            rec = {"iteration": it, "residual": rn, "jacobian_nnz": int(J.nnz)}
-            hist.append(rec)
-            if verbose:
-                print(rec, flush=True)
-            if rn <= tol * max(r0, 1e-300) or it == max_iterations:
-                break
-            if linear_solver is not None:
-                dx = linear_solver(J, rhs)
-            else:
-                from . import krylov
-                n = J.shape[0]
-                loc = krylov.LocalSystem(0, 1, np.arange(n), np.zeros(0, np.int64), J, [0], [np.zeros(0, np.int64)])
-                dx, info = krylov.solve_local(loc, rhs, diag_own=J.diagonal(), tol=linear_tol, maxiter=5000)
-                rec.update(linear_iterations=int(info["iterations"]), linear_converged=bool(info["converged"]))
-            x = x + dx
-        return x, hist
+        solver = krylov.bicgstab_solver(linear_tol) if linear_solver is None else linear_solver
+        return newton_loop(lambda x: self.linearize(x, x_prev, dt), x_prev, solver, tol, max_iterations, verbose)

@@ -26,8 +26,10 @@ from types import SimpleNamespace
 import numpy as np
 import scipy.sparse as sps
 
-from . import ad
-from .fv import Biot, Mpfa, Upwind
+from . import ad, krylov
+from .advection import advective_flux, rediscretize_upwind
+from .fv import Biot, Mpfa
+from .newton import newton_loop
 from .params import DISCRETIZATION_MATRICES, PARAMETERS, SecondOrderTensor
 
 
@@ -123,9 +125,7 @@ class Thermoporomechanics:
         q = ((k.flux @ p) + k.q_b).cpu().numpy()
         for kw, bc in ((self.mobility_keyword, self.bc["fluid_flux_type"]),
                        (self.enthalpy_upwind_keyword, self.bc["enthalpy_flux_type"])):
-            prm = self.data.setdefault(PARAMETERS, {}).setdefault(kw, {})
-            prm["darcy_flux"], prm["bc"] = q, bc
-            Upwind(kw).discretize(self.sd, self.data)
+            rediscretize_upwind(self.sd, self.data, kw, q, bc)
         if self.rediscretize_fourier:
             self._discretize_fourier(self._porosity(u, p, t, k).cpu().numpy())
 
@@ -146,10 +146,10 @@ class Thermoporomechanics:
         momentum = -(k.div3 @ stress)
         q = (k.flux @ p) + k.q_b
         w = rho * (1.0 / fl.viscosity)
-        ff = q * (csr(Tm["transport"]) @ w) + (csr(Tm["rhs_dir"]) @ (q * k.bcw)) + (csr(Tm["rhs_neu"]) @ k.bcw)
+        ff = advective_flux(Tm, q, w, k.bcw, k.bcw)
         mass = (rho * phi - rho_n * phi_n) * (k.vol * (1.0 / dt)) + (k.div @ ff)
         we = w * (t - fl.reference_temperature) * fl.heat_capacity
-        fe = q * (csr(Te["transport"]) @ we) + (csr(Te["rhs_dir"]) @ (q * k.bce)) + (csr(Te["rhs_neu"]) @ k.bce)
+        fe = advective_flux(Te, q, we, k.bce, k.bce)
         fo = (csr(Fo["flux"]) @ t) + (csr(Fo["bound_flux"]) @ k.bct)
         energy = (self._energy(p, t, phi) - self._energy(pn, tn, phi_n)) * (k.vol * (1.0 / dt)) + (k.div @ (fe + fo))
         return [momentum, mass, energy]
@@ -163,27 +163,6 @@ class Thermoporomechanics:
                   linear_solver=None, verbose: bool = False):
         """One implicit time step by Newton's method; ``linear_solver(J, rhs) -> dx`` overrides the device Krylov solve
         (fused Jacobi-BiCGStab, csrc/krylov.cu).  Returns (x, history)."""
-        import torch
         x_prev = ad.device_vector(x_prev)
-        x = x_prev.clone()
-        hist, r0 = [], None
-        for it in range(max_iterations + 1):
-            J, rhs = self.linearize(x, x_prev, dt)
-            rn = float(torch.linalg.vector_norm(rhs))
-            r0 = rn if r0 is None else r0
-            rec = {"iteration": it, "residual": rn, "jacobian_nnz": int(J.nnz)}
-            hist.append(rec)
-            if verbose:
-                print(rec, flush=True)
-            if rn <= tol * max(r0, 1e-300) or it == max_iterations:
-                break
-            if linear_solver is not None:
-                dx = linear_solver(J, rhs)
-            else:
-                from . import krylov
-                n = J.shape[0]
-                loc = krylov.LocalSystem(0, 1, np.arange(n), np.zeros(0, np.int64), J, [0], [np.zeros(0, np.int64)])
-                dx, info = krylov.solve_local(loc, rhs, diag_own=J.diagonal(), tol=linear_tol, maxiter=5000)
-                rec.update(linear_iterations=int(info["iterations"]), linear_converged=bool(info["converged"]))
-            x = x + dx
-        return x, hist
+        solver = krylov.bicgstab_solver(linear_tol) if linear_solver is None else linear_solver
+        return newton_loop(lambda x: self.linearize(x, x_prev, dt), x_prev, solver, tol, max_iterations, verbose)

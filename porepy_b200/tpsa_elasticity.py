@@ -90,10 +90,8 @@ class TpsaElasticity:
         """Block-Jacobi BiCGStab (one inverted cell block per cell) on the device: (x as a CUDA tensor, solver info)."""
         from . import krylov
         A, b = self.assemble()
-        n = self.num_dofs
-        bs = self.block_size
-        loc = krylov.LocalSystem(0, 1, np.arange(n), np.zeros(0, np.int64), A, [0], [np.zeros(0, np.int64)])
-        return krylov.solve_local(loc, b, tol=tol, maxiter=maxiter, block_inv=(A.block_diagonal_inverse(bs), bs))
+        solver = krylov.bicgstab_solver(tol, maxiter, self.block_size)
+        return solver(A, b), solver.last_info
 
     def to_model_order(self, A, b=None):
         """A (scipy) and b permuted to the rows / columns of the model's ``EquationSystem``."""

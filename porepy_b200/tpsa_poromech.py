@@ -25,7 +25,9 @@ from __future__ import annotations
 import numpy as np
 import scipy.sparse as sps
 
-from . import ad, fv
+from . import ad, fv, krylov
+from .advection import advective_flux, rediscretize_upwind
+from .newton import newton_loop
 from .params import DISCRETIZATION_MATRICES, PARAMETERS
 
 
@@ -150,18 +152,13 @@ class TpsaPoromechanics:
         return x[:, -2].contiguous(), x[:, -1].contiguous()
 
     def update_upwind(self, p) -> None:
-        from .fv import Upwind
         k = self._operands()
         q = (k.flux @ ad.device_vector(p)) + k.q_b
-        prm = self.data.setdefault(PARAMETERS, {}).setdefault(self.mobility_keyword, {})
-        prm["darcy_flux"] = q.cpu().numpy()
-        prm["bc"] = self.bc_fluid_flux
-        Upwind(self.mobility_keyword).discretize(self.sd, self.data)
+        rediscretize_upwind(self.sd, self.data, self.mobility_keyword, q.cpu().numpy(), self.bc_fluid_flux)
 
     def fluid_equation(self, x, x_prev, dt: float):
         """The fluid mass balance as a ``DeviceAdArray`` in the variables [p_t | p] at the iterate ``x``."""
         k = self._operands()
-        csr = ad.as_device_csr
         pt, p = ad.variables(list(self._fields(x)))
         ptn, pn = self._fields(x_prev)
         T = self.data[DISCRETIZATION_MATRICES][self.mobility_keyword]
@@ -169,7 +166,7 @@ class TpsaPoromechanics:
         mass_n = self._density(pn) * self._porosity(ptn, pn, k) * k.vol
         q = (k.flux @ p) + k.q_b
         w = self._density(p) * (1.0 / self.mu_f)
-        ff = q * (csr(T["transport"]) @ w) + (csr(T["rhs_dir"]) @ (q * k.bcw)) + (csr(T["rhs_neu"]) @ k.bcw)
+        ff = advective_flux(T, q, w, k.bcw, k.bcw)
         return (mass - mass_n) * (1.0 / dt) + (k.div @ ff) - k.src
 
     def linearize(self, x, x_prev, dt: float):
@@ -194,33 +191,16 @@ class TpsaPoromechanics:
                   linear_solver=None, verbose: bool = False):
         """One implicit time step by Newton's method.  ``linear_solver(J, rhs) -> dx`` overrides the device
         block-Jacobi BiCGStab (one inverted cell block per cell).  Returns (x, history)."""
-        import torch
         x_prev = ad.device_vector(x_prev)
-        x = x_prev.clone()
-        hist, r0 = [], None
-        for it in range(max_iterations + 1):
+
+        def linearize(x):
             J, rhs = self.linearize(x, x_prev, dt)
-            rn = float(torch.linalg.vector_norm(rhs))
             if int(self._missing.sum()):
                 raise RuntimeError("fluid Jacobian entries outside the TPSA poromechanics row pattern")
-            r0 = rn if r0 is None else r0
-            rec = {"iteration": it, "residual": rn, "jacobian_nnz": int(J.nnz)}
-            hist.append(rec)
-            if verbose:
-                print(rec, flush=True)
-            if rn <= tol * max(r0, 1e-300) or it == max_iterations:
-                break
-            if linear_solver is not None:
-                dx = linear_solver(J, rhs)
-            else:
-                from . import krylov
-                n, bs = J.shape[0], self.block_size
-                loc = krylov.LocalSystem(0, 1, np.arange(n), np.zeros(0, np.int64), J, [0], [np.zeros(0, np.int64)])
-                dx, info = krylov.solve_local(loc, rhs, tol=linear_tol, maxiter=5000,
-                                              block_inv=(J.block_diagonal_inverse(bs), bs))
-                rec.update(linear_iterations=int(info["iterations"]), linear_converged=bool(info["converged"]))
-            x = x + dx
-        return x, hist
+            return J, rhs
+        if linear_solver is None:
+            linear_solver = krylov.bicgstab_solver(linear_tol, block_size=self.block_size)
+        return newton_loop(linearize, x_prev, linear_solver, tol, max_iterations, verbose)
 
     def to_model_order(self, A, b=None):
         """A (scipy) and b permuted to the rows / columns of the model's ``EquationSystem``."""

@@ -82,3 +82,68 @@ def test_device_newton_loop_matches_scipy_newton():
     assert h[-1]["residual"] <= 1e-11 * h[0]["residual"] and len(h) <= len(hist) + 2
     assert all(r.get("linear_converged", True) for r in h)
     assert np.linalg.norm(p.cpu().numpy() - sol) <= 1e-8 * np.linalg.norm(sol)
+
+
+class _Dense:
+    """A dense Jacobian with an ``nnz``, as ``DeviceCsr`` has."""
+
+    def __init__(self, a):
+        self.a, self.nnz = a, int((a != 0).sum())
+
+
+def _cubic(with_nnz=True):
+    """R(x) = x^3 + x - b on CPU tensors: (linearize, linear solver, b, the list of solved right-hand sides)."""
+    import torch
+    b = torch.tensor([1.0, 2.0, -3.0], dtype=torch.float64)
+    solved = []
+
+    def linearize(x):
+        J = torch.diag(3 * x * x + 1)
+        return (_Dense(J) if with_nnz else J), -(x ** 3 + x - b)
+
+    def solver(J, rhs):
+        solved.append(rhs.clone())
+        return torch.linalg.solve(J.a if with_nnz else J, rhs)
+    return linearize, solver, b, solved
+
+
+def test_newton_loop_stops_at_the_relative_tolerance_and_keeps_x0():
+    import torch
+    linearize, solver, b, solved = _cubic()
+    x0 = torch.zeros(3, dtype=torch.float64)
+    x, hist = newton.newton_loop(linearize, x0, solver, tol=1e-12, max_iterations=30)
+    assert torch.equal(x0, torch.zeros(3, dtype=torch.float64))
+    assert hist[-1]["residual"] <= 1e-12 * hist[0]["residual"] < hist[-2]["residual"]
+    assert [h["iteration"] for h in hist] == list(range(len(hist))) and len(solved) == len(hist) - 1
+    assert float(torch.linalg.vector_norm(x ** 3 + x - b)) <= 1e-12 * float(torch.linalg.vector_norm(b))
+    assert all(h["jacobian_nnz"] == 3 for h in hist) and "linear_iterations" not in hist[0]
+
+
+def test_newton_loop_zero_initial_residual_and_iteration_limit():
+    import torch
+    linearize, solver, _, solved = _cubic()
+    x, hist = newton.newton_loop(linearize, torch.zeros(3, dtype=torch.float64), solver, tol=0.0, max_iterations=2)
+    assert len(hist) == 3 and len(solved) == 2                         # max_iterations + 1 records, no last solve
+    # r0 = 0: the stopping test is against 1e-300, met at once, nothing solved
+    linearize, solver, _, solved = _cubic()
+    x0 = torch.ones(3, dtype=torch.float64)
+    x, hist = newton.newton_loop(lambda x: (linearize(x)[0], torch.zeros(3, dtype=torch.float64)), x0, solver, 1e-10, 4)
+    assert [h["residual"] for h in hist] == [0.0] and not solved and torch.equal(x, x0) and x is not x0
+
+
+def test_newton_loop_records_linear_solver_info_and_nnz_only_when_present():
+    import torch
+    linearize, solver, _, _ = _cubic(with_nnz=False)
+    infos = iter([{"iterations": 7, "converged": True}, {"iterations": 5, "converged": False, "true_relres": 1e-3}])
+
+    def with_info(J, rhs):
+        with_info.last_info = next(infos)
+        return solver(J, rhs)
+    with_info.last_info = None
+    _, hist = newton.newton_loop(linearize, torch.zeros(3, dtype=torch.float64), with_info, tol=0.0, max_iterations=2)
+    assert all("jacobian_nnz" not in h for h in hist)
+    assert hist[0]["linear_iterations"] == 7 and hist[0]["linear_converged"] is True
+    assert "linear_true_relres" not in hist[0]
+    assert hist[1]["linear_iterations"] == 5 and hist[1]["linear_converged"] is False
+    assert hist[1]["linear_true_relres"] == 1e-3
+    assert "linear_iterations" not in hist[2]                          # the last record: no solve

@@ -15,7 +15,7 @@
 #include <string>
 #include <vector>
 
-#include "plan.hpp"
+#include "csr_build.cuh"
 #include <nvtx3/nvToolsExt.h>
 
 // NVTX range for the lifetime of a scope: one range per C-ABI phase (SURVEY.md 5: the reference logs per-phase times,
@@ -212,65 +212,11 @@ __global__ void pattern_kernel(int64_t nrows, const int32_t *__restrict__ rn_ptr
         while (P < total) P <<= 1;
         for (int i = total + lane; i < P; i += 32) buf[i] = 0x7fffffff;
         __syncwarp();
-        for (int k = 2; k <= P; k <<= 1)
-            for (int j = k >> 1; j > 0; j >>= 1) {
-                for (int i = lane; i < P; i += 32) {
-                    const int l = i ^ j;
-                    if (l > i) {
-                        const int32_t a = buf[i], c = buf[l];
-                        const bool asc = (i & k) == 0;
-                        if ((a > c) == asc) { buf[i] = c; buf[l] = a; }
-                    }
-                }
-                __syncwarp();
-            }
-        int off = 0;
-        for (int i0 = 0; i0 < total; i0 += 32) {
-            const int i = i0 + lane;
-            const bool flag = i < total && (i == 0 || buf[i] != buf[i - 1]);
-            const unsigned m = __ballot_sync(0xffffffffu, flag);
-            if (pass == 1 && flag) indices[indptr[r] + off + __popc(m & ((1u << lane) - 1u))] = buf[i];
-            off += __popc(m);
-        }
+        warp_bitonic_sort(P, [&](int i, int l, bool asc) { warp_cas(buf, i, l, asc); });
+        const int off = warp_unique(buf, total, pass == 1 ? indices + indptr[r] : (int32_t *)nullptr);
         if (pass == 0 && lane == 0) counts[r] = off;
         __syncwarp();
     }
-}
-
-// exclusive scan of nrows+1 int32 counts (single block, serial over chunks: nrows <= ~10^7, a few ms)
-__global__ void scan_kernel(int64_t n, const int32_t *__restrict__ counts, int32_t *__restrict__ indptr,
-                            long long *total_out) {
-    __shared__ long long wsum[32];
-    __shared__ long long carry;
-    if (threadIdx.x == 0) carry = 0;
-    __syncthreads();
-    const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
-    for (int64_t base = 0; base < n; base += blockDim.x) {
-        const int64_t i = base + threadIdx.x;
-        long long v = i < n ? counts[i] : 0;
-        long long x = v;
-        for (int o = 1; o < 32; o <<= 1) {
-            long long y = __shfl_up_sync(0xffffffffu, x, o);
-            if (lane >= o) x += y;
-        }
-        if (lane == 31) wsum[w] = x;
-        __syncthreads();
-        if (w == 0) {
-            long long t = lane < (blockDim.x >> 5) ? wsum[lane] : 0;
-            for (int o = 1; o < 32; o <<= 1) {
-                long long y = __shfl_up_sync(0xffffffffu, t, o);
-                if (lane >= o) t += y;
-            }
-            wsum[lane] = t;
-        }
-        __syncthreads();
-        const long long excl = carry + (w ? wsum[w - 1] : 0) + x - v;
-        if (i < n) indptr[i] = (int32_t)excl;
-        __syncthreads();
-        if (threadIdx.x == blockDim.x - 1) carry += wsum[(blockDim.x >> 5) - 1];
-        __syncthreads();
-    }
-    if (threadIdx.x == 0) { indptr[n] = (int32_t)carry; *total_out = carry; }
 }
 
 // Position maps: one warp per node, lanes over the node's (local row, local column) pairs;
@@ -310,7 +256,6 @@ extern "C" int pb_plan_create(int nd, int64_t nc, int64_t nf, int64_t nn, const 
     if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev < 1)
         return fail(PB_ECUDA, "no CUDA device: libporeb200 has no CPU path");
     pb_plan *p = new pb_plan;
-    std::string err;
     {
         // torchrun exports OMP_NUM_THREADS=1; the plan builder is the one OpenMP user here, so give
         // it this rank's share of the cores (POREB200_PLAN_THREADS overrides) -- through a num_threads clause on
@@ -339,8 +284,8 @@ extern "C" int pb_plan_create(int nd, int64_t nc, int64_t nf, int64_t nn, const 
     // for interaction regions beyond the shared-memory sort capacity, and can be forced with POREB200_HOST_PLAN=1
     int rc = getenv("POREB200_HOST_PLAN") ? -1
              : pb_build_device_topology_(p, nd, nc, nf, nn, cf_indptr, cf_indices, cf_data, fn_indptr, fn_indices,
-                                         fn_idx_dev, err);
-    if (rc > 0) { delete p; return fail(rc, err); }
+                                         fn_idx_dev);
+    if (rc > 0) { delete p; return rc; }
     const bool device_topology = rc == 0;
     if (getenv("POREB200_PLAN_TIMING")) {
         cudaStreamSynchronize(st);
@@ -349,6 +294,7 @@ extern "C" int pb_plan_create(int nd, int64_t nc, int64_t nf, int64_t nn, const 
     }
     if (!device_topology) {
         p->H = HostPlan{};
+        std::string err;
         rc = build_host_plan(nd, nc, nf, nn, cf_indptr, cf_indices, cf_data, fn_indptr, fn_indices,
                              p->H, err, /*build_pos_maps=*/false, /*build_patterns=*/false);
         if (rc) {
@@ -371,38 +317,35 @@ extern "C" int pb_plan_create(int nd, int64_t nc, int64_t nf, int64_t nn, const 
     }
     {
         // ---- structural patterns on the device (host fallback when a row has > 256 candidates)
-        struct PJob { int which; int64_t nrows, ncols; DevBuf *rnp, *rn, *cp, *ci, *ip; };
-        PJob pj[4] = {{0, nf, nc, &p->fn_indptr, &fn_idx_dev, &p->node_sc_ptr, &p->sc_cell, &p->fc_indptr},
-                      {1, nf, nf, &p->fn_indptr, &fn_idx_dev, &p->nbf_ptr, &p->nbf_idx, &p->fb_indptr},
-                      {2, nc, nc, &p->cn_ptr, &p->cn_idx, &p->node_sc_ptr, &p->sc_cell, &p->cc_indptr},
-                      {3, nc, nf, &p->cn_ptr, &p->cn_idx, &p->nbf_ptr, &p->nbf_idx, &p->cb_indptr}};
-        DevBuf counts, flag, total;
+        struct PJob { int which; int64_t nrows, ncols; DevBuf *rnp, *rn, *cp, *ci; };
+        PJob pj[4] = {{0, nf, nc, &p->fn_indptr, &fn_idx_dev, &p->node_sc_ptr, &p->sc_cell},
+                      {1, nf, nf, &p->fn_indptr, &fn_idx_dev, &p->nbf_ptr, &p->nbf_idx},
+                      {2, nc, nc, &p->cn_ptr, &p->cn_idx, &p->node_sc_ptr, &p->sc_cell},
+                      {3, nc, nf, &p->cn_ptr, &p->cn_idx, &p->nbf_ptr, &p->nbf_idx}};
+        DevBuf counts, flag;
         if ((e = flag.ensure(sizeof(int))) != cudaSuccess) return bail("flag", e);
-        if ((e = total.ensure(sizeof(long long))) != cudaSuccess) return bail("total", e);
         if ((e = cudaMemsetAsync(flag.p, 0, sizeof(int), st)) != cudaSuccess) return bail("memset", e);
         bool host_fallback = false;
         for (auto &j : pj) {
-            if ((e = counts.ensure((size_t)(j.nrows + 1) * sizeof(int32_t))) != cudaSuccess) return bail("counts", e);
-            if ((e = j.ip->ensure((size_t)(j.nrows + 1) * sizeof(int32_t))) != cudaSuccess) return bail("indptr", e);
+            DevBuf &ip = p->pat_ip[j.which];
+            if ((e = counts.ensure((size_t)j.nrows * sizeof(int32_t))) != cudaSuccess) return bail("counts", e);
+            if ((e = ip.ensure((size_t)(j.nrows + 1) * sizeof(int32_t))) != cudaSuccess) return bail("indptr", e);
             const int block = 256;
             int grid = (int)std::max<int64_t>(1, std::min<int64_t>((j.nrows + 7) / 8, (int64_t)pb_sm_count() * 8));
             pattern_kernel<256><<<grid, block, 0, st>>>(j.nrows, j.rnp->as<int32_t>(), j.rn->as<int32_t>(),
                                                         j.cp->as<int32_t>(), j.ci->as<int32_t>(),
                                                         counts.as<int32_t>(), nullptr, nullptr, 0, flag.as<int>());
-            scan_kernel<<<1, 1024, 0, st>>>(j.nrows, counts.as<int32_t>(), j.ip->as<int32_t>(),
-                                            total.as<long long>());
-            long long tot = 0;
+            g_launches++;
             int ov = 0;
-            if ((e = cudaMemcpyAsync(&tot, total.p, sizeof(tot), cudaMemcpyDeviceToHost, st)) != cudaSuccess) return bail("copy", e);
             if ((e = cudaMemcpyAsync(&ov, flag.p, sizeof(ov), cudaMemcpyDeviceToHost, st)) != cudaSuccess) return bail("copy", e);
-            if ((e = cudaStreamSynchronize(st)) != cudaSuccess) return bail("pattern pass 0", e);
-            g_launches += 2;
+            int64_t tot = 0;
+            if ((rc = pb_scan_offsets_(counts.as<int32_t>(), ip.as<int32_t>(), j.nrows, st, &tot))) { delete p; return rc; }
             if (ov) { host_fallback = true; break; }
             if (tot > 0x7FFFFFFFll) { delete p; return fail(PB_EINVAL, "pattern exceeds 2^31 entries; split the grid"); }
-            if ((e = p->pat_idx[j.which].ensure((size_t)std::max<long long>(1, tot) * sizeof(int32_t))) != cudaSuccess) return bail("indices", e);
+            if ((e = p->pat_idx[j.which].ensure((size_t)std::max<int64_t>(1, tot) * sizeof(int32_t))) != cudaSuccess) return bail("indices", e);
             pattern_kernel<256><<<grid, block, 0, st>>>(j.nrows, j.rnp->as<int32_t>(), j.rn->as<int32_t>(),
                                                         j.cp->as<int32_t>(), j.ci->as<int32_t>(), nullptr,
-                                                        j.ip->as<int32_t>(), p->pat_idx[j.which].as<int32_t>(), 1,
+                                                        ip.as<int32_t>(), p->pat_idx[j.which].as<int32_t>(), 1,
                                                         flag.as<int>());
             g_launches++;
             p->pat_rows[j.which] = j.nrows; p->pat_cols[j.which] = j.ncols; p->pat_nnz[j.which] = tot;
@@ -415,8 +358,7 @@ extern "C" int pb_plan_create(int nd, int64_t nc, int64_t nf, int64_t nn, const 
                                       H2, err2, false, true);
             if (rc2) { delete p; return fail(rc2, err2); }
             for (int w = 0; w < 4; ++w) {
-                DevBuf *ip = w == 0 ? &p->fc_indptr : w == 1 ? &p->fb_indptr : w == 2 ? &p->cc_indptr : &p->cb_indptr;
-                if ((e = ip->upload(H2.pat[w].indptr, st)) != cudaSuccess) return bail("indptr", e);
+                if ((e = p->pat_ip[w].upload(H2.pat[w].indptr, st)) != cudaSuccess) return bail("indptr", e);
                 if ((e = p->pat_idx[w].upload(H2.pat[w].indices, st)) != cudaSuccess) return bail("indices", e);
                 p->pat_rows[w] = H2.pat[w].nrows; p->pat_cols[w] = H2.pat[w].ncols; p->pat_nnz[w] = H2.pat[w].nnz();
             }
@@ -430,12 +372,12 @@ extern "C" int pb_plan_create(int nd, int64_t nc, int64_t nf, int64_t nn, const 
     }
     {
         struct Job { DevBuf *pos; const std::vector<int64_t> *ptr; DevBuf *pptr; int pat;
-                     DevBuf *rp, *re, *cp, *ce; DevBuf *ip; };
+                     DevBuf *rp, *re, *cp, *ce; };
         Job jobs[4] = {
-            {&p->pos_fc, &H.posfc_ptr, &p->posfc_ptr, 0, &p->node_sf_ptr, &p->sf_face, &p->node_sc_ptr, &p->sc_cell, &p->fc_indptr},
-            {&p->pos_fb, &H.posfb_ptr, &p->posfb_ptr, 1, &p->node_sf_ptr, &p->sf_face, &p->nbf_ptr, &p->nbf_idx, &p->fb_indptr},
-            {&p->pos_cc, &H.poscc_ptr, &p->poscc_ptr, 2, &p->node_sc_ptr, &p->sc_cell, &p->node_sc_ptr, &p->sc_cell, &p->cc_indptr},
-            {&p->pos_cb, &H.poscb_ptr, &p->poscb_ptr, 3, &p->node_sc_ptr, &p->sc_cell, &p->nbf_ptr, &p->nbf_idx, &p->cb_indptr},
+            {&p->pos_fc, &H.posfc_ptr, &p->posfc_ptr, 0, &p->node_sf_ptr, &p->sf_face, &p->node_sc_ptr, &p->sc_cell},
+            {&p->pos_fb, &H.posfb_ptr, &p->posfb_ptr, 1, &p->node_sf_ptr, &p->sf_face, &p->nbf_ptr, &p->nbf_idx},
+            {&p->pos_cc, &H.poscc_ptr, &p->poscc_ptr, 2, &p->node_sc_ptr, &p->sc_cell, &p->node_sc_ptr, &p->sc_cell},
+            {&p->pos_cb, &H.poscb_ptr, &p->poscb_ptr, 3, &p->node_sc_ptr, &p->sc_cell, &p->nbf_ptr, &p->nbf_idx},
         };
         for (auto &j : jobs) {
             if ((e = j.pos->ensure((size_t)std::max<int64_t>(1, j.ptr->back()) * sizeof(int32_t))) != cudaSuccess)
@@ -445,7 +387,7 @@ extern "C" int pb_plan_create(int nd, int64_t nc, int64_t nf, int64_t nn, const 
             int grid = (int)std::max<int64_t>(1, std::min<int64_t>(need, (int64_t)pb_sm_count() * 16));
             posmap_kernel<<<grid, block, 0, st>>>(nn, j.rp->as<int32_t>(), j.re->as<int32_t>(),
                                                   j.cp->as<int32_t>(), j.ce->as<int32_t>(),
-                                                  j.ip->as<int32_t>(), p->pat_idx[j.pat].as<int32_t>(),
+                                                  p->pat_ip[j.pat].as<int32_t>(), p->pat_idx[j.pat].as<int32_t>(),
                                                   j.pptr->as<int64_t>(), j.pos->as<int32_t>());
             g_launches++;
             if ((e = cudaGetLastError()) != cudaSuccess) return bail("posmap_kernel", e);
@@ -464,8 +406,8 @@ extern "C" int pb_plan_create(int nd, int64_t nc, int64_t nf, int64_t nn, const 
     v.poscc_ptr = p->poscc_ptr.as<int64_t>(); v.poscb_ptr = p->poscb_ptr.as<int64_t>();
     v.pos_fc = p->pos_fc.as<int32_t>(); v.pos_fb = p->pos_fb.as<int32_t>();
     v.pos_cc = p->pos_cc.as<int32_t>(); v.pos_cb = p->pos_cb.as<int32_t>();
-    v.fc_indptr = p->fc_indptr.as<int32_t>(); v.fb_indptr = p->fb_indptr.as<int32_t>();
-    v.cc_indptr = p->cc_indptr.as<int32_t>(); v.cb_indptr = p->cb_indptr.as<int32_t>();
+    v.fc_indptr = p->pat_ip[0].as<int32_t>(); v.fb_indptr = p->pat_ip[1].as<int32_t>();
+    v.cc_indptr = p->pat_ip[2].as<int32_t>(); v.cb_indptr = p->pat_ip[3].as<int32_t>();
     rc = build_mpfa_classes(p);
     if (rc) { delete p; return rc; }
     if ((e = cudaStreamSynchronize(st)) != cudaSuccess) return bail("sync", e);
@@ -530,8 +472,7 @@ extern "C" int pb_plan_pattern_size(const pb_plan *p, int which, int64_t *nrows,
 
 extern "C" int pb_plan_pattern_get(const pb_plan *p, int which, int32_t *indptr, int32_t *indices) {
     if (!p || which < 0 || which > 3) return fail(PB_EINVAL, "bad pattern id");
-    const DevBuf *ip = which == 0 ? &p->fc_indptr : which == 1 ? &p->fb_indptr : which == 2 ? &p->cc_indptr : &p->cb_indptr;
-    CUDA_TRY(cudaMemcpyAsync(indptr, ip->p, (p->pat_rows[which] + 1) * sizeof(int32_t), cudaMemcpyDeviceToHost, p->stream));
+    CUDA_TRY(cudaMemcpyAsync(indptr, p->pat_ip[which].p, (p->pat_rows[which] + 1) * sizeof(int32_t), cudaMemcpyDeviceToHost, p->stream));
     if (p->pat_nnz[which])
         CUDA_TRY(cudaMemcpyAsync(indices, p->pat_idx[which].p, p->pat_nnz[which] * sizeof(int32_t),
                                  cudaMemcpyDeviceToHost, p->stream));
@@ -561,6 +502,18 @@ __global__ void expand_pattern_kernel(int64_t nrows, const int32_t *__restrict__
     if (warp == 0 && lane == 0) nip[nrows * br] = (int32_t)((int64_t)br * bc * ip[nrows]);
 }
 
+// pattern `which` expanded into br x bc blocks (layout as documented at pb_plan_pattern_expanded), on the plan's stream
+static int expand_pattern(pb_plan *p, int which, int br, int bc, int32_t *nip, int32_t *nix) {
+    const int64_t nrows = p->pat_rows[which];
+    const int block = 256;
+    int grid = (int)std::max<int64_t>(1, std::min<int64_t>((nrows * 32 + block - 1) / block, (int64_t)pb_sm_count() * 16));
+    expand_pattern_kernel<<<grid, block, 0, p->stream>>>(nrows, p->pat_ip[which].as<int32_t>(),
+                                                         p->pat_idx[which].as<int32_t>(), br, bc, nip, nix);
+    g_launches++;
+    CUDA_TRY(cudaGetLastError());
+    return PB_OK;
+}
+
 extern "C" int pb_plan_pattern_expanded(pb_plan *p, int which, int br, int bc, int32_t *indptr,
                                         int32_t *indices) {
     if (!p || which < 0 || which > 3 || br < 1 || bc < 1 || !indptr || !indices)
@@ -569,19 +522,12 @@ extern "C" int pb_plan_pattern_expanded(pb_plan *p, int which, int br, int bc, i
     const int64_t nnz = p->pat_nnz[which] * br * bc;
     if (nnz >= 0x7FFFFFFFll || c.ncols * bc >= 0x7FFFFFFFll)
         return fail(PB_ENOTIMPL, "expanded pattern does not fit int32 indices");
-    DevBuf *bip = which == 0 ? &p->fc_indptr : which == 1 ? &p->fb_indptr : which == 2 ? &p->cc_indptr : &p->cb_indptr;
     DevBuf nip, nix;
-    DevBuf &dix = p->pat_idx[which];
     cudaStream_t st = p->stream;
     CUDA_TRY(nip.ensure((c.nrows * br + 1) * sizeof(int32_t)));
     CUDA_TRY(nix.ensure((nnz ? nnz : 1) * sizeof(int32_t)));
-    const int block = 256;
-    int64_t need = (c.nrows * 32 + block - 1) / block;
-    int grid = (int)std::max<int64_t>(1, std::min<int64_t>(need, (int64_t)pb_sm_count() * 16));
-    expand_pattern_kernel<<<grid, block, 0, st>>>(c.nrows, bip->as<int32_t>(), dix.as<int32_t>(), br, bc,
-                                                  nip.as<int32_t>(), nix.as<int32_t>());
-    g_launches++;
-    CUDA_TRY(cudaGetLastError());
+    int rc = expand_pattern(p, which, br, bc, nip.as<int32_t>(), nix.as<int32_t>());
+    if (rc) return rc;
     CUDA_TRY(cudaMemcpyAsync(indptr, nip.p, (c.nrows * br + 1) * sizeof(int32_t), cudaMemcpyDeviceToHost, st));
     if (nnz) CUDA_TRY(cudaMemcpyAsync(indices, nix.p, nnz * sizeof(int32_t), cudaMemcpyDeviceToHost, st));
     CUDA_TRY(cudaStreamSynchronize(st));
@@ -975,13 +921,8 @@ extern "C" int pb_plan_output_csr(pb_plan *p, const pb_values *v, int which, int
     pb_csr *a = nullptr;
     int rc = pb_csr_alloc_(nrows * br, p->pat_cols[which] * bc, nnz, &a);
     if (rc) return rc;
-    DevBuf *bip = which == 0 ? &p->fc_indptr : which == 1 ? &p->fb_indptr : which == 2 ? &p->cc_indptr : &p->cb_indptr;
-    const int block = 256;
-    int grid = (int)std::max<int64_t>(1, std::min<int64_t>((nrows * 32 + block - 1) / block, (int64_t)pb_sm_count() * 16));
-    expand_pattern_kernel<<<grid, block, 0, p->stream>>>(nrows, bip->as<int32_t>(), p->pat_idx[which].as<int32_t>(), br, bc,
-                                                         pb_csr_indptr_(a), pb_csr_indices_(a));
-    g_launches++;
-    CUDA_TRY(cudaGetLastError());
+    rc = expand_pattern(p, which, br, bc, pb_csr_indptr_(a), pb_csr_indices_(a));
+    if (rc) return rc;
     if (nnz) CUDA_TRY(cudaMemcpyAsync(pb_csr_data_(a), v->buf.p, (size_t)nnz * sizeof(double), cudaMemcpyDeviceToDevice, p->stream));
     CUDA_TRY(cudaStreamSynchronize(p->stream));
     *out = a;
@@ -999,14 +940,14 @@ extern "C" int pb_mpfa_system(pb_plan *p, const pb_values *flux, pb_csr **out) {
     if (rc) return rc;
     CUDA_TRY(cudaStreamSynchronize(p->stream));
     pb_csr *a = nullptr;
-    rc = pb_csr_from_device_pattern_(H.nc, H.nc, p->pat_nnz[2], p->cc_indptr.as<int32_t>(),
+    rc = pb_csr_from_device_pattern_(H.nc, H.nc, p->pat_nnz[2], p->pat_ip[2].as<int32_t>(),
                                      p->pat_idx[2].as<int32_t>(), &a);
     if (rc) return rc;
     const int block = 256;
     int grid = (int)std::max<int64_t>(1, std::min<int64_t>((H.nf * 32 + block - 1) / block, (int64_t)pb_sm_count() * 16));
-    div_flux_kernel<<<grid, block, 0, p->stream>>>(H.nf, p->fc_indptr.as<int32_t>(), p->pat_idx[0].as<int32_t>(),
+    div_flux_kernel<<<grid, block, 0, p->stream>>>(H.nf, p->pat_ip[0].as<int32_t>(), p->pat_idx[0].as<int32_t>(),
                                                    flux_dev, p->face_cells.as<int32_t>(),
-                                                   p->cc_indptr.as<int32_t>(), p->pat_idx[2].as<int32_t>(),
+                                                   p->pat_ip[2].as<int32_t>(), p->pat_idx[2].as<int32_t>(),
                                                    pb_csr_data_(a));
     g_launches++;
     CUDA_TRY(cudaGetLastError());
@@ -1038,12 +979,12 @@ extern "C" int pb_mpfa_rhs(pb_plan *p, const pb_values *bound_flux, const pb_val
     CUDA_TRY(cudaMemsetAsync(r.p, 0, (size_t)H.nc * sizeof(double), st));
     const int block = 256;
     int grid = (int)std::max<int64_t>(1, std::min<int64_t>((H.nf * 32 + block - 1) / block, (int64_t)pb_sm_count() * 16));
-    face_row_dot_kernel<<<grid, block, 0, st>>>(H.nf, p->fb_indptr.as<int32_t>(), p->pat_idx[1].as<int32_t>(),
+    face_row_dot_kernel<<<grid, block, 0, st>>>(H.nf, p->pat_ip[1].as<int32_t>(), p->pat_idx[1].as<int32_t>(),
                                                 bflux_dev, 1, bc.as<double>(), w.as<double>());
     g_launches++;
     if (vector_source) {
         CUDA_TRY(vs.upload(vector_source, (size_t)H.nc * H.nd, st));
-        face_row_dot_kernel<<<grid, block, 0, st>>>(H.nf, p->fc_indptr.as<int32_t>(), p->pat_idx[0].as<int32_t>(),
+        face_row_dot_kernel<<<grid, block, 0, st>>>(H.nf, p->pat_ip[0].as<int32_t>(), p->pat_idx[0].as<int32_t>(),
                                                     vs_dev, H.nd, vs.as<double>(), w.as<double>());
         g_launches++;
     }
@@ -1155,21 +1096,17 @@ extern "C" int pb_mpsa_system(pb_plan *p, const pb_values *stress, pb_csr **out)
     DevBuf nip, nix;
     CUDA_TRY(nip.ensure((size_t)(H.nc * nd + 1) * sizeof(int32_t)));
     CUDA_TRY(nix.ensure((size_t)std::max<int64_t>(1, p->pat_nnz[2] * nd2) * sizeof(int32_t)));
-    const int block = 256;
-    int grid = (int)std::max<int64_t>(1, std::min<int64_t>((H.nc * 32 + block - 1) / block, (int64_t)pb_sm_count() * 16));
-    expand_pattern_kernel<<<grid, block, 0, st>>>(H.nc, p->cc_indptr.as<int32_t>(), p->pat_idx[2].as<int32_t>(), nd, nd,
-                                                  nip.as<int32_t>(), nix.as<int32_t>());
-    g_launches++;
-    CUDA_TRY(cudaGetLastError());
+    int rc = expand_pattern(p, 2, nd, nd, nip.as<int32_t>(), nix.as<int32_t>());
+    if (rc) return rc;
     CUDA_TRY(cudaStreamSynchronize(st));
     pb_csr *a = nullptr;
-    int rc = pb_csr_from_device_pattern_(H.nc * nd, H.nc * nd, p->pat_nnz[2] * nd2, nip.as<int32_t>(), nix.as<int32_t>(), &a);
+    rc = pb_csr_from_device_pattern_(H.nc * nd, H.nc * nd, p->pat_nnz[2] * nd2, nip.as<int32_t>(), nix.as<int32_t>(), &a);
     if (rc) return rc;
     constexpr int kWarps = 4, kCap = 128;           // 4 x 128 x 9 doubles = 36 KB of shared memory per block
     int gridg = (int)std::max<int64_t>(1, std::min<int64_t>((H.nc + kWarps - 1) / kWarps, (int64_t)pb_sm_count() * 24));
     div_stress_gather_kernel<kWarps><<<gridg, kWarps * 32, (size_t)kWarps * kCap * nd2 * sizeof(double), st>>>(
-        H.nc, nd, p->cf_ip.as<int32_t>(), p->cf_ix.as<int32_t>(), p->cf_sg.as<int8_t>(), p->fc_indptr.as<int32_t>(),
-        p->pat_idx[0].as<int32_t>(), stress_dev, p->cc_indptr.as<int32_t>(), p->pat_idx[2].as<int32_t>(),
+        H.nc, nd, p->cf_ip.as<int32_t>(), p->cf_ix.as<int32_t>(), p->cf_sg.as<int8_t>(), p->pat_ip[0].as<int32_t>(),
+        p->pat_idx[0].as<int32_t>(), stress_dev, p->pat_ip[2].as<int32_t>(), p->pat_idx[2].as<int32_t>(),
         pb_csr_data_(a), kCap);
     g_launches++;
     CUDA_TRY(cudaGetLastError());
@@ -1199,7 +1136,7 @@ extern "C" int pb_mpsa_rhs(pb_plan *p, const pb_values *bound_stress, const doub
     else CUDA_TRY(cudaMemsetAsync(r.p, 0, (size_t)H.nc * nd * sizeof(double), st));
     const int block = 256;
     int grid = (int)std::max<int64_t>(1, std::min<int64_t>((H.nf * nd * 32 + block - 1) / block, (int64_t)pb_sm_count() * 16));
-    bound_stress_dot_kernel<<<grid, block, 0, st>>>(H.nf, nd, p->fb_indptr.as<int32_t>(), p->pat_idx[1].as<int32_t>(),
+    bound_stress_dot_kernel<<<grid, block, 0, st>>>(H.nf, nd, p->pat_ip[1].as<int32_t>(), p->pat_idx[1].as<int32_t>(),
                                                     bstress_dev, bc.as<double>(), w.as<double>());
     int grid2 = (int)std::max<int64_t>(1, std::min<int64_t>((H.nf * nd + block - 1) / block, (int64_t)pb_sm_count() * 16));
     neg_div_nd_kernel<<<grid2, block, 0, st>>>(H.nf, nd, p->face_cells.as<int32_t>(), w.as<double>(), r.as<double>());

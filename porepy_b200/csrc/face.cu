@@ -2,12 +2,10 @@
 // face-indexed grid handle: the face -> cell table and the three geometry arrays these schemes read.  Works
 // for grids of any dimension (the reference delegates its 1-D MPFA / MPSA to TPFA, numerics/fv/mpfa.py:
 // 690-712, mpsa.py:666-697); no interaction-region plan is built.
-#include "plan.hpp"
+#include "csr_build.cuh"
 #include "tpfa_diff.cuh"
 #include "tpsa_face.cuh"
 #include "tpsa_system.cuh"
-
-#include <cub/device/device_scan.cuh>
 
 struct pb_facegrid {
     int64_t nc = 0, nf = 0;
@@ -401,30 +399,23 @@ static TpsaTopo tpsa_topo(pb_facegrid *g) {
 
 // Neighbour counts of every cell, scanned into cc_ptr; *total = number of (cell, neighbour) pairs.  cc_ix / cc_cell are
 // sized for them.
-static int tpsa_neighbour_counts(pb_facegrid *g, int32_t *total_out) {
+static int tpsa_neighbour_counts(pb_facegrid *g, int64_t *total_out) {
     cudaStream_t st = g->stream;
     const int64_t nc = g->nc;
     const TpsaTopo t = tpsa_topo(g);
-    DevBuf count, bad, scratch;
-    CUDA_TRY(count.ensure((size_t)(nc + 1) * sizeof(int32_t)));
+    DevBuf count, bad;
+    CUDA_TRY(count.ensure((size_t)nc * sizeof(int32_t)));
     CUDA_TRY(bad.ensure(sizeof(int)));
     CUDA_TRY(cudaMemsetAsync(bad.p, 0, sizeof(int), st));
-    CUDA_TRY(cudaMemsetAsync(count.as<int32_t>() + nc, 0, sizeof(int32_t), st));
     tpsa_nb_count_kernel<<<fg_grid(nc), 256, 0, st>>>(t, count.as<int32_t>(), bad.as<int>());
     pb_count_launch_();
     CUDA_TRY(cudaGetLastError());
     CUDA_TRY(g->cc_ptr.ensure((size_t)(nc + 1) * sizeof(int32_t)));
-    size_t tmp_bytes = 0;
-    CUDA_TRY(cub::DeviceScan::ExclusiveSum(nullptr, tmp_bytes, count.as<int32_t>(), g->cc_ptr.as<int32_t>(),
-                                           (int)(nc + 1), st));
-    CUDA_TRY(scratch.ensure(tmp_bytes));
-    CUDA_TRY(cub::DeviceScan::ExclusiveSum(scratch.p, tmp_bytes, count.as<int32_t>(), g->cc_ptr.as<int32_t>(),
-                                           (int)(nc + 1), st));
     int hbad = 0;
-    int32_t total = 0;
     CUDA_TRY(cudaMemcpyAsync(&hbad, bad.p, sizeof(int), cudaMemcpyDeviceToHost, st));
-    CUDA_TRY(cudaMemcpyAsync(&total, g->cc_ptr.as<int32_t>() + nc, sizeof(int32_t), cudaMemcpyDeviceToHost, st));
-    CUDA_TRY(cudaStreamSynchronize(st));
+    int64_t total = 0;
+    const int rc = pb_scan_offsets_(count.as<int32_t>(), g->cc_ptr.as<int32_t>(), nc, st, &total);
+    if (rc) return rc;
     if (hbad) return pb_fail_(PB_ENOTIMPL, "Tpsa system: a cell has more than 31 face neighbours");
     CUDA_TRY(g->cc_ix.ensure((size_t)std::max<int64_t>(1, total) * sizeof(int32_t)));
     CUDA_TRY(g->cc_cell.ensure((size_t)std::max<int64_t>(1, total) * sizeof(int32_t)));
@@ -438,7 +429,7 @@ static int tpsa_build_pattern(pb_facegrid *g, int nd) {
     const int64_t nc = g->nc;
     const int B = nd == 3 ? 7 : 4, NZ = nd == 3 ? 37 : 12;
     const TpsaTopo t = tpsa_topo(g);
-    int32_t total = 0;
+    int64_t total = 0;
     int rc0 = tpsa_neighbour_counts(g, &total);
     if (rc0) return rc0;
     const int64_t nnz = (int64_t)NZ * total;
@@ -641,9 +632,10 @@ __global__ void tpsa_nb_list_kernel(TpsaTopo t, const int32_t *__restrict__ cc_p
 
 template <int ND>
 __global__ void tpsa_poro_count_kernel(int64_t nc, const int32_t *__restrict__ cc_ptr, const int32_t *__restrict__ fp_ip,
-                                       const int32_t *__restrict__ fp_ix, int64_t *__restrict__ count) {
+                                       const int32_t *__restrict__ fp_ix, int32_t *__restrict__ count) {
+    // clamped: a row past the int32 limit still makes the total overflow the limit of the caller
     for (int64_t c = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; c < nc; c += (int64_t)gridDim.x * blockDim.x)
-        count[c] = tpsa_poro_row_count<ND>(c, cc_ptr[c + 1] - cc_ptr[c], fp_ip, fp_ix);
+        count[c] = (int32_t)min(tpsa_poro_row_count<ND>(c, cc_ptr[c + 1] - cc_ptr[c], fp_ip, fp_ix), (int64_t)0x7fffffff);
 }
 
 template <int ND>
@@ -704,7 +696,7 @@ static int tpsa_poro_build_pattern(pb_facegrid *g, int nd, const CsrView &fp) {
     const int B = nd == 3 ? 8 : 5;
     const TpsaTopo t = tpsa_topo(g);
     if (!g->nb_ready) {
-        int32_t total = 0;
+        int64_t total = 0;
         int rc = tpsa_neighbour_counts(g, &total);
         if (rc) return rc;
         tpsa_nb_list_kernel<<<fg_grid(nc), 256, 0, st>>>(t, g->cc_ptr.as<int32_t>(), g->cc_ix.as<int32_t>(),
@@ -714,23 +706,16 @@ static int tpsa_poro_build_pattern(pb_facegrid *g, int nd, const CsrView &fp) {
         g->sys_npairs = total;
         g->nb_ready = true;
     }
-    DevBuf count, scratch;
-    CUDA_TRY(count.ensure((size_t)(nc + 1) * sizeof(int64_t)));
-    CUDA_TRY(cudaMemsetAsync(count.as<int64_t>() + nc, 0, sizeof(int64_t), st));
-    if (nd == 3) tpsa_poro_count_kernel<3><<<fg_grid(nc), 256, 0, st>>>(nc, g->cc_ptr.as<int32_t>(), fp.indptr, fp.indices, count.as<int64_t>());
-    else tpsa_poro_count_kernel<2><<<fg_grid(nc), 256, 0, st>>>(nc, g->cc_ptr.as<int32_t>(), fp.indptr, fp.indices, count.as<int64_t>());
+    DevBuf count;
+    CUDA_TRY(count.ensure((size_t)nc * sizeof(int32_t)));
+    if (nd == 3) tpsa_poro_count_kernel<3><<<fg_grid(nc), 256, 0, st>>>(nc, g->cc_ptr.as<int32_t>(), fp.indptr, fp.indices, count.as<int32_t>());
+    else tpsa_poro_count_kernel<2><<<fg_grid(nc), 256, 0, st>>>(nc, g->cc_ptr.as<int32_t>(), fp.indptr, fp.indices, count.as<int32_t>());
     pb_count_launch_();
     CUDA_TRY(cudaGetLastError());
     CUDA_TRY(g->blk_ptr.ensure((size_t)(nc + 1) * sizeof(int64_t)));
-    size_t tmp_bytes = 0;
-    CUDA_TRY(cub::DeviceScan::ExclusiveSum(nullptr, tmp_bytes, count.as<int64_t>(), g->blk_ptr.as<int64_t>(),
-                                           (int)(nc + 1), st));
-    CUDA_TRY(scratch.ensure(tmp_bytes));
-    CUDA_TRY(cub::DeviceScan::ExclusiveSum(scratch.p, tmp_bytes, count.as<int64_t>(), g->blk_ptr.as<int64_t>(),
-                                           (int)(nc + 1), st));
     int64_t nnz = 0;
-    CUDA_TRY(cudaMemcpyAsync(&nnz, g->blk_ptr.as<int64_t>() + nc, sizeof(int64_t), cudaMemcpyDeviceToHost, st));
-    CUDA_TRY(cudaStreamSynchronize(st));
+    const int rc = pb_scan_offsets_(count.as<int32_t>(), g->blk_ptr.as<int64_t>(), nc, st, &nnz);
+    if (rc) return rc;
     if (nnz >= 0x7FFFFFFFll) return pb_fail_(PB_ENOTIMPL, "Tpsa system: the matrix does not fit int32 indices");
     CUDA_TRY(g->poro_ip.ensure((size_t)(nc * B + 1) * sizeof(int32_t)));
     CUDA_TRY(g->poro_ix.ensure((size_t)std::max<int64_t>(1, nnz) * sizeof(int32_t)));

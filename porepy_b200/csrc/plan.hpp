@@ -167,8 +167,9 @@ struct pb_plan {
     cudaEvent_t e0 = nullptr, e1 = nullptr;
     // plan arrays
     DevBuf fn_indptr, node_sc_ptr, sc_cell, node_sf_ptr, sf_face, sf_sides, sf_bloc, slot_sf, node_nb,
-        sc_ncn, posfc_ptr, posfb_ptr, poscc_ptr, poscb_ptr, pos_fc, pos_fb, pos_cc, pos_cb, fc_indptr,
-        fb_indptr, cc_indptr, cb_indptr, pat_idx[4], nbf_ptr, nbf_idx, cn_ptr, cn_idx, face_cells;
+        sc_ncn, posfc_ptr, posfb_ptr, poscc_ptr, poscb_ptr, pos_fc, pos_fb, pos_cc, pos_cb, nbf_ptr, nbf_idx,
+        cn_ptr, cn_idx, face_cells;
+    DevBuf pat_ip[4], pat_idx[4];  // CSR of the structural pattern `which` (PB_PAT_*)
     DevBuf cf_ip, cf_ix, cf_sg;    // cell -> faces (CSC of cell_faces): the gather form of div_nd @ stress
     int64_t pat_rows[4] = {0, 0, 0, 0}, pat_cols[4] = {0, 0, 0, 0}, pat_nnz[4] = {0, 0, 0, 0};
     // geometry
@@ -278,7 +279,7 @@ int pb_launch_mpsa2_(pb_plan *p, const MpsaParams &prm, const MpsaOut &o);
 int pb_launch_mpsa3_(pb_plan *p, const MpsaParams &prm, const MpsaOut &o);
 // (ncomp, n) row-major host array -> entity-major records on the device (api.cu)
 int pb_upload_repacked_(cudaStream_t st, DevBuf &tmp, DevBuf &dst, const double *host, int ncomp, int64_t n);
-// sub-cell topology built on the device (plan_device.cu): 0 ok, > 0 error code with `err`, -1 = fall back to the host
+// sub-cell topology built on the device (plan_device.cu): 0 ok, > 0 error code (pb_fail_), -1 = fall back to the host
 int pb_build_device_topology_(pb_plan *p, int nd, int64_t nc, int64_t nf, int64_t nn, const int32_t *cf_indptr,
                               const int32_t *cf_indices, const int8_t *cf_data, const int32_t *fn_indptr,
-                              const int32_t *fn_indices, DevBuf &fn_idx_dev, std::string &err);
+                              const int32_t *fn_indices, DevBuf &fn_idx_dev);

@@ -12,7 +12,7 @@
 //   5. nodes per cell, cell -> node lists, boundary faces per node, face -> cell table
 // Only three per-node integer arrays (sub-cell / sub-face / boundary counts) return to the host, where the solver
 // classes and the position-map offsets are derived from them.
-#include "plan.hpp"
+#include "csr_build.cuh"
 
 struct HalfFace { int32_t c, f, u, sg; };
 
@@ -32,36 +32,6 @@ __global__ void pd_count_kernel(int64_t nc, const int32_t *__restrict__ cf_ip, c
 __global__ void pd_count_sf_kernel(int64_t U, const int32_t *__restrict__ fn_ix, int32_t *__restrict__ sfcount) {
     for (int64_t q = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; q < U; q += (int64_t)gridDim.x * blockDim.x)
         atomicAdd(sfcount + fn_ix[q], 1);
-}
-
-// exclusive scan of int32 counts (single block, serial over chunks), int32 result with n+1 entries
-__global__ void pd_scan_kernel(int64_t n, const int32_t *__restrict__ counts, int32_t *__restrict__ ptr, int div,
-                               int *bad) {
-    __shared__ long long wsum[32];
-    __shared__ long long carry;
-    if (threadIdx.x == 0) carry = 0;
-    __syncthreads();
-    const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
-    for (int64_t base = 0; base < n; base += blockDim.x) {
-        const int64_t i = base + threadIdx.x;
-        long long v = i < n ? counts[i] : 0;
-        if (div > 1) { if (v % div) atomicExch(bad, 3); v /= div; }
-        long long x = v;
-        for (int o = 1; o < 32; o <<= 1) { long long y = __shfl_up_sync(0xffffffffu, x, o); if (lane >= o) x += y; }
-        if (lane == 31) wsum[w] = x;
-        __syncthreads();
-        if (w == 0) {
-            long long t = lane < (blockDim.x >> 5) ? wsum[lane] : 0;
-            for (int o = 1; o < 32; o <<= 1) { long long y = __shfl_up_sync(0xffffffffu, t, o); if (lane >= o) t += y; }
-            wsum[lane] = t;
-        }
-        __syncthreads();
-        if (i < n) ptr[i] = (int32_t)(carry + (w ? wsum[w - 1] : 0) + x - v);
-        __syncthreads();
-        if (threadIdx.x == blockDim.x - 1) carry += wsum[(blockDim.x >> 5) - 1];
-        __syncthreads();
-    }
-    if (threadIdx.x == 0) { ptr[n] = (int32_t)carry; if (carry > 0x7fffffffll) atomicExch(bad, 8); }
 }
 
 __global__ void pd_scatter_kernel(int64_t nc, const int32_t *__restrict__ cf_ip, const int32_t *__restrict__ cf_ix,
@@ -121,33 +91,13 @@ __global__ void pd_node_kernel(int64_t nn, int nd, int64_t nf, const HalfFace *_
             } else { key[i] = ~0ull; pay[i] = 0; us[i] = 0x7fffffff; }
         }
         __syncwarp();
-        // bitonic sorts: (key, pay) by (cell, face); us by u
-        for (int kk = 2; kk <= P; kk <<= 1)
-            for (int j = kk >> 1; j > 0; j >>= 1) {
-                for (int i = lane; i < P; i += 32) {
-                    const int l = i ^ j;
-                    if (l > i) {
-                        const bool asc = (i & kk) == 0;
-                        const unsigned long long a = key[i], c = key[l];
-                        if ((a > c) == asc) { key[i] = c; key[l] = a; const int t = pay[i]; pay[i] = pay[l]; pay[l] = t; }
-                        const int ua = us[i], uc = us[l];
-                        if ((ua > uc) == asc) { us[i] = uc; us[l] = ua; }
-                    }
-                }
-                __syncwarp();
-            }
-        // unique sub-faces: in-place compaction of the sorted u's (a write never lands behind its source index)
-        int cnt = 0;
-        for (int i0 = 0; i0 < nh; i0 += 32) {
-            const int i = i0 + lane;
-            const bool flag = i < nh && (i == 0 || us[i] != us[i - 1]);
-            const int v = i < nh ? us[i] : 0;
-            const unsigned m = __ballot_sync(0xffffffffu, flag);
-            __syncwarp();
-            if (flag) us[cnt + __popc(m & ((1u << lane) - 1u))] = v;
-            cnt += __popc(m);
-            __syncwarp();
-        }
+        // bitonic sorts in one network: (key, pay) by (cell, face); us by u
+        warp_bitonic_sort(P, [&](int i, int l, bool asc) {
+            if (warp_cas(key, i, l, asc)) { const int t = pay[i]; pay[i] = pay[l]; pay[l] = t; }
+            warp_cas(us, i, l, asc);
+        });
+        // unique sub-faces: in-place compaction of the sorted u's
+        const int cnt = warp_unique(us, nh, us);
         if (cnt != nsf) { if (lane == 0) atomicOr(bad, 4); continue; }
         for (int i = lane; i < nsf; i += 32) { smin[i] = 0x7fffffff; smax[i] = -1; scnt[i] = 0; }
         __syncwarp();
@@ -198,9 +148,12 @@ __global__ void pd_node_kernel(int64_t nn, int nd, int64_t nf, const HalfFace *_
     if (lane == 0) { atomicMax(maxima, mx_sf); atomicMax(maxima + 1, mx_sc); atomicMax(maxima + 2, mx_nb); }
 }
 
-__global__ void pd_ncn_kernel(int64_t nc, int nd, const int32_t *__restrict__ ncn_x_nd, int32_t *__restrict__ sc_ncn) {
-    for (int64_t c = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; c < nc; c += (int64_t)gridDim.x * blockDim.x)
-        sc_ncn[c] = ncn_x_nd[c] / nd;
+// out = in / nd (in place allowed); with `bad`, flags 3 where nd does not divide the count
+__global__ void pd_div_kernel(int64_t n, int nd, const int32_t *in, int32_t *out, int *bad) {
+    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
+        if (bad && in[i] % nd) atomicExch(bad, 3);
+        out[i] = in[i] / nd;
+    }
 }
 
 // cell -> nodes (order inside a cell arbitrary) and boundary faces of every node (local boundary order)
@@ -236,79 +189,79 @@ __global__ void pd_face_cells_order_kernel(int64_t nf, int32_t *__restrict__ fc)
     }
 }
 
-#define PD_TRY(x)                                                                              \
-    do {                                                                                       \
-        cudaError_t e_ = (x);                                                                  \
-        if (e_ != cudaSuccess) { err = std::string(#x) + ": " + cudaGetErrorString(e_); return PB_ECUDA; } \
-    } while (0)
-
-// Returns PB_OK, an error code with `err`, or -1 when the per-node sort capacity was exceeded (caller falls back to
+// Returns PB_OK, an error code (pb_fail_), or -1 when the per-node sort capacity was exceeded (caller falls back to
 // the host plan).  On success the plan's topology DevBufs are filled and H holds the sizes and the three per-node arrays.
 int pb_build_device_topology_(pb_plan *p, int nd, int64_t nc, int64_t nf, int64_t nn, const int32_t *cf_indptr,
                               const int32_t *cf_indices, const int8_t *cf_data, const int32_t *fn_indptr,
-                              const int32_t *fn_indices, DevBuf &fn_idx_dev, std::string &err) {
+                              const int32_t *fn_indices, DevBuf &fn_idx_dev) {
     HostPlan &H = p->H;
     cudaStream_t st = p->stream;
-    if (nd != 2 && nd != 3) { err = "nd must be 2 or 3"; return PB_EINVAL; }
-    if (nc <= 0 || nf <= 0 || nn <= 0) { err = "empty grid"; return PB_EINVAL; }
+    if (nd != 2 && nd != 3) return pb_fail_(PB_EINVAL, "nd must be 2 or 3");
+    if (nc <= 0 || nf <= 0 || nn <= 0) return pb_fail_(PB_EINVAL, "empty grid");
     const int64_t U = fn_indptr[nf], CF = cf_indptr[nc];
     H.nd = nd; H.nc = nc; H.nf = nf; H.nn = nn; H.U = U;
     // cheap host validation of the index ranges (one pass over the inputs; also needed before trusting them on the device)
     for (int64_t q = 0; q < CF; ++q) {
-        if (cf_indices[q] < 0 || cf_indices[q] >= nf) { err = "cell_faces index out of range"; return PB_EINVAL; }
-        if (cf_data[q] != 1 && cf_data[q] != -1) { err = "cell_faces data must be +-1"; return PB_EINVAL; }
+        if (cf_indices[q] < 0 || cf_indices[q] >= nf) return pb_fail_(PB_EINVAL, "cell_faces index out of range");
+        if (cf_data[q] != 1 && cf_data[q] != -1) return pb_fail_(PB_EINVAL, "cell_faces data must be +-1");
     }
     for (int64_t q = 0; q < U; ++q)
-        if (fn_indices[q] < 0 || fn_indices[q] >= nn) { err = "face_nodes index out of range"; return PB_EINVAL; }
+        if (fn_indices[q] < 0 || fn_indices[q] >= nn) return pb_fail_(PB_EINVAL, "face_nodes index out of range");
     DevBuf cf_ip, cf_ix, cf_da, hcount, sfcount, ncnx, fill, hfbuf, flags, cfill;
-    PD_TRY(cf_ip.upload(cf_indptr, (size_t)nc + 1, st));
-    PD_TRY(cf_ix.upload(cf_indices, (size_t)CF, st));
-    PD_TRY(cf_da.upload(cf_data, (size_t)CF, st));
-    PD_TRY(p->fn_indptr.upload(fn_indptr, (size_t)nf + 1, st));
-    PD_TRY(fn_idx_dev.upload(fn_indices, (size_t)U, st));
-    PD_TRY(hcount.ensure((size_t)(nn + 1) * 4));
-    PD_TRY(sfcount.ensure((size_t)(nn + 1) * 4));
-    PD_TRY(fill.ensure((size_t)(nn + 1) * 4));
-    PD_TRY(ncnx.ensure((size_t)nc * 4));
-    PD_TRY(flags.ensure(8 * sizeof(int)));
-    PD_TRY(cudaMemsetAsync(hcount.p, 0, (size_t)(nn + 1) * 4, st));
-    PD_TRY(cudaMemsetAsync(sfcount.p, 0, (size_t)(nn + 1) * 4, st));
-    PD_TRY(cudaMemsetAsync(fill.p, 0, (size_t)(nn + 1) * 4, st));
-    PD_TRY(cudaMemsetAsync(flags.p, 0, 8 * sizeof(int), st));
+    CUDA_TRY(cf_ip.upload(cf_indptr, (size_t)nc + 1, st));
+    CUDA_TRY(cf_ix.upload(cf_indices, (size_t)CF, st));
+    CUDA_TRY(cf_da.upload(cf_data, (size_t)CF, st));
+    CUDA_TRY(p->fn_indptr.upload(fn_indptr, (size_t)nf + 1, st));
+    CUDA_TRY(fn_idx_dev.upload(fn_indices, (size_t)U, st));
+    CUDA_TRY(hcount.ensure((size_t)(nn + 1) * 4));
+    CUDA_TRY(sfcount.ensure((size_t)(nn + 1) * 4));
+    CUDA_TRY(fill.ensure((size_t)(nn + 1) * 4));
+    CUDA_TRY(ncnx.ensure((size_t)nc * 4));
+    CUDA_TRY(flags.ensure(8 * sizeof(int)));
+    CUDA_TRY(cudaMemsetAsync(hcount.p, 0, (size_t)(nn + 1) * 4, st));
+    CUDA_TRY(cudaMemsetAsync(sfcount.p, 0, (size_t)(nn + 1) * 4, st));
+    CUDA_TRY(cudaMemsetAsync(fill.p, 0, (size_t)(nn + 1) * 4, st));
+    CUDA_TRY(cudaMemsetAsync(flags.p, 0, 8 * sizeof(int), st));
     const int block = 256;
     auto grid_for = [&](int64_t n) { return (int)std::max<int64_t>(1, std::min<int64_t>((n + block - 1) / block, (int64_t)pb_sm_count() * 16)); };
     pd_count_kernel<<<grid_for(nc), block, 0, st>>>(nc, cf_ip.as<int32_t>(), cf_ix.as<int32_t>(), p->fn_indptr.as<int32_t>(),
                                                     fn_idx_dev.as<int32_t>(), hcount.as<int32_t>(), ncnx.as<int32_t>());
     pd_count_sf_kernel<<<grid_for(U), block, 0, st>>>(U, fn_idx_dev.as<int32_t>(), sfcount.as<int32_t>());
-    PD_TRY(p->node_sc_ptr.ensure((size_t)(nn + 1) * 4));
-    PD_TRY(p->node_sf_ptr.ensure((size_t)(nn + 1) * 4));
-    pd_scan_kernel<<<1, 1024, 0, st>>>(nn, hcount.as<int32_t>(), p->node_sc_ptr.as<int32_t>(), nd, flags.as<int>());
-    pd_scan_kernel<<<1, 1024, 0, st>>>(nn, sfcount.as<int32_t>(), p->node_sf_ptr.as<int32_t>(), 1, flags.as<int>());
+    // sub-cells per node = half-faces per node / nd
+    pd_div_kernel<<<grid_for(nn), block, 0, st>>>(nn, nd, hcount.as<int32_t>(), hcount.as<int32_t>(), flags.as<int>());
+    CUDA_TRY(p->node_sc_ptr.ensure((size_t)(nn + 1) * 4));
+    CUDA_TRY(p->node_sf_ptr.ensure((size_t)(nn + 1) * 4));
+    int64_t S = 0, sf_total = 0;
+    int rc = pb_scan_offsets_(hcount.as<int32_t>(), p->node_sc_ptr.as<int32_t>(), nn, st, &S);
+    if (rc) return rc;
+    rc = pb_scan_offsets_(sfcount.as<int32_t>(), p->node_sf_ptr.as<int32_t>(), nn, st, &sf_total);
+    if (rc) return rc;
     H.node_sc_ptr.resize(nn + 1);
     H.node_sf_ptr.resize(nn + 1);
-    PD_TRY(cudaMemcpyAsync(H.node_sc_ptr.data(), p->node_sc_ptr.p, (size_t)(nn + 1) * 4, cudaMemcpyDeviceToHost, st));
-    PD_TRY(cudaMemcpyAsync(H.node_sf_ptr.data(), p->node_sf_ptr.p, (size_t)(nn + 1) * 4, cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(cudaMemcpyAsync(H.node_sc_ptr.data(), p->node_sc_ptr.p, (size_t)(nn + 1) * 4, cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(cudaMemcpyAsync(H.node_sf_ptr.data(), p->node_sf_ptr.p, (size_t)(nn + 1) * 4, cudaMemcpyDeviceToHost, st));
     int hflags[8];
-    PD_TRY(cudaMemcpyAsync(hflags, flags.p, sizeof(hflags), cudaMemcpyDeviceToHost, st));
-    PD_TRY(cudaStreamSynchronize(st));
-    if (hflags[0] == 3) { err = "cells must have exactly nd faces meeting in each vertex"; return PB_ECELLTYPE; }
-    if (hflags[0] == 8) { err = "grid too large for 32-bit sub-cell indices; split the grid"; return PB_EINVAL; }
-    const int64_t S = H.node_sc_ptr[nn], Hh = S * nd;
+    CUDA_TRY(cudaMemcpyAsync(hflags, flags.p, sizeof(hflags), cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(cudaStreamSynchronize(st));
+    if (S > 0x7fffffffll || sf_total > 0x7fffffffll)
+        return pb_fail_(PB_EINVAL, "grid too large for 32-bit sub-cell indices; split the grid");
+    if (hflags[0] == 3) return pb_fail_(PB_ECELLTYPE, "cells must have exactly nd faces meeting in each vertex");
+    const int64_t Hh = S * nd;
     H.S = S; H.H = Hh;
-    if (H.node_sf_ptr[nn] != U) { err = "internal: sub-face count"; return PB_EINVAL; }
-    PD_TRY(hfbuf.ensure((size_t)std::max<int64_t>(1, Hh) * sizeof(HalfFace)));
+    if (sf_total != U) return pb_fail_(PB_EINVAL, "internal: sub-face count");
+    CUDA_TRY(hfbuf.ensure((size_t)std::max<int64_t>(1, Hh) * sizeof(HalfFace)));
     pd_scatter_kernel<<<grid_for(nc), block, 0, st>>>(nc, cf_ip.as<int32_t>(), cf_ix.as<int32_t>(), cf_da.as<int8_t>(),
                                                       p->fn_indptr.as<int32_t>(), fn_idx_dev.as<int32_t>(),
                                                       p->node_sc_ptr.as<int32_t>(), nd, fill.as<int32_t>(), hfbuf.as<HalfFace>());
-    PD_TRY(p->sc_cell.ensure((size_t)std::max<int64_t>(1, S) * 4));
-    PD_TRY(p->slot_sf.ensure((size_t)std::max<int64_t>(1, Hh) * 2));
-    PD_TRY(p->sf_face.ensure((size_t)std::max<int64_t>(1, U) * 4));
-    PD_TRY(p->sf_sides.ensure((size_t)std::max<int64_t>(1, U) * 4));
-    PD_TRY(p->sf_bloc.ensure((size_t)std::max<int64_t>(1, U) * 2));
-    PD_TRY(p->node_nb.ensure((size_t)(nn + 1) * 4));
+    CUDA_TRY(p->sc_cell.ensure((size_t)std::max<int64_t>(1, S) * 4));
+    CUDA_TRY(p->slot_sf.ensure((size_t)std::max<int64_t>(1, Hh) * 2));
+    CUDA_TRY(p->sf_face.ensure((size_t)std::max<int64_t>(1, U) * 4));
+    CUDA_TRY(p->sf_sides.ensure((size_t)std::max<int64_t>(1, U) * 4));
+    CUDA_TRY(p->sf_bloc.ensure((size_t)std::max<int64_t>(1, U) * 2));
+    CUDA_TRY(p->node_nb.ensure((size_t)(nn + 1) * 4));
     constexpr int CAP = 1024, WPB = 4;
     const size_t smem = (size_t)WPB * CAP * (8 + 5 * 4);
-    PD_TRY(cudaFuncSetAttribute(pd_node_kernel<CAP>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    CUDA_TRY(cudaFuncSetAttribute(pd_node_kernel<CAP>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     const int gridn = (int)std::max<int64_t>(1, std::min<int64_t>((nn + WPB - 1) / WPB, (int64_t)pb_sm_count() * 2));
     pd_node_kernel<CAP><<<gridn, WPB * 32, smem, st>>>(nn, nd, nf, hfbuf.as<HalfFace>(), p->node_sc_ptr.as<int32_t>(),
                                                        p->node_sf_ptr.as<int32_t>(), p->fn_indptr.as<int32_t>(),
@@ -317,41 +270,42 @@ int pb_build_device_topology_(pb_plan *p, int nd, int64_t nc, int64_t nf, int64_
                                                        p->sf_bloc.as<uint16_t>(), p->node_nb.as<int32_t>(),
                                                        flags.as<int>() + 1, flags.as<int>() + 4);
     // nodes per cell, cell -> nodes, boundary faces per node, face -> cells
-    PD_TRY(p->sc_ncn.ensure((size_t)nc * 4));
-    pd_ncn_kernel<<<grid_for(nc), block, 0, st>>>(nc, nd, ncnx.as<int32_t>(), p->sc_ncn.as<int32_t>());
-    PD_TRY(p->cn_ptr.ensure((size_t)(nc + 1) * 4));
-    PD_TRY(p->nbf_ptr.ensure((size_t)(nn + 1) * 4));
-    pd_scan_kernel<<<1, 1024, 0, st>>>(nc, p->sc_ncn.as<int32_t>(), p->cn_ptr.as<int32_t>(), 1, flags.as<int>());
-    pd_scan_kernel<<<1, 1024, 0, st>>>(nn, p->node_nb.as<int32_t>(), p->nbf_ptr.as<int32_t>(), 1, flags.as<int>());
+    CUDA_TRY(p->sc_ncn.ensure((size_t)nc * 4));
+    pd_div_kernel<<<grid_for(nc), block, 0, st>>>(nc, nd, ncnx.as<int32_t>(), p->sc_ncn.as<int32_t>(), nullptr);
+    CUDA_TRY(p->cn_ptr.ensure((size_t)(nc + 1) * 4));
+    CUDA_TRY(p->nbf_ptr.ensure((size_t)(nn + 1) * 4));
+    int64_t cn_total = 0, nbf_total = 0;
+    rc = pb_scan_offsets_(p->sc_ncn.as<int32_t>(), p->cn_ptr.as<int32_t>(), nc, st, &cn_total);
+    if (rc) return rc;
+    rc = pb_scan_offsets_(p->node_nb.as<int32_t>(), p->nbf_ptr.as<int32_t>(), nn, st, &nbf_total);
+    if (rc) return rc;
     H.node_nb.resize(nn);
-    int32_t nbf_total = 0;
-    PD_TRY(cudaMemcpyAsync(H.node_nb.data(), p->node_nb.p, (size_t)nn * 4, cudaMemcpyDeviceToHost, st));
-    PD_TRY(cudaMemcpyAsync(&nbf_total, p->nbf_ptr.as<int32_t>() + nn, 4, cudaMemcpyDeviceToHost, st));
-    PD_TRY(cudaMemcpyAsync(hflags, flags.p, sizeof(hflags), cudaMemcpyDeviceToHost, st));
-    PD_TRY(cudaStreamSynchronize(st));
+    CUDA_TRY(cudaMemcpyAsync(H.node_nb.data(), p->node_nb.p, (size_t)nn * 4, cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(cudaMemcpyAsync(hflags, flags.p, sizeof(hflags), cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(cudaStreamSynchronize(st));
     if (hflags[1] & 64) return -1;   // an interaction region exceeds the shared-memory sort: host plan
-    if (hflags[1] & 3) { err = "cells must have exactly nd faces meeting in each vertex"; return PB_ECELLTYPE; }
-    if (hflags[1] & 4) { err = "face_nodes holds nodes without neighbouring cells"; return PB_EINVAL; }
-    if (hflags[1] & 16) { err = "face with more than two neighbouring cells"; return PB_EINVAL; }
-    if (hflags[1]) { err = "internal: topology plan"; return PB_EINVAL; }
+    if (hflags[1] & 3) return pb_fail_(PB_ECELLTYPE, "cells must have exactly nd faces meeting in each vertex");
+    if (hflags[1] & 4) return pb_fail_(PB_EINVAL, "face_nodes holds nodes without neighbouring cells");
+    if (hflags[1] & 16) return pb_fail_(PB_EINVAL, "face with more than two neighbouring cells");
+    if (hflags[1]) return pb_fail_(PB_EINVAL, "internal: topology plan");
     H.max_nsf = hflags[4]; H.max_nsc = hflags[5]; H.max_nb = hflags[6];
-    if (H.max_nsf > 32767 || H.max_nsc > 21000) { err = "interaction region too large"; return PB_EINVAL; }
-    PD_TRY(cfill.ensure((size_t)nc * 4));
-    PD_TRY(cudaMemsetAsync(cfill.p, 0, (size_t)nc * 4, st));
-    PD_TRY(p->cn_idx.ensure((size_t)std::max<int64_t>(1, S) * 4));
-    PD_TRY(p->nbf_idx.ensure((size_t)std::max<int64_t>(1, nbf_total) * 4));
+    if (H.max_nsf > 32767 || H.max_nsc > 21000) return pb_fail_(PB_EINVAL, "interaction region too large");
+    CUDA_TRY(cfill.ensure((size_t)nc * 4));
+    CUDA_TRY(cudaMemsetAsync(cfill.p, 0, (size_t)nc * 4, st));
+    CUDA_TRY(p->cn_idx.ensure((size_t)std::max<int64_t>(1, S) * 4));
+    CUDA_TRY(p->nbf_idx.ensure((size_t)std::max<int64_t>(1, nbf_total) * 4));
     pd_adjacency_kernel<<<grid_for(nn), block, 0, st>>>(nn, p->node_sc_ptr.as<int32_t>(), p->sc_cell.as<int32_t>(),
                                                         p->cn_ptr.as<int32_t>(), cfill.as<int32_t>(), p->cn_idx.as<int32_t>(),
                                                         p->node_sf_ptr.as<int32_t>(), p->sf_face.as<int32_t>(),
                                                         p->sf_bloc.as<uint16_t>(), p->nbf_ptr.as<int32_t>(),
                                                         p->nbf_idx.as<int32_t>());
-    PD_TRY(p->face_cells.ensure((size_t)2 * nf * 4));
-    PD_TRY(cudaMemsetAsync(p->face_cells.p, 0xFF, (size_t)2 * nf * 4, st));
+    CUDA_TRY(p->face_cells.ensure((size_t)2 * nf * 4));
+    CUDA_TRY(cudaMemsetAsync(p->face_cells.p, 0xFF, (size_t)2 * nf * 4, st));
     pd_face_cells_kernel<<<grid_for(nc), block, 0, st>>>(nc, cf_ip.as<int32_t>(), cf_ix.as<int32_t>(), cf_da.as<int8_t>(),
                                                          p->face_cells.as<int32_t>(), flags.as<int>() + 2);
     pd_face_cells_order_kernel<<<grid_for(nf), block, 0, st>>>(nf, p->face_cells.as<int32_t>());
-    for (int i = 0; i < 12; ++i) pb_count_launch_();
-    PD_TRY(cudaGetLastError());
+    for (int i = 0; i < 9; ++i) pb_count_launch_();
+    CUDA_TRY(cudaGetLastError());
     // position-map offsets on the host from the three per-node arrays
     H.posfc_ptr.assign(nn + 1, 0); H.posfb_ptr.assign(nn + 1, 0);
     H.poscc_ptr.assign(nn + 1, 0); H.poscb_ptr.assign(nn + 1, 0);
@@ -364,13 +318,13 @@ int pb_build_device_topology_(pb_plan *p, int nd, int64_t nc, int64_t nf, int64_
         H.poscc_ptr[s + 1] = H.poscc_ptr[s] + nsc * nsc;
         H.poscb_ptr[s + 1] = H.poscb_ptr[s] + nsc * nb;
     }
-    PD_TRY(p->posfc_ptr.upload(H.posfc_ptr, st));
-    PD_TRY(p->posfb_ptr.upload(H.posfb_ptr, st));
-    PD_TRY(p->poscc_ptr.upload(H.poscc_ptr, st));
-    PD_TRY(p->poscb_ptr.upload(H.poscb_ptr, st));
-    PD_TRY(cudaMemcpyAsync(hflags, flags.p, sizeof(hflags), cudaMemcpyDeviceToHost, st));
-    PD_TRY(cudaStreamSynchronize(st));
-    if (hflags[2]) { err = "face with more than two neighbouring cells"; return PB_EINVAL; }
+    CUDA_TRY(p->posfc_ptr.upload(H.posfc_ptr, st));
+    CUDA_TRY(p->posfb_ptr.upload(H.posfb_ptr, st));
+    CUDA_TRY(p->poscc_ptr.upload(H.poscc_ptr, st));
+    CUDA_TRY(p->poscb_ptr.upload(H.poscb_ptr, st));
+    CUDA_TRY(cudaMemcpyAsync(hflags, flags.p, sizeof(hflags), cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(cudaStreamSynchronize(st));
+    if (hflags[2]) return pb_fail_(PB_EINVAL, "face with more than two neighbouring cells");
     p->cf_ip = std::move(cf_ip);
     p->cf_ix = std::move(cf_ix);
     p->cf_sg = std::move(cf_da);

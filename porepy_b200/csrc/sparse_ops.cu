@@ -6,7 +6,7 @@
 //   block_diag(mats)   MergedOperator.parse (csr_matrix_from_sparse_blocks)   numerics/ad/ad_utils.py:597-664
 //   vstack(blocks)     EquationSystem.assemble                      numerics/ad/equation_system.py:1695-1713
 // on pb_csr matrices that never leave HBM.  FP64 values, int32 indices, sorted rows (canonical CSR, like scipy's).
-#include "plan.hpp"
+#include "csr_build.cuh"
 
 struct pb_csr;
 int pb_csr_alloc_(int64_t nrows, int64_t ncols, int64_t nnz, pb_csr **out);  // spmv.cu
@@ -14,32 +14,32 @@ struct CsrView { int64_t nrows, ncols, nnz; int32_t *indptr, *indices; double *d
 CsrView pb_csr_view_(const pb_csr *a);                                        // spmv.cu
 void pb_csr_set_nnz_(pb_csr *a, int64_t nnz);                                 // spmv.cu (shrink only)
 
-// ---- exclusive scan of int32 counts into int32 row pointers (single block; rows <= ~10^7) ----------------------
-__global__ void so_scan_kernel(int64_t n, const int32_t *__restrict__ counts, int32_t *__restrict__ indptr,
-                               long long *total_out) {
-    __shared__ long long wsum[32];
-    __shared__ long long carry;
-    if (threadIdx.x == 0) carry = 0;
-    __syncthreads();
-    const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
-    for (int64_t base = 0; base < n; base += blockDim.x) {
-        const int64_t i = base + threadIdx.x;
-        long long v = i < n ? counts[i] : 0, x = v;
-        for (int o = 1; o < 32; o <<= 1) { long long y = __shfl_up_sync(0xffffffffu, x, o); if (lane >= o) x += y; }
-        if (lane == 31) wsum[w] = x;
-        __syncthreads();
-        if (w == 0) {
-            long long t = lane < (blockDim.x >> 5) ? wsum[lane] : 0;
-            for (int o = 1; o < 32; o <<= 1) { long long y = __shfl_up_sync(0xffffffffu, t, o); if (lane >= o) t += y; }
-            wsum[lane] = t;
-        }
-        __syncthreads();
-        if (i < n) indptr[i] = (int32_t)(carry + (w ? wsum[w - 1] : 0) + x - v);
-        __syncthreads();
-        if (threadIdx.x == blockDim.x - 1) carry += wsum[(blockDim.x >> 5) - 1];
-        __syncthreads();
-    }
-    if (threadIdx.x == 0) { indptr[n] = (int32_t)carry; *total_out = carry; }
+// The two passes of every operation here, on the legacy default stream: count(counts) launches the pass that writes
+// the length of each of the nrows rows of C (and may refuse), the lengths are scanned into C's row offsets, and
+// fill(C) launches the pass that writes C's entries.  `what` names the result in the overflow message.
+template <class Count, class Fill>
+static int csr_two_pass(int64_t nrows, int64_t ncols, const char *what, Count count, Fill fill, pb_csr **out) {
+    DevBuf counts, ip;
+    CUDA_TRY(counts.ensure((size_t)nrows * sizeof(int32_t)));
+    CUDA_TRY(ip.ensure((size_t)(nrows + 1) * sizeof(int32_t)));
+    pb_count_launch_();
+    int rc = count(counts.as<int32_t>());
+    if (rc) return rc;
+    int64_t nnz = 0;
+    rc = pb_scan_offsets_(counts.as<int32_t>(), ip.as<int32_t>(), nrows, 0, &nnz);
+    if (rc) return rc;
+    if (nnz >= 0x7fffffffll) return pb_fail_(PB_ENOTIMPL, std::string(what) + " exceeds int32 indices");
+    pb_csr *c = nullptr;
+    rc = pb_csr_alloc_(nrows, ncols, nnz, &c);
+    if (rc) return rc;
+    const CsrView C = pb_csr_view_(c);
+    CUDA_TRY(cudaMemcpy(C.indptr, ip.p, (size_t)(nrows + 1) * sizeof(int32_t), cudaMemcpyDeviceToDevice));
+    fill(C);
+    pb_count_launch_();
+    CUDA_TRY(cudaGetLastError());
+    CUDA_TRY(cudaDeviceSynchronize());
+    *out = c;
+    return PB_OK;
 }
 
 // ---- SpGEMM: one warp per row of A, hash table in shared memory -------------------------------------------------
@@ -112,20 +112,9 @@ __global__ void spgemm_kernel(int64_t nrows, const int32_t *__restrict__ aip, co
             vals[i] = i < len ? cda[base + i] : 0.0;
         }
         __syncwarp();
-        for (int kk = 2; kk <= P; kk <<= 1)
-            for (int j = kk >> 1; j > 0; j >>= 1) {
-                for (int i = lane; i < P; i += 32) {
-                    const int l = i ^ j;
-                    if (l > i) {
-                        const int a = keys[i], c = keys[l];
-                        if ((a > c) == ((i & kk) == 0)) {
-                            keys[i] = c; keys[l] = a;
-                            const double t = vals[i]; vals[i] = vals[l]; vals[l] = t;
-                        }
-                    }
-                }
-                __syncwarp();
-            }
+        warp_bitonic_sort(P, [&](int i, int l, bool asc) {
+            if (warp_cas(keys, i, l, asc)) { const double t = vals[i]; vals[i] = vals[l]; vals[l] = t; }
+        });
         for (int i = lane; i < len; i += 32) { cix[base + i] = keys[i]; cda[base + i] = vals[i]; }
         __syncwarp();
     }
@@ -135,14 +124,12 @@ extern "C" int pb_csr_spgemm(const pb_csr *a_, const pb_csr *b_, pb_csr **out) {
     if (!a_ || !b_ || !out) return pb_fail_(PB_EINVAL, "null pointer");
     const CsrView A = pb_csr_view_(a_), B = pb_csr_view_(b_);
     if (A.ncols != B.nrows) return pb_fail_(PB_EINVAL, "dimension mismatch in sparse product");
-    DevBuf counts, ip, flag, total;
-    CUDA_TRY(counts.ensure((size_t)(A.nrows + 1) * sizeof(int32_t)));
-    CUDA_TRY(ip.ensure((size_t)(A.nrows + 1) * sizeof(int32_t)));
+    DevBuf flag;
     CUDA_TRY(flag.ensure(2 * sizeof(int)));
-    CUDA_TRY(total.ensure(sizeof(long long)));
     CUDA_TRY(cudaMemset(flag.p, 0, 2 * sizeof(int)));
     const int g1 = (int)std::max<int64_t>(1, std::min<int64_t>((A.nrows + 255) / 256, (int64_t)pb_sm_count() * 8));
     spgemm_bound_kernel<<<g1, 256>>>(A.nrows, A.indptr, A.indices, B.indptr, flag.as<int>() + 1);
+    pb_count_launch_();
     int hb[2] = {0, 0};
     CUDA_TRY(cudaMemcpy(hb, flag.p, sizeof(hb), cudaMemcpyDeviceToHost));
     long long want = std::min<long long>(2ll * hb[1], 2ll * (long long)B.ncols);
@@ -155,26 +142,20 @@ extern "C" int pb_csr_spgemm(const pb_csr *a_, const pb_csr *b_, pb_csr **out) {
     CUDA_TRY(cudaFuncSetAttribute(spgemm_kernel<0>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     CUDA_TRY(cudaFuncSetAttribute(spgemm_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     const int grid = (int)std::max<int64_t>(1, std::min<int64_t>((A.nrows + wpb - 1) / wpb, (int64_t)pb_sm_count() * 4));
-    spgemm_kernel<0><<<grid, wpb * 32, smem>>>(A.nrows, A.indptr, A.indices, A.data, B.indptr, B.indices, B.data, tsize,
-                                               counts.as<int32_t>(), nullptr, nullptr, nullptr, flag.as<int>());
-    so_scan_kernel<<<1, 1024>>>(A.nrows, counts.as<int32_t>(), ip.as<int32_t>(), total.as<long long>());
-    long long nnz = 0;
-    CUDA_TRY(cudaMemcpy(&nnz, total.p, sizeof(nnz), cudaMemcpyDeviceToHost));
-    CUDA_TRY(cudaMemcpy(hb, flag.p, sizeof(int), cudaMemcpyDeviceToHost));
-    if (hb[0]) return pb_fail_(PB_ECUDA, "sparse product: hash table overflow");
-    if (nnz >= 0x7fffffffll) return pb_fail_(PB_ENOTIMPL, "sparse product exceeds int32 indices");
-    pb_csr *c = nullptr;
-    int rc = pb_csr_alloc_(A.nrows, B.ncols, nnz, &c);
-    if (rc) return rc;
-    const CsrView C = pb_csr_view_(c);
-    CUDA_TRY(cudaMemcpy(C.indptr, ip.p, (size_t)(A.nrows + 1) * sizeof(int32_t), cudaMemcpyDeviceToDevice));
-    spgemm_kernel<1><<<grid, wpb * 32, smem>>>(A.nrows, A.indptr, A.indices, A.data, B.indptr, B.indices, B.data, tsize,
-                                               nullptr, C.indptr, C.indices, C.data, flag.as<int>());
-    for (int i = 0; i < 4; ++i) pb_count_launch_();
-    CUDA_TRY(cudaGetLastError());
-    CUDA_TRY(cudaDeviceSynchronize());
-    *out = c;
-    return PB_OK;
+    return csr_two_pass(
+        A.nrows, B.ncols, "sparse product",
+        [&](int32_t *counts) {
+            spgemm_kernel<0><<<grid, wpb * 32, smem>>>(A.nrows, A.indptr, A.indices, A.data, B.indptr, B.indices, B.data,
+                                                       tsize, counts, nullptr, nullptr, nullptr, flag.as<int>());
+            CUDA_TRY(cudaMemcpy(hb, flag.p, sizeof(int), cudaMemcpyDeviceToHost));
+            if (hb[0]) return pb_fail_(PB_ECUDA, "sparse product: hash table overflow");
+            return PB_OK;
+        },
+        [&](const CsrView &C) {
+            spgemm_kernel<1><<<grid, wpb * 32, smem>>>(A.nrows, A.indptr, A.indices, A.data, B.indptr, B.indices, B.data,
+                                                       tsize, nullptr, C.indptr, C.indices, C.data, flag.as<int>());
+        },
+        out);
 }
 
 // ---- C = alpha A + beta B on the union pattern (sorted-row merge; one thread per row) ---------------------------
@@ -207,29 +188,19 @@ extern "C" int pb_csr_axpby(double alpha, const pb_csr *a_, double beta, const p
     if (!a_ || !b_ || !out) return pb_fail_(PB_EINVAL, "null pointer");
     const CsrView A = pb_csr_view_(a_), B = pb_csr_view_(b_);
     if (A.nrows != B.nrows || A.ncols != B.ncols) return pb_fail_(PB_EINVAL, "dimension mismatch in sparse sum");
-    DevBuf counts, ip, total;
-    CUDA_TRY(counts.ensure((size_t)(A.nrows + 1) * sizeof(int32_t)));
-    CUDA_TRY(ip.ensure((size_t)(A.nrows + 1) * sizeof(int32_t)));
-    CUDA_TRY(total.ensure(sizeof(long long)));
     const int grid = (int)std::max<int64_t>(1, std::min<int64_t>((A.nrows + 127) / 128, (int64_t)pb_sm_count() * 16));
-    axpby_kernel<0><<<grid, 128>>>(A.nrows, alpha, A.indptr, A.indices, A.data, beta, B.indptr, B.indices, B.data,
-                                   counts.as<int32_t>(), nullptr, nullptr, nullptr);
-    so_scan_kernel<<<1, 1024>>>(A.nrows, counts.as<int32_t>(), ip.as<int32_t>(), total.as<long long>());
-    long long nnz = 0;
-    CUDA_TRY(cudaMemcpy(&nnz, total.p, sizeof(nnz), cudaMemcpyDeviceToHost));
-    if (nnz >= 0x7fffffffll) return pb_fail_(PB_ENOTIMPL, "sparse sum exceeds int32 indices");
-    pb_csr *c = nullptr;
-    int rc = pb_csr_alloc_(A.nrows, A.ncols, nnz, &c);
-    if (rc) return rc;
-    const CsrView C = pb_csr_view_(c);
-    CUDA_TRY(cudaMemcpy(C.indptr, ip.p, (size_t)(A.nrows + 1) * sizeof(int32_t), cudaMemcpyDeviceToDevice));
-    axpby_kernel<1><<<grid, 128>>>(A.nrows, alpha, A.indptr, A.indices, A.data, beta, B.indptr, B.indices, B.data,
-                                   nullptr, C.indptr, C.indices, C.data);
-    for (int i = 0; i < 3; ++i) pb_count_launch_();
-    CUDA_TRY(cudaGetLastError());
-    CUDA_TRY(cudaDeviceSynchronize());
-    *out = c;
-    return PB_OK;
+    return csr_two_pass(
+        A.nrows, A.ncols, "sparse sum",
+        [&](int32_t *counts) {
+            axpby_kernel<0><<<grid, 128>>>(A.nrows, alpha, A.indptr, A.indices, A.data, beta, B.indptr, B.indices, B.data,
+                                           counts, nullptr, nullptr, nullptr);
+            return PB_OK;
+        },
+        [&](const CsrView &C) {
+            axpby_kernel<1><<<grid, 128>>>(A.nrows, alpha, A.indptr, A.indices, A.data, beta, B.indptr, B.indices, B.data,
+                                           nullptr, C.indptr, C.indices, C.data);
+        },
+        out);
 }
 
 // ---- diag(d) @ A and A @ diag(d): same pattern, scaled values (d: DEVICE vector) -------------------------------
@@ -309,30 +280,21 @@ extern "C" int pb_csr_bmat(int nbr, int nbc, const pb_csr *const *blocks, const 
         }
     if (co[nbc] >= 0x7fffffffll) return pb_fail_(PB_ENOTIMPL, "block matrix exceeds int32 column indices");
     const int64_t nrows = ro[nbr];
-    DevBuf dblocks, drow, dcol, counts, ip, total;
+    DevBuf dblocks, drow, dcol;
     CUDA_TRY(dblocks.upload(hb, 0));
     CUDA_TRY(drow.upload(ro, 0));
     CUDA_TRY(dcol.upload(co, 0));
-    CUDA_TRY(counts.ensure((size_t)(nrows + 1) * sizeof(int32_t)));
-    CUDA_TRY(ip.ensure((size_t)(nrows + 1) * sizeof(int32_t)));
-    CUDA_TRY(total.ensure(sizeof(long long)));
     const int grid = (int)std::max<int64_t>(1, std::min<int64_t>((nrows + 127) / 128, (int64_t)pb_sm_count() * 16));
-    bmat_kernel<0><<<grid, 128>>>(nbr, nbc, dblocks.as<BlockDesc>(), drow.as<int64_t>(), dcol.as<int64_t>(), nrows,
-                                  counts.as<int32_t>(), nullptr, nullptr, nullptr);
-    so_scan_kernel<<<1, 1024>>>(nrows, counts.as<int32_t>(), ip.as<int32_t>(), total.as<long long>());
-    long long nnz = 0;
-    CUDA_TRY(cudaMemcpy(&nnz, total.p, sizeof(nnz), cudaMemcpyDeviceToHost));
-    if (nnz >= 0x7fffffffll) return pb_fail_(PB_ENOTIMPL, "block matrix exceeds int32 indices");
-    pb_csr *c = nullptr;
-    int rc = pb_csr_alloc_(nrows, co[nbc], nnz, &c);
-    if (rc) return rc;
-    const CsrView C = pb_csr_view_(c);
-    CUDA_TRY(cudaMemcpy(C.indptr, ip.p, (size_t)(nrows + 1) * sizeof(int32_t), cudaMemcpyDeviceToDevice));
-    bmat_kernel<1><<<grid, 128>>>(nbr, nbc, dblocks.as<BlockDesc>(), drow.as<int64_t>(), dcol.as<int64_t>(), nrows,
-                                  nullptr, C.indptr, C.indices, C.data);
-    for (int i = 0; i < 3; ++i) pb_count_launch_();
-    CUDA_TRY(cudaGetLastError());
-    CUDA_TRY(cudaDeviceSynchronize());
-    *out = c;
-    return PB_OK;
+    return csr_two_pass(
+        nrows, co[nbc], "block matrix",
+        [&](int32_t *counts) {
+            bmat_kernel<0><<<grid, 128>>>(nbr, nbc, dblocks.as<BlockDesc>(), drow.as<int64_t>(), dcol.as<int64_t>(), nrows,
+                                          counts, nullptr, nullptr, nullptr);
+            return PB_OK;
+        },
+        [&](const CsrView &C) {
+            bmat_kernel<1><<<grid, 128>>>(nbr, nbc, dblocks.as<BlockDesc>(), drow.as<int64_t>(), dcol.as<int64_t>(), nrows,
+                                          nullptr, C.indptr, C.indices, C.data);
+        },
+        out);
 }

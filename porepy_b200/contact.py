@@ -1,10 +1,11 @@
 """Frictional contact on fractures, the reference's ``pp.MomentumBalance`` on the device AD chain -- the contact part of
 BASELINE config[4]: MPSA elasticity in the 3-D matrix (``porepy_b200.Mpsa``; the two sides of every fracture are internal
 Dirichlet boundaries carrying the interface displacement), force balance on the matrix-fracture interfaces and the
-semismooth complementarity laws of the contact traction.
+semismooth complementarity laws of the contact traction.  The matrix is 2-D or 3-D (``nd = sd.dim``), the fractures are
+lines or planes of dimension ``nd - 1``.
 
-Unknowns: [u (3 per matrix cell) | t (contact traction, 3 per fracture cell, in the fracture's local frame: two tangential
-components, then the normal one; scaled by the characteristic traction) | u_j (3 per mortar cell)];
+Unknowns: [u (nd per matrix cell) | t (contact traction, nd per fracture cell, in the fracture's local frame: the nd - 1
+tangential components, then the normal one; scaled by the characteristic traction) | u_j (nd per mortar cell)];
 equations, in the reference's order:
 
 * ``momentum_balance_equation``        -div_nd (stress u + bound_stress (u_b + Pi^avg u_j)) - f          models/momentum_balance.py
@@ -42,21 +43,41 @@ class FractureContact:
     """One fracture and its two-sided interface: ``mortar_to_primary_avg``, ``primary_to_mortar_int`` (faces of the matrix
     grid), ``mortar_to_secondary_avg``, ``secondary_to_mortar_int`` (cells of the fracture): the SCALAR projections of the
     reference's ``MortarGrid``; ``mortar_sign`` (+-1 per mortar cell: ``sign_of_mortar_sides``), ``mortar_volumes``,
-    ``local_coordinates`` (3 nfc x 3 nfc, rows per cell: tangent, tangent, normal)."""
+    ``local_coordinates`` (nd nfc x nd nfc, rows per cell: the nd - 1 tangents, then the normal; ``nd`` follows from its
+size)."""
 
     def __init__(self, mortar_to_primary_avg, primary_to_mortar_int, mortar_to_secondary_avg, secondary_to_mortar_int,
                  mortar_sign, mortar_volumes, local_coordinates):
-        i3 = sps.identity(3, format="csr")
-        self.m2p = sps.kron(sps.csr_matrix(mortar_to_primary_avg), i3).tocsr()
-        self.p2m = sps.kron(sps.csr_matrix(primary_to_mortar_int), i3).tocsr()
-        self.m2s = sps.kron(sps.csr_matrix(mortar_to_secondary_avg), i3).tocsr()
-        self.s2m = sps.kron(sps.csr_matrix(secondary_to_mortar_int), i3).tocsr()
-        self.sign = sps.diags(np.repeat(np.asarray(mortar_sign, float), 3)).tocsr()
-        self.volumes = np.repeat(np.asarray(mortar_volumes, float), 3)
+        self.mortar_to_secondary = sps.csr_matrix(mortar_to_secondary_avg)
         self.rotation = sps.csr_matrix(local_coordinates)
         self.num_mortar = int(np.asarray(mortar_sign).size)
-        self.num_cells = int(self.rotation.shape[0] // 3)
-        self.mortar_to_secondary = sps.csr_matrix(mortar_to_secondary_avg)
+        self.num_cells = int(self.mortar_to_secondary.shape[0])
+        self.nd = local_dimension(self.rotation, self.num_cells)
+        eye = sps.identity(self.nd, format="csr")
+        self.m2p = sps.kron(sps.csr_matrix(mortar_to_primary_avg), eye).tocsr()
+        self.p2m = sps.kron(sps.csr_matrix(primary_to_mortar_int), eye).tocsr()
+        self.m2s = sps.kron(self.mortar_to_secondary, eye).tocsr()
+        self.s2m = sps.kron(sps.csr_matrix(secondary_to_mortar_int), eye).tocsr()
+        self.sign = sps.diags(np.repeat(np.asarray(mortar_sign, float), self.nd)).tocsr()
+        self.volumes = np.repeat(np.asarray(mortar_volumes, float), self.nd)
+
+
+def matrix_dimension(sd) -> int:
+    """``sd.dim`` of a matrix grid that carries mechanics: 2 or 3, anything else raises ``NotImplementedError``."""
+    nd = int(sd.dim)
+    if nd not in (2, 3):
+        raise NotImplementedError(f"the mechanics equations are stated for a 2-D or 3-D matrix grid, not a {nd}-D one")
+    return nd
+
+
+def local_dimension(local_coordinates, num_cells: int) -> int:
+    """``nd`` of the square ``local_coordinates`` (nd num_cells rows) of a fracture with ``num_cells`` cells; anything
+    but a 2 x 2 or 3 x 3 frame per cell raises ``ValueError``."""
+    rows = int(local_coordinates.shape[0])
+    if num_cells < 1 or rows % num_cells or rows // num_cells not in (2, 3) or int(local_coordinates.shape[1]) != rows:
+        raise ValueError(f"local coordinates of shape {tuple(local_coordinates.shape)} do not hold a 2 x 2 or 3 x 3 "
+                         f"frame per cell of a fracture with {num_cells} cells")
+    return rows // num_cells
 
 
 def mortar_pairs(mortar_to_secondary) -> np.ndarray:
@@ -84,58 +105,65 @@ def block_groups(blocks):
                        np.concatenate([c.ravel() for _, c in blocks]))
 
 
-def contact_operators(rotation, mortar_to_secondary, sign, secondary_to_mortar, volumes, characteristic_traction: float):
-    """Device operators of the contact laws of one fracture with n cells: ``sel_n`` / ``sel_t`` (normal / tangential
-    components of a local 3-vector per cell), ``s2t`` (one value per cell to its two tangential components), ``jump``
-    (u_j -> local displacement jump) and ``traction`` (contact traction -> force on the mortar cells).  ``rotation``:
-    ``local_coordinates``; ``mortar_to_secondary``, ``sign``, ``secondary_to_mortar``: the 3-component projections and
-    side signs; ``volumes``: mortar volumes, 3 per mortar cell."""
+def contact_operators(rotation, mortar_to_secondary, sign, secondary_to_mortar, volumes, characteristic_traction: float,
+                      nd: int = 3):
+    """Device operators of the contact laws of one fracture with n cells in an ``nd``-D matrix: ``sel_n`` / ``sel_t``
+    (normal / tangential components of a local nd-vector per cell: the last one / the nd - 1 first ones), ``s2t`` (one
+    value per cell to its nd - 1 tangential components), ``jump`` (u_j -> local displacement jump) and ``traction``
+    (contact traction -> force on the mortar cells), and ``nd`` itself.  ``rotation``: ``local_coordinates``;
+    ``mortar_to_secondary``, ``sign``, ``secondary_to_mortar``: the nd-component projections and side signs;
+    ``volumes``: mortar volumes, nd per mortar cell."""
     csr = ad.as_device_csr
-    n = rotation.shape[0] // 3
-    sel_n = sps.csr_matrix((np.ones(n), (np.arange(n), 3 * np.arange(n) + 2)), shape=(n, 3 * n))
-    sel_t = sps.csr_matrix((np.ones(2 * n), (np.arange(2 * n), 3 * np.repeat(np.arange(n), 2)
-                                             + np.tile([0, 1], n))), shape=(2 * n, 3 * n))
-    s2t = sps.csr_matrix((np.ones(2 * n), (np.arange(2 * n), np.repeat(np.arange(n), 2))), shape=(2 * n, n))
+    nt = nd - 1
+    n = rotation.shape[0] // nd
+    sel_n = sps.csr_matrix((np.ones(n), (np.arange(n), nd * np.arange(n) + nt)), shape=(n, nd * n))
+    sel_t = sps.csr_matrix((np.ones(nt * n), (np.arange(nt * n), nd * np.repeat(np.arange(n), nt)
+                                              + np.tile(np.arange(nt), n))), shape=(nt * n, nd * n))
+    s2t = sps.csr_matrix((np.ones(nt * n), (np.arange(nt * n), np.repeat(np.arange(n), nt))), shape=(nt * n, n))
     jump = rotation @ mortar_to_secondary @ sign
     traction = sps.diags(volumes * characteristic_traction) @ sign @ secondary_to_mortar @ rotation.T
-    return dict(sel_n=csr(sel_n), sel_t=csr(sel_t), s2t=csr(s2t), jump=csr(jump), traction=csr(traction))
+    return dict(sel_n=csr(sel_n), sel_t=csr(sel_t), s2t=csr(s2t), jump=csr(jump), traction=csr(traction), nd=nd)
 
 
 def contact_laws(q, t, u_j, u_j_prev, c):
     """(normal, tangential) complementarity laws of one fracture: ``q`` holds the ``contact_operators``, ``t`` and
     ``u_j`` are the contact traction and the mortar displacement of the iterate, ``u_j_prev`` that of the previous time
-    step, ``c`` the contact constants."""
+    step, ``c`` the contact constants.  Tangential norms are over the ``q.nd - 1`` tangential components, as in
+    models/contact_mechanics.py:177-201 (for a line fracture: the absolute value)."""
+    nt = q.nd - 1
     jump, jump_n = q.jump @ u_j, q.jump @ u_j_prev
     t_n, u_n = q.sel_n @ t, q.sel_n @ jump
     t_t, u_t, u_t_prev = q.sel_t @ t, q.sel_t @ jump, q.sel_t @ jump_n
-    gap = fn.l2_norm(2, u_t) * float(np.tan(c.dilation_angle)) + c.reference_gap
+    gap = fn.l2_norm(nt, u_t) * float(np.tan(c.dilation_angle)) + c.reference_gap
     normal = t_n + fn.maximum(-t_n - (u_n - gap) * c.numerical_constant, 0.0)
     s = t_t + (u_t - u_t_prev) * c.numerical_constant
     b_p = fn.maximum(t_n * (-c.friction_coefficient), 0.0)
     chi = q.s2t @ fn.characteristic_function(c.open_state_tolerance, b_p).val
-    tangential = ((q.s2t @ b_p) * s - (q.s2t @ fn.maximum(b_p, fn.l2_norm(2, s))) * t_t) * (1.0 - chi) + t_t * chi
+    tangential = ((q.s2t @ b_p) * s - (q.s2t @ fn.maximum(b_p, fn.l2_norm(nt, s))) * t_t) * (1.0 - chi) + t_t * chi
     return normal, tangential
 
 
 class FracturedMomentumBalance:
-    """``sd``: the 3-D matrix grid (faces split along the fractures, ``fracture_faces`` tag), ``data``:
+    """``sd``: the 2-D or 3-D matrix grid (faces split along the fractures, ``fracture_faces`` tag), ``data``:
     ``parameters[keyword]`` with ``fourth_order_tensor`` and the vectorial ``bc`` (fracture faces Dirichlet,
-    ``internal_to_dirichlet``); ``bc_values``: 3 nf face-major (displacement / traction); ``fractures``: list of
-    ``FractureContact``; ``constants``: ``numerical_constant, characteristic_traction, friction_coefficient,
-    dilation_angle, reference_gap, open_state_tolerance``."""
+    ``internal_to_dirichlet``); ``bc_values``: nd nf face-major (displacement / traction); ``fractures``: list of
+    ``FractureContact`` (dimension nd - 1); ``constants``: ``numerical_constant, characteristic_traction,
+    friction_coefficient, dilation_angle, reference_gap, open_state_tolerance``."""
 
     def __init__(self, sd, data: dict, bc_values, fractures, constants: dict, body_force=None, keyword: str = "mechanics"):
-        if int(sd.dim) != 3:
-            raise NotImplementedError("a 3-D matrix grid is expected")
+        self.nd = nd = matrix_dimension(sd)
         self.sd, self.data, self.kw = sd, data, keyword
         self.bc_values = np.asarray(bc_values, float)
         self.fractures = list(fractures)
+        for f in self.fractures:
+            if f.nd != nd:
+                raise ValueError(f"a fracture with {f.nd}-D local coordinates in a {nd}-D matrix")
         self.k = SimpleNamespace(**{k: float(v) for k, v in constants.items()})
         self.nc, self.nf = int(sd.num_cells), int(sd.num_faces)
-        self.body_force = np.zeros(3 * self.nc) if body_force is None else np.asarray(body_force, float)
-        nt = [3 * f.num_cells for f in self.fractures]
-        nj = [3 * f.num_mortar for f in self.fractures]
-        self.sizes = [3 * self.nc] + nt + nj
+        self.body_force = np.zeros(nd * self.nc) if body_force is None else np.asarray(body_force, float)
+        nt = [nd * f.num_cells for f in self.fractures]
+        nj = [nd * f.num_mortar for f in self.fractures]
+        self.sizes = [nd * self.nc] + nt + nj
         self.offsets = np.concatenate(([0], np.cumsum(self.sizes))).astype(np.int64)
         self._const = None
 
@@ -155,13 +183,13 @@ class FracturedMomentumBalance:
             frac = np.asarray(self.sd.tags["fracture_faces"], bool)
             out = np.where(frac, np.asarray(cf.sum(axis=1)).ravel(), 0.0)      # +-1 on fracture faces: outward normal
             k = SimpleNamespace(
-                div3=csr(sps.kron(sps.csr_matrix(self.sd.cell_faces.T), sps.identity(3)).tocsr()),
+                div_nd=csr(sps.kron(sps.csr_matrix(self.sd.cell_faces.T), sps.identity(self.nd)).tocsr()),
                 stress=csr(M["stress"]), bound=csr(M["bound_stress"]),
-                outward=dev(np.repeat(out, 3)), f=dev(self.body_force), fr=[])
+                outward=dev(np.repeat(out, self.nd)), f=dev(self.body_force), fr=[])
             k.stress_b = k.bound @ dev(self.bc_values)
             for fc in self.fractures:
                 k.fr.append(SimpleNamespace(m2p=csr(fc.m2p), p2m=csr(fc.p2m), **contact_operators(
-                    fc.rotation, fc.m2s, fc.sign, fc.s2m, fc.volumes, self.k.characteristic_traction)))
+                    fc.rotation, fc.m2s, fc.sign, fc.s2m, fc.volumes, self.k.characteristic_traction, self.nd)))
             self._const = k
         return self._const
 
@@ -179,7 +207,7 @@ class FracturedMomentumBalance:
         stress = (k.stress @ u) + k.stress_b
         if boundary is not None:
             stress = stress + (k.bound @ boundary)
-        momentum = -(k.div3 @ stress) - k.f
+        momentum = -(k.div_nd @ stress) - k.f
         force, normal, tangential = [], [], []
         for j in range(nfr):
             q = k.fr[j]
@@ -191,20 +219,20 @@ class FracturedMomentumBalance:
 
     def preconditioner_groups(self):
         """Groups of the grouped block-Jacobi preconditioner of ``krylov.gmres`` in this problem's ordering: per matrix
-        cell c, momentum_c <-> u_c (3); per fracture cell k with mortar cells m1, m2, the normal and tangential laws of k
-        and the force balances of m1, m2 <-> t_k, u_j of m1, m2 (9)."""
-        nfr, nc = len(self.fractures), self.nc
-        eq = np.concatenate(([0], np.cumsum([3 * nc] + [3 * f.num_mortar for f in self.fractures]
+        cell c, momentum_c <-> u_c (nd); per fracture cell k with mortar cells m1, m2, the normal and tangential laws of k
+        and the force balances of m1, m2 <-> t_k, u_j of m1, m2 (3 nd: 9 in 3-D, 6 in 2-D)."""
+        nfr, nc, nd = len(self.fractures), self.nc, self.nd
+        eq = np.concatenate(([0], np.cumsum([nd * nc] + [nd * f.num_mortar for f in self.fractures]
                                             + [f.num_cells for f in self.fractures]
-                                            + [2 * f.num_cells for f in self.fractures])))
+                                            + [(nd - 1) * f.num_cells for f in self.fractures])))
         cells = np.arange(nc)
-        blocks = [(span(eq[0], cells, 3), span(self.offsets[0], cells, 3))]
+        blocks = [(span(eq[0], cells, nd), span(self.offsets[0], cells, nd))]
         for j, fc in enumerate(self.fractures):
             pair, k = mortar_pairs(fc.mortar_to_secondary), np.arange(fc.num_cells)
             frc, jmp = eq[1 + j], self.offsets[1 + nfr + j]
-            rows = [span(eq[1 + nfr + j], k, 1), span(eq[1 + 2 * nfr + j], k, 2), span(frc, pair[:, 0], 3),
-                    span(frc, pair[:, 1], 3)]
-            cols = [span(self.offsets[1 + j], k, 3), span(jmp, pair[:, 0], 3), span(jmp, pair[:, 1], 3)]
+            rows = [span(eq[1 + nfr + j], k, 1), span(eq[1 + 2 * nfr + j], k, nd - 1), span(frc, pair[:, 0], nd),
+                    span(frc, pair[:, 1], nd)]
+            cols = [span(self.offsets[1 + j], k, nd), span(jmp, pair[:, 0], nd), span(jmp, pair[:, 1], nd)]
             blocks.append((np.hstack(rows), np.hstack(cols)))
         return block_groups(blocks)
 

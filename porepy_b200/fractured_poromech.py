@@ -1,8 +1,9 @@
 """Poromechanics of a fractured medium with frictional contact -- the reference's ``pp.Poromechanics`` on a matrix cut by
-fractures, BASELINE configs[3] + [4] in one model: Biot poromechanics in the 3-D matrix (``porepy_b200.Mpfa`` + ``Biot``),
-compressible flow in the 2-D fractures whose aperture follows the displacement jump, the interface Darcy law with that
-aperture, the fluid pressure acting on the fracture walls, and the semismooth contact laws -- every term and its Jacobian
-by ``DeviceAdArray`` on device-resident matrices.
+fractures, BASELINE configs[3] + [4] in one model: Biot poromechanics in the 2-D or 3-D matrix (``nd = sd.dim``;
+``porepy_b200.Mpfa`` + ``Biot``), compressible flow in the fractures of dimension nd - 1 (planes in 3-D; lines in 2-D,
+whose fluxes run through the TPFA delegation of ``Mpfa``) with an aperture that follows the displacement jump, the
+interface Darcy law with that aperture, the fluid pressure acting on the fracture walls, and the semismooth contact laws --
+every term and its Jacobian by ``DeviceAdArray`` on device-resident matrices.
 
 Couplings on top of ``porepy_b200.poromech`` (matrix), ``mdflow_nl`` (fracture flow, interface law) and ``contact``
 (interface force balance, complementarity laws):
@@ -21,7 +22,7 @@ upwinding.  Unknowns: [p matrix | p fractures | u | contact tractions | lambda |
 [mass matrix | mass fractures | momentum | Darcy laws | force balances | normal laws | tangential laws] (the fixtures carry
 the maps to the reference's numbering).  One matrix subdomain, fractures without intersections; saddle-point Jacobian: the
 linear solver of ``time_step`` is the caller's; ``krylov.gmres_solver(prob.preconditioner_groups())`` is the device one.  ``tests/golden/contact_poromech*.npz`` pin Jacobian, residual, the residual
-history of the semismooth Newton loop and the converged state.
+history of the semismooth Newton loop and the converged state, ``contact_poromech_2d.npz`` the same on a line fracture.
 """
 from __future__ import annotations
 
@@ -32,7 +33,7 @@ import scipy.sparse as sps
 
 from . import ad, ad_functions as fn
 from .advection import advective_flux, rediscretize_upwind, rediscretize_upwind_coupling
-from .contact import block_groups, contact_laws, contact_operators, mortar_pairs, span
+from .contact import block_groups, contact_laws, contact_operators, local_dimension, matrix_dimension, mortar_pairs, span
 from .fv import Biot, Mpfa
 from .newton import newton_loop
 from .params import DISCRETIZATION_MATRICES, PARAMETERS
@@ -42,8 +43,9 @@ class FractureCoupling:
     """One fracture: its grid and data dictionary (``parameters[flow_keyword]``: ``bc``, ``ambient_dimension``; the
     ``second_order_tensor`` entry is written at every linearization: ``intrinsic_permeability`` (3, 3, nfc) times the
     aperture), the eight scalar mortar projections of its two-sided interface (``*_int`` / ``*_avg`` of the
-    reference's ``MortarGrid``), ``mortar_sign``, ``mortar_volumes``, ``local_coordinates`` (3 nfc x 3 nfc) and the normal
-    permeability per mortar cell; ``bc``: boundary data of a fracture that reaches the domain boundary."""
+    reference's ``MortarGrid``), ``mortar_sign``, ``mortar_volumes``, ``local_coordinates`` (nd nfc x nd nfc: nd - 1
+    tangents, then the normal, per cell) and the normal permeability per mortar cell; ``bc``: boundary data of a fracture
+    that reaches the domain boundary."""
 
     def __init__(self, sd, data, projections: dict, mortar_sign, mortar_volumes, local_coordinates, normal_permeability,
                  intrinsic_permeability, bc: dict | None = None):
@@ -58,12 +60,13 @@ class FractureCoupling:
         self.rotation = sps.csr_matrix(local_coordinates)
         self.kappa = np.asarray(normal_permeability, float)
         self.num_cells, self.num_mortar = int(sd.num_cells), int(self.sign.size)
+        self.nd = local_dimension(self.rotation, self.num_cells)
 
 
 class FracturedPoromechanics:
-    """``sd`` / ``data``: the matrix grid (fracture faces split) with ``parameters[flow_keyword]`` and
+    """``sd`` / ``data``: the 2-D or 3-D matrix grid (fracture faces split) with ``parameters[flow_keyword]`` and
     ``parameters[mechanics_keyword]`` (``scalar_vector_mappings`` = {flow_keyword: Biot coefficient}).  ``bc``: dict of face
-    arrays ``flow``, ``mechanics`` (3 nf), ``fluid_flux`` and the object ``fluid_flux_type``.  ``fluid``: ``compressibility,
+    arrays ``flow``, ``mechanics`` (nd nf), ``fluid_flux`` and the object ``fluid_flux_type``.  ``fluid``: ``compressibility,
     density, viscosity, reference_pressure``; ``solid``: ``reference_porosity, n_inv, residual_aperture``; ``contact``: the
     constants of ``porepy_b200.contact``."""
 
@@ -71,10 +74,12 @@ class FracturedPoromechanics:
 
     def __init__(self, sd, data: dict, fractures, fluid: dict, solid: dict, contact: dict, bc: dict,
                  flow_keyword: str = "flow", mechanics_keyword: str = "mechanics"):
-        if int(sd.dim) != 3:
-            raise NotImplementedError("a 3-D matrix grid is expected")
+        self.nd = nd = matrix_dimension(sd)
         self.sd, self.data = sd, data
         self.fractures = list(fractures)
+        for f in self.fractures:
+            if f.nd != nd or int(f.sd.dim) != nd - 1:
+                raise ValueError(f"a {int(f.sd.dim)}-D fracture with {f.nd}-D local coordinates in a {nd}-D matrix")
         self.fk, self.mk = flow_keyword, mechanics_keyword
         self.fl = SimpleNamespace(**{k: float(v) for k, v in fluid.items()})
         self.so = SimpleNamespace(**{k: float(v) for k, v in solid.items()})
@@ -83,7 +88,7 @@ class FracturedPoromechanics:
         self.nc, self.nf = int(sd.num_cells), int(sd.num_faces)
         nfc = [f.num_cells for f in self.fractures]
         nm = [f.num_mortar for f in self.fractures]
-        self.sizes = [self.nc] + nfc + [3 * self.nc] + [3 * n for n in nfc] + nm + [3 * n for n in nm]
+        self.sizes = [self.nc] + nfc + [nd * self.nc] + [nd * n for n in nfc] + nm + [nd * n for n in nm]
         self.offsets = np.concatenate(([0], np.cumsum(self.sizes))).astype(np.int64)
         self._intf_data = [{} for _ in self.fractures]
         self._const = None
@@ -110,7 +115,8 @@ class FracturedPoromechanics:
     def _operands(self):
         if self._const is None:
             csr, dev = ad.as_device_csr, ad.device_vector
-            i3 = sps.identity(3, format="csr")
+            nd = self.nd
+            eye = sps.identity(nd, format="csr")
             F = self.data[DISCRETIZATION_MATRICES][self.fk]
             M = self.data[DISCRETIZATION_MATRICES][self.mk]
             cf = sps.csr_matrix(self.sd.cell_faces)
@@ -118,32 +124,32 @@ class FracturedPoromechanics:
             out = np.where(frac_faces, np.asarray(cf.sum(axis=1)).ravel(), 0.0)
             vol = np.asarray(self.sd.cell_volumes, float)
             k = SimpleNamespace(
-                div=csr(sps.csr_matrix(self.sd.cell_faces.T)), div3=csr(sps.kron(sps.csr_matrix(self.sd.cell_faces.T), i3).tocsr()),
+                div=csr(sps.csr_matrix(self.sd.cell_faces.T)), div_nd=csr(sps.kron(sps.csr_matrix(self.sd.cell_faces.T), eye).tocsr()),
                 trace=csr(abs(cf)), vol=dev(vol), inv_vol=dev(1.0 / vol),
                 F={key: csr(F[key]) for key in ("flux", "bound_flux", "bound_pressure_cell", "bound_pressure_face")},
                 stress=csr(M["stress"]), bound=csr(M["bound_stress"]), grad_p=csr(M["scalar_gradient"][self.fk]),
                 div_u=csr(M["displacement_divergence"][self.fk]), div_u_b=csr(M["boundary_displacement_divergence"][self.fk]),
-                cons=csr(M["mpsa_consistency"][self.fk]), outward=dev(np.repeat(out, 3)),
+                cons=csr(M["mpsa_consistency"][self.fk]), outward=dev(np.repeat(out, nd)),
                 bcq=dev(self.bc["flow"]), ubc=dev(self.bc["mechanics"]), bcw=dev(self.bc["fluid_flux"]), fr=[])
             for fc in self.fractures:
                 p = fc.p
                 # unit normal of the primary face of every mortar cell, pointing out of the matrix, times the mortar volume
                 pf = p["primary_to_mortar_avg"].tocsr().indices
-                n_out = np.asarray(self.sd.face_normals)[:, pf] / np.asarray(self.sd.face_areas)[pf] * out[pf]
-                rows = np.arange(3 * fc.num_mortar)
-                pressure_load = sps.csr_matrix(((n_out * fc.volumes).ravel("F"), (rows, np.repeat(np.arange(fc.num_mortar), 3))),
-                                               shape=(3 * fc.num_mortar, fc.num_mortar)) @ p["secondary_to_mortar_avg"]
+                n_out = np.asarray(self.sd.face_normals)[:nd, pf] / np.asarray(self.sd.face_areas)[pf] * out[pf]
+                rows = np.arange(nd * fc.num_mortar)
+                pressure_load = sps.csr_matrix(((n_out * fc.volumes).ravel("F"), (rows, np.repeat(np.arange(fc.num_mortar), nd))),
+                                               shape=(nd * fc.num_mortar, fc.num_mortar)) @ p["secondary_to_mortar_avg"]
                 k.fr.append(SimpleNamespace(
                     m2p=csr(p["mortar_to_primary_int"]), p2m=csr(p["primary_to_mortar_avg"]),
                     m2s=csr(p["mortar_to_secondary_int"]), s2m=csr(p["secondary_to_mortar_avg"]),
-                    m2p3=csr(sps.kron(p["mortar_to_primary_avg"], i3).tocsr()),
-                    p2m3=csr(sps.kron(p["primary_to_mortar_int"], i3).tocsr()),
+                    m2p_nd=csr(sps.kron(p["mortar_to_primary_avg"], eye).tocsr()),
+                    p2m_nd=csr(sps.kron(p["primary_to_mortar_int"], eye).tocsr()),
                     pressure_load=csr(pressure_load), coef=dev(fc.volumes * fc.kappa * 2.0),
                     div=csr(sps.csr_matrix(fc.sd.cell_faces.T)), vol=dev(np.asarray(fc.sd.cell_volumes, float)),
                     bc=None if fc.bc is None else {key: dev(v) for key, v in fc.bc.items() if not key.endswith("_type")},
-                    **contact_operators(fc.rotation, sps.kron(p["mortar_to_secondary_avg"], i3),
-                                        sps.diags(np.repeat(fc.sign, 3)), sps.kron(p["secondary_to_mortar_int"], i3),
-                                        np.repeat(fc.volumes, 3), self.ct.characteristic_traction)))
+                    **contact_operators(fc.rotation, sps.kron(p["mortar_to_secondary_avg"], eye),
+                                        sps.diags(np.repeat(fc.sign, nd)), sps.kron(p["secondary_to_mortar_int"], eye),
+                                        np.repeat(fc.volumes, nd), self.ct.characteristic_traction, nd)))
             self._const = k
         return self._const
 
@@ -154,7 +160,7 @@ class FracturedPoromechanics:
         dp = p - self.fl.reference_pressure
         b = k.ubc
         for j in range(len(self.fractures)):
-            b = (k.fr[j].m2p3 @ uj[j]) + b
+            b = (k.fr[j].m2p_nd @ uj[j]) + b
         return ((k.div_u @ u) + (k.div_u_b @ b) + (k.cons @ dp)) * k.inv_vol + dp * self.so.n_inv + self.so.reference_porosity
 
     def _fracture_flux(self, fc, q, p, keyword=None, bc_key="flow"):
@@ -230,7 +236,7 @@ class FracturedPoromechanics:
             ifl.append(lam[j] * ((csr(U["upwind_primary"]) @ (q.p2m @ (k.trace @ w3)))
                                  + (csr(U["upwind_secondary"]) @ (q.s2m @ wf[j]))))
             b_flow = (q.m2p @ lam[j]) + b_flow
-            b_mech = (q.m2p3 @ uj[j]) + b_mech
+            b_mech = (q.m2p_nd @ uj[j]) + b_mech
         # ---- matrix: mass and momentum balance
         Tm = self.data[DISCRETIZATION_MATRICES][mk]
         q3 = (k.F["flux"] @ p3) + (k.F["bound_flux"] @ b_flow)
@@ -241,7 +247,7 @@ class FracturedPoromechanics:
         mass3 = (self._density(p3) * self._porosity(p3, u, uj, k) - self._density(p3n) * self._porosity(p3n, un, ujn, k)) \
             * (k.vol * (1.0 / dt)) + (k.div @ ff3)
         stress = (k.stress @ u) + (k.bound @ b_mech) + (k.grad_p @ (p3 - fl.reference_pressure))
-        momentum = -(k.div3 @ stress)
+        momentum = -(k.div_nd @ stress)
         trace_p = (k.F["bound_pressure_cell"] @ p3) + (k.F["bound_pressure_face"] @ b_flow)
         mass_f, darcy, force, normal, tangential = [], [], [], [], []
         for j, fc in enumerate(self.fractures):
@@ -255,34 +261,34 @@ class FracturedPoromechanics:
                           + (q.div @ advective_flux(Tf, qf, wf[j], bw, bw)) - (q.m2s @ ifl[j]))
             # ---- interface: Darcy law with the current aperture; force balance with the fluid pressure on the walls
             darcy.append(lam[j] - ((q.p2m @ trace_p) - (q.s2m @ pf[j])) * (q.s2m @ a.reciprocal()) * q.coef)
-            force.append((q.p2m3 @ (stress * k.outward)) + (q.traction @ t[j]) + (q.pressure_load @ pf[j]))
+            force.append((q.p2m_nd @ (stress * k.outward)) + (q.traction @ t[j]) + (q.pressure_load @ pf[j]))
             nrm, tan = contact_laws(q, t[j], uj[j], ujn[j], ct)
             normal.append(nrm)
             tangential.append(tan)
         return [mass3] + mass_f + [momentum] + darcy + force + normal + tangential
 
     def _equation_offsets(self) -> np.ndarray:
-        nc, nfc, nm = self.nc, [f.num_cells for f in self.fractures], [f.num_mortar for f in self.fractures]
-        sizes = [nc] + nfc + [3 * nc] + nm + [3 * n for n in nm] + nfc + [2 * n for n in nfc]
+        nc, nfc, nm, nd = self.nc, [f.num_cells for f in self.fractures], [f.num_mortar for f in self.fractures], self.nd
+        sizes = [nc] + nfc + [nd * nc] + nm + [nd * n for n in nm] + nfc + [(nd - 1) * n for n in nfc]
         return np.concatenate(([0], np.cumsum(sizes))).astype(np.int64)
 
     def preconditioner_groups(self):
         """Groups of the grouped block-Jacobi preconditioner of ``krylov.gmres`` in this problem's ordering: per matrix
-        cell c, mass_c and momentum_c <-> p_c, u_c (4); per fracture cell k with mortar cells m1, m2, the contact laws of
-        k, the force balances of m1, m2, the fracture mass balance of k and the Darcy laws of m1, m2 <-> t_k, u_j of
-        m1, m2, p_f of k, lambda of m1, m2 (12)."""
-        nfr, eq, var = len(self.fractures), self._equation_offsets(), self.offsets
+        cell c, mass_c and momentum_c <-> p_c, u_c (nd + 1); per fracture cell k with mortar cells m1, m2, the contact
+        laws of k, the force balances of m1, m2, the fracture mass balance of k and the Darcy laws of m1, m2 <-> t_k, u_j
+        of m1, m2, p_f of k, lambda of m1, m2 (3 nd + 3: 12 in 3-D, 9 in 2-D)."""
+        nfr, eq, var, nd = len(self.fractures), self._equation_offsets(), self.offsets, self.nd
         cells = np.arange(self.nc)
-        blocks = [(np.hstack([span(eq[0], cells, 1), span(eq[1 + nfr], cells, 3)]),
-                   np.hstack([span(var[0], cells, 1), span(var[1 + nfr], cells, 3)]))]
+        blocks = [(np.hstack([span(eq[0], cells, 1), span(eq[1 + nfr], cells, nd)]),
+                   np.hstack([span(var[0], cells, 1), span(var[1 + nfr], cells, nd)]))]
         for j, fc in enumerate(self.fractures):
             pair, k = mortar_pairs(fc.p["mortar_to_secondary_avg"]), np.arange(fc.num_cells)
             m1, m2 = pair[:, 0], pair[:, 1]
             frc, darcy = eq[2 + 2 * nfr + j], eq[2 + nfr + j]
-            rows = [span(eq[2 + 3 * nfr + j], k, 1), span(eq[2 + 4 * nfr + j], k, 2), span(frc, m1, 3), span(frc, m2, 3),
+            rows = [span(eq[2 + 3 * nfr + j], k, 1), span(eq[2 + 4 * nfr + j], k, nd - 1), span(frc, m1, nd), span(frc, m2, nd),
                     span(eq[1 + j], k, 1), span(darcy, m1, 1), span(darcy, m2, 1)]
             jmp, lam = var[2 + 3 * nfr + j], var[2 + 2 * nfr + j]
-            cols = [span(var[2 + nfr + j], k, 3), span(jmp, m1, 3), span(jmp, m2, 3), span(var[1 + j], k, 1),
+            cols = [span(var[2 + nfr + j], k, nd), span(jmp, m1, nd), span(jmp, m2, nd), span(var[1 + j], k, 1),
                     span(lam, m1, 1), span(lam, m2, 1)]
             blocks.append((np.hstack(rows), np.hstack(cols)))
         return block_groups(blocks)

@@ -17,7 +17,8 @@ Unknowns: [p matrix | p fractures | T matrix | T fractures | u | contact tractio
 [mass matrix | mass fractures | energy matrix | energy fractures | momentum | Darcy laws | Fourier laws | enthalpy laws |
 force balances | normal laws | tangential laws].  ``tests/golden/contact_thm*.npz`` pin the Jacobian at the zero state and at
 the fourth Newton iterate, the residual history of the semismooth Newton loop and the converged state.  The Newton updates
-are solved on the device by ``krylov.gmres_solver(prob.preconditioner_groups())`` (17 unknowns per fracture-cell group).
+are solved on the device by ``krylov.gmres_solver(prob.preconditioner_groups())`` (3 nd + 8 unknowns per fracture-cell
+group: 17 in 3-D, 14 in 2-D).  A 2-D matrix with line fractures is handled as the 3-D one (``contact_thm_2d.npz``).
 """
 from __future__ import annotations
 
@@ -49,17 +50,19 @@ class FracturedThermoporomechanics(FracturedPoromechanics):
         self.kappa_t = [np.asarray(v, float) for v in normal_thermal_conductivity]
         nfc = [f.num_cells for f in self.fractures]
         nm = [f.num_mortar for f in self.fractures]
-        self.sizes = [self.nc] + nfc + [self.nc] + nfc + [3 * self.nc] + [3 * n for n in nfc] + nm + nm + nm + [3 * n for n in nm]
+        nd = self.nd
+        self.sizes = [self.nc] + nfc + [self.nc] + nfc + [nd * self.nc] + [nd * n for n in nfc] + nm + nm + nm + [nd * n for n in nm]
         self.offsets = np.concatenate(([0], np.cumsum(self.sizes))).astype(np.int64)
 
     def preconditioner_groups(self):
         """Groups of the grouped block-Jacobi preconditioner of ``krylov.gmres`` in this problem's ordering: per matrix
-        cell c, mass_c, energy_c and momentum_c <-> p_c, T_c, u_c (5); per fracture cell k with mortar cells m1, m2, the
-        twelve rows and columns of ``FracturedPoromechanics.preconditioner_groups`` plus the fracture energy balance of k
-        and the Fourier and enthalpy laws of m1, m2 <-> T_f of k, eta and eps of m1, m2 (17)."""
-        n, var = len(self.fractures), self.offsets
+        cell c, mass_c, energy_c and momentum_c <-> p_c, T_c, u_c (nd + 2); per fracture cell k with mortar cells m1, m2,
+        the 3 nd + 3 rows and columns of ``FracturedPoromechanics.preconditioner_groups`` plus the fracture energy balance
+        of k and the Fourier and enthalpy laws of m1, m2 <-> T_f of k, eta and eps of m1, m2 (3 nd + 8: 17 in 3-D, 14 in
+        2-D)."""
+        n, var, nd = len(self.fractures), self.offsets, self.nd
         nc, nfc, nm = self.nc, [f.num_cells for f in self.fractures], [f.num_mortar for f in self.fractures]
-        sizes = [nc] + nfc + [nc] + nfc + [3 * nc] + nm + nm + nm + [3 * m for m in nm] + nfc + [2 * f for f in nfc]
+        sizes = [nc] + nfc + [nc] + nfc + [nd * nc] + nm + nm + nm + [nd * m for m in nm] + nfc + [(nd - 1) * f for f in nfc]
         eq = np.concatenate(([0], np.cumsum(sizes))).astype(np.int64)
         # equation groups: mass | mass_f | energy | energy_f | momentum | darcy | fourier | enthalpy | force | normal |
         # tangential; variable groups: p | p_f | T | T_f | u | t | lambda | eta | eps | u_j
@@ -68,16 +71,16 @@ class FracturedThermoporomechanics(FracturedPoromechanics):
         v_p, v_pf, v_t, v_tf, v_u = 0, 1, 1 + n, 2 + n, 2 + 2 * n
         v_trac, v_lam, v_eta, v_eps, v_jmp = (3 + 2 * n + q * n for q in range(5))
         cells = np.arange(nc)
-        blocks = [(np.hstack([span(eq[e_mass], cells, 1), span(eq[e_en], cells, 1), span(eq[e_mom], cells, 3)]),
-                   np.hstack([span(var[v_p], cells, 1), span(var[v_t], cells, 1), span(var[v_u], cells, 3)]))]
+        blocks = [(np.hstack([span(eq[e_mass], cells, 1), span(eq[e_en], cells, 1), span(eq[e_mom], cells, nd)]),
+                   np.hstack([span(var[v_p], cells, 1), span(var[v_t], cells, 1), span(var[v_u], cells, nd)]))]
         for j, fc in enumerate(self.fractures):
             pair, k = mortar_pairs(fc.p["mortar_to_secondary_avg"]), np.arange(fc.num_cells)
             m1, m2 = pair[:, 0], pair[:, 1]
             pair_rows = lambda off, w: [span(off, m1, w), span(off, m2, w)]  # noqa: E731
-            rows = [span(eq[e_nrm + j], k, 1), span(eq[e_tan + j], k, 2), *pair_rows(eq[e_force + j], 3),
+            rows = [span(eq[e_nrm + j], k, 1), span(eq[e_tan + j], k, nd - 1), *pair_rows(eq[e_force + j], nd),
                     span(eq[e_massf + j], k, 1), *pair_rows(eq[e_darcy + j], 1),
                     span(eq[e_enf + j], k, 1), *pair_rows(eq[e_four + j], 1), *pair_rows(eq[e_enth + j], 1)]
-            cols = [span(var[v_trac + j], k, 3), *pair_rows(var[v_jmp + j], 3),
+            cols = [span(var[v_trac + j], k, nd), *pair_rows(var[v_jmp + j], nd),
                     span(var[v_pf + j], k, 1), *pair_rows(var[v_lam + j], 1),
                     span(var[v_tf + j], k, 1), *pair_rows(var[v_eta + j], 1), *pair_rows(var[v_eps + j], 1)]
             blocks.append((np.hstack(rows), np.hstack(cols)))
@@ -92,7 +95,7 @@ class FracturedThermoporomechanics(FracturedPoromechanics):
         super()._discretize_fracture(fc, aperture)
         fc.data.setdefault(PARAMETERS, {}).setdefault(self.tk, {})["second_order_tensor"] = SecondOrderTensor(
             self.fl.conductivity * np.asarray(aperture, float))          # porosity 1 in the fracture, specific volume a
-        fc.data[PARAMETERS][self.tk].setdefault("ambient_dimension", 3)
+        fc.data[PARAMETERS][self.tk].setdefault("ambient_dimension", self.nd)
         Mpfa(self.tk).discretize(fc.sd, fc.data)
 
     def discretize(self) -> None:
@@ -172,7 +175,7 @@ class FracturedThermoporomechanics(FracturedPoromechanics):
             enthalpy.append(eps[j] - lam[j] * upwinded(we3, wef[j]))
             b_flow = (q.m2p @ lam[j]) + b_flow
             b_heat = (q.m2p @ eta[j]) + b_heat
-            b_mech = (q.m2p3 @ uj[j]) + b_mech
+            b_mech = (q.m2p_nd @ uj[j]) + b_mech
         # ---- matrix
         Tm, Te = self.data[DISCRETIZATION_MATRICES][mk], self.data[DISCRETIZATION_MATRICES][ek]
         q3 = (k.F["flux"] @ p3) + (k.F["bound_flux"] @ b_flow)
@@ -192,7 +195,7 @@ class FracturedThermoporomechanics(FracturedPoromechanics):
             return (rho * dtm * fl.heat_capacity - p) * por + (dtm * (so.density * so.heat_capacity)) * (-por + 1.0)
         energy3 = (energy(p3, t3, rho3, phi) - energy(p3n, t3n, rho3n, phi_n)) * (k.vol * (1.0 / dt)) + (k.div @ (fe3 + fo3))
         stress = (k.stress @ u) + (k.bound @ b_mech) + (k.grad_p @ (p3 - fl.reference_pressure)) + (k.grad_t @ (t3 - t0))
-        momentum = -(k.div3 @ stress)
+        momentum = -(k.div_nd @ stress)
         trace_p = (k.F["bound_pressure_cell"] @ p3) + (k.F["bound_pressure_face"] @ b_flow)
         trace_t = (k.Fo["bound_pressure_cell"] @ t3) + (k.Fo["bound_pressure_face"] @ b_heat)
         mass_f, energy_f, darcy, fourier, force, normal, tangential = [], [], [], [], [], [], []
@@ -214,7 +217,7 @@ class FracturedThermoporomechanics(FracturedPoromechanics):
             inv_a = q.s2m @ a.reciprocal()
             darcy.append(lam[j] - ((q.p2m @ trace_p) - (q.s2m @ pf[j])) * inv_a * q.coef)
             fourier.append(eta[j] - ((q.p2m @ trace_t) - (q.s2m @ tf[j])) * inv_a * q.coef_t)
-            force.append((q.p2m3 @ (stress * k.outward)) + (q.traction @ t[j]) + (q.pressure_load @ pf[j]))
+            force.append((q.p2m_nd @ (stress * k.outward)) + (q.traction @ t[j]) + (q.pressure_load @ pf[j]))
             nrm, tan = contact_laws(q, t[j], uj[j], ujn[j], self.ct)
             normal.append(nrm)
             tangential.append(tan)

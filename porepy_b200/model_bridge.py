@@ -1,6 +1,7 @@
 """From a prepared PorePy model to the device problems of this package: the glue a PorePy user needs to hand a live
 ``pp.SinglePhaseFlow`` / ``pp.MassAndEnergyBalance`` (on a fracture network) or ``pp.Poromechanics`` /
-``pp.Thermoporomechanics`` (3-D subdomain) over to ``porepy_b200`` -- grids, parameter dictionaries and mortar projections
+``pp.Thermoporomechanics`` (one 2-D or 3-D subdomain, or such a matrix cut by non-intersecting fractures of one dimension
+less) over to ``porepy_b200`` -- grids, parameter dictionaries and mortar projections
 of ``model.mdg`` as they are; boundary data, coefficients and constants evaluated from the model's own methods
 (``bc_values_*``, ``bc_type_*``, ``normal_permeability``, ``aperture``, ``specific_volume``, ``porosity``, the fluid and
 solid constants).  Reached through ``porepy_plugin.plugin(pp)``: ``b200.compressible_flow_from_model(model)`` etc.
@@ -165,11 +166,42 @@ def mass_energy_from_model(model):
 
 
 def _mechanics_boundary(model, sd, data, mk):
+    """Displacement on the Dirichlet faces of the vectorial ``bc``, traction elsewhere: nd nf, face-major."""
     bg = model.mdg.subdomain_to_boundary_grid(sd)
-    proj3 = sps.kron(bg.projection(), sps.identity(3)).tocsr()
+    proj = sps.kron(bg.projection(), sps.identity(int(sd.dim))).tocsr()
     bc = data[PARAMETERS][mk]["bc"]
-    return np.where(np.asarray(bc.is_dir).ravel("F"), proj3.T @ model.bc_values_displacement(bg),
-                    proj3.T @ model.bc_values_stress(bg))
+    return np.where(np.asarray(bc.is_dir).ravel("F"), proj.T @ model.bc_values_displacement(bg),
+                    proj.T @ model.bc_values_stress(bg))
+
+
+def _single_matrix(model):
+    """The one subdomain of a model without fractures; it must be 2-D or 3-D."""
+    sds = list(model.mdg.subdomains())
+    if len(sds) != 1:
+        raise NotImplementedError(f"one subdomain without fractures is expected, the model has {len(sds)} (of dimensions "
+                                  f"{sorted({int(sd.dim) for sd in sds}, reverse=True)})")
+    if sds[0].dim not in (2, 3):
+        raise NotImplementedError(f"the mechanics equations need a 2-D or 3-D subdomain, the model's is {sds[0].dim}-D")
+    return sds[0]
+
+
+def _matrix_and_fractures(model):
+    """(matrix, fractures) of a model with one nd-D matrix (nd = 2 or 3) and fractures of dimension nd - 1 that do not
+    intersect; anything else -- intersection lines or points, a 1-D matrix, several matrices -- raises
+    ``NotImplementedError``."""
+    mdg = model.mdg
+    nd = int(mdg.dim_max())
+    if nd not in (2, 3):
+        raise NotImplementedError(f"a {nd}-D matrix: the contact mechanics equations need a 2-D or 3-D matrix with "
+                                  f"fractures of one dimension less")
+    mats = list(mdg.subdomains(dim=nd))
+    if len(mats) != 1:
+        raise NotImplementedError(f"one {nd}-D matrix subdomain is expected, the model has {len(mats)}")
+    low = sorted({int(sd.dim) for sd in mdg.subdomains() if sd.dim < nd - 1}, reverse=True)
+    if low:
+        raise NotImplementedError(f"{low[0]}-D subdomains (fracture intersections) in a {nd}-D matrix: only {nd - 1}-D "
+                                  f"fractures without intersections are supported")
+    return mats[0], list(mdg.subdomains(dim=nd - 1))
 
 
 def _n_inv(model):
@@ -179,13 +211,10 @@ def _n_inv(model):
 
 
 def poromechanics_from_model(model):
-    """``pp.Poromechanics`` on a 3-D subdomain without fractures -> ``Poromechanics`` (unknowns [p | u], the model's
-    own order)."""
+    """``pp.Poromechanics`` on one 2-D or 3-D subdomain without fractures -> ``Poromechanics`` (unknowns [p | u], the
+    model's own order)."""
     from .poromech import Poromechanics
-    sds = list(model.mdg.subdomains())
-    if len(sds) != 1 or sds[0].dim != 3:
-        raise NotImplementedError("one 3-D subdomain without fractures is expected")
-    sd = sds[0]
+    sd = _single_matrix(model)
     fk, mk = model.darcy_keyword, model.stress_keyword
     data = _own_data(model.mdg.subdomain_data(sd), [fk, mk])
     fluid = _fluid(model, False)
@@ -200,13 +229,10 @@ def poromechanics_from_model(model):
 
 
 def thermoporomechanics_from_model(model):
-    """``pp.Thermoporomechanics`` on a 3-D subdomain without fractures -> ``Thermoporomechanics`` (unknowns [u | p | T],
-    the model's own order)."""
+    """``pp.Thermoporomechanics`` on one 2-D or 3-D subdomain without fractures -> ``Thermoporomechanics`` (unknowns
+    [u | p | T], the model's own order)."""
     from .thermoporomech import Thermoporomechanics
-    sds = list(model.mdg.subdomains())
-    if len(sds) != 1 or sds[0].dim != 3:
-        raise NotImplementedError("one 3-D subdomain without fractures is expected")
-    sd = sds[0]
+    sd = _single_matrix(model)
     fk, tk, mk, ck = model.darcy_keyword, model.fourier_keyword, model.stress_keyword, model.enthalpy_keyword
     data = _own_data(model.mdg.subdomain_data(sd), [fk, tk, mk])
     fluid = _fluid(model, True)
@@ -230,16 +256,13 @@ def thermoporomechanics_from_model(model):
 
 
 def fractured_momentum_from_model(model):
-    """``pp.MomentumBalance`` with fractures in frictional contact -> (``FracturedMomentumBalance``, column_map): one 3-D
-    matrix subdomain, any number of 2-D fractures (each with its two-sided interface); unknown k of the problem is dof
-    ``column_map[k]`` of the model ([u | contact tractions | interface displacements])."""
+    """``pp.MomentumBalance`` with fractures in frictional contact -> (``FracturedMomentumBalance``, column_map): one
+    nd-D matrix subdomain (nd = 2 or 3), any number of (nd - 1)-D fractures without intersections (each with its
+    two-sided interface); unknown k of the problem is dof ``column_map[k]`` of the model ([u | contact tractions |
+    interface displacements])."""
     from .contact import FractureContact, FracturedMomentumBalance
+    mat, fracs = _matrix_and_fractures(model)
     mdg, es = model.mdg, model.equation_system
-    mats = list(mdg.subdomains(dim=3))
-    fracs = list(mdg.subdomains(dim=2))
-    if len(mats) != 1 or any(sd.dim < 2 for sd in mdg.subdomains()):
-        raise NotImplementedError("one 3-D matrix subdomain and 2-D fractures without intersections are expected")
-    mat = mats[0]
     mk = model.stress_keyword
     data = _own_data(mdg.subdomain_data(mat), [mk])
 
@@ -280,11 +303,8 @@ def _contact_constants(model, fracs):
 def _fractured_problem(model, thermal: bool):
     """Shared part of the two fractured (thermo-)poromechanics bridges."""
     from .fractured_poromech import FractureCoupling
+    mat, fracs = _matrix_and_fractures(model)
     mdg, es = model.mdg, model.equation_system
-    mats, fracs = list(mdg.subdomains(dim=3)), list(mdg.subdomains(dim=2))
-    if len(mats) != 1 or any(sd.dim < 2 for sd in mdg.subdomains()):
-        raise NotImplementedError("one 3-D matrix subdomain and 2-D fractures without intersections are expected")
-    mat = mats[0]
     fk, mk = model.darcy_keyword, model.stress_keyword
     kws = [fk, mk] + ([model.fourier_keyword] if thermal else [])
     data = _own_data(mdg.subdomain_data(mat), kws)
@@ -356,15 +376,16 @@ def fractured_poromechanics_from_model(model):
     prob = FracturedPoromechanics(mat, data, couplings, fluid, solid, _contact_constants(model, fracs), bc,
                                   flow_keyword=model.darcy_keyword, mechanics_keyword=model.stress_keyword)
     prob.mobility_keyword = "b200_mobility"
+    nd = int(mat.dim)
     cols = [dofs(model.pressure_variable, mat)] + [dofs(model.pressure_variable, f) for f in fracs] \
         + [dofs(model.displacement_variable, mat)] + [dofs(model.contact_traction_variable, f) for f in fracs] \
         + [dofs(model.interface_darcy_flux_variable, it) for it in intfs] \
         + [dofs(model.interface_displacement_variable, it) for it in intfs]
-    order = [("mass_balance_equation", [(mat, 1)] + [(f, 1) for f in fracs]), ("momentum_balance_equation", [(mat, 3)]),
+    order = [("mass_balance_equation", [(mat, 1)] + [(f, 1) for f in fracs]), ("momentum_balance_equation", [(mat, nd)]),
              ("interface_darcy_flux_equation", [(it, 1) for it in intfs]),
-             ("interface_force_balance_equation", [(it, 3) for it in intfs]),
+             ("interface_force_balance_equation", [(it, nd) for it in intfs]),
              ("normal_fracture_deformation_equation", [(f, 1) for f in fracs]),
-             ("tangential_fracture_deformation_equation", [(f, 2) for f in fracs])]
+             ("tangential_fracture_deformation_equation", [(f, nd - 1) for f in fracs])]
     return prob, np.concatenate(cols), _row_map(model, order)
 
 
@@ -385,6 +406,7 @@ def fractured_thermoporomechanics_from_model(model):
                                         mechanics_keyword=model.stress_keyword, thermal_keyword=model.enthalpy_keyword)
     prob.mobility_keyword, prob.enthalpy_upwind_keyword = "b200_mobility", "b200_enthalpy_upwind"
     pv, tv = model.pressure_variable, model.temperature_variable
+    nd = int(mat.dim)
     cols = [dofs(pv, mat)] + [dofs(pv, f) for f in fracs] + [dofs(tv, mat)] + [dofs(tv, f) for f in fracs] \
         + [dofs(model.displacement_variable, mat)] + [dofs(model.contact_traction_variable, f) for f in fracs] \
         + [dofs(model.interface_darcy_flux_variable, it) for it in intfs] \
@@ -392,13 +414,13 @@ def fractured_thermoporomechanics_from_model(model):
         + [dofs(model.interface_enthalpy_flux_variable, it) for it in intfs] \
         + [dofs(model.interface_displacement_variable, it) for it in intfs]
     order = [("mass_balance_equation", [(mat, 1)] + [(f, 1) for f in fracs]),
-             ("energy_balance_equation", [(mat, 1)] + [(f, 1) for f in fracs]), ("momentum_balance_equation", [(mat, 3)]),
+             ("energy_balance_equation", [(mat, 1)] + [(f, 1) for f in fracs]), ("momentum_balance_equation", [(mat, nd)]),
              ("interface_darcy_flux_equation", [(it, 1) for it in intfs]),
              ("interface_fourier_flux_equation", [(it, 1) for it in intfs]),
              ("interface_enthalpy_flux_equation", [(it, 1) for it in intfs]),
-             ("interface_force_balance_equation", [(it, 3) for it in intfs]),
+             ("interface_force_balance_equation", [(it, nd) for it in intfs]),
              ("normal_fracture_deformation_equation", [(f, 1) for f in fracs]),
-             ("tangential_fracture_deformation_equation", [(f, 2) for f in fracs])]
+             ("tangential_fracture_deformation_equation", [(f, nd - 1) for f in fracs])]
     return prob, np.concatenate(cols), _row_map(model, order)
 
 

@@ -1,6 +1,7 @@
 """Biot poromechanics, the reference's model equations on the device AD chain -- BASELINE config[3] ("Biot poromechanics,
-coupled MPFA + MPSA"): mass and momentum balance of ``pp.Poromechanics`` on a 3-D subdomain, every term taken from the
-device-resident outputs of ``porepy_b200.Mpfa`` and ``porepy_b200.Biot``, value and Jacobian by ``DeviceAdArray``.
+coupled MPFA + MPSA"): mass and momentum balance of ``pp.Poromechanics`` on a 2-D or 3-D subdomain (``nd = sd.dim``),
+every term taken from the device-resident outputs of ``porepy_b200.Mpfa`` and ``porepy_b200.Biot``, value and Jacobian by
+``DeviceAdArray``.
 
 * ``momentum_balance_equation``   -div_nd (stress u + bound_stress u_b + scalar_gradient (p - p_ref)) - f = 0
                                   models/momentum_balance.py, ``pressure_stress`` constitutive_laws.py
@@ -11,11 +12,11 @@ device-resident outputs of ``porepy_b200.Mpfa`` and ``porepy_b200.Biot``, value 
                                   constitutive_laws.py:2521-2569
 * ``mass_balance_equation``       (mass - mass_n) / dt + div fluid_flux - source = 0
 
-Unknown order as in the reference's ``EquationSystem``: pressures, then displacements (cell-major, 3 per cell); equations:
+Unknown order as in the reference's ``EquationSystem``: pressures, then displacements (cell-major, nd per cell); equations:
 mass balance, then momentum balance.  ``pb.Upwind`` is re-discretized from the iterate's Darcy flux in front of every
 linearization (models/solution_strategy.py:433-441).  The Newton update is solved by the fused Jacobi-BiCGStab
 (csrc/krylov.cu) on the coupled Jacobian.  ``tests/golden/poromech_model.npz`` pins Jacobian, residual, residual history
-and converged state to the unmodified reference (tools/make_poromech_golden.py).
+and converged state to the unmodified reference (tools/make_poromech_golden.py), ``poromech_model_2d.npz`` the same in 2-D.
 """
 from __future__ import annotations
 
@@ -24,6 +25,7 @@ import scipy.sparse as sps
 
 from . import ad, krylov
 from .advection import advective_flux, rediscretize_upwind
+from .contact import matrix_dimension
 from .fv import Biot, Mpfa
 from .newton import newton_loop
 from .params import DISCRETIZATION_MATRICES
@@ -34,7 +36,7 @@ class Poromechanics:
     ``parameters[mechanics_keyword]`` (``fourth_order_tensor``, vectorial ``bc``, ``scalar_vector_mappings`` =
     {flow_keyword: Biot coefficient or tensor}).  ``fluid``: ``compressibility, density, viscosity, reference_pressure``;
     ``solid``: ``reference_porosity, n_inv`` (= (alpha - phi_ref)(1 - alpha) / K_bulk).  Face data: ``flow_bc_values``
-    (pressure on Dirichlet faces, flux elsewhere), ``mech_bc_values`` (3 nf, face-major: displacement / traction),
+    (pressure on Dirichlet faces, flux elsewhere), ``mech_bc_values`` (nd nf, face-major: displacement / traction),
     ``bc_fluid_flux`` + ``fluid_flux_values`` (the boundary operator of the advective flux)."""
 
     mobility_keyword = "mobility"
@@ -42,8 +44,7 @@ class Poromechanics:
     def __init__(self, sd, data: dict, fluid: dict, solid: dict, flow_bc_values, mech_bc_values, bc_fluid_flux,
                  fluid_flux_values, source=None, body_force=None, flow_keyword: str = "flow",
                  mechanics_keyword: str = "mechanics"):
-        if int(sd.dim) != 3:
-            raise NotImplementedError("the poromechanics equations are stated for a 3-D subdomain")
+        self.nd = matrix_dimension(sd)
         self.sd, self.data = sd, data
         self.fk, self.mk = flow_keyword, mechanics_keyword
         self.c, self.rho0, self.mu = (float(fluid[k]) for k in ("compressibility", "density", "viscosity"))
@@ -55,12 +56,12 @@ class Poromechanics:
         self.bc_fluid_flux = bc_fluid_flux
         self.ff_values = np.asarray(fluid_flux_values, float)
         self.source = np.zeros(self.nc) if source is None else np.asarray(source, float)
-        self.body_force = np.zeros(3 * self.nc) if body_force is None else np.asarray(body_force, float)
+        self.body_force = np.zeros(self.nd * self.nc) if body_force is None else np.asarray(body_force, float)
         self._const = None
 
     @property
     def num_dofs(self) -> int:
-        return 4 * self.nc
+        return (self.nd + 1) * self.nc
 
     def discretize(self) -> None:
         Mpfa(self.fk).discretize(self.sd, self.data)
@@ -80,7 +81,7 @@ class Poromechanics:
             vol = np.asarray(self.sd.cell_volumes, float)
             k = SimpleNamespace(
                 div=csr(sps.csr_matrix(self.sd.cell_faces.T)),
-                div3=csr(sps.kron(sps.csr_matrix(self.sd.cell_faces.T), sps.identity(3)).tocsr()),
+                div_nd=csr(sps.kron(sps.csr_matrix(self.sd.cell_faces.T), sps.identity(self.nd)).tocsr()),
                 flux=csr(F["flux"]), stress=csr(M["stress"]), grad_p=csr(self._coupling("scalar_gradient")),
                 div_u=csr(self._coupling("displacement_divergence")), cons=csr(self._coupling("mpsa_consistency")),
                 vol=dev(vol), inv_vol=dev(1.0 / vol), bcw=dev(self.ff_values), src=dev(self.source), f=dev(self.body_force))
@@ -120,7 +121,7 @@ class Poromechanics:
         ff = advective_flux(T, q, w, k.bcw, k.bcw)
         mass_eq = (mass - mass_n) * (1.0 / dt) + (k.div @ ff) - k.src
         stress = (k.stress @ u) + (k.grad_p @ (p - self.p_ref)) + k.stress_b
-        momentum_eq = -(k.div3 @ stress) - k.f
+        momentum_eq = -(k.div_nd @ stress) - k.f
         return [mass_eq, momentum_eq]
 
     def linearize(self, x, x_prev, dt: float):

@@ -1,7 +1,8 @@
 """Thermo-poromechanics, the reference's model equations on the device AD chain -- BASELINE config[4] ("thermo-
-poromechanics ..., full Newton loop") on a 3-D subdomain without fractures: momentum, mass and energy balance of
-``pp.Thermoporomechanics``, every term from the device-resident outputs of ``porepy_b200.Mpfa`` (Darcy and Fourier) and
-``porepy_b200.Biot`` (two coupling tensors: Biot's and the thermal stress), value and Jacobian by ``DeviceAdArray``.
+poromechanics ..., full Newton loop") on a 2-D or 3-D subdomain (``nd = sd.dim``) without fractures: momentum, mass and
+energy balance of ``pp.Thermoporomechanics``, every term from the device-resident outputs of ``porepy_b200.Mpfa`` (Darcy
+and Fourier) and ``porepy_b200.Biot`` (two coupling tensors: Biot's and the thermal stress), value and Jacobian by
+``DeviceAdArray``.
 
 * density                  rho = rho0 exp(c (p - p0) - beta_f (T - T0))                    fluid_property_library.py
 * porosity                 poromechanical porosity of ``porepy_b200.poromech`` - (alpha - phi0) beta_s (T - T0)
@@ -15,9 +16,9 @@ poromechanics ..., full Newton loop") on a 3-D subdomain without fractures: mome
                            c_f (T - T0) rho / mu                                            energy_balance.py:236-352
 * balance equations        momentum: -div_nd stress - f;  mass / energy: d/dt (vol x) + div flux - source
 
-Unknown order as in the reference's ``EquationSystem``: displacements (3 per cell), pressures, temperatures; equations:
+Unknown order as in the reference's ``EquationSystem``: displacements (nd per cell), pressures, temperatures; equations:
 momentum, mass, energy.  ``tests/golden/thm_model.npz`` pins Jacobian, residual, residual history and converged state to the
-unmodified reference (tools/make_thm_golden.py).
+unmodified reference (tools/make_thm_golden.py), ``thm_model_2d.npz`` the same in 2-D.
 """
 from __future__ import annotations
 
@@ -28,6 +29,7 @@ import scipy.sparse as sps
 
 from . import ad, krylov
 from .advection import advective_flux, rediscretize_upwind
+from .contact import matrix_dimension
 from .fv import Biot, Mpfa
 from .newton import newton_loop
 from .params import DISCRETIZATION_MATRICES, PARAMETERS, SecondOrderTensor
@@ -39,7 +41,7 @@ class Thermoporomechanics:
     vectorial ``bc``, ``scalar_vector_mappings`` = {flow_keyword: Biot tensor, thermal_keyword: thermal-stress tensor}).
     ``fluid``: ``compressibility, density, viscosity, thermal_expansion, heat_capacity, conductivity, reference_pressure,
     reference_temperature``; ``solid``: ``reference_porosity, n_inv, biot_coefficient, thermal_expansion, heat_capacity,
-    conductivity, density``.  ``bc``: face arrays ``flow``, ``fourier``, ``mechanics`` (3 nf), ``fluid_flux``,
+    conductivity, density``.  ``bc``: face arrays ``flow``, ``fourier``, ``mechanics`` (nd nf), ``fluid_flux``,
     ``enthalpy_flux`` and the boundary-condition objects ``fluid_flux_type``, ``enthalpy_flux_type`` of the two upwind
     discretizations."""
 
@@ -49,8 +51,7 @@ class Thermoporomechanics:
     def __init__(self, sd, data: dict, fluid: dict, solid: dict, bc: dict, flow_keyword: str = "flow",
                  fourier_keyword: str = "fourier", mechanics_keyword: str = "mechanics", thermal_keyword: str = "thermal",
                  rediscretize_fourier: bool = False):
-        if int(sd.dim) != 3:
-            raise NotImplementedError("the thermo-poromechanics equations are stated for a 3-D subdomain")
+        self.nd = matrix_dimension(sd)
         self.sd, self.data = sd, data
         self.fk, self.tk, self.mk, self.ck = flow_keyword, fourier_keyword, mechanics_keyword, thermal_keyword
         self.fl = SimpleNamespace(**{k: float(v) for k, v in fluid.items()})
@@ -62,7 +63,7 @@ class Thermoporomechanics:
 
     @property
     def num_dofs(self) -> int:
-        return 5 * self.nc
+        return (self.nd + 2) * self.nc
 
     def _discretize_fourier(self, phi) -> None:
         self.data[PARAMETERS][self.tk]["second_order_tensor"] = SecondOrderTensor(
@@ -85,7 +86,7 @@ class Thermoporomechanics:
             vol = np.asarray(self.sd.cell_volumes, float)
             k = SimpleNamespace(
                 div=csr(sps.csr_matrix(self.sd.cell_faces.T)),
-                div3=csr(sps.kron(sps.csr_matrix(self.sd.cell_faces.T), sps.identity(3)).tocsr()),
+                div_nd=csr(sps.kron(sps.csr_matrix(self.sd.cell_faces.T), sps.identity(self.nd)).tocsr()),
                 flux=csr(F["flux"]), stress=csr(M["stress"]), grad_p=csr(M["scalar_gradient"][self.fk]),
                 grad_t=csr(M["scalar_gradient"][self.ck]), div_u=csr(M["displacement_divergence"][self.fk]),
                 cons=csr(M["mpsa_consistency"][self.fk]), vol=dev(vol), inv_vol=dev(1.0 / vol),
@@ -114,8 +115,8 @@ class Thermoporomechanics:
         return fluid + solid
 
     def _split(self, x):
-        n3 = 3 * self.nc
-        return x[:n3], x[n3:n3 + self.nc], x[n3 + self.nc:]
+        nu = self.nd * self.nc
+        return x[:nu], x[nu:nu + self.nc], x[nu + self.nc:]
 
     # ---- what follows the iterate: upwind directions (and, by request, the porosity-weighted conductivity)
     def update_discretizations(self, x) -> None:
@@ -143,7 +144,7 @@ class Thermoporomechanics:
         rho, rho_n = self._density(p, t), self._density(pn, tn)
         stress = (k.stress @ u) + (k.grad_p @ (p - fl.reference_pressure)) + (k.grad_t @ (t - fl.reference_temperature)) \
             + k.stress_b
-        momentum = -(k.div3 @ stress)
+        momentum = -(k.div_nd @ stress)
         q = (k.flux @ p) + k.q_b
         w = rho * (1.0 / fl.viscosity)
         ff = advective_flux(Tm, q, w, k.bcw, k.bcw)

@@ -4,7 +4,9 @@ displacements, contact traction; force balance on the interface; the semismooth 
 models/contact_mechanics.py:80-245 with Coulomb friction and shear dilation) -- the contact part of BASELINE config[4] in
 miniature: a compressed and sheared fracture in the sliding regime.  Stored: grids, parameters, the geometric pieces of the
 interface (scalar mortar projections, side signs, local fracture coordinates), the Jacobian / right-hand side at the second
-Newton iterate, the residual history and the converged state.   python tools/make_contact_golden.py"""
+Newton iterate, the residual history and the converged state.  ``Model2d`` is the 2-D counterpart (an 8 x 8 Cartesian unit
+square cut by a vertical line fracture that does not reach the boundary; fixtures ``*_2d``).
+   python tools/make_contact_golden.py"""
 from __future__ import annotations
 
 import os
@@ -68,15 +70,44 @@ class Model(pp.MomentumBalance):
         return v.ravel("F")
 
 
-def main(scenario="sliding", name="contact_model"):
+class Model2d(Model):
+    """The 2-D counterpart of ``Model``: the unit square, 8 x 8 cells, the line fracture x = 0.5, 0.25 <= y <= 0.75; the
+    east side is pushed and sheared as in 3-D, with the variation along y.  The grid is built by ``pp.meshing.cart_grid``
+    directly (the fracture network of the default ``set_geometry`` needs shapely for a 2-D domain)."""
+
+    def set_domain(self):
+        self._domain = pp.Domain({"xmin": 0, "xmax": 1, "ymin": 0, "ymax": 1})
+
+    def set_geometry(self):
+        self.set_domain()
+        self.mdg = pp.meshing.cart_grid([np.array([[0.5, 0.5], [0.25, 0.75]])], [8, 8], physdims=[1, 1])
+        self.nd = self.mdg.dim_max()
+        pp.set_local_coordinate_projections(self.mdg)
+        self.set_well_network()
+
+    def bc_values_displacement(self, bg):
+        s = self.domain_boundary_sides(bg)
+        v = np.zeros((2, bg.num_cells))
+        y = bg.cell_centers[1, s.east]
+        if self.scenario == "sliding":
+            v[0, s.east] = -0.01 * (1 + 0.3 * y)                               # compress across the fracture, unevenly
+            v[1, s.east] = 0.02                                                # and shear it
+        elif self.scenario == "mixed":                                         # a rotation-like load: the lower part
+            v[0, s.east] = 0.03 * (y - 0.5)                                    # closes and slides, the upper part opens
+            v[1, s.east] = 0.01
+        return v.ravel("F")
+
+
+def main(scenario="sliding", name="contact_model", base=Model):
     solid = pp.SolidConstants(lame_lambda=2.0, shear_modulus=1.5, friction_coefficient=0.4, fracture_gap=1e-4,
                               dilation_angle=0.1)
-    m = Model({"times_to_export": [], "time_manager": pp.TimeManager([0, 1.0], 1.0, constant_dt=True),
+    m = base({"times_to_export": [], "time_manager": pp.TimeManager([0, 1.0], 1.0, constant_dt=True),
                "material_constants": {"solid": solid}})
     m.scenario = scenario
     m.prepare_simulation()
     es, mdg = m.equation_system, m.mdg
-    mat, frac, intf = mdg.subdomains(dim=3)[0], mdg.subdomains(dim=2)[0], mdg.interfaces()[0]
+    nd = m.nd
+    mat, frac, intf = mdg.subdomains(dim=nd)[0], mdg.subdomains(dim=nd - 1)[0], mdg.interfaces()[0]
     assert list(es.equations) == ["momentum_balance_equation", "interface_force_balance_equation",
                                   "normal_fracture_deformation_equation", "tangential_fracture_deformation_equation"]
 
@@ -105,7 +136,7 @@ def main(scenario="sliding", name="contact_model"):
         m.after_nonlinear_iteration(m.solve_linear_system())
     bcm = mdg.subdomain_data(mat)[pp.PARAMETERS]["mechanics"]["bc"]
     bg = mdg.subdomain_to_boundary_grid(mat)
-    proj3 = sps.kron(bg.projection(), sps.eye(3)).tocsr()
+    proj3 = sps.kron(bg.projection(), sps.eye(nd)).tocsr()
 
     def scalar(op):
         v = es.evaluate(op)
@@ -127,35 +158,48 @@ def main(scenario="sliding", name="contact_model"):
     for key in ("mortar_to_primary_avg", "primary_to_mortar_int", "mortar_to_secondary_avg", "secondary_to_mortar_int"):
         put_csr(d, key, getattr(intf, key)())
     np.savez_compressed(os.path.join(OUT, name + ".npz"), **d)
-    t = d["solution"][dofs("contact_traction")].reshape(-1, 3)
+    t = d["solution"][dofs("contact_traction")].reshape(-1, nd)
     print(name, "dofs", es.num_dofs(), "Newton residuals", ["%.2e" % v for v in norms])
-    print("   contact traction (t1, t2, n) per fracture cell:\\n", t, "\\n   |t_t| / (mu |t_n|):",
-          np.linalg.norm(t[:, :2], axis=1) / (0.4 * np.abs(t[:, 2])))
+    print("   contact traction (tangential, normal) per fracture cell:\\n", t, "\\n   |t_t| / (mu |t_n|):",
+          np.linalg.norm(t[:, :nd - 1], axis=1) / (0.4 * np.abs(t[:, nd - 1])))
 
 
-def main_poromechanics(scenario="sliding", name="contact_poromech"):
+def permeability(model, subdomains):
+    """Seeded heterogeneous, anisotropic permeability; 20 times larger in the fractures.  In 2-D the tensor is in-plane
+    (k_zz = 1, no out-of-plane coupling)."""
+    vals = []
+    for sd in subdomains:
+        rng = np.random.default_rng(5 + sd.num_cells)
+        nc = sd.num_cells
+        t = np.zeros((3, 3, nc))
+        scale = 1.0 if sd.dim == model.nd else 20.0
+        if model.nd == 3:
+            t[0, 0], t[1, 1], t[2, 2] = scale * (1 + rng.random((3, nc)))
+            o = 0.3 * scale * rng.random((3, nc))
+            t[0, 1] = t[1, 0] = o[0]
+            t[0, 2] = t[2, 0] = o[1]
+            t[1, 2] = t[2, 1] = o[2]
+        else:
+            t[0, 0], t[1, 1] = scale * (1 + rng.random((2, nc)))
+            t[0, 1] = t[1, 0] = 0.3 * scale * rng.random(nc)
+            t[2, 2] = 1.0
+        vals.append(t.reshape(9, nc).ravel("F"))
+    return pp.wrap_as_dense_ad_array(np.hstack(vals) if vals else np.zeros(0), name="permeability")
+
+
+def _geometry(base):
+    """The geometry, stiffness and mechanical loads of ``base`` (``Model`` or ``Model2d``) as a mixin."""
+    keys = ("set_domain", "grid_type", "meshing_arguments", "set_fractures", "stiffness_tensor", "bc_type_mechanics",
+            "bc_values_displacement") + (("set_geometry",) if base is Model2d else ())
+    return type("Geometry", (), {k: getattr(base, k) for k in keys})
+
+
+def main_poromechanics(scenario="sliding", name="contact_poromech", base=Model):
     """``pp.Poromechanics`` on the same fractured domain: Biot poromechanics in the matrix, compressible flow in the
     fracture (aperture = residual aperture + normal jump), the interface Darcy law with that aperture, the fluid pressure
     in the interface force balance, frictional contact -- BASELINE configs[3] + [4] in one model."""
-    class PoroModel(pp.Poromechanics):
-        set_domain, grid_type, meshing_arguments = Model.set_domain, Model.grid_type, Model.meshing_arguments
-        set_fractures, stiffness_tensor = Model.set_fractures, Model.stiffness_tensor
-        bc_type_mechanics, bc_values_displacement = Model.bc_type_mechanics, Model.bc_values_displacement
-
-        def permeability(self, subdomains):
-            vals = []
-            for sd in subdomains:
-                rng = np.random.default_rng(5 + sd.num_cells)
-                nc = sd.num_cells
-                t = np.zeros((3, 3, nc))
-                scale = 1.0 if sd.dim == 3 else 20.0
-                t[0, 0], t[1, 1], t[2, 2] = scale * (1 + rng.random((3, nc)))
-                o = 0.3 * scale * rng.random((3, nc))
-                t[0, 1] = t[1, 0] = o[0]
-                t[0, 2] = t[2, 0] = o[1]
-                t[1, 2] = t[2, 1] = o[2]
-                vals.append(t.reshape(9, nc).ravel("F"))
-            return pp.wrap_as_dense_ad_array(np.hstack(vals) if vals else np.zeros(0), name="permeability")
+    class PoroModel(_geometry(base), pp.Poromechanics):
+        permeability = permeability
 
         def bc_type_darcy_flux(self, sd):
             s = self.domain_boundary_sides(sd)
@@ -179,7 +223,8 @@ def main_poromechanics(scenario="sliding", name="contact_poromech"):
     m.scenario = scenario
     m.prepare_simulation()
     es, mdg = m.equation_system, m.mdg
-    mat, frac, intf = mdg.subdomains(dim=3)[0], mdg.subdomains(dim=2)[0], mdg.interfaces()[0]
+    nd = m.nd
+    mat, frac, intf = mdg.subdomains(dim=nd)[0], mdg.subdomains(dim=nd - 1)[0], mdg.interfaces()[0]
 
     def dofs(name, g=None):
         return es.dofs_of([v for v in es.variables if v.name == name and (g is None or v.domain is g)])
@@ -195,9 +240,9 @@ def main_poromechanics(scenario="sliding", name="contact_poromech"):
         for f in ("is_dir", "is_neu", "is_rob", "is_internal"):
             d[f"{key}__flow_{f}"] = getattr(prm["bc"], f)
     rows, r0 = {}, 0
-    layout = {"normal_fracture_deformation_equation": [(frac, 1)], "tangential_fracture_deformation_equation": [(frac, 2)],
+    layout = {"normal_fracture_deformation_equation": [(frac, 1)], "tangential_fracture_deformation_equation": [(frac, nd - 1)],
               "mass_balance_equation": [(mat, 1), (frac, 1)], "interface_darcy_flux_equation": [(intf, 1)],
-              "momentum_balance_equation": [(mat, 3)], "interface_force_balance_equation": [(intf, 3)]}
+              "momentum_balance_equation": [(mat, nd)], "interface_force_balance_equation": [(intf, nd)]}
     for eq in es.equations:
         for g, k in layout.get(eq, []):
             rows[(eq, id(g))] = np.arange(r0, r0 + k * g.num_cells)
@@ -227,7 +272,7 @@ def main_poromechanics(scenario="sliding", name="contact_poromech"):
         m.after_nonlinear_iteration(m.solve_linear_system())
     bg = mdg.subdomain_to_boundary_grid(mat)
     proj = bg.projection()
-    proj3 = sps.kron(proj, sps.eye(3)).tocsr()
+    proj3 = sps.kron(proj, sps.eye(nd)).tocsr()
     bcm = mdg.subdomain_data(mat)[pp.PARAMETERS]["mechanics"]["bc"]
     bcf = mdg.subdomain_data(mat)[pp.PARAMETERS]["flow"]["bc"]
     bff = m.bc_type_fluid_flux(mat)
@@ -275,33 +320,16 @@ def main_poromechanics(scenario="sliding", name="contact_poromech"):
                 "mortar_to_primary_int", "primary_to_mortar_avg", "mortar_to_secondary_int", "secondary_to_mortar_avg"):
         put_csr(d, key, getattr(intf, key)())
     np.savez_compressed(os.path.join(OUT, name + ".npz"), **d)
-    t = d["solution"][dofs("contact_traction")].reshape(-1, 3)
+    t = d["solution"][dofs("contact_traction")].reshape(-1, nd)
     print(name, "dofs", es.num_dofs(), "Newton residuals", ["%.2e" % v for v in norms])
     print("   contact traction:", np.array2string(t, precision=4).replace("\n", ";"))
 
 
-def main_thm(scenario="sliding", name="contact_thm"):
+def main_thm(scenario="sliding", name="contact_thm", base=Model):
     """``pp.Thermoporomechanics`` on the fractured domain: BASELINE config[4] (thermo-poromechanics + frictional contact, full
     Newton loop) on one fracture."""
-    class ThmModel(pp.Thermoporomechanics):
-        set_domain, grid_type, meshing_arguments = Model.set_domain, Model.grid_type, Model.meshing_arguments
-        set_fractures, stiffness_tensor = Model.set_fractures, Model.stiffness_tensor
-        bc_type_mechanics, bc_values_displacement = Model.bc_type_mechanics, Model.bc_values_displacement
-
-        def permeability(self, subdomains):
-            vals = []
-            for sd in subdomains:
-                rng = np.random.default_rng(5 + sd.num_cells)
-                nc = sd.num_cells
-                t = np.zeros((3, 3, nc))
-                scale = 1.0 if sd.dim == 3 else 20.0
-                t[0, 0], t[1, 1], t[2, 2] = scale * (1 + rng.random((3, nc)))
-                o = 0.3 * scale * rng.random((3, nc))
-                t[0, 1] = t[1, 0] = o[0]
-                t[0, 2] = t[2, 0] = o[1]
-                t[1, 2] = t[2, 1] = o[2]
-                vals.append(t.reshape(9, nc).ravel("F"))
-            return pp.wrap_as_dense_ad_array(np.hstack(vals) if vals else np.zeros(0), name="permeability")
+    class ThmModel(_geometry(base), pp.Thermoporomechanics):
+        permeability = permeability
 
         def bc_type_darcy_flux(self, sd):
             s = self.domain_boundary_sides(sd)
@@ -317,7 +345,7 @@ def main_thm(scenario="sliding", name="contact_thm"):
         def bc_values_temperature(self, bg):
             s = self.domain_boundary_sides(bg)
             v = np.zeros(bg.num_cells)
-            v[s.south] = 0.3 + 0.1 * bg.cell_centers[2, s.south]
+            v[s.south] = 0.3 + 0.1 * bg.cell_centers[2 if self.nd == 3 else 0, s.south]      # varies along z, x in 2-D
             return v
     fluid = pp.FluidComponent(compressibility=0.05, viscosity=1.3, density=1.7, thermal_expansion=0.03,
                               specific_heat_capacity=2.0, thermal_conductivity=0.7)
@@ -330,7 +358,8 @@ def main_thm(scenario="sliding", name="contact_thm"):
     m.scenario = scenario
     m.prepare_simulation()
     es, mdg = m.equation_system, m.mdg
-    mat, frac, intf = mdg.subdomains(dim=3)[0], mdg.subdomains(dim=2)[0], mdg.interfaces()[0]
+    nd = m.nd
+    mat, frac, intf = mdg.subdomains(dim=nd)[0], mdg.subdomains(dim=nd - 1)[0], mdg.interfaces()[0]
 
     def dofs(name, g=None):
         return es.dofs_of([v for v in es.variables if v.name == name and (g is None or v.domain is g)])
@@ -347,8 +376,8 @@ def main_thm(scenario="sliding", name="contact_thm"):
                 d[f"{key}__{short}_{f}"] = getattr(prm["bc"], f)
     svm = mdg.subdomain_data(mat)[pp.PARAMETERS]["mechanics"]["scalar_vector_mappings"]
     d["alpha_flow"], d["alpha_thermal"] = svm["flow"].values, svm[m.enthalpy_keyword].values
-    layout = {"normal_fracture_deformation_equation": [(frac, 1)], "tangential_fracture_deformation_equation": [(frac, 2)],
-              "momentum_balance_equation": [(mat, 3)], "interface_force_balance_equation": [(intf, 3)],
+    layout = {"normal_fracture_deformation_equation": [(frac, 1)], "tangential_fracture_deformation_equation": [(frac, nd - 1)],
+              "momentum_balance_equation": [(mat, nd)], "interface_force_balance_equation": [(intf, nd)],
               "mass_balance_equation": [(mat, 1), (frac, 1)], "interface_darcy_flux_equation": [(intf, 1)],
               "energy_balance_equation": [(mat, 1), (frac, 1)], "interface_fourier_flux_equation": [(intf, 1)],
               "interface_enthalpy_flux_equation": [(intf, 1)]}
@@ -379,7 +408,7 @@ def main_thm(scenario="sliding", name="contact_thm"):
         m.after_nonlinear_iteration(m.solve_linear_system())
     bg = mdg.subdomain_to_boundary_grid(mat)
     proj = bg.projection()
-    proj3 = sps.kron(proj, sps.eye(3)).tocsr()
+    proj3 = sps.kron(proj, sps.eye(nd)).tocsr()
     prm = mdg.subdomain_data(mat)[pp.PARAMETERS]
     bcm, bcf, bct = prm["mechanics"]["bc"], prm["flow"]["bc"], prm["fourier_discretization"]["bc"]
     bff, bfe = m.bc_type_fluid_flux(mat), m.bc_type_enthalpy_flux(mat)
@@ -453,3 +482,7 @@ if __name__ == "__main__":
     main("sticking", "contact_sticking")
     main("open", "contact_open")
     main("mixed", "contact_mixed")
+    main_thm("sliding", "contact_thm_2d", Model2d)
+    main_poromechanics("sliding", "contact_poromech_2d", Model2d)
+    main("sliding", "contact_2d", Model2d)
+    main("mixed", "contact_2d_mixed", Model2d)

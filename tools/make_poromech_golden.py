@@ -1,7 +1,8 @@
 """Generate tests/golden/poromech_model.npz: the Jacobian, residual, residual history and converged state of one implicit
 time step of the unmodified reference's ``pp.Poromechanics`` (Biot coupling through ``pp.Biot``, compressible fluid,
-upwinded mobility, stabilised poromechanical porosity) on a small 3-D grid -- BASELINE config[3] in miniature.  Run in the
-build container:  python tools/make_poromech_golden.py"""
+upwinded mobility, stabilised poromechanical porosity) on a small 3-D grid -- BASELINE config[3] in miniature -- and
+tests/golden/poromech_model_2d.npz, the same on a 10 x 8 Cartesian grid in 2-D (``Model2d``).  Run in the build
+container:  python tools/make_poromech_golden.py"""
 from __future__ import annotations
 
 import os
@@ -82,10 +83,54 @@ class Model(pp.Poromechanics):
         return v.ravel("F")
 
 
-def main():
+def permeability_2d(sd, seed):
+    """Seeded heterogeneous, anisotropic in-plane permeability of a 2-D (or 1-D) grid: k_xx, k_yy, k_xy; k_zz = 1."""
+    rng = np.random.default_rng(seed)
+    nc = sd.num_cells
+    t = np.zeros((3, 3, nc))
+    t[0, 0], t[1, 1] = 1 + rng.random((2, nc))
+    t[0, 1] = t[1, 0] = 0.3 * rng.random(nc)
+    t[2, 2] = 1.0
+    return t
+
+
+class Model2d(Model):
+    """The 2-D counterpart of ``Model``: the same kind of loads on a 1.25 x 1 rectangle with 10 x 8 cells (west: Dirichlet
+    pressure and displacement, south: fixed, north: a compressive traction)."""
+
+    def set_domain(self):
+        self._domain = pp.Domain({"xmin": 0, "xmax": 1.25, "ymin": 0, "ymax": 1})
+
+    def meshing_arguments(self):
+        return {"cell_size": 0.125}
+
+    def permeability(self, subdomains):
+        vals = [permeability_2d(sd, sd.num_cells).reshape(9, sd.num_cells).ravel("F") for sd in subdomains]
+        return pp.wrap_as_dense_ad_array(np.hstack(vals) if vals else np.zeros(0), name="permeability")
+
+    def bc_type_mechanics(self, sd):
+        s = self.domain_boundary_sides(sd)
+        bc = pp.BoundaryConditionVectorial(sd, s.west + s.south, "dir")
+        bc.internal_to_dirichlet(sd)
+        return bc
+
+    def bc_values_stress(self, bg):
+        s = self.domain_boundary_sides(bg)
+        v = np.zeros((2, bg.num_cells))
+        v[1, s.north] = -0.05 * bg.cell_volumes[s.north]
+        return v.ravel("F")
+
+    def bc_values_displacement(self, bg):
+        s = self.domain_boundary_sides(bg)
+        v = np.zeros((2, bg.num_cells))
+        v[0, s.west] = 0.01 * bg.cell_centers[1, s.west]
+        return v.ravel("F")
+
+
+def main(model_class=Model, name="poromech_model"):
     fluid = pp.FluidComponent(compressibility=0.05, viscosity=1.3, density=1.7)
     solid = pp.SolidConstants(porosity=0.2, biot_coefficient=0.8, lame_lambda=2.0, shear_modulus=1.5, permeability=1.0)
-    m = Model({"times_to_export": [], "time_manager": pp.TimeManager([0, 1.0], 0.25, constant_dt=True),
+    m = model_class({"times_to_export": [], "time_manager": pp.TimeManager([0, 1.0], 0.25, constant_dt=True),
                "material_constants": {"fluid": fluid, "solid": solid}})
     m.prepare_simulation()
     es = m.equation_system
@@ -114,7 +159,7 @@ def main():
     fl = m.fluid.reference_component
     bg = m.mdg.subdomain_to_boundary_grid(sd)
     proj = bg.projection()
-    proj3 = sps.kron(proj, sps.eye(3)).tocsr()
+    proj3 = sps.kron(proj, sps.eye(sd.dim)).tocsr()
     bcf = data[pp.PARAMETERS]["flow"]["bc"]
     bcm = data[pp.PARAMETERS]["mechanics"]["bc"]
     bff = m.bc_type_fluid_flux(sd)
@@ -136,9 +181,10 @@ def main():
              mech_is_dir=bcm.is_dir, mech_is_neu=bcm.is_neu, mech_is_rob=bcm.is_rob, mech_is_internal=bcm.is_internal,
              mech_bc_values=np.where(bcm.is_dir.ravel("F"), proj3.T @ m.bc_values_displacement(bg),
                                      proj3.T @ m.bc_values_stress(bg)))
-    np.savez_compressed(os.path.join(OUT, "poromech_model.npz"), **d)
-    print("poromech_model", "cells", nc, "dofs", es.num_dofs(), "Newton residuals", ["%.2e" % v for v in norms])
+    np.savez_compressed(os.path.join(OUT, name + ".npz"), **d)
+    print(name, "cells", nc, "dofs", es.num_dofs(), "Newton residuals", ["%.2e" % v for v in norms])
 
 
 if __name__ == "__main__":
     main()
+    main(Model2d, "poromech_model_2d")

@@ -2,7 +2,8 @@
 of the unmodified reference's ``pp.Thermoporomechanics`` (momentum, mass and energy balance; Biot and thermal stress
 coupling through ``pp.Biot``; compressible, thermally expanding fluid; upwinded mass and enthalpy fluxes; Fourier flux
 discretized at the reference porosity, the model's default) on a small 3-D grid -- BASELINE config[4] without
-the fractures.  Run in the build container:  python tools/make_thm_golden.py"""
+the fractures -- and tests/golden/thm_model_2d.npz, the same on the 2-D grid of ``make_poromech_golden.Model2d``.  Run in
+the build container:  python tools/make_thm_golden.py"""
 from __future__ import annotations
 
 import os
@@ -40,12 +41,23 @@ class Model(Shared, pp.Thermoporomechanics):
         return v
 
 
-def main():
+Shared2d = type("Shared2d", (), {k: v for k, v in pm.Model2d.__dict__.items() if callable(v) and not k.startswith("__")})
+
+
+class Model2d(Shared2d, Model):
+    def bc_values_temperature(self, bg):
+        s = self.domain_boundary_sides(bg)
+        v = np.zeros(bg.num_cells)
+        v[s.west] = 0.5 + 0.2 * bg.cell_centers[1, s.west]
+        return v
+
+
+def main(model_class=Model, name="thm_model"):
     fluid = pp.FluidComponent(compressibility=0.05, viscosity=1.3, density=1.7, thermal_expansion=0.03,
                               specific_heat_capacity=2.0, thermal_conductivity=0.7)
     solid = pp.SolidConstants(porosity=0.2, biot_coefficient=0.8, lame_lambda=2.0, shear_modulus=1.5, permeability=1.0,
                               thermal_expansion=0.02, specific_heat_capacity=1.5, thermal_conductivity=1.1, density=2.5)
-    m = Model({"times_to_export": [], "time_manager": pp.TimeManager([0, 1.0], 0.25, constant_dt=True),
+    m = model_class({"times_to_export": [], "time_manager": pp.TimeManager([0, 1.0], 0.25, constant_dt=True),
                "material_constants": {"fluid": fluid, "solid": solid}})
     m.prepare_simulation()
     es = m.equation_system
@@ -73,7 +85,7 @@ def main():
     fl, so = m.fluid.reference_component, m.solid
     bg = m.mdg.subdomain_to_boundary_grid(sd)
     proj = bg.projection()
-    proj3 = sps.kron(proj, sps.eye(3)).tocsr()
+    proj3 = sps.kron(proj, sps.eye(sd.dim)).tocsr()
     prm = data[pp.PARAMETERS]
     p_ref, t_ref = m.reference_variable_values.pressure, m.reference_variable_values.temperature
     pb_, tb = proj.T @ m.bc_values_pressure(bg), proj.T @ m.bc_values_temperature(bg)
@@ -106,9 +118,10 @@ def main():
              mech_is_dir=bcm.is_dir, mech_is_neu=bcm.is_neu, mech_is_rob=bcm.is_rob, mech_is_internal=bcm.is_internal,
              mech_bc_values=np.where(bcm.is_dir.ravel("F"), proj3.T @ m.bc_values_displacement(bg),
                                      proj3.T @ m.bc_values_stress(bg)))
-    np.savez_compressed(os.path.join(OUT, "thm_model.npz"), **d)
-    print("thm_model", "cells", sd.num_cells, "dofs", es.num_dofs(), "Newton residuals", ["%.2e" % v for v in norms])
+    np.savez_compressed(os.path.join(OUT, name + ".npz"), **d)
+    print(name, "cells", sd.num_cells, "dofs", es.num_dofs(), "Newton residuals", ["%.2e" % v for v in norms])
 
 
 if __name__ == "__main__":
     main()
+    main(Model2d, "thm_model_2d")

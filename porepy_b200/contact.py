@@ -35,6 +35,7 @@ import scipy.sparse as sps
 
 from . import ad, ad_functions as fn
 from .fv import Mpsa
+from .layout import BlockLayout, LayoutModel
 from .newton import newton_loop
 from .params import DISCRETIZATION_MATRICES
 
@@ -92,14 +93,31 @@ def mortar_pairs(mortar_to_secondary) -> np.ndarray:
     return m.indices.reshape(-1, 2).astype(np.int64)
 
 
-def span(offset, index, width: int) -> np.ndarray:
-    """(len(index), width): the unknowns or equations ``offset + width * index + 0 .. width - 1``."""
-    return int(offset) + width * np.asarray(index, np.int64)[:, None] + np.arange(width)
+def fracture_parts(fractures, width: int) -> list:
+    """``BlockLayout`` parts of ``width`` entries per cell on every fracture."""
+    return [(("fracture", j), f.num_cells, width) for j, f in enumerate(fractures)]
 
 
-def block_groups(blocks):
-    """``krylov.BlockGroups`` from a list of (rows, cols) pairs of (number of groups, group size) arrays."""
+def interface_parts(fractures, width: int) -> list:
+    """``BlockLayout`` parts of ``width`` entries per mortar cell on the interface of every fracture."""
+    return [(("interface", j), f.num_mortar, width) for j, f in enumerate(fractures)]
+
+
+def block_groups(prob):
+    """``krylov.BlockGroups`` of the grouped block-Jacobi preconditioner of ``krylov.gmres`` for ``prob``: one group per
+    matrix cell c and one per fracture cell k with its mortar cells m1, m2, declared by ``prob.matrix_group`` /
+    ``prob.fracture_group`` as (rows, cols) lists of (equation block, cell) / (unknown block, cell)."""
     from .krylov import BlockGroups
+
+    def group(decl, cells):
+        rows, cols = decl
+        return (np.hstack([prob.equation_layout.span(b, *cells[c]) for b, c in rows]),
+                np.hstack([prob.unknown_layout.span(b, *cells[c]) for b, c in cols]))
+    blocks = [group(prob.matrix_group, {"c": (("matrix",), np.arange(prob.nc))})]
+    for j, fc in enumerate(prob.fractures):
+        m = mortar_pairs(fc.mortar_to_secondary)
+        blocks.append(group(prob.fracture_group, {"k": (("fracture", j), np.arange(fc.num_cells)),
+                                                  "m1": (("interface", j), m[:, 0]), "m2": (("interface", j), m[:, 1])}))
     sizes = np.concatenate([np.full(r.shape[0], r.shape[1], np.int64) for r, _ in blocks])
     return BlockGroups(np.concatenate(([0], np.cumsum(sizes))), np.concatenate([r.ravel() for r, _ in blocks]),
                        np.concatenate([c.ravel() for _, c in blocks]))
@@ -143,7 +161,7 @@ def contact_laws(q, t, u_j, u_j_prev, c):
     return normal, tangential
 
 
-class FracturedMomentumBalance:
+class FracturedMomentumBalance(LayoutModel):
     """``sd``: the 2-D or 3-D matrix grid (faces split along the fractures, ``fracture_faces`` tag), ``data``:
     ``parameters[keyword]`` with ``fourth_order_tensor`` and the vectorial ``bc`` (fracture faces Dirichlet,
     ``internal_to_dirichlet``); ``bc_values``: nd nf face-major (displacement / traction); ``fractures``: list of
@@ -161,15 +179,14 @@ class FracturedMomentumBalance:
         self.k = SimpleNamespace(**{k: float(v) for k, v in constants.items()})
         self.nc, self.nf = int(sd.num_cells), int(sd.num_faces)
         self.body_force = np.zeros(nd * self.nc) if body_force is None else np.asarray(body_force, float)
-        nt = [nd * f.num_cells for f in self.fractures]
-        nj = [nd * f.num_mortar for f in self.fractures]
-        self.sizes = [nd * self.nc] + nt + nj
-        self.offsets = np.concatenate(([0], np.cumsum(self.sizes))).astype(np.int64)
+        fr, mat = self.fractures, [(("matrix",), self.nc, nd)]
+        self.unknown_layout = BlockLayout([("displacement", mat), ("contact_traction", fracture_parts(fr, nd)),
+                                           ("interface_displacement", interface_parts(fr, nd))])
+        self.equation_layout = BlockLayout([
+            ("momentum_balance_equation", mat), ("interface_force_balance_equation", interface_parts(fr, nd)),
+            ("normal_fracture_deformation_equation", fracture_parts(fr, 1)),
+            ("tangential_fracture_deformation_equation", fracture_parts(fr, nd - 1))])
         self._const = None
-
-    @property
-    def num_dofs(self) -> int:
-        return int(self.offsets[-1])
 
     def discretize(self) -> None:
         Mpsa(self.kw).discretize(self.sd, self.data)
@@ -197,9 +214,9 @@ class FracturedMomentumBalance:
         k, c = self._operands(), self.k
         nfr = len(self.fractures)
         x, x_prev = ad.device_vector(x), ad.device_vector(x_prev)
-        var = ad.variables([x[self.offsets[q]:self.offsets[q + 1]] for q in range(len(self.sizes))])
-        u, t, uj = var[0], var[1:1 + nfr], var[1 + nfr:]
-        ujn = [x_prev[self.offsets[1 + nfr + j]:self.offsets[2 + nfr + j]] for j in range(nfr)]
+        var = self.unknown_layout.variables(x)
+        u, t, uj = var["displacement"][0], var["contact_traction"], var["interface_displacement"]
+        ujn = self.unknown_layout.parts(x_prev)["interface_displacement"]
         boundary = None
         for j in range(nfr):
             term = k.fr[j].m2p @ uj[j]
@@ -215,26 +232,17 @@ class FracturedMomentumBalance:
             nrm, tan = contact_laws(q, t[j], uj[j], ujn[j], c)
             normal.append(nrm)
             tangential.append(tan)
-        return [momentum] + force + normal + tangential
+        return self.equation_layout.stack({
+            "momentum_balance_equation": [momentum], "interface_force_balance_equation": force,
+            "normal_fracture_deformation_equation": normal, "tangential_fracture_deformation_equation": tangential})
 
-    def preconditioner_groups(self):
-        """Groups of the grouped block-Jacobi preconditioner of ``krylov.gmres`` in this problem's ordering: per matrix
-        cell c, momentum_c <-> u_c (nd); per fracture cell k with mortar cells m1, m2, the normal and tangential laws of k
-        and the force balances of m1, m2 <-> t_k, u_j of m1, m2 (3 nd: 9 in 3-D, 6 in 2-D)."""
-        nfr, nc, nd = len(self.fractures), self.nc, self.nd
-        eq = np.concatenate(([0], np.cumsum([nd * nc] + [nd * f.num_mortar for f in self.fractures]
-                                            + [f.num_cells for f in self.fractures]
-                                            + [(nd - 1) * f.num_cells for f in self.fractures])))
-        cells = np.arange(nc)
-        blocks = [(span(eq[0], cells, nd), span(self.offsets[0], cells, nd))]
-        for j, fc in enumerate(self.fractures):
-            pair, k = mortar_pairs(fc.mortar_to_secondary), np.arange(fc.num_cells)
-            frc, jmp = eq[1 + j], self.offsets[1 + nfr + j]
-            rows = [span(eq[1 + nfr + j], k, 1), span(eq[1 + 2 * nfr + j], k, nd - 1), span(frc, pair[:, 0], nd),
-                    span(frc, pair[:, 1], nd)]
-            cols = [span(self.offsets[1 + j], k, nd), span(jmp, pair[:, 0], nd), span(jmp, pair[:, 1], nd)]
-            blocks.append((np.hstack(rows), np.hstack(cols)))
-        return block_groups(blocks)
+    # ``preconditioner_groups()``: momentum_c <-> u_c (nd) per matrix cell c; the normal and tangential laws of fracture
+    # cell k and the force balances of its mortar cells m1, m2 <-> t_k, u_j of m1, m2 (3 nd: 9 in 3-D, 6 in 2-D)
+    matrix_group = ([("momentum_balance_equation", "c")], [("displacement", "c")])
+    fracture_group = ([("normal_fracture_deformation_equation", "k"), ("tangential_fracture_deformation_equation", "k"),
+                       ("interface_force_balance_equation", "m1"), ("interface_force_balance_equation", "m2")],
+                      [("contact_traction", "k"), ("interface_displacement", "m1"), ("interface_displacement", "m2")])
+    preconditioner_groups = block_groups
 
     def linearize(self, x, x_prev):
         """(J as ``DeviceCsr``, -R as a CUDA tensor) at the iterate ``x`` (previous time step ``x_prev``)."""

@@ -18,9 +18,8 @@ Couplings on top of ``porepy_b200.poromech`` (matrix), ``mdflow_nl`` (fracture f
 As in the reference's Newton loop (``Poromechanics.add_nonlinear_darcy_flux_discretization``, models/poromechanics.py), the
 fracture flux is RE-DISCRETIZED in front of every linearization with the tangential permeability times the current
 aperture (``operator_to_SecondOrderTensor``: the specific volume of the iterate; not differentiated), next to the
-upwinding.  Unknowns: [p matrix | p fractures | u | contact tractions | lambda | u_j]; equations:
-[mass matrix | mass fractures | momentum | Darcy laws | force balances | normal laws | tangential laws] (the fixtures carry
-the maps to the reference's numbering).  One matrix subdomain, fractures without intersections; saddle-point Jacobian: the
+upwinding.  Unknowns and equations: ``unknown_layout``, ``equation_layout`` (the fixtures carry the maps to the
+reference's numbering).  One matrix subdomain, fractures without intersections; saddle-point Jacobian: the
 linear solver of ``time_step`` is the caller's; ``krylov.gmres_solver(prob.preconditioner_groups())`` is the device one.  ``tests/golden/contact_poromech*.npz`` pin Jacobian, residual, the residual
 history of the semismooth Newton loop and the converged state, ``contact_poromech_2d.npz`` the same on a line fracture.
 """
@@ -33,8 +32,10 @@ import scipy.sparse as sps
 
 from . import ad, ad_functions as fn
 from .advection import advective_flux, rediscretize_upwind, rediscretize_upwind_coupling
-from .contact import block_groups, contact_laws, contact_operators, local_dimension, matrix_dimension, mortar_pairs, span
+from .contact import (block_groups, contact_laws, contact_operators, fracture_parts, interface_parts, local_dimension,
+                      matrix_dimension)
 from .fv import Biot, Mpfa
+from .layout import BlockLayout, LayoutModel
 from .newton import newton_loop
 from .params import DISCRETIZATION_MATRICES, PARAMETERS
 
@@ -55,6 +56,7 @@ class FractureCoupling:
         self.bc = bc
         self.k_intrinsic = np.asarray(intrinsic_permeability, float)
         self.p = {k: sps.csr_matrix(v) for k, v in projections.items()}
+        self.mortar_to_secondary = self.p["mortar_to_secondary_avg"]
         self.sign = np.asarray(mortar_sign, float)
         self.volumes = np.asarray(mortar_volumes, float)
         self.rotation = sps.csr_matrix(local_coordinates)
@@ -63,7 +65,7 @@ class FractureCoupling:
         self.nd = local_dimension(self.rotation, self.num_cells)
 
 
-class FracturedPoromechanics:
+class FracturedPoromechanics(LayoutModel):
     """``sd`` / ``data``: the 2-D or 3-D matrix grid (fracture faces split) with ``parameters[flow_keyword]`` and
     ``parameters[mechanics_keyword]`` (``scalar_vector_mappings`` = {flow_keyword: Biot coefficient}).  ``bc``: dict of face
     arrays ``flow``, ``mechanics`` (nd nf), ``fluid_flux`` and the object ``fluid_flux_type``.  ``fluid``: ``compressibility,
@@ -86,16 +88,19 @@ class FracturedPoromechanics:
         self.ct = SimpleNamespace(**{k: float(v) for k, v in contact.items()})
         self.bc = bc
         self.nc, self.nf = int(sd.num_cells), int(sd.num_faces)
-        nfc = [f.num_cells for f in self.fractures]
-        nm = [f.num_mortar for f in self.fractures]
-        self.sizes = [self.nc] + nfc + [nd * self.nc] + [nd * n for n in nfc] + nm + [nd * n for n in nm]
-        self.offsets = np.concatenate(([0], np.cumsum(self.sizes))).astype(np.int64)
+        fr = self.fractures
+        scalar, vector = [(("matrix",), self.nc, 1)] + fracture_parts(fr, 1), [(("matrix",), self.nc, nd)]
+        flux, mortar = interface_parts(fr, 1), interface_parts(fr, nd)
+        self.unknown_layout = BlockLayout([
+            ("pressure", scalar), ("displacement", vector), ("contact_traction", fracture_parts(fr, nd)),
+            ("interface_darcy_flux", flux), ("interface_displacement", mortar)])
+        self.equation_layout = BlockLayout([
+            ("mass_balance_equation", scalar), ("momentum_balance_equation", vector),
+            ("interface_darcy_flux_equation", flux), ("interface_force_balance_equation", mortar),
+            ("normal_fracture_deformation_equation", fracture_parts(fr, 1)),
+            ("tangential_fracture_deformation_equation", fracture_parts(fr, nd - 1))])
         self._intf_data = [{} for _ in self.fractures]
         self._const = None
-
-    @property
-    def num_dofs(self) -> int:
-        return int(self.offsets[-1])
 
     def _discretize_fracture(self, fc, aperture) -> None:
         from .params import SecondOrderTensor
@@ -184,23 +189,12 @@ class FracturedPoromechanics:
     def _aperture(self, uj_j, q):
         return fn.maximum((q.sel_n @ (q.jump @ uj_j)) + self.so.residual_aperture, self.so.residual_aperture)
 
-    def _group(self, parts):
-        n = len(self.fractures)
-        return parts[0], parts[1:1 + n], parts[1 + n], parts[2 + n:2 + 2 * n], parts[2 + 2 * n:2 + 3 * n], parts[2 + 3 * n:]
-
-    def _parts(self, x):
-        return self._group([x[self.offsets[q]:self.offsets[q + 1]] for q in range(len(self.sizes))])
-
-    def _flow_parts(self, x):
-        """(p matrix, p fractures, lambda, u_j) of ``x``: what the discretizations follow."""
-        p3, pf, _, _, lam, uj = self._parts(x)
-        return p3, pf, lam, uj
-
     def update_discretizations(self, x) -> None:
         """What follows the iterate: the fracture flux discretization (aperture) and every upwind direction."""
         x = ad.device_vector(x)
         k = self._operands()
-        p3, pf, lam, uj = self._flow_parts(x)
+        parts = self.unknown_layout.parts(x)
+        (p3, *pf), lam, uj = parts["pressure"], parts["interface_darcy_flux"], parts["interface_displacement"]
         for j, fc in enumerate(self.fractures):
             self._discretize_fracture(fc, self._aperture(uj[j], k.fr[j]).cpu().numpy())
         b = k.bcq
@@ -223,9 +217,10 @@ class FracturedPoromechanics:
         nfr = len(self.fractures)
         mk = self.mobility_keyword
         x, x_prev = ad.device_vector(x), ad.device_vector(x_prev)
-        var = ad.variables([x[self.offsets[q]:self.offsets[q + 1]] for q in range(len(self.sizes))])
-        p3, pf, u, t, lam, uj = self._group(var)
-        p3n, pfn, un, _, _, ujn = self._parts(x_prev)
+        var, prev = self.unknown_layout.variables(x), self.unknown_layout.parts(x_prev)
+        (p3, *pf), (u,), t = var["pressure"], var["displacement"], var["contact_traction"]
+        lam, uj = var["interface_darcy_flux"], var["interface_displacement"]
+        (p3n, *pfn), (un,), ujn = prev["pressure"], prev["displacement"], prev["interface_displacement"]
         w3 = self._density(p3) * (1.0 / fl.viscosity)
         wf = [self._density(pf[j]) * (1.0 / fl.viscosity) for j in range(nfr)]
         # interface mass fluxes, boundary operators of the matrix
@@ -265,33 +260,22 @@ class FracturedPoromechanics:
             nrm, tan = contact_laws(q, t[j], uj[j], ujn[j], ct)
             normal.append(nrm)
             tangential.append(tan)
-        return [mass3] + mass_f + [momentum] + darcy + force + normal + tangential
+        return self.equation_layout.stack({
+            "mass_balance_equation": [mass3] + mass_f, "momentum_balance_equation": [momentum],
+            "interface_darcy_flux_equation": darcy, "interface_force_balance_equation": force,
+            "normal_fracture_deformation_equation": normal, "tangential_fracture_deformation_equation": tangential})
 
-    def _equation_offsets(self) -> np.ndarray:
-        nc, nfc, nm, nd = self.nc, [f.num_cells for f in self.fractures], [f.num_mortar for f in self.fractures], self.nd
-        sizes = [nc] + nfc + [nd * nc] + nm + [nd * n for n in nm] + nfc + [(nd - 1) * n for n in nfc]
-        return np.concatenate(([0], np.cumsum(sizes))).astype(np.int64)
-
-    def preconditioner_groups(self):
-        """Groups of the grouped block-Jacobi preconditioner of ``krylov.gmres`` in this problem's ordering: per matrix
-        cell c, mass_c and momentum_c <-> p_c, u_c (nd + 1); per fracture cell k with mortar cells m1, m2, the contact
-        laws of k, the force balances of m1, m2, the fracture mass balance of k and the Darcy laws of m1, m2 <-> t_k, u_j
-        of m1, m2, p_f of k, lambda of m1, m2 (3 nd + 3: 12 in 3-D, 9 in 2-D)."""
-        nfr, eq, var, nd = len(self.fractures), self._equation_offsets(), self.offsets, self.nd
-        cells = np.arange(self.nc)
-        blocks = [(np.hstack([span(eq[0], cells, 1), span(eq[1 + nfr], cells, nd)]),
-                   np.hstack([span(var[0], cells, 1), span(var[1 + nfr], cells, nd)]))]
-        for j, fc in enumerate(self.fractures):
-            pair, k = mortar_pairs(fc.p["mortar_to_secondary_avg"]), np.arange(fc.num_cells)
-            m1, m2 = pair[:, 0], pair[:, 1]
-            frc, darcy = eq[2 + 2 * nfr + j], eq[2 + nfr + j]
-            rows = [span(eq[2 + 3 * nfr + j], k, 1), span(eq[2 + 4 * nfr + j], k, nd - 1), span(frc, m1, nd), span(frc, m2, nd),
-                    span(eq[1 + j], k, 1), span(darcy, m1, 1), span(darcy, m2, 1)]
-            jmp, lam = var[2 + 3 * nfr + j], var[2 + 2 * nfr + j]
-            cols = [span(var[2 + nfr + j], k, nd), span(jmp, m1, nd), span(jmp, m2, nd), span(var[1 + j], k, 1),
-                    span(lam, m1, 1), span(lam, m2, 1)]
-            blocks.append((np.hstack(rows), np.hstack(cols)))
-        return block_groups(blocks)
+    # ``preconditioner_groups()``: nd + 1 unknowns per matrix cell c; per fracture cell k, those of ``contact`` plus the
+    # fracture mass balance of k and the Darcy laws of its mortar cells (3 nd + 3: 12 in 3-D, 9 in 2-D)
+    matrix_group = ([("mass_balance_equation", "c"), ("momentum_balance_equation", "c")],
+                    [("pressure", "c"), ("displacement", "c")])
+    fracture_group = ([("normal_fracture_deformation_equation", "k"), ("tangential_fracture_deformation_equation", "k"),
+                       ("interface_force_balance_equation", "m1"), ("interface_force_balance_equation", "m2"),
+                       ("mass_balance_equation", "k"), ("interface_darcy_flux_equation", "m1"),
+                       ("interface_darcy_flux_equation", "m2")],
+                      [("contact_traction", "k"), ("interface_displacement", "m1"), ("interface_displacement", "m2"),
+                       ("pressure", "k"), ("interface_darcy_flux", "m1"), ("interface_darcy_flux", "m2")])
+    preconditioner_groups = block_groups
 
     def linearize(self, x, x_prev, dt: float):
         self.update_discretizations(x)

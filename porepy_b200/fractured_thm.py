@@ -13,12 +13,12 @@ fracture's internal energy and in the interface Fourier law:
                          flux (measured on the reference: both flux matrices x 1.002 at the second iterate); the matrix's
                          flux matrices stay those of the initial state.
 
-Unknowns: [p matrix | p fractures | T matrix | T fractures | u | contact tractions | lambda | eta | eps | u_j]; equations:
-[mass matrix | mass fractures | energy matrix | energy fractures | momentum | Darcy laws | Fourier laws | enthalpy laws |
-force balances | normal laws | tangential laws].  ``tests/golden/contact_thm*.npz`` pin the Jacobian at the zero state and at
-the fourth Newton iterate, the residual history of the semismooth Newton loop and the converged state.  The Newton updates
-are solved on the device by ``krylov.gmres_solver(prob.preconditioner_groups())`` (3 nd + 8 unknowns per fracture-cell
-group: 17 in 3-D, 14 in 2-D).  A 2-D matrix with line fractures is handled as the 3-D one (``contact_thm_2d.npz``).
+Unknowns and equations: those of ``FracturedPoromechanics`` with the temperatures, the interface Fourier and enthalpy
+fluxes and their equations inserted (``unknown_layout``, ``equation_layout``).  ``tests/golden/contact_thm*.npz`` pin
+the Jacobian at the zero state and at the fourth Newton iterate, the residual history of the semismooth Newton loop and
+the converged state.  The Newton updates are solved on the device by ``krylov.gmres_solver(prob.preconditioner_groups())``
+(3 nd + 8 unknowns per fracture-cell group: 17 in 3-D, 14 in 2-D).  A 2-D matrix with line fractures is handled as the
+3-D one (``contact_thm_2d.npz``).
 """
 from __future__ import annotations
 
@@ -26,7 +26,7 @@ import numpy as np
 
 from . import ad
 from .advection import advective_flux
-from .contact import block_groups, contact_laws, mortar_pairs, span
+from .contact import contact_laws, fracture_parts, interface_parts
 from .fractured_poromech import FracturedPoromechanics
 from .fv import Mpfa
 from .params import DISCRETIZATION_MATRICES, PARAMETERS, SecondOrderTensor
@@ -48,43 +48,25 @@ class FracturedThermoporomechanics(FracturedPoromechanics):
         super().__init__(sd, data, fractures, fluid, solid, contact, bc, flow_keyword, mechanics_keyword)
         self.tk, self.ck = fourier_keyword, thermal_keyword
         self.kappa_t = [np.asarray(v, float) for v in normal_thermal_conductivity]
-        nfc = [f.num_cells for f in self.fractures]
-        nm = [f.num_mortar for f in self.fractures]
-        nd = self.nd
-        self.sizes = [self.nc] + nfc + [self.nc] + nfc + [nd * self.nc] + [nd * n for n in nfc] + nm + nm + nm + [nd * n for n in nm]
-        self.offsets = np.concatenate(([0], np.cumsum(self.sizes))).astype(np.int64)
+        scalar = [(("matrix",), self.nc, 1)] + fracture_parts(self.fractures, 1)
+        flux = interface_parts(self.fractures, 1)
+        self.unknown_layout = self.unknown_layout.insert("pressure", [("temperature", scalar)]).insert(
+            "interface_darcy_flux", [("interface_fourier_flux", flux), ("interface_enthalpy_flux", flux)])
+        self.equation_layout = self.equation_layout.insert("mass_balance_equation", [("energy_balance_equation", scalar)]
+                                                           ).insert("interface_darcy_flux_equation", [
+            ("interface_fourier_flux_equation", flux), ("interface_enthalpy_flux_equation", flux)])
 
-    def preconditioner_groups(self):
-        """Groups of the grouped block-Jacobi preconditioner of ``krylov.gmres`` in this problem's ordering: per matrix
-        cell c, mass_c, energy_c and momentum_c <-> p_c, T_c, u_c (nd + 2); per fracture cell k with mortar cells m1, m2,
-        the 3 nd + 3 rows and columns of ``FracturedPoromechanics.preconditioner_groups`` plus the fracture energy balance
-        of k and the Fourier and enthalpy laws of m1, m2 <-> T_f of k, eta and eps of m1, m2 (3 nd + 8: 17 in 3-D, 14 in
-        2-D)."""
-        n, var, nd = len(self.fractures), self.offsets, self.nd
-        nc, nfc, nm = self.nc, [f.num_cells for f in self.fractures], [f.num_mortar for f in self.fractures]
-        sizes = [nc] + nfc + [nc] + nfc + [nd * nc] + nm + nm + nm + [nd * m for m in nm] + nfc + [(nd - 1) * f for f in nfc]
-        eq = np.concatenate(([0], np.cumsum(sizes))).astype(np.int64)
-        # equation groups: mass | mass_f | energy | energy_f | momentum | darcy | fourier | enthalpy | force | normal |
-        # tangential; variable groups: p | p_f | T | T_f | u | t | lambda | eta | eps | u_j
-        e_mass, e_massf, e_en, e_enf, e_mom = 0, 1, 1 + n, 2 + n, 2 + 2 * n
-        e_darcy, e_four, e_enth, e_force, e_nrm, e_tan = (3 + 2 * n + q * n for q in range(6))
-        v_p, v_pf, v_t, v_tf, v_u = 0, 1, 1 + n, 2 + n, 2 + 2 * n
-        v_trac, v_lam, v_eta, v_eps, v_jmp = (3 + 2 * n + q * n for q in range(5))
-        cells = np.arange(nc)
-        blocks = [(np.hstack([span(eq[e_mass], cells, 1), span(eq[e_en], cells, 1), span(eq[e_mom], cells, nd)]),
-                   np.hstack([span(var[v_p], cells, 1), span(var[v_t], cells, 1), span(var[v_u], cells, nd)]))]
-        for j, fc in enumerate(self.fractures):
-            pair, k = mortar_pairs(fc.p["mortar_to_secondary_avg"]), np.arange(fc.num_cells)
-            m1, m2 = pair[:, 0], pair[:, 1]
-            pair_rows = lambda off, w: [span(off, m1, w), span(off, m2, w)]  # noqa: E731
-            rows = [span(eq[e_nrm + j], k, 1), span(eq[e_tan + j], k, nd - 1), *pair_rows(eq[e_force + j], nd),
-                    span(eq[e_massf + j], k, 1), *pair_rows(eq[e_darcy + j], 1),
-                    span(eq[e_enf + j], k, 1), *pair_rows(eq[e_four + j], 1), *pair_rows(eq[e_enth + j], 1)]
-            cols = [span(var[v_trac + j], k, nd), *pair_rows(var[v_jmp + j], nd),
-                    span(var[v_pf + j], k, 1), *pair_rows(var[v_lam + j], 1),
-                    span(var[v_tf + j], k, 1), *pair_rows(var[v_eta + j], 1), *pair_rows(var[v_eps + j], 1)]
-            blocks.append((np.hstack(rows), np.hstack(cols)))
-        return block_groups(blocks)
+    # ``preconditioner_groups()``: nd + 2 unknowns per matrix cell; per fracture cell k, those of ``FracturedPoromechanics``
+    # plus the fracture energy balance of k and the Fourier and enthalpy laws of its mortar cells (3 nd + 8: 17 in 3-D)
+    matrix_group = ([("mass_balance_equation", "c"), ("energy_balance_equation", "c"),
+                     ("momentum_balance_equation", "c")], [("pressure", "c"), ("temperature", "c"), ("displacement", "c")])
+    fracture_group = (FracturedPoromechanics.fracture_group[0] + [
+                          ("energy_balance_equation", "k"), ("interface_fourier_flux_equation", "m1"),
+                          ("interface_fourier_flux_equation", "m2"), ("interface_enthalpy_flux_equation", "m1"),
+                          ("interface_enthalpy_flux_equation", "m2")],
+                      FracturedPoromechanics.fracture_group[1] + [
+                          ("temperature", "k"), ("interface_fourier_flux", "m1"), ("interface_fourier_flux", "m2"),
+                          ("interface_enthalpy_flux", "m1"), ("interface_enthalpy_flux", "m2")])
 
     # ---- discretizations
     def _matrix_conductivity(self):
@@ -130,20 +112,6 @@ class FracturedThermoporomechanics(FracturedPoromechanics):
         return super()._porosity(p, u, uj, k) \
             - (t - self.fl.reference_temperature) * ((so.biot_coefficient - so.reference_porosity) * so.thermal_expansion)
 
-    def _group(self, parts):
-        n = len(self.fractures)
-        i = 0
-        out = []
-        for size in (1, n, 1, n, 1, n, n, n, n, n):
-            out.append(parts[i:i + size])
-            i += size
-        p3, pf, t3, tf, u, t, lam, eta, eps, uj = out
-        return p3[0], pf, t3[0], tf, u[0], t, lam, eta, eps, uj
-
-    def _flow_parts(self, x):
-        p3, pf, _, _, _, _, lam, _, _, uj = self._parts(x)
-        return p3, pf, lam, uj
-
     def _upwind_keywords(self):
         return super()._upwind_keywords() + [(self.enthalpy_upwind_keyword, "enthalpy_flux_type")]
 
@@ -153,9 +121,12 @@ class FracturedThermoporomechanics(FracturedPoromechanics):
         nfr = len(self.fractures)
         mk, ek = self.mobility_keyword, self.enthalpy_upwind_keyword
         x, x_prev = ad.device_vector(x), ad.device_vector(x_prev)
-        var = ad.variables([x[self.offsets[q]:self.offsets[q + 1]] for q in range(len(self.sizes))])
-        p3, pf, t3, tf, u, t, lam, eta, eps, uj = self._group(var)
-        p3n, pfn, t3n, tfn, un, _, _, _, _, ujn = self._parts(x_prev)
+        var, prev = self.unknown_layout.variables(x), self.unknown_layout.parts(x_prev)
+        (p3, *pf), (t3, *tf), (u,) = var["pressure"], var["temperature"], var["displacement"]
+        lam, eta, eps = var["interface_darcy_flux"], var["interface_fourier_flux"], var["interface_enthalpy_flux"]
+        t, uj = var["contact_traction"], var["interface_displacement"]
+        (p3n, *pfn), (t3n, *tfn), (un,) = prev["pressure"], prev["temperature"], prev["displacement"]
+        ujn = prev["interface_displacement"]
         t0 = fl.reference_temperature
 
         def weights(p, tt):
@@ -221,4 +192,9 @@ class FracturedThermoporomechanics(FracturedPoromechanics):
             nrm, tan = contact_laws(q, t[j], uj[j], ujn[j], self.ct)
             normal.append(nrm)
             tangential.append(tan)
-        return [mass3] + mass_f + [energy3] + energy_f + [momentum] + darcy + fourier + enthalpy + force + normal + tangential
+        return self.equation_layout.stack({
+            "mass_balance_equation": [mass3] + mass_f, "energy_balance_equation": [energy3] + energy_f,
+            "momentum_balance_equation": [momentum], "interface_darcy_flux_equation": darcy,
+            "interface_fourier_flux_equation": fourier, "interface_enthalpy_flux_equation": enthalpy,
+            "interface_force_balance_equation": force, "normal_fracture_deformation_equation": normal,
+            "tangential_fracture_deformation_equation": tangential})

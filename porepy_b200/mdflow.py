@@ -31,6 +31,7 @@ import scipy.sparse as sps
 
 from . import ad
 from .fv import Mpfa
+from .layout import BlockLayout, LayoutModel
 from .params import DISCRETIZATION_MATRICES
 
 
@@ -71,24 +72,21 @@ class MdInterface:
                 * 2.0 * (s2m @ (1.0 / np.asarray(self.secondary_aperture, float))))
 
 
-class MixedDimensionalFlow:
+class MixedDimensionalFlow(LayoutModel):
     """Discretize and assemble the mixed-dimensional Darcy problem; see the module docstring."""
 
     def __init__(self, subdomains, interfaces, keyword: str = "flow"):
         self.subdomains = list(subdomains)
         self.interfaces = list(interfaces)
         self.keyword = keyword
-        sizes = [int(s.sd.num_cells) for s in self.subdomains] + [i.num_cells for i in self.interfaces]
-        self.sizes = sizes
-        self.offsets = np.concatenate(([0], np.cumsum(sizes))).astype(np.int64)
+        sub = [(("subdomain", i), int(s.sd.num_cells), 1) for i, s in enumerate(self.subdomains)]
+        intf = [(("interface", j), it.num_cells, 1) for j, it in enumerate(self.interfaces)]
+        self.unknown_layout = BlockLayout([("pressure", sub), ("interface_darcy_flux", intf)])
+        self.equation_layout = BlockLayout([("mass_balance_equation", sub), ("interface_darcy_flux_equation", intf)])
         for it in self.interfaces:
             h, l = self.subdomains[it.primary].sd, self.subdomains[it.secondary].sd
             if h.dim != l.dim + 1:
                 raise ValueError("interfaces couple subdomains one dimension apart")
-
-    @property
-    def num_dofs(self) -> int:
-        return int(self.offsets[-1])
 
     @property
     def num_cells(self) -> int:
@@ -156,8 +154,8 @@ class MixedDimensionalFlow:
         if x is None:
             x = torch.zeros(self.num_dofs, dtype=torch.float64, device="cuda")
         x = ad.device_vector(x)
-        var = ad.variables([x[self.offsets[k]:self.offsets[k + 1]] for k in range(len(self.sizes))])
-        p, lam = var[:nsd], var[nsd:]
+        var = self.unknown_layout.variables(x)
+        p, lam = var["pressure"], var["interface_darcy_flux"]
         as_primary = [[] for _ in range(nsd)]
         as_secondary = [[] for _ in range(nsd)]
         for j, it in enumerate(self.interfaces):
@@ -165,7 +163,7 @@ class MixedDimensionalFlow:
             as_secondary[it.secondary].append(j)
         def mm(m, v):
             return ad.as_device_csr(m) @ v          # DeviceAdArray: SpMV + SpGEMM; tensor: SpMV
-        eqs, boundary = [], [None] * nsd
+        mass, darcy, boundary = [], [], [None] * nsd
         for i, s in enumerate(self.subdomains):
             eq = None
             if s.sd.num_faces > 0:
@@ -181,13 +179,13 @@ class MixedDimensionalFlow:
                 eq = -t if eq is None else eq - t
             if eq is None:
                 raise ValueError("a subdomain without faces and without interfaces has no equation")
-            eqs.append(eq - ad.device_vector(self._source(i)))
+            mass.append(eq - ad.device_vector(self._source(i)))
         for j, it in enumerate(self.interfaces):
             M = self._matrices(it.primary)
             tr = mm(M["bound_pressure_cell"], p[it.primary]) + mm(M["bound_pressure_face"], boundary[it.primary])
             jump = mm(it.primary_to_mortar_avg, tr) - mm(it.secondary_to_mortar_avg, p[it.secondary])
-            eqs.append(lam[j] - jump * ad.device_vector(it.coefficient()))
-        return eqs
+            darcy.append(lam[j] - jump * ad.device_vector(it.coefficient()))
+        return self.equation_layout.stack({"mass_balance_equation": mass, "interface_darcy_flux_equation": darcy})
 
     def assemble_ad(self, x=None):
         """(Jacobian ``DeviceCsr``, right-hand side ``-residual`` CUDA tensor) by the reference's own evaluation order:
@@ -217,9 +215,9 @@ class MixedDimensionalFlow:
         from .params import PARAMETERS
         nsd = len(self.subdomains)
         csr, dev, D = ad.as_device_csr, ad.device_vector, ad.DeviceCsr
-        nm = int(self.offsets[-1] - self.offsets[nsd])
-        lam0 = self.offsets[nsd:] - self.offsets[nsd]            # start of every interface inside the interface block
-        bsizes = self.sizes[:nsd] + [nm]
+        lam0 = self.unknown_layout.offsets[nsd:] - self.unknown_layout.offsets[nsd]   # interfaces in the interface block
+        nm = int(lam0[-1])
+        bsizes = [n * w for _, _, n, w in self.unknown_layout.items()[:nsd]] + [nm]
         n = nsd + (1 if self.interfaces else 0)
         blocks = [[None] * n for _ in range(n)]
         rhs = [None] * n
@@ -318,10 +316,10 @@ class MixedDimensionalFlow:
 
     # ---- host restatement with scipy (the checker of the tests; materialises the discretization matrices)
     def assemble_host(self):
-        n = len(self.sizes)
-        nsd = len(self.subdomains)
+        sizes, nsd = np.diff(self.unknown_layout.offsets), len(self.subdomains)
+        n = len(sizes)
         blocks = [[None] * n for _ in range(n)]
-        rhs = [np.zeros(k) for k in self.sizes]
+        rhs = [np.zeros(k) for k in sizes]
 
         def add(i, j, m):
             blocks[i][j] = m if blocks[i][j] is None else blocks[i][j] + m
@@ -350,14 +348,13 @@ class MixedDimensionalFlow:
         for i in range(n):
             for j in range(n):
                 if blocks[i][j] is None:
-                    blocks[i][j] = sps.csr_matrix((self.sizes[i], self.sizes[j]))
+                    blocks[i][j] = sps.csr_matrix((sizes[i], sizes[j]))
         return sps.bmat(blocks, format="csr"), np.concatenate(rhs)
 
     def split(self, x):
         """(pressures per subdomain, interface fluxes per interface) of a global vector."""
-        x = np.asarray(x)
-        parts = [x[self.offsets[k]:self.offsets[k + 1]] for k in range(len(self.sizes))]
-        return parts[:len(self.subdomains)], parts[len(self.subdomains):]
+        parts = self.unknown_layout.parts(np.asarray(x))
+        return parts["pressure"], parts["interface_darcy_flux"]
 
 
 def schur_solve(A, B, E, Dm, bp, bl, tol: float = 1e-8, maxiter: int = 4000, sweeps: int | None = None):

@@ -82,9 +82,9 @@ class CompressibleMixedDimensionalFlow(MixedDimensionalFlow):
     # ---- upwind directions from the current iterate (the reference's rediscretization in front of every iteration)
     def update_upwind(self, x) -> None:
         x = ad.device_vector(x)
-        nsd = len(self.subdomains)
         k = self._operands()
-        parts = [x[self.offsets[q]:self.offsets[q + 1]] for q in range(len(self.sizes))]
+        parts = self.unknown_layout.parts(x)
+        p, lam = parts["pressure"], parts["interface_darcy_flux"]
         mk = self.mobility_keyword
         for i, s in enumerate(self.subdomains):
             if s.sd.num_faces == 0:
@@ -92,14 +92,14 @@ class CompressibleMixedDimensionalFlow(MixedDimensionalFlow):
             b = k.bcv[i]
             for j, it in enumerate(self.interfaces):
                 if it.primary == i:
-                    b = b + (k.m2p[j] @ parts[nsd + j])
+                    b = b + (k.m2p[j] @ lam[j])
             M = self._matrices(i)
-            q = (ad.as_device_csr(M["flux"]) @ parts[i]) + (ad.as_device_csr(M["bound_flux"]) @ b)
+            q = (ad.as_device_csr(M["flux"]) @ p[i]) + (ad.as_device_csr(M["bound_flux"]) @ b)
             rediscretize_upwind(s.sd, s.data, mk, q.cpu().numpy(), self.bc_fluid_flux[i])
         for j, it in enumerate(self.interfaces):
             h, l = self.subdomains[it.primary], self.subdomains[it.secondary]
             rediscretize_upwind_coupling(h.sd, l.sd, it.num_cells, h.data, l.data, self._intf_data[j], mk,
-                                         parts[nsd + j].cpu().numpy())
+                                         lam[j].cpu().numpy())
 
     # ---- value and Jacobian of every equation at x (previous time step: x_prev)
     def equations(self, x, x_prev=None, dt: float = 1.0) -> list:
@@ -109,8 +109,9 @@ class CompressibleMixedDimensionalFlow(MixedDimensionalFlow):
         k = self._operands()
         csr = ad.as_device_csr
         x, x_prev = ad.device_vector(x), ad.device_vector(x_prev)
-        var = ad.variables([x[self.offsets[q]:self.offsets[q + 1]] for q in range(len(self.sizes))])
-        p, lam = var[:nsd], var[nsd:]
+        var = self.unknown_layout.variables(x)
+        p, lam = var["pressure"], var["interface_darcy_flux"]
+        pn = self.unknown_layout.parts(x_prev)["pressure"]
         mk = self.mobility_keyword
         w = [self._density(pi) * (1.0 / self.mu) for pi in p]                    # rho / mu, cell-wise
         # interface mass fluxes
@@ -120,9 +121,9 @@ class CompressibleMixedDimensionalFlow(MixedDimensionalFlow):
             up = (csr(U["upwind_primary"]) @ (k.p2m[j] @ (k.trace[it.primary] @ w[it.primary])))
             us = (csr(U["upwind_secondary"]) @ (k.s2m[j] @ w[it.secondary]))
             ifl.append(lam[j] * (up + us))
-        eqs, boundary = [], [None] * nsd
+        mass, darcy, boundary = [], [], [None] * nsd
         for i, s in enumerate(self.subdomains):
-            rho_prev = self._density(x_prev[self.offsets[i]:self.offsets[i + 1]])
+            rho_prev = self._density(pn[i])
             eq = (w[i] * self.mu - rho_prev) * (k.sto[i] * (1.0 / dt))
             if s.sd.num_faces > 0:
                 b, mass_in = None, None
@@ -143,13 +144,13 @@ class CompressibleMixedDimensionalFlow(MixedDimensionalFlow):
             for j, it in enumerate(self.interfaces):
                 if it.secondary == i:
                     eq = eq - (k.m2s[j] @ ifl[j])
-            eqs.append(eq - k.src[i])
+            mass.append(eq - k.src[i])
         for j, it in enumerate(self.interfaces):
             M = self._matrices(it.primary)
             tr = (csr(M["bound_pressure_cell"]) @ p[it.primary]) + (csr(M["bound_pressure_face"]) @ boundary[it.primary])
             jump = (k.p2m[j] @ tr) - (k.s2m[j] @ p[it.secondary])
-            eqs.append(lam[j] - jump * k.coef[j])
-        return eqs
+            darcy.append(lam[j] - jump * k.coef[j])
+        return self.equation_layout.stack({"mass_balance_equation": mass, "interface_darcy_flux_equation": darcy})
 
     def linearize(self, x, x_prev, dt: float):
         """(J, -R) at the iterate ``x``: upwind directions from ``x``, then the AD evaluation."""
@@ -159,13 +160,12 @@ class CompressibleMixedDimensionalFlow(MixedDimensionalFlow):
     def time_step(self, x_prev, dt: float, tol: float = 1e-10, max_iterations: int = 15, linear_tol: float = 1e-10,
                   verbose: bool = False):
         """One implicit time step by Newton's method from the state ``x_prev``.  Returns (x as a tensor, history)."""
-        nsd = len(self.subdomains)
         x_prev = ad.device_vector(x_prev)
 
         def linearize(x):
             self.update_upwind(x)
             return equation_system(self.equations(x, x_prev, dt))
-        solver = schur_solver(nsd, int(self.offsets[nsd]), self.num_dofs, linear_tol)
+        solver = schur_solver(self.unknown_layout, self.equation_layout, linear_tol)
         return newton_loop(linearize, x_prev, solver, tol, max_iterations, verbose)
 
 
@@ -175,13 +175,14 @@ def equation_system(eqs):
     return eqs, -torch.cat([e.val for e in eqs])
 
 
-def schur_solver(n_primary_equations: int, n_primary_unknowns: int, n: int, tol: float = 1e-10):
-    """A ``linear_solver(eqs, rhs) -> dx`` for equation lists whose first ``n_primary_equations`` entries are the
-    subdomain balances and whose unknown vector starts with the ``n_primary_unknowns`` subdomain unknowns: the interface
-    unknowns behind them are eliminated (``mdflow.schur_solve``).  Rows are split by equation group, columns by two
-    selection matrices (SpGEMM).  The info of the last solve is kept in ``solve.last_info``."""
+def schur_solver(unknown_layout, equation_layout, tol: float = 1e-10):
+    """A ``linear_solver(eqs, rhs) -> dx`` for the equations of ``equation_layout``: the interface unknowns behind the
+    subdomain parts (domain ``("subdomain", i)``, first in both layouts) are eliminated (``mdflow.schur_solve``).  Rows are
+    split by equation part, columns by two selection matrices (SpGEMM); ``solve.last_info``: the info of the last solve."""
     D_ = ad.DeviceCsr
-    npd, nq = int(n_primary_unknowns), int(n_primary_equations)
+    nq = sum(1 for _, d, _, _ in equation_layout.items() if d[0] == "subdomain")
+    npd = sum(n * w for _, d, n, w in unknown_layout.items() if d[0] == "subdomain")
+    n = unknown_layout.size
     sel_p = D_(sps.csr_matrix((np.ones(npd), (np.arange(npd), np.arange(npd))), shape=(n, npd)))
     sel_l = D_(sps.csr_matrix((np.ones(n - npd), (np.arange(npd, n), np.arange(n - npd))), shape=(n, n - npd)))
 

@@ -14,11 +14,10 @@ Per subdomain: pressure and temperature; per interface: Darcy flux ``lambda``, F
                            eta    - vol kappa_T (2 / a) (Pi tr(T) - Pi T_l)     constitutive_laws.py:2342-2386
                            eps    - lambda (U_h Pi tr(w_e) + U_l Pi w_e)        energy_balance.py:353-376
 
-Unknowns: [p per subdomain | T per subdomain | lambda | eta | eps per interface]; equations: [mass | energy | Darcy law |
-Fourier law | enthalpy law] (the reference interleaves both per grid; ``tests/golden/mdthermal_*.npz`` carry the index
-maps).  Upwinding (``porepy_b200.Upwind`` / ``UpwindCoupling``, shared by the mass and the enthalpy flux: same Darcy flux)
-is re-discretized from the iterate in front of every linearization.  Every Newton step eliminates the three interface
-unknown sets (``mdflow_nl.schur_solver``).
+Unknowns and equations: ``unknown_layout``, ``equation_layout`` (the reference interleaves both per grid;
+``tests/golden/mdthermal_*.npz`` carry the index maps).  Upwinding (``porepy_b200.Upwind`` / ``UpwindCoupling``, shared
+by the mass and the enthalpy flux: same Darcy flux) is re-discretized from the iterate in front of every linearization.
+Every Newton step eliminates the three interface unknown sets (``mdflow_nl.schur_solver``).
 """
 from __future__ import annotations
 
@@ -30,12 +29,13 @@ import scipy.sparse as sps
 from . import ad
 from .advection import advective_flux, rediscretize_upwind, rediscretize_upwind_coupling
 from .fv import Mpfa
+from .layout import BlockLayout, LayoutModel
 from .mdflow_nl import equation_system, schur_solver
 from .newton import newton_loop
 from .params import DISCRETIZATION_MATRICES
 
 
-class MixedDimensionalMassEnergy:
+class MixedDimensionalMassEnergy(LayoutModel):
     """``subdomains``: ``mdflow.MdSubdomain`` records whose data dictionaries hold ``parameters[flow_keyword]`` and
     ``parameters[fourier_keyword]`` (``second_order_tensor``, ``bc``, ``ambient_dimension``); ``interfaces``:
     ``mdflow.MdInterface`` records.  Per subdomain (lists): ``volume`` (cell volume x specific volume), ``porosity``,
@@ -59,17 +59,15 @@ class MixedDimensionalMassEnergy:
         self.kappa_t = [np.asarray(v, float) for v in normal_thermal_conductivity]
         self.sources = [np.zeros(s.sd.num_cells) if (sources is None or sources[i] is None) else np.asarray(sources[i], float)
                         for i, s in enumerate(self.subdomains)]
-        nc = [int(s.sd.num_cells) for s in self.subdomains]
-        nm = [it.num_cells for it in self.interfaces]
-        self.sizes = nc + nc + nm + nm + nm
-        self.offsets = np.concatenate(([0], np.cumsum(self.sizes))).astype(np.int64)
-        self.n_primary = 2 * sum(nc)
+        sub = [(("subdomain", i), int(s.sd.num_cells), 1) for i, s in enumerate(self.subdomains)]
+        intf = [(("interface", j), it.num_cells, 1) for j, it in enumerate(self.interfaces)]
+        self.unknown_layout = BlockLayout([("pressure", sub), ("temperature", sub), ("interface_darcy_flux", intf),
+                                           ("interface_fourier_flux", intf), ("interface_enthalpy_flux", intf)])
+        self.equation_layout = BlockLayout([
+            ("mass_balance_equation", sub), ("energy_balance_equation", sub), ("interface_darcy_flux_equation", intf),
+            ("interface_fourier_flux_equation", intf), ("interface_enthalpy_flux_equation", intf)])
         self._intf_data = [{} for _ in self.interfaces]
         self._const = None
-
-    @property
-    def num_dofs(self) -> int:
-        return int(self.offsets[-1])
 
     def discretize(self) -> None:
         """Darcy and Fourier flux of every subdomain with faces (``porepy_b200.Mpfa``; lines: TPFA), once."""
@@ -118,15 +116,6 @@ class MixedDimensionalMassEnergy:
         return (self._density(p, t) * dtm * self.fl.heat_capacity - p) * phi \
             + (dtm * (self.so.density * self.so.heat_capacity)) * (-phi + 1.0)
 
-    def _group(self, parts):
-        """(p, T, lambda, eta, eps) lists from the per-variable list."""
-        nsd, ni = len(self.subdomains), len(self.interfaces)
-        return (parts[:nsd], parts[nsd:2 * nsd], parts[2 * nsd:2 * nsd + ni], parts[2 * nsd + ni:2 * nsd + 2 * ni],
-                parts[2 * nsd + 2 * ni:])
-
-    def _parts(self, x):
-        return self._group([x[self.offsets[q]:self.offsets[q + 1]] for q in range(len(self.sizes))])
-
     def _boundary(self, i, key, flux, k):
         """bc + sum of the projected interface fluxes: what bound_flux / bound_pressure_face act on."""
         b = k.bc[i][key]
@@ -138,7 +127,8 @@ class MixedDimensionalMassEnergy:
     def update_upwind(self, x) -> None:
         x = ad.device_vector(x)
         k = self._operands()
-        p, _, lam, _, _ = self._parts(x)
+        parts = self.unknown_layout.parts(x)
+        p, lam = parts["pressure"], parts["interface_darcy_flux"]
         for i, s in enumerate(self.subdomains):
             if s.sd.num_faces == 0:
                 continue
@@ -156,9 +146,10 @@ class MixedDimensionalMassEnergy:
         fl = self.fl
         nsd = len(self.subdomains)
         x, x_prev = ad.device_vector(x), ad.device_vector(x_prev)
-        var = ad.variables([x[self.offsets[q]:self.offsets[q + 1]] for q in range(len(self.sizes))])
-        p, t, lam, eta, eps = self._group(var)
-        pn, tn, _, _, _ = self._parts(x_prev)
+        var, prev = self.unknown_layout.variables(x), self.unknown_layout.parts(x_prev)
+        p, t = var["pressure"], var["temperature"]
+        lam, eta, eps = var["interface_darcy_flux"], var["interface_fourier_flux"], var["interface_enthalpy_flux"]
+        pn, tn = prev["pressure"], prev["temperature"]
         w = [self._density(p[i], t[i]) * (1.0 / fl.viscosity) for i in range(nsd)]
         we = [w[i] * (t[i] - fl.reference_temperature) * fl.heat_capacity for i in range(nsd)]
         ifl, enthalpy_law = [], []
@@ -199,7 +190,10 @@ class MixedDimensionalMassEnergy:
                                                         (fourier_law, k.Fo[h], t[h], t[l], bt[h], eta[j], k.coef_t[j])):
                 trace = (mats["bound_pressure_cell"] @ hv) + (mats["bound_pressure_face"] @ bnd)
                 laws.append(flux - ((k.p2m[j] @ trace) - (k.s2m[j] @ lv)) * coef)
-        return mass + energy + darcy_law + fourier_law + enthalpy_law
+        return self.equation_layout.stack({
+            "mass_balance_equation": mass, "energy_balance_equation": energy,
+            "interface_darcy_flux_equation": darcy_law, "interface_fourier_flux_equation": fourier_law,
+            "interface_enthalpy_flux_equation": enthalpy_law})
 
     def linearize(self, x, x_prev, dt: float):
         self.update_upwind(x)
@@ -213,5 +207,5 @@ class MixedDimensionalMassEnergy:
         def linearize(x):
             self.update_upwind(x)
             return equation_system(self.equations(x, x_prev, dt))
-        solver = schur_solver(2 * len(self.subdomains), self.n_primary, self.num_dofs, linear_tol)
+        solver = schur_solver(self.unknown_layout, self.equation_layout, linear_tol)
         return newton_loop(linearize, x_prev, solver, tol, max_iterations, verbose)

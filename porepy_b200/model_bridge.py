@@ -14,7 +14,33 @@ from __future__ import annotations
 import numpy as np
 import scipy.sparse as sps
 
+from .layout import BlockLayout
 from .params import DISCRETIZATION_MATRICES, PARAMETERS
+
+
+def _dofs(model, name, grid):
+    """Dofs of the variable ``name`` on ``grid`` in the model's ``EquationSystem``."""
+    es = model.equation_system
+    return es.dofs_of([v for v in es.variables if v.name == name and v.domain is grid])
+
+
+def _column_map(model, layout, grids):
+    """Dof of the model of every unknown of ``layout``: block ``name`` is the model's ``{name}_variable``, the part on
+    domain d lives on ``grids[d]``."""
+    return np.concatenate([_dofs(model, getattr(model, f"{name}_variable"), grids[d]) for name, d, _, _ in
+                           layout.items()])
+
+
+def _row_map(model, layout):
+    """Row of the model of every equation of ``layout``: the model numbers its equations in the order of
+    ``equation_system.equations``, the parts of one equation in the layout's order."""
+    rows, r0 = {}, 0
+    for eq in model.equation_system.equations:
+        for name, d, n, w in layout.items():
+            if name == eq:
+                rows[(name, d)] = np.arange(r0, r0 + n * w)
+                r0 += n * w
+    return np.concatenate([rows[(name, d)] for name, d, _, _ in layout.items()])
 
 
 def _evaluated(model, op, n):
@@ -118,7 +144,7 @@ def mass_energy_from_model(model):
     of the problem is dof ``column_map[k]`` of the model's ``EquationSystem``, equation k its row ``row_map[k]``."""
     from .mdflow import MdSubdomain
     from .mdthermal import MixedDimensionalMassEnergy
-    mdg, es = model.mdg, model.equation_system
+    mdg = model.mdg
     fk, tk = model.darcy_keyword, model.fourier_keyword
     fluid = _fluid(model, True)
     solid = dict(density=model.solid.density, heat_capacity=model.solid.specific_heat_capacity)
@@ -147,22 +173,8 @@ def mass_energy_from_model(model):
                                       fourier_keyword=tk)
     prob.mobility_keyword, prob.enthalpy_upwind_keyword = "b200_mobility", "b200_enthalpy_upwind"
     its = [it for it in mdg.interfaces() if getattr(it, "codim", 1) == 1]
-
-    def dofs(name, g):
-        return es.dofs_of([v for v in es.variables if v.name == name and v.domain is g])
-    cols = [dofs(name, g) for name, grids in ((model.pressure_variable, sds), (model.temperature_variable, sds),
-                                               (model.interface_darcy_flux_variable, its),
-                                               (model.interface_fourier_flux_variable, its),
-                                               (model.interface_enthalpy_flux_variable, its)) for g in grids]
-    rows, r0 = {}, 0
-    for eq in es.equations:
-        grids = sds if eq in ("mass_balance_equation", "energy_balance_equation") else its if eq.startswith("interface") else []
-        for g in grids:
-            rows[(eq, id(g))] = np.arange(r0, r0 + g.num_cells)
-            r0 += g.num_cells
-    order = [("mass_balance_equation", sds), ("energy_balance_equation", sds), ("interface_darcy_flux_equation", its),
-             ("interface_fourier_flux_equation", its), ("interface_enthalpy_flux_equation", its)]
-    return prob, np.concatenate(cols), np.concatenate([rows[(eq, id(g))] for eq, grids in order for g in grids])
+    grids = {**{("subdomain", i): sd for i, sd in enumerate(sds)}, **{("interface", j): it for j, it in enumerate(its)}}
+    return prob, _column_map(model, prob.unknown_layout, grids), _row_map(model, prob.equation_layout)
 
 
 def _mechanics_boundary(model, sd, data, mk):
@@ -186,9 +198,9 @@ def _single_matrix(model):
 
 
 def _matrix_and_fractures(model):
-    """(matrix, fractures) of a model with one nd-D matrix (nd = 2 or 3) and fractures of dimension nd - 1 that do not
-    intersect; anything else -- intersection lines or points, a 1-D matrix, several matrices -- raises
-    ``NotImplementedError``."""
+    """(matrix, fractures, the grids of the layout domains ``("matrix",)``, ``("fracture", j)``, ``("interface", j)``) of
+    a model with one nd-D matrix (nd = 2 or 3) and fractures of dimension nd - 1 that do not intersect; anything else --
+    intersection lines or points, a 1-D matrix, several matrices -- raises ``NotImplementedError``."""
     mdg = model.mdg
     nd = int(mdg.dim_max())
     if nd not in (2, 3):
@@ -201,7 +213,12 @@ def _matrix_and_fractures(model):
     if low:
         raise NotImplementedError(f"{low[0]}-D subdomains (fracture intersections) in a {nd}-D matrix: only {nd - 1}-D "
                                   f"fractures without intersections are supported")
-    return mats[0], list(mdg.subdomains(dim=nd - 1))
+    fracs = list(mdg.subdomains(dim=nd - 1))
+    grids = {("matrix",): mats[0]}
+    for j, f in enumerate(fracs):
+        grids[("fracture", j)] = f
+        grids[("interface", j)] = [it for it in mdg.interfaces() if mdg.interface_to_subdomain_pair(it)[1] is f][0]
+    return mats[0], fracs, grids
 
 
 def _n_inv(model):
@@ -261,33 +278,20 @@ def fractured_momentum_from_model(model):
     two-sided interface); unknown k of the problem is dof ``column_map[k]`` of the model ([u | contact tractions |
     interface displacements])."""
     from .contact import FractureContact, FracturedMomentumBalance
-    mat, fracs = _matrix_and_fractures(model)
-    mdg, es = model.mdg, model.equation_system
+    mat, fracs, grids = _matrix_and_fractures(model)
+    mdg = model.mdg
     mk = model.stress_keyword
     data = _own_data(mdg.subdomain_data(mat), [mk])
-
-    def scalar(op):
-        return float(np.atleast_1d(_evaluated(model, op, 1))[0])
-    contacts, intfs = [], []
-    for frac in fracs:
-        intf = [it for it in mdg.interfaces() if mdg.interface_to_subdomain_pair(it)[1] is frac][0]
+    contacts = []
+    for j, frac in enumerate(fracs):
+        intf = grids[("interface", j)]
         rot = mdg.subdomain_data(frac)["tangential_normal_projection"].project_tangential_normal(frac.num_cells)
         contacts.append(FractureContact(intf.mortar_to_primary_avg(), intf.primary_to_mortar_int(),
                                         intf.mortar_to_secondary_avg(), intf.secondary_to_mortar_int(),
                                         sps.csr_matrix(intf.sign_of_mortar_sides(1)).diagonal(), intf.cell_volumes, rot))
-        intfs.append(intf)
-    constants = dict(numerical_constant=scalar(model.contact_mechanics_numerical_constant(fracs)),
-                     characteristic_traction=scalar(model.characteristic_contact_traction(fracs)),
-                     friction_coefficient=scalar(model.friction_coefficient(fracs)),
-                     dilation_angle=model.solid.dilation_angle, reference_gap=model.solid.fracture_gap,
-                     open_state_tolerance=model.numerical.open_state_tolerance)
-    prob = FracturedMomentumBalance(mat, data, _mechanics_boundary(model, mat, data, mk), contacts, constants, keyword=mk)
-
-    def dofs(name, g):
-        return es.dofs_of([v for v in es.variables if v.name == name and v.domain is g])
-    cols = [dofs(model.displacement_variable, mat)] + [dofs(model.contact_traction_variable, f) for f in fracs] \
-        + [dofs(model.interface_displacement_variable, it) for it in intfs]
-    return prob, np.concatenate(cols)
+    prob = FracturedMomentumBalance(mat, data, _mechanics_boundary(model, mat, data, mk), contacts,
+                                    _contact_constants(model, fracs), keyword=mk)
+    return prob, _column_map(model, prob.unknown_layout, grids)
 
 
 def _contact_constants(model, fracs):
@@ -303,15 +307,15 @@ def _contact_constants(model, fracs):
 def _fractured_problem(model, thermal: bool):
     """Shared part of the two fractured (thermo-)poromechanics bridges."""
     from .fractured_poromech import FractureCoupling
-    mat, fracs = _matrix_and_fractures(model)
-    mdg, es = model.mdg, model.equation_system
+    mat, fracs, grids = _matrix_and_fractures(model)
+    mdg = model.mdg
     fk, mk = model.darcy_keyword, model.stress_keyword
     kws = [fk, mk] + ([model.fourier_keyword] if thermal else [])
     data = _own_data(mdg.subdomain_data(mat), kws)
     a_res = model.solid.residual_aperture
-    couplings, intfs, kappa_t = [], [], []
-    for frac in fracs:
-        intf = [it for it in mdg.interfaces() if mdg.interface_to_subdomain_pair(it)[1] is frac][0]
+    couplings, kappa_t = [], []
+    for j, frac in enumerate(fracs):
+        intf = grids[("interface", j)]
         fdata = _own_data(mdg.subdomain_data(frac), [fk] + ([model.fourier_keyword] if thermal else []))
         k_now = np.asarray(fdata[PARAMETERS][fk]["second_order_tensor"].values, float)
         a_now = _evaluated(model, model.specific_volume([frac]), frac.num_cells)       # the tensor holds k x specific volume
@@ -335,7 +339,6 @@ def _fractured_problem(model, thermal: bool):
         couplings.append(FractureCoupling(frac, fdata, proj, sps.csr_matrix(intf.sign_of_mortar_sides(1)).diagonal(),
                                           intf.cell_volumes, rot, _evaluated(model, model.normal_permeability([intf]), intf.num_cells),
                                           k_now / a_now[None, None, :], bc=fbc))
-        intfs.append(intf)
         if thermal:
             kappa_t.append(_evaluated(model, model.normal_thermal_conductivity([intf]), intf.num_cells))
     fluid = _fluid(model, thermal)
@@ -347,53 +350,25 @@ def _fractured_problem(model, thermal: bool):
     bc = dict(flow=_face_values(model, mat, prm[fk]["bc"], model.bc_values_pressure, model.bc_values_darcy_flux),
               mechanics=_mechanics_boundary(model, mat, data, mk),
               fluid_flux=_face_values(model, mat, ff, w, model.bc_values_fluid_flux), fluid_flux_type=ff)
-
-    def dofs(name, g):
-        return es.dofs_of([v for v in es.variables if v.name == name and v.domain is g])
-    return mat, fracs, intfs, data, couplings, fluid, solid, bc, kappa_t, (w, we), dofs
-
-
-def _row_map(model, layout_order):
-    es = model.equation_system
-    rows, r0 = {}, 0
-    sizes = {}
-    for eq, groups in layout_order:
-        for g, mult in groups:
-            sizes[(eq, id(g))] = mult * g.num_cells
-    for eq in es.equations:
-        for (name, gid), n in sizes.items():
-            if name == eq:
-                rows[(name, gid)] = np.arange(r0, r0 + n)
-                r0 += n
-    return np.concatenate([rows[(eq, id(g))] for eq, groups in layout_order for g, _ in groups])
+    return mat, fracs, data, couplings, fluid, solid, bc, kappa_t, (w, we), grids
 
 
 def fractured_poromechanics_from_model(model):
     """``pp.Poromechanics`` on a fractured medium with frictional contact -> (``FracturedPoromechanics``, column_map,
     row_map)."""
     from .fractured_poromech import FracturedPoromechanics
-    mat, fracs, intfs, data, couplings, fluid, solid, bc, _, _, dofs = _fractured_problem(model, False)
+    mat, fracs, data, couplings, fluid, solid, bc, _, _, grids = _fractured_problem(model, False)
     prob = FracturedPoromechanics(mat, data, couplings, fluid, solid, _contact_constants(model, fracs), bc,
                                   flow_keyword=model.darcy_keyword, mechanics_keyword=model.stress_keyword)
     prob.mobility_keyword = "b200_mobility"
-    nd = int(mat.dim)
-    cols = [dofs(model.pressure_variable, mat)] + [dofs(model.pressure_variable, f) for f in fracs] \
-        + [dofs(model.displacement_variable, mat)] + [dofs(model.contact_traction_variable, f) for f in fracs] \
-        + [dofs(model.interface_darcy_flux_variable, it) for it in intfs] \
-        + [dofs(model.interface_displacement_variable, it) for it in intfs]
-    order = [("mass_balance_equation", [(mat, 1)] + [(f, 1) for f in fracs]), ("momentum_balance_equation", [(mat, nd)]),
-             ("interface_darcy_flux_equation", [(it, 1) for it in intfs]),
-             ("interface_force_balance_equation", [(it, nd) for it in intfs]),
-             ("normal_fracture_deformation_equation", [(f, 1) for f in fracs]),
-             ("tangential_fracture_deformation_equation", [(f, nd - 1) for f in fracs])]
-    return prob, np.concatenate(cols), _row_map(model, order)
+    return prob, _column_map(model, prob.unknown_layout, grids), _row_map(model, prob.equation_layout)
 
 
 def fractured_thermoporomechanics_from_model(model):
     """``pp.Thermoporomechanics`` on a fractured medium with frictional contact (BASELINE config[4]) ->
     (``FracturedThermoporomechanics``, column_map, row_map)."""
     from .fractured_thm import FracturedThermoporomechanics
-    mat, fracs, intfs, data, couplings, fluid, solid, bc, kappa_t, (w, we), dofs = _fractured_problem(model, True)
+    mat, fracs, data, couplings, fluid, solid, bc, kappa_t, (w, we), grids = _fractured_problem(model, True)
     so = model.solid
     solid.update(biot_coefficient=so.biot_coefficient, thermal_expansion=so.thermal_expansion,
                  heat_capacity=so.specific_heat_capacity, conductivity=so.thermal_conductivity, density=so.density)
@@ -405,23 +380,7 @@ def fractured_thermoporomechanics_from_model(model):
                                         flow_keyword=model.darcy_keyword, fourier_keyword=tk,
                                         mechanics_keyword=model.stress_keyword, thermal_keyword=model.enthalpy_keyword)
     prob.mobility_keyword, prob.enthalpy_upwind_keyword = "b200_mobility", "b200_enthalpy_upwind"
-    pv, tv = model.pressure_variable, model.temperature_variable
-    nd = int(mat.dim)
-    cols = [dofs(pv, mat)] + [dofs(pv, f) for f in fracs] + [dofs(tv, mat)] + [dofs(tv, f) for f in fracs] \
-        + [dofs(model.displacement_variable, mat)] + [dofs(model.contact_traction_variable, f) for f in fracs] \
-        + [dofs(model.interface_darcy_flux_variable, it) for it in intfs] \
-        + [dofs(model.interface_fourier_flux_variable, it) for it in intfs] \
-        + [dofs(model.interface_enthalpy_flux_variable, it) for it in intfs] \
-        + [dofs(model.interface_displacement_variable, it) for it in intfs]
-    order = [("mass_balance_equation", [(mat, 1)] + [(f, 1) for f in fracs]),
-             ("energy_balance_equation", [(mat, 1)] + [(f, 1) for f in fracs]), ("momentum_balance_equation", [(mat, nd)]),
-             ("interface_darcy_flux_equation", [(it, 1) for it in intfs]),
-             ("interface_fourier_flux_equation", [(it, 1) for it in intfs]),
-             ("interface_enthalpy_flux_equation", [(it, 1) for it in intfs]),
-             ("interface_force_balance_equation", [(it, nd) for it in intfs]),
-             ("normal_fracture_deformation_equation", [(f, 1) for f in fracs]),
-             ("tangential_fracture_deformation_equation", [(f, nd - 1) for f in fracs])]
-    return prob, np.concatenate(cols), _row_map(model, order)
+    return prob, _column_map(model, prob.unknown_layout, grids), _row_map(model, prob.equation_layout)
 
 
 def tpsa_momentum_from_model(model):
@@ -452,13 +411,11 @@ def tpsa_momentum_from_model(model):
                           body_force=_evaluated(model, model.body_force([sd]), nd * nc),
                           angular_source=_evaluated(model, model.source_angular_momentum([sd]), nr * nc),
                           mass_source=_evaluated(model, model.solid_mass_source([sd]), nc))
-
-    def dofs(name):
-        return es.dofs_of([v for v in es.variables if v.name == name and v.domain is sd])
-    cols = [dofs(model.displacement_variable), dofs(model.rotation_stress_variable), dofs(model.total_pressure_variable)]
-    order = [("momentum_balance_equation", [(sd, nd)]), ("angular_momentum_balance_equation", [(sd, nr)]),
-             ("solid_mass_equation", [(sd, 1)])]
-    rows = _row_map(model, order)
+    cols = [_dofs(model, name, sd) for name in (model.displacement_variable, model.rotation_stress_variable,
+                                                 model.total_pressure_variable)]
+    rows = _row_map(model, BlockLayout([("momentum_balance_equation", [(("matrix",), nc, nd)]),
+                                        ("angular_momentum_balance_equation", [(("matrix",), nc, nr)]),
+                                        ("solid_mass_equation", [(("matrix",), nc, 1)])]))
     prob.column_map = interleave(cols, nd, nr, nc)
     prob.row_map = interleave([rows[:nd * nc], rows[nd * nc:(nd + nr) * nc], rows[(nd + nr) * nc:]], nd, nr, nc)
     return prob, prob.column_map, prob.row_map
@@ -499,15 +456,13 @@ def tpsa_poromechanics_from_model(model):
         mass_source=_evaluated(model, model.solid_mass_source([sd]), nc),
         fluid_source=_evaluated(model, model.fluid_source([sd]), nc), flow_keyword=fk, mechanics_keyword=mk)
     prob.mobility_keyword = "b200_mobility"
-
-    def dofs(name):
-        return es.dofs_of([v for v in es.variables if v.name == name and v.domain is sd])
-    cols = [dofs(model.displacement_variable), dofs(model.rotation_stress_variable), dofs(model.total_pressure_variable),
-            dofs(model.pressure_variable)]
+    cols = [_dofs(model, name, sd) for name in (model.displacement_variable, model.rotation_stress_variable,
+                                                 model.total_pressure_variable, model.pressure_variable)]
     solid_mass = [eq for eq in es.equations if eq.lower().startswith("solid_mass_equation")][0]
-    order = [("momentum_balance_equation", [(sd, nd)]), ("angular_momentum_balance_equation", [(sd, nr)]),
-             (solid_mass, [(sd, 1)]), ("mass_balance_equation", [(sd, 1)])]
-    rows = _row_map(model, order)
+    rows = _row_map(model, BlockLayout([("momentum_balance_equation", [(("matrix",), nc, nd)]),
+                                        ("angular_momentum_balance_equation", [(("matrix",), nc, nr)]),
+                                        (solid_mass, [(("matrix",), nc, 1)]),
+                                        ("mass_balance_equation", [(("matrix",), nc, 1)])]))
     prob.column_map = interleave(cols, nd, nr, nc)
     o = np.cumsum([0, nd * nc, nr * nc, nc, nc])
     prob.row_map = interleave([rows[o[i]:o[i + 1]] for i in range(4)], nd, nr, nc)

@@ -12,8 +12,8 @@ every term taken from the device-resident outputs of ``porepy_b200.Mpfa`` and ``
                                   constitutive_laws.py:2521-2569
 * ``mass_balance_equation``       (mass - mass_n) / dt + div fluid_flux - source = 0
 
-Unknown order as in the reference's ``EquationSystem``: pressures, then displacements (cell-major, nd per cell); equations:
-mass balance, then momentum balance.  ``pb.Upwind`` is re-discretized from the iterate's Darcy flux in front of every
+Unknowns and equations in the order of the reference's ``EquationSystem`` (``unknown_layout``, ``equation_layout``;
+displacements cell-major, nd per cell).  ``pb.Upwind`` is re-discretized from the iterate's Darcy flux in front of every
 linearization (models/solution_strategy.py:433-441).  The Newton update is solved by the fused Jacobi-BiCGStab
 (csrc/krylov.cu) on the coupled Jacobian.  ``tests/golden/poromech_model.npz`` pins Jacobian, residual, residual history
 and converged state to the unmodified reference (tools/make_poromech_golden.py), ``poromech_model_2d.npz`` the same in 2-D.
@@ -27,11 +27,12 @@ from . import ad, krylov
 from .advection import advective_flux, rediscretize_upwind
 from .contact import matrix_dimension
 from .fv import Biot, Mpfa
+from .layout import BlockLayout, LayoutModel
 from .newton import newton_loop
 from .params import DISCRETIZATION_MATRICES
 
 
-class Poromechanics:
+class Poromechanics(LayoutModel):
     """``data``: PorePy-style dictionary with ``parameters[flow_keyword]`` (``second_order_tensor``, ``bc``) and
     ``parameters[mechanics_keyword]`` (``fourth_order_tensor``, vectorial ``bc``, ``scalar_vector_mappings`` =
     {flow_keyword: Biot coefficient or tensor}).  ``fluid``: ``compressibility, density, viscosity, reference_pressure``;
@@ -57,11 +58,10 @@ class Poromechanics:
         self.ff_values = np.asarray(fluid_flux_values, float)
         self.source = np.zeros(self.nc) if source is None else np.asarray(source, float)
         self.body_force = np.zeros(self.nd * self.nc) if body_force is None else np.asarray(body_force, float)
+        scalar, vector = [(("matrix",), self.nc, 1)], [(("matrix",), self.nc, self.nd)]
+        self.unknown_layout = BlockLayout([("pressure", scalar), ("displacement", vector)])
+        self.equation_layout = BlockLayout([("mass_balance_equation", scalar), ("momentum_balance_equation", vector)])
         self._const = None
-
-    @property
-    def num_dofs(self) -> int:
-        return (self.nd + 1) * self.nc
 
     def discretize(self) -> None:
         Mpfa(self.fk).discretize(self.sd, self.data)
@@ -103,16 +103,16 @@ class Poromechanics:
     def update_upwind(self, x) -> None:
         x = ad.device_vector(x)
         k = self._operands()
-        q = (k.flux @ x[:self.nc]) + k.q_b
+        q = (k.flux @ self.unknown_layout.parts(x)["pressure"][0]) + k.q_b
         rediscretize_upwind(self.sd, self.data, self.mobility_keyword, q.cpu().numpy(), self.bc_fluid_flux)
 
     def equations(self, x, x_prev, dt: float) -> list:
         """[mass balance, momentum balance] as ``DeviceAdArray`` at the iterate ``x``."""
         k = self._operands()
         x, x_prev = ad.device_vector(x), ad.device_vector(x_prev)
-        nc = self.nc
-        p, u = ad.variables([x[:nc], x[nc:]])
-        pn, un = x_prev[:nc], x_prev[nc:]
+        var, prev = self.unknown_layout.variables(x), self.unknown_layout.parts(x_prev)
+        (p,), (u,) = var["pressure"], var["displacement"]
+        (pn,), (un,) = prev["pressure"], prev["displacement"]
         T = self.data[DISCRETIZATION_MATRICES][self.mobility_keyword]
         mass = self._density(p) * self._porosity(p, u, k) * k.vol
         mass_n = self._density(pn) * self._porosity(pn, un, k) * k.vol
@@ -122,7 +122,8 @@ class Poromechanics:
         mass_eq = (mass - mass_n) * (1.0 / dt) + (k.div @ ff) - k.src
         stress = (k.stress @ u) + (k.grad_p @ (p - self.p_ref)) + k.stress_b
         momentum_eq = -(k.div_nd @ stress) - k.f
-        return [mass_eq, momentum_eq]
+        return self.equation_layout.stack({"mass_balance_equation": [mass_eq],
+                                           "momentum_balance_equation": [momentum_eq]})
 
     def linearize(self, x, x_prev, dt: float):
         """(J as ``DeviceCsr``, -R as a CUDA tensor): upwind directions from ``x``, then the AD evaluation."""

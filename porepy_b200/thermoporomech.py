@@ -16,8 +16,8 @@ and Fourier) and ``porepy_b200.Biot`` (two coupling tensors: Biot's and the ther
                            c_f (T - T0) rho / mu                                            energy_balance.py:236-352
 * balance equations        momentum: -div_nd stress - f;  mass / energy: d/dt (vol x) + div flux - source
 
-Unknown order as in the reference's ``EquationSystem``: displacements (nd per cell), pressures, temperatures; equations:
-momentum, mass, energy.  ``tests/golden/thm_model.npz`` pins Jacobian, residual, residual history and converged state to the
+Unknowns and equations in the order of the reference's ``EquationSystem`` (``unknown_layout``, ``equation_layout``).
+``tests/golden/thm_model.npz`` pins Jacobian, residual, residual history and converged state to the
 unmodified reference (tools/make_thm_golden.py), ``thm_model_2d.npz`` the same in 2-D.
 """
 from __future__ import annotations
@@ -31,11 +31,12 @@ from . import ad, krylov
 from .advection import advective_flux, rediscretize_upwind
 from .contact import matrix_dimension
 from .fv import Biot, Mpfa
+from .layout import BlockLayout, LayoutModel
 from .newton import newton_loop
 from .params import DISCRETIZATION_MATRICES, PARAMETERS, SecondOrderTensor
 
 
-class Thermoporomechanics:
+class Thermoporomechanics(LayoutModel):
     """``data``: ``parameters[flow_keyword]`` (``second_order_tensor``, ``bc``), ``parameters[fourier_keyword]`` (``bc``; the
     conductivity tensor is written here by ``discretize``), ``parameters[mechanics_keyword]`` (``fourth_order_tensor``,
     vectorial ``bc``, ``scalar_vector_mappings`` = {flow_keyword: Biot tensor, thermal_keyword: thermal-stress tensor}).
@@ -59,11 +60,11 @@ class Thermoporomechanics:
         self.bc = bc
         self.nc, self.nf = int(sd.num_cells), int(sd.num_faces)
         self.rediscretize_fourier = bool(rediscretize_fourier)
+        scalar, vector = [(("matrix",), self.nc, 1)], [(("matrix",), self.nc, self.nd)]
+        self.unknown_layout = BlockLayout([("displacement", vector), ("pressure", scalar), ("temperature", scalar)])
+        self.equation_layout = BlockLayout([("momentum_balance_equation", vector), ("mass_balance_equation", scalar),
+                                            ("energy_balance_equation", scalar)])
         self._const = None
-
-    @property
-    def num_dofs(self) -> int:
-        return (self.nd + 2) * self.nc
 
     def _discretize_fourier(self, phi) -> None:
         self.data[PARAMETERS][self.tk]["second_order_tensor"] = SecondOrderTensor(
@@ -114,15 +115,12 @@ class Thermoporomechanics:
         solid = (dtm * (self.so.density * self.so.heat_capacity)) * (-phi + 1.0)
         return fluid + solid
 
-    def _split(self, x):
-        nu = self.nd * self.nc
-        return x[:nu], x[nu:nu + self.nc], x[nu + self.nc:]
-
     # ---- what follows the iterate: upwind directions (and, by request, the porosity-weighted conductivity)
     def update_discretizations(self, x) -> None:
         x = ad.device_vector(x)
         k = self._operands()
-        u, p, t = self._split(x)
+        parts = self.unknown_layout.parts(x)
+        (u,), (p,), (t,) = parts["displacement"], parts["pressure"], parts["temperature"]
         q = ((k.flux @ p) + k.q_b).cpu().numpy()
         for kw, bc in ((self.mobility_keyword, self.bc["fluid_flux_type"]),
                        (self.enthalpy_upwind_keyword, self.bc["enthalpy_flux_type"])):
@@ -135,8 +133,9 @@ class Thermoporomechanics:
         k = self._operands()
         csr = ad.as_device_csr
         x, x_prev = ad.device_vector(x), ad.device_vector(x_prev)
-        u, p, t = ad.variables(list(self._split(x)))
-        un, pn, tn = self._split(x_prev)
+        var, prev = self.unknown_layout.variables(x), self.unknown_layout.parts(x_prev)
+        (u,), (p,), (t,) = var["displacement"], var["pressure"], var["temperature"]
+        (un,), (pn,), (tn,) = prev["displacement"], prev["pressure"], prev["temperature"]
         DM = self.data[DISCRETIZATION_MATRICES]
         Tm, Te, Fo = DM[self.mobility_keyword], DM[self.enthalpy_upwind_keyword], DM[self.tk]
         fl = self.fl
@@ -153,7 +152,8 @@ class Thermoporomechanics:
         fe = advective_flux(Te, q, we, k.bce, k.bce)
         fo = (csr(Fo["flux"]) @ t) + (csr(Fo["bound_flux"]) @ k.bct)
         energy = (self._energy(p, t, phi) - self._energy(pn, tn, phi_n)) * (k.vol * (1.0 / dt)) + (k.div @ (fe + fo))
-        return [momentum, mass, energy]
+        return self.equation_layout.stack({"momentum_balance_equation": [momentum], "mass_balance_equation": [mass],
+                                           "energy_balance_equation": [energy]})
 
     def linearize(self, x, x_prev, dt: float):
         """(J as ``DeviceCsr``, -R as a CUDA tensor) at the iterate ``x``."""

@@ -346,7 +346,7 @@ def test_time_step_with_device_gmres_gpu(name, monkeypatch):
     assert np.linalg.norm(xh - d["solution"][cm]) <= 1e-8 * np.linalg.norm(d["solution"])
     assert solver.last_info["converged"] and solver.last_info["cuda_graph"]
     if mod is tcm:                                 # the contact state of the pure-contact cases
-        t = xh[prob.offsets[1]:prob.offsets[2]].reshape(-1, 3)
+        t = prob.unknown_layout.parts(xh)["contact_traction"][0].reshape(-1, 3)
         mu = float(d["friction_coefficient"])
         is_open = np.abs(t[:, 2]) < 1e-12
         assert np.all(np.abs(t[is_open]) < 1e-12) and np.all(t[~is_open, 2] < 0)

@@ -62,7 +62,7 @@ def check(prob, d, to_host, make_tensor):
     assert np.linalg.norm(xh - d["solution"]) <= 1e-8 * np.linalg.norm(d["solution"])
     # the contact conditions at the converged state: open cells carry no traction, closed ones a compressive normal
     # traction and a tangential one inside (sticking) or on (sliding) the friction cone
-    t = xh[prob.offsets[1]:prob.offsets[2]].reshape(-1, 3)
+    t = prob.unknown_layout.parts(xh)["contact_traction"][0].reshape(-1, 3)
     mu = float(d["friction_coefficient"])
     is_open = np.abs(t[:, 2]) < 1e-12
     assert np.all(np.abs(t[is_open]) < 1e-12) and np.all(t[~is_open, 2] < 0)

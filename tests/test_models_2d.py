@@ -188,8 +188,7 @@ def check_contact_state(prob, d, x, name):
     """Open cells carry no traction, closed ones a compressive normal traction on (sliding) or inside (sticking) the
     friction cone; the load cases are sliding everywhere, and two open cells next to two sliding ones."""
     nd = prob.nd
-    i = {FracturedMomentumBalance: 1, FracturedPoromechanics: 3, FracturedThermoporomechanics: 5}[type(prob)]
-    t = x[prob.offsets[i]:prob.offsets[i + 1]].reshape(-1, nd)
+    t = prob.unknown_layout.parts(x)["contact_traction"][0].reshape(-1, nd)
     tt, tn = np.abs(t[:, 0]), t[:, nd - 1]                       # a line fracture: one tangential component
     mu = float(d["friction_coefficient"])
     is_open = np.abs(tn) < 1e-12

@@ -358,6 +358,24 @@ int pb_tpsa_poro_rhs(pb_facegrid *g, const double *bc_values, const double *body
 int pb_tpsa_poro_fluid_rows(pb_facegrid *g, struct pb_csr *a, const struct pb_csr *jf, const double *neg_res_dev,
                             double *rhs_dev, int *missing_dev, uint64_t stream);
 
+/* The Jacobian of the TPSA thermo-poromechanics model (pp.Thermoporomechanics + TpsaPoromechanicsMixin) on one grid
+ * without fractures: five fields per cell, [u_c (nd), r_c (nr), p_t_c, p_c, T_c], B = nd + nr + 3 (6 in 2-D, 9 in 3-D).
+ * The mechanics rows are those of pb_tpsa_poro_system, with no T column (the reference's TPSA stress has no thermal
+ * term).  The mass row and then the energy row of c each hold the whole own block and the p and T columns of every
+ * other cell of row c of flux_pattern (the union of the Darcy and Fourier div @ flux patterns, nc x nc, sorted rows).
+ * pb_tpsa_thm_system / pb_tpsa_thm_rhs: as pb_tpsa_poro_system / pb_tpsa_poro_rhs, 0 in the mass and energy rows.
+ * pb_tpsa_thm_balance_rows: the mass and energy rows at one Newton step, on `stream`: row c (mass) and nc + c (energy)
+ * of jf (2 nc x 3 nc device CSR, columns [p_t | p | T]) into the fixed pattern of a, neg_res_dev[c] / [nc + c] into
+ * rhs_dev[c*B + B-2] / [c*B + B-1]; entries outside the pattern are counted into *missing_dev (may be NULL). */
+int pb_tpsa_thm_system(pb_facegrid *g, int nd, const double *mu, const double *lambda, const double *alpha,
+                       const double *cell_volumes, const uint8_t *codes, const double *robin_diag,
+                       const uint8_t *face_flags, const struct pb_csr *flux_pattern, struct pb_csr **out,
+                       float *stage_ms);
+int pb_tpsa_thm_rhs(pb_facegrid *g, const double *bc_values, const double *body_force, const double *angular_source,
+                    const double *mass_source, double *rhs_dev);
+int pb_tpsa_thm_balance_rows(pb_facegrid *g, struct pb_csr *a, const struct pb_csr *jf, const double *neg_res_dev,
+                             double *rhs_dev, int *missing_dev, uint64_t stream);
+
 /* Interface upwinding (UpwindCoupling.discretize, numerics/fv/upwind.py:427-528): per mortar cell the sign of the
  * interface flux and the masks "upstream is the higher-dimensional side" / "... the lower-dimensional side".
  * Host pointers, n doubles each. */

@@ -19,9 +19,10 @@ struct pb_facegrid {
     int sys_nd = 0, terms_nd = 0;
     int64_t sys_nnz = 0, sys_npairs = 0;
     DevBuf fc_ptr, cc_ptr, cc_ix, cc_cell, sys_ip, sys_ix, terms[PB_TPSA_NTERMS];
-    // TPSA poromechanics system (pb_tpsa_poro_system): its row pattern, built once per dimension and flux pattern
+    // TPSA poromechanics / thermo-poromechanics system (pb_tpsa_poro_system, pb_tpsa_thm_system): its row pattern,
+    // built once per dimension, number of scalar balances and flux pattern
     bool nb_ready = false;
-    int poro_nd = 0;
+    int poro_nd = 0, poro_ns = 0;
     int64_t poro_nnz = 0, poro_fp_nnz = -1;
     DevBuf blk_ptr, poro_ip, poro_ix;
 };
@@ -630,25 +631,25 @@ __global__ void tpsa_nb_list_kernel(TpsaTopo t, const int32_t *__restrict__ cc_p
     }
 }
 
-template <int ND>
+template <int ND, int NS>
 __global__ void tpsa_poro_count_kernel(int64_t nc, const int32_t *__restrict__ cc_ptr, const int32_t *__restrict__ fp_ip,
                                        const int32_t *__restrict__ fp_ix, int32_t *__restrict__ count) {
     // clamped: a row past the int32 limit still makes the total overflow the limit of the caller
     for (int64_t c = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; c < nc; c += (int64_t)gridDim.x * blockDim.x)
-        count[c] = (int32_t)min(tpsa_poro_row_count<ND>(c, cc_ptr[c + 1] - cc_ptr[c], fp_ip, fp_ix), (int64_t)0x7fffffff);
+        count[c] = (int32_t)min(tpsa_poro_row_count<ND, NS>(c, cc_ptr[c + 1] - cc_ptr[c], fp_ip, fp_ix), (int64_t)0x7fffffff);
 }
 
-template <int ND>
+template <int ND, int NS>
 __global__ void tpsa_poro_pattern_kernel(int64_t nc, const int32_t *__restrict__ cc_ptr,
                                          const int32_t *__restrict__ cc_ix, const int64_t *__restrict__ blk_ptr,
                                          const int32_t *__restrict__ fp_ip, const int32_t *__restrict__ fp_ix,
                                          int32_t *__restrict__ ip, int32_t *__restrict__ ix) {
     for (int64_t c = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; c < nc; c += (int64_t)gridDim.x * blockDim.x)
-        tpsa_poro_pattern_rows<ND>(c, cc_ptr[c + 1] - cc_ptr[c], cc_ix + cc_ptr[c], blk_ptr[c], fp_ip, fp_ix, ip, ix);
+        tpsa_poro_pattern_rows<ND, NS>(c, cc_ptr[c + 1] - cc_ptr[c], cc_ix + cc_ptr[c], blk_ptr[c], fp_ip, fp_ix, ip, ix);
 }
 
 // one thread per block (c, k), as tpsa_system_kernel
-template <int ND>
+template <int ND, int NS>
 __global__ void tpsa_poro_system_kernel(int64_t npairs, TpsaTopo t, const int32_t *__restrict__ cc_ptr,
                                         const int32_t *__restrict__ cc_ix, const int32_t *__restrict__ cc_cell,
                                         const int64_t *__restrict__ blk_ptr, TpsaTerms T, const double *__restrict__ mu,
@@ -656,44 +657,59 @@ __global__ void tpsa_poro_system_kernel(int64_t npairs, TpsaTopo t, const int32_
                                         const double *__restrict__ vol, double *__restrict__ a) {
     for (int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; e < npairs; e += (int64_t)gridDim.x * blockDim.x) {
         const int64_t c = cc_cell[e];
-        tpsa_poro_block<ND>(c, (int)(e - cc_ptr[c]), t, cc_ptr, cc_ix, blk_ptr, T, mu, lam, alpha, vol, a);
+        tpsa_poro_block<ND, NS>(c, (int)(e - cc_ptr[c]), t, cc_ptr, cc_ix, blk_ptr, T, mu, lam, alpha, vol, a);
     }
 }
 
-template <int ND>
+template <int ND, int NS>
 __global__ void tpsa_poro_rhs_kernel(TpsaTopo t, TpsaTerms T, const double *__restrict__ g, const double *__restrict__ f,
                                      const double *__restrict__ sr, const double *__restrict__ sp,
                                      double *__restrict__ b) {
-    constexpr int NR = TpsaDims<ND>::NR, B = TpsaPoroDims<ND>::B;
+    constexpr int NR = TpsaDims<ND>::NR, B = TpsaPoroDims<ND, NS>::B;
     for (int64_t q = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; q < t.nc * B; q += (int64_t)gridDim.x * blockDim.x) {
         const int64_t c = q / B;
         const int l = (int)(q - c * B);
-        if (l == B - 1) { b[q] = 0.0; continue; }   // the fluid rows are written at every linearization
+        if (l > ND + NR) { b[q] = 0.0; continue; }   // the scalar rows are written at every linearization
         const double src = l < ND ? (f ? f[c * ND + l] : 0.0)
                                    : (l < ND + NR ? (sr ? sr[c * NR + l - ND] : 0.0) : (sp ? sp[c] : 0.0));
         b[q] = tpsa_rhs_row<ND>(c, l, t, T, g, src);
     }
 }
 
-// one thread per cell: its fluid row; the mechanics rows of the block row come first
-template <int ND>
+// one thread per cell: its scalar rows; the mechanics rows of the block row come first
+template <int ND, int NS>
 __global__ void tpsa_poro_fluid_kernel(int64_t nc, const int32_t *__restrict__ cc_ptr,
                                        const int64_t *__restrict__ blk_ptr, const int32_t *__restrict__ ix,
                                        const int32_t *__restrict__ jf_ip, const int32_t *__restrict__ jf_ix,
                                        const double *__restrict__ jf_a, const double *__restrict__ neg_res,
                                        double *__restrict__ a, double *__restrict__ b, int *__restrict__ missing) {
     for (int64_t c = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; c < nc; c += (int64_t)gridDim.x * blockDim.x) {
-        const int64_t row0 = blk_ptr[c] + (int64_t)TpsaPoroDims<ND>::NZ * (cc_ptr[c + 1] - cc_ptr[c]);
-        const int m = tpsa_poro_fluid_row<ND>(c, nc, blk_ptr, row0, ix, jf_ip, jf_ix, jf_a, neg_res, a, b);
+        const int64_t row0 = blk_ptr[c] + (int64_t)TpsaPoroDims<ND, NS>::NZ * (cc_ptr[c + 1] - cc_ptr[c]);
+        const int m = tpsa_poro_fluid_row<ND, NS>(c, nc, blk_ptr, row0, ix, jf_ip, jf_ix, jf_a, neg_res, a, b);
         if (m && missing) atomicAdd(missing, m);
     }
 }
 
-// Row pattern of the four-field system for dimension nd and the flux pattern fp (nc x nc, sorted rows).
+// The names the poromechanics (NS = 1) and thermo-poromechanics (NS = 2) entry points report in their errors.
+template <int NS>
+struct TpsaPoroNames;
+template <>
+struct TpsaPoroNames<1> {
+    static constexpr const char *system = "pb_tpsa_poro_system", *model = "TPSA poromechanics",
+                                *jac = "fluid Jacobian must be num_cells x 2 num_cells ([p_t | p])";
+};
+template <>
+struct TpsaPoroNames<2> {
+    static constexpr const char *system = "pb_tpsa_thm_system", *model = "TPSA thermo-poromechanics",
+                                *jac = "balance Jacobian must be 2 num_cells x 3 num_cells ([p_t | p | T])";
+};
+
+// Row pattern of the system for dimension nd, NS scalar balances and the flux pattern fp (nc x nc, sorted rows).
+template <int NS>
 static int tpsa_poro_build_pattern(pb_facegrid *g, int nd, const CsrView &fp) {
     cudaStream_t st = g->stream;
     const int64_t nc = g->nc;
-    const int B = nd == 3 ? 8 : 5;
+    const int B = (nd == 3 ? 7 : 4) + NS;
     const TpsaTopo t = tpsa_topo(g);
     if (!g->nb_ready) {
         int64_t total = 0;
@@ -708,8 +724,8 @@ static int tpsa_poro_build_pattern(pb_facegrid *g, int nd, const CsrView &fp) {
     }
     DevBuf count;
     CUDA_TRY(count.ensure((size_t)nc * sizeof(int32_t)));
-    if (nd == 3) tpsa_poro_count_kernel<3><<<fg_grid(nc), 256, 0, st>>>(nc, g->cc_ptr.as<int32_t>(), fp.indptr, fp.indices, count.as<int32_t>());
-    else tpsa_poro_count_kernel<2><<<fg_grid(nc), 256, 0, st>>>(nc, g->cc_ptr.as<int32_t>(), fp.indptr, fp.indices, count.as<int32_t>());
+    if (nd == 3) tpsa_poro_count_kernel<3, NS><<<fg_grid(nc), 256, 0, st>>>(nc, g->cc_ptr.as<int32_t>(), fp.indptr, fp.indices, count.as<int32_t>());
+    else tpsa_poro_count_kernel<2, NS><<<fg_grid(nc), 256, 0, st>>>(nc, g->cc_ptr.as<int32_t>(), fp.indptr, fp.indices, count.as<int32_t>());
     pb_count_launch_();
     CUDA_TRY(cudaGetLastError());
     CUDA_TRY(g->blk_ptr.ensure((size_t)(nc + 1) * sizeof(int64_t)));
@@ -722,26 +738,27 @@ static int tpsa_poro_build_pattern(pb_facegrid *g, int nd, const CsrView &fp) {
     const int32_t last = (int32_t)nnz;
     CUDA_TRY(cudaMemcpyAsync(g->poro_ip.as<int32_t>() + nc * B, &last, sizeof(int32_t), cudaMemcpyHostToDevice, st));
     if (nd == 3)
-        tpsa_poro_pattern_kernel<3><<<fg_grid(nc), 256, 0, st>>>(nc, g->cc_ptr.as<int32_t>(), g->cc_ix.as<int32_t>(),
-                                                                  g->blk_ptr.as<int64_t>(), fp.indptr, fp.indices,
-                                                                  g->poro_ip.as<int32_t>(), g->poro_ix.as<int32_t>());
+        tpsa_poro_pattern_kernel<3, NS><<<fg_grid(nc), 256, 0, st>>>(nc, g->cc_ptr.as<int32_t>(), g->cc_ix.as<int32_t>(),
+                                                                      g->blk_ptr.as<int64_t>(), fp.indptr, fp.indices,
+                                                                      g->poro_ip.as<int32_t>(), g->poro_ix.as<int32_t>());
     else
-        tpsa_poro_pattern_kernel<2><<<fg_grid(nc), 256, 0, st>>>(nc, g->cc_ptr.as<int32_t>(), g->cc_ix.as<int32_t>(),
-                                                                  g->blk_ptr.as<int64_t>(), fp.indptr, fp.indices,
-                                                                  g->poro_ip.as<int32_t>(), g->poro_ix.as<int32_t>());
+        tpsa_poro_pattern_kernel<2, NS><<<fg_grid(nc), 256, 0, st>>>(nc, g->cc_ptr.as<int32_t>(), g->cc_ix.as<int32_t>(),
+                                                                      g->blk_ptr.as<int64_t>(), fp.indptr, fp.indices,
+                                                                      g->poro_ip.as<int32_t>(), g->poro_ix.as<int32_t>());
     pb_count_launch_();
     CUDA_TRY(cudaGetLastError());
     CUDA_TRY(cudaStreamSynchronize(st));
     g->poro_nd = nd;
+    g->poro_ns = NS;
     g->poro_nnz = nnz;
     g->poro_fp_nnz = fp.nnz;
     return PB_OK;
 }
 
-extern "C" int pb_tpsa_poro_system(pb_facegrid *g, int nd, const double *mu, const double *lambda, const double *alpha,
-                                   const double *cell_volumes, const uint8_t *codes, const double *robin_diag,
-                                   const uint8_t *face_flags, const pb_csr *flux_pattern, pb_csr **out,
-                                   float *stage_ms) {
+template <int NS>
+static int tpsa_poro_system(pb_facegrid *g, int nd, const double *mu, const double *lambda, const double *alpha,
+                            const double *cell_volumes, const uint8_t *codes, const double *robin_diag,
+                            const uint8_t *face_flags, const pb_csr *flux_pattern, pb_csr **out, float *stage_ms) {
     if (!g || !mu || !lambda || !alpha || !cell_volumes || !codes || !face_flags || !flux_pattern || !out)
         return pb_fail_(PB_EINVAL, "null pointer");
     const int64_t nc = g->nc;
@@ -752,12 +769,12 @@ extern "C" int pb_tpsa_poro_system(pb_facegrid *g, int nd, const double *mu, con
     TpsaInputs in;
     int rc = tpsa_prepare(g, nd, mu, lambda, cell_volumes, codes, robin_diag, face_flags, in);
     if (rc) return rc;
-    if (g->poro_nd != nd || g->poro_fp_nnz != fp.nnz) {
+    if (g->poro_nd != nd || g->poro_ns != NS || g->poro_fp_nnz != fp.nnz) {
         g->poro_nd = 0;
-        if ((rc = tpsa_poro_build_pattern(g, nd, fp))) return rc;
+        if ((rc = tpsa_poro_build_pattern<NS>(g, nd, fp))) return rc;
     }
     cudaStream_t st = g->stream;
-    const int B = nd == 3 ? 8 : 5;
+    const int B = (nd == 3 ? 7 : 4) + NS;
     DevBuf dal;
     CUDA_TRY(dal.upload(alpha, (size_t)nc, st));
     pb_csr *a = nullptr;
@@ -778,15 +795,15 @@ extern "C" int pb_tpsa_poro_system(pb_facegrid *g, int nd, const double *mu, con
     const TpsaTopo t = tpsa_topo(g);
     const int64_t np = g->sys_npairs;
     if (nd == 3)
-        tpsa_poro_system_kernel<3><<<fg_grid(np), 256, 0, st>>>(np, t, g->cc_ptr.as<int32_t>(), g->cc_ix.as<int32_t>(),
-                                                                 g->cc_cell.as<int32_t>(), g->blk_ptr.as<int64_t>(), T,
-                                                                 in.mu.as<double>(), in.lam.as<double>(),
-                                                                 dal.as<double>(), in.vol.as<double>(), pb_csr_data_(a));
+        tpsa_poro_system_kernel<3, NS><<<fg_grid(np), 256, 0, st>>>(np, t, g->cc_ptr.as<int32_t>(), g->cc_ix.as<int32_t>(),
+                                                                     g->cc_cell.as<int32_t>(), g->blk_ptr.as<int64_t>(), T,
+                                                                     in.mu.as<double>(), in.lam.as<double>(),
+                                                                     dal.as<double>(), in.vol.as<double>(), pb_csr_data_(a));
     else
-        tpsa_poro_system_kernel<2><<<fg_grid(np), 256, 0, st>>>(np, t, g->cc_ptr.as<int32_t>(), g->cc_ix.as<int32_t>(),
-                                                                 g->cc_cell.as<int32_t>(), g->blk_ptr.as<int64_t>(), T,
-                                                                 in.mu.as<double>(), in.lam.as<double>(),
-                                                                 dal.as<double>(), in.vol.as<double>(), pb_csr_data_(a));
+        tpsa_poro_system_kernel<2, NS><<<fg_grid(np), 256, 0, st>>>(np, t, g->cc_ptr.as<int32_t>(), g->cc_ix.as<int32_t>(),
+                                                                     g->cc_cell.as<int32_t>(), g->blk_ptr.as<int64_t>(), T,
+                                                                     in.mu.as<double>(), in.lam.as<double>(),
+                                                                     dal.as<double>(), in.vol.as<double>(), pb_csr_data_(a));
     pb_count_launch_();
     SYS_TRY(cudaGetLastError());
     if (stage_ms) SYS_TRY(cudaEventRecord(ev.e[2], st));
@@ -801,11 +818,13 @@ extern "C" int pb_tpsa_poro_system(pb_facegrid *g, int nd, const double *mu, con
     return PB_OK;
 }
 
-extern "C" int pb_tpsa_poro_rhs(pb_facegrid *g, const double *bc_values, const double *body_force,
-                                const double *angular_source, const double *mass_source, double *rhs_dev) {
+template <int NS>
+static int tpsa_poro_rhs(pb_facegrid *g, const double *bc_values, const double *body_force,
+                         const double *angular_source, const double *mass_source, double *rhs_dev) {
     if (!g || !bc_values || !rhs_dev) return pb_fail_(PB_EINVAL, "null pointer");
     const int nd = g->poro_nd;
-    if ((nd != 2 && nd != 3) || g->terms_nd != nd) return pb_fail_(PB_EINVAL, "pb_tpsa_poro_system has not been called");
+    if ((nd != 2 && nd != 3) || g->poro_ns != NS || g->terms_nd != nd)
+        return pb_fail_(PB_EINVAL, std::string(TpsaPoroNames<NS>::system) + " has not been called");
     const int64_t nf = g->nf, nc = g->nc;
     const int nr = nd == 3 ? 3 : 1;
     cudaStream_t st = g->stream;
@@ -817,39 +836,72 @@ extern "C" int pb_tpsa_poro_rhs(pb_facegrid *g, const double *bc_values, const d
     TpsaTerms T{};
     for (int k = PB_TPSA_BOUND_STRESS; k <= PB_TPSA_BOUND_MASS_DISPLACEMENT; ++k) T.t[k] = g->terms[k].as<double>();
     const TpsaTopo t = tpsa_topo(g);
-    const int64_t rows = nc * (nd + nr + 2);
+    const int64_t rows = nc * (nd + nr + 1 + NS);
     const double *pf = body_force ? df.as<double>() : nullptr, *psr = angular_source ? dsr.as<double>() : nullptr,
                  *psp = mass_source ? dsp.as<double>() : nullptr;
-    if (nd == 3) tpsa_poro_rhs_kernel<3><<<fg_grid(rows), 256, 0, st>>>(t, T, dg.as<double>(), pf, psr, psp, rhs_dev);
-    else tpsa_poro_rhs_kernel<2><<<fg_grid(rows), 256, 0, st>>>(t, T, dg.as<double>(), pf, psr, psp, rhs_dev);
+    if (nd == 3) tpsa_poro_rhs_kernel<3, NS><<<fg_grid(rows), 256, 0, st>>>(t, T, dg.as<double>(), pf, psr, psp, rhs_dev);
+    else tpsa_poro_rhs_kernel<2, NS><<<fg_grid(rows), 256, 0, st>>>(t, T, dg.as<double>(), pf, psr, psp, rhs_dev);
     pb_count_launch_();
     CUDA_TRY(cudaGetLastError());
     CUDA_TRY(cudaStreamSynchronize(st));
     return PB_OK;
 }
 
-extern "C" int pb_tpsa_poro_fluid_rows(pb_facegrid *g, pb_csr *a, const pb_csr *jf, const double *neg_res_dev,
-                                       double *rhs_dev, int *missing_dev, uint64_t stream) {
+template <int NS>
+static int tpsa_poro_fluid_rows(pb_facegrid *g, pb_csr *a, const pb_csr *jf, const double *neg_res_dev,
+                                double *rhs_dev, int *missing_dev, uint64_t stream) {
     if (!g || !a || !jf || !neg_res_dev || !rhs_dev) return pb_fail_(PB_EINVAL, "null pointer");
     const int nd = g->poro_nd;
-    if (nd != 2 && nd != 3) return pb_fail_(PB_EINVAL, "pb_tpsa_poro_system has not been called");
+    if ((nd != 2 && nd != 3) || g->poro_ns != NS)
+        return pb_fail_(PB_EINVAL, std::string(TpsaPoroNames<NS>::system) + " has not been called");
     const int64_t nc = g->nc;
-    const int B = nd == 3 ? 8 : 5;
+    const int B = (nd == 3 ? 7 : 4) + NS;
     const CsrView va = pb_csr_view_(a), vj = pb_csr_view_(jf);
     if (va.nrows != nc * B || va.ncols != nc * B || va.nnz != g->poro_nnz)
-        return pb_fail_(PB_EINVAL, "the matrix is not the TPSA poromechanics system of this grid");
-    if (vj.nrows != nc || vj.ncols != 2 * nc)
-        return pb_fail_(PB_EINVAL, "fluid Jacobian must be num_cells x 2 num_cells ([p_t | p])");
+        return pb_fail_(PB_EINVAL, std::string("the matrix is not the ") + TpsaPoroNames<NS>::model +
+                                       " system of this grid");
+    if (vj.nrows != NS * nc || vj.ncols != (1 + NS) * nc) return pb_fail_(PB_EINVAL, TpsaPoroNames<NS>::jac);
     cudaStream_t st = (cudaStream_t)stream;
     if (nd == 3)
-        tpsa_poro_fluid_kernel<3><<<fg_grid(nc), 256, 0, st>>>(nc, g->cc_ptr.as<int32_t>(), g->blk_ptr.as<int64_t>(),
-                                                                va.indices, vj.indptr, vj.indices, vj.data, neg_res_dev,
-                                                                va.data, rhs_dev, missing_dev);
+        tpsa_poro_fluid_kernel<3, NS><<<fg_grid(nc), 256, 0, st>>>(nc, g->cc_ptr.as<int32_t>(), g->blk_ptr.as<int64_t>(),
+                                                                    va.indices, vj.indptr, vj.indices, vj.data, neg_res_dev,
+                                                                    va.data, rhs_dev, missing_dev);
     else
-        tpsa_poro_fluid_kernel<2><<<fg_grid(nc), 256, 0, st>>>(nc, g->cc_ptr.as<int32_t>(), g->blk_ptr.as<int64_t>(),
-                                                                va.indices, vj.indptr, vj.indices, vj.data, neg_res_dev,
-                                                                va.data, rhs_dev, missing_dev);
+        tpsa_poro_fluid_kernel<2, NS><<<fg_grid(nc), 256, 0, st>>>(nc, g->cc_ptr.as<int32_t>(), g->blk_ptr.as<int64_t>(),
+                                                                    va.indices, vj.indptr, vj.indices, vj.data, neg_res_dev,
+                                                                    va.data, rhs_dev, missing_dev);
     pb_count_launch_();
     CUDA_TRY(cudaGetLastError());
     return PB_OK;
+}
+
+extern "C" int pb_tpsa_poro_system(pb_facegrid *g, int nd, const double *mu, const double *lambda, const double *alpha,
+                                   const double *cell_volumes, const uint8_t *codes, const double *robin_diag,
+                                   const uint8_t *face_flags, const pb_csr *flux_pattern, pb_csr **out,
+                                   float *stage_ms) {
+    return tpsa_poro_system<1>(g, nd, mu, lambda, alpha, cell_volumes, codes, robin_diag, face_flags, flux_pattern, out,
+                               stage_ms);
+}
+extern "C" int pb_tpsa_poro_rhs(pb_facegrid *g, const double *bc_values, const double *body_force,
+                                const double *angular_source, const double *mass_source, double *rhs_dev) {
+    return tpsa_poro_rhs<1>(g, bc_values, body_force, angular_source, mass_source, rhs_dev);
+}
+extern "C" int pb_tpsa_poro_fluid_rows(pb_facegrid *g, pb_csr *a, const pb_csr *jf, const double *neg_res_dev,
+                                       double *rhs_dev, int *missing_dev, uint64_t stream) {
+    return tpsa_poro_fluid_rows<1>(g, a, jf, neg_res_dev, rhs_dev, missing_dev, stream);
+}
+
+extern "C" int pb_tpsa_thm_system(pb_facegrid *g, int nd, const double *mu, const double *lambda, const double *alpha,
+                                  const double *cell_volumes, const uint8_t *codes, const double *robin_diag,
+                                  const uint8_t *face_flags, const pb_csr *flux_pattern, pb_csr **out, float *stage_ms) {
+    return tpsa_poro_system<2>(g, nd, mu, lambda, alpha, cell_volumes, codes, robin_diag, face_flags, flux_pattern, out,
+                               stage_ms);
+}
+extern "C" int pb_tpsa_thm_rhs(pb_facegrid *g, const double *bc_values, const double *body_force,
+                               const double *angular_source, const double *mass_source, double *rhs_dev) {
+    return tpsa_poro_rhs<2>(g, bc_values, body_force, angular_source, mass_source, rhs_dev);
+}
+extern "C" int pb_tpsa_thm_balance_rows(pb_facegrid *g, pb_csr *a, const pb_csr *jf, const double *neg_res_dev,
+                                        double *rhs_dev, int *missing_dev, uint64_t stream) {
+    return tpsa_poro_fluid_rows<2>(g, a, jf, neg_res_dev, rhs_dev, missing_dev, stream);
 }

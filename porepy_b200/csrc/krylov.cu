@@ -58,8 +58,9 @@ __global__ void kry_init_kernel(int64_t n, const double *__restrict__ b, double 
 // Preconditioner application z = M^-1 y on one block of BS consecutive entries: BS == 1 -- minv holds the inverse
 // diagonal (Jacobi); BS > 1 -- minv holds the inverted BS x BS diagonal blocks, row-major (block Jacobi: the nd
 // displacement components of a cell in the mechanics system A = div_nd @ stress, the nd + nr + 1 unknowns [u, r, p]
-// of a cell in the TPSA system, BS = 4 in 2-D and 7 in 3-D, or the nd + nr + 2 unknowns [u, r, p_t, p] of a cell in the
-// TPSA poromechanics system, BS = 5 and 8).
+// of a cell in the TPSA system, BS = 4 in 2-D and 7 in 3-D, the nd + nr + 2 unknowns [u, r, p_t, p] of a cell in the
+// TPSA poromechanics system, BS = 5 and 8, or the nd + nr + 3 unknowns [u, r, p_t, p, T] of a cell in the TPSA
+// thermo-poromechanics system, BS = 6 and 9).
 template <int BS>
 __device__ __forceinline__ void apply_minv(const double *__restrict__ minv, int64_t b, const double (&y)[BS], double (&z)[BS]) {
     if (!minv) {
@@ -181,7 +182,7 @@ extern "C" int pb_kry_seed(double *scal, uint64_t stream) {
     CUDA_TRY(cudaGetLastError());
     return PB_OK;
 }
-static bool kry_block_size_ok(int bs) { return (bs >= 1 && bs <= 5) || bs == 7 || bs == 8; }
+static bool kry_block_size_ok(int bs) { return bs >= 1 && bs <= 9; }
 
 // bs: size of the diagonal blocks of the preconditioner (1 = Jacobi, 2 / 3 / 4 / 5 / 7 / 8 = block Jacobi; n must be a
 // multiple)
@@ -195,8 +196,10 @@ extern "C" int pb_kry_p(int64_t n, const double *r, double *p, const double *v, 
     else if (bs == 3) kry_p_kernel<3><<<kgrid(n / 3), 256, 0, st>>>(n, r, p, v, minv, ph, scal, cur & 1);
     else if (bs == 4) kry_p_kernel<4><<<kgrid(n / 4), 256, 0, st>>>(n, r, p, v, minv, ph, scal, cur & 1);
     else if (bs == 5) kry_p_kernel<5><<<kgrid(n / 5), 256, 0, st>>>(n, r, p, v, minv, ph, scal, cur & 1);
+    else if (bs == 6) kry_p_kernel<6><<<kgrid(n / 6), 256, 0, st>>>(n, r, p, v, minv, ph, scal, cur & 1);
     else if (bs == 7) kry_p_kernel<7><<<kgrid(n / 7), 256, 0, st>>>(n, r, p, v, minv, ph, scal, cur & 1);
-    else kry_p_kernel<8><<<kgrid(n / 8), 256, 0, st>>>(n, r, p, v, minv, ph, scal, cur & 1);
+    else if (bs == 8) kry_p_kernel<8><<<kgrid(n / 8), 256, 0, st>>>(n, r, p, v, minv, ph, scal, cur & 1);
+    else kry_p_kernel<9><<<kgrid(n / 9), 256, 0, st>>>(n, r, p, v, minv, ph, scal, cur & 1);
     pb_count_launch_();
     CUDA_TRY(cudaGetLastError());
     return PB_OK;
@@ -211,8 +214,10 @@ extern "C" int pb_kry_s(int64_t n, const double *r, const double *v, const doubl
     else if (bs == 3) kry_s_kernel<3><<<kgrid(n / 3), 256, 0, st>>>(n, r, v, minv, s, sh, scal, cur & 1);
     else if (bs == 4) kry_s_kernel<4><<<kgrid(n / 4), 256, 0, st>>>(n, r, v, minv, s, sh, scal, cur & 1);
     else if (bs == 5) kry_s_kernel<5><<<kgrid(n / 5), 256, 0, st>>>(n, r, v, minv, s, sh, scal, cur & 1);
+    else if (bs == 6) kry_s_kernel<6><<<kgrid(n / 6), 256, 0, st>>>(n, r, v, minv, s, sh, scal, cur & 1);
     else if (bs == 7) kry_s_kernel<7><<<kgrid(n / 7), 256, 0, st>>>(n, r, v, minv, s, sh, scal, cur & 1);
-    else kry_s_kernel<8><<<kgrid(n / 8), 256, 0, st>>>(n, r, v, minv, s, sh, scal, cur & 1);
+    else if (bs == 8) kry_s_kernel<8><<<kgrid(n / 8), 256, 0, st>>>(n, r, v, minv, s, sh, scal, cur & 1);
+    else kry_s_kernel<9><<<kgrid(n / 9), 256, 0, st>>>(n, r, v, minv, s, sh, scal, cur & 1);
     pb_count_launch_();
     CUDA_TRY(cudaGetLastError());
     return PB_OK;
@@ -278,8 +283,8 @@ __global__ void block_diag_inv_kernel(int64_t nb, const int32_t *__restrict__ ip
     }
 }
 
-// BS = 8: the same inverse and fallback, Gauss-Jordan in place (the pivot rows are recorded and the columns of the
-// result swapped back at the end), so one 8 x 8 block instead of two stays in registers.
+// BS = 6, 8, 9: the same inverse and fallback, Gauss-Jordan in place (the pivot rows are recorded and the columns of
+// the result swapped back at the end), so one block instead of two stays in registers (9 x 9: 232 registers, no spills).
 template <int BS>
 __global__ void block_diag_inv_inplace_kernel(int64_t nb, const int32_t *__restrict__ ip, const int32_t *__restrict__ ix,
                                               const double *__restrict__ data, double *__restrict__ out) {
@@ -364,8 +369,10 @@ extern "C" int pb_csr_block_diag_inv_dev(const pb_csr *a, int bs, int64_t nblock
     else if (bs == 3) block_diag_inv_kernel<3><<<grid, 256, 0, st>>>(nblocks, v.indptr, v.indices, v.data, out_dev);
     else if (bs == 4) block_diag_inv_kernel<4><<<grid, 256, 0, st>>>(nblocks, v.indptr, v.indices, v.data, out_dev);
     else if (bs == 5) block_diag_inv_kernel<5><<<grid, 256, 0, st>>>(nblocks, v.indptr, v.indices, v.data, out_dev);
+    else if (bs == 6) block_diag_inv_inplace_kernel<6><<<grid, 256, 0, st>>>(nblocks, v.indptr, v.indices, v.data, out_dev);
     else if (bs == 7) block_diag_inv_kernel<7><<<grid, 256, 0, st>>>(nblocks, v.indptr, v.indices, v.data, out_dev);
-    else block_diag_inv_inplace_kernel<8><<<grid, 256, 0, st>>>(nblocks, v.indptr, v.indices, v.data, out_dev);
+    else if (bs == 8) block_diag_inv_inplace_kernel<8><<<grid, 256, 0, st>>>(nblocks, v.indptr, v.indices, v.data, out_dev);
+    else block_diag_inv_inplace_kernel<9><<<grid, 256, 0, st>>>(nblocks, v.indptr, v.indices, v.data, out_dev);
     pb_count_launch_();
     CUDA_TRY(cudaGetLastError());
     return PB_OK;

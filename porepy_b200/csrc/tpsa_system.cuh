@@ -174,39 +174,43 @@ PB_HD double tpsa_rhs_row(int64_t c, int l, const TpsaTopo &t, const TpsaTerms &
     return acc + src;
 }
 
-// ---- TPSA poromechanics (reference models/poromechanics.py:92-136, 177-213): four fields per cell ------------------
-// Unknowns and equations per cell [u_c (nd), r_c (nr), p_t_c, p_c], B = nd + nr + 2 (5 in 2-D, 8 in 3-D).  The
-// mechanics rows are the three-field rows (columns relative to k * B) with the solid-mass row extended by the fluid
-// pressure: [u_0 .. u_ND-1, p_t, p] per neighbour k, whose p entry is -vol alpha / lambda for k = c and 0 otherwise.
-// The fluid-mass row of c holds the p column of every cell in row c of div @ flux (MPFA), ascending, with the whole
-// own block [u_c, r_c, p_t_c, p_c] in place of p_c.  Block row c starts at blk_ptr[c]: the mechanics rows first, row l
-// at blk_ptr[c] + off(l) * n_c, then the fluid row at blk_ptr[c] + NZ * n_c.
-template <int ND>
+// ---- TPSA poromechanics and thermo-poromechanics (reference models/poromechanics.py:92-136, 177-213) --------------
+// Unknowns and equations per cell [u_c (nd), r_c (nr), p_t_c, s_c (NS)]: NS scalar balances after the total pressure,
+// s = [p] for poromechanics (NS = 1) and [p, T] for thermo-poromechanics (NS = 2), so B = nd + nr + 1 + NS (5 / 8 and
+// 6 / 9).  The mechanics rows are the three-field rows (columns relative to k * B) with the solid-mass row extended by
+// the fluid pressure: [u_0 .. u_ND-1, p_t, p] per neighbour k, whose p entry is -vol alpha / lambda for k = c and 0
+// otherwise; they have no T column (the TPSA stress of the reference has no thermal term).  Scalar row s of c holds the
+// whole own block [u_c, r_c, p_t_c, s_c] and the NS scalar columns of every other cell in row c of the flux pattern
+// (div @ flux, MPFA; with NS = 2 the union of the Darcy and Fourier patterns), ascending.  Block row c starts at
+// blk_ptr[c]: the mechanics rows first, row l at blk_ptr[c] + off(l) * n_c, then scalar row s at
+// blk_ptr[c] + NZ * n_c + s * (B + NS * m_c), m_c the other cells of the flux-pattern row.
+template <int ND, int NS = 1>
 struct TpsaPoroDims {
     using M = TpsaDims<ND>;
-    static constexpr int NR = M::NR, B = M::B + 1, LP = M::LP + 1;
+    static constexpr int NR = M::NR, B = M::B + NS, LP = M::LP + 1;
     static constexpr int NZ = ND * M::LU + NR * M::LR + LP;   // mechanics entries per neighbour
     PB_HD static int len(int l) { return l < ND + NR ? M::len(l) : LP; }
     PB_HD static int off(int l) { return M::off(l); }
     PB_HD static int col(int l, int t) { return l < ND + NR ? M::col(l, t) : (t < ND ? t : ND + NR + (t - ND)); }
 };
 
-// Entries of block row c in the fixed pattern: NZ per face neighbour, B for the own block, one per other cell of row c
-// of the flux pattern (fp_*: sorted CSR of div @ flux).
-template <int ND>
+// Entries of block row c in the fixed pattern: NZ per face neighbour, and per scalar row B for the own block and NS per
+// other cell of row c of the flux pattern (fp_*: sorted CSR).
+template <int ND, int NS = 1>
 PB_HD int64_t tpsa_poro_row_count(int64_t c, int n, const int32_t *fp_ip, const int32_t *fp_ix) {
-    using D = TpsaPoroDims<ND>;
+    using D = TpsaPoroDims<ND, NS>;
     int64_t m = 0;
     for (int q = fp_ip[c]; q < fp_ip[c + 1]; ++q) m += fp_ix[q] != c;
-    return (int64_t)D::NZ * n + D::B + m;
+    return (int64_t)D::NZ * n + NS * (D::B + NS * m);
 }
 
 // Row pointers and column indices of block row c (n face neighbours nb, ascending; the block row starts at blk0).
-template <int ND>
+template <int ND, int NS = 1>
 PB_HD void tpsa_poro_pattern_rows(int64_t c, int n, const int32_t *nb, int64_t blk0, const int32_t *fp_ip,
                                   const int32_t *fp_ix, int32_t *ip, int32_t *ix) {
-    using D = TpsaPoroDims<ND>;
-    for (int l = 0; l < D::B - 1; ++l) {
+    using D = TpsaPoroDims<ND, NS>;
+    constexpr int MB = D::M::B;   // mechanics rows per cell; scalar s sits at column MB + s of a block
+    for (int l = 0; l < MB; ++l) {
         const int len = D::len(l);
         const int64_t r0 = blk0 + (int64_t)D::off(l) * n;
         ip[c * D::B + l] = (int32_t)r0;
@@ -214,61 +218,72 @@ PB_HD void tpsa_poro_pattern_rows(int64_t c, int n, const int32_t *nb, int64_t b
             for (int t = 0; t < len; ++t) ix[r0 + j * len + t] = nb[j] * D::B + D::col(l, t);
     }
     int64_t q0 = blk0 + (int64_t)D::NZ * n;
-    ip[c * D::B + D::B - 1] = (int32_t)q0;
-    bool own = false;
-    for (int q = fp_ip[c]; q <= fp_ip[c + 1]; ++q) {
-        const int32_t k = q < fp_ip[c + 1] ? fp_ix[q] : INT32_MAX;
-        if (!own && k >= c) {
-            for (int t = 0; t < D::B; ++t) ix[q0++] = (int32_t)(c * D::B + t);
-            own = true;
+    for (int s = 0; s < NS; ++s) {
+        ip[c * D::B + MB + s] = (int32_t)q0;
+        bool own = false;
+        for (int q = fp_ip[c]; q <= fp_ip[c + 1]; ++q) {
+            const int32_t k = q < fp_ip[c + 1] ? fp_ix[q] : INT32_MAX;
+            if (!own && k >= c) {
+                for (int t = 0; t < D::B; ++t) ix[q0++] = (int32_t)(c * D::B + t);
+                own = true;
+            }
+            if (k != c && k != INT32_MAX)
+                for (int u = 0; u < NS; ++u) ix[q0++] = k * D::B + MB + u;
         }
-        if (k != c && k != INT32_MAX) ix[q0++] = k * D::B + D::B - 1;
     }
 }
 
-// Mechanics rows of block (c, cc_ix[j0 + j]) into the CSR values a; thread j = 0 also zeroes the fluid row of c.
-template <int ND>
+// Mechanics rows of block (c, cc_ix[j0 + j]) into the CSR values a; thread j = 0 also zeroes the scalar rows of c.
+template <int ND, int NS = 1>
 PB_HD void tpsa_poro_block(int64_t c, int j, const TpsaTopo &t, const int32_t *cc_ptr, const int32_t *cc_ix,
                            const int64_t *blk_ptr, const TpsaTerms &T, const double *mu, const double *lam,
                            const double *alpha, const double *vol, double *a) {
-    using D = TpsaPoroDims<ND>;
+    using D = TpsaPoroDims<ND, NS>;
+    constexpr int MB = D::M::B;
     const int64_t j0 = cc_ptr[c];
     const int n = (int)(cc_ptr[c + 1] - j0);
     const int64_t k = cc_ix[j0 + j];
     const int64_t b0 = blk_ptr[c];
 #pragma unroll
-    for (int l = 0; l < D::B - 1; ++l) {
+    for (int l = 0; l < MB; ++l) {
         double *dst = a + b0 + (int64_t)D::off(l) * n + (int64_t)j * D::len(l);
         tpsa_system_segment<ND>(c, l, k, t, T, mu, lam, vol, dst);
-        if (l == D::B - 2) dst[ND + 1] = k == c ? -vol[c] * alpha[c] / lam[c] : 0.0;
+        if (l == MB - 1) dst[ND + 1] = k == c ? -vol[c] * alpha[c] / lam[c] : 0.0;
     }
     if (j == 0)
         for (int64_t q = b0 + (int64_t)D::NZ * n; q < blk_ptr[c + 1]; ++q) a[q] = 0.0;
 }
 
-// Fluid row of cell c at one Newton step: the row c of the field-ordered Jacobian jf (columns [p_t (nc) | p (nc)]) placed
-// into the fixed pattern (sorted; binary search per entry, duplicates summed in row order) and -R_c into
-// b[c * B + B - 1].  Returns the number of entries that are not in the pattern (0 by construction).
-template <int ND>
+// Scalar rows of cell c at one Newton step: row s * nc + c of the field-ordered Jacobian jf (NS nc rows, columns
+// [p_t (nc) | s_0 (nc) .. s_NS-1 (nc)]) placed into the fixed pattern of scalar row s (sorted, from row0 = the first
+// scalar row of c; binary search per entry, duplicates summed in row order), and -R into b[c * B + MB + s].  Returns
+// the number of entries that are not in the pattern (0 by construction).
+template <int ND, int NS = 1>
 PB_HD int tpsa_poro_fluid_row(int64_t c, int64_t nc, const int64_t *blk_ptr, int64_t row0, const int32_t *ix,
                               const int32_t *jf_ip, const int32_t *jf_ix, const double *jf_a, const double *neg_res,
                               double *a, double *b) {
-    using D = TpsaPoroDims<ND>;
-    const int64_t s = row0, e = blk_ptr[c + 1];
-    for (int64_t q = s; q < e; ++q) a[q] = 0.0;
+    using D = TpsaPoroDims<ND, NS>;
+    constexpr int MB = D::M::B;
+    const int64_t len = (blk_ptr[c + 1] - row0) / NS;
     int missing = 0;
-    for (int q = jf_ip[c]; q < jf_ip[c + 1]; ++q) {
-        const int64_t col = jf_ix[q];
-        const int32_t want = (int32_t)(col < nc ? col * D::B + D::B - 2 : (col - nc) * D::B + D::B - 1);
-        int64_t lo = s, hi = e;
-        while (lo < hi) {
-            const int64_t mid = (lo + hi) >> 1;
-            if (ix[mid] < want) lo = mid + 1; else hi = mid;
+    for (int s = 0; s < NS; ++s) {
+        const int64_t s0 = row0 + s * len, e = s0 + len, r = s * nc + c;
+        for (int64_t q = s0; q < e; ++q) a[q] = 0.0;
+        for (int q = jf_ip[r]; q < jf_ip[r + 1]; ++q) {
+            int64_t col = jf_ix[q];
+            int fld = 0;   // 0: p_t, 1 + u: scalar u
+            while (fld < NS && col >= nc) { col -= nc; ++fld; }
+            const int32_t want = (int32_t)(col * D::B + MB - 1 + fld);
+            int64_t lo = s0, hi = e;
+            while (lo < hi) {
+                const int64_t mid = (lo + hi) >> 1;
+                if (ix[mid] < want) lo = mid + 1; else hi = mid;
+            }
+            if (lo < e && ix[lo] == want) a[lo] += jf_a[q];
+            else ++missing;
         }
-        if (lo < e && ix[lo] == want) a[lo] += jf_a[q];
-        else ++missing;
+        b[c * D::B + MB + s] = neg_res[r];
     }
-    b[c * D::B + D::B - 1] = neg_res[c];
     return missing;
 }
 

@@ -670,6 +670,19 @@ class FaceGrid:
         """The TPSA poromechanics Jacobian with its mechanics rows (``pb_tpsa_poro_system``, layout in
         include/poreb200.h) as a ``DeviceCsr`` and the device times of its two stages in ms.  ``flux_pattern``: the
         ``DeviceCsr`` div @ flux whose rows give the fluid-row patterns."""
+        return self._poro_system(self.lib.pb_tpsa_poro_system, nd, mu, lmbda, alpha, cell_volumes, codes, robin_diag,
+                                 face_flags, face_areas, flux_pattern)
+
+    def tpsa_thm_system(self, nd: int, mu, lmbda, alpha, cell_volumes, codes, robin_diag, face_flags, face_areas,
+                        flux_pattern) -> tuple:
+        """The TPSA thermo-poromechanics Jacobian with its mechanics rows (``pb_tpsa_thm_system``, layout in
+        include/poreb200.h) as a ``DeviceCsr`` and the device times of its two stages in ms.  ``flux_pattern``: a
+        ``DeviceCsr`` whose rows hold the union of the Darcy and Fourier div @ flux patterns."""
+        return self._poro_system(self.lib.pb_tpsa_thm_system, nd, mu, lmbda, alpha, cell_volumes, codes, robin_diag,
+                                 face_flags, face_areas, flux_pattern)
+
+    def _poro_system(self, fn, nd, mu, lmbda, alpha, cell_volumes, codes, robin_diag, face_flags, face_areas,
+                     flux_pattern):
         from .sparse import DeviceCsr
         mu, lam, al, vol = _lib.f64(mu), _lib.f64(lmbda), _lib.f64(alpha), _lib.f64(cell_volumes)
         if mu.shape != (self.nc,) or lam.shape != (self.nc,) or al.shape != (self.nc,):
@@ -682,40 +695,53 @@ class FaceGrid:
         _lib.check(self.lib.pb_facegrid_set_face_areas(self.h, _lib.ptr(_lib.f64(face_areas), _lib._f64p)))
         h = C.c_void_p()
         ms = (C.c_float * 2)()
-        _lib.check(self.lib.pb_tpsa_poro_system(self.h, int(nd), _lib.ptr(mu, _lib._f64p), _lib.ptr(lam, _lib._f64p),
-                                                _lib.ptr(al, _lib._f64p), _lib.ptr(vol, _lib._f64p),
-                                                _lib.ptr(cod, _lib._u8p), _lib.ptr(rob, _lib._f64p),
-                                                _lib.ptr(flags, _lib._u8p), flux_pattern.h, C.byref(h),
-                                                C.cast(ms, _lib._f32p)))
+        _lib.check(fn(self.h, int(nd), _lib.ptr(mu, _lib._f64p), _lib.ptr(lam, _lib._f64p), _lib.ptr(al, _lib._f64p),
+                      _lib.ptr(vol, _lib._f64p), _lib.ptr(cod, _lib._u8p), _lib.ptr(rob, _lib._f64p),
+                      _lib.ptr(flags, _lib._u8p), flux_pattern.h, C.byref(h), C.cast(ms, _lib._f32p)))
         return DeviceCsr.from_handle(h), [float(ms[0]), float(ms[1])]
 
     def tpsa_poro_rhs(self, n: int, bc_values, body_force=None, angular_source=None, mass_source=None):
         """-R(0) of the mechanics rows of the poromechanics system last assembled on this grid (``pb_tpsa_poro_rhs``),
         0 in the fluid rows, as a CUDA tensor of ``n`` doubles."""
+        return self._poro_rhs(self.lib.pb_tpsa_poro_rhs, n, bc_values, body_force, angular_source, mass_source)
+
+    def tpsa_thm_rhs(self, n: int, bc_values, body_force=None, angular_source=None, mass_source=None):
+        """-R(0) of the mechanics rows of the thermo-poromechanics system last assembled on this grid
+        (``pb_tpsa_thm_rhs``), 0 in the mass and energy rows, as a CUDA tensor of ``n`` doubles."""
+        return self._poro_rhs(self.lib.pb_tpsa_thm_rhs, n, bc_values, body_force, angular_source, mass_source)
+
+    def _poro_rhs(self, fn, n, bc_values, body_force, angular_source, mass_source):
         import torch
         arrs = [None if a is None else _lib.f64(a) for a in (bc_values, body_force, angular_source, mass_source)]
         b = torch.empty(int(n), dtype=torch.float64, device="cuda")
-        _lib.check(self.lib.pb_tpsa_poro_rhs(self.h, *[_lib.ptr(a, _lib._f64p) for a in arrs],
-                                             C.c_void_p(b.data_ptr())))
+        _lib.check(fn(self.h, *[_lib.ptr(a, _lib._f64p) for a in arrs], C.c_void_p(b.data_ptr())))
         return b
 
     def tpsa_poro_fluid_rows(self, A, jf, neg_res, rhs, missing=None) -> None:
         """Write the fluid rows of ``A`` (the matrix of ``tpsa_poro_system``) from the field-ordered fluid Jacobian
         ``jf`` (``DeviceCsr``, columns [p_t | p]) and the fluid entries of ``rhs`` from ``neg_res``, on the current
         stream (``pb_tpsa_poro_fluid_rows``).  ``missing``: int32 CUDA tensor counting entries outside the pattern."""
+        self._balance_rows(self.lib.pb_tpsa_poro_fluid_rows, self.nc, A, jf, neg_res, rhs, missing)
+
+    def tpsa_thm_balance_rows(self, A, jf, neg_res, rhs, missing=None) -> None:
+        """Write the mass and energy rows of ``A`` (the matrix of ``tpsa_thm_system``) from the field-ordered Jacobian
+        ``jf`` (``DeviceCsr``, rows [mass | energy], columns [p_t | p | T]) and their entries of ``rhs`` from
+        ``neg_res`` (2 nc), on the current stream (``pb_tpsa_thm_balance_rows``).  ``missing``: int32 CUDA tensor
+        counting entries outside the pattern."""
+        self._balance_rows(self.lib.pb_tpsa_thm_balance_rows, 2 * self.nc, A, jf, neg_res, rhs, missing)
+
+    def _balance_rows(self, fn, n, A, jf, neg_res, rhs, missing):
         import torch
         from .sparse import device_operand
-        nc = self.nc
-        neg_res = device_operand(neg_res.contiguous(), nc, "neg_res")
+        neg_res = device_operand(neg_res.contiguous(), n, "neg_res")
         rhs = device_operand(rhs, A.shape[0], "rhs")
         mp = 0
         if missing is not None:
             if not (missing.is_cuda and missing.dtype == torch.int32 and missing.numel() == 1):
                 raise TypeError("missing: one int32 CUDA element is required")
             mp = missing.data_ptr()
-        _lib.check(self.lib.pb_tpsa_poro_fluid_rows(self.h, A.h, jf.h, C.c_void_p(neg_res.data_ptr()),
-                                                    C.c_void_p(rhs.data_ptr()), C.c_void_p(mp),
-                                                    torch.cuda.current_stream().cuda_stream))
+        _lib.check(fn(self.h, A.h, jf.h, C.c_void_p(neg_res.data_ptr()), C.c_void_p(rhs.data_ptr()), C.c_void_p(mp),
+                      torch.cuda.current_stream().cuda_stream))
 
 
 # (rows per face, columns per cell or face) of the 14 TPSA terms in PB_TPSA_* order; "k" marks kron(., I_nd), "r" the

@@ -433,6 +433,9 @@ def tpsa_poromechanics_from_model(model):
         raise NotImplementedError("TpsaPoromechanics: fractures are not supported")
     if len(sds) != 1:
         raise NotImplementedError("TpsaPoromechanics: one subdomain is expected")
+    if "energy_balance_equation" in es.equations:
+        raise NotImplementedError("TpsaPoromechanics: the TPSA thermo-poromechanics model (five fields) is not "
+                                  "supported; use tpsa_thermoporomechanics_from_model")
     sd = sds[0]
     nd, nc, nf = sd.dim, sd.num_cells, sd.num_faces
     if nd not in (2, 3):
@@ -466,4 +469,63 @@ def tpsa_poromechanics_from_model(model):
     prob.column_map = interleave(cols, nd, nr, nc)
     o = np.cumsum([0, nd * nc, nr * nc, nc, nc])
     prob.row_map = interleave([rows[o[i]:o[i + 1]] for i in range(4)], nd, nr, nc)
+    return prob, prob.column_map, prob.row_map
+
+
+def tpsa_thermoporomechanics_from_model(model):
+    """A prepared ``pp.Thermoporomechanics`` with ``TpsaPoromechanicsMixin`` on one 2-D or 3-D grid without fractures ->
+    (``TpsaThermoporomechanics``, column_map, row_map): unknown k of the problem (cell-interleaved
+    [u_c, r_c, p_t_c, p_c, T_c]) is dof ``column_map[k]`` of the model's ``EquationSystem``, equation k its row
+    ``row_map[k]``.  The mechanical boundary operator, body force, sources, Darcy, Fourier, fluid- and enthalpy-flux
+    boundary data are the model's own operators, evaluated.  The Fourier conductivity is the one of the zero state, which
+    the model discretizes with when its initial values are zero (its default); for other initial values set
+    ``prob.conductivity`` before ``discretize``."""
+    from .tpsa_thermoporomech import TpsaThermoporomechanics, interleave
+    mdg, es = model.mdg, model.equation_system
+    sds = list(mdg.subdomains())
+    if any(sd.dim < model.nd for sd in sds) or any(True for _ in mdg.interfaces()):
+        raise NotImplementedError("TpsaThermoporomechanics: fractures are not supported")
+    if len(sds) != 1:
+        raise NotImplementedError("TpsaThermoporomechanics: one subdomain is expected")
+    sd = sds[0]
+    nd, nc, nf = sd.dim, sd.num_cells, sd.num_faces
+    if nd not in (2, 3):
+        raise NotImplementedError("Tpsa is only implemented for 2d and 3d grids.")
+    nr = model.rotation_dimension()
+    fk, tk, mk = model.darcy_keyword, model.fourier_keyword, model.stress_keyword
+    data = _own_data(mdg.subdomain_data(sd), [fk, tk, mk])
+    fluid = _fluid(model, True)
+    w, we = _boundary_weights(model, sd, fluid, True)
+    ff, ef = model.bc_type_fluid_flux(sd), model.bc_type_enthalpy_flux(sd)
+    so = model.solid
+    solid = dict(reference_porosity=so.porosity, biot_coefficient=_evaluated(model, model.biot_coefficient([sd]), nc),
+                 bulk_modulus=float(np.atleast_1d(_evaluated(model, model.bulk_modulus([sd]), 1))[0]),
+                 thermal_expansion=so.thermal_expansion, heat_capacity=so.specific_heat_capacity,
+                 conductivity=so.thermal_conductivity, density=so.density)
+    prm = data[PARAMETERS]
+    prob = TpsaThermoporomechanics(
+        sd, data, fluid, solid,
+        _face_values(model, sd, prm[fk]["bc"], model.bc_values_pressure, model.bc_values_darcy_flux),
+        _face_values(model, sd, prm[tk]["bc"], model.bc_values_temperature, model.bc_values_fourier_flux),
+        _evaluated(model, model.combine_boundary_operators_mechanical_stress([sd]), nd * nf), ff,
+        _face_values(model, sd, ff, w, model.bc_values_fluid_flux), ef,
+        _face_values(model, sd, ef, we, model.bc_values_enthalpy_flux),
+        body_force=_evaluated(model, model.body_force([sd]), nd * nc),
+        angular_source=_evaluated(model, model.source_angular_momentum([sd]), nr * nc),
+        mass_source=_evaluated(model, model.solid_mass_source([sd]), nc),
+        fluid_source=_evaluated(model, model.fluid_source([sd]), nc), flow_keyword=fk, fourier_keyword=tk,
+        mechanics_keyword=mk)
+    prob.mobility_keyword, prob.enthalpy_upwind_keyword = "b200_mobility", "b200_enthalpy_upwind"
+    cols = [_dofs(model, name, sd) for name in (model.displacement_variable, model.rotation_stress_variable,
+                                                 model.total_pressure_variable, model.pressure_variable,
+                                                 model.temperature_variable)]
+    solid_mass = [eq for eq in es.equations if eq.lower().startswith("solid_mass_equation")][0]
+    rows = _row_map(model, BlockLayout([("momentum_balance_equation", [(("matrix",), nc, nd)]),
+                                        ("angular_momentum_balance_equation", [(("matrix",), nc, nr)]),
+                                        (solid_mass, [(("matrix",), nc, 1)]),
+                                        ("mass_balance_equation", [(("matrix",), nc, 1)]),
+                                        ("energy_balance_equation", [(("matrix",), nc, 1)])]))
+    prob.column_map = interleave(cols, nd, nr, nc)
+    o = np.cumsum([0, nd * nc, nr * nc, nc, nc, nc])
+    prob.row_map = interleave([rows[o[i]:o[i + 1]] for i in range(5)], nd, nr, nc)
     return prob, prob.column_map, prob.row_map

@@ -260,4 +260,5 @@ def plugin(pp, allow_reference_fallback: bool = False) -> SimpleNamespace:
                            fractured_thermoporomechanics_from_model=bridge.fractured_thermoporomechanics_from_model,
                            tpsa_momentum_from_model=bridge.tpsa_momentum_from_model,
                            tpsa_poromechanics_from_model=bridge.tpsa_poromechanics_from_model,
+                           tpsa_thermoporomechanics_from_model=bridge.tpsa_thermoporomechanics_from_model,
                            fallback_calls=fallback_calls, gpu_calls=gpu_calls)

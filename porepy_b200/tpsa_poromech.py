@@ -41,6 +41,9 @@ class TpsaPoromechanics:
     zero): ``body_force`` (nd per cell), ``angular_source`` (nr), ``mass_source`` (solid mass), ``fluid_source``."""
 
     mobility_keyword = "mobility"
+    # the FaceGrid entry points of this system and what its balance rows are called in errors
+    _fg_system, _fg_rhs, _fg_rows = "tpsa_poro_system", "tpsa_poro_rhs", "tpsa_poro_fluid_rows"
+    _rows_name = "fluid Jacobian entries outside the TPSA poromechanics row pattern"
 
     def __init__(self, sd, data: dict, fluid: dict, solid: dict, flow_bc_values, mech_bc_values, bc_fluid_flux,
                  fluid_flux_values, body_force=None, angular_source=None, mass_source=None, fluid_source=None,
@@ -98,7 +101,6 @@ class TpsaPoromechanics:
         """MPFA of the flow, the TPSA face terms and the mechanics rows of the Jacobian (device), the fluid-row pattern
         from div @ flux, and -R(0) of the mechanics rows."""
         import time
-        from .fv import Mpfa
         sd, nd = self.sd, self.nd
         if getattr(sd, "periodic_face_map", None) is not None:
             raise NotImplementedError("periodic faces are not supported by porepy_b200")
@@ -111,19 +113,27 @@ class TpsaPoromechanics:
         flags = np.zeros(self.nf, np.uint8)
         flags[np.asarray(sd.get_all_boundary_faces(), dtype=np.int64)] = 1
         t0 = time.perf_counter()
-        Mpfa(self.fk).discretize(sd, self.data)
+        self._discretize_fluxes()
         t1 = time.perf_counter()
         self._const = None
         k = self._operands()
         if self._fg is None:
             self._fg = fv.FaceGrid.for_grid(sd)
         self.lmbda = np.asarray(C.lmbda, float)
-        self.A, stage_ms = self._fg.tpsa_poro_system(nd, C.mu, self.lmbda, self.alpha, sd.cell_volumes, codes, robin,
-                                                     flags, sd.face_areas, k.div.matmul(k.flux))
-        self.b0 = self._fg.tpsa_poro_rhs(self.num_dofs, self.mech_bc, self.body_force, self.angular_source,
-                                         self.mass_source)
+        self.A, stage_ms = getattr(self._fg, self._fg_system)(nd, C.mu, self.lmbda, self.alpha, sd.cell_volumes, codes,
+                                                              robin, flags, sd.face_areas, self._balance_pattern(k))
+        self.b0 = getattr(self._fg, self._fg_rhs)(self.num_dofs, self.mech_bc, self.body_force, self.angular_source,
+                                                  self.mass_source)
         self.last_timing = dict(mpfa_s=t1 - t0, face_terms_ms=stage_ms[0], rows_ms=stage_ms[1],
                                 total_s=time.perf_counter() - t0)
+
+    def _discretize_fluxes(self) -> None:
+        from .fv import Mpfa
+        Mpfa(self.fk).discretize(self.sd, self.data)
+
+    def _balance_pattern(self, k):
+        """The nc x nc pattern of the couplings of the balance rows to the other cells: div @ flux."""
+        return k.div.matmul(k.flux)
 
     def _operands(self):
         if self._const is None:
@@ -147,9 +157,9 @@ class TpsaPoromechanics:
         return (p - self.p_ref) * k.n_inv + (pt + p * k.alpha) * k.a_lam + self.phi_ref
 
     def _fields(self, x):
-        """(p_t, p) of a cell-interleaved vector, as contiguous device vectors."""
+        """(p_t, p) of a cell-interleaved vector, as contiguous device vectors (the scalar fields after r_c)."""
         x = ad.device_vector(x).reshape(self.nc, self.block_size)
-        return x[:, -2].contiguous(), x[:, -1].contiguous()
+        return tuple(x[:, j].contiguous() for j in range(self.nd + self.nr, self.block_size))
 
     def update_upwind(self, p) -> None:
         k = self._operands()
@@ -169,6 +179,11 @@ class TpsaPoromechanics:
         ff = advective_flux(T, q, w, k.bcw, k.bcw)
         return (mass - mass_n) * (1.0 / dt) + (k.div @ ff) - k.src
 
+    def balance_rows(self, x, x_prev, dt: float):
+        """(field-ordered Jacobian, -R) of the balance rows at the iterate ``x``: here the fluid mass balance."""
+        eq = self.fluid_equation(x, x_prev, dt)
+        return eq.jac, -eq.val
+
     def linearize(self, x, x_prev, dt: float):
         """(J as ``DeviceCsr``, -R as a CUDA tensor) in the cell-interleaved order: upwind directions from ``x``, the
         fluid rows from the AD chain written into the fixed pattern, -R of the mechanics rows = b0 - A x.  ``J`` is
@@ -180,11 +195,11 @@ class TpsaPoromechanics:
         if x.numel() != self.num_dofs:
             raise ValueError(f"x must have {self.num_dofs} values")
         self.update_upwind(self._fields(x)[1])
-        eq = self.fluid_equation(x, x_prev, dt)
+        jac, neg_res = self.balance_rows(x, x_prev, dt)
         rhs = self.b0 - (self.A @ x)
         if getattr(self, "_missing", None) is None:
             self._missing = torch.zeros(1, dtype=torch.int32, device=rhs.device)
-        self._fg.tpsa_poro_fluid_rows(self.A, eq.jac, -eq.val, rhs, self._missing)
+        getattr(self._fg, self._fg_rows)(self.A, jac, neg_res, rhs, self._missing)
         return self.A, rhs
 
     def time_step(self, x_prev, dt: float, tol: float = 1e-10, max_iterations: int = 15, linear_tol: float = 1e-10,
@@ -196,7 +211,7 @@ class TpsaPoromechanics:
         def linearize(x):
             J, rhs = self.linearize(x, x_prev, dt)
             if int(self._missing.sum()):
-                raise RuntimeError("fluid Jacobian entries outside the TPSA poromechanics row pattern")
+                raise RuntimeError(self._rows_name)
             return J, rhs
         if linear_solver is None:
             linear_solver = krylov.bicgstab_solver(linear_tol, block_size=self.block_size)
@@ -218,11 +233,11 @@ class TpsaPoromechanics:
 
 
 def interleave(blocks, nd: int, nr: int, nc: int) -> np.ndarray:
-    """Cell-interleaved order [u_c, r_c, p_t_c, p_c] from the four field-wise index arrays."""
-    u, r, pt, p = (np.asarray(x, np.int64) for x in blocks)
-    out = np.empty((nc, nd + nr + 2), np.int64)
+    """Cell-interleaved order [u_c, r_c, p_t_c, p_c] (or [u_c, r_c, p_t_c, p_c, T_c]) from the field-wise index arrays."""
+    u, r, *scalars = (np.asarray(x, np.int64) for x in blocks)
+    out = np.empty((nc, nd + nr + len(scalars)), np.int64)
     out[:, :nd] = u.reshape(nc, nd)
     out[:, nd:nd + nr] = r.reshape(nc, nr)
-    out[:, nd + nr] = pt
-    out[:, nd + nr + 1] = p
+    for j, v in enumerate(scalars):
+        out[:, nd + nr + j] = v
     return out.reshape(-1)

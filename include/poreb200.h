@@ -376,6 +376,49 @@ int pb_tpsa_thm_rhs(pb_facegrid *g, const double *bc_values, const double *body_
 int pb_tpsa_thm_balance_rows(pb_facegrid *g, struct pb_csr *a, const struct pb_csr *jf, const double *neg_res_dev,
                              double *rhs_dev, int *missing_dev, uint64_t stream);
 
+/* The Jacobian of the TPSA elasticity model with fractures in frictional contact (pp.MomentumBalance +
+ * TpsaMomentumBalanceMixin on a fractured medium; reference models/momentum_balance.py:127-183,
+ * models/constitutive_laws.py:3064-3248, models/contact_mechanics.py:80-245) on a 2-D or 3-D matrix whose fracture faces
+ * are internal Dirichlet faces (one cell each) matched one to one with the mortar cells of the interfaces.  Fracture cells
+ * (nk) and mortar cells (nm = 2 nk) are numbered over all fractures / interfaces one after the other.
+ *   unknowns   [u_c, r_c, p_c per cell (B = nd+nr+1) | t: nd per fracture cell | u_j: nd per mortar cell]
+ *   equations  [the three TPSA balances per cell | interface force balance: nd per mortar cell | normal law: one per
+ *               fracture cell | tangential law: nd-1 per fracture cell]
+ * The balance rows are those of pb_tpsa_system with the interface displacement on the fracture faces, g + Pi^avg u_j:
+ * momentum row i of c gains -s_f B_s[f,i] w_m2p in column u_j(m,i), the angular and solid-mass rows +s_f B_r[f] w_m2p
+ * and +s_f B_m[f] w_m2p in the nd columns of u_j(m) (s_f: the sign of c on f).  Force row (m, i) is
+ * w_p2m s_f sigma[f,i] + vol_m T_c sign_m sum_j R_k[j,i] t_k,j with the three-field stress
+ * sigma = S_u u + S_r r + S_p p + B_s (g + w_m2p u_j).  Each contact row holds the 3 nd columns [t_k | u_j(m1) | u_j(m2)],
+ * 0 until pb_tpsa_contact_rows writes them.  Rows are sorted.
+ * pb_tpsa_contact_system: the matrix as a new device CSR.  Arguments as for pb_tpsa_system, plus per mortar cell (host
+ * arrays of num_mortar): its matrix face, fracture cell, mortar_to_primary_avg and primary_to_mortar_int weights, side
+ * sign and volume (times its secondary_to_mortar_int weight); frames: the nd x nd local coordinates of every fracture cell,
+ * row-major (the nd-1 tangents, then the normal); characteristic_traction: T_c.  A face with more than one mortar cell,
+ * a fracture face without exactly one cell, a fracture cell without exactly two mortar cells or an index out of range
+ * is PB_EINVAL.  The row pattern is built on the device at the first call for a dimension and interface topology and
+ * kept on the handle; the patterns of pb_tpsa_system / pb_tpsa_poro_system / pb_tpsa_thm_system are not touched.  The
+ * face values are shared: like those entry points, a call replaces the face values that pb_tpsa_rhs, pb_tpsa_poro_rhs and
+ * pb_tpsa_thm_rhs read (the right-hand sides follow the last system assembled on g).  No
+ * atomics: two calls give bit-identical values.  stage_ms (may be NULL): device times of the face kernel and of the
+ * row writes, 2 floats.
+ * pb_tpsa_contact_rhs: b = -R(0) of the balance and force rows (the right-hand side of pb_tpsa_rhs, and
+ * -w_p2m s_f B_s g in the force rows), 0 in the contact rows, to the DEVICE array rhs_dev.  Reads the face values of
+ * the last system assembled on g.
+ * pb_tpsa_contact_rows: the contact rows at one Newton step, on `stream`, nothing copied to the host: row r of jc
+ * (nd nk x nd (nk + nm) device CSR, the Jacobian of the [normal | tangential] laws in the variables [t | u_j]) into the
+ * fixed pattern of a at column offset B nc, and neg_res_dev[r] into the entry of rhs_dev of that row.  Entries of jc
+ * outside the pattern are counted into *missing_dev (device int, may be NULL). */
+int pb_tpsa_contact_system(pb_facegrid *g, int nd, const double *mu, const double *lambda, const double *cell_volumes,
+                           const uint8_t *codes, const double *robin_diag, const uint8_t *face_flags,
+                           int64_t num_mortar, int64_t num_fracture_cells, const int32_t *mortar_face,
+                           const int32_t *mortar_cell, const double *m2p_weight, const double *p2m_weight,
+                           const double *mortar_sign, const double *mortar_volume, const double *frames,
+                           double characteristic_traction, struct pb_csr **out, float *stage_ms);
+int pb_tpsa_contact_rhs(pb_facegrid *g, const double *bc_values, const double *body_force, const double *angular_source,
+                        const double *mass_source, double *rhs_dev);
+int pb_tpsa_contact_rows(pb_facegrid *g, struct pb_csr *a, const struct pb_csr *jc, const double *neg_res_dev,
+                         double *rhs_dev, int *missing_dev, uint64_t stream);
+
 /* Interface upwinding (UpwindCoupling.discretize, numerics/fv/upwind.py:427-528): per mortar cell the sign of the
  * interface flux and the masks "upstream is the higher-dimensional side" / "... the lower-dimensional side".
  * Host pointers, n doubles each. */

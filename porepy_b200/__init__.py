@@ -23,10 +23,11 @@ from .thermoporomech import Thermoporomechanics  # noqa: F401
 from .tpsa_elasticity import TpsaElasticity  # noqa: F401
 from .tpsa_poromech import TpsaPoromechanics  # noqa: F401
 from .tpsa_thermoporomech import TpsaThermoporomechanics  # noqa: F401
+from .tpsa_contact import TpsaFracturedMomentumBalance  # noqa: F401
 from .tpfa_ad import DifferentiableTpfa  # noqa: F401
 
 __all__ = ["Mpfa", "Mpsa", "Biot", "Tpfa", "Tpsa", "Upwind", "UpwindCoupling", "DevicePlan", "FaceGrid", "DeviceCsr", "Grid", "cart_grid_2d", "cart_grid_3d",
            "structured_tet_grid", "tet_grid_from_cells", "SecondOrderTensor", "FourthOrderTensor",
            "BoundaryCondition", "BoundaryConditionVectorial", "initialize_data", "PARAMETERS",
            "DISCRETIZATION_MATRICES", "determine_eta", "compute_geometry", "DifferentiableTpfa",
-           "MixedDimensionalFlow", "MdSubdomain", "MdInterface", "CompressibleMixedDimensionalFlow", "Poromechanics", "Thermoporomechanics", "MixedDimensionalMassEnergy", "FracturedMomentumBalance", "FractureContact", "FracturedPoromechanics", "FractureCoupling", "FracturedThermoporomechanics", "TpsaElasticity", "TpsaPoromechanics", "TpsaThermoporomechanics"]
+           "MixedDimensionalFlow", "MdSubdomain", "MdInterface", "CompressibleMixedDimensionalFlow", "Poromechanics", "Thermoporomechanics", "MixedDimensionalMassEnergy", "FracturedMomentumBalance", "FractureContact", "FracturedPoromechanics", "FractureCoupling", "FracturedThermoporomechanics", "TpsaElasticity", "TpsaPoromechanics", "TpsaThermoporomechanics", "TpsaFracturedMomentumBalance"]

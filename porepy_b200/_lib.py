@@ -82,6 +82,12 @@ _SIGNATURES = {
     "pb_tpsa_thm_rhs": (C.c_int, [C.c_void_p, _f64p, _f64p, _f64p, _f64p, C.c_void_p]),
     "pb_tpsa_thm_balance_rows": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
                                            C.c_uint64]),
+    "pb_tpsa_contact_system": (C.c_int, [C.c_void_p, C.c_int, _f64p, _f64p, _f64p, _u8p, _f64p, _u8p, C.c_int64,
+                                         C.c_int64, _i32p, _i32p] + [_f64p] * 5 + [C.c_double, C.POINTER(C.c_void_p),
+                                                                                   _f32p]),
+    "pb_tpsa_contact_rhs": (C.c_int, [C.c_void_p, _f64p, _f64p, _f64p, _f64p, C.c_void_p]),
+    "pb_tpsa_contact_rows": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                       C.c_uint64]),
     "pb_upwind_coupling": (C.c_int, [C.c_int64, _f64p, _f64p, _f64p, _f64p]),
     "pb_compute_geometry_3d": (C.c_int, [C.c_int64, C.c_int64, C.c_int64, _i32p, _i32p, _i8p, _i32p, _i32p] + [_f64p] * 6
                                + [_f32p]),

@@ -25,6 +25,13 @@ struct pb_facegrid {
     int poro_nd = 0, poro_ns = 0;
     int64_t poro_nnz = 0, poro_fp_nnz = -1;
     DevBuf blk_ptr, poro_ip, poro_ix;
+    // TPSA contact system (pb_tpsa_contact_system): the interfaces of the last call (host copies of their topology) and
+    // the row pattern, built once per dimension and interface topology
+    int ctc_nd = 0;
+    int64_t ctc_nm = -1, ctc_nk = -1, ctc_ncell = 0, ctc_nnz = 0;
+    double ctc_ct = 0.0;
+    std::vector<int32_t> ctc_face_h, ctc_cell_h;
+    DevBuf ctc_fm, ctc_face, ctc_cell, ctc_pair, ctc_w, ctc_frame, ctc_blk, ctc_ip, ctc_ix;
 };
 
 // one thread per cell: claim the first free slot of each of its faces
@@ -904,4 +911,328 @@ extern "C" int pb_tpsa_thm_rhs(pb_facegrid *g, const double *bc_values, const do
 extern "C" int pb_tpsa_thm_balance_rows(pb_facegrid *g, pb_csr *a, const pb_csr *jf, const double *neg_res_dev,
                                         double *rhs_dev, int *missing_dev, uint64_t stream) {
     return tpsa_poro_fluid_rows<2>(g, a, jf, neg_res_dev, rhs_dev, missing_dev, stream);
+}
+
+// ---- TPSA elasticity with fractures in frictional contact (tpsa_system.cuh) ---------------------------------------
+template <int ND>
+__global__ void tpsa_contact_count_kernel(TpsaTopo t, const int32_t *__restrict__ cc_ptr,
+                                          const int32_t *__restrict__ face_mortar, int32_t *__restrict__ count) {
+    using D = TpsaContactDims<ND>;
+    for (int64_t c = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; c < t.nc; c += (int64_t)gridDim.x * blockDim.x)
+        count[c] = D::M::NZ * (cc_ptr[c + 1] - cc_ptr[c]) + D::EXT * tpsa_contact_nfrac(c, t, face_mortar);
+}
+
+template <int ND>
+__global__ void tpsa_contact_pattern_kernel(TpsaTopo t, const int32_t *__restrict__ cc_ptr,
+                                            const int32_t *__restrict__ cc_ix, const int64_t *__restrict__ blk_ptr,
+                                            TpsaMortars I, int32_t *__restrict__ ip, int32_t *__restrict__ ix) {
+    for (int64_t c = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; c < t.nc; c += (int64_t)gridDim.x * blockDim.x)
+        tpsa_contact_pattern_rows<ND>(c, cc_ptr[c + 1] - cc_ptr[c], cc_ix + cc_ptr[c], blk_ptr[c], t, I, ip, ix);
+}
+
+// one thread per interface row (force and contact rows)
+template <int ND>
+__global__ void tpsa_contact_iface_pattern_kernel(TpsaTopo t, const int64_t *__restrict__ blk_ptr, TpsaMortars I,
+                                                  int32_t *__restrict__ ip, int32_t *__restrict__ ix) {
+    const int64_t n = (int64_t)ND * (I.nm + I.nk);
+    for (int64_t q = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; q < n; q += (int64_t)gridDim.x * blockDim.x)
+        tpsa_contact_iface_pattern<ND>(q, t.nc, blk_ptr[t.nc], t, I, ip, ix);
+}
+
+// one thread per block (c, k), as tpsa_system_kernel
+template <int ND>
+__global__ void tpsa_contact_block_kernel(int64_t npairs, TpsaTopo t, const int32_t *__restrict__ cc_ptr,
+                                          const int32_t *__restrict__ cc_ix, const int32_t *__restrict__ cc_cell,
+                                          const int64_t *__restrict__ blk_ptr, TpsaMortars I, TpsaTerms T,
+                                          const double *__restrict__ mu, const double *__restrict__ lam,
+                                          const double *__restrict__ vol, double *__restrict__ a) {
+    for (int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; e < npairs; e += (int64_t)gridDim.x * blockDim.x) {
+        const int64_t c = cc_cell[e];
+        tpsa_contact_block<ND>(c, (int)(e - cc_ptr[c]), t, cc_ptr, cc_ix, blk_ptr, I, T, mu, lam, vol, a);
+    }
+}
+
+template <int ND>
+__global__ void tpsa_contact_iface_kernel(TpsaTopo t, const int64_t *__restrict__ blk_ptr, TpsaMortars I, TpsaTerms T,
+                                          double *__restrict__ a) {
+    const int64_t n = (int64_t)ND * (I.nm + I.nk);
+    for (int64_t q = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; q < n; q += (int64_t)gridDim.x * blockDim.x)
+        tpsa_contact_iface_row<ND>(q, blk_ptr[t.nc], t, I, T, a);
+}
+
+template <int ND>
+__global__ void tpsa_contact_rhs_kernel(TpsaTopo t, TpsaMortars I, TpsaTerms T, const double *__restrict__ g,
+                                        const double *__restrict__ f, const double *__restrict__ sr,
+                                        const double *__restrict__ sp, double *__restrict__ b) {
+    constexpr int NR = TpsaDims<ND>::NR, B = TpsaDims<ND>::B;
+    const int64_t n = t.nc * B + (int64_t)ND * (I.nm + I.nk);
+    for (int64_t q = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; q < n; q += (int64_t)gridDim.x * blockDim.x) {
+        if (q >= t.nc * B) { b[q] = tpsa_contact_iface_rhs<ND>(q - t.nc * B, t, I, T, g); continue; }
+        const int64_t c = q / B;
+        const int l = (int)(q - c * B);
+        const double src = l < ND ? (f ? f[c * ND + l] : 0.0)
+                                   : (l < ND + NR ? (sr ? sr[c * NR + l - ND] : 0.0) : (sp ? sp[c] : 0.0));
+        b[q] = tpsa_rhs_row<ND>(c, l, t, T, g, src);
+    }
+}
+
+// one thread per contact row
+template <int ND>
+__global__ void tpsa_contact_law_kernel(int64_t nrows, int64_t c0, int64_t row0, int64_t e0,
+                                        const int32_t *__restrict__ ix, const int32_t *__restrict__ jc_ip,
+                                        const int32_t *__restrict__ jc_ix, const double *__restrict__ jc_a,
+                                        const double *__restrict__ neg_res, double *__restrict__ a,
+                                        double *__restrict__ b, int *__restrict__ missing) {
+    for (int64_t r = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; r < nrows; r += (int64_t)gridDim.x * blockDim.x) {
+        const int m = tpsa_contact_law_row<ND>(r, c0, e0, row0 + r, ix, jc_ip, jc_ix, jc_a, neg_res, a, b);
+        if (m && missing) atomicAdd(missing, m);
+    }
+}
+
+static TpsaMortars tpsa_mortars(pb_facegrid *g) {
+    const int64_t nm = g->ctc_nm;
+    const double *w = g->ctc_w.as<double>();
+    return TpsaMortars{nm, g->ctc_nk, g->ctc_face.as<int32_t>(), g->ctc_cell.as<int32_t>(), g->ctc_fm.as<int32_t>(),
+                       g->ctc_pair.as<int32_t>(), w, w + nm, w + 2 * nm, w + 3 * nm, g->ctc_frame.as<double>(), g->ctc_ct};
+}
+
+// Row pattern of the contact system: neighbour lists (shared with the other TPSA systems), block-row offsets and the
+// CSR arrays, from the interface topology already on the handle.
+static int tpsa_contact_build_pattern(pb_facegrid *g, int nd) {
+    cudaStream_t st = g->stream;
+    const int64_t nc = g->nc, nm = g->ctc_nm, nk = g->ctc_nk;
+    const int B = nd == 3 ? 7 : 4;
+    const TpsaTopo t = tpsa_topo(g);
+    if (!g->nb_ready) {
+        int64_t total = 0;
+        int rc = tpsa_neighbour_counts(g, &total);
+        if (rc) return rc;
+        tpsa_nb_list_kernel<<<fg_grid(nc), 256, 0, st>>>(t, g->cc_ptr.as<int32_t>(), g->cc_ix.as<int32_t>(),
+                                                          g->cc_cell.as<int32_t>());
+        pb_count_launch_();
+        CUDA_TRY(cudaGetLastError());
+        g->sys_npairs = total;
+        g->nb_ready = true;
+    }
+    const TpsaMortars I = tpsa_mortars(g);
+    DevBuf count;
+    CUDA_TRY(count.ensure((size_t)nc * sizeof(int32_t)));
+    if (nd == 3) tpsa_contact_count_kernel<3><<<fg_grid(nc), 256, 0, st>>>(t, g->cc_ptr.as<int32_t>(), I.face_mortar, count.as<int32_t>());
+    else tpsa_contact_count_kernel<2><<<fg_grid(nc), 256, 0, st>>>(t, g->cc_ptr.as<int32_t>(), I.face_mortar, count.as<int32_t>());
+    pb_count_launch_();
+    CUDA_TRY(cudaGetLastError());
+    CUDA_TRY(g->ctc_blk.ensure((size_t)(nc + 1) * sizeof(int64_t)));
+    int64_t ncell = 0;
+    const int rc = pb_scan_offsets_(count.as<int32_t>(), g->ctc_blk.as<int64_t>(), nc, st, &ncell);
+    if (rc) return rc;
+    const int64_t nr = nd == 3 ? 3 : 1, nnz = ncell + (int64_t)nd * nm * (nd + nr + 3) + (int64_t)nd * nk * 3 * nd;
+    if (nnz >= 0x7FFFFFFFll) return pb_fail_(PB_ENOTIMPL, "Tpsa system: the matrix does not fit int32 indices");
+    const int64_t nrows = nc * B + (int64_t)nd * (nm + nk);
+    CUDA_TRY(g->ctc_ip.ensure((size_t)(nrows + 1) * sizeof(int32_t)));
+    CUDA_TRY(g->ctc_ix.ensure((size_t)std::max<int64_t>(1, nnz) * sizeof(int32_t)));
+    const int32_t last = (int32_t)nnz;
+    CUDA_TRY(cudaMemcpyAsync(g->ctc_ip.as<int32_t>() + nrows, &last, sizeof(int32_t), cudaMemcpyHostToDevice, st));
+    const int64_t ni = (int64_t)nd * (nm + nk);
+    if (nd == 3) {
+        tpsa_contact_pattern_kernel<3><<<fg_grid(nc), 256, 0, st>>>(t, g->cc_ptr.as<int32_t>(), g->cc_ix.as<int32_t>(),
+                                                                     g->ctc_blk.as<int64_t>(), I, g->ctc_ip.as<int32_t>(),
+                                                                     g->ctc_ix.as<int32_t>());
+        if (ni) tpsa_contact_iface_pattern_kernel<3><<<fg_grid(ni), 256, 0, st>>>(t, g->ctc_blk.as<int64_t>(), I,
+                                                                              g->ctc_ip.as<int32_t>(), g->ctc_ix.as<int32_t>());
+    } else {
+        tpsa_contact_pattern_kernel<2><<<fg_grid(nc), 256, 0, st>>>(t, g->cc_ptr.as<int32_t>(), g->cc_ix.as<int32_t>(),
+                                                                     g->ctc_blk.as<int64_t>(), I, g->ctc_ip.as<int32_t>(),
+                                                                     g->ctc_ix.as<int32_t>());
+        if (ni) tpsa_contact_iface_pattern_kernel<2><<<fg_grid(ni), 256, 0, st>>>(t, g->ctc_blk.as<int64_t>(), I,
+                                                                              g->ctc_ip.as<int32_t>(), g->ctc_ix.as<int32_t>());
+    }
+    pb_count_launch_();
+    CUDA_TRY(cudaGetLastError());
+    CUDA_TRY(cudaStreamSynchronize(st));
+    g->ctc_nd = nd;
+    g->ctc_ncell = ncell;
+    g->ctc_nnz = nnz;
+    return PB_OK;
+}
+
+// Checks the interface description and puts it on the handle; *same: its topology is the one of the cached pattern.
+static int tpsa_contact_interfaces(pb_facegrid *g, int nd, int64_t nm, int64_t nk, const int32_t *mortar_face,
+                                   const int32_t *mortar_cell, const double *m2p, const double *p2m, const double *sign,
+                                   const double *vol, const double *frames, double ct, bool *same) {
+    const int64_t nf = g->nf;
+    if (nm < 0 || nk < 0 || nm != 2 * nk) return pb_fail_(PB_EINVAL, "every fracture cell needs two mortar cells");
+    if (nm && (!mortar_face || !mortar_cell || !m2p || !p2m || !sign || !vol || !frames))
+        return pb_fail_(PB_EINVAL, "null pointer");
+    if (!std::isfinite(ct)) return pb_fail_(PB_EINVAL, "characteristic traction must be finite");
+    std::vector<int32_t> fm((size_t)nf, -1), pair((size_t)2 * nk, -1);
+    for (int64_t m = 0; m < nm; ++m) {
+        const int32_t f = mortar_face[m], k = mortar_cell[m];
+        if (f < 0 || f >= nf || k < 0 || k >= nk) return pb_fail_(PB_EINVAL, "mortar face or fracture cell out of range");
+        if (fm[f] >= 0) return pb_fail_(PB_EINVAL, "a face with more than one mortar cell (non-matching mortar grid)");
+        if (g->face_ncell[f] != 1) return pb_fail_(PB_EINVAL, "a fracture face must have exactly one cell");
+        fm[f] = (int32_t)m;
+        if (pair[2 * k] < 0) pair[2 * k] = (int32_t)m;
+        else if (pair[2 * k + 1] < 0) pair[2 * k + 1] = (int32_t)m;
+        else return pb_fail_(PB_EINVAL, "a fracture cell with more than two mortar cells");
+        for (const double *v : {m2p + m, p2m + m, sign + m, vol + m})
+            if (!std::isfinite(*v)) return pb_fail_(PB_EINVAL, "mortar weights must be finite");
+    }
+    for (int64_t q = 0; q < (int64_t)nd * nd * nk; ++q)
+        if (!std::isfinite(frames[q])) return pb_fail_(PB_EINVAL, "local coordinates must be finite");
+    *same = g->ctc_nm == nm && g->ctc_nk == nk &&
+            std::equal(mortar_face, mortar_face + nm, g->ctc_face_h.begin()) &&
+            std::equal(mortar_cell, mortar_cell + nm, g->ctc_cell_h.begin());
+    cudaStream_t st = g->stream;
+    std::vector<double> w((size_t)std::max<int64_t>(1, 4 * nm));
+    for (int64_t m = 0; m < nm; ++m) { w[m] = m2p[m]; w[nm + m] = p2m[m]; w[2 * nm + m] = sign[m]; w[3 * nm + m] = vol[m]; }
+    std::vector<int32_t> face_h(mortar_face, mortar_face + nm), cell_h(mortar_cell, mortar_cell + nm);
+    face_h.push_back(0);
+    cell_h.push_back(0);
+    for (int64_t k = 0; k < nk; ++k)
+        if (pair[2 * k] > pair[2 * k + 1]) std::swap(pair[2 * k], pair[2 * k + 1]);
+    pair.push_back(0);
+    CUDA_TRY(g->ctc_fm.upload(fm, st));
+    CUDA_TRY(g->ctc_face.upload(face_h, st));
+    CUDA_TRY(g->ctc_cell.upload(cell_h, st));
+    CUDA_TRY(g->ctc_pair.upload(pair, st));
+    CUDA_TRY(g->ctc_w.upload(w, st));
+    std::vector<double> fr((size_t)nd * nd * nk + 1, 0.0);
+    if (nk) std::copy(frames, frames + (size_t)nd * nd * nk, fr.begin());
+    CUDA_TRY(g->ctc_frame.upload(fr, st));
+    CUDA_TRY(cudaStreamSynchronize(st));
+    face_h.pop_back();
+    cell_h.pop_back();
+    g->ctc_face_h = face_h;
+    g->ctc_cell_h = cell_h;
+    g->ctc_nm = nm;
+    g->ctc_nk = nk;
+    g->ctc_ct = ct;
+    return PB_OK;
+}
+
+extern "C" int pb_tpsa_contact_system(pb_facegrid *g, int nd, const double *mu, const double *lambda,
+                                      const double *cell_volumes, const uint8_t *codes, const double *robin_diag,
+                                      const uint8_t *face_flags, int64_t num_mortar, int64_t num_fracture_cells,
+                                      const int32_t *mortar_face, const int32_t *mortar_cell, const double *m2p_weight,
+                                      const double *p2m_weight, const double *mortar_sign, const double *mortar_volume,
+                                      const double *frames, double characteristic_traction, pb_csr **out,
+                                      float *stage_ms) {
+    if (!g || !mu || !lambda || !cell_volumes || !codes || !face_flags || !out)
+        return pb_fail_(PB_EINVAL, "null pointer");
+    TpsaInputs in;
+    int rc = tpsa_prepare(g, nd, mu, lambda, cell_volumes, codes, robin_diag, face_flags, in);
+    if (rc) return rc;
+    bool same = false;
+    const bool had = g->ctc_nd == nd;
+    g->ctc_nd = 0;   // set again once the pattern on the handle belongs to the interfaces uploaded below
+    rc = tpsa_contact_interfaces(g, nd, num_mortar, num_fracture_cells, mortar_face, mortar_cell, m2p_weight,
+                                 p2m_weight, mortar_sign, mortar_volume, frames, characteristic_traction, &same);
+    if (rc) return rc;
+    if (had && same) g->ctc_nd = nd;
+    else if ((rc = tpsa_contact_build_pattern(g, nd))) return rc;
+    cudaStream_t st = g->stream;
+    const int64_t nc = g->nc, nrows = nc * (nd == 3 ? 7 : 4) + (int64_t)nd * (g->ctc_nm + g->ctc_nk);
+    pb_csr *a = nullptr;
+    rc = pb_csr_from_device_pattern_(nrows, nrows, g->ctc_nnz, g->ctc_ip.as<int32_t>(), g->ctc_ix.as<int32_t>(), &a);
+    if (rc) return rc;
+    FgEvents ev;
+    auto fail_cuda = [&](cudaError_t e, const char *what) {
+        pb_csr_destroy(a);
+        return pb_fail_(PB_ECUDA, std::string(what) + ": " + cudaGetErrorString(e));
+    };
+#define SYS_TRY(x) do { cudaError_t e_ = (x); if (e_ != cudaSuccess) return fail_cuda(e_, #x); } while (0)
+    if (stage_ms)
+        for (auto &x : ev.e) SYS_TRY(cudaEventCreate(&x));
+    if (stage_ms) SYS_TRY(cudaEventRecord(ev.e[0], st));
+    TpsaTerms T{};
+    if ((rc = tpsa_face_terms(g, nd, in, T))) { pb_csr_destroy(a); return rc; }
+    if (stage_ms) SYS_TRY(cudaEventRecord(ev.e[1], st));
+    const TpsaTopo t = tpsa_topo(g);
+    const TpsaMortars I = tpsa_mortars(g);
+    const int64_t np = g->sys_npairs, ni = (int64_t)nd * (g->ctc_nm + g->ctc_nk);
+    double *av = pb_csr_data_(a);
+    if (nd == 3) {
+        tpsa_contact_block_kernel<3><<<fg_grid(np), 256, 0, st>>>(np, t, g->cc_ptr.as<int32_t>(), g->cc_ix.as<int32_t>(),
+                                                                   g->cc_cell.as<int32_t>(), g->ctc_blk.as<int64_t>(), I, T,
+                                                                   in.mu.as<double>(), in.lam.as<double>(),
+                                                                   in.vol.as<double>(), av);
+        if (ni) tpsa_contact_iface_kernel<3><<<fg_grid(ni), 256, 0, st>>>(t, g->ctc_blk.as<int64_t>(), I, T, av);
+    } else {
+        tpsa_contact_block_kernel<2><<<fg_grid(np), 256, 0, st>>>(np, t, g->cc_ptr.as<int32_t>(), g->cc_ix.as<int32_t>(),
+                                                                   g->cc_cell.as<int32_t>(), g->ctc_blk.as<int64_t>(), I, T,
+                                                                   in.mu.as<double>(), in.lam.as<double>(),
+                                                                   in.vol.as<double>(), av);
+        if (ni) tpsa_contact_iface_kernel<2><<<fg_grid(ni), 256, 0, st>>>(t, g->ctc_blk.as<int64_t>(), I, T, av);
+    }
+    pb_count_launch_();
+    SYS_TRY(cudaGetLastError());
+    if (stage_ms) SYS_TRY(cudaEventRecord(ev.e[2], st));
+    SYS_TRY(cudaStreamSynchronize(st));
+    if (stage_ms) {
+        SYS_TRY(cudaEventElapsedTime(stage_ms, ev.e[0], ev.e[1]));
+        SYS_TRY(cudaEventElapsedTime(stage_ms + 1, ev.e[1], ev.e[2]));
+    }
+#undef SYS_TRY
+    g->terms_nd = nd;
+    *out = a;
+    return PB_OK;
+}
+
+extern "C" int pb_tpsa_contact_rhs(pb_facegrid *g, const double *bc_values, const double *body_force,
+                                   const double *angular_source, const double *mass_source, double *rhs_dev) {
+    if (!g || !bc_values || !rhs_dev) return pb_fail_(PB_EINVAL, "null pointer");
+    const int nd = g->ctc_nd;
+    if ((nd != 2 && nd != 3) || g->terms_nd != nd) return pb_fail_(PB_EINVAL, "pb_tpsa_contact_system has not been called");
+    const int64_t nf = g->nf, nc = g->nc;
+    const int nr = nd == 3 ? 3 : 1;
+    cudaStream_t st = g->stream;
+    DevBuf dg, df, dsr, dsp;
+    CUDA_TRY(dg.upload(bc_values, (size_t)nd * nf, st));
+    if (body_force) CUDA_TRY(df.upload(body_force, (size_t)nd * nc, st));
+    if (angular_source) CUDA_TRY(dsr.upload(angular_source, (size_t)nr * nc, st));
+    if (mass_source) CUDA_TRY(dsp.upload(mass_source, (size_t)nc, st));
+    TpsaTerms T{};
+    for (int k = PB_TPSA_BOUND_STRESS; k <= PB_TPSA_BOUND_MASS_DISPLACEMENT; ++k) T.t[k] = g->terms[k].as<double>();
+    const TpsaTopo t = tpsa_topo(g);
+    const TpsaMortars I = tpsa_mortars(g);
+    const int64_t rows = nc * (nd + nr + 1) + (int64_t)nd * (g->ctc_nm + g->ctc_nk);
+    const double *pf = body_force ? df.as<double>() : nullptr, *psr = angular_source ? dsr.as<double>() : nullptr,
+                 *psp = mass_source ? dsp.as<double>() : nullptr;
+    if (nd == 3) tpsa_contact_rhs_kernel<3><<<fg_grid(rows), 256, 0, st>>>(t, I, T, dg.as<double>(), pf, psr, psp, rhs_dev);
+    else tpsa_contact_rhs_kernel<2><<<fg_grid(rows), 256, 0, st>>>(t, I, T, dg.as<double>(), pf, psr, psp, rhs_dev);
+    pb_count_launch_();
+    CUDA_TRY(cudaGetLastError());
+    CUDA_TRY(cudaStreamSynchronize(st));
+    return PB_OK;
+}
+
+extern "C" int pb_tpsa_contact_rows(pb_facegrid *g, pb_csr *a, const pb_csr *jc, const double *neg_res_dev,
+                                    double *rhs_dev, int *missing_dev, uint64_t stream) {
+    if (!g || !a || !jc || !neg_res_dev || !rhs_dev) return pb_fail_(PB_EINVAL, "null pointer");
+    const int nd = g->ctc_nd;
+    if (nd != 2 && nd != 3) return pb_fail_(PB_EINVAL, "pb_tpsa_contact_system has not been called");
+    const int64_t nc = g->nc, nm = g->ctc_nm, nk = g->ctc_nk, c0 = nc * (nd == 3 ? 7 : 4);
+    const int64_t nrows = c0 + (int64_t)nd * (nm + nk);
+    const CsrView va = pb_csr_view_(a), vj = pb_csr_view_(jc);
+    if (va.nrows != nrows || va.ncols != nrows || va.nnz != g->ctc_nnz)
+        return pb_fail_(PB_EINVAL, "the matrix is not the TPSA contact system of this grid");
+    if (vj.nrows != (int64_t)nd * nk || vj.ncols != (int64_t)nd * (nk + nm))
+        return pb_fail_(PB_EINVAL, "contact Jacobian must be nd num_fracture_cells x nd (num_fracture_cells + num_mortar) "
+                                   "([t | u_j])");
+    if (!nk) return PB_OK;
+    cudaStream_t st = (cudaStream_t)stream;
+    // the contact rows start nd nm LF entries after the balance rows
+    const int64_t lf = nd + (nd == 3 ? 3 : 1) + 3, e0 = g->ctc_ncell + (int64_t)nd * nm * lf;
+    const int64_t n = (int64_t)nd * nk;
+    if (nd == 3)
+        tpsa_contact_law_kernel<3><<<fg_grid(n), 256, 0, st>>>(n, c0, c0 + (int64_t)nd * nm, e0, va.indices,
+                                                               vj.indptr, vj.indices, vj.data, neg_res_dev, va.data,
+                                                               rhs_dev, missing_dev);
+    else
+        tpsa_contact_law_kernel<2><<<fg_grid(n), 256, 0, st>>>(n, c0, c0 + (int64_t)nd * nm, e0, va.indices,
+                                                               vj.indptr, vj.indices, vj.data, neg_res_dev, va.data,
+                                                               rhs_dev, missing_dev);
+    pb_count_launch_();
+    CUDA_TRY(cudaGetLastError());
+    return PB_OK;
 }

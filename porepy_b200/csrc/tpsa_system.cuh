@@ -287,4 +287,205 @@ PB_HD int tpsa_poro_fluid_row(int64_t c, int64_t nc, const int64_t *blk_ptr, int
     return missing;
 }
 
+// ---- TPSA elasticity with fractures in frictional contact (reference models/momentum_balance.py:127-183,
+// constitutive_laws.py:3064-3248, contact_mechanics.py:80-245) -----------------------------------------------------
+// Unknowns [three-field cell blocks (B nc) | t (nd per fracture cell, nk) | u_j (nd per mortar cell, nm)]; equations
+// [three-field balances (B nc) | interface force balances (nd per mortar cell) | normal laws (nk) | tangential laws
+// ((nd - 1) nk)].  Fracture cells and mortar cells are numbered over all fractures / interfaces one after the other.
+// The fracture faces of the matrix are internal Dirichlet faces carrying Pi^avg u_j, so the balance rows of a cell with
+// fracture faces gain u_j columns after the three-field segments: block row c holds, per row l, the n len(l) entries of
+// its face neighbours, then per fracture face (mortar cells ascending) one u_j entry in a momentum row and nd in an
+// angular or solid-mass row:
+//   momentum i   -s_f B_s[f, i] w_m2p      angular  +s_f B_r[f, :, :] w_m2p      solid mass  +s_f B_m[f, :] w_m2p
+// Block row c starts at blk_ptr[c], row l at blk_ptr[c] + off(l) n_c + eoff(l) m_c (m_c: fracture faces of c).  The
+// force row (M, i) (face f, cell c, fracture cell K) has LF entries, at blk_ptr[nc] + (M nd + i) LF:
+//   [u_c,i | r_c | p_c]  w_p2m s_f (S_u | S_r | S_p)[f, i],   t_K  vol_M T_c sign_M R_K[:, i],   u_j(M, i)  w_p2m s_f B_s w_m2p
+// and contact row r (r < nk: the normal law of K = r, else a tangential law of K = (r - nk) / (nd - 1)) the 3 nd
+// columns [t_K | u_j(m1) | u_j(m2)] (m1 < m2 the mortar cells of K), at blk_ptr[nc] + nm nd LF + 3 nd r.
+struct TpsaMortars {
+    int64_t nm, nk;
+    const int32_t *face, *cell, *face_mortar, *pair;   // pair: the two mortar cells of every fracture cell, ascending
+    const double *w_m2p, *w_p2m, *sign, *vol, *frame;   // vol: volume x secondary_to_mortar_int weight; frame: nd x nd
+    double ct;                                           // per fracture cell, row-major (tangents, then the normal)
+};
+
+template <int ND>
+struct TpsaContactDims {
+    using M = TpsaDims<ND>;
+    static constexpr int NR = M::NR, B = M::B, LF = ND + NR + 3, LC = 3 * ND;
+    static constexpr int EXT = ND + NR * ND + ND;   // u_j entries of one fracture face in a block row
+    PB_HD static int ext(int l) { return l < ND ? 1 : ND; }
+    PB_HD static int eoff(int l) { return l < ND ? l : ND + (l - ND) * ND; }
+    PB_HD static int64_t roff(int l, int n, int m) { return (int64_t)M::off(l) * n + (int64_t)eoff(l) * m; }
+};
+
+// Fracture faces of c (faces with a mortar cell).
+PB_HD int tpsa_contact_nfrac(int64_t c, const TpsaTopo &t, const int32_t *face_mortar) {
+    int m = 0;
+    for (int q = t.cf_ip[c]; q < t.cf_ip[c + 1]; ++q) m += face_mortar[t.cf_ix[q]] >= 0;
+    return m;
+}
+
+// The fracture face of c with the smallest mortar cell above `last` (-1: from the start); its mortar cell, or -1.
+PB_HD int32_t tpsa_contact_next(int64_t c, const TpsaTopo &t, const int32_t *face_mortar, int32_t last, int64_t *face) {
+    int32_t best = -1;
+    for (int q = t.cf_ip[c]; q < t.cf_ip[c + 1]; ++q) {
+        const int64_t f = t.cf_ix[q];
+        const int32_t m = face_mortar[f];
+        if (m > last && (best < 0 || m < best)) { best = m; *face = f; }
+    }
+    return best;
+}
+
+// Row pointers and column indices of block row c (n face neighbours nb, ascending; the block row starts at blk0).
+template <int ND>
+PB_HD void tpsa_contact_pattern_rows(int64_t c, int n, const int32_t *nb, int64_t blk0, const TpsaTopo &t,
+                                     const TpsaMortars &I, int32_t *ip, int32_t *ix) {
+    using D = TpsaContactDims<ND>;
+    const int m = tpsa_contact_nfrac(c, t, I.face_mortar);
+    const int64_t u0 = (int64_t)D::B * t.nc + (int64_t)ND * I.nk;
+    for (int l = 0; l < D::B; ++l) {
+        const int len = D::M::len(l);
+        const int64_t r0 = blk0 + D::roff(l, n, m);
+        ip[c * D::B + l] = (int32_t)r0;
+        for (int j = 0; j < n; ++j)
+            for (int q = 0; q < len; ++q) ix[r0 + j * len + q] = nb[j] * D::B + D::M::col(l, q);
+        int64_t q = r0 + (int64_t)n * len, f = 0;
+        for (int32_t mc = tpsa_contact_next(c, t, I.face_mortar, -1, &f); mc >= 0;
+             mc = tpsa_contact_next(c, t, I.face_mortar, mc, &f)) {
+            if (l < ND) ix[q++] = (int32_t)(u0 + (int64_t)mc * ND + l);
+            else
+                for (int i = 0; i < ND; ++i) ix[q++] = (int32_t)(u0 + (int64_t)mc * ND + i);
+        }
+    }
+}
+
+// Row pointer and column indices of interface row q (q < nd nm: force row (q / nd, q % nd); else contact row
+// q - nd nm); the interface rows start at row0 = B nc and entry e0 = blk_ptr[nc].
+template <int ND>
+PB_HD void tpsa_contact_iface_pattern(int64_t q, int64_t nc, int64_t e0, const TpsaTopo &t, const TpsaMortars &I,
+                                      int32_t *ip, int32_t *ix) {
+    using D = TpsaContactDims<ND>;
+    const int64_t t0 = (int64_t)D::B * nc, u0 = t0 + (int64_t)ND * I.nk;
+    if (q < ND * I.nm) {
+        const int64_t mc = q / ND, f = I.face[mc];
+        const int i = (int)(q - mc * ND);
+        const int64_t c = t.face_cells[2 * f] >> 1, k = I.cell[mc];
+        int64_t p = e0 + q * D::LF;
+        ip[t0 + q] = (int32_t)p;
+        ix[p++] = (int32_t)(c * D::B + i);
+        for (int r = 0; r <= D::NR; ++r) ix[p++] = (int32_t)(c * D::B + ND + r);
+        for (int j = 0; j < ND; ++j) ix[p++] = (int32_t)(t0 + k * ND + j);
+        ix[p] = (int32_t)(u0 + mc * ND + i);
+    } else {
+        const int64_t r = q - ND * I.nm;
+        const int64_t k = r < I.nk ? r : (r - I.nk) / (ND - 1);
+        int64_t p = e0 + (int64_t)ND * I.nm * D::LF + r * D::LC;
+        ip[t0 + q] = (int32_t)p;
+        for (int j = 0; j < ND; ++j) ix[p++] = (int32_t)(t0 + k * ND + j);
+        for (int s = 0; s < 2; ++s)
+            for (int j = 0; j < ND; ++j) ix[p++] = (int32_t)(u0 + (int64_t)I.pair[2 * k + s] * ND + j);
+    }
+}
+
+// Block (c, cc_ix[j0 + j]) of the balance rows into the CSR values a; thread j = 0 also writes the u_j entries of c.
+template <int ND>
+PB_HD void tpsa_contact_block(int64_t c, int j, const TpsaTopo &t, const int32_t *cc_ptr, const int32_t *cc_ix,
+                              const int64_t *blk_ptr, const TpsaMortars &I, const TpsaTerms &T, const double *mu,
+                              const double *lam, const double *vol, double *a) {
+    using D = TpsaContactDims<ND>;
+    constexpr int NR = D::NR;
+    const int64_t j0 = cc_ptr[c];
+    const int n = (int)(cc_ptr[c + 1] - j0);
+    const int64_t k = cc_ix[j0 + j];
+    const int m = tpsa_contact_nfrac(c, t, I.face_mortar);
+    const int64_t b0 = blk_ptr[c];
+#pragma unroll
+    for (int l = 0; l < D::B; ++l)
+        tpsa_system_segment<ND>(c, l, k, t, T, mu, lam, vol, a + b0 + D::roff(l, n, m) + (int64_t)j * D::M::len(l));
+    if (j != 0 || m == 0) return;
+    int64_t f = 0;
+    int e = 0;   // fracture faces of c done
+    for (int32_t mc = tpsa_contact_next(c, t, I.face_mortar, -1, &f); mc >= 0;
+         mc = tpsa_contact_next(c, t, I.face_mortar, mc, &f), ++e) {
+        const double s = (t.face_cells[2 * f] & 1) ? -1.0 : 1.0, w = s * I.w_m2p[mc];
+#pragma unroll
+        for (int l = 0; l < D::B; ++l) {
+            double *dst = a + b0 + D::roff(l, n, m) + (int64_t)n * D::M::len(l) + (int64_t)e * D::ext(l);
+            if (l < ND) {
+                dst[0] = -w * T.t[10][f * ND + l];
+            } else if (l < ND + NR) {
+#pragma unroll
+                for (int i = 0; i < ND; ++i) dst[i] = w * T.t[11][f * NR * ND + (l - ND) * ND + i];
+            } else {
+#pragma unroll
+                for (int i = 0; i < ND; ++i) dst[i] = w * T.t[12][f * ND + i];
+            }
+        }
+    }
+}
+
+// Values of interface row q (see tpsa_contact_iface_pattern): the force rows, 0 in the contact rows.
+template <int ND>
+PB_HD void tpsa_contact_iface_row(int64_t q, int64_t e0, const TpsaTopo &t, const TpsaMortars &I, const TpsaTerms &T,
+                                  double *a) {
+    using D = TpsaContactDims<ND>;
+    constexpr int NR = D::NR;
+    if (q < ND * I.nm) {
+        const int64_t mc = q / ND, f = I.face[mc], k = I.cell[mc];
+        const int i = (int)(q - mc * ND);
+        const double w = ((t.face_cells[2 * f] & 1) ? -1.0 : 1.0) * I.w_p2m[mc];
+        const int64_t p0 = t.fc_ptr[f];   // the face's one (face, cell) entry
+        double *dst = a + e0 + q * D::LF;
+        dst[0] = w * T.t[0][ND * p0 + i];
+#pragma unroll
+        for (int r = 0; r < NR; ++r) dst[1 + r] = w * T.t[1][ND * NR * p0 + i * NR + r];
+        dst[1 + NR] = w * T.t[2][ND * p0 + i];
+        const double tw = I.vol[mc] * I.ct * I.sign[mc];
+#pragma unroll
+        for (int j = 0; j < ND; ++j) dst[2 + NR + j] = tw * I.frame[k * ND * ND + j * ND + i];
+        dst[2 + NR + ND] = w * T.t[10][f * ND + i] * I.w_m2p[mc];
+    } else {
+        double *dst = a + e0 + (int64_t)ND * I.nm * D::LF + (q - ND * I.nm) * D::LC;
+#pragma unroll
+        for (int p = 0; p < D::LC; ++p) dst[p] = 0.0;
+    }
+}
+
+// Entry q of b = -R(0) for q >= B nc (interface rows): -w_p2m s_f B_s[f, i] g[f, i] in the force rows, 0 in the
+// contact rows (written at every linearization).
+template <int ND>
+PB_HD double tpsa_contact_iface_rhs(int64_t q, const TpsaTopo &t, const TpsaMortars &I, const TpsaTerms &T,
+                                    const double *g) {
+    if (q >= ND * I.nm) return 0.0;
+    const int64_t mc = q / ND, f = I.face[mc];
+    const int i = (int)(q - mc * ND);
+    const double s = (t.face_cells[2 * f] & 1) ? -1.0 : 1.0;
+    return -I.w_p2m[mc] * s * T.t[10][f * ND + i] * g[f * ND + i];
+}
+
+// Contact row r at one Newton step: row r of jc (the Jacobian of the laws in the variables [t | u_j]) placed into the
+// fixed pattern at its column + B nc (binary search, duplicates summed in row order), -R into b[row].  Returns the
+// number of entries that are not in the pattern.
+template <int ND>
+PB_HD int tpsa_contact_law_row(int64_t r, int64_t c0, int64_t e0, int64_t row, const int32_t *ix, const int32_t *jc_ip,
+                               const int32_t *jc_ix, const double *jc_a, const double *neg_res, double *a, double *b) {
+    constexpr int LC = TpsaContactDims<ND>::LC;
+    const int64_t s0 = e0 + r * LC, e = s0 + LC;   // e0: the first entry of the contact rows
+    int missing = 0;
+    for (int64_t q = s0; q < e; ++q) a[q] = 0.0;
+    for (int q = jc_ip[r]; q < jc_ip[r + 1]; ++q) {
+        const int32_t want = (int32_t)(jc_ix[q] + c0);
+        int64_t lo = s0, hi = e;
+        while (lo < hi) {
+            const int64_t mid = (lo + hi) >> 1;
+            if (ix[mid] < want) lo = mid + 1; else hi = mid;
+        }
+        if (lo < e && ix[lo] == want) a[lo] += jc_a[q];
+        else ++missing;
+    }
+    b[row] = neg_res[r];
+    return missing;
+}
+
 }  // namespace pb

@@ -730,6 +730,47 @@ class FaceGrid:
         counting entries outside the pattern."""
         self._balance_rows(self.lib.pb_tpsa_thm_balance_rows, 2 * self.nc, A, jf, neg_res, rhs, missing)
 
+    def tpsa_contact_system(self, nd: int, mu, lmbda, cell_volumes, codes, robin_diag, face_flags, face_areas,
+                            mortars: dict, frames, characteristic_traction: float) -> tuple:
+        """The TPSA contact Jacobian with its balance and force rows (``pb_tpsa_contact_system``, layout in
+        include/poreb200.h) as a ``DeviceCsr`` and the device times of its two stages in ms.  ``mortars``: per mortar
+        cell (all interfaces in order) ``face``, ``cell`` (fracture cell, all fractures in order), ``m2p``, ``p2m``,
+        ``sign`` and ``volume``; ``frames``: nd x nd per fracture cell, row-major."""
+        from .sparse import DeviceCsr
+        mu, lam, vol = _lib.f64(mu), _lib.f64(lmbda), _lib.f64(cell_volumes)
+        if mu.shape != (self.nc,) or lam.shape != (self.nc,) or vol.shape != (self.nc,):
+            raise ValueError("mu, lmbda and cell_volumes must have one value per cell")
+        face, cell = (np.ascontiguousarray(mortars[k], dtype=np.int32) for k in ("face", "cell"))
+        w = [_lib.f64(mortars[k]) for k in ("m2p", "p2m", "sign", "volume")]
+        nm, nk = face.size, int(np.asarray(frames).size) // (nd * nd)
+        if cell.size != nm or any(a.size != nm for a in w):
+            raise ValueError("every mortar array must have one value per mortar cell")
+        fr = _lib.f64(frames)
+        cod = np.ascontiguousarray(codes, dtype=np.uint8)
+        rob = None if robin_diag is None else _lib.f64(robin_diag)
+        flags = np.ascontiguousarray(face_flags, dtype=np.uint8)
+        _lib.check(self.lib.pb_facegrid_set_face_areas(self.h, _lib.ptr(_lib.f64(face_areas), _lib._f64p)))
+        h = C.c_void_p()
+        ms = (C.c_float * 2)()
+        _lib.check(self.lib.pb_tpsa_contact_system(
+            self.h, int(nd), _lib.ptr(mu, _lib._f64p), _lib.ptr(lam, _lib._f64p), _lib.ptr(vol, _lib._f64p),
+            _lib.ptr(cod, _lib._u8p), _lib.ptr(rob, _lib._f64p), _lib.ptr(flags, _lib._u8p), int(nm), int(nk),
+            _lib.ptr(face, _lib._i32p), _lib.ptr(cell, _lib._i32p), *[_lib.ptr(a, _lib._f64p) for a in w],
+            _lib.ptr(fr, _lib._f64p), float(characteristic_traction), C.byref(h), C.cast(ms, _lib._f32p)))
+        return DeviceCsr.from_handle(h), [float(ms[0]), float(ms[1])]
+
+    def tpsa_contact_rhs(self, n: int, bc_values, body_force=None, angular_source=None, mass_source=None):
+        """-R(0) of the balance and force rows of the contact system last assembled on this grid
+        (``pb_tpsa_contact_rhs``), 0 in the contact rows, as a CUDA tensor of ``n`` doubles."""
+        return self._poro_rhs(self.lib.pb_tpsa_contact_rhs, n, bc_values, body_force, angular_source, mass_source)
+
+    def tpsa_contact_rows(self, A, jc, neg_res, rhs, missing=None) -> None:
+        """Write the contact rows of ``A`` (the matrix of ``tpsa_contact_system``) from the Jacobian ``jc`` of the
+        [normal | tangential] laws in the variables [t | u_j] (``DeviceCsr``) and their entries of ``rhs`` from
+        ``neg_res``, on the current stream (``pb_tpsa_contact_rows``).  ``missing``: int32 CUDA tensor counting entries
+        outside the pattern."""
+        self._balance_rows(self.lib.pb_tpsa_contact_rows, jc.shape[0], A, jc, neg_res, rhs, missing)
+
     def _balance_rows(self, fn, n, A, jf, neg_res, rhs, missing):
         import torch
         from .sparse import device_operand

@@ -529,3 +529,49 @@ def tpsa_thermoporomechanics_from_model(model):
     o = np.cumsum([0, nd * nc, nr * nc, nc, nc, nc])
     prob.row_map = interleave([rows[o[i]:o[i + 1]] for i in range(5)], nd, nr, nc)
     return prob, prob.column_map, prob.row_map
+
+
+def tpsa_fractured_momentum_from_model(model):
+    """A prepared ``pp.MomentumBalance`` with ``TpsaMomentumBalanceMixin`` on one 2-D or 3-D matrix with fractures in
+    frictional contact (one dimension less, no intersections, matching mortar grids) ->
+    (``TpsaFracturedMomentumBalance``, column_map, row_map): unknown k of the problem ([u_c, r_c, p_c per matrix cell |
+    contact traction | interface displacement]) is dof ``column_map[k]`` of the model's ``EquationSystem``, equation k its
+    row ``row_map[k]``.  The boundary operator is the model's own ``combine_boundary_operators_mechanical_stress``,
+    evaluated; the body force and the angular and solid-mass sources are its own operators, evaluated."""
+    from .contact import FractureContact
+    from .tpsa_contact import TpsaFracturedMomentumBalance
+    from .tpsa_elasticity import interleave
+    es = model.equation_system
+    if "mass_balance_equation" in es.equations:
+        raise NotImplementedError("TpsaFracturedMomentumBalance: fractured TPSA poromechanics is not supported")
+    mat, fracs, grids = _matrix_and_fractures(model)
+    if getattr(mat, "periodic_face_map", None) is not None:
+        raise NotImplementedError("periodic faces are not supported by porepy_b200")
+    mdg = model.mdg
+    nd, nc, nf = int(mat.dim), mat.num_cells, mat.num_faces
+    nr = model.rotation_dimension()
+    mk = model.stress_keyword
+    data = _own_data(mdg.subdomain_data(mat), [mk])
+    contacts = []
+    for j, frac in enumerate(fracs):
+        intf = grids[("interface", j)]
+        rot = mdg.subdomain_data(frac)["tangential_normal_projection"].project_tangential_normal(frac.num_cells)
+        contacts.append(FractureContact(intf.mortar_to_primary_avg(), intf.primary_to_mortar_int(),
+                                        intf.mortar_to_secondary_avg(), intf.secondary_to_mortar_int(),
+                                        sps.csr_matrix(intf.sign_of_mortar_sides(1)).diagonal(), intf.cell_volumes, rot))
+    prob = TpsaFracturedMomentumBalance(
+        mat, data, _evaluated(model, model.combine_boundary_operators_mechanical_stress([mat]), nd * nf), contacts,
+        _contact_constants(model, fracs), body_force=_evaluated(model, model.body_force([mat]), nd * nc),
+        angular_source=_evaluated(model, model.source_angular_momentum([mat]), nr * nc),
+        mass_source=_evaluated(model, model.solid_mass_source([mat]), nc), keyword=mk)
+    cols = [_dofs(model, name, mat) for name in (model.displacement_variable, model.rotation_stress_variable,
+                                                  model.total_pressure_variable)]
+    tail = BlockLayout(prob.unknown_layout.blocks[1:])
+    solid_mass = [eq for eq in es.equations if eq.lower().startswith("solid_mass_equation")][0]
+    rows = _row_map(model, BlockLayout([("momentum_balance_equation", [(("matrix",), nc, nd)]),
+                                        ("angular_momentum_balance_equation", [(("matrix",), nc, nr)]),
+                                        (solid_mass, [(("matrix",), nc, 1)])] + prob.equation_layout.blocks[1:]))
+    o = np.cumsum([0, nd * nc, nr * nc, nc])
+    prob.column_map = np.concatenate([interleave(cols, nd, nr, nc), _column_map(model, tail, grids)])
+    prob.row_map = np.concatenate([interleave([rows[o[i]:o[i + 1]] for i in range(3)], nd, nr, nc), rows[o[3]:]])
+    return prob, prob.column_map, prob.row_map

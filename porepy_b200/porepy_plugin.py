@@ -261,4 +261,5 @@ def plugin(pp, allow_reference_fallback: bool = False) -> SimpleNamespace:
                            tpsa_momentum_from_model=bridge.tpsa_momentum_from_model,
                            tpsa_poromechanics_from_model=bridge.tpsa_poromechanics_from_model,
                            tpsa_thermoporomechanics_from_model=bridge.tpsa_thermoporomechanics_from_model,
+                           tpsa_fractured_momentum_from_model=bridge.tpsa_fractured_momentum_from_model,
                            fallback_calls=fallback_calls, gpu_calls=gpu_calls)

@@ -256,6 +256,40 @@ int pb_tpfa_diff(pb_facegrid *g, const double *k, const int32_t *fc_indptr, doub
 int pb_upwind(pb_facegrid *g, const double *darcy_flux, const uint8_t *bc_bits, int32_t *upstream_cell,
               double *neumann_diag, double *dirichlet_diag);
 
+/* ---- mixed (dual) discretizations of Darcy flow: MVEM and RT0 (csrc/dual_cell.cuh; reference numerics/vem/mvem.py,
+ * numerics/fem/rt0.py) -------------------------------------------------------------------------------------------------
+ * A pb_dual holds the topology of a grid of dimension nd (1, 2 or 3): cell_faces (nf x nc CSC, +-1 data, the faces of
+ * every cell in ascending order) and face_nodes (nn x nf CSC).  pb_dual_mass_pattern returns the FACE x FACE pattern of
+ * the mass matrix (row f: every face sharing a cell with f, ascending), built on the device at the first call and kept
+ * on the handle; indptr (nf + 1) / indices (*nnz) may be NULL to query the size.  pb_dual_discretize runs one thread
+ * per entry of cell_faces.  Geometry in the grid's own frame, each (3 x n) row-major: nodes, face_normals,
+ * face_centers, cell_centers; cell_volumes (nc); perm (3 x 3 x nc) row-major, expressed in the frame; rot (3 x 3)
+ * row-major, the frame's axes as rows.  Outputs (host): mass values (*nnz) in the pattern; proj values
+ * (3 cf_indptr[nc]): row 3c + a of the (3 nc x nf) flux reconstruction holds the faces of c in cell_faces order, at
+ * 3 cf_indptr[c] + a n_c + i.  *bad_cell: the smallest cell failing the MVEM consistency test allclose(G, F D) of
+ * mvem.py, or -1.  PB_DUAL_RT0 needs nd + 1 faces in every cell.  mass / proj may be NULL: the values stay on the
+ * handle either way (until the next call), for pb_dual_download and pb_dual_system.
+ * pb_dual_system assembles the saddle-point system of dual_elliptic.py assemble_matrix_rhs from those values on the
+ * device: the (nf + nc) square matrix [[mass, div^T], [div, 0]], div = -cell_faces^T, faces first (row f: the mass row,
+ * then the columns nf + c of the face's cells; row nf + c: the cell's faces), with codes (nf, PB_BC_*; internal and
+ * interior faces PB_BC_INTERIOR): Neumann rows cleared with *norm = |mass|_inf (device reduction) on the diagonal,
+ * 1 / (robin_weight area) added on Robin diagonals; rhs (nf + nc, host) = proj^T vector_source (vector_source: 3 nc or
+ * NULL) + the Dirichlet / Robin / Neumann terms of assemble_rhs with the sign of each face's first cell. */
+#define PB_DUAL_MVEM 0
+#define PB_DUAL_RT0 1
+typedef struct pb_dual pb_dual; /* opaque */
+int pb_dual_create(int nd, int64_t nc, int64_t nf, int64_t nn, const int32_t *cf_indptr, const int32_t *cf_indices,
+                   const int8_t *cf_data, const int32_t *fn_indptr, const int32_t *fn_indices, pb_dual **out);
+void pb_dual_destroy(pb_dual *d);
+int pb_dual_mass_pattern(pb_dual *d, int64_t *nnz, int32_t *indptr, int32_t *indices);
+int pb_dual_discretize(pb_dual *d, int method, const double *nodes, const double *face_normals,
+                       const double *face_centers, const double *cell_centers, const double *cell_volumes,
+                       const double *perm, const double *rot, double *mass, double *proj, int64_t *bad_cell,
+                       float *kernel_ms);
+int pb_dual_download(pb_dual *d, double *mass, double *proj);
+int pb_dual_system(pb_dual *d, const uint8_t *codes, const double *robin_weight, const double *face_areas,
+                   const double *bc_values, const double *vector_source, pb_csr **out, double *rhs, double *norm);
+
 /* ---- two-point stress approximation (csrc/tpsa_face.cuh; reference numerics/fv/tpsa.py:376-1430) ------------------
  * One thread per face writes every value of the 14 TPSA matrices in that face's rows.  nr = nd in 3-D (the rotation
  * is a 3-vector) and nr = 1 in 2-D (a scalar).  Shapes (rows x columns) and the block of one (face, cell) entry or of

@@ -82,3 +82,41 @@ __device__ __forceinline__ int warp_unique(const K *key, int n, K *out) {
     }
     return cnt;
 }
+
+// Structural patterns on the device: row r = sorted union over the nodes of row entity r of the
+// node's column entities.  One warp per row: gather the (<= CAP) candidates into shared memory,
+// bitonic sort, unique.  pass 0 writes the row length, pass 1 the indices.
+template <int CAP>
+__global__ void pattern_kernel(int64_t nrows, const int32_t *__restrict__ rn_ptr, const int32_t *__restrict__ rn,
+                               const int32_t *__restrict__ col_ptr, const int32_t *__restrict__ col_idx,
+                               int32_t *__restrict__ counts, const int32_t *__restrict__ indptr,
+                               int32_t *__restrict__ indices, int pass, int *overflow) {
+    __shared__ int32_t sbuf[8][CAP];
+    const int lane = threadIdx.x & 31, wib = threadIdx.x >> 5;
+    int32_t *buf = sbuf[wib];
+    const int64_t warp = (int64_t)blockIdx.x * (blockDim.x >> 5) + wib;
+    const int64_t nwarps = (int64_t)gridDim.x * (blockDim.x >> 5);
+    for (int64_t r = warp; r < nrows; r += nwarps) {
+        int total = 0;
+        bool over = false;
+        for (int q = rn_ptr[r]; q < rn_ptr[r + 1]; ++q) {
+            const int s = rn[q];
+            const int b = col_ptr[s], len = col_ptr[s + 1] - b;
+            if (total + len > CAP) { over = true; break; }
+            for (int i = lane; i < len; i += 32) buf[total + i] = col_idx[b + i];
+            total += len;
+        }
+        if (over) {
+            if (lane == 0) { atomicExch(overflow, 1); if (pass == 0) counts[r] = 0; }
+            continue;
+        }
+        int P = 1;
+        while (P < total) P <<= 1;
+        for (int i = total + lane; i < P; i += 32) buf[i] = 0x7fffffff;
+        __syncwarp();
+        warp_bitonic_sort(P, [&](int i, int l, bool asc) { warp_cas(buf, i, l, asc); });
+        const int off = warp_unique(buf, total, pass == 1 ? indices + indptr[r] : (int32_t *)nullptr);
+        if (pass == 0 && lane == 0) counts[r] = off;
+        __syncwarp();
+    }
+}

@@ -1452,6 +1452,342 @@ class Tpsa(_Base):
         return mats
 
 
+def line_frame(sd, tol: float = 1e-5) -> np.ndarray:
+    """Rotation ``R`` (3, 3) whose first row is the direction of a straight 1-D grid (the frame the mixed schemes
+    discretize a line in; any orthonormal completion gives the same matrices).  Raises ``ValueError`` when the nodes
+    deviate from the line by more than ``tol`` relative to the grid's extent."""
+    x = np.asarray(sd.nodes, dtype=np.float64)
+    xc = x - x.mean(axis=1, keepdims=True)
+    _, v = np.linalg.eigh(xc @ xc.T)          # ascending: v[:, 2] is the line's direction
+    t = v[:, 2]
+    off = xc - np.outer(t, t @ xc)
+    if np.abs(off).max() > tol * max(np.abs(xc).max(), 1e-300):
+        raise ValueError("1-D grid is not straight")
+    return np.vstack((t, v[:, 1], v[:, 0]))
+
+
+def dual_frame(sd, tol: float = 1e-5) -> np.ndarray:
+    """The rotation that takes a grid into its own frame for MVEM / RT0: identity in 3-D and for 2-D grids in a plane
+    z = const, ``line_frame`` for lines.  Other planes (checked by ``plane_frame`` with the same
+    ``deviation_from_plane_tol``) are turned about n x e_z until their normal n is e_z, as ``map_geometry.map_grid``
+    does, with n the cross product of the longest centred node vector and the one giving the longest product.  MVEM
+    needs that very in-plane basis: its stabilization weight |K^-1|_inf is not invariant under in-plane rotations."""
+    if sd.dim == 1:
+        return line_frame(sd, tol)
+    if sd.dim != 2 or plane_frame(sd, tol) is None:
+        return np.eye(3)
+    v = np.asarray(sd.nodes, dtype=np.float64)
+    v = v - v.mean(axis=1, keepdims=True)
+    v1 = v[:, np.argmax(np.linalg.norm(v, axis=0))]
+    cross = np.cross(v1, v.T).T
+    n = cross[:, np.argmax(np.linalg.norm(cross, axis=0))]
+    n = n / np.linalg.norm(n)
+    axis = np.cross(n, [0.0, 0.0, 1.0])
+    if np.allclose(axis, 0.0):   # the reference's test in map_geometry.rotation_matrix
+        return np.eye(3)
+    axis = axis / np.linalg.norm(axis)
+    a = np.arccos(n[2])
+    W = np.array([[0.0, -axis[2], axis[1]], [axis[2], 0.0, -axis[0]], [-axis[1], axis[0], 0.0]])
+    return np.eye(3) + np.sin(a) * W + (1.0 - np.cos(a)) * (W @ W)
+
+
+class DualGrid:
+    """Device topology of a grid for the mixed schemes (``pb_dual``): cell_faces with the faces of every cell sorted,
+    face_nodes, and the FACE x FACE mass pattern, built on the device at the first use and kept here.  Cached on the
+    grid object and rebuilt when the topology changes."""
+
+    def __init__(self, sd):
+        lib = _lib.load()
+        _lib.require_gpu()
+        self.lib = lib
+        cf = sps.csc_matrix(sd.cell_faces, copy=True)
+        cf.sort_indices()
+        fn = sps.csc_matrix(sd.face_nodes)
+        self.nd, self.nc, self.nf, self.nn = int(sd.dim), sd.num_cells, sd.num_faces, sd.num_nodes
+        self.cf_ip, self.cf_ix = cf.indptr.astype(np.int32), cf.indices.astype(np.int32)
+        cfd = np.asarray(cf.data).astype(np.int8)
+        fnp, fni = fn.indptr.astype(np.int32), fn.indices.astype(np.int32)
+        h = C.c_void_p()
+        _lib.check(lib.pb_dual_create(self.nd, self.nc, self.nf, self.nn, _lib.ptr(self.cf_ip, _lib._i32p),
+                                      _lib.ptr(self.cf_ix, _lib._i32p), _lib.ptr(cfd, _lib._i8p),
+                                      _lib.ptr(fnp, _lib._i32p), _lib.ptr(fni, _lib._i32p), C.byref(h)))
+        self.h = h
+        self.fingerprint = DevicePlan._fingerprint(sd, sd.cell_faces, sd.face_nodes)
+        self._mass = None
+        self._proj = None
+        self.pattern_seconds = 0.0
+        self.live, self.current = [], None
+
+    def __del__(self):
+        h = getattr(self, "h", None)
+        if h is not None and h.value:
+            try:
+                self.lib.pb_dual_destroy(h)
+            except Exception:
+                pass
+            self.h = None
+
+    @classmethod
+    def for_grid(cls, sd) -> "DualGrid":
+        fp = DevicePlan._fingerprint(sd, sd.cell_faces, sd.face_nodes)
+        dg = getattr(sd, "_b200_dual", None)
+        if dg is None or dg.fingerprint != fp:
+            dg = cls(sd)
+            try:
+                sd._b200_dual = dg
+            except AttributeError:
+                pass
+        return dg
+
+    def mass_pattern(self):
+        """(indptr, indices) of the FACE x FACE mass pattern."""
+        if self._mass is None:
+            t0 = time.perf_counter()
+            nnz = C.c_int64(0)
+            _lib.check(self.lib.pb_dual_mass_pattern(self.h, C.byref(nnz), None, None))
+            ip, ix = np.empty(self.nf + 1, np.int32), np.empty(nnz.value, np.int32)
+            _lib.check(self.lib.pb_dual_mass_pattern(self.h, C.byref(nnz), _lib.ptr(ip, _lib._i32p),
+                                                     _lib.ptr(ix, _lib._i32p)))
+            self._mass = (ip, ix)
+            self.pattern_seconds = time.perf_counter() - t0
+        return self._mass
+
+    def proj_pattern(self):
+        """(indptr, indices) of the (3 nc x nf) flux reconstruction: row 3c + a holds the faces of c."""
+        if self._proj is None:
+            n = np.diff(self.cf_ip).astype(np.int64)
+            start = 3 * self.cf_ip[:-1].astype(np.int64)[:, None] + np.arange(3) * n[:, None]
+            ip = np.append(start.ravel(), 3 * int(self.cf_ip[-1]))
+            lens = np.repeat(n, 3)
+            cell = np.repeat(np.arange(3 * self.nc) // 3, lens)
+            off = np.arange(int(ip[-1])) - np.repeat(ip[:-1], lens)
+            self._proj = (ip.astype(np.int32), self.cf_ix[self.cf_ip[cell] + off])
+        return self._proj
+
+    def discretize(self, method: int, geo, perm, rot):
+        """Run the per-cell kernel; the mass values (in ``mass_pattern``) and flux reconstruction values (in
+        ``proj_pattern``) stay on the device until ``download``.  Returns the first cell failing the MVEM consistency
+        test (-1: none) and the kernel time in ms.  ``geo``: nodes, face normals, face centres, cell centres (each
+        (3, n)) and cell volumes, in the frame ``rot``; ``perm`` (3, 3, nc) in that frame."""
+        self.mass_pattern()
+        arrs = [_lib.f64(a) for a in geo] + [_lib.f64(perm), _lib.f64(rot)]
+        bad, ms = C.c_int64(-1), C.c_float(0.0)
+        _lib.check(self.lib.pb_dual_discretize(self.h, int(method), *[_lib.ptr(a, _lib._f64p) for a in arrs], None,
+                                               None, C.byref(bad), C.byref(ms)))
+        return int(bad.value), float(ms.value)
+
+    def download(self):
+        """Mass and flux reconstruction values of the last ``discretize``."""
+        mass, proj = np.empty(self.mass_pattern()[1].size), np.empty(3 * int(self.cf_ip[-1]))
+        _lib.check(self.lib.pb_dual_download(self.h, _lib.ptr(mass, _lib._f64p), _lib.ptr(proj, _lib._f64p)))
+        return mass, proj
+
+    def system(self, codes, robin_weight, face_areas, bc_values, vector_source=None):
+        """The saddle-point system of the last ``discretize`` assembled on the device (``pb_dual_system``): a
+        ``DeviceCsr``, the right-hand side and |mass|_inf."""
+        from .sparse import DeviceCsr
+        arrs = [_lib.f64(a) for a in (robin_weight, face_areas, bc_values)]
+        vs = None if vector_source is None else _lib.f64(vector_source)
+        cod = np.ascontiguousarray(codes, dtype=np.uint8)
+        rhs, norm, h = np.empty(self.nf + self.nc), C.c_double(0.0), C.c_void_p()
+        _lib.check(self.lib.pb_dual_system(self.h, _lib.ptr(cod, _lib._u8p), *[_lib.ptr(a, _lib._f64p) for a in arrs],
+                                           _lib.ptr(vs, _lib._f64p), C.byref(h), _lib.ptr(rhs, _lib._f64p),
+                                           C.byref(norm)))
+        return DeviceCsr.from_handle(h), rhs, float(norm.value)
+
+
+class _DualElliptic(_Base):
+    """Mixed (dual) discretizations of Darcy flow (numerics/vem/dual_elliptic.py ``DualElliptic``): the same
+    constructor, matrix keys (``mass``, ``div``, ``vector_proj``), ``ndof`` and helpers.  ``discretize`` computes the
+    local matrices of every cell on the GPU (csrc/dual_cell.cuh), one thread per (cell, face); the matrices are scipy
+    CSR.  Always the whole grid: the reference has no partial mode."""
+
+    _method = -1
+
+    def __init__(self, keyword: str, name: str = "") -> None:
+        super().__init__(keyword)
+        self.name = name or type(self).__name__
+        self.mass_matrix_key = "mass"
+        self.div_matrix_key = "div"
+        self.vector_proj_key = "vector_proj"
+        self.vector_source_key = "vector_source"
+
+    def ndof(self, sd) -> int:
+        return sd.num_cells + sd.num_faces
+
+    def discretize(self, sd, data: dict) -> None:
+        mats = data.setdefault(DISCRETIZATION_MATRICES, {}).setdefault(self.keyword, {})
+        if sd.dim == 0:   # mvem.py / rt0.py: identity mass, empty divergence and projection
+            mats[self.mass_matrix_key] = sps.dia_matrix(([1], 0), (sd.num_faces, sd.num_faces))
+            mats[self.div_matrix_key] = sps.csr_matrix((sd.num_faces, sd.num_cells))
+            mats[self.vector_proj_key] = sps.csr_matrix((3, 0))
+            return
+        params = data[PARAMETERS][self.keyword]
+        if sd.dim < 3 and data.get("is_tangential", False):
+            raise NotImplementedError(f"{self.name}: is_tangential=True (a tensor in the map_grid frame) is not supported")
+        self._check_unsupported(params, sd)
+        if self._method == _lib.DUAL_RT0:
+            n = np.diff(sps.csc_matrix(sd.cell_faces).indptr)
+            if np.any(n != sd.dim + 1):
+                c = int(np.flatnonzero(n != sd.dim + 1)[0])
+                raise ValueError(f"RT0 needs simplices: cell {c} has {n[c]} faces")
+        t0 = time.perf_counter()
+        rot = dual_frame(sd, data.get("deviation_from_plane_tol", 1e-5))
+        geo = [rot @ np.asarray(a, dtype=np.float64) for a in (sd.nodes, sd.face_normals, sd.face_centers,
+                                                                 sd.cell_centers)]
+        geo.append(sd.cell_volumes)
+        perm = rotate_second_order(params["second_order_tensor"].values, rot)
+        dg = DualGrid.for_grid(sd)
+        first = dg._mass is None
+        for m in dg.live:   # the device values are about to be overwritten: fetch those still referenced
+            if m.__dict__.get("_lazy_data") is None:
+                m.data
+        bad, ms = dg.discretize(self._method, geo, perm, rot)
+        if bad >= 0:   # mvem.py massHdiv: assert np.allclose(G, F @ D)
+            raise AssertionError(f"MVEM: the consistency test G == F D fails in cell {bad}")
+        t1 = time.perf_counter()
+        mip, mix = dg.mass_pattern()
+        pip, pix = dg.proj_pattern()
+        nf, nc = sd.num_faces, sd.num_cells
+        from .sparse import LazyCsr
+        cache = {}
+
+        def values():
+            if "v" not in cache:
+                cache["v"] = dg.download()
+            return cache["v"]
+        mass = LazyCsr.lazy((nf, nf), mix.size, lambda: values()[0], lambda: mix.copy(), lambda: mip.copy())
+        proj = LazyCsr.lazy((3 * nc, nf), pix.size, lambda: values()[1], lambda: pix.copy(), lambda: pip.copy())
+        div = -sps.csc_matrix(sd.cell_faces).T.tocsr()
+        dg.live = [mass, proj]
+        dg.current = (mass, proj, div)
+        out = {self.mass_matrix_key: mass, self.div_matrix_key: div, self.vector_proj_key: proj}
+        mats.update(out)
+        self.last_timing = dict(kernel_ms=ms, pattern_s=dg.pattern_seconds if first else 0.0, device_s=t1 - t0,
+                                total_s=time.perf_counter() - t0)
+        _log_throughput(self.name, self.keyword, sd, ms, self.last_timing["total_s"], out)
+
+    def assemble_matrix(self, sd, data: dict) -> sps.csr_matrix:
+        """dual_elliptic.py ``assemble_matrix``: [[mass, div^T], [div, 0]]."""
+        mats = data[DISCRETIZATION_MATRICES][self.keyword]
+        div = mats[self.div_matrix_key]
+        return sps.bmat([[mats[self.mass_matrix_key], div.T], [div, None]], format="csr")
+
+    def assemble_neumann_robin(self, sd, data: dict, M, bc_weight: bool = False):
+        """dual_elliptic.py ``assemble_neumann_robin``: Neumann rows (not internal) cleared with |mass|_inf on the
+        diagonal (1 without ``bc_weight``), 1 / (robin_weight area) added on Robin diagonals."""
+        mass = data[DISCRETIZATION_MATRICES][self.keyword][self.mass_matrix_key]
+        norm = 1.0
+        if mass.shape[0] and bc_weight:
+            norm = sps.linalg.norm(mass, np.inf)
+        bc = data[PARAMETERS][self.keyword]["bc"]
+        internal = np.asarray(bc.is_internal, bool)
+        is_neu = np.flatnonzero(np.asarray(bc.is_neu, bool) & ~internal)
+        M = sps.csr_matrix(M)
+        if is_neu.size:
+            for row in is_neu:
+                M.data[M.indptr[row]:M.indptr[row + 1]] = 0.0
+            d = M.diagonal()
+            d[is_neu] = norm
+            M.setdiag(d)
+        is_rob = np.flatnonzero(np.asarray(bc.is_rob, bool) & ~internal)
+        if is_rob.size:
+            rob = np.zeros(self.ndof(sd))
+            rob[is_rob] = 1.0 / (np.asarray(bc.robin_weight)[is_rob] * sd.face_areas[is_rob])
+            M = M + sps.dia_matrix((rob, 0), shape=(rob.size, rob.size))
+        return M, norm
+
+    def assemble_rhs(self, sd, data: dict, bc_weight: float = 1.0) -> np.ndarray:
+        """dual_elliptic.py ``assemble_rhs``: proj^T vector_source, Dirichlet and Robin terms with the face sign,
+        Neumann values times ``bc_weight``."""
+        params = data[PARAMETERS][self.keyword]
+        proj = data[DISCRETIZATION_MATRICES][self.keyword][self.vector_proj_key]
+        rhs = np.zeros(self.ndof(sd))
+        if sd.dim == 0:
+            return rhs
+        bc, bc_val = params["bc"], params["bc_values"]
+        assert not bool(bc is None) != bool(bc_val is None)
+        vs = params.get("vector_source", np.zeros(proj.shape[0]))
+        rhs[:sd.num_faces] += proj.T @ vs
+        if bc is None:
+            return rhs
+        if getattr(sd, "periodic_face_map", None) is not None:
+            raise NotImplementedError("Periodic boundary conditions are not implemented for DualElliptic")
+        internal = np.asarray(bc.is_internal, bool)
+        is_neu = np.flatnonzero(np.asarray(bc.is_neu, bool) & ~internal)
+        is_dir = np.flatnonzero(np.asarray(bc.is_dir, bool) & ~internal)
+        is_rob = np.flatnonzero(np.asarray(bc.is_rob, bool) & ~internal)
+        cf = sps.csc_matrix(sd.cell_faces).tocoo()
+        sign = np.zeros(sd.num_faces)
+        faces, first = np.unique(cf.row, return_index=True)
+        sign[faces] = cf.data[first]
+        bc_val = np.asarray(bc_val, dtype=np.float64)
+        rhs[is_dir] += -sign[is_dir] * bc_val[is_dir]
+        rhs[is_rob] += -sign[is_rob] * bc_val[is_rob] / np.asarray(bc.robin_weight)[is_rob]
+        rhs[is_neu] = sign[is_neu] * bc_weight * bc_val[is_neu]
+        return rhs
+
+    def assemble_matrix_rhs(self, sd, data: dict):
+        """dual_elliptic.py ``assemble_matrix_rhs``: the saddle-point matrix (faces first, then cells) with the
+        Neumann / Robin rows, and the right-hand side scaled by the same |mass|_inf.  While the stored matrices are
+        the device-resident ones of the last ``discretize`` (``LazyCsr`` not yet touched), the system is assembled on
+        the GPU from exactly those values (``pb_dual_system``) and ``A`` comes back as a ``LazyCsr`` backed by the
+        device system (``A.device_csr``); otherwise the host formulas of the reference."""
+        mats = data[DISCRETIZATION_MATRICES][self.keyword]
+        params = data[PARAMETERS][self.keyword]
+        dg = getattr(sd, "_b200_dual", None)
+        cur = None if dg is None else dg.current
+        if (sd.dim > 0 and cur is not None and getattr(dg, "h", None) is not None and params.get("bc") is not None
+                and cur[0] is mats[self.mass_matrix_key] and cur[1] is mats[self.vector_proj_key]
+                and cur[2] is mats[self.div_matrix_key] and not cur[0].on_host and not cur[1].on_host):
+            bc = params["bc"]
+            if getattr(sd, "periodic_face_map", None) is not None:
+                raise NotImplementedError("Periodic boundary conditions are not implemented for DualElliptic")
+            internal = np.asarray(bc.is_internal, bool)
+            codes = np.zeros(sd.num_faces, np.uint8)
+            codes[np.asarray(bc.is_dir, bool) & ~internal] = _lib.BC_DIR
+            codes[np.asarray(bc.is_rob, bool) & ~internal] = _lib.BC_ROB
+            codes[np.asarray(bc.is_neu, bool) & ~internal] = _lib.BC_NEU
+            vs = params.get("vector_source")
+            a, rhs, _ = dg.system(codes, np.broadcast_to(np.asarray(bc.robin_weight, float), (sd.num_faces,)),
+                                  sd.face_areas, params["bc_values"], vs)
+            return _lazy_system(a), rhs
+        M = self.assemble_matrix(sd, data)
+        M, norm = self.assemble_neumann_robin(sd, data, M, bc_weight=True)
+        return M, self.assemble_rhs(sd, data, norm)
+
+    def project_flux(self, sd, u: np.ndarray, data: dict) -> np.ndarray:
+        """dual_elliptic.py ``project_flux``: one 3-vector per cell, (3, nc)."""
+        if sd.dim == 0:
+            return np.zeros(3).reshape((3, 1))
+        proj = data[DISCRETIZATION_MATRICES][self.keyword][self.vector_proj_key]
+        return (proj @ u).reshape((3, -1), order="F")
+
+    def extract_flux(self, sd, solution_array: np.ndarray, data: dict) -> np.ndarray:
+        return solution_array[:sd.num_faces]
+
+    def extract_pressure(self, sd, solution_array: np.ndarray, data: dict) -> np.ndarray:
+        return solution_array[sd.num_faces:]
+
+
+class MVEM(_DualElliptic):
+    """Lowest-order mixed virtual element method (numerics/vem/mvem.py ``MVEM``)."""
+
+    _method = _lib.DUAL_MVEM
+
+    def __init__(self, keyword: str) -> None:
+        super().__init__(keyword, "MVEM")
+
+
+class RT0(_DualElliptic):
+    """Lowest-order Raviart-Thomas element on simplices (numerics/fem/rt0.py ``RT0``)."""
+
+    _method = _lib.DUAL_RT0
+
+    def __init__(self, keyword: str) -> None:
+        super().__init__(keyword, "RT0")
+
+
 class Upwind(_Base):
     """First-order upwinding of an advective flux (numerics/fv/upwind.py:13).  ``discretize`` reads
     ``bc`` and the face fluxes under ``flux_array_key`` (default ``"darcy_flux"``) and writes the

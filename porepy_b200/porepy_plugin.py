@@ -56,6 +56,7 @@ def plugin(pp, allow_reference_fallback: bool = False) -> SimpleNamespace:
     RefTpfa, RefUpwind = pp.Tpfa, pp.Upwind
     RefTpsa, RefTpsaAd = pp.Tpsa, pp.ad.TpsaAd
     RefUpwindCoupling = pp.UpwindCoupling
+    RefMVEM, RefRT0 = pp.MVEM, pp.RT0
     RefMpfaAd, RefMpsaAd, RefBiotAd = pp.ad.MpfaAd, pp.ad.MpsaAd, pp.ad.BiotAd
 
     def _core(name, gpu_cls, ref_cls, flow):
@@ -95,7 +96,9 @@ def plugin(pp, allow_reference_fallback: bool = False) -> SimpleNamespace:
 
         body = {"__init__": __init__, "discretize": discretize, "update_discretization": update_discretization,
                 "__doc__": f"pp.{name} with the GPU discretization (porepy_b200.fv.{name})."}
-        if name != "Biot":
+        if name in ("MVEM", "RT0"):   # the device system while the matrices are resident, else the host formulas
+            body["assemble_matrix_rhs"] = lambda self, sd, data: gpu_cls.assemble_matrix_rhs(self, sd, data)
+        elif name != "Biot":
             body["assemble_matrix_rhs"] = lambda self, sd, data: ref_cls.assemble_matrix_rhs(self, sd, data)
         return type(name, (gpu_cls, ref_cls), body)
 
@@ -104,6 +107,8 @@ def plugin(pp, allow_reference_fallback: bool = False) -> SimpleNamespace:
     Mpsa = _core("Mpsa", fv.Mpsa, RefMpsa, False)
     Biot = _core("Biot", fv.Biot, RefBiot, False)
     Tpsa = _core("Tpsa", fv.Tpsa, RefTpsa, False)
+    MVEM = _core("MVEM", fv.MVEM, RefMVEM, True)
+    RT0 = _core("RT0", fv.RT0, RefRT0, True)
 
     class Upwind(fv.Upwind, RefUpwind):
         """pp.Upwind with the per-face GPU kernel (grids of any dimension)."""
@@ -209,12 +214,14 @@ def plugin(pp, allow_reference_fallback: bool = False) -> SimpleNamespace:
         pp.Tpfa, pp.Upwind = Tpfa, Upwind
         pp.UpwindCoupling = UpwindCoupling
         pp.Tpsa = Tpsa
+        pp.MVEM, pp.RT0 = MVEM, RT0
 
     def uninstall() -> None:
         pp.Mpfa, pp.Mpsa, pp.Biot = RefMpfa, RefMpsa, RefBiot
         pp.Tpfa, pp.Upwind = RefTpfa, RefUpwind
         pp.UpwindCoupling = RefUpwindCoupling
         pp.Tpsa = RefTpsa
+        pp.MVEM, pp.RT0 = RefMVEM, RefRT0
 
     def md_flow_from_model(model, keyword=None):
         """The mixed-dimensional Darcy problem of a prepared single-phase flow model (``pp.SinglePhaseFlow`` after
@@ -247,7 +254,7 @@ def plugin(pp, allow_reference_fallback: bool = False) -> SimpleNamespace:
             specific_volume=lambda it: evaluated(model.specific_volume([it]), it.num_cells))
 
     from . import model_bridge as bridge
-    return SimpleNamespace(Mpfa=Mpfa, Mpsa=Mpsa, Biot=Biot, Tpfa=Tpfa, Tpsa=Tpsa, Upwind=Upwind, UpwindCoupling=UpwindCoupling,
+    return SimpleNamespace(Mpfa=Mpfa, Mpsa=Mpsa, Biot=Biot, Tpfa=Tpfa, Tpsa=Tpsa, MVEM=MVEM, RT0=RT0, Upwind=Upwind, UpwindCoupling=UpwindCoupling,
                            MpfaAd=MpfaAd, MpsaAd=MpsaAd, BiotAd=BiotAd, TpsaAd=TpsaAd,
                            ModelMixin=ModelMixin, install=install, uninstall=uninstall, md_flow_from_model=md_flow_from_model,
                            # nonlinear model problems on the device AD chain (porepy_b200/model_bridge.py)

@@ -1,6 +1,8 @@
 """Run the REFERENCE's own finite-volume unit tests (tests/numerics/fv/test_{mpfa,mpsa,biot,tpsa}.py of the
-read-only tree) with pp.Mpfa / pp.Mpsa / pp.Biot / pp.Tpsa (and pp.Tpfa / pp.Upwind) rebound to the porepy_b200
-plugin classes.
+read-only tree) with pp.Mpfa / pp.Mpsa / pp.Biot / pp.Tpsa (and pp.Tpfa / pp.Upwind / pp.MVEM / pp.RT0) rebound to the
+porepy_b200 plugin classes.  The mixed schemes' tests are named on the command line:
+
+    python tools/run_reference_tests.py numerics/vem/test_dual_vem.py numerics/vem/test_rt0.py
 
     python tools/run_reference_tests.py            # build container or any box with /root/reference
     python tools/run_reference_tests.py functional/test_terzaghi.py [--stock] [pytest options]
@@ -37,12 +39,14 @@ class Rebind:
         if not gpu:
             from emu_binding import EmuBackedPlan
             from emu_tpsa import EmuTpsaFaceGrid   # the host build of the per-face routines, TPSA included
+            from emu_dual import EmuDualGrid   # the host build of the MVEM / RT0 routines
             fv.DevicePlan = EmuBackedPlan
             fv.FaceGrid = EmuTpsaFaceGrid
+            fv.DualGrid = EmuDualGrid
             import emu_binding
             fv.interface_upwind_masks = emu_binding.emu_interface_upwind_masks
         COUNTS["backend: " + ("cuda" if gpu else "host build of the node routines")] = 1
-        for name in ("Mpfa", "Mpsa", "Biot", "Tpfa", "Upwind", "Tpsa"):
+        for name in ("Mpfa", "Mpsa", "Biot", "Tpfa", "Upwind", "Tpsa", "MVEM", "RT0"):
             for owner, tag in ((getattr(fv, name), "porepy_b200"), (getattr(pp, name), "reference")):
                 stock = owner.discretize
 

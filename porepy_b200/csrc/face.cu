@@ -7,6 +7,19 @@
 #include "tpsa_face.cuh"
 #include "tpsa_system.cuh"
 
+#include <array>
+
+// {nd, scalar balances, flux-pattern nnz}: what a TPSA row pattern was built for; nd = 0: no pattern
+using TpsaKey = std::array<int64_t, 3>;
+
+// The row pattern of one TPSA system: CSR arrays of nnz entries and, for the poromechanics and contact systems, the
+// first entry of each block row.  Rebuilt when a call asks for another key.
+struct TpsaPattern {
+    TpsaKey key{};
+    int64_t nnz = 0;
+    DevBuf blk, ip, ix;
+};
+
 struct pb_facegrid {
     int64_t nc = 0, nf = 0;
     cudaStream_t stream = nullptr;
@@ -14,24 +27,17 @@ struct pb_facegrid {
     DevBuf cf_ip, cf_ix;                                  // cell -> face lists (cell_faces, CSC)
     std::vector<uint8_t> face_ncell;                      // host: cells per face
     GeoView geo{};
-    // TPSA system (pb_tpsa_system): the row pattern, built once per topology and dimension, and the face values of
-    // the last assembly (read again by pb_tpsa_rhs)
-    int sys_nd = 0, terms_nd = 0;
-    int64_t sys_nnz = 0, sys_npairs = 0;
-    DevBuf fc_ptr, cc_ptr, cc_ix, cc_cell, sys_ip, sys_ix, terms[PB_TPSA_NTERMS];
-    // TPSA poromechanics / thermo-poromechanics system (pb_tpsa_poro_system, pb_tpsa_thm_system): its row pattern,
-    // built once per dimension, number of scalar balances and flux pattern
-    bool nb_ready = false;
-    int poro_nd = 0, poro_ns = 0;
-    int64_t poro_nnz = 0, poro_fp_nnz = -1;
-    DevBuf blk_ptr, poro_ip, poro_ix;
-    // TPSA contact system (pb_tpsa_contact_system): the interfaces of the last call (host copies of their topology) and
-    // the row pattern, built once per dimension and interface topology
-    int ctc_nd = 0;
-    int64_t ctc_nm = -1, ctc_nk = -1, ctc_ncell = 0, ctc_nnz = 0;
+    // TPSA systems: the neighbour lists of every cell (npairs < 0: not built yet), the face values of the last assembly
+    // (read again by the pb_tpsa*_rhs calls) and the row pattern of each system; the three patterns live side by side
+    int terms_nd = 0;
+    int64_t npairs = -1;
+    DevBuf fc_ptr, cc_ptr, cc_ix, cc_cell, terms[PB_TPSA_NTERMS];
+    TpsaPattern sys, poro, ctc;
+    // TPSA contact system: the interfaces of the last call (host copies of their topology)
+    int64_t ctc_nm = -1, ctc_nk = -1;
     double ctc_ct = 0.0;
     std::vector<int32_t> ctc_face_h, ctc_cell_h;
-    DevBuf ctc_fm, ctc_face, ctc_cell, ctc_pair, ctc_w, ctc_frame, ctc_blk, ctc_ip, ctc_ix;
+    DevBuf ctc_fm, ctc_face, ctc_cell, ctc_pair, ctc_w, ctc_frame;
 };
 
 // one thread per cell: claim the first free slot of each of its faces
@@ -276,80 +282,153 @@ extern "C" int pb_facegrid_set_face_areas(pb_facegrid *g, const double *face_are
     return PB_OK;
 }
 
-// Two-point stress approximation (tpsa_face.cuh): value arrays of the 14 terms, layouts in include/poreb200.h.
-extern "C" int pb_tpsa(pb_facegrid *g, int nd, const double *mu, const uint8_t *codes, const double *robin_diag,
-                       const uint8_t *face_flags, const int32_t *fc_indptr, double **out, float *kernel_ms) {
-    if (!g || !mu || !codes || !face_flags || !fc_indptr || !out) return pb_fail_(PB_EINVAL, "null pointer");
-    if (nd != 2 && nd != 3) return pb_fail_(PB_EINVAL, "Tpsa is only implemented for 2d and 3d grids.");
-    if (!g->geo.farea) return pb_fail_(PB_EINVAL, "face areas not set (pb_facegrid_set_face_areas)");
-    const int64_t nf = g->nf, nc = g->nc;
-    for (int64_t c = 0; c < nc; ++c)   // the scheme divides by mu and by mu / distance
-        if (!(mu[c] > 0.0) || !std::isfinite(mu[c])) return pb_fail_(PB_EINVAL, "shear modulus must be finite and > 0");
-    bool any_rob = false;
-    for (int64_t q = 0; q < nd * nf; ++q) {
-        if (codes[q] > PB_BC_ROB) return pb_fail_(PB_EINVAL, "boundary code out of range");
-        any_rob |= codes[q] == PB_BC_ROB;
-    }
-    if (any_rob && !robin_diag) return pb_fail_(PB_EINVAL, "Robin faces need robin_diag");
-    for (int64_t f = 0; f < nf; ++f) {
-        const int32_t len = fc_indptr[f + 1] - fc_indptr[f];
-        if (len < 1 || len > 2) return pb_fail_(PB_EINVAL, "fc_indptr: a face has one or two cells");
-        if (face_flags[f] && len != 1) return pb_fail_(PB_EINVAL, "sign of internal faces does not make sense");
-    }
-    cudaStream_t st = g->stream;
-    const size_t nnz = (size_t)fc_indptr[nf];
-    const size_t nr = nd == 3 ? 3 : 1;
-    // values per (face, cell) entry or per face, in PB_TPSA_* order
-    const size_t per[PB_TPSA_NTERMS] = {(size_t)nd, nd * nr, (size_t)nd, nr * nd, nr * nr, (size_t)nd, 1, (size_t)nd,
-                                        nd * nr, (size_t)nd, (size_t)nd, nr * nd, (size_t)nd, (size_t)nd};
-    DevBuf dmu, dcodes, drob, dflags, dip, o_buf[PB_TPSA_NTERMS];
-    CUDA_TRY(dmu.upload(mu, (size_t)nc, st));
-    CUDA_TRY(dcodes.upload(codes, (size_t)nd * nf, st));
-    if (any_rob) CUDA_TRY(drob.upload(robin_diag, (size_t)nd * nf, st));
-    CUDA_TRY(dflags.upload(face_flags, (size_t)nf, st));
-    CUDA_TRY(dip.upload(fc_indptr, (size_t)nf + 1, st));
-    TpsaOut o{};
-    size_t count[PB_TPSA_NTERMS];
-    for (int k = 0; k < PB_TPSA_NTERMS; ++k) {
-        count[k] = per[k] * (k < PB_TPSA_BOUND_STRESS ? nnz : (size_t)nf);
-        if (!out[k]) continue;
-        CUDA_TRY(o_buf[k].ensure(count[k] * sizeof(double)));
-        o.t[k] = o_buf[k].as<double>();
-    }
-    struct Events {
-        cudaEvent_t e0 = nullptr, e1 = nullptr;
-        ~Events() { if (e0) cudaEventDestroy(e0); if (e1) cudaEventDestroy(e1); }
-    } ev;
-    if (kernel_ms) {
-        CUDA_TRY(cudaEventCreate(&ev.e0));
-        CUDA_TRY(cudaEventCreate(&ev.e1));
-        CUDA_TRY(cudaEventRecord(ev.e0, st));
-    }
-    const int block = 256;
-    const int grid = (int)std::max<int64_t>(1, std::min<int64_t>((nf + block - 1) / block, (int64_t)pb_sm_count() * 16));
-    const double *rw = any_rob ? drob.as<double>() : nullptr;
-    if (nd == 3)
-        tpsa_kernel<3><<<grid, block, 0, st>>>(nf, g->geo, dmu.as<double>(), dcodes.as<uint8_t>(), rw,
-                                              dflags.as<uint8_t>(), g->face_cells.as<int32_t>(), dip.as<int32_t>(), o);
-    else
-        tpsa_kernel<2><<<grid, block, 0, st>>>(nf, g->geo, dmu.as<double>(), dcodes.as<uint8_t>(), rw,
-                                              dflags.as<uint8_t>(), g->face_cells.as<int32_t>(), dip.as<int32_t>(), o);
-    pb_count_launch_();
-    CUDA_TRY(cudaGetLastError());
-    if (kernel_ms) CUDA_TRY(cudaEventRecord(ev.e1, st));
-    for (int k = 0; k < PB_TPSA_NTERMS; ++k)
-        if (out[k]) CUDA_TRY(cudaMemcpyAsync(out[k], o_buf[k].p, count[k] * sizeof(double), cudaMemcpyDeviceToHost, st));
-    CUDA_TRY(cudaStreamSynchronize(st));
-    if (kernel_ms) CUDA_TRY(cudaEventElapsedTime(kernel_ms, ev.e0, ev.e1));
-    return PB_OK;
-}
-
-// ---- TPSA three-field system (tpsa_system.cuh) -----------------------------------------------------------------
+// ---- TPSA: the per-face terms (tpsa_face.cuh) and the assembled systems (tpsa_system.cuh) -------------------------
 struct pb_csr;
 int pb_csr_from_device_pattern_(int64_t nrows, int64_t ncols, int64_t nnz, const int32_t *indptr_dev,
                                 const int32_t *indices_dev, pb_csr **out);   // spmv.cu
 double *pb_csr_data_(pb_csr *a);                                              // spmv.cu
+struct CsrView { int64_t nrows, ncols, nnz; int32_t *indptr, *indices; double *data; };
+CsrView pb_csr_view_(const pb_csr *a);                                        // spmv.cu
 
+static int fg_grid(int64_t n) {
+    return (int)std::max<int64_t>(1, std::min<int64_t>((n + 255) / 256, (int64_t)pb_sm_count() * 16));
+}
+
+// Calls f with std::integral_constant<int, nd> (nd = 2 or 3): a launch site names its kernel<ND> once.
+template <class F>
+static void tpsa_nd(int nd, F &&f) {
+    if (nd == 3) f(std::integral_constant<int, 3>{});
+    else f(std::integral_constant<int, 2>{});
+}
+
+struct FgEvents {
+    cudaEvent_t e[3] = {nullptr, nullptr, nullptr};
+    ~FgEvents() { for (auto x : e) if (x) cudaEventDestroy(x); }
+};
+
+// Inputs of the TPSA calls on the device.
+struct TpsaInputs {
+    DevBuf mu, lam, vol, codes, rob, flags;
+    bool any_rob = false;
+};
+
+// Checks the inputs and uploads them: lambda and cell_volumes only when given (the systems), the cells of each face from
+// fc_indptr when given (pb_tpsa), else from the handle, whose fc_ptr is then built once.
+static int tpsa_prepare(pb_facegrid *g, int nd, const double *mu, const double *lambda, const double *cell_volumes,
+                        const uint8_t *codes, const double *robin_diag, const uint8_t *face_flags,
+                        const int32_t *fc_indptr, TpsaInputs &in) {
+    if (nd != 2 && nd != 3) return pb_fail_(PB_EINVAL, "Tpsa is only implemented for 2d and 3d grids.");
+    if (!g->geo.farea) return pb_fail_(PB_EINVAL, "face areas not set (pb_facegrid_set_face_areas)");
+    const int64_t nf = g->nf, nc = g->nc;
+    for (int64_t c = 0; c < nc; ++c) {   // the scheme divides by mu and by mu / distance, the systems by lambda
+        if (!(mu[c] > 0.0) || !std::isfinite(mu[c])) return pb_fail_(PB_EINVAL, "shear modulus must be finite and > 0");
+        if (lambda && (!(lambda[c] > 0.0) || !std::isfinite(lambda[c])))
+            return pb_fail_(PB_EINVAL, "first Lame parameter lambda must be finite and > 0");
+    }
+    for (int64_t q = 0; q < nd * nf; ++q) {
+        if (codes[q] > PB_BC_ROB) return pb_fail_(PB_EINVAL, "boundary code out of range");
+        in.any_rob |= codes[q] == PB_BC_ROB;
+    }
+    if (in.any_rob && !robin_diag) return pb_fail_(PB_EINVAL, "Robin faces need robin_diag");
+    for (int64_t f = 0; f < nf; ++f) {
+        const int len = fc_indptr ? fc_indptr[f + 1] - fc_indptr[f] : g->face_ncell[f];
+        if (len < 1 || len > 2) return pb_fail_(PB_EINVAL, "fc_indptr: a face has one or two cells");
+        if (face_flags[f] && len != 1) return pb_fail_(PB_EINVAL, "sign of internal faces does not make sense");
+    }
+    cudaStream_t st = g->stream;
+    if (!fc_indptr && !g->fc_ptr.p) {   // CSR-by-face row pointer of cell_faces: where each face's (face, cell) values start
+        std::vector<int32_t> fp((size_t)nf + 1, 0);
+        for (int64_t f = 0; f < nf; ++f) fp[f + 1] = fp[f] + g->face_ncell[f];
+        CUDA_TRY(g->fc_ptr.upload(fp, st));
+        CUDA_TRY(cudaStreamSynchronize(st));
+    }
+    CUDA_TRY(in.mu.upload(mu, (size_t)nc, st));
+    if (lambda) CUDA_TRY(in.lam.upload(lambda, (size_t)nc, st));
+    if (cell_volumes) CUDA_TRY(in.vol.upload(cell_volumes, (size_t)nc, st));
+    CUDA_TRY(in.codes.upload(codes, (size_t)nd * nf, st));
+    if (in.any_rob) CUDA_TRY(in.rob.upload(robin_diag, (size_t)nd * nf, st));
+    CUDA_TRY(in.flags.upload(face_flags, (size_t)nf, st));
+    return PB_OK;
+}
+
+// The per-face kernel on the inputs in; fc_ptr[f]: the first (face, cell) entry of face f.
+static int tpsa_face_launch(pb_facegrid *g, int nd, const TpsaInputs &in, const int32_t *fc_ptr, const TpsaOut &o) {
+    const int64_t nf = g->nf;
+    const double *rw = in.any_rob ? in.rob.as<double>() : nullptr;
+    tpsa_nd(nd, [&](auto ND) {
+        tpsa_kernel<ND><<<fg_grid(nf), 256, 0, g->stream>>>(nf, g->geo, in.mu.as<double>(), in.codes.as<uint8_t>(), rw,
+                                                             in.flags.as<uint8_t>(), g->face_cells.as<int32_t>(), fc_ptr,
+                                                             o);
+    });
+    pb_count_launch_();
+    CUDA_TRY(cudaGetLastError());
+    return PB_OK;
+}
+
+// Two-point stress approximation (tpsa_face.cuh): value arrays of the 14 terms, layouts in include/poreb200.h.
+extern "C" int pb_tpsa(pb_facegrid *g, int nd, const double *mu, const uint8_t *codes, const double *robin_diag,
+                       const uint8_t *face_flags, const int32_t *fc_indptr, double **out, float *kernel_ms) {
+    if (!g || !mu || !codes || !face_flags || !fc_indptr || !out) return pb_fail_(PB_EINVAL, "null pointer");
+    TpsaInputs in;
+    int rc = tpsa_prepare(g, nd, mu, nullptr, nullptr, codes, robin_diag, face_flags, fc_indptr, in);
+    if (rc) return rc;
+    cudaStream_t st = g->stream;
+    const int64_t nf = g->nf;
+    DevBuf dip, o_buf[PB_TPSA_NTERMS];
+    CUDA_TRY(dip.upload(fc_indptr, (size_t)nf + 1, st));
+    TpsaOut o{};
+    size_t count[PB_TPSA_NTERMS];
+    for (int k = 0; k < PB_TPSA_NTERMS; ++k) {
+        count[k] = tpsa_term_size(k, nd, (size_t)fc_indptr[nf], (size_t)nf);
+        if (!out[k]) continue;
+        CUDA_TRY(o_buf[k].ensure(count[k] * sizeof(double)));
+        o.t[k] = o_buf[k].as<double>();
+    }
+    FgEvents ev;
+    if (kernel_ms) {
+        CUDA_TRY(cudaEventCreate(&ev.e[0]));
+        CUDA_TRY(cudaEventCreate(&ev.e[1]));
+        CUDA_TRY(cudaEventRecord(ev.e[0], st));
+    }
+    if ((rc = tpsa_face_launch(g, nd, in, dip.as<int32_t>(), o))) return rc;
+    if (kernel_ms) CUDA_TRY(cudaEventRecord(ev.e[1], st));
+    for (int k = 0; k < PB_TPSA_NTERMS; ++k)
+        if (out[k]) CUDA_TRY(cudaMemcpyAsync(out[k], o_buf[k].p, count[k] * sizeof(double), cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(cudaStreamSynchronize(st));
+    if (kernel_ms) CUDA_TRY(cudaEventElapsedTime(kernel_ms, ev.e[0], ev.e[1]));
+    return PB_OK;
+}
+
+// Stage 1 of the systems: the ten face terms they read, into buffers kept on the handle (T points at them).
+static int tpsa_face_terms(pb_facegrid *g, int nd, const TpsaInputs &in, TpsaTerms &T) {
+    const int64_t nf = g->nf;
+    int64_t nfc = 0;   // (face, cell) entries
+    for (int64_t f = 0; f < nf; ++f) nfc += g->face_ncell[f];
+    const bool used[PB_TPSA_NTERMS] = {true, true, true, true, true, true, true, false, false, false, true, true, true,
+                                       false};
+    TpsaOut o{};
+    for (int k = 0; k < PB_TPSA_NTERMS; ++k) {
+        if (!used[k]) continue;
+        CUDA_TRY(g->terms[k].ensure(tpsa_term_size(k, nd, (size_t)nfc, (size_t)nf) * sizeof(double)));
+        o.t[k] = g->terms[k].as<double>();
+        T.t[k] = o.t[k];
+    }
+    return tpsa_face_launch(g, nd, in, g->fc_ptr.as<int32_t>(), o);
+}
+
+static TpsaTopo tpsa_topo(pb_facegrid *g) {
+    return TpsaTopo{g->nc, g->cf_ip.as<int32_t>(), g->cf_ix.as<int32_t>(), g->face_cells.as<int32_t>(),
+                    g->fc_ptr.as<int32_t>()};
+}
+
+static TpsaMortars tpsa_mortars(pb_facegrid *g) {
+    const int64_t nm = g->ctc_nm;
+    const double *w = g->ctc_w.as<double>();
+    return TpsaMortars{nm, g->ctc_nk, g->ctc_face.as<int32_t>(), g->ctc_cell.as<int32_t>(), g->ctc_fm.as<int32_t>(),
+                       g->ctc_pair.as<int32_t>(), w, w + nm, w + 2 * nm, w + 3 * nm, g->ctc_frame.as<double>(), g->ctc_ct};
+}
+
+// ---- neighbour lists and row patterns ------------------------------------------------------------------------------
 __global__ void tpsa_nb_count_kernel(TpsaTopo t, int32_t *__restrict__ count, int *bad) {
     for (int64_t c = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; c < t.nc; c += (int64_t)gridDim.x * blockDim.x) {
         int32_t nb[kTpsaMaxNb];
@@ -359,55 +438,20 @@ __global__ void tpsa_nb_count_kernel(TpsaTopo t, int32_t *__restrict__ count, in
     }
 }
 
-template <int ND>
-__global__ void tpsa_pattern_kernel(TpsaTopo t, const int32_t *__restrict__ cc_ptr, int32_t *__restrict__ cc_ix,
-                                    int32_t *__restrict__ cc_cell, int32_t *__restrict__ ip, int32_t *__restrict__ ix) {
+__global__ void tpsa_nb_list_kernel(TpsaTopo t, const int32_t *__restrict__ cc_ptr, int32_t *__restrict__ cc_ix,
+                                    int32_t *__restrict__ cc_cell) {
     for (int64_t c = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; c < t.nc; c += (int64_t)gridDim.x * blockDim.x) {
         int32_t nb[kTpsaMaxNb];
         const int n = tpsa_cell_neighbours(c, t, nb);
         for (int j = 0; j < n; ++j) { cc_ix[cc_ptr[c] + j] = nb[j]; cc_cell[cc_ptr[c] + j] = (int32_t)c; }
-        tpsa_pattern_rows<ND>(c, n, nb, cc_ptr[c], ip, ix);
     }
 }
 
-// one thread per block (c, k) of A, i.e. per entry of the neighbour lists: consecutive threads write consecutive
-// segments of the same rows
-template <int ND>
-__global__ void tpsa_system_kernel(int64_t npairs, TpsaTopo t, const int32_t *__restrict__ cc_ptr,
-                                   const int32_t *__restrict__ cc_ix, const int32_t *__restrict__ cc_cell, TpsaTerms T,
-                                   const double *__restrict__ mu, const double *__restrict__ lam,
-                                   const double *__restrict__ vol, double *__restrict__ a) {
-    for (int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; e < npairs; e += (int64_t)gridDim.x * blockDim.x) {
-        const int64_t c = cc_cell[e];
-        tpsa_system_block<ND>(c, (int)(e - cc_ptr[c]), t, cc_ptr, cc_ix, T, mu, lam, vol, a);
-    }
-}
-
-template <int ND>
-__global__ void tpsa_rhs_kernel(TpsaTopo t, TpsaTerms T, const double *__restrict__ g, const double *__restrict__ f,
-                                const double *__restrict__ sr, const double *__restrict__ sp, double *__restrict__ b) {
-    constexpr int NR = TpsaDims<ND>::NR, B = TpsaDims<ND>::B;
-    for (int64_t q = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; q < t.nc * B; q += (int64_t)gridDim.x * blockDim.x) {
-        const int64_t c = q / B;
-        const int l = (int)(q - c * B);
-        const double src = l < ND ? (f ? f[c * ND + l] : 0.0)
-                                   : (l < ND + NR ? (sr ? sr[c * NR + l - ND] : 0.0) : (sp ? sp[c] : 0.0));
-        b[q] = tpsa_rhs_row<ND>(c, l, t, T, g, src);
-    }
-}
-
-static int fg_grid(int64_t n) {
-    return (int)std::max<int64_t>(1, std::min<int64_t>((n + 255) / 256, (int64_t)pb_sm_count() * 16));
-}
-
-static TpsaTopo tpsa_topo(pb_facegrid *g) {
-    return TpsaTopo{g->nc, g->cf_ip.as<int32_t>(), g->cf_ix.as<int32_t>(), g->face_cells.as<int32_t>(),
-                    g->fc_ptr.as<int32_t>()};
-}
-
-// Neighbour counts of every cell, scanned into cc_ptr; *total = number of (cell, neighbour) pairs.  cc_ix / cc_cell are
-// sized for them.
-static int tpsa_neighbour_counts(pb_facegrid *g, int64_t *total_out) {
+// The neighbour lists of every cell, built once per handle and read by the patterns and block kernels of every TPSA
+// system: cc_ix[cc_ptr[c] ..] the distinct cells sharing a face with c, c included, ascending; cc_cell the cell of
+// each of the npairs entries.
+static int tpsa_neighbours(pb_facegrid *g) {
+    if (g->npairs >= 0) return PB_OK;
     cudaStream_t st = g->stream;
     const int64_t nc = g->nc;
     const TpsaTopo t = tpsa_topo(g);
@@ -427,215 +471,71 @@ static int tpsa_neighbour_counts(pb_facegrid *g, int64_t *total_out) {
     if (hbad) return pb_fail_(PB_ENOTIMPL, "Tpsa system: a cell has more than 31 face neighbours");
     CUDA_TRY(g->cc_ix.ensure((size_t)std::max<int64_t>(1, total) * sizeof(int32_t)));
     CUDA_TRY(g->cc_cell.ensure((size_t)std::max<int64_t>(1, total) * sizeof(int32_t)));
-    *total_out = total;
+    tpsa_nb_list_kernel<<<fg_grid(nc), 256, 0, st>>>(t, g->cc_ptr.as<int32_t>(), g->cc_ix.as<int32_t>(),
+                                                      g->cc_cell.as<int32_t>());
+    pb_count_launch_();
+    CUDA_TRY(cudaGetLastError());
+    g->npairs = total;
     return PB_OK;
 }
 
-// Row pattern of the system for dimension nd: neighbour lists, block-row offsets and the CSR arrays of A.
-static int tpsa_build_pattern(pb_facegrid *g, int nd) {
-    cudaStream_t st = g->stream;
-    const int64_t nc = g->nc;
-    const int B = nd == 3 ? 7 : 4, NZ = nd == 3 ? 37 : 12;
-    const TpsaTopo t = tpsa_topo(g);
-    int64_t total = 0;
-    int rc0 = tpsa_neighbour_counts(g, &total);
-    if (rc0) return rc0;
-    const int64_t nnz = (int64_t)NZ * total;
+// Sizes the CSR arrays of P for nrows rows and nnz entries and writes the last row pointer; the pattern kernels write
+// the others.
+static int tpsa_pattern_alloc(pb_facegrid *g, TpsaPattern &P, int64_t nrows, int64_t nnz) {
     if (nnz >= 0x7FFFFFFFll) return pb_fail_(PB_ENOTIMPL, "Tpsa system: the matrix does not fit int32 indices");
-    CUDA_TRY(g->sys_ip.ensure((size_t)(nc * B + 1) * sizeof(int32_t)));
-    CUDA_TRY(g->sys_ix.ensure((size_t)std::max<int64_t>(1, nnz) * sizeof(int32_t)));
+    CUDA_TRY(P.ip.ensure((size_t)(nrows + 1) * sizeof(int32_t)));
+    CUDA_TRY(P.ix.ensure((size_t)std::max<int64_t>(1, nnz) * sizeof(int32_t)));
     const int32_t last = (int32_t)nnz;
-    CUDA_TRY(cudaMemcpyAsync(g->sys_ip.as<int32_t>() + nc * B, &last, sizeof(int32_t), cudaMemcpyHostToDevice, st));
-    if (nd == 3)
-        tpsa_pattern_kernel<3><<<fg_grid(nc), 256, 0, st>>>(t, g->cc_ptr.as<int32_t>(), g->cc_ix.as<int32_t>(),
-                                                             g->cc_cell.as<int32_t>(), g->sys_ip.as<int32_t>(),
-                                                             g->sys_ix.as<int32_t>());
-    else
-        tpsa_pattern_kernel<2><<<fg_grid(nc), 256, 0, st>>>(t, g->cc_ptr.as<int32_t>(), g->cc_ix.as<int32_t>(),
-                                                             g->cc_cell.as<int32_t>(), g->sys_ip.as<int32_t>(),
-                                                             g->sys_ix.as<int32_t>());
+    CUDA_TRY(cudaMemcpyAsync(P.ip.as<int32_t>() + nrows, &last, sizeof(int32_t), cudaMemcpyHostToDevice, g->stream));
+    P.nnz = nnz;
+    return PB_OK;
+}
+
+// P.blk: the first entry of every block row, from the entries per row that count(n) writes into n; *total: their sum.
+template <class Count>
+static int tpsa_block_offsets(pb_facegrid *g, TpsaPattern &P, int64_t *total, Count &&count) {
+    DevBuf n;
+    CUDA_TRY(n.ensure((size_t)g->nc * sizeof(int32_t)));
+    count(n.as<int32_t>());
     pb_count_launch_();
     CUDA_TRY(cudaGetLastError());
-    CUDA_TRY(cudaStreamSynchronize(st));
-    g->sys_nd = nd;
-    g->sys_nnz = nnz;
-    g->sys_npairs = total;
-    g->nb_ready = true;
-    return PB_OK;
+    CUDA_TRY(P.blk.ensure((size_t)(g->nc + 1) * sizeof(int64_t)));
+    return pb_scan_offsets_(n.as<int32_t>(), P.blk.as<int64_t>(), g->nc, g->stream, total);
 }
 
-struct FgEvents {
-    cudaEvent_t e[3] = {nullptr, nullptr, nullptr};
-    ~FgEvents() { for (auto x : e) if (x) cudaEventDestroy(x); }
-};
-
-// Inputs of both TPSA systems on the device, checked as pb_tpsa checks them (lambda also finite and > 0).
-struct TpsaInputs {
-    DevBuf mu, lam, vol, codes, rob, flags;
-    bool any_rob = false;
-};
-
-static int tpsa_prepare(pb_facegrid *g, int nd, const double *mu, const double *lambda, const double *cell_volumes,
-                        const uint8_t *codes, const double *robin_diag, const uint8_t *face_flags, TpsaInputs &in) {
-    if (nd != 2 && nd != 3) return pb_fail_(PB_EINVAL, "Tpsa is only implemented for 2d and 3d grids.");
-    if (!g->geo.farea) return pb_fail_(PB_EINVAL, "face areas not set (pb_facegrid_set_face_areas)");
-    const int64_t nf = g->nf, nc = g->nc;
-    for (int64_t c = 0; c < nc; ++c) {
-        if (!(mu[c] > 0.0) || !std::isfinite(mu[c])) return pb_fail_(PB_EINVAL, "shear modulus must be finite and > 0");
-        if (!(lambda[c] > 0.0) || !std::isfinite(lambda[c]))
-            return pb_fail_(PB_EINVAL, "first Lame parameter lambda must be finite and > 0");
-    }
-    for (int64_t q = 0; q < nd * nf; ++q) {
-        if (codes[q] > PB_BC_ROB) return pb_fail_(PB_EINVAL, "boundary code out of range");
-        in.any_rob |= codes[q] == PB_BC_ROB;
-    }
-    if (in.any_rob && !robin_diag) return pb_fail_(PB_EINVAL, "Robin faces need robin_diag");
-    for (int64_t f = 0; f < nf; ++f) {
-        const int len = g->face_ncell[f];
-        if (len < 1 || len > 2) return pb_fail_(PB_EINVAL, "fc_indptr: a face has one or two cells");
-        if (face_flags[f] && len != 1) return pb_fail_(PB_EINVAL, "sign of internal faces does not make sense");
-    }
-    cudaStream_t st = g->stream;
-    if (!g->fc_ptr.p) {   // CSR-by-face row pointer of cell_faces: where each face's (face, cell) values start
-        std::vector<int32_t> fp((size_t)nf + 1, 0);
-        for (int64_t f = 0; f < nf; ++f) fp[f + 1] = fp[f] + g->face_ncell[f];
-        CUDA_TRY(g->fc_ptr.upload(fp, st));
-        CUDA_TRY(cudaStreamSynchronize(st));
-    }
-    CUDA_TRY(in.mu.upload(mu, (size_t)nc, st));
-    CUDA_TRY(in.lam.upload(lambda, (size_t)nc, st));
-    CUDA_TRY(in.vol.upload(cell_volumes, (size_t)nc, st));
-    CUDA_TRY(in.codes.upload(codes, (size_t)nd * nf, st));
-    if (in.any_rob) CUDA_TRY(in.rob.upload(robin_diag, (size_t)nd * nf, st));
-    CUDA_TRY(in.flags.upload(face_flags, (size_t)nf, st));
-    return PB_OK;
-}
-
-// Stage 1: the ten face terms the systems read, into buffers kept on the handle (T points at them).
-static int tpsa_face_terms(pb_facegrid *g, int nd, const TpsaInputs &in, TpsaTerms &T) {
-    const int64_t nf = g->nf;
-    int64_t nfc = 0;   // (face, cell) entries
-    for (int64_t f = 0; f < nf; ++f) nfc += g->face_ncell[f];
-    const size_t nr = nd == 3 ? 3 : 1;
-    const size_t per[PB_TPSA_NTERMS] = {(size_t)nd, nd * nr, (size_t)nd, nr * nd, nr * nr, (size_t)nd, 1, (size_t)nd,
-                                        nd * nr, (size_t)nd, (size_t)nd, nr * nd, (size_t)nd, (size_t)nd};
-    const bool used[PB_TPSA_NTERMS] = {true, true, true, true, true, true, true, false, false, false, true, true, true,
-                                       false};
-    TpsaOut o{};
-    for (int k = 0; k < PB_TPSA_NTERMS; ++k) {
-        if (!used[k]) continue;
-        CUDA_TRY(g->terms[k].ensure(per[k] * (k < PB_TPSA_BOUND_STRESS ? (size_t)nfc : (size_t)nf) * sizeof(double)));
-        o.t[k] = g->terms[k].as<double>();
-        T.t[k] = o.t[k];
-    }
-    cudaStream_t st = g->stream;
-    const double *rw = in.any_rob ? in.rob.as<double>() : nullptr;
-    const int32_t *fcp = g->fc_ptr.as<int32_t>();
-    if (nd == 3)
-        tpsa_kernel<3><<<fg_grid(nf), 256, 0, st>>>(nf, g->geo, in.mu.as<double>(), in.codes.as<uint8_t>(), rw,
-                                                     in.flags.as<uint8_t>(), g->face_cells.as<int32_t>(), fcp, o);
-    else
-        tpsa_kernel<2><<<fg_grid(nf), 256, 0, st>>>(nf, g->geo, in.mu.as<double>(), in.codes.as<uint8_t>(), rw,
-                                                     in.flags.as<uint8_t>(), g->face_cells.as<int32_t>(), fcp, o);
-    pb_count_launch_();
-    CUDA_TRY(cudaGetLastError());
-    return PB_OK;
-}
-
-extern "C" int pb_tpsa_system(pb_facegrid *g, int nd, const double *mu, const double *lambda,
-                              const double *cell_volumes, const uint8_t *codes, const double *robin_diag,
-                              const uint8_t *face_flags, pb_csr **out, float *stage_ms) {
-    if (!g || !mu || !lambda || !cell_volumes || !codes || !face_flags || !out)
-        return pb_fail_(PB_EINVAL, "null pointer");
-    TpsaInputs in;
-    int rc = tpsa_prepare(g, nd, mu, lambda, cell_volumes, codes, robin_diag, face_flags, in);
+// Makes P the row pattern for key unless it already is: build(ND), ND = key[0], sizes P and launches the pattern
+// kernels on the neighbour lists.
+template <class Build>
+static int tpsa_pattern(pb_facegrid *g, TpsaPattern &P, const TpsaKey &key, Build &&build) {
+    if (P.key == key) return PB_OK;
+    P.key = {};
+    int rc = tpsa_neighbours(g);
+    if (!rc) tpsa_nd((int)key[0], [&](auto ND) { rc = build(ND); });
     if (rc) return rc;
-    if (g->sys_nd != nd) {
-        g->sys_nd = 0;
-        rc = tpsa_build_pattern(g, nd);
-        if (rc) return rc;
-    }
-    cudaStream_t st = g->stream;
+    pb_count_launch_();
+    CUDA_TRY(cudaGetLastError());
+    CUDA_TRY(cudaStreamSynchronize(g->stream));
+    P.key = key;
+    return PB_OK;
+}
+
+template <int ND>
+__global__ void tpsa_pattern_kernel(int64_t nc, const int32_t *__restrict__ cc_ptr, const int32_t *__restrict__ cc_ix,
+                                    int32_t *__restrict__ ip, int32_t *__restrict__ ix) {
+    for (int64_t c = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; c < nc; c += (int64_t)gridDim.x * blockDim.x)
+        tpsa_pattern_rows<ND>(c, cc_ptr[c + 1] - cc_ptr[c], cc_ix + cc_ptr[c], cc_ptr[c], ip, ix);
+}
+
+// Row pattern of the three-field system: NZ entries per neighbour.
+template <int ND>
+static int tpsa_sys_pattern(pb_facegrid *g) {
     const int64_t nc = g->nc;
-    pb_csr *a = nullptr;
-    rc = pb_csr_from_device_pattern_(nc * (nd == 3 ? 7 : 4), nc * (nd == 3 ? 7 : 4), g->sys_nnz,
-                                     g->sys_ip.as<int32_t>(), g->sys_ix.as<int32_t>(), &a);
+    TpsaPattern &P = g->sys;
+    const int rc = tpsa_pattern_alloc(g, P, nc * TpsaDims<ND>::B, (int64_t)TpsaDims<ND>::NZ * g->npairs);
     if (rc) return rc;
-    FgEvents ev;
-    auto fail_cuda = [&](cudaError_t e, const char *what) {
-        pb_csr_destroy(a);
-        return pb_fail_(PB_ECUDA, std::string(what) + ": " + cudaGetErrorString(e));
-    };
-#define SYS_TRY(x) do { cudaError_t e_ = (x); if (e_ != cudaSuccess) return fail_cuda(e_, #x); } while (0)
-    if (stage_ms)
-        for (auto &x : ev.e) SYS_TRY(cudaEventCreate(&x));
-    if (stage_ms) SYS_TRY(cudaEventRecord(ev.e[0], st));
-    TpsaTerms T{};
-    if ((rc = tpsa_face_terms(g, nd, in, T))) { pb_csr_destroy(a); return rc; }
-    if (stage_ms) SYS_TRY(cudaEventRecord(ev.e[1], st));
-    // stage 2: every block of A gathered from the faces of its cell
-    const TpsaTopo t = tpsa_topo(g);
-    const int64_t np = g->sys_npairs;
-    if (nd == 3)
-        tpsa_system_kernel<3><<<fg_grid(np), 256, 0, st>>>(np, t, g->cc_ptr.as<int32_t>(), g->cc_ix.as<int32_t>(),
-                                                            g->cc_cell.as<int32_t>(), T, in.mu.as<double>(),
-                                                            in.lam.as<double>(), in.vol.as<double>(), pb_csr_data_(a));
-    else
-        tpsa_system_kernel<2><<<fg_grid(np), 256, 0, st>>>(np, t, g->cc_ptr.as<int32_t>(), g->cc_ix.as<int32_t>(),
-                                                            g->cc_cell.as<int32_t>(), T, in.mu.as<double>(),
-                                                            in.lam.as<double>(), in.vol.as<double>(), pb_csr_data_(a));
-    pb_count_launch_();
-    SYS_TRY(cudaGetLastError());
-    if (stage_ms) SYS_TRY(cudaEventRecord(ev.e[2], st));
-    SYS_TRY(cudaStreamSynchronize(st));
-    if (stage_ms) {
-        SYS_TRY(cudaEventElapsedTime(stage_ms, ev.e[0], ev.e[1]));
-        SYS_TRY(cudaEventElapsedTime(stage_ms + 1, ev.e[1], ev.e[2]));
-    }
-#undef SYS_TRY
-    g->terms_nd = nd;
-    *out = a;
+    tpsa_pattern_kernel<ND><<<fg_grid(nc), 256, 0, g->stream>>>(nc, g->cc_ptr.as<int32_t>(), g->cc_ix.as<int32_t>(),
+                                                                 P.ip.as<int32_t>(), P.ix.as<int32_t>());
     return PB_OK;
-}
-
-extern "C" int pb_tpsa_rhs(pb_facegrid *g, const double *bc_values, const double *body_force,
-                           const double *angular_source, const double *mass_source, double *rhs_dev) {
-    if (!g || !bc_values || !rhs_dev) return pb_fail_(PB_EINVAL, "null pointer");
-    const int nd = g->terms_nd;
-    if (nd != 2 && nd != 3) return pb_fail_(PB_EINVAL, "pb_tpsa_system has not been called");
-    const int64_t nf = g->nf, nc = g->nc;
-    const int nr = nd == 3 ? 3 : 1;
-    cudaStream_t st = g->stream;
-    DevBuf dg, df, dsr, dsp;
-    CUDA_TRY(dg.upload(bc_values, (size_t)nd * nf, st));
-    if (body_force) CUDA_TRY(df.upload(body_force, (size_t)nd * nc, st));
-    if (angular_source) CUDA_TRY(dsr.upload(angular_source, (size_t)nr * nc, st));
-    if (mass_source) CUDA_TRY(dsp.upload(mass_source, (size_t)nc, st));
-    TpsaTerms T{};
-    for (int k = PB_TPSA_BOUND_STRESS; k <= PB_TPSA_BOUND_MASS_DISPLACEMENT; ++k) T.t[k] = g->terms[k].as<double>();
-    const TpsaTopo t = tpsa_topo(g);
-    const int64_t rows = nc * (nd + nr + 1);
-    const double *pf = body_force ? df.as<double>() : nullptr, *psr = angular_source ? dsr.as<double>() : nullptr,
-                 *psp = mass_source ? dsp.as<double>() : nullptr;
-    if (nd == 3) tpsa_rhs_kernel<3><<<fg_grid(rows), 256, 0, st>>>(t, T, dg.as<double>(), pf, psr, psp, rhs_dev);
-    else tpsa_rhs_kernel<2><<<fg_grid(rows), 256, 0, st>>>(t, T, dg.as<double>(), pf, psr, psp, rhs_dev);
-    pb_count_launch_();
-    CUDA_TRY(cudaGetLastError());
-    CUDA_TRY(cudaStreamSynchronize(st));
-    return PB_OK;
-}
-
-// ---- TPSA poromechanics system (tpsa_system.cuh, four fields) ---------------------------------------------------
-struct CsrView { int64_t nrows, ncols, nnz; int32_t *indptr, *indices; double *data; };
-CsrView pb_csr_view_(const pb_csr *a);   // spmv.cu
-
-__global__ void tpsa_nb_list_kernel(TpsaTopo t, const int32_t *__restrict__ cc_ptr, int32_t *__restrict__ cc_ix,
-                                    int32_t *__restrict__ cc_cell) {
-    for (int64_t c = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; c < t.nc; c += (int64_t)gridDim.x * blockDim.x) {
-        int32_t nb[kTpsaMaxNb];
-        const int n = tpsa_cell_neighbours(c, t, nb);
-        for (int j = 0; j < n; ++j) { cc_ix[cc_ptr[c] + j] = nb[j]; cc_cell[cc_ptr[c] + j] = (int32_t)c; }
-    }
 }
 
 template <int ND, int NS>
@@ -655,6 +555,204 @@ __global__ void tpsa_poro_pattern_kernel(int64_t nc, const int32_t *__restrict__
         tpsa_poro_pattern_rows<ND, NS>(c, cc_ptr[c + 1] - cc_ptr[c], cc_ix + cc_ptr[c], blk_ptr[c], fp_ip, fp_ix, ip, ix);
 }
 
+// Row pattern of the system with NS scalar balances on the flux pattern fp (nc x nc, sorted rows).
+template <int ND, int NS>
+static int tpsa_poro_pattern(pb_facegrid *g, const CsrView &fp) {
+    const int64_t nc = g->nc;
+    const int32_t *cc_ptr = g->cc_ptr.as<int32_t>();
+    TpsaPattern &P = g->poro;
+    int64_t nnz = 0;
+    int rc = tpsa_block_offsets(g, P, &nnz, [&](int32_t *count) {
+        tpsa_poro_count_kernel<ND, NS><<<fg_grid(nc), 256, 0, g->stream>>>(nc, cc_ptr, fp.indptr, fp.indices, count);
+    });
+    if (rc || (rc = tpsa_pattern_alloc(g, P, nc * TpsaPoroDims<ND, NS>::B, nnz))) return rc;
+    tpsa_poro_pattern_kernel<ND, NS><<<fg_grid(nc), 256, 0, g->stream>>>(nc, cc_ptr, g->cc_ix.as<int32_t>(),
+                                                                          P.blk.as<int64_t>(), fp.indptr, fp.indices,
+                                                                          P.ip.as<int32_t>(), P.ix.as<int32_t>());
+    return PB_OK;
+}
+
+template <int ND>
+__global__ void tpsa_contact_count_kernel(TpsaTopo t, const int32_t *__restrict__ cc_ptr,
+                                          const int32_t *__restrict__ face_mortar, int32_t *__restrict__ count) {
+    using D = TpsaContactDims<ND>;
+    for (int64_t c = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; c < t.nc; c += (int64_t)gridDim.x * blockDim.x)
+        count[c] = D::M::NZ * (cc_ptr[c + 1] - cc_ptr[c]) + D::EXT * tpsa_contact_nfrac(c, t, face_mortar);
+}
+
+template <int ND>
+__global__ void tpsa_contact_pattern_kernel(TpsaTopo t, const int32_t *__restrict__ cc_ptr,
+                                            const int32_t *__restrict__ cc_ix, const int64_t *__restrict__ blk_ptr,
+                                            TpsaMortars I, int32_t *__restrict__ ip, int32_t *__restrict__ ix) {
+    for (int64_t c = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; c < t.nc; c += (int64_t)gridDim.x * blockDim.x)
+        tpsa_contact_pattern_rows<ND>(c, cc_ptr[c + 1] - cc_ptr[c], cc_ix + cc_ptr[c], blk_ptr[c], t, I, ip, ix);
+}
+
+// one thread per interface row (force and contact rows)
+template <int ND>
+__global__ void tpsa_contact_iface_pattern_kernel(TpsaTopo t, const int64_t *__restrict__ blk_ptr, TpsaMortars I,
+                                                  int32_t *__restrict__ ip, int32_t *__restrict__ ix) {
+    const int64_t n = (int64_t)ND * (I.nm + I.nk);
+    for (int64_t q = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; q < n; q += (int64_t)gridDim.x * blockDim.x)
+        tpsa_contact_iface_pattern<ND>(q, t.nc, blk_ptr[t.nc], t, I, ip, ix);
+}
+
+// Row pattern of the contact system, from the interface topology already on the handle: the block rows, then ND nm
+// force rows of LF entries and ND nk contact rows of LC entries.
+template <int ND>
+static int tpsa_contact_pattern(pb_facegrid *g) {
+    using D = TpsaContactDims<ND>;
+    const int64_t nc = g->nc, ni = (int64_t)ND * (g->ctc_nm + g->ctc_nk);
+    const int32_t *cc_ptr = g->cc_ptr.as<int32_t>();
+    const TpsaTopo t = tpsa_topo(g);
+    const TpsaMortars I = tpsa_mortars(g);
+    TpsaPattern &P = g->ctc;
+    int64_t ncell = 0;
+    int rc = tpsa_block_offsets(g, P, &ncell, [&](int32_t *count) {
+        tpsa_contact_count_kernel<ND><<<fg_grid(nc), 256, 0, g->stream>>>(t, cc_ptr, I.face_mortar, count);
+    });
+    const int64_t nnz = ncell + (int64_t)ND * I.nm * D::LF + (int64_t)ND * I.nk * D::LC;
+    if (rc || (rc = tpsa_pattern_alloc(g, P, nc * D::B + ni, nnz))) return rc;
+    tpsa_contact_pattern_kernel<ND><<<fg_grid(nc), 256, 0, g->stream>>>(t, cc_ptr, g->cc_ix.as<int32_t>(),
+                                                                         P.blk.as<int64_t>(), I, P.ip.as<int32_t>(),
+                                                                         P.ix.as<int32_t>());
+    if (ni) tpsa_contact_iface_pattern_kernel<ND><<<fg_grid(ni), 256, 0, g->stream>>>(t, P.blk.as<int64_t>(), I,
+                                                                                      P.ip.as<int32_t>(), P.ix.as<int32_t>());
+    return PB_OK;
+}
+
+// ---- assembly ------------------------------------------------------------------------------------------------------
+// A TPSA system on the pattern P (nrows x nrows), in two stages: the face terms (tpsa_face_terms), then
+// launch(ND, T, values of A), which gathers the blocks of A from them.  stage_ms (optional): the two stage times in ms.
+// A is destroyed on every error.
+template <class Launch>
+static int tpsa_assemble(pb_facegrid *g, int nd, const TpsaInputs &in, const TpsaPattern &P, int64_t nrows,
+                         pb_csr **out, float *stage_ms, Launch &&launch) {
+    pb_csr *a = nullptr;
+    int rc = pb_csr_from_device_pattern_(nrows, nrows, P.nnz, P.ip.as<int32_t>(), P.ix.as<int32_t>(), &a);
+    if (rc) return rc;
+    cudaStream_t st = g->stream;
+    FgEvents ev;
+    auto stages = [&]() -> int {
+        if (stage_ms) {
+            for (auto &x : ev.e) CUDA_TRY(cudaEventCreate(&x));
+            CUDA_TRY(cudaEventRecord(ev.e[0], st));
+        }
+        TpsaTerms T{};
+        const int rt = tpsa_face_terms(g, nd, in, T);
+        if (rt) return rt;
+        if (stage_ms) CUDA_TRY(cudaEventRecord(ev.e[1], st));
+        tpsa_nd(nd, [&](auto ND) { launch(ND, T, pb_csr_data_(a)); });
+        pb_count_launch_();
+        CUDA_TRY(cudaGetLastError());
+        if (stage_ms) CUDA_TRY(cudaEventRecord(ev.e[2], st));
+        CUDA_TRY(cudaStreamSynchronize(st));
+        if (stage_ms) {
+            CUDA_TRY(cudaEventElapsedTime(stage_ms, ev.e[0], ev.e[1]));
+            CUDA_TRY(cudaEventElapsedTime(stage_ms + 1, ev.e[1], ev.e[2]));
+        }
+        return PB_OK;
+    };
+    if ((rc = stages())) {
+        pb_csr_destroy(a);
+        return rc;
+    }
+    g->terms_nd = nd;
+    *out = a;
+    return PB_OK;
+}
+
+// one thread per row of b: the mechanics rows of every cell, its NS scalar rows (0: they are written at every
+// linearization), then the ND (nm + nk) interface rows of the contact system (none for the others: I.nm = I.nk = 0)
+template <int ND, int NS>
+__global__ void tpsa_rhs_kernel(TpsaTopo t, TpsaMortars I, TpsaTerms T, const double *__restrict__ g,
+                                const double *__restrict__ f, const double *__restrict__ sr,
+                                const double *__restrict__ sp, double *__restrict__ b) {
+    constexpr int NR = TpsaDims<ND>::NR, B = TpsaDims<ND>::B + NS;
+    const int64_t ncell = t.nc * B, n = ncell + (int64_t)ND * (I.nm + I.nk);
+    for (int64_t q = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; q < n; q += (int64_t)gridDim.x * blockDim.x) {
+        if (q >= ncell) { b[q] = tpsa_contact_iface_rhs<ND>(q - ncell, t, I, T, g); continue; }
+        const int64_t c = q / B;
+        const int l = (int)(q - c * B);
+        if (l > ND + NR) { b[q] = 0.0; continue; }
+        const double src = l < ND ? (f ? f[c * ND + l] : 0.0)
+                                   : (l < ND + NR ? (sr ? sr[c * NR + l - ND] : 0.0) : (sp ? sp[c] : 0.0));
+        b[q] = tpsa_rhs_row<ND>(c, l, t, T, g, src);
+    }
+}
+
+// b of the last assembly on the handle (dimension nd, NS scalar balances, with the interface rows when contact): the
+// boundary values and the optional sources uploaded, the boundary terms read from the handle.
+template <int NS>
+static int tpsa_rhs(pb_facegrid *g, int nd, bool contact, const double *bc_values, const double *body_force,
+                    const double *angular_source, const double *mass_source, double *rhs_dev) {
+    const int64_t nf = g->nf, nc = g->nc;
+    const int nr = nd == 3 ? 3 : 1;
+    cudaStream_t st = g->stream;
+    DevBuf dg, df, dsr, dsp;
+    CUDA_TRY(dg.upload(bc_values, (size_t)nd * nf, st));
+    if (body_force) CUDA_TRY(df.upload(body_force, (size_t)nd * nc, st));
+    if (angular_source) CUDA_TRY(dsr.upload(angular_source, (size_t)nr * nc, st));
+    if (mass_source) CUDA_TRY(dsp.upload(mass_source, (size_t)nc, st));
+    TpsaTerms T{};
+    for (int k = PB_TPSA_BOUND_STRESS; k <= PB_TPSA_BOUND_MASS_DISPLACEMENT; ++k) T.t[k] = g->terms[k].as<double>();
+    const TpsaTopo t = tpsa_topo(g);
+    const TpsaMortars I = contact ? tpsa_mortars(g) : TpsaMortars{};
+    const int64_t rows = nc * (nd + nr + 1 + NS) + (int64_t)nd * (I.nm + I.nk);
+    const double *pf = body_force ? df.as<double>() : nullptr, *psr = angular_source ? dsr.as<double>() : nullptr,
+                 *psp = mass_source ? dsp.as<double>() : nullptr;
+    tpsa_nd(nd, [&](auto ND) {
+        tpsa_rhs_kernel<ND, NS><<<fg_grid(rows), 256, 0, st>>>(t, I, T, dg.as<double>(), pf, psr, psp, rhs_dev);
+    });
+    pb_count_launch_();
+    CUDA_TRY(cudaGetLastError());
+    CUDA_TRY(cudaStreamSynchronize(st));
+    return PB_OK;
+}
+
+// ---- TPSA three-field system ---------------------------------------------------------------------------------------
+// one thread per block (c, k) of A, i.e. per entry of the neighbour lists: consecutive threads write consecutive
+// segments of the same rows
+template <int ND>
+__global__ void tpsa_system_kernel(int64_t npairs, TpsaTopo t, const int32_t *__restrict__ cc_ptr,
+                                   const int32_t *__restrict__ cc_ix, const int32_t *__restrict__ cc_cell, TpsaTerms T,
+                                   const double *__restrict__ mu, const double *__restrict__ lam,
+                                   const double *__restrict__ vol, double *__restrict__ a) {
+    for (int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; e < npairs; e += (int64_t)gridDim.x * blockDim.x) {
+        const int64_t c = cc_cell[e];
+        tpsa_system_block<ND>(c, (int)(e - cc_ptr[c]), t, cc_ptr, cc_ix, T, mu, lam, vol, a);
+    }
+}
+
+extern "C" int pb_tpsa_system(pb_facegrid *g, int nd, const double *mu, const double *lambda,
+                              const double *cell_volumes, const uint8_t *codes, const double *robin_diag,
+                              const uint8_t *face_flags, pb_csr **out, float *stage_ms) {
+    if (!g || !mu || !lambda || !cell_volumes || !codes || !face_flags || !out)
+        return pb_fail_(PB_EINVAL, "null pointer");
+    TpsaInputs in;
+    int rc = tpsa_prepare(g, nd, mu, lambda, cell_volumes, codes, robin_diag, face_flags, nullptr, in);
+    if (rc) return rc;
+    rc = tpsa_pattern(g, g->sys, {nd, 0, 0}, [&](auto ND) { return tpsa_sys_pattern<ND>(g); });
+    if (rc) return rc;
+    const TpsaTopo t = tpsa_topo(g);
+    const int64_t np = g->npairs;
+    return tpsa_assemble(g, nd, in, g->sys, g->nc * (nd == 3 ? 7 : 4), out, stage_ms,
+                         [&](auto ND, const TpsaTerms &T, double *a) {
+        tpsa_system_kernel<ND><<<fg_grid(np), 256, 0, g->stream>>>(np, t, g->cc_ptr.as<int32_t>(), g->cc_ix.as<int32_t>(),
+                                                                    g->cc_cell.as<int32_t>(), T, in.mu.as<double>(),
+                                                                    in.lam.as<double>(), in.vol.as<double>(), a);
+    });
+}
+
+extern "C" int pb_tpsa_rhs(pb_facegrid *g, const double *bc_values, const double *body_force,
+                           const double *angular_source, const double *mass_source, double *rhs_dev) {
+    if (!g || !bc_values || !rhs_dev) return pb_fail_(PB_EINVAL, "null pointer");
+    const int nd = g->terms_nd;
+    if (nd != 2 && nd != 3) return pb_fail_(PB_EINVAL, "pb_tpsa_system has not been called");
+    return tpsa_rhs<0>(g, nd, false, bc_values, body_force, angular_source, mass_source, rhs_dev);
+}
+
+// ---- TPSA poromechanics (NS = 1) and thermo-poromechanics (NS = 2) systems -----------------------------------------
 // one thread per block (c, k), as tpsa_system_kernel
 template <int ND, int NS>
 __global__ void tpsa_poro_system_kernel(int64_t npairs, TpsaTopo t, const int32_t *__restrict__ cc_ptr,
@@ -665,21 +763,6 @@ __global__ void tpsa_poro_system_kernel(int64_t npairs, TpsaTopo t, const int32_
     for (int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; e < npairs; e += (int64_t)gridDim.x * blockDim.x) {
         const int64_t c = cc_cell[e];
         tpsa_poro_block<ND, NS>(c, (int)(e - cc_ptr[c]), t, cc_ptr, cc_ix, blk_ptr, T, mu, lam, alpha, vol, a);
-    }
-}
-
-template <int ND, int NS>
-__global__ void tpsa_poro_rhs_kernel(TpsaTopo t, TpsaTerms T, const double *__restrict__ g, const double *__restrict__ f,
-                                     const double *__restrict__ sr, const double *__restrict__ sp,
-                                     double *__restrict__ b) {
-    constexpr int NR = TpsaDims<ND>::NR, B = TpsaPoroDims<ND, NS>::B;
-    for (int64_t q = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; q < t.nc * B; q += (int64_t)gridDim.x * blockDim.x) {
-        const int64_t c = q / B;
-        const int l = (int)(q - c * B);
-        if (l > ND + NR) { b[q] = 0.0; continue; }   // the scalar rows are written at every linearization
-        const double src = l < ND ? (f ? f[c * ND + l] : 0.0)
-                                   : (l < ND + NR ? (sr ? sr[c * NR + l - ND] : 0.0) : (sp ? sp[c] : 0.0));
-        b[q] = tpsa_rhs_row<ND>(c, l, t, T, g, src);
     }
 }
 
@@ -711,57 +794,6 @@ struct TpsaPoroNames<2> {
                                 *jac = "balance Jacobian must be 2 num_cells x 3 num_cells ([p_t | p | T])";
 };
 
-// Row pattern of the system for dimension nd, NS scalar balances and the flux pattern fp (nc x nc, sorted rows).
-template <int NS>
-static int tpsa_poro_build_pattern(pb_facegrid *g, int nd, const CsrView &fp) {
-    cudaStream_t st = g->stream;
-    const int64_t nc = g->nc;
-    const int B = (nd == 3 ? 7 : 4) + NS;
-    const TpsaTopo t = tpsa_topo(g);
-    if (!g->nb_ready) {
-        int64_t total = 0;
-        int rc = tpsa_neighbour_counts(g, &total);
-        if (rc) return rc;
-        tpsa_nb_list_kernel<<<fg_grid(nc), 256, 0, st>>>(t, g->cc_ptr.as<int32_t>(), g->cc_ix.as<int32_t>(),
-                                                          g->cc_cell.as<int32_t>());
-        pb_count_launch_();
-        CUDA_TRY(cudaGetLastError());
-        g->sys_npairs = total;
-        g->nb_ready = true;
-    }
-    DevBuf count;
-    CUDA_TRY(count.ensure((size_t)nc * sizeof(int32_t)));
-    if (nd == 3) tpsa_poro_count_kernel<3, NS><<<fg_grid(nc), 256, 0, st>>>(nc, g->cc_ptr.as<int32_t>(), fp.indptr, fp.indices, count.as<int32_t>());
-    else tpsa_poro_count_kernel<2, NS><<<fg_grid(nc), 256, 0, st>>>(nc, g->cc_ptr.as<int32_t>(), fp.indptr, fp.indices, count.as<int32_t>());
-    pb_count_launch_();
-    CUDA_TRY(cudaGetLastError());
-    CUDA_TRY(g->blk_ptr.ensure((size_t)(nc + 1) * sizeof(int64_t)));
-    int64_t nnz = 0;
-    const int rc = pb_scan_offsets_(count.as<int32_t>(), g->blk_ptr.as<int64_t>(), nc, st, &nnz);
-    if (rc) return rc;
-    if (nnz >= 0x7FFFFFFFll) return pb_fail_(PB_ENOTIMPL, "Tpsa system: the matrix does not fit int32 indices");
-    CUDA_TRY(g->poro_ip.ensure((size_t)(nc * B + 1) * sizeof(int32_t)));
-    CUDA_TRY(g->poro_ix.ensure((size_t)std::max<int64_t>(1, nnz) * sizeof(int32_t)));
-    const int32_t last = (int32_t)nnz;
-    CUDA_TRY(cudaMemcpyAsync(g->poro_ip.as<int32_t>() + nc * B, &last, sizeof(int32_t), cudaMemcpyHostToDevice, st));
-    if (nd == 3)
-        tpsa_poro_pattern_kernel<3, NS><<<fg_grid(nc), 256, 0, st>>>(nc, g->cc_ptr.as<int32_t>(), g->cc_ix.as<int32_t>(),
-                                                                      g->blk_ptr.as<int64_t>(), fp.indptr, fp.indices,
-                                                                      g->poro_ip.as<int32_t>(), g->poro_ix.as<int32_t>());
-    else
-        tpsa_poro_pattern_kernel<2, NS><<<fg_grid(nc), 256, 0, st>>>(nc, g->cc_ptr.as<int32_t>(), g->cc_ix.as<int32_t>(),
-                                                                      g->blk_ptr.as<int64_t>(), fp.indptr, fp.indices,
-                                                                      g->poro_ip.as<int32_t>(), g->poro_ix.as<int32_t>());
-    pb_count_launch_();
-    CUDA_TRY(cudaGetLastError());
-    CUDA_TRY(cudaStreamSynchronize(st));
-    g->poro_nd = nd;
-    g->poro_ns = NS;
-    g->poro_nnz = nnz;
-    g->poro_fp_nnz = fp.nnz;
-    return PB_OK;
-}
-
 template <int NS>
 static int tpsa_poro_system(pb_facegrid *g, int nd, const double *mu, const double *lambda, const double *alpha,
                             const double *cell_volumes, const uint8_t *codes, const double *robin_diag,
@@ -774,109 +806,51 @@ static int tpsa_poro_system(pb_facegrid *g, int nd, const double *mu, const doub
     const CsrView fp = pb_csr_view_(flux_pattern);
     if (fp.nrows != nc || fp.ncols != nc) return pb_fail_(PB_EINVAL, "flux pattern must be num_cells x num_cells");
     TpsaInputs in;
-    int rc = tpsa_prepare(g, nd, mu, lambda, cell_volumes, codes, robin_diag, face_flags, in);
+    int rc = tpsa_prepare(g, nd, mu, lambda, cell_volumes, codes, robin_diag, face_flags, nullptr, in);
     if (rc) return rc;
-    if (g->poro_nd != nd || g->poro_ns != NS || g->poro_fp_nnz != fp.nnz) {
-        g->poro_nd = 0;
-        if ((rc = tpsa_poro_build_pattern<NS>(g, nd, fp))) return rc;
-    }
-    cudaStream_t st = g->stream;
-    const int B = (nd == 3 ? 7 : 4) + NS;
+    rc = tpsa_pattern(g, g->poro, {nd, NS, fp.nnz}, [&](auto ND) { return tpsa_poro_pattern<ND, NS>(g, fp); });
+    if (rc) return rc;
     DevBuf dal;
-    CUDA_TRY(dal.upload(alpha, (size_t)nc, st));
-    pb_csr *a = nullptr;
-    rc = pb_csr_from_device_pattern_(nc * B, nc * B, g->poro_nnz, g->poro_ip.as<int32_t>(), g->poro_ix.as<int32_t>(), &a);
-    if (rc) return rc;
-    FgEvents ev;
-    auto fail_cuda = [&](cudaError_t e, const char *what) {
-        pb_csr_destroy(a);
-        return pb_fail_(PB_ECUDA, std::string(what) + ": " + cudaGetErrorString(e));
-    };
-#define SYS_TRY(x) do { cudaError_t e_ = (x); if (e_ != cudaSuccess) return fail_cuda(e_, #x); } while (0)
-    if (stage_ms)
-        for (auto &x : ev.e) SYS_TRY(cudaEventCreate(&x));
-    if (stage_ms) SYS_TRY(cudaEventRecord(ev.e[0], st));
-    TpsaTerms T{};
-    if ((rc = tpsa_face_terms(g, nd, in, T))) { pb_csr_destroy(a); return rc; }
-    if (stage_ms) SYS_TRY(cudaEventRecord(ev.e[1], st));
+    CUDA_TRY(dal.upload(alpha, (size_t)nc, g->stream));
     const TpsaTopo t = tpsa_topo(g);
-    const int64_t np = g->sys_npairs;
-    if (nd == 3)
-        tpsa_poro_system_kernel<3, NS><<<fg_grid(np), 256, 0, st>>>(np, t, g->cc_ptr.as<int32_t>(), g->cc_ix.as<int32_t>(),
-                                                                     g->cc_cell.as<int32_t>(), g->blk_ptr.as<int64_t>(), T,
-                                                                     in.mu.as<double>(), in.lam.as<double>(),
-                                                                     dal.as<double>(), in.vol.as<double>(), pb_csr_data_(a));
-    else
-        tpsa_poro_system_kernel<2, NS><<<fg_grid(np), 256, 0, st>>>(np, t, g->cc_ptr.as<int32_t>(), g->cc_ix.as<int32_t>(),
-                                                                     g->cc_cell.as<int32_t>(), g->blk_ptr.as<int64_t>(), T,
-                                                                     in.mu.as<double>(), in.lam.as<double>(),
-                                                                     dal.as<double>(), in.vol.as<double>(), pb_csr_data_(a));
-    pb_count_launch_();
-    SYS_TRY(cudaGetLastError());
-    if (stage_ms) SYS_TRY(cudaEventRecord(ev.e[2], st));
-    SYS_TRY(cudaStreamSynchronize(st));
-    if (stage_ms) {
-        SYS_TRY(cudaEventElapsedTime(stage_ms, ev.e[0], ev.e[1]));
-        SYS_TRY(cudaEventElapsedTime(stage_ms + 1, ev.e[1], ev.e[2]));
-    }
-#undef SYS_TRY
-    g->terms_nd = nd;
-    *out = a;
-    return PB_OK;
+    const int64_t np = g->npairs;
+    return tpsa_assemble(g, nd, in, g->poro, nc * ((nd == 3 ? 7 : 4) + NS), out, stage_ms,
+                         [&](auto ND, const TpsaTerms &T, double *a) {
+        tpsa_poro_system_kernel<ND, NS><<<fg_grid(np), 256, 0, g->stream>>>(
+            np, t, g->cc_ptr.as<int32_t>(), g->cc_ix.as<int32_t>(), g->cc_cell.as<int32_t>(), g->poro.blk.as<int64_t>(), T,
+            in.mu.as<double>(), in.lam.as<double>(), dal.as<double>(), in.vol.as<double>(), a);
+    });
 }
 
 template <int NS>
 static int tpsa_poro_rhs(pb_facegrid *g, const double *bc_values, const double *body_force,
                          const double *angular_source, const double *mass_source, double *rhs_dev) {
     if (!g || !bc_values || !rhs_dev) return pb_fail_(PB_EINVAL, "null pointer");
-    const int nd = g->poro_nd;
-    if ((nd != 2 && nd != 3) || g->poro_ns != NS || g->terms_nd != nd)
+    const int nd = (int)g->poro.key[0];
+    if ((nd != 2 && nd != 3) || g->poro.key[1] != NS || g->terms_nd != nd)
         return pb_fail_(PB_EINVAL, std::string(TpsaPoroNames<NS>::system) + " has not been called");
-    const int64_t nf = g->nf, nc = g->nc;
-    const int nr = nd == 3 ? 3 : 1;
-    cudaStream_t st = g->stream;
-    DevBuf dg, df, dsr, dsp;
-    CUDA_TRY(dg.upload(bc_values, (size_t)nd * nf, st));
-    if (body_force) CUDA_TRY(df.upload(body_force, (size_t)nd * nc, st));
-    if (angular_source) CUDA_TRY(dsr.upload(angular_source, (size_t)nr * nc, st));
-    if (mass_source) CUDA_TRY(dsp.upload(mass_source, (size_t)nc, st));
-    TpsaTerms T{};
-    for (int k = PB_TPSA_BOUND_STRESS; k <= PB_TPSA_BOUND_MASS_DISPLACEMENT; ++k) T.t[k] = g->terms[k].as<double>();
-    const TpsaTopo t = tpsa_topo(g);
-    const int64_t rows = nc * (nd + nr + 1 + NS);
-    const double *pf = body_force ? df.as<double>() : nullptr, *psr = angular_source ? dsr.as<double>() : nullptr,
-                 *psp = mass_source ? dsp.as<double>() : nullptr;
-    if (nd == 3) tpsa_poro_rhs_kernel<3, NS><<<fg_grid(rows), 256, 0, st>>>(t, T, dg.as<double>(), pf, psr, psp, rhs_dev);
-    else tpsa_poro_rhs_kernel<2, NS><<<fg_grid(rows), 256, 0, st>>>(t, T, dg.as<double>(), pf, psr, psp, rhs_dev);
-    pb_count_launch_();
-    CUDA_TRY(cudaGetLastError());
-    CUDA_TRY(cudaStreamSynchronize(st));
-    return PB_OK;
+    return tpsa_rhs<NS>(g, nd, false, bc_values, body_force, angular_source, mass_source, rhs_dev);
 }
 
 template <int NS>
 static int tpsa_poro_fluid_rows(pb_facegrid *g, pb_csr *a, const pb_csr *jf, const double *neg_res_dev,
                                 double *rhs_dev, int *missing_dev, uint64_t stream) {
     if (!g || !a || !jf || !neg_res_dev || !rhs_dev) return pb_fail_(PB_EINVAL, "null pointer");
-    const int nd = g->poro_nd;
-    if ((nd != 2 && nd != 3) || g->poro_ns != NS)
+    const int nd = (int)g->poro.key[0];
+    if ((nd != 2 && nd != 3) || g->poro.key[1] != NS)
         return pb_fail_(PB_EINVAL, std::string(TpsaPoroNames<NS>::system) + " has not been called");
     const int64_t nc = g->nc;
     const int B = (nd == 3 ? 7 : 4) + NS;
     const CsrView va = pb_csr_view_(a), vj = pb_csr_view_(jf);
-    if (va.nrows != nc * B || va.ncols != nc * B || va.nnz != g->poro_nnz)
+    if (va.nrows != nc * B || va.ncols != nc * B || va.nnz != g->poro.nnz)
         return pb_fail_(PB_EINVAL, std::string("the matrix is not the ") + TpsaPoroNames<NS>::model +
                                        " system of this grid");
     if (vj.nrows != NS * nc || vj.ncols != (1 + NS) * nc) return pb_fail_(PB_EINVAL, TpsaPoroNames<NS>::jac);
-    cudaStream_t st = (cudaStream_t)stream;
-    if (nd == 3)
-        tpsa_poro_fluid_kernel<3, NS><<<fg_grid(nc), 256, 0, st>>>(nc, g->cc_ptr.as<int32_t>(), g->blk_ptr.as<int64_t>(),
-                                                                    va.indices, vj.indptr, vj.indices, vj.data, neg_res_dev,
-                                                                    va.data, rhs_dev, missing_dev);
-    else
-        tpsa_poro_fluid_kernel<2, NS><<<fg_grid(nc), 256, 0, st>>>(nc, g->cc_ptr.as<int32_t>(), g->blk_ptr.as<int64_t>(),
-                                                                    va.indices, vj.indptr, vj.indices, vj.data, neg_res_dev,
-                                                                    va.data, rhs_dev, missing_dev);
+    tpsa_nd(nd, [&](auto ND) {
+        tpsa_poro_fluid_kernel<ND, NS><<<fg_grid(nc), 256, 0, (cudaStream_t)stream>>>(
+            nc, g->cc_ptr.as<int32_t>(), g->poro.blk.as<int64_t>(), va.indices, vj.indptr, vj.indices, vj.data,
+            neg_res_dev, va.data, rhs_dev, missing_dev);
+    });
     pb_count_launch_();
     CUDA_TRY(cudaGetLastError());
     return PB_OK;
@@ -913,32 +887,7 @@ extern "C" int pb_tpsa_thm_balance_rows(pb_facegrid *g, pb_csr *a, const pb_csr 
     return tpsa_poro_fluid_rows<2>(g, a, jf, neg_res_dev, rhs_dev, missing_dev, stream);
 }
 
-// ---- TPSA elasticity with fractures in frictional contact (tpsa_system.cuh) ---------------------------------------
-template <int ND>
-__global__ void tpsa_contact_count_kernel(TpsaTopo t, const int32_t *__restrict__ cc_ptr,
-                                          const int32_t *__restrict__ face_mortar, int32_t *__restrict__ count) {
-    using D = TpsaContactDims<ND>;
-    for (int64_t c = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; c < t.nc; c += (int64_t)gridDim.x * blockDim.x)
-        count[c] = D::M::NZ * (cc_ptr[c + 1] - cc_ptr[c]) + D::EXT * tpsa_contact_nfrac(c, t, face_mortar);
-}
-
-template <int ND>
-__global__ void tpsa_contact_pattern_kernel(TpsaTopo t, const int32_t *__restrict__ cc_ptr,
-                                            const int32_t *__restrict__ cc_ix, const int64_t *__restrict__ blk_ptr,
-                                            TpsaMortars I, int32_t *__restrict__ ip, int32_t *__restrict__ ix) {
-    for (int64_t c = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; c < t.nc; c += (int64_t)gridDim.x * blockDim.x)
-        tpsa_contact_pattern_rows<ND>(c, cc_ptr[c + 1] - cc_ptr[c], cc_ix + cc_ptr[c], blk_ptr[c], t, I, ip, ix);
-}
-
-// one thread per interface row (force and contact rows)
-template <int ND>
-__global__ void tpsa_contact_iface_pattern_kernel(TpsaTopo t, const int64_t *__restrict__ blk_ptr, TpsaMortars I,
-                                                  int32_t *__restrict__ ip, int32_t *__restrict__ ix) {
-    const int64_t n = (int64_t)ND * (I.nm + I.nk);
-    for (int64_t q = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; q < n; q += (int64_t)gridDim.x * blockDim.x)
-        tpsa_contact_iface_pattern<ND>(q, t.nc, blk_ptr[t.nc], t, I, ip, ix);
-}
-
+// ---- TPSA elasticity with fractures in frictional contact ----------------------------------------------------------
 // one thread per block (c, k), as tpsa_system_kernel
 template <int ND>
 __global__ void tpsa_contact_block_kernel(int64_t npairs, TpsaTopo t, const int32_t *__restrict__ cc_ptr,
@@ -960,22 +909,6 @@ __global__ void tpsa_contact_iface_kernel(TpsaTopo t, const int64_t *__restrict_
         tpsa_contact_iface_row<ND>(q, blk_ptr[t.nc], t, I, T, a);
 }
 
-template <int ND>
-__global__ void tpsa_contact_rhs_kernel(TpsaTopo t, TpsaMortars I, TpsaTerms T, const double *__restrict__ g,
-                                        const double *__restrict__ f, const double *__restrict__ sr,
-                                        const double *__restrict__ sp, double *__restrict__ b) {
-    constexpr int NR = TpsaDims<ND>::NR, B = TpsaDims<ND>::B;
-    const int64_t n = t.nc * B + (int64_t)ND * (I.nm + I.nk);
-    for (int64_t q = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; q < n; q += (int64_t)gridDim.x * blockDim.x) {
-        if (q >= t.nc * B) { b[q] = tpsa_contact_iface_rhs<ND>(q - t.nc * B, t, I, T, g); continue; }
-        const int64_t c = q / B;
-        const int l = (int)(q - c * B);
-        const double src = l < ND ? (f ? f[c * ND + l] : 0.0)
-                                   : (l < ND + NR ? (sr ? sr[c * NR + l - ND] : 0.0) : (sp ? sp[c] : 0.0));
-        b[q] = tpsa_rhs_row<ND>(c, l, t, T, g, src);
-    }
-}
-
 // one thread per contact row
 template <int ND>
 __global__ void tpsa_contact_law_kernel(int64_t nrows, int64_t c0, int64_t row0, int64_t e0,
@@ -987,72 +920,6 @@ __global__ void tpsa_contact_law_kernel(int64_t nrows, int64_t c0, int64_t row0,
         const int m = tpsa_contact_law_row<ND>(r, c0, e0, row0 + r, ix, jc_ip, jc_ix, jc_a, neg_res, a, b);
         if (m && missing) atomicAdd(missing, m);
     }
-}
-
-static TpsaMortars tpsa_mortars(pb_facegrid *g) {
-    const int64_t nm = g->ctc_nm;
-    const double *w = g->ctc_w.as<double>();
-    return TpsaMortars{nm, g->ctc_nk, g->ctc_face.as<int32_t>(), g->ctc_cell.as<int32_t>(), g->ctc_fm.as<int32_t>(),
-                       g->ctc_pair.as<int32_t>(), w, w + nm, w + 2 * nm, w + 3 * nm, g->ctc_frame.as<double>(), g->ctc_ct};
-}
-
-// Row pattern of the contact system: neighbour lists (shared with the other TPSA systems), block-row offsets and the
-// CSR arrays, from the interface topology already on the handle.
-static int tpsa_contact_build_pattern(pb_facegrid *g, int nd) {
-    cudaStream_t st = g->stream;
-    const int64_t nc = g->nc, nm = g->ctc_nm, nk = g->ctc_nk;
-    const int B = nd == 3 ? 7 : 4;
-    const TpsaTopo t = tpsa_topo(g);
-    if (!g->nb_ready) {
-        int64_t total = 0;
-        int rc = tpsa_neighbour_counts(g, &total);
-        if (rc) return rc;
-        tpsa_nb_list_kernel<<<fg_grid(nc), 256, 0, st>>>(t, g->cc_ptr.as<int32_t>(), g->cc_ix.as<int32_t>(),
-                                                          g->cc_cell.as<int32_t>());
-        pb_count_launch_();
-        CUDA_TRY(cudaGetLastError());
-        g->sys_npairs = total;
-        g->nb_ready = true;
-    }
-    const TpsaMortars I = tpsa_mortars(g);
-    DevBuf count;
-    CUDA_TRY(count.ensure((size_t)nc * sizeof(int32_t)));
-    if (nd == 3) tpsa_contact_count_kernel<3><<<fg_grid(nc), 256, 0, st>>>(t, g->cc_ptr.as<int32_t>(), I.face_mortar, count.as<int32_t>());
-    else tpsa_contact_count_kernel<2><<<fg_grid(nc), 256, 0, st>>>(t, g->cc_ptr.as<int32_t>(), I.face_mortar, count.as<int32_t>());
-    pb_count_launch_();
-    CUDA_TRY(cudaGetLastError());
-    CUDA_TRY(g->ctc_blk.ensure((size_t)(nc + 1) * sizeof(int64_t)));
-    int64_t ncell = 0;
-    const int rc = pb_scan_offsets_(count.as<int32_t>(), g->ctc_blk.as<int64_t>(), nc, st, &ncell);
-    if (rc) return rc;
-    const int64_t nr = nd == 3 ? 3 : 1, nnz = ncell + (int64_t)nd * nm * (nd + nr + 3) + (int64_t)nd * nk * 3 * nd;
-    if (nnz >= 0x7FFFFFFFll) return pb_fail_(PB_ENOTIMPL, "Tpsa system: the matrix does not fit int32 indices");
-    const int64_t nrows = nc * B + (int64_t)nd * (nm + nk);
-    CUDA_TRY(g->ctc_ip.ensure((size_t)(nrows + 1) * sizeof(int32_t)));
-    CUDA_TRY(g->ctc_ix.ensure((size_t)std::max<int64_t>(1, nnz) * sizeof(int32_t)));
-    const int32_t last = (int32_t)nnz;
-    CUDA_TRY(cudaMemcpyAsync(g->ctc_ip.as<int32_t>() + nrows, &last, sizeof(int32_t), cudaMemcpyHostToDevice, st));
-    const int64_t ni = (int64_t)nd * (nm + nk);
-    if (nd == 3) {
-        tpsa_contact_pattern_kernel<3><<<fg_grid(nc), 256, 0, st>>>(t, g->cc_ptr.as<int32_t>(), g->cc_ix.as<int32_t>(),
-                                                                     g->ctc_blk.as<int64_t>(), I, g->ctc_ip.as<int32_t>(),
-                                                                     g->ctc_ix.as<int32_t>());
-        if (ni) tpsa_contact_iface_pattern_kernel<3><<<fg_grid(ni), 256, 0, st>>>(t, g->ctc_blk.as<int64_t>(), I,
-                                                                              g->ctc_ip.as<int32_t>(), g->ctc_ix.as<int32_t>());
-    } else {
-        tpsa_contact_pattern_kernel<2><<<fg_grid(nc), 256, 0, st>>>(t, g->cc_ptr.as<int32_t>(), g->cc_ix.as<int32_t>(),
-                                                                     g->ctc_blk.as<int64_t>(), I, g->ctc_ip.as<int32_t>(),
-                                                                     g->ctc_ix.as<int32_t>());
-        if (ni) tpsa_contact_iface_pattern_kernel<2><<<fg_grid(ni), 256, 0, st>>>(t, g->ctc_blk.as<int64_t>(), I,
-                                                                              g->ctc_ip.as<int32_t>(), g->ctc_ix.as<int32_t>());
-    }
-    pb_count_launch_();
-    CUDA_TRY(cudaGetLastError());
-    CUDA_TRY(cudaStreamSynchronize(st));
-    g->ctc_nd = nd;
-    g->ctc_ncell = ncell;
-    g->ctc_nnz = nnz;
-    return PB_OK;
 }
 
 // Checks the interface description and puts it on the handle; *same: its topology is the one of the cached pattern.
@@ -1120,118 +987,58 @@ extern "C" int pb_tpsa_contact_system(pb_facegrid *g, int nd, const double *mu, 
     if (!g || !mu || !lambda || !cell_volumes || !codes || !face_flags || !out)
         return pb_fail_(PB_EINVAL, "null pointer");
     TpsaInputs in;
-    int rc = tpsa_prepare(g, nd, mu, lambda, cell_volumes, codes, robin_diag, face_flags, in);
+    int rc = tpsa_prepare(g, nd, mu, lambda, cell_volumes, codes, robin_diag, face_flags, nullptr, in);
     if (rc) return rc;
     bool same = false;
-    const bool had = g->ctc_nd == nd;
-    g->ctc_nd = 0;   // set again once the pattern on the handle belongs to the interfaces uploaded below
+    const TpsaKey key{nd, 0, 0}, had = g->ctc.key;
+    g->ctc.key = {};   // set again once the pattern on the handle belongs to the interfaces uploaded below
     rc = tpsa_contact_interfaces(g, nd, num_mortar, num_fracture_cells, mortar_face, mortar_cell, m2p_weight,
                                  p2m_weight, mortar_sign, mortar_volume, frames, characteristic_traction, &same);
     if (rc) return rc;
-    if (had && same) g->ctc_nd = nd;
-    else if ((rc = tpsa_contact_build_pattern(g, nd))) return rc;
-    cudaStream_t st = g->stream;
-    const int64_t nc = g->nc, nrows = nc * (nd == 3 ? 7 : 4) + (int64_t)nd * (g->ctc_nm + g->ctc_nk);
-    pb_csr *a = nullptr;
-    rc = pb_csr_from_device_pattern_(nrows, nrows, g->ctc_nnz, g->ctc_ip.as<int32_t>(), g->ctc_ix.as<int32_t>(), &a);
+    if (same) g->ctc.key = had;
+    rc = tpsa_pattern(g, g->ctc, key, [&](auto ND) { return tpsa_contact_pattern<ND>(g); });
     if (rc) return rc;
-    FgEvents ev;
-    auto fail_cuda = [&](cudaError_t e, const char *what) {
-        pb_csr_destroy(a);
-        return pb_fail_(PB_ECUDA, std::string(what) + ": " + cudaGetErrorString(e));
-    };
-#define SYS_TRY(x) do { cudaError_t e_ = (x); if (e_ != cudaSuccess) return fail_cuda(e_, #x); } while (0)
-    if (stage_ms)
-        for (auto &x : ev.e) SYS_TRY(cudaEventCreate(&x));
-    if (stage_ms) SYS_TRY(cudaEventRecord(ev.e[0], st));
-    TpsaTerms T{};
-    if ((rc = tpsa_face_terms(g, nd, in, T))) { pb_csr_destroy(a); return rc; }
-    if (stage_ms) SYS_TRY(cudaEventRecord(ev.e[1], st));
     const TpsaTopo t = tpsa_topo(g);
     const TpsaMortars I = tpsa_mortars(g);
-    const int64_t np = g->sys_npairs, ni = (int64_t)nd * (g->ctc_nm + g->ctc_nk);
-    double *av = pb_csr_data_(a);
-    if (nd == 3) {
-        tpsa_contact_block_kernel<3><<<fg_grid(np), 256, 0, st>>>(np, t, g->cc_ptr.as<int32_t>(), g->cc_ix.as<int32_t>(),
-                                                                   g->cc_cell.as<int32_t>(), g->ctc_blk.as<int64_t>(), I, T,
-                                                                   in.mu.as<double>(), in.lam.as<double>(),
-                                                                   in.vol.as<double>(), av);
-        if (ni) tpsa_contact_iface_kernel<3><<<fg_grid(ni), 256, 0, st>>>(t, g->ctc_blk.as<int64_t>(), I, T, av);
-    } else {
-        tpsa_contact_block_kernel<2><<<fg_grid(np), 256, 0, st>>>(np, t, g->cc_ptr.as<int32_t>(), g->cc_ix.as<int32_t>(),
-                                                                   g->cc_cell.as<int32_t>(), g->ctc_blk.as<int64_t>(), I, T,
-                                                                   in.mu.as<double>(), in.lam.as<double>(),
-                                                                   in.vol.as<double>(), av);
-        if (ni) tpsa_contact_iface_kernel<2><<<fg_grid(ni), 256, 0, st>>>(t, g->ctc_blk.as<int64_t>(), I, T, av);
-    }
-    pb_count_launch_();
-    SYS_TRY(cudaGetLastError());
-    if (stage_ms) SYS_TRY(cudaEventRecord(ev.e[2], st));
-    SYS_TRY(cudaStreamSynchronize(st));
-    if (stage_ms) {
-        SYS_TRY(cudaEventElapsedTime(stage_ms, ev.e[0], ev.e[1]));
-        SYS_TRY(cudaEventElapsedTime(stage_ms + 1, ev.e[1], ev.e[2]));
-    }
-#undef SYS_TRY
-    g->terms_nd = nd;
-    *out = a;
-    return PB_OK;
+    const int64_t np = g->npairs, ni = (int64_t)nd * (g->ctc_nm + g->ctc_nk);
+    return tpsa_assemble(g, nd, in, g->ctc, g->nc * (nd == 3 ? 7 : 4) + ni, out, stage_ms,
+                         [&](auto ND, const TpsaTerms &T, double *a) {
+        tpsa_contact_block_kernel<ND><<<fg_grid(np), 256, 0, g->stream>>>(
+            np, t, g->cc_ptr.as<int32_t>(), g->cc_ix.as<int32_t>(), g->cc_cell.as<int32_t>(), g->ctc.blk.as<int64_t>(), I,
+            T, in.mu.as<double>(), in.lam.as<double>(), in.vol.as<double>(), a);
+        if (ni) tpsa_contact_iface_kernel<ND><<<fg_grid(ni), 256, 0, g->stream>>>(t, g->ctc.blk.as<int64_t>(), I, T, a);
+    });
 }
 
 extern "C" int pb_tpsa_contact_rhs(pb_facegrid *g, const double *bc_values, const double *body_force,
                                    const double *angular_source, const double *mass_source, double *rhs_dev) {
     if (!g || !bc_values || !rhs_dev) return pb_fail_(PB_EINVAL, "null pointer");
-    const int nd = g->ctc_nd;
+    const int nd = (int)g->ctc.key[0];
     if ((nd != 2 && nd != 3) || g->terms_nd != nd) return pb_fail_(PB_EINVAL, "pb_tpsa_contact_system has not been called");
-    const int64_t nf = g->nf, nc = g->nc;
-    const int nr = nd == 3 ? 3 : 1;
-    cudaStream_t st = g->stream;
-    DevBuf dg, df, dsr, dsp;
-    CUDA_TRY(dg.upload(bc_values, (size_t)nd * nf, st));
-    if (body_force) CUDA_TRY(df.upload(body_force, (size_t)nd * nc, st));
-    if (angular_source) CUDA_TRY(dsr.upload(angular_source, (size_t)nr * nc, st));
-    if (mass_source) CUDA_TRY(dsp.upload(mass_source, (size_t)nc, st));
-    TpsaTerms T{};
-    for (int k = PB_TPSA_BOUND_STRESS; k <= PB_TPSA_BOUND_MASS_DISPLACEMENT; ++k) T.t[k] = g->terms[k].as<double>();
-    const TpsaTopo t = tpsa_topo(g);
-    const TpsaMortars I = tpsa_mortars(g);
-    const int64_t rows = nc * (nd + nr + 1) + (int64_t)nd * (g->ctc_nm + g->ctc_nk);
-    const double *pf = body_force ? df.as<double>() : nullptr, *psr = angular_source ? dsr.as<double>() : nullptr,
-                 *psp = mass_source ? dsp.as<double>() : nullptr;
-    if (nd == 3) tpsa_contact_rhs_kernel<3><<<fg_grid(rows), 256, 0, st>>>(t, I, T, dg.as<double>(), pf, psr, psp, rhs_dev);
-    else tpsa_contact_rhs_kernel<2><<<fg_grid(rows), 256, 0, st>>>(t, I, T, dg.as<double>(), pf, psr, psp, rhs_dev);
-    pb_count_launch_();
-    CUDA_TRY(cudaGetLastError());
-    CUDA_TRY(cudaStreamSynchronize(st));
-    return PB_OK;
+    return tpsa_rhs<0>(g, nd, true, bc_values, body_force, angular_source, mass_source, rhs_dev);
 }
 
 extern "C" int pb_tpsa_contact_rows(pb_facegrid *g, pb_csr *a, const pb_csr *jc, const double *neg_res_dev,
                                     double *rhs_dev, int *missing_dev, uint64_t stream) {
     if (!g || !a || !jc || !neg_res_dev || !rhs_dev) return pb_fail_(PB_EINVAL, "null pointer");
-    const int nd = g->ctc_nd;
+    const int nd = (int)g->ctc.key[0];
     if (nd != 2 && nd != 3) return pb_fail_(PB_EINVAL, "pb_tpsa_contact_system has not been called");
     const int64_t nc = g->nc, nm = g->ctc_nm, nk = g->ctc_nk, c0 = nc * (nd == 3 ? 7 : 4);
     const int64_t nrows = c0 + (int64_t)nd * (nm + nk);
     const CsrView va = pb_csr_view_(a), vj = pb_csr_view_(jc);
-    if (va.nrows != nrows || va.ncols != nrows || va.nnz != g->ctc_nnz)
+    if (va.nrows != nrows || va.ncols != nrows || va.nnz != g->ctc.nnz)
         return pb_fail_(PB_EINVAL, "the matrix is not the TPSA contact system of this grid");
     if (vj.nrows != (int64_t)nd * nk || vj.ncols != (int64_t)nd * (nk + nm))
         return pb_fail_(PB_EINVAL, "contact Jacobian must be nd num_fracture_cells x nd (num_fracture_cells + num_mortar) "
                                    "([t | u_j])");
     if (!nk) return PB_OK;
-    cudaStream_t st = (cudaStream_t)stream;
-    // the contact rows start nd nm LF entries after the balance rows
-    const int64_t lf = nd + (nd == 3 ? 3 : 1) + 3, e0 = g->ctc_ncell + (int64_t)nd * nm * lf;
-    const int64_t n = (int64_t)nd * nk;
-    if (nd == 3)
-        tpsa_contact_law_kernel<3><<<fg_grid(n), 256, 0, st>>>(n, c0, c0 + (int64_t)nd * nm, e0, va.indices,
-                                                               vj.indptr, vj.indices, vj.data, neg_res_dev, va.data,
-                                                               rhs_dev, missing_dev);
-    else
-        tpsa_contact_law_kernel<2><<<fg_grid(n), 256, 0, st>>>(n, c0, c0 + (int64_t)nd * nm, e0, va.indices,
-                                                               vj.indptr, vj.indices, vj.data, neg_res_dev, va.data,
-                                                               rhs_dev, missing_dev);
+    // the contact rows are the last nd nk rows, of 3 nd entries each
+    const int64_t n = (int64_t)nd * nk, e0 = g->ctc.nnz - n * 3 * nd;
+    tpsa_nd(nd, [&](auto ND) {
+        tpsa_contact_law_kernel<ND><<<fg_grid(n), 256, 0, (cudaStream_t)stream>>>(
+            n, c0, c0 + (int64_t)nd * nm, e0, va.indices, vj.indptr, vj.indices, vj.data, neg_res_dev, va.data, rhs_dev,
+            missing_dev);
+    });
     pb_count_launch_();
     CUDA_TRY(cudaGetLastError());
     return PB_OK;

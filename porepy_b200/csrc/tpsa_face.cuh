@@ -6,6 +6,7 @@
 // no atomics.  The CUDA kernel (face.cu) runs one thread per face; the test-only host build loops over faces.
 #pragma once
 #include <cmath>
+#include <cstddef>
 
 #include "views.hpp"
 
@@ -15,6 +16,14 @@ namespace pb {
 struct TpsaOut {
     double *t[14];
 };
+
+// Length of o.t[k] on a grid of nf faces and nfc (face, cell) entries: the values per entry of the cell terms
+// (k < PB_TPSA_BOUND_STRESS = 10) or per face of the bound_* face terms, in the layout below.
+constexpr size_t tpsa_term_size(int k, int nd, size_t nfc, size_t nf) {
+    const size_t d = nd, r = nd == 3 ? 3 : 1;
+    const size_t per[14] = {d, d * r, d, r * d, r * r, d, 1, d, d * r, d, d, r * d, d, d};
+    return per[k] * (k < 10 ? nfc : nf);
+}
 
 // Value layout, with L = number of cells of face f (1 or 2) and p0 = fc_ptr[f]:
 //  * cell terms with br x bc blocks: the CSR order of the expanded pattern (fv.block_expand), i.e. block

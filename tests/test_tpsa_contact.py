@@ -6,9 +6,6 @@ tools/make_tpsa_contact_golden.py), live stock models with two fractures through
 block-Jacobi GMRES on every fixture Jacobian and the register use of the new kernels.
 CPU: host build of tpsa_system.cuh + the scipy stand-in for the device sparse algebra."""
 import os
-import re
-import shutil
-import subprocess
 import sys
 from types import SimpleNamespace
 
@@ -107,9 +104,9 @@ def check_time_step(prob, d, tol, linear_solver):
 def host_build(monkeypatch):
     import emu_sparse
     from emu_binding import EmuBackedPlan
-    from emu_tpsa_contact import EmuTpsaContactFaceGrid
+    from emu_tpsa import EmuTpsaFaceGrid
     monkeypatch.setattr(fv, "DevicePlan", EmuBackedPlan)
-    monkeypatch.setattr(fv, "FaceGrid", EmuTpsaContactFaceGrid)
+    monkeypatch.setattr(fv, "FaceGrid", EmuTpsaFaceGrid)
     emu_sparse.install(monkeypatch)
 
 
@@ -201,7 +198,7 @@ def test_refusals_host(host_build):
 
 def test_too_many_face_neighbours_host(host_build):
     """A cell with 32 face neighbours (a fan of 32 triangles around one centre cell) is refused."""
-    from emu_tpsa_contact import EmuTpsaContactFaceGrid
+    from emu_tpsa import EmuTpsaFaceGrid
     n = 32
     # one centre cell with n faces, each shared with one outer cell; every outer cell also has two boundary faces
     rows, cols, vals = [], [], []
@@ -221,7 +218,7 @@ def test_too_many_face_neighbours_host(host_build):
                         face_normals=np.vstack([np.cos(ang), np.sin(ang), np.zeros(nf)]),
                         face_centers=np.vstack([np.cos(ang), np.sin(ang), np.zeros(nf)]),
                         cell_centers=np.zeros((3, n + 1)))
-    fg = EmuTpsaContactFaceGrid(g)
+    fg = EmuTpsaFaceGrid(g)
     codes = np.zeros((nf, 2), np.uint8)
     flags = np.zeros(nf, np.uint8)
     flags[n:] = 1
@@ -317,26 +314,6 @@ def test_bridge_host_build(nd, host_build):
     _check_bridge(nd)
 
 
-# ---- register use of the new instantiations (compile only) -------------------------------------------------------
-
-NEW_KERNELS = re.compile(r"tpsa_contact_\w+_kernelILi[23]E")
-
-
-def test_new_kernels_do_not_spill(tmp_path):
-    nvcc = os.environ.get("NVCC") or shutil.which("nvcc") or "/usr/local/cuda/bin/nvcc"
-    if not os.path.exists(nvcc):
-        pytest.skip("nvcc not available")
-    out = subprocess.run([nvcc, "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-std=c++17", "-Xptxas", "-v",
-                          "-I", os.path.join(ROOT, "include"), "-c", os.path.join(ROOT, "porepy_b200", "csrc", "face.cu"),
-                          "-o", str(tmp_path / "face.o")], capture_output=True, text=True, check=True)
-    seen = []
-    for fn, props in re.findall(r"Function properties for (\S+)\n\s*(.*)", out.stderr):
-        if NEW_KERNELS.search(fn):
-            seen.append(fn)
-            assert props.startswith("0 bytes stack frame, 0 bytes spill stores, 0 bytes spill loads"), (fn, props)
-    assert len(seen) == 14, seen
-
-
 # ---- GPU ----------------------------------------------------------------------------------------------------------
 
 
@@ -353,9 +330,9 @@ def test_gpu_matches_reference_and_host_build(name, monkeypatch):
     with monkeypatch.context() as mp:
         import emu_sparse
         from emu_binding import EmuBackedPlan
-        from emu_tpsa_contact import EmuTpsaContactFaceGrid
+        from emu_tpsa import EmuTpsaFaceGrid
         mp.setattr(fv, "DevicePlan", EmuBackedPlan)
-        mp.setattr(fv, "FaceGrid", EmuTpsaContactFaceGrid)
+        mp.setattr(fv, "FaceGrid", EmuTpsaFaceGrid)
         emu_sparse.install(mp)
         ph, _ = _problem(name)
         host = check_linearizations(ph, d, 1e-12)

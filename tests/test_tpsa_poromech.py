@@ -100,9 +100,9 @@ def check_time_steps(prob, d, tol, linear_solver=None, linear_tol=1e-13):
 def host_build(monkeypatch):
     import emu_sparse
     from emu_binding import EmuBackedPlan
-    from emu_tpsa_poromech import EmuTpsaPoroFaceGrid
+    from emu_tpsa import EmuTpsaFaceGrid
     monkeypatch.setattr(fv, "DevicePlan", EmuBackedPlan)
-    monkeypatch.setattr(fv, "FaceGrid", EmuTpsaPoroFaceGrid)
+    monkeypatch.setattr(fv, "FaceGrid", EmuTpsaFaceGrid)
     emu_sparse.install(monkeypatch)
 
 
@@ -213,9 +213,9 @@ def test_gpu_matches_reference_and_host_build(name, monkeypatch):
     with monkeypatch.context() as mp:
         import emu_sparse
         from emu_binding import EmuBackedPlan
-        from emu_tpsa_poromech import EmuTpsaPoroFaceGrid
+        from emu_tpsa import EmuTpsaFaceGrid
         mp.setattr(fv, "DevicePlan", EmuBackedPlan)
-        mp.setattr(fv, "FaceGrid", EmuTpsaPoroFaceGrid)
+        mp.setattr(fv, "FaceGrid", EmuTpsaFaceGrid)
         emu_sparse.install(mp)
         ph, _ = _problem(name)
         host = check_linearizations(ph, d, 1e-12)

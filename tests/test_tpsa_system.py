@@ -3,6 +3,9 @@
 against the unmodified reference model's Jacobian and right-hand side (fixtures of tools/make_tpsa_model_golden.py),
 the block-Jacobi BiCGStab solve, the 4 x 4 and 7 x 7 block inverses, the refusals, and the bench-size mesh."""
 import os
+import re
+import shutil
+import subprocess
 import sys
 from types import SimpleNamespace
 
@@ -25,8 +28,8 @@ MODEL_CASES = case_names("tpsa_model_")
 
 @pytest.fixture()
 def host_build(monkeypatch):
-    from emu_tpsa_system import EmuTpsaSystemFaceGrid
-    monkeypatch.setattr(fv, "FaceGrid", EmuTpsaSystemFaceGrid)
+    from emu_tpsa import EmuTpsaFaceGrid
+    monkeypatch.setattr(fv, "FaceGrid", EmuTpsaFaceGrid)
 
 
 def _nr(nd):
@@ -235,20 +238,64 @@ def test_bridge_refuses_tpsa_poromechanics():
         model_bridge.tpsa_momentum_from_model(m)
 
 
+# ---- register use of every TPSA kernel of face.cu (compile only) --------------------------------------------------
+
+_ND = ["<2>", "<3>"]
+_ND_NS = [f"<{nd}, {ns}>" for nd in (2, 3) for ns in (1, 2)]
+TPSA_KERNELS = {
+    "tpsa_kernel": _ND, "tpsa_nb_count_kernel": [""], "tpsa_nb_list_kernel": [""], "tpsa_pattern_kernel": _ND,
+    "tpsa_system_kernel": _ND, "tpsa_rhs_kernel": [f"<{nd}, {ns}>" for nd in (2, 3) for ns in (0, 1, 2)],
+    "tpsa_poro_count_kernel": _ND_NS, "tpsa_poro_pattern_kernel": _ND_NS, "tpsa_poro_system_kernel": _ND_NS,
+    "tpsa_poro_fluid_kernel": _ND_NS, "tpsa_contact_count_kernel": _ND, "tpsa_contact_pattern_kernel": _ND,
+    "tpsa_contact_iface_pattern_kernel": _ND, "tpsa_contact_block_kernel": _ND, "tpsa_contact_iface_kernel": _ND,
+    "tpsa_contact_law_kernel": _ND,
+}
+# the kernels that enumerate the face neighbours of a cell hold them in a kTpsaMaxNb = 32 int32 array on the stack
+NB_STACK = {"tpsa_nb_count_kernel": 128, "tpsa_nb_list_kernel": 128}
+
+
+def _kernel_name(mangled):
+    """'stem<a, b>' of an Itanium-mangled kernel whose template arguments are ints ('_Z<len><stem>ILi2ELi1EE...')."""
+    m = re.match(r"_Z(\d+)", mangled)
+    n = int(m.group(1))
+    stem, rest = mangled[m.end():m.end() + n], mangled[m.end() + n:]
+    args = re.match(r"I((?:Li-?\d+E)+)E", rest)
+    return stem + (f"<{', '.join(re.findall(r'Li(-?\d+)E', args.group(1)))}>" if args else "")
+
+
+def test_tpsa_kernels_do_not_spill(tmp_path):
+    nvcc = os.environ.get("NVCC") or shutil.which("nvcc") or "/usr/local/cuda/bin/nvcc"
+    if not os.path.exists(nvcc):
+        pytest.skip("nvcc not available")
+    out = subprocess.run([nvcc, "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-std=c++17", "-Xptxas", "-v",
+                          "-I", os.path.join(ROOT, "include"), "-c", os.path.join(ROOT, "porepy_b200", "csrc", "face.cu"),
+                          "-o", str(tmp_path / "face.o")], capture_output=True, text=True, check=True)
+    seen = set()
+    for fn, props in re.findall(r"Function properties for (\S+)\n\s*(.*)", out.stderr):
+        if "tpsa" not in fn:
+            continue
+        name = _kernel_name(fn)
+        seen.add(name)
+        stack = NB_STACK.get(name, 0)
+        assert props.startswith(f"{stack} bytes stack frame, 0 bytes spill stores, 0 bytes spill loads"), (name, props)
+    want = {stem + args for stem, all_args in TPSA_KERNELS.items() for args in all_args}
+    assert want <= seen, sorted(want - seen)
+
+
 # ---- GPU ----------------------------------------------------------------------------------------------------------
 
 
 @pytest.mark.gpu
 @pytest.mark.parametrize("name", CASES)
 def test_gpu_matches_restatement_and_host_build(name, monkeypatch):
-    from emu_tpsa_system import EmuTpsaSystemFaceGrid
+    from emu_tpsa import EmuTpsaFaceGrid
     _check_restatement(name, 1e-13)
     c = load_case(name)
     lam, bcv, f, sr, sp = _seeded_inputs(c.g, 11)
     A, b = _problem(c, lam, bcv, f, sr, sp).assemble()
     A, b = A.to_scipy(), b.cpu().numpy()
     with monkeypatch.context() as mp:
-        mp.setattr(fv, "FaceGrid", EmuTpsaSystemFaceGrid)
+        mp.setattr(fv, "FaceGrid", EmuTpsaFaceGrid)
         Ah, bh = _problem(load_case(name), lam, bcv, f, sr, sp).assemble()
     assert np.array_equal(A.indptr, Ah.indptr) and np.array_equal(A.indices, Ah.indices)
     assert np.abs(A.data - Ah.data).max() <= 1e-13 * np.abs(Ah.data).max()

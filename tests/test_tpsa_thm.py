@@ -3,7 +3,7 @@
 ``pp.Thermoporomechanics`` + ``TpsaPoromechanicsMixin``: the couplings the fixtures carry, Jacobian and -R at the zero
 state and at an intermediate Newton iterate of two time steps, the residual histories and converged states (fixtures of
 tools/make_tpsa_thm_golden.py), a live stock model through the bridge, the refusals, the 6 x 6 and 9 x 9 block inverses,
-the register use of the new kernels and the bench-size mesh.
+the register use of the 6 x 6 and 9 x 9 Krylov kernels and the bench-size mesh.
 CPU: host build of tpsa_system.cuh + the scipy stand-in for the device sparse algebra."""
 import os
 import re
@@ -82,9 +82,9 @@ def check_linearizations(prob, d, tol):
 def host_build(monkeypatch):
     import emu_sparse
     from emu_binding import EmuBackedPlan
-    from emu_tpsa_thm import EmuTpsaThmFaceGrid
+    from emu_tpsa import EmuTpsaFaceGrid
     monkeypatch.setattr(fv, "DevicePlan", EmuBackedPlan)
-    monkeypatch.setattr(fv, "FaceGrid", EmuTpsaThmFaceGrid)
+    monkeypatch.setattr(fv, "FaceGrid", EmuTpsaFaceGrid)
     emu_sparse.install(monkeypatch)
 
 
@@ -197,25 +197,24 @@ def test_bridge_host_build(nd, host_build):
     _check_bridge(nd)
 
 
-# ---- register use of the new instantiations (compile only) -------------------------------------------------------
+# ---- register use of the new block-size instantiations (compile only; the TPSA kernels: test_tpsa_system.py) ------
 
-NEW_KERNELS = re.compile(r"tpsa_poro_\w+_kernelILi[23]ELi2E|block_diag_inv_inplace_kernelILi[69]E|kry_[ps]_kernelILi[69]E")
+KRYLOV_KERNELS = re.compile(r"block_diag_inv_inplace_kernelILi[69]E|kry_[ps]_kernelILi[69]E")
 
 
-def test_new_kernels_do_not_spill(tmp_path):
+def test_krylov_kernels_do_not_spill(tmp_path):
     nvcc = os.environ.get("NVCC") or shutil.which("nvcc") or "/usr/local/cuda/bin/nvcc"
     if not os.path.exists(nvcc):
         pytest.skip("nvcc not available")
+    out = subprocess.run([nvcc, "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-std=c++17", "-Xptxas", "-v",
+                          "-I", os.path.join(ROOT, "include"), "-c", os.path.join(ROOT, "porepy_b200", "csrc", "krylov.cu"),
+                          "-o", str(tmp_path / "krylov.o")], capture_output=True, text=True, check=True)
     seen = []
-    for name in ("face.cu", "krylov.cu"):
-        out = subprocess.run([nvcc, "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-std=c++17", "-Xptxas", "-v",
-                              "-I", os.path.join(ROOT, "include"), "-c", os.path.join(ROOT, "porepy_b200", "csrc", name),
-                              "-o", str(tmp_path / (name + ".o"))], capture_output=True, text=True, check=True)
-        for fn, props in re.findall(r"Function properties for (\S+)\n\s*(.*)", out.stderr):
-            if NEW_KERNELS.search(fn):
-                seen.append(fn)
-                assert props.startswith("0 bytes stack frame, 0 bytes spill stores, 0 bytes spill loads"), (fn, props)
-    assert len(seen) == 10 + 6, seen
+    for fn, props in re.findall(r"Function properties for (\S+)\n\s*(.*)", out.stderr):
+        if KRYLOV_KERNELS.search(fn):
+            seen.append(fn)
+            assert props.startswith("0 bytes stack frame, 0 bytes spill stores, 0 bytes spill loads"), (fn, props)
+    assert len(seen) == 6, seen
 
 
 # ---- GPU ----------------------------------------------------------------------------------------------------------
@@ -230,9 +229,9 @@ def test_gpu_matches_reference_and_host_build(name, monkeypatch):
     with monkeypatch.context() as mp:
         import emu_sparse
         from emu_binding import EmuBackedPlan
-        from emu_tpsa_thm import EmuTpsaThmFaceGrid
+        from emu_tpsa import EmuTpsaFaceGrid
         mp.setattr(fv, "DevicePlan", EmuBackedPlan)
-        mp.setattr(fv, "FaceGrid", EmuTpsaThmFaceGrid)
+        mp.setattr(fv, "FaceGrid", EmuTpsaFaceGrid)
         emu_sparse.install(mp)
         ph, _ = _problem(name)
         host = check_linearizations(ph, d, 1e-12)

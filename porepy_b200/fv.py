@@ -638,84 +638,46 @@ class FaceGrid:
     def tpsa_system(self, nd: int, mu, lmbda, cell_volumes, codes, robin_diag, face_flags, face_areas) -> tuple:
         """The TPSA three-field system matrix (``pb_tpsa_system``, layout in include/poreb200.h) as a ``DeviceCsr`` and
         the device times of its two stages in ms.  ``codes`` / ``robin_diag``: (nf, nd), ``face_flags``: nf."""
-        from .sparse import DeviceCsr
-        mu, lam, vol = _lib.f64(mu), _lib.f64(lmbda), _lib.f64(cell_volumes)
-        if mu.shape != (self.nc,) or lam.shape != (self.nc,):
-            raise ValueError("fourth_order_tensor.mu and .lmbda must have one value per cell")
-        if vol.shape != (self.nc,):
-            raise ValueError("cell_volumes must have one value per cell")
-        cod = np.ascontiguousarray(codes, dtype=np.uint8)
-        rob = None if robin_diag is None else _lib.f64(robin_diag)
-        flags = np.ascontiguousarray(face_flags, dtype=np.uint8)
-        _lib.check(self.lib.pb_facegrid_set_face_areas(self.h, _lib.ptr(_lib.f64(face_areas), _lib._f64p)))
-        h = C.c_void_p()
-        ms = (C.c_float * 2)()
-        _lib.check(self.lib.pb_tpsa_system(self.h, int(nd), _lib.ptr(mu, _lib._f64p), _lib.ptr(lam, _lib._f64p),
-                                           _lib.ptr(vol, _lib._f64p), _lib.ptr(cod, _lib._u8p),
-                                           _lib.ptr(rob, _lib._f64p), _lib.ptr(flags, _lib._u8p), C.byref(h),
-                                           C.cast(ms, _lib._f32p)))
-        return DeviceCsr.from_handle(h), [float(ms[0]), float(ms[1])]
+        return self._system(self.lib.pb_tpsa_system, nd, {"fourth_order_tensor.mu": mu,
+                                                          "fourth_order_tensor.lmbda": lmbda,
+                                                          "cell_volumes": cell_volumes},
+                            codes, robin_diag, face_flags, face_areas)
 
     def tpsa_rhs(self, n: int, bc_values, body_force=None, angular_source=None, mass_source=None):
         """b = -R(0) of the TPSA system last assembled on this grid (``pb_tpsa_rhs``) as a CUDA tensor of ``n``
         doubles."""
-        import torch
-        arrs = [None if a is None else _lib.f64(a) for a in (bc_values, body_force, angular_source, mass_source)]
-        b = torch.empty(int(n), dtype=torch.float64, device="cuda")
-        _lib.check(self.lib.pb_tpsa_rhs(self.h, *[_lib.ptr(a, _lib._f64p) for a in arrs], C.c_void_p(b.data_ptr())))
-        return b
+        return self._rhs(self.lib.pb_tpsa_rhs, n, bc_values, body_force, angular_source, mass_source)
 
     def tpsa_poro_system(self, nd: int, mu, lmbda, alpha, cell_volumes, codes, robin_diag, face_flags, face_areas,
                          flux_pattern) -> tuple:
         """The TPSA poromechanics Jacobian with its mechanics rows (``pb_tpsa_poro_system``, layout in
         include/poreb200.h) as a ``DeviceCsr`` and the device times of its two stages in ms.  ``flux_pattern``: the
         ``DeviceCsr`` div @ flux whose rows give the fluid-row patterns."""
-        return self._poro_system(self.lib.pb_tpsa_poro_system, nd, mu, lmbda, alpha, cell_volumes, codes, robin_diag,
-                                 face_flags, face_areas, flux_pattern)
+        return self._system(self.lib.pb_tpsa_poro_system, nd, self._poro_cells(mu, lmbda, alpha, cell_volumes), codes,
+                            robin_diag, face_flags, face_areas, flux_pattern.h)
 
     def tpsa_thm_system(self, nd: int, mu, lmbda, alpha, cell_volumes, codes, robin_diag, face_flags, face_areas,
                         flux_pattern) -> tuple:
         """The TPSA thermo-poromechanics Jacobian with its mechanics rows (``pb_tpsa_thm_system``, layout in
         include/poreb200.h) as a ``DeviceCsr`` and the device times of its two stages in ms.  ``flux_pattern``: a
         ``DeviceCsr`` whose rows hold the union of the Darcy and Fourier div @ flux patterns."""
-        return self._poro_system(self.lib.pb_tpsa_thm_system, nd, mu, lmbda, alpha, cell_volumes, codes, robin_diag,
-                                 face_flags, face_areas, flux_pattern)
+        return self._system(self.lib.pb_tpsa_thm_system, nd, self._poro_cells(mu, lmbda, alpha, cell_volumes), codes,
+                            robin_diag, face_flags, face_areas, flux_pattern.h)
 
-    def _poro_system(self, fn, nd, mu, lmbda, alpha, cell_volumes, codes, robin_diag, face_flags, face_areas,
-                     flux_pattern):
-        from .sparse import DeviceCsr
-        mu, lam, al, vol = _lib.f64(mu), _lib.f64(lmbda), _lib.f64(alpha), _lib.f64(cell_volumes)
-        if mu.shape != (self.nc,) or lam.shape != (self.nc,) or al.shape != (self.nc,):
-            raise ValueError("mu, lmbda and the Biot coefficient must have one value per cell")
-        if vol.shape != (self.nc,):
-            raise ValueError("cell_volumes must have one value per cell")
-        cod = np.ascontiguousarray(codes, dtype=np.uint8)
-        rob = None if robin_diag is None else _lib.f64(robin_diag)
-        flags = np.ascontiguousarray(face_flags, dtype=np.uint8)
-        _lib.check(self.lib.pb_facegrid_set_face_areas(self.h, _lib.ptr(_lib.f64(face_areas), _lib._f64p)))
-        h = C.c_void_p()
-        ms = (C.c_float * 2)()
-        _lib.check(fn(self.h, int(nd), _lib.ptr(mu, _lib._f64p), _lib.ptr(lam, _lib._f64p), _lib.ptr(al, _lib._f64p),
-                      _lib.ptr(vol, _lib._f64p), _lib.ptr(cod, _lib._u8p), _lib.ptr(rob, _lib._f64p),
-                      _lib.ptr(flags, _lib._u8p), flux_pattern.h, C.byref(h), C.cast(ms, _lib._f32p)))
-        return DeviceCsr.from_handle(h), [float(ms[0]), float(ms[1])]
+    @staticmethod
+    def _poro_cells(mu, lmbda, alpha, cell_volumes) -> dict:
+        return {"fourth_order_tensor.mu": mu, "fourth_order_tensor.lmbda": lmbda, "the Biot coefficient": alpha,
+                "cell_volumes": cell_volumes}
 
     def tpsa_poro_rhs(self, n: int, bc_values, body_force=None, angular_source=None, mass_source=None):
         """-R(0) of the mechanics rows of the poromechanics system last assembled on this grid (``pb_tpsa_poro_rhs``),
         0 in the fluid rows, as a CUDA tensor of ``n`` doubles."""
-        return self._poro_rhs(self.lib.pb_tpsa_poro_rhs, n, bc_values, body_force, angular_source, mass_source)
+        return self._rhs(self.lib.pb_tpsa_poro_rhs, n, bc_values, body_force, angular_source, mass_source)
 
     def tpsa_thm_rhs(self, n: int, bc_values, body_force=None, angular_source=None, mass_source=None):
         """-R(0) of the mechanics rows of the thermo-poromechanics system last assembled on this grid
         (``pb_tpsa_thm_rhs``), 0 in the mass and energy rows, as a CUDA tensor of ``n`` doubles."""
-        return self._poro_rhs(self.lib.pb_tpsa_thm_rhs, n, bc_values, body_force, angular_source, mass_source)
-
-    def _poro_rhs(self, fn, n, bc_values, body_force, angular_source, mass_source):
-        import torch
-        arrs = [None if a is None else _lib.f64(a) for a in (bc_values, body_force, angular_source, mass_source)]
-        b = torch.empty(int(n), dtype=torch.float64, device="cuda")
-        _lib.check(fn(self.h, *[_lib.ptr(a, _lib._f64p) for a in arrs], C.c_void_p(b.data_ptr())))
-        return b
+        return self._rhs(self.lib.pb_tpsa_thm_rhs, n, bc_values, body_force, angular_source, mass_source)
 
     def tpsa_poro_fluid_rows(self, A, jf, neg_res, rhs, missing=None) -> None:
         """Write the fluid rows of ``A`` (the matrix of ``tpsa_poro_system``) from the field-ordered fluid Jacobian
@@ -736,33 +698,23 @@ class FaceGrid:
         include/poreb200.h) as a ``DeviceCsr`` and the device times of its two stages in ms.  ``mortars``: per mortar
         cell (all interfaces in order) ``face``, ``cell`` (fracture cell, all fractures in order), ``m2p``, ``p2m``,
         ``sign`` and ``volume``; ``frames``: nd x nd per fracture cell, row-major."""
-        from .sparse import DeviceCsr
-        mu, lam, vol = _lib.f64(mu), _lib.f64(lmbda), _lib.f64(cell_volumes)
-        if mu.shape != (self.nc,) or lam.shape != (self.nc,) or vol.shape != (self.nc,):
-            raise ValueError("mu, lmbda and cell_volumes must have one value per cell")
         face, cell = (np.ascontiguousarray(mortars[k], dtype=np.int32) for k in ("face", "cell"))
         w = [_lib.f64(mortars[k]) for k in ("m2p", "p2m", "sign", "volume")]
         nm, nk = face.size, int(np.asarray(frames).size) // (nd * nd)
         if cell.size != nm or any(a.size != nm for a in w):
             raise ValueError("every mortar array must have one value per mortar cell")
         fr = _lib.f64(frames)
-        cod = np.ascontiguousarray(codes, dtype=np.uint8)
-        rob = None if robin_diag is None else _lib.f64(robin_diag)
-        flags = np.ascontiguousarray(face_flags, dtype=np.uint8)
-        _lib.check(self.lib.pb_facegrid_set_face_areas(self.h, _lib.ptr(_lib.f64(face_areas), _lib._f64p)))
-        h = C.c_void_p()
-        ms = (C.c_float * 2)()
-        _lib.check(self.lib.pb_tpsa_contact_system(
-            self.h, int(nd), _lib.ptr(mu, _lib._f64p), _lib.ptr(lam, _lib._f64p), _lib.ptr(vol, _lib._f64p),
-            _lib.ptr(cod, _lib._u8p), _lib.ptr(rob, _lib._f64p), _lib.ptr(flags, _lib._u8p), int(nm), int(nk),
-            _lib.ptr(face, _lib._i32p), _lib.ptr(cell, _lib._i32p), *[_lib.ptr(a, _lib._f64p) for a in w],
-            _lib.ptr(fr, _lib._f64p), float(characteristic_traction), C.byref(h), C.cast(ms, _lib._f32p)))
-        return DeviceCsr.from_handle(h), [float(ms[0]), float(ms[1])]
+        return self._system(self.lib.pb_tpsa_contact_system, nd, {"fourth_order_tensor.mu": mu,
+                                                                  "fourth_order_tensor.lmbda": lmbda,
+                                                                  "cell_volumes": cell_volumes},
+                            codes, robin_diag, face_flags, face_areas, int(nm), int(nk), _lib.ptr(face, _lib._i32p),
+                            _lib.ptr(cell, _lib._i32p), *[_lib.ptr(a, _lib._f64p) for a in w],
+                            _lib.ptr(fr, _lib._f64p), float(characteristic_traction))
 
     def tpsa_contact_rhs(self, n: int, bc_values, body_force=None, angular_source=None, mass_source=None):
         """-R(0) of the balance and force rows of the contact system last assembled on this grid
         (``pb_tpsa_contact_rhs``), 0 in the contact rows, as a CUDA tensor of ``n`` doubles."""
-        return self._poro_rhs(self.lib.pb_tpsa_contact_rhs, n, bc_values, body_force, angular_source, mass_source)
+        return self._rhs(self.lib.pb_tpsa_contact_rhs, n, bc_values, body_force, angular_source, mass_source)
 
     def tpsa_contact_rows(self, A, jc, neg_res, rhs, missing=None) -> None:
         """Write the contact rows of ``A`` (the matrix of ``tpsa_contact_system``) from the Jacobian ``jc`` of the
@@ -770,6 +722,35 @@ class FaceGrid:
         ``neg_res``, on the current stream (``pb_tpsa_contact_rows``).  ``missing``: int32 CUDA tensor counting entries
         outside the pattern."""
         self._balance_rows(self.lib.pb_tpsa_contact_rows, jc.shape[0], A, jc, neg_res, rhs, missing)
+
+    def _system(self, fn, nd, cells: dict, codes, robin_diag, face_flags, face_areas, *extra) -> tuple:
+        """``fn(handle, nd, *cells, codes, robin_diag, face_flags, *extra, &matrix, stage_ms)`` of a
+        ``pb_tpsa_*_system`` entry point after checking that every array of ``cells`` (by name) has one value per cell
+        and setting the face areas: the matrix as a ``DeviceCsr`` and the device times of its two stages in ms."""
+        from .sparse import DeviceCsr
+        cells = {name: _lib.f64(a) for name, a in cells.items()}
+        for name, a in cells.items():
+            if a.shape != (self.nc,):
+                raise ValueError(f"{name} must have one value per cell")
+        cod = np.ascontiguousarray(codes, dtype=np.uint8)
+        rob = None if robin_diag is None else _lib.f64(robin_diag)
+        flags = np.ascontiguousarray(face_flags, dtype=np.uint8)
+        _lib.check(self.lib.pb_facegrid_set_face_areas(self.h, _lib.ptr(_lib.f64(face_areas), _lib._f64p)))
+        h = C.c_void_p()
+        ms = (C.c_float * 2)()
+        _lib.check(fn(self.h, int(nd), *[_lib.ptr(a, _lib._f64p) for a in cells.values()], _lib.ptr(cod, _lib._u8p),
+                      _lib.ptr(rob, _lib._f64p), _lib.ptr(flags, _lib._u8p), *extra, C.byref(h),
+                      C.cast(ms, _lib._f32p)))
+        return DeviceCsr.from_handle(h), [float(ms[0]), float(ms[1])]
+
+    def _rhs(self, fn, n, bc_values, body_force, angular_source, mass_source):
+        """``fn(handle, bc_values, body_force, angular_source, mass_source, b)`` of a ``pb_tpsa_*_rhs`` entry point
+        (None: zero): b as a CUDA tensor of ``n`` doubles."""
+        import torch
+        arrs = [None if a is None else _lib.f64(a) for a in (bc_values, body_force, angular_source, mass_source)]
+        b = torch.empty(int(n), dtype=torch.float64, device="cuda")
+        _lib.check(fn(self.h, *[_lib.ptr(a, _lib._f64p) for a in arrs], C.c_void_p(b.data_ptr())))
+        return b
 
     def _balance_rows(self, fn, n, A, jf, neg_res, rhs, missing):
         import torch
@@ -1361,6 +1342,20 @@ def tpsa_bc_arrays(bc, nd: int, nf: int):
     return codes, robin
 
 
+def tpsa_face_inputs(sd, bc, nd: int):
+    """(codes, robin, flags) of the TPSA face kernels on ``sd``: ``tpsa_bc_arrays`` of the vectorial ``bc`` and the
+    boundary-face flags (nf uint8), after the refusals of ``tpsa_bc_arrays`` and of a 2-D grid whose face normals leave
+    the xy-plane."""
+    codes, robin = tpsa_bc_arrays(bc, nd, sd.num_faces)
+    if nd == 2 and np.any(np.abs(sd.face_normals[2]) > np.maximum(np.abs(sd.face_normals[0]),
+                                                                   np.abs(sd.face_normals[1]))):
+        # tpsa.py:1053-1054 indexes is_dir (2 rows) with the argmax over all three rows of the normals
+        raise IndexError("Tpsa: a face normal of a 2d grid points mostly out of the xy-plane")
+    flags = np.zeros(sd.num_faces, np.uint8)
+    flags[np.asarray(sd.get_all_boundary_faces(), dtype=np.int64)] = 1
+    return codes, robin, flags
+
+
 class Tpsa(_Base):
     """Two-point stress approximation (numerics/fv/tpsa.py:136, Nordbotten & Keilegavlen): the same constructor,
     matrix keys (:265-331), ``ndof`` and ``discretize`` outputs as the reference, computed by one thread per face on a
@@ -1422,18 +1417,12 @@ class Tpsa(_Base):
             raise NotImplementedError("Tpsa is only implemented for 2d and 3d grids.")
         self._check_unsupported(params, sd)
         mu = params["fourth_order_tensor"].mu
-        codes, robin = tpsa_bc_arrays(params["bc"], nd, nf)
-        if nd == 2 and np.any(np.abs(sd.face_normals[2]) > np.maximum(np.abs(sd.face_normals[0]),
-                                                                       np.abs(sd.face_normals[1]))):
-            # tpsa.py:1053-1054 indexes is_dir (2 rows) with the argmax over all three rows of the normals
-            raise IndexError("Tpsa: a face normal of a 2d grid points mostly out of the xy-plane")
+        codes, robin, flags = tpsa_face_inputs(sd, params["bc"], nd)
         t0 = time.perf_counter()
         fg = FaceGrid.for_grid(sd)
         fc = sps.csr_matrix(sd.cell_faces)
         fc.sort_indices()
         ip, ix = fc.indptr, fc.indices
-        flags = np.zeros(nf, np.uint8)
-        flags[np.asarray(sd.get_all_boundary_faces(), dtype=np.int64)] = 1
         vals, kernel_ms = fg.tpsa(nd, mu, codes, robin, flags, ip, sd.face_areas)
         t1 = time.perf_counter()
         # the index arrays depend on the topology only: built once per grid, copied per matrix (scipy may edit a

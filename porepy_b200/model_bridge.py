@@ -383,42 +383,78 @@ def fractured_thermoporomechanics_from_model(model):
     return prob, _column_map(model, prob.unknown_layout, grids), _row_map(model, prob.equation_layout)
 
 
+def _tpsa_grid(model, name: str, other=None):
+    """The one 2-D or 3-D subdomain of a TPSA model without fractures, for the problem class ``name``.  ``other``:
+    (equation, message) of a model family the class does not solve, refused when the model has that equation."""
+    mdg = model.mdg
+    sds = list(mdg.subdomains())
+    if any(sd.dim < model.nd for sd in sds) or any(True for _ in mdg.interfaces()):
+        raise NotImplementedError(f"{name}: fractures are not supported")
+    if len(sds) != 1:
+        raise NotImplementedError(f"{name}: one subdomain is expected")
+    if other is not None and other[0] in model.equation_system.equations:
+        raise NotImplementedError(f"{name}: {other[1]}")
+    if sds[0].dim not in (2, 3):
+        raise NotImplementedError("Tpsa is only implemented for 2d and 3d grids.")
+    return sds[0]
+
+
+def _tpsa_mechanics(model, sd) -> tuple:
+    """(the mechanical boundary operator, {body_force, angular_source, mass_source}) of ``sd``: the model's own
+    ``combine_boundary_operators_mechanical_stress``, ``body_force``, ``source_angular_momentum`` and
+    ``solid_mass_source``, evaluated."""
+    nd, nc = int(sd.dim), sd.num_cells
+    g = _evaluated(model, model.combine_boundary_operators_mechanical_stress([sd]), nd * sd.num_faces)
+    return g, dict(body_force=_evaluated(model, model.body_force([sd]), nd * nc),
+                   angular_source=_evaluated(model, model.source_angular_momentum([sd]),
+                                             model.rotation_dimension() * nc),
+                   mass_source=_evaluated(model, model.solid_mass_source([sd]), nc))
+
+
+def _tpsa_maps(model, prob, grids) -> tuple:
+    """Set and return (column_map, row_map) of a TPSA problem: the model's dofs of ``prob.fields`` and rows of
+    ``prob.balances`` on the matrix, interleaved cell by cell, then those of the blocks behind the cell block of its
+    layouts.  The poromechanics models call the solid-mass equation ``Solid_mass_equation_poromechanics``."""
+    from .tpsa_elasticity import interleave
+    nc, equations = prob.nc, model.equation_system.equations
+
+    def cell_interleaved(cell_blocks, tail, model_order):
+        layout = BlockLayout([(name, [(("matrix",), nc, w)]) for name, w in cell_blocks] + tail)
+        idx, ends, k = model_order(layout), layout.offsets, len(cell_blocks)
+        return np.concatenate([interleave([idx[a:b] for a, b in zip(ends[:k], ends[1:k + 1])], prob.nd, prob.nr, nc),
+                               idx[ends[k]:]])
+
+    prob.column_map = cell_interleaved(prob.fields, prob.unknown_layout.blocks[1:],
+                                       lambda layout: _column_map(model, layout, grids))
+    balances = [(name if name in equations else next(eq for eq in equations if eq.lower().startswith(name)), w)
+                for name, w in prob.balances]
+    prob.row_map = cell_interleaved(balances, prob.equation_layout.blocks[1:], lambda layout: _row_map(model, layout))
+    return prob.column_map, prob.row_map
+
+
 def tpsa_momentum_from_model(model):
     """A prepared ``pp.MomentumBalance`` with ``TpsaMomentumBalanceMixin`` on one 2-D or 3-D grid without fractures ->
     (``TpsaElasticity``, column_map, row_map): unknown k of the problem (cell-interleaved [u_c, r_c, p_c]) is dof
     ``column_map[k]`` of the model's ``EquationSystem``, equation k its row ``row_map[k]``.  The boundary operator g is
     the model's own ``combine_boundary_operators_mechanical_stress``, evaluated; f is its ``body_force``, s_r / s_p its
     ``source_angular_momentum`` / ``solid_mass_source``."""
-    from .tpsa_elasticity import TpsaElasticity, interleave
-    mdg, es = model.mdg, model.equation_system
-    sds = list(mdg.subdomains())
-    if any(sd.dim < model.nd for sd in sds) or any(True for _ in mdg.interfaces()):
-        raise NotImplementedError("TpsaElasticity: fractures are not supported")
-    if len(sds) != 1:
-        raise NotImplementedError("TpsaElasticity: one subdomain is expected")
-    if "mass_balance_equation" in es.equations:
-        raise NotImplementedError("TpsaElasticity: the TPSA poromechanics model (four fields) is not supported; use "
-                                  "tpsa_poromechanics_from_model")
-    sd = sds[0]
-    nd, nc = sd.dim, sd.num_cells
-    if nd not in (2, 3):
-        raise NotImplementedError("Tpsa is only implemented for 2d and 3d grids.")
-    nr = model.rotation_dimension()
+    from .tpsa_elasticity import TpsaElasticity
+    sd = _tpsa_grid(model, "TpsaElasticity", ("mass_balance_equation", "the TPSA poromechanics model (four fields) is "
+                                              "not supported; use tpsa_poromechanics_from_model"))
     mk = model.stress_keyword
-    data = _own_data(mdg.subdomain_data(sd), [mk])
-    prob = TpsaElasticity(sd, data, mk,
-                          _evaluated(model, model.combine_boundary_operators_mechanical_stress([sd]), nd * sd.num_faces),
-                          body_force=_evaluated(model, model.body_force([sd]), nd * nc),
-                          angular_source=_evaluated(model, model.source_angular_momentum([sd]), nr * nc),
-                          mass_source=_evaluated(model, model.solid_mass_source([sd]), nc))
-    cols = [_dofs(model, name, sd) for name in (model.displacement_variable, model.rotation_stress_variable,
-                                                 model.total_pressure_variable)]
-    rows = _row_map(model, BlockLayout([("momentum_balance_equation", [(("matrix",), nc, nd)]),
-                                        ("angular_momentum_balance_equation", [(("matrix",), nc, nr)]),
-                                        ("solid_mass_equation", [(("matrix",), nc, 1)])]))
-    prob.column_map = interleave(cols, nd, nr, nc)
-    prob.row_map = interleave([rows[:nd * nc], rows[nd * nc:(nd + nr) * nc], rows[(nd + nr) * nc:]], nd, nr, nc)
-    return prob, prob.column_map, prob.row_map
+    g, sources = _tpsa_mechanics(model, sd)
+    prob = TpsaElasticity(sd, _own_data(model.mdg.subdomain_data(sd), [mk]), mk, g, **sources)
+    return (prob, *_tpsa_maps(model, prob, {("matrix",): sd}))
+
+
+def _tpsa_solid(model, sd, thermal: bool) -> dict:
+    so, nc = model.solid, sd.num_cells
+    solid = dict(reference_porosity=so.porosity, biot_coefficient=_evaluated(model, model.biot_coefficient([sd]), nc),
+                 bulk_modulus=float(np.atleast_1d(_evaluated(model, model.bulk_modulus([sd]), 1))[0]))
+    if thermal:
+        solid.update(thermal_expansion=so.thermal_expansion, heat_capacity=so.specific_heat_capacity,
+                     conductivity=so.thermal_conductivity, density=so.density)
+    return solid
 
 
 def tpsa_poromechanics_from_model(model):
@@ -426,50 +462,22 @@ def tpsa_poromechanics_from_model(model):
     (``TpsaPoromechanics``, column_map, row_map): unknown k of the problem (cell-interleaved [u_c, r_c, p_t_c, p_c]) is
     dof ``column_map[k]`` of the model's ``EquationSystem``, equation k its row ``row_map[k]``.  The mechanical boundary
     operator, body force, sources, Darcy and fluid-flux boundary data are the model's own operators, evaluated."""
-    from .tpsa_poromech import TpsaPoromechanics, interleave
-    mdg, es = model.mdg, model.equation_system
-    sds = list(mdg.subdomains())
-    if any(sd.dim < model.nd for sd in sds) or any(True for _ in mdg.interfaces()):
-        raise NotImplementedError("TpsaPoromechanics: fractures are not supported")
-    if len(sds) != 1:
-        raise NotImplementedError("TpsaPoromechanics: one subdomain is expected")
-    if "energy_balance_equation" in es.equations:
-        raise NotImplementedError("TpsaPoromechanics: the TPSA thermo-poromechanics model (five fields) is not "
-                                  "supported; use tpsa_thermoporomechanics_from_model")
-    sd = sds[0]
-    nd, nc, nf = sd.dim, sd.num_cells, sd.num_faces
-    if nd not in (2, 3):
-        raise NotImplementedError("Tpsa is only implemented for 2d and 3d grids.")
-    nr = model.rotation_dimension()
+    from .tpsa_poromech import TpsaPoromechanics
+    sd = _tpsa_grid(model, "TpsaPoromechanics", ("energy_balance_equation", "the TPSA thermo-poromechanics model (five "
+                                                 "fields) is not supported; use tpsa_thermoporomechanics_from_model"))
     fk, mk = model.darcy_keyword, model.stress_keyword
-    data = _own_data(mdg.subdomain_data(sd), [fk, mk])
+    data = _own_data(model.mdg.subdomain_data(sd), [fk, mk])
     fluid = _fluid(model, False)
     w, _ = _boundary_weights(model, sd, fluid, False)
     bc_ff = model.bc_type_fluid_flux(sd)
-    so = model.solid
-    solid = dict(reference_porosity=so.porosity, biot_coefficient=_evaluated(model, model.biot_coefficient([sd]), nc),
-                 bulk_modulus=float(np.atleast_1d(_evaluated(model, model.bulk_modulus([sd]), 1))[0]))
+    g, sources = _tpsa_mechanics(model, sd)
     prob = TpsaPoromechanics(
-        sd, data, fluid, solid,
+        sd, data, fluid, _tpsa_solid(model, sd, False),
         _face_values(model, sd, data[PARAMETERS][fk]["bc"], model.bc_values_pressure, model.bc_values_darcy_flux),
-        _evaluated(model, model.combine_boundary_operators_mechanical_stress([sd]), nd * nf), bc_ff,
-        _face_values(model, sd, bc_ff, w, model.bc_values_fluid_flux),
-        body_force=_evaluated(model, model.body_force([sd]), nd * nc),
-        angular_source=_evaluated(model, model.source_angular_momentum([sd]), nr * nc),
-        mass_source=_evaluated(model, model.solid_mass_source([sd]), nc),
-        fluid_source=_evaluated(model, model.fluid_source([sd]), nc), flow_keyword=fk, mechanics_keyword=mk)
+        g, bc_ff, _face_values(model, sd, bc_ff, w, model.bc_values_fluid_flux), **sources,
+        fluid_source=_evaluated(model, model.fluid_source([sd]), sd.num_cells), flow_keyword=fk, mechanics_keyword=mk)
     prob.mobility_keyword = "b200_mobility"
-    cols = [_dofs(model, name, sd) for name in (model.displacement_variable, model.rotation_stress_variable,
-                                                 model.total_pressure_variable, model.pressure_variable)]
-    solid_mass = [eq for eq in es.equations if eq.lower().startswith("solid_mass_equation")][0]
-    rows = _row_map(model, BlockLayout([("momentum_balance_equation", [(("matrix",), nc, nd)]),
-                                        ("angular_momentum_balance_equation", [(("matrix",), nc, nr)]),
-                                        (solid_mass, [(("matrix",), nc, 1)]),
-                                        ("mass_balance_equation", [(("matrix",), nc, 1)])]))
-    prob.column_map = interleave(cols, nd, nr, nc)
-    o = np.cumsum([0, nd * nc, nr * nc, nc, nc])
-    prob.row_map = interleave([rows[o[i]:o[i + 1]] for i in range(4)], nd, nr, nc)
-    return prob, prob.column_map, prob.row_map
+    return (prob, *_tpsa_maps(model, prob, {("matrix",): sd}))
 
 
 def tpsa_thermoporomechanics_from_model(model):
@@ -480,55 +488,25 @@ def tpsa_thermoporomechanics_from_model(model):
     boundary data are the model's own operators, evaluated.  The Fourier conductivity is the one of the zero state, which
     the model discretizes with when its initial values are zero (its default); for other initial values set
     ``prob.conductivity`` before ``discretize``."""
-    from .tpsa_thermoporomech import TpsaThermoporomechanics, interleave
-    mdg, es = model.mdg, model.equation_system
-    sds = list(mdg.subdomains())
-    if any(sd.dim < model.nd for sd in sds) or any(True for _ in mdg.interfaces()):
-        raise NotImplementedError("TpsaThermoporomechanics: fractures are not supported")
-    if len(sds) != 1:
-        raise NotImplementedError("TpsaThermoporomechanics: one subdomain is expected")
-    sd = sds[0]
-    nd, nc, nf = sd.dim, sd.num_cells, sd.num_faces
-    if nd not in (2, 3):
-        raise NotImplementedError("Tpsa is only implemented for 2d and 3d grids.")
-    nr = model.rotation_dimension()
+    from .tpsa_thermoporomech import TpsaThermoporomechanics
+    sd = _tpsa_grid(model, "TpsaThermoporomechanics")
     fk, tk, mk = model.darcy_keyword, model.fourier_keyword, model.stress_keyword
-    data = _own_data(mdg.subdomain_data(sd), [fk, tk, mk])
+    data = _own_data(model.mdg.subdomain_data(sd), [fk, tk, mk])
     fluid = _fluid(model, True)
     w, we = _boundary_weights(model, sd, fluid, True)
     ff, ef = model.bc_type_fluid_flux(sd), model.bc_type_enthalpy_flux(sd)
-    so = model.solid
-    solid = dict(reference_porosity=so.porosity, biot_coefficient=_evaluated(model, model.biot_coefficient([sd]), nc),
-                 bulk_modulus=float(np.atleast_1d(_evaluated(model, model.bulk_modulus([sd]), 1))[0]),
-                 thermal_expansion=so.thermal_expansion, heat_capacity=so.specific_heat_capacity,
-                 conductivity=so.thermal_conductivity, density=so.density)
     prm = data[PARAMETERS]
+    g, sources = _tpsa_mechanics(model, sd)
     prob = TpsaThermoporomechanics(
-        sd, data, fluid, solid,
+        sd, data, fluid, _tpsa_solid(model, sd, True),
         _face_values(model, sd, prm[fk]["bc"], model.bc_values_pressure, model.bc_values_darcy_flux),
         _face_values(model, sd, prm[tk]["bc"], model.bc_values_temperature, model.bc_values_fourier_flux),
-        _evaluated(model, model.combine_boundary_operators_mechanical_stress([sd]), nd * nf), ff,
-        _face_values(model, sd, ff, w, model.bc_values_fluid_flux), ef,
-        _face_values(model, sd, ef, we, model.bc_values_enthalpy_flux),
-        body_force=_evaluated(model, model.body_force([sd]), nd * nc),
-        angular_source=_evaluated(model, model.source_angular_momentum([sd]), nr * nc),
-        mass_source=_evaluated(model, model.solid_mass_source([sd]), nc),
-        fluid_source=_evaluated(model, model.fluid_source([sd]), nc), flow_keyword=fk, fourier_keyword=tk,
+        g, ff, _face_values(model, sd, ff, w, model.bc_values_fluid_flux), ef,
+        _face_values(model, sd, ef, we, model.bc_values_enthalpy_flux), **sources,
+        fluid_source=_evaluated(model, model.fluid_source([sd]), sd.num_cells), flow_keyword=fk, fourier_keyword=tk,
         mechanics_keyword=mk)
     prob.mobility_keyword, prob.enthalpy_upwind_keyword = "b200_mobility", "b200_enthalpy_upwind"
-    cols = [_dofs(model, name, sd) for name in (model.displacement_variable, model.rotation_stress_variable,
-                                                 model.total_pressure_variable, model.pressure_variable,
-                                                 model.temperature_variable)]
-    solid_mass = [eq for eq in es.equations if eq.lower().startswith("solid_mass_equation")][0]
-    rows = _row_map(model, BlockLayout([("momentum_balance_equation", [(("matrix",), nc, nd)]),
-                                        ("angular_momentum_balance_equation", [(("matrix",), nc, nr)]),
-                                        (solid_mass, [(("matrix",), nc, 1)]),
-                                        ("mass_balance_equation", [(("matrix",), nc, 1)]),
-                                        ("energy_balance_equation", [(("matrix",), nc, 1)])]))
-    prob.column_map = interleave(cols, nd, nr, nc)
-    o = np.cumsum([0, nd * nc, nr * nc, nc, nc, nc])
-    prob.row_map = interleave([rows[o[i]:o[i + 1]] for i in range(5)], nd, nr, nc)
-    return prob, prob.column_map, prob.row_map
+    return (prob, *_tpsa_maps(model, prob, {("matrix",): sd}))
 
 
 def tpsa_fractured_momentum_from_model(model):
@@ -540,18 +518,13 @@ def tpsa_fractured_momentum_from_model(model):
     evaluated; the body force and the angular and solid-mass sources are its own operators, evaluated."""
     from .contact import FractureContact
     from .tpsa_contact import TpsaFracturedMomentumBalance
-    from .tpsa_elasticity import interleave
-    es = model.equation_system
-    if "mass_balance_equation" in es.equations:
+    if "mass_balance_equation" in model.equation_system.equations:
         raise NotImplementedError("TpsaFracturedMomentumBalance: fractured TPSA poromechanics is not supported")
     mat, fracs, grids = _matrix_and_fractures(model)
     if getattr(mat, "periodic_face_map", None) is not None:
         raise NotImplementedError("periodic faces are not supported by porepy_b200")
     mdg = model.mdg
-    nd, nc, nf = int(mat.dim), mat.num_cells, mat.num_faces
-    nr = model.rotation_dimension()
     mk = model.stress_keyword
-    data = _own_data(mdg.subdomain_data(mat), [mk])
     contacts = []
     for j, frac in enumerate(fracs):
         intf = grids[("interface", j)]
@@ -559,19 +532,7 @@ def tpsa_fractured_momentum_from_model(model):
         contacts.append(FractureContact(intf.mortar_to_primary_avg(), intf.primary_to_mortar_int(),
                                         intf.mortar_to_secondary_avg(), intf.secondary_to_mortar_int(),
                                         sps.csr_matrix(intf.sign_of_mortar_sides(1)).diagonal(), intf.cell_volumes, rot))
-    prob = TpsaFracturedMomentumBalance(
-        mat, data, _evaluated(model, model.combine_boundary_operators_mechanical_stress([mat]), nd * nf), contacts,
-        _contact_constants(model, fracs), body_force=_evaluated(model, model.body_force([mat]), nd * nc),
-        angular_source=_evaluated(model, model.source_angular_momentum([mat]), nr * nc),
-        mass_source=_evaluated(model, model.solid_mass_source([mat]), nc), keyword=mk)
-    cols = [_dofs(model, name, mat) for name in (model.displacement_variable, model.rotation_stress_variable,
-                                                  model.total_pressure_variable)]
-    tail = BlockLayout(prob.unknown_layout.blocks[1:])
-    solid_mass = [eq for eq in es.equations if eq.lower().startswith("solid_mass_equation")][0]
-    rows = _row_map(model, BlockLayout([("momentum_balance_equation", [(("matrix",), nc, nd)]),
-                                        ("angular_momentum_balance_equation", [(("matrix",), nc, nr)]),
-                                        (solid_mass, [(("matrix",), nc, 1)])] + prob.equation_layout.blocks[1:]))
-    o = np.cumsum([0, nd * nc, nr * nc, nc])
-    prob.column_map = np.concatenate([interleave(cols, nd, nr, nc), _column_map(model, tail, grids)])
-    prob.row_map = np.concatenate([interleave([rows[o[i]:o[i + 1]] for i in range(3)], nd, nr, nc), rows[o[3]:]])
-    return prob, prob.column_map, prob.row_map
+    g, sources = _tpsa_mechanics(model, mat)
+    prob = TpsaFracturedMomentumBalance(mat, _own_data(mdg.subdomain_data(mat), [mk]), g, contacts,
+                                        _contact_constants(model, fracs), **sources, keyword=mk)
+    return (prob, *_tpsa_maps(model, prob, grids))

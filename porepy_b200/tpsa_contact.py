@@ -7,7 +7,7 @@ and the solid-mass flux.
 Unknowns: [u_c, r_c, p_c per matrix cell (cell by cell, as in ``TpsaElasticity``) | t (contact traction, nd per fracture
 cell, local frame, scaled by the characteristic traction) | u_j (nd per mortar cell)]; equations, in the same blocks:
 
-* ``three_field_balance``               momentum, angular momentum and solid mass of ``TpsaElasticity`` per cell, with
+* ``cell_balances``                     momentum, angular momentum and solid mass of ``TpsaElasticity`` per cell, with
                                         the u_j columns of the cell's fracture faces
 * ``interface_force_balance_equation``  Pi^int (n_out . sigma) + vol S Pi^int R^T t T_c,
                                         sigma = S_u u + S_r r + S_p p + B_s (g + Pi^avg u_j)
@@ -26,12 +26,11 @@ from types import SimpleNamespace
 import numpy as np
 import scipy.sparse as sps
 
-from . import ad, fv, krylov
+from . import ad, krylov
 from .contact import (block_groups, contact_laws, contact_operators, fracture_parts, interface_parts,
                       matrix_dimension)
-from .layout import BlockLayout, LayoutModel
-from .newton import newton_loop
-from .params import PARAMETERS
+from .layout import BlockLayout
+from .tpsa_elasticity import TpsaNewtonProblem
 
 
 def _one_per_row(m, what: str):
@@ -47,54 +46,31 @@ def _one_per_row(m, what: str):
     return m.indices.astype(np.int64), np.asarray(m.data, float)
 
 
-class TpsaFracturedMomentumBalance(LayoutModel):
+class TpsaFracturedMomentumBalance(TpsaNewtonProblem):
     """``sd``: the 2-D or 3-D matrix grid (faces split along the fractures); ``data``: ``parameters[keyword]`` with the
     ``fourth_order_tensor`` (``mu``, ``lmbda``) and the vectorial ``bc`` of ``pp.Tpsa`` (fracture faces Dirichlet);
     ``bc_values``: the combined mechanical boundary operator, nd per face, face-major; ``fractures``: ``FractureContact``
     per fracture; ``constants``: as for ``FracturedMomentumBalance``; ``body_force`` (nd per cell), ``angular_source``
     (nr per cell), ``mass_source`` (one per cell): cell-major, integrated over the cells (None: zero)."""
 
+    bridge = "tpsa_fractured_momentum_from_model"
+    outside_pattern = "contact Jacobian entries outside the TPSA contact row pattern"
+
     def __init__(self, sd, data: dict, bc_values, fractures, constants: dict, body_force=None, angular_source=None,
                  mass_source=None, keyword: str = "mechanics"):
-        self.nd = nd = matrix_dimension(sd)
-        self.nr = 3 if nd == 3 else 1
-        self.block_size = B = nd + self.nr + 1
-        self.sd, self.data, self.kw = sd, data, keyword
-        self.nc, self.nf = int(sd.num_cells), int(sd.num_faces)
-        self.fractures = list(fractures)
+        nd = matrix_dimension(sd)        # its refusal, ahead of the one of ``TpsaProblem``
+        fr = self.fractures = list(fractures)
+        laws = [("contact_traction", fracture_parts(fr, nd)), ("interface_displacement", interface_parts(fr, nd))]
+        eqs = [("normal_fracture_deformation_equation", fracture_parts(fr, 1)),
+               ("tangential_fracture_deformation_equation", fracture_parts(fr, nd - 1))]
+        super().__init__(sd, data, keyword, bc_values, body_force, angular_source, mass_source, unknowns=laws,
+                         equations=[("interface_force_balance_equation", interface_parts(fr, nd))] + eqs)
         for f in self.fractures:
             if f.nd != nd:
                 raise ValueError(f"a fracture with {f.nd}-D local coordinates in a {nd}-D matrix")
         self.k = SimpleNamespace(**{k: float(v) for k, v in constants.items()})
-        vec = TpsaFracturedMomentumBalance._vector
-        self.bc_values = vec(bc_values, nd * self.nf, "bc_values")
-        self.body_force = vec(body_force, nd * self.nc, "body_force")
-        self.angular_source = vec(angular_source, self.nr * self.nc, "angular_source")
-        self.mass_source = vec(mass_source, self.nc, "mass_source")
-        fr, mat = self.fractures, [(("matrix",), self.nc, B)]
-        laws = [("contact_traction", fracture_parts(fr, nd)), ("interface_displacement", interface_parts(fr, nd))]
-        self.unknown_layout = BlockLayout([("three_field", mat)] + laws)
-        eqs = [("normal_fracture_deformation_equation", fracture_parts(fr, 1)),
-               ("tangential_fracture_deformation_equation", fracture_parts(fr, nd - 1))]
-        self.equation_layout = BlockLayout([("three_field_balance", mat),
-                                            ("interface_force_balance_equation", interface_parts(fr, nd))] + eqs)
         self._law_unknowns, self._law_equations = BlockLayout(laws), BlockLayout(eqs)
-        self.column_map = None
-        self.row_map = None
-        self.A = None
-        self._fg = None
         self._ops = None
-        self._missing = None
-        self.last_timing: dict = {}
-
-    @staticmethod
-    def _vector(v, n: int, name: str):
-        if v is None:
-            return None
-        v = np.ascontiguousarray(v, dtype=np.float64).reshape(-1)
-        if v.size != n:
-            raise ValueError(f"{name} must have {n} values, got {v.size}")
-        return v
 
     def interfaces(self):
         """(per mortar cell: ``face``, ``cell``, ``m2p``, ``p2m``, ``sign``, ``volume``; the frames, nd x nd per fracture
@@ -127,29 +103,14 @@ class TpsaFracturedMomentumBalance(LayoutModel):
         cat = {k: np.concatenate(v) if v else np.zeros(0) for k, v in out.items()}
         return cat, (np.concatenate(frames) if frames else np.zeros(0))
 
-    def discretize(self) -> None:
-        """The TPSA face terms, the balance and force rows of the Jacobian and their -R(0) on the device."""
-        import time
-        sd, nd = self.sd, self.nd
-        if getattr(sd, "periodic_face_map", None) is not None:
-            raise NotImplementedError("periodic faces are not supported by porepy_b200")
-        params = self.data[PARAMETERS][self.kw]
-        C = params["fourth_order_tensor"]
-        codes, robin = fv.tpsa_bc_arrays(params["bc"], nd, self.nf)
-        if nd == 2 and np.any(np.abs(sd.face_normals[2]) > np.maximum(np.abs(sd.face_normals[0]),
-                                                                       np.abs(sd.face_normals[1]))):
-            raise IndexError("Tpsa: a face normal of a 2d grid points mostly out of the xy-plane")
-        flags = np.zeros(self.nf, np.uint8)
-        flags[np.asarray(sd.get_all_boundary_faces(), dtype=np.int64)] = 1
+    def _system(self, C, codes, robin, flags):
         mortars, frames = self.interfaces()
-        t0 = time.perf_counter()
-        if self._fg is None:
-            self._fg = fv.FaceGrid.for_grid(sd)
-        self.A, stage_ms = self._fg.tpsa_contact_system(nd, C.mu, C.lmbda, sd.cell_volumes, codes, robin, flags,
-                                                        sd.face_areas, mortars, frames, self.k.characteristic_traction)
-        self.b0 = self._fg.tpsa_contact_rhs(self.num_dofs, self.bc_values, self.body_force, self.angular_source,
-                                            self.mass_source)
-        self.last_timing = dict(face_terms_ms=stage_ms[0], rows_ms=stage_ms[1], total_s=time.perf_counter() - t0)
+        return self._fg.tpsa_contact_system(self.nd, C.mu, C.lmbda, self.sd.cell_volumes, codes, robin, flags,
+                                            self.sd.face_areas, mortars, frames, self.k.characteristic_traction)
+
+    def _rhs(self):
+        return self._fg.tpsa_contact_rhs(self.num_dofs, self.bc_values, self.body_force, self.angular_source,
+                                         self.mass_source)
 
     def _operators(self):
         if self._ops is None:
@@ -174,30 +135,21 @@ class TpsaFracturedMomentumBalance(LayoutModel):
 
     # ``preconditioner_groups()``: the B x B cell block per matrix cell; the laws of fracture cell k and the force
     # balances of its mortar cells m1, m2 <-> t_k, u_j of m1, m2
-    matrix_group = ([("three_field_balance", "c")], [("three_field", "c")])
+    matrix_group = ([("cell_balances", "c")], [("cell_fields", "c")])
     fracture_group = ([("normal_fracture_deformation_equation", "k"), ("tangential_fracture_deformation_equation", "k"),
                        ("interface_force_balance_equation", "m1"), ("interface_force_balance_equation", "m2")],
                       [("contact_traction", "k"), ("interface_displacement", "m1"), ("interface_displacement", "m2")])
     preconditioner_groups = block_groups
 
-    def linearize(self, x, x_prev):
-        """(J as ``DeviceCsr``, -R as a CUDA tensor) at the iterate ``x`` (previous time step ``x_prev``): -R of the
-        linear rows is b0 - A x, the contact rows come from the AD chain, written into the fixed pattern.  ``J`` is the
-        problem's own matrix, overwritten by the next call."""
-        import torch
-        if self.A is None:
-            self.discretize()
-        x = ad.device_vector(x)
-        if x.numel() != self.num_dofs:
-            raise ValueError(f"x must have {self.num_dofs} values")
-        rhs = self.b0 - (self.A @ x)
+    def _iterate_rows(self, x, x_prev):
+        """The rows ``linearize(x, x_prev)`` writes (``x_prev``: the previous time step): the contact laws from the
+        AD chain; none without fractures."""
         if not self.fractures:
-            return self.A, rhs
-        jac, neg_res = ad.assemble(self.contact_equations(x, x_prev))
-        if self._missing is None:
-            self._missing = torch.zeros(1, dtype=torch.int32, device=rhs.device)
+            return None
+        return ad.assemble(self.contact_equations(x, x_prev))
+
+    def _write_rows(self, jac, neg_res, rhs):
         self._fg.tpsa_contact_rows(self.A, jac, neg_res, rhs, self._missing)
-        return self.A, rhs
 
     def time_step(self, x_prev, linear_solver=None, x0=None, tol: float = 1e-10, max_iterations: int = 30,
                   verbose: bool = False):
@@ -208,26 +160,6 @@ class TpsaFracturedMomentumBalance(LayoutModel):
         such grids pass ``krylov.gmres_solver(prob.preconditioner_groups(), maxiter=...)``.  Returns (x, history)."""
         x_prev = ad.device_vector(x_prev)
         x0 = x_prev if x0 is None else ad.device_vector(x0)
-
-        def linearize(x):
-            J, rhs = self.linearize(x, x_prev)
-            if self._missing is not None and int(self._missing.sum()):
-                raise RuntimeError("contact Jacobian entries outside the TPSA contact row pattern")
-            return J, rhs
         if linear_solver is None:
             linear_solver = krylov.gmres_solver(self.preconditioner_groups())
-        return newton_loop(linearize, x0, linear_solver, tol, max_iterations, verbose)
-
-    def to_model_order(self, A, b=None):
-        """A (scipy) and b permuted to the rows / columns of the model's ``EquationSystem``."""
-        if self.column_map is None or self.row_map is None:
-            raise ValueError("no dof maps: build the problem with model_bridge.tpsa_fractured_momentum_from_model")
-        n = self.num_dofs
-        P = sps.csr_matrix((np.ones(n), (self.row_map, np.arange(n))), shape=(n, n))
-        Q = sps.csr_matrix((np.ones(n), (np.arange(n), self.column_map)), shape=(n, n))
-        Am = (P @ sps.csr_matrix(A) @ Q).tocsr()
-        if b is None:
-            return Am
-        bm = np.empty(n)
-        bm[self.row_map] = np.asarray(b)
-        return Am, bm
+        return self._newton(lambda x: self.linearize(x, x_prev), x0, linear_solver, tol, max_iterations, verbose)

@@ -22,16 +22,18 @@ from the iterate's Darcy flux in front of every linearization (models/solution_s
 """
 from __future__ import annotations
 
+import time
+
 import numpy as np
 import scipy.sparse as sps
 
-from . import ad, fv, krylov
+from . import ad, krylov
 from .advection import advective_flux, rediscretize_upwind
-from .newton import newton_loop
 from .params import DISCRETIZATION_MATRICES, PARAMETERS
+from .tpsa_elasticity import TpsaNewtonProblem
 
 
-class TpsaPoromechanics:
+class TpsaPoromechanics(TpsaNewtonProblem):
     """``data``: PorePy-style dictionary with ``parameters[flow_keyword]`` (``second_order_tensor``, ``bc``) and
     ``parameters[mechanics_keyword]`` (``fourth_order_tensor`` with ``mu`` / ``lmbda``, the ``bc`` of ``pp.Tpsa``).
     ``fluid``: ``compressibility, density, viscosity, reference_pressure``; ``solid``: ``reference_porosity,
@@ -41,21 +43,17 @@ class TpsaPoromechanics:
     zero): ``body_force`` (nd per cell), ``angular_source`` (nr), ``mass_source`` (solid mass), ``fluid_source``."""
 
     mobility_keyword = "mobility"
-    # the FaceGrid entry points of this system and what its balance rows are called in errors
-    _fg_system, _fg_rhs, _fg_rows = "tpsa_poro_system", "tpsa_poro_rhs", "tpsa_poro_fluid_rows"
-    _rows_name = "fluid Jacobian entries outside the TPSA poromechanics row pattern"
+    scalar_fields = ("total_pressure", "pressure")
+    scalar_balances = ("solid_mass_equation", "mass_balance_equation")
+    bridge = "tpsa_poromechanics_from_model"
+    outside_pattern = "fluid Jacobian entries outside the TPSA poromechanics row pattern"
 
     def __init__(self, sd, data: dict, fluid: dict, solid: dict, flow_bc_values, mech_bc_values, bc_fluid_flux,
                  fluid_flux_values, body_force=None, angular_source=None, mass_source=None, fluid_source=None,
                  flow_keyword: str = "flow", mechanics_keyword: str = "mechanics") -> None:
-        self.nd = int(sd.dim)
-        if self.nd not in (2, 3):
-            raise NotImplementedError("Tpsa is only implemented for 2d and 3d grids.")
-        self.sd, self.data = sd, data
-        self.fk, self.mk = flow_keyword, mechanics_keyword
-        self.nr = 3 if self.nd == 3 else 1
-        self.block_size = self.nd + self.nr + 2
-        self.nc, self.nf = int(sd.num_cells), int(sd.num_faces)
+        super().__init__(sd, data, mechanics_keyword, mech_bc_values, body_force, angular_source, mass_source,
+                         bc_name="mech_bc_values")
+        self.fk = flow_keyword
         self.c, self.rho0, self.mu_f = (float(fluid[k]) for k in ("compressibility", "density", "viscosity"))
         self.p_ref = float(fluid.get("reference_pressure", 0.0))
         if not all(np.isfinite(v) and v > 0 for v in (self.c, self.rho0, self.mu_f)):
@@ -66,66 +64,40 @@ class TpsaPoromechanics:
             raise ValueError("Biot coefficient alpha must be finite")
         self.alpha = np.ascontiguousarray(alpha)
         self.n_inv = (self.alpha - self.phi_ref) * (1.0 - self.alpha) / float(solid["bulk_modulus"])
-        nc, nf, nd = self.nc, self.nf, self.nd
+        nc, nf = self.nc, self.nf
         self.flow_bc = self._vector(flow_bc_values, nf, "flow_bc_values")
-        self.mech_bc = self._vector(mech_bc_values, nd * nf, "mech_bc_values")
         self.bc_fluid_flux = bc_fluid_flux
         self.ff_values = self._vector(fluid_flux_values, nf, "fluid_flux_values")
-        self.body_force = self._vector(body_force, nd * nc, "body_force")
-        self.angular_source = self._vector(angular_source, self.nr * nc, "angular_source")
-        self.mass_source = self._vector(mass_source, nc, "mass_source")
         self.fluid_source = self._vector(fluid_source, nc, "fluid_source")
         if self.fluid_source is None:
             self.fluid_source = np.zeros(nc)
-        self.column_map = None
-        self.row_map = None
-        self.A = None
-        self._fg = None
         self._const = None
-        self.last_timing: dict = {}
-
-    @staticmethod
-    def _vector(v, n: int, name: str):
-        if v is None:
-            return None
-        v = np.ascontiguousarray(v, dtype=np.float64).reshape(-1)
-        if v.size != n:
-            raise ValueError(f"{name} must have {n} values, got {v.size}")
-        return v
 
     @property
-    def num_dofs(self) -> int:
-        return self.block_size * self.nc
+    def mech_bc(self):
+        """``mech_bc_values``: the combined mechanical boundary operator."""
+        return self.bc_values
 
-    def discretize(self) -> None:
-        """MPFA of the flow, the TPSA face terms and the mechanics rows of the Jacobian (device), the fluid-row pattern
-        from div @ flux, and -R(0) of the mechanics rows."""
-        import time
-        sd, nd = self.sd, self.nd
-        if getattr(sd, "periodic_face_map", None) is not None:
-            raise NotImplementedError("periodic faces are not supported by porepy_b200")
-        params = self.data[PARAMETERS][self.mk]
-        C = params["fourth_order_tensor"]
-        codes, robin = fv.tpsa_bc_arrays(params["bc"], nd, self.nf)
-        if nd == 2 and np.any(np.abs(sd.face_normals[2]) > np.maximum(np.abs(sd.face_normals[0]),
-                                                                       np.abs(sd.face_normals[1]))):
-            raise IndexError("Tpsa: a face normal of a 2d grid points mostly out of the xy-plane")
-        flags = np.zeros(self.nf, np.uint8)
-        flags[np.asarray(sd.get_all_boundary_faces(), dtype=np.int64)] = 1
+    def _system(self, C, codes, robin, flags):
+        """MPFA of the flow, then the TPSA face terms and the mechanics rows of the Jacobian (device) with the
+        balance-row pattern from div @ flux."""
         t0 = time.perf_counter()
         self._discretize_fluxes()
-        t1 = time.perf_counter()
+        self.last_timing["mpfa_s"] = time.perf_counter() - t0
         self._const = None
-        k = self._operands()
-        if self._fg is None:
-            self._fg = fv.FaceGrid.for_grid(sd)
         self.lmbda = np.asarray(C.lmbda, float)
-        self.A, stage_ms = getattr(self._fg, self._fg_system)(nd, C.mu, self.lmbda, self.alpha, sd.cell_volumes, codes,
-                                                              robin, flags, sd.face_areas, self._balance_pattern(k))
-        self.b0 = getattr(self._fg, self._fg_rhs)(self.num_dofs, self.mech_bc, self.body_force, self.angular_source,
-                                                  self.mass_source)
-        self.last_timing = dict(mpfa_s=t1 - t0, face_terms_ms=stage_ms[0], rows_ms=stage_ms[1],
-                                total_s=time.perf_counter() - t0)
+        return self._mechanics_rows(C.mu, codes, robin, flags, self._balance_pattern(self._operands()))
+
+    def _mechanics_rows(self, mu, codes, robin, flags, pattern):
+        return self._fg.tpsa_poro_system(self.nd, mu, self.lmbda, self.alpha, self.sd.cell_volumes, codes, robin,
+                                         flags, self.sd.face_areas, pattern)
+
+    def _rhs(self):
+        return self._fg.tpsa_poro_rhs(self.num_dofs, self.bc_values, self.body_force, self.angular_source,
+                                      self.mass_source)
+
+    def _write_rows(self, jac, neg_res, rhs):
+        self._fg.tpsa_poro_fluid_rows(self.A, jac, neg_res, rhs, self._missing)
 
     def _discretize_fluxes(self) -> None:
         from .fv import Mpfa
@@ -141,7 +113,7 @@ class TpsaPoromechanics:
             csr, dev = ad.as_device_csr, ad.device_vector
             F = self.data[DISCRETIZATION_MATRICES][self.fk]
             vol = np.asarray(self.sd.cell_volumes, float)
-            lam = np.asarray(self.data[PARAMETERS][self.mk]["fourth_order_tensor"].lmbda, float)
+            lam = np.asarray(self.data[PARAMETERS][self.keyword]["fourth_order_tensor"].lmbda, float)
             k = SimpleNamespace(div=csr(sps.csr_matrix(self.sd.cell_faces.T)), flux=csr(F["flux"]), vol=dev(vol),
                                 bcw=dev(self.ff_values), src=dev(self.fluid_source), a_lam=dev(self.alpha / lam),
                                 alpha=dev(self.alpha), n_inv=dev(self.n_inv))
@@ -157,9 +129,10 @@ class TpsaPoromechanics:
         return (p - self.p_ref) * k.n_inv + (pt + p * k.alpha) * k.a_lam + self.phi_ref
 
     def _fields(self, x):
-        """(p_t, p) of a cell-interleaved vector, as contiguous device vectors (the scalar fields after r_c)."""
+        """The ``scalar_fields`` of a cell-interleaved vector (the unknowns behind r_c), as contiguous device
+        vectors."""
         x = ad.device_vector(x).reshape(self.nc, self.block_size)
-        return tuple(x[:, j].contiguous() for j in range(self.nd + self.nr, self.block_size))
+        return tuple(x[:, j].contiguous() for j in range(self.block_size - len(self.scalar_fields), self.block_size))
 
     def update_upwind(self, p) -> None:
         k = self._operands()
@@ -184,60 +157,17 @@ class TpsaPoromechanics:
         eq = self.fluid_equation(x, x_prev, dt)
         return eq.jac, -eq.val
 
-    def linearize(self, x, x_prev, dt: float):
-        """(J as ``DeviceCsr``, -R as a CUDA tensor) in the cell-interleaved order: upwind directions from ``x``, the
-        fluid rows from the AD chain written into the fixed pattern, -R of the mechanics rows = b0 - A x.  ``J`` is
-        the problem's own matrix, overwritten by the next call."""
-        import torch
-        if self.A is None:
-            self.discretize()
-        x = ad.device_vector(x)
-        if x.numel() != self.num_dofs:
-            raise ValueError(f"x must have {self.num_dofs} values")
+    def _iterate_rows(self, x, x_prev, dt: float):
+        """The rows ``linearize(x, x_prev, dt)`` writes: upwind directions from ``x``, then ``balance_rows``."""
         self.update_upwind(self._fields(x)[1])
-        jac, neg_res = self.balance_rows(x, x_prev, dt)
-        rhs = self.b0 - (self.A @ x)
-        if getattr(self, "_missing", None) is None:
-            self._missing = torch.zeros(1, dtype=torch.int32, device=rhs.device)
-        getattr(self._fg, self._fg_rows)(self.A, jac, neg_res, rhs, self._missing)
-        return self.A, rhs
+        return self.balance_rows(x, x_prev, dt)
 
     def time_step(self, x_prev, dt: float, tol: float = 1e-10, max_iterations: int = 15, linear_tol: float = 1e-10,
                   linear_solver=None, verbose: bool = False):
         """One implicit time step by Newton's method.  ``linear_solver(J, rhs) -> dx`` overrides the device
         block-Jacobi BiCGStab (one inverted cell block per cell).  Returns (x, history)."""
         x_prev = ad.device_vector(x_prev)
-
-        def linearize(x):
-            J, rhs = self.linearize(x, x_prev, dt)
-            if int(self._missing.sum()):
-                raise RuntimeError(self._rows_name)
-            return J, rhs
         if linear_solver is None:
             linear_solver = krylov.bicgstab_solver(linear_tol, block_size=self.block_size)
-        return newton_loop(linearize, x_prev, linear_solver, tol, max_iterations, verbose)
-
-    def to_model_order(self, A, b=None):
-        """A (scipy) and b permuted to the rows / columns of the model's ``EquationSystem``."""
-        if self.column_map is None or self.row_map is None:
-            raise ValueError("no dof maps: build the problem with model_bridge.tpsa_poromechanics_from_model")
-        n = self.num_dofs
-        P = sps.csr_matrix((np.ones(n), (self.row_map, np.arange(n))), shape=(n, n))
-        Q = sps.csr_matrix((np.ones(n), (np.arange(n), self.column_map)), shape=(n, n))
-        Am = (P @ sps.csr_matrix(A) @ Q).tocsr()
-        if b is None:
-            return Am
-        bm = np.empty(n)
-        bm[self.row_map] = np.asarray(b)
-        return Am, bm
-
-
-def interleave(blocks, nd: int, nr: int, nc: int) -> np.ndarray:
-    """Cell-interleaved order [u_c, r_c, p_t_c, p_c] (or [u_c, r_c, p_t_c, p_c, T_c]) from the field-wise index arrays."""
-    u, r, *scalars = (np.asarray(x, np.int64) for x in blocks)
-    out = np.empty((nc, nd + nr + len(scalars)), np.int64)
-    out[:, :nd] = u.reshape(nc, nd)
-    out[:, nd:nd + nr] = r.reshape(nc, nr)
-    for j, v in enumerate(scalars):
-        out[:, nd + nr + j] = v
-    return out.reshape(-1)
+        return self._newton(lambda x: self.linearize(x, x_prev, dt), x_prev, linear_solver, tol, max_iterations,
+                            verbose)

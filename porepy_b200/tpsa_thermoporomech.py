@@ -42,7 +42,7 @@ from .advection import advective_flux, rediscretize_upwind
 from .fv import Mpfa
 from .params import DISCRETIZATION_MATRICES, PARAMETERS, SecondOrderTensor
 from .thermoporomech import Thermoporomechanics
-from .tpsa_poromech import TpsaPoromechanics, interleave  # noqa: F401  (interleave: the bridge's dof order)
+from .tpsa_poromech import TpsaPoromechanics
 
 
 class TpsaThermoporomechanics(TpsaPoromechanics):
@@ -54,8 +54,10 @@ class TpsaThermoporomechanics(TpsaPoromechanics):
     ``conductivity``: the cell conductivities of the Fourier flux (None: phi k_f + (1 - phi) k_s at the zero state)."""
 
     enthalpy_upwind_keyword = "enthalpy_upwind"
-    _fg_system, _fg_rhs, _fg_rows = "tpsa_thm_system", "tpsa_thm_rhs", "tpsa_thm_balance_rows"
-    _rows_name = "mass or energy Jacobian entries outside the TPSA thermo-poromechanics row pattern"
+    scalar_fields = TpsaPoromechanics.scalar_fields + ("temperature",)
+    scalar_balances = TpsaPoromechanics.scalar_balances + ("energy_balance_equation",)
+    bridge = "tpsa_thermoporomechanics_from_model"
+    outside_pattern = "mass or energy Jacobian entries outside the TPSA thermo-poromechanics row pattern"
 
     # the density and internal energy of the MPSA thermo-poromechanics model
     _density = Thermoporomechanics._density
@@ -69,7 +71,6 @@ class TpsaThermoporomechanics(TpsaPoromechanics):
                          body_force=body_force, angular_source=angular_source, mass_source=mass_source,
                          fluid_source=fluid_source, flow_keyword=flow_keyword, mechanics_keyword=mechanics_keyword)
         self.tk = fourier_keyword
-        self.block_size = self.nd + self.nr + 3
         self.fl = SimpleNamespace(**{k: float(v) for k, v in fluid.items()})
         self.fl.reference_pressure = self.p_ref
         self.fl.reference_temperature = float(fluid.get("reference_temperature", 0.0))
@@ -95,6 +96,17 @@ class TpsaThermoporomechanics(TpsaPoromechanics):
         self.conductivity = np.ascontiguousarray(np.broadcast_to(np.asarray(conductivity, float), (self.nc,)))
         if not np.all(np.isfinite(self.conductivity) & (self.conductivity > 0)):
             raise ValueError("the Fourier conductivity must be finite and > 0")
+
+    def _mechanics_rows(self, mu, codes, robin, flags, pattern):
+        return self._fg.tpsa_thm_system(self.nd, mu, self.lmbda, self.alpha, self.sd.cell_volumes, codes, robin,
+                                        flags, self.sd.face_areas, pattern)
+
+    def _rhs(self):
+        return self._fg.tpsa_thm_rhs(self.num_dofs, self.bc_values, self.body_force, self.angular_source,
+                                     self.mass_source)
+
+    def _write_rows(self, jac, neg_res, rhs):
+        self._fg.tpsa_thm_balance_rows(self.A, jac, neg_res, rhs, self._missing)
 
     def _discretize_fluxes(self) -> None:
         super()._discretize_fluxes()

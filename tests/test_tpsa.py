@@ -12,6 +12,7 @@ import scipy.sparse as sps
 import porepy_b200 as pb
 from porepy_b200 import fv
 from golden_io import case_names, load_case, rel_err
+from tpsa_checks import full_size_mechanics, use_host_build
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, os.path.join(ROOT, "tools"))
@@ -27,8 +28,7 @@ TOL = 1e-12
 
 @pytest.fixture()
 def host_build(monkeypatch):
-    from emu_tpsa import EmuTpsaFaceGrid
-    monkeypatch.setattr(fv, "FaceGrid", EmuTpsaFaceGrid)
+    use_host_build(monkeypatch, plan=False, sparse=False)
 
 
 def _discretize(c):
@@ -129,12 +129,11 @@ def test_ndof_and_keys():
 @pytest.mark.gpu
 @pytest.mark.parametrize("name", CASES)
 def test_gpu_matches_reference_and_host_build(name, monkeypatch):
-    from emu_tpsa import EmuTpsaFaceGrid
     c = load_case(name)
     got = _discretize(c)
     _assert_matches(c.mats, got)
     with monkeypatch.context() as m:
-        m.setattr(fv, "FaceGrid", EmuTpsaFaceGrid)
+        use_host_build(m, plan=False, sparse=False)
         host = _discretize(load_case(name))
     for key in KEYS:   # same routine, the device build contracts some products into FMAs
         a, b = host[key], got[key]
@@ -152,31 +151,6 @@ def test_gpu_refuses_bad_shear_modulus():
         pb.Tpsa("mech").discretize(g, data)
 
 
-def _full_size_problem():
-    g = pb.structured_tet_grid((55, 55, 55))
-    nf, nd = g.num_faces, 3
-    bf = g.get_all_boundary_faces()
-    xf = g.face_centers[:, bf]
-    bc = pb.BoundaryConditionVectorial(g)
-    west = bf[xf[0] < 1e-10]
-    south = bf[(xf[1] < 1e-10) & (xf[0] > 1e-10)]
-    top = bf[(xf[2] > 1 - 1e-10) & (xf[0] > 1e-10) & (xf[1] > 1e-10)]
-    bc.is_dir[:, west] = True
-    bc.is_neu[:, west] = False
-    bc.is_dir[1, south] = True          # roller
-    bc.is_neu[1, south] = False
-    bc.is_rob[:, top] = True
-    bc.is_neu[:, top] = False
-    rng = np.random.default_rng(7)
-    w = np.zeros((nd, nd, nf))
-    for i in range(nd):
-        w[i, i] = 0.2 + 5 * rng.random(nf)
-    bc.robin_weight = w
-    mu = np.exp(rng.standard_normal(g.num_cells))
-    mu[g.cell_centers[0] < 0.3] *= 1e6
-    return g, bc, mu
-
-
 @pytest.mark.gpu
 @pytest.mark.skipif(not reference_available(), reason="oracle/_ref not present (run oracle/make_ref.sh)")
 def test_full_size_matches_reference():
@@ -184,7 +158,7 @@ def test_full_size_matches_reference():
     reference's run on the same host arrays."""
     from oracle.ref_loader import reference_grid
     pp = load_porepy()
-    g, bc, mu = _full_size_problem()
+    g, bc, mu = full_size_mechanics()
     assert g.num_cells == 998_250
     data = pb.initialize_data({}, "mech", {"fourth_order_tensor": pb.FourthOrderTensor(mu, np.ones_like(mu)),
                                            "bc": bc})
@@ -286,10 +260,8 @@ MODELS = [("momentum", 2), ("momentum", 3), ("poromechanics", 2)]
 @pytest.mark.skipif(not reference_available(), reason="reference tree not present")
 @pytest.mark.parametrize("family,nd", MODELS)
 def test_models_through_the_plugin_host_build(family, nd, monkeypatch):
-    from emu_binding import EmuBackedPlan, emu_interface_upwind_masks
-    from emu_tpsa import EmuTpsaFaceGrid
-    monkeypatch.setattr(fv, "DevicePlan", EmuBackedPlan)
-    monkeypatch.setattr(fv, "FaceGrid", EmuTpsaFaceGrid)
+    from emu_binding import emu_interface_upwind_masks
+    use_host_build(monkeypatch, sparse=False)
     monkeypatch.setattr(fv, "interface_upwind_masks", emu_interface_upwind_masks)
     _check_models(load_porepy(), family, nd)
 

@@ -3,7 +3,8 @@
 ``pp.MomentumBalance`` + ``TpsaMomentumBalanceMixin``: Jacobian and -R at the zero state and at the stored iterate, the
 residual histories and converged states of the sliding, sticking, open and mixed loads in 3-D and 2-D (fixtures of
 tools/make_tpsa_contact_golden.py), live stock models with two fractures through the bridge, the refusals, the grouped
-block-Jacobi GMRES on every fixture Jacobian and the register use of the new kernels.
+block-Jacobi GMRES on every fixture Jacobian.  The checks shared with the other TPSA systems are those of
+tpsa_checks.py.
 CPU: host build of tpsa_system.cuh + the scipy stand-in for the device sparse algebra."""
 import os
 import sys
@@ -15,10 +16,11 @@ import scipy.sparse as sps
 import scipy.sparse.linalg as spla
 
 import porepy_b200 as pb
-from porepy_b200 import fv
 from porepy_b200.contact import FractureContact
 from porepy_b200.tpsa_contact import TpsaFracturedMomentumBalance
 from golden_io import case_names
+from tpsa_checks import (ZERO, check_bridge_linearization, check_linearizations, compare_with_host_build, csr, direct,
+                         host, to_model, to_solver, use_host_build)
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, os.path.join(ROOT, "tools"))
@@ -27,14 +29,6 @@ from ref_loader import load_porepy, reference_available  # noqa: E402
 CASES = case_names("tpsacontact_")
 CONSTANTS = ("numerical_constant", "characteristic_traction", "friction_coefficient", "dilation_angle", "reference_gap",
              "open_state_tolerance")
-
-
-def _csr(d, key):
-    return sps.csr_matrix((d[key + "__data"], d[key + "__indices"], d[key + "__indptr"]), shape=tuple(d[key + "__shape"]))
-
-
-def _host(t):
-    return t.cpu().numpy() if hasattr(t, "cpu") else np.asarray(t)
 
 
 def _problem(name, fractures=None):
@@ -47,9 +41,9 @@ def _problem(name, fractures=None):
     data = pb.initialize_data({}, "mechanics", {"fourth_order_tensor": pb.FourthOrderTensor(d["mu"], d["lmbda"]),
                                                 "bc": bc})
     if fractures is None:
-        fractures = [FractureContact(_csr(d, "mortar_to_primary_avg"), _csr(d, "primary_to_mortar_int"),
-                                     _csr(d, "mortar_to_secondary_avg"), _csr(d, "secondary_to_mortar_int"),
-                                     d["mortar_sign"], d["mortar_volumes"], _csr(d, "local_coordinates"))]
+        fractures = [FractureContact(csr(d, "mortar_to_primary_avg"), csr(d, "primary_to_mortar_int"),
+                                     csr(d, "mortar_to_secondary_avg"), csr(d, "secondary_to_mortar_int"),
+                                     d["mortar_sign"], d["mortar_volumes"], csr(d, "local_coordinates"))]
     prob = TpsaFracturedMomentumBalance(g, data, d["bc_values"], fractures, {k: float(d[k]) for k in CONSTANTS},
                                         body_force=d["body_force"], angular_source=d["angular_source"],
                                         mass_source=d["mass_source"])
@@ -57,30 +51,11 @@ def _problem(name, fractures=None):
     return prob, d
 
 
-def _solver_order(prob, x):
-    return np.asarray(x)[prob.column_map]
-
-
-def _direct(J, rhs):
-    import torch
-    dx = spla.spsolve(J.to_scipy().tocsc(), _host(rhs))
-    return torch.as_tensor(dx, device=rhs.device) if hasattr(rhs, "device") else dx
-
-
-def check_linearizations(prob, d, tol):
-    prob.discretize()
-    got = []
-    for x, xp, jk, rk in ((d["previous"], d["previous"], "J0", "rhs0"),
-                          (d["iterate"], d["previous"], "iterate_jacobian", "iterate_rhs")):
-        J, rhs = prob.linearize(_solver_order(prob, x), _solver_order(prob, xp))
-        Jm, bm = prob.to_model_order(J.to_scipy(), _host(rhs))
-        Jr, br = _csr(d, jk), d[rk]
-        assert abs(Jm - Jr).max() <= tol * abs(Jr).max(), jk
-        # the stored iterate of the sticking case is converged: -R is compared on the scale of -R(0)
-        assert np.abs(bm - br).max() <= tol * np.abs(d["rhs0"]).max(), rk
-        got.append((J.to_scipy(), _host(rhs).copy()))
-    assert int(prob._missing.sum()) == 0
-    return got
+def _linearizations(prob, d):
+    # the stored iterate of the sticking case is converged: -R is compared on the scale of -R(0)
+    return check_linearizations(prob, d, [("zero", d["previous"], d["previous"], "J0", "rhs0"),
+                                          ("iterate", d["iterate"], d["previous"], "iterate_jacobian", "iterate_rhs")],
+                                1e-12, ZERO)
 
 
 def check_time_step(prob, d, tol, linear_solver):
@@ -88,13 +63,11 @@ def check_time_step(prob, d, tol, linear_solver):
     stored iterate for the two steps it pins: after that the tangential jump is zero up to round-off and sign(u_t),
     the Jacobian of |u_t|, is decided by round-off on either side (as test_models_2d explains), so later steps of the
     two semismooth loops may take different, equally converging paths."""
-    prev, ref = _solver_order(prob, d["previous"]), d["residual_norms"]
+    prev, ref = to_solver(prob, d["previous"]), d["residual_norms"]
     x, hist = prob.time_step(prev, linear_solver, tol=1e-14)       # to round-off, as the stored state
     assert abs(hist[0]["residual"] - ref[0]) <= tol * ref[0]
-    xm = np.empty(prob.num_dofs)
-    xm[prob.column_map] = _host(x)
-    assert np.linalg.norm(xm - d["solution"]) <= tol * np.linalg.norm(d["solution"]), hist
-    _, hist = prob.time_step(prev, linear_solver, x0=_solver_order(prob, d["iterate"]), tol=1e-11)
+    assert np.linalg.norm(to_model(prob, x) - d["solution"]) <= tol * np.linalg.norm(d["solution"]), hist
+    _, hist = prob.time_step(prev, linear_solver, x0=to_solver(prob, d["iterate"]), tol=1e-11)
     mine = np.array([h["residual"] for h in hist])
     n = min(len(mine), len(ref) - 1, 2)
     assert np.abs(mine[:n] - ref[1:1 + n]).max() <= tol * ref[0], (mine, ref)
@@ -102,12 +75,7 @@ def check_time_step(prob, d, tol, linear_solver):
 
 @pytest.fixture()
 def host_build(monkeypatch):
-    import emu_sparse
-    from emu_binding import EmuBackedPlan
-    from emu_tpsa import EmuTpsaFaceGrid
-    monkeypatch.setattr(fv, "DevicePlan", EmuBackedPlan)
-    monkeypatch.setattr(fv, "FaceGrid", EmuTpsaFaceGrid)
-    emu_sparse.install(monkeypatch)
+    use_host_build(monkeypatch)
 
 
 def test_fixtures_present():
@@ -118,8 +86,8 @@ def test_fixtures_present():
 @pytest.mark.parametrize("name", CASES)
 def test_host_build_matches_reference(name, host_build):
     prob, d = _problem(name)
-    check_linearizations(prob, d, 1e-12)
-    check_time_step(prob, d, 1e-10, _direct)
+    _linearizations(prob, d)
+    check_time_step(prob, d, 1e-10, direct)
 
 
 @pytest.mark.parametrize("name", CASES)
@@ -130,8 +98,8 @@ def test_gmres_with_groups_converges_on_fixture_jacobians(name, host_build):
     groups = prob.preconditioner_groups()
     rows, cols, ptr = np.asarray(groups.rows), np.asarray(groups.cols), np.asarray(groups.ptr)
     for x in (d["previous"], d["iterate"]):
-        J, rhs = prob.linearize(_solver_order(prob, x), _solver_order(prob, d["previous"]))
-        A, b = J.to_scipy().tocsr(), _host(rhs)
+        J, rhs = prob.linearize(to_solver(prob, x), to_solver(prob, d["previous"]))
+        A, b = J.to_scipy().tocsr(), host(rhs)
         inv = [np.linalg.inv(A[rows[ptr[q]:ptr[q + 1]]][:, cols[ptr[q]:ptr[q + 1]]].toarray())
                for q in range(len(ptr) - 1)]
 
@@ -145,27 +113,27 @@ def test_gmres_with_groups_converges_on_fixture_jacobians(name, host_build):
         assert info == 0 and np.linalg.norm(A @ y - b) <= 1e-9 * np.linalg.norm(b)
 
 
-def _refusals(host):
+def _refusals():
     prob, d = _problem(CASES[0])
     fc = prob.fractures[0]
     # a mortar cell on two faces (non-matching mortar grid)
-    m2p = _csr(d, "mortar_to_primary_avg").tolil()
-    f0, f1 = np.flatnonzero(_csr(d, "mortar_to_primary_avg")[:, 0].toarray().ravel())[0], 0
+    m2p = csr(d, "mortar_to_primary_avg").tolil()
+    f0, f1 = np.flatnonzero(csr(d, "mortar_to_primary_avg")[:, 0].toarray().ravel())[0], 0
     m2p[f1, 0] = 0.5
-    bad = FractureContact(m2p.tocsr(), _csr(d, "primary_to_mortar_int"), _csr(d, "mortar_to_secondary_avg"),
-                          _csr(d, "secondary_to_mortar_int"), d["mortar_sign"], d["mortar_volumes"],
-                          _csr(d, "local_coordinates"))
+    bad = FractureContact(m2p.tocsr(), csr(d, "primary_to_mortar_int"), csr(d, "mortar_to_secondary_avg"),
+                          csr(d, "secondary_to_mortar_int"), d["mortar_sign"], d["mortar_volumes"],
+                          csr(d, "local_coordinates"))
     with pytest.raises(ValueError, match="matching mortar grids"):
         _problem(CASES[0], [bad])[0].discretize()
     # two mortar cells on one face
-    p2m = _csr(d, "primary_to_mortar_int").tolil()
-    m2p = _csr(d, "mortar_to_primary_avg").tolil()
+    p2m = csr(d, "primary_to_mortar_int").tolil()
+    m2p = csr(d, "mortar_to_primary_avg").tolil()
     g0 = int(np.flatnonzero(m2p[:, 0].toarray().ravel())[0])
     g1 = int(np.flatnonzero(m2p[:, 1].toarray().ravel())[0])
     m2p[g1, 1], m2p[g0, 1], p2m[1, g1], p2m[1, g0] = 0.0, 1.0, 0.0, 1.0
-    bad = FractureContact(m2p.tocsr(), p2m.tocsr(), _csr(d, "mortar_to_secondary_avg"),
-                          _csr(d, "secondary_to_mortar_int"), d["mortar_sign"], d["mortar_volumes"],
-                          _csr(d, "local_coordinates"))
+    bad = FractureContact(m2p.tocsr(), p2m.tocsr(), csr(d, "mortar_to_secondary_avg"),
+                          csr(d, "secondary_to_mortar_int"), d["mortar_sign"], d["mortar_volumes"],
+                          csr(d, "local_coordinates"))
     with pytest.raises(ValueError, match="more than one mortar cell"):
         _problem(CASES[0], [bad])[0].discretize()
     assert f0 >= 0 and fc.num_mortar == 2 * fc.num_cells
@@ -184,7 +152,7 @@ def _refusals(host):
 
 
 def test_refusals_host(host_build):
-    _refusals(True)
+    _refusals()
     from porepy_b200 import model_bridge
     fake = SimpleNamespace(equation_system=SimpleNamespace(equations={"mass_balance_equation": None}))
     with pytest.raises(NotImplementedError, match="fractured TPSA poromechanics"):
@@ -283,17 +251,11 @@ def _check_bridge(nd, solve=False):
     es = m.equation_system
     prob, cols, rows = plugin(pp).tpsa_fractured_momentum_from_model(m)
     assert len(prob.fractures) == 2 and prob.num_dofs == es.num_dofs()
-    assert np.array_equal(np.sort(cols), np.arange(es.num_dofs())) and np.array_equal(np.sort(rows),
-                                                                                       np.arange(es.num_dofs()))
-    J, rhs = es.assemble()
-    x, xp = es.get_variable_values(iterate_index=0), es.get_variable_values(time_step_index=0)
-    A, b = prob.linearize(x[cols], xp[cols])
-    Am, bm = prob.to_model_order(A.to_scipy(), _host(b))
-    assert abs(Am - J).max() <= 1e-12 * abs(J).max()
-    assert np.abs(bm - rhs).max() <= 1e-12 * np.abs(rhs).max()
+    check_bridge_linearization(m, prob, cols, rows)
     with pytest.raises(NotImplementedError, match="fractures are not supported"):
         plugin(pp).tpsa_momentum_from_model(m)
     if solve:                                        # the device problem reaches the reference's own state
+        xp = es.get_variable_values(time_step_index=0)
         es.set_variable_values(xp, iterate_index=0)
         m.before_nonlinear_loop()
         for _ in range(30):                          # the reference's own semismooth Newton loop
@@ -303,9 +265,9 @@ def _check_bridge(nd, solve=False):
                 break
             m.after_nonlinear_iteration(m.solve_linear_system())
         xr = es.get_variable_values(iterate_index=0)
-        xd, hist = prob.time_step(xp[cols], _direct, tol=1e-11)
+        xd, hist = prob.time_step(xp[cols], direct, tol=1e-11)
         assert hist[-1]["residual"] <= 1e-10 * hist[0]["residual"], hist
-        assert np.linalg.norm(_host(xd) - xr[cols]) <= 1e-8 * np.linalg.norm(xr), hist
+        assert np.linalg.norm(host(xd) - xr[cols]) <= 1e-8 * np.linalg.norm(xr), hist
 
 
 @pytest.mark.skipif(not reference_available(), reason="reference tree not present")
@@ -319,28 +281,15 @@ def test_bridge_host_build(nd, host_build):
 
 @pytest.mark.gpu
 @pytest.mark.parametrize("name", CASES)
-def test_gpu_matches_reference_and_host_build(name, monkeypatch):
+def test_gpu_matches_reference_and_host_build(name):
     prob, d = _problem(name)
-    dev = check_linearizations(prob, d, 1e-12)
-    dev2 = check_linearizations(prob, d, 1e-12)                  # a second assembly: bit-identical
+    dev = _linearizations(prob, d)
+    dev2 = _linearizations(prob, d)                              # a second assembly: bit-identical
     for (A, b), (A2, b2) in zip(dev, dev2):
         assert np.array_equal(A.indptr, A2.indptr) and np.array_equal(A.indices, A2.indices)
         assert np.array_equal(A.data, A2.data) and np.array_equal(b, b2)
-    check_time_step(prob, d, 1e-10, _direct)
-    with monkeypatch.context() as mp:
-        import emu_sparse
-        from emu_binding import EmuBackedPlan
-        from emu_tpsa import EmuTpsaFaceGrid
-        mp.setattr(fv, "DevicePlan", EmuBackedPlan)
-        mp.setattr(fv, "FaceGrid", EmuTpsaFaceGrid)
-        emu_sparse.install(mp)
-        ph, _ = _problem(name)
-        host = check_linearizations(ph, d, 1e-12)
-    rscale = np.abs(host[0][1]).max()
-    for (A, b), (Ah, bh) in zip(dev, host):
-        assert np.array_equal(A.indptr, Ah.indptr) and np.array_equal(A.indices, Ah.indices)
-        assert abs(A - Ah).max() <= 1e-13 * abs(Ah).max()
-        assert np.abs(b - bh).max() <= 1e-13 * rscale
+    check_time_step(prob, d, 1e-10, direct)
+    compare_with_host_build(lambda: _linearizations(*_problem(name)), dev, same_pattern=True)
 
 
 @pytest.mark.gpu
@@ -373,17 +322,15 @@ def test_gpu_time_step_with_device_gmres(name, monkeypatch):
     def refuse(self):
         raise AssertionError("to_scipy inside the Newton loop")
     monkeypatch.setattr(DeviceCsr, "to_scipy", refuse)
-    x, hist = prob.time_step(_solver_order(prob, d["previous"]), tol=1e-14)
+    x, hist = prob.time_step(to_solver(prob, d["previous"]), tol=1e-14)
     monkeypatch.undo()
-    xm = np.empty(prob.num_dofs)
-    xm[prob.column_map] = _host(x)
-    assert np.linalg.norm(xm - d["solution"]) <= 1e-10 * np.linalg.norm(d["solution"]), hist
+    assert np.linalg.norm(to_model(prob, x) - d["solution"]) <= 1e-10 * np.linalg.norm(d["solution"]), hist
 
 
 @pytest.mark.gpu
 def test_gpu_refusals():
     import torch
-    _refusals(False)
+    _refusals()
     prob, d = _problem(CASES[0])
     prob.discretize()
     fg, nk = prob._fg, prob.fractures[0].num_cells

@@ -1,11 +1,10 @@
 """The TPSA three-field elasticity system (``pb_tpsa_system`` / ``pb_tpsa_rhs``, csrc/tpsa_system.cuh,
 ``porepy_b200.TpsaElasticity``): the host build and the GPU against a scipy restatement of the model equations and
 against the unmodified reference model's Jacobian and right-hand side (fixtures of tools/make_tpsa_model_golden.py),
-the block-Jacobi BiCGStab solve, the 4 x 4 and 7 x 7 block inverses, the refusals, and the bench-size mesh."""
+the block-Jacobi BiCGStab solve, the refusals and the bench-size mesh; the block-diagonal inverses of every TPSA block
+size (4 to 9), and the register use of every TPSA kernel of face.cu and of the 6 x 6 and 9 x 9 Krylov kernels."""
 import os
 import re
-import shutil
-import subprocess
 import sys
 from types import SimpleNamespace
 
@@ -15,8 +14,10 @@ import scipy.sparse as sps
 
 import porepy_b200 as pb
 from porepy_b200 import fv
-from porepy_b200.tpsa_elasticity import TpsaElasticity, interleave
+from porepy_b200.tpsa_elasticity import TpsaElasticity
 from golden_io import case_names, load_case
+from tpsa_checks import (check_model_order, check_single_grid_refusals, compare_with_host_build, csr, field_order,
+                         field_ordered_reference, full_size_problem, host, ptxas_properties, to_model, use_host_build)
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, os.path.join(ROOT, "tools"))
@@ -28,44 +29,47 @@ MODEL_CASES = case_names("tpsa_model_")
 
 @pytest.fixture()
 def host_build(monkeypatch):
-    from emu_tpsa import EmuTpsaFaceGrid
-    monkeypatch.setattr(fv, "FaceGrid", EmuTpsaFaceGrid)
+    use_host_build(monkeypatch, plan=False, sparse=False)
 
 
-def _nr(nd):
-    return 3 if nd == 3 else 1
+def _divergences(prob):
+    div = sps.csr_matrix(prob.sd.cell_faces).T.tocsr()
+    return div, sps.kron(div, sps.eye(prob.nd)).tocsr(), sps.kron(div, sps.eye(prob.nr)).tocsr()
 
 
-def _field_order(nd, nc):
-    """For each cell-interleaved index, the index in the field-wise order [u | r | p]."""
-    nr = _nr(nd)
-    return interleave([np.arange(nd * nc), nd * nc + np.arange(nr * nc), (nd + nr) * nc + np.arange(nc)], nd, nr, nc)
+def _restated_rhs(prob, mats):
+    """b of the three equations of ``prob`` from its inputs and the TPSA boundary matrices with scipy, in the
+    cell-interleaved order."""
+    div, dn, dr = _divergences(prob)
+    M = {k: sps.csr_matrix(mats[k]) for k in ("bound_stress", "bound_rotation_displacement", "bound_mass_displacement")}
+    bcv = prob.bc_values
+    b = np.concatenate([dn @ (M["bound_stress"] @ bcv) + prob.body_force,
+                        -(dr @ (M["bound_rotation_displacement"] @ bcv)) + prob.angular_source,
+                        -(div @ (M["bound_mass_displacement"] @ bcv)) + prob.mass_source])
+    return b[field_order(prob)]
 
 
-def _restated(g, mats, mu, lam, bcv, f, sr, sp):
-    """A and b of the three equations from the 14 TPSA matrices with scipy, in the cell-interleaved order."""
-    nd, nc = g.dim, g.num_cells
-    nr = _nr(nd)
-    div = sps.csr_matrix(g.cell_faces).T.tocsr()
-    dn, dr = sps.kron(div, sps.eye(nd)).tocsr(), sps.kron(div, sps.eye(nr)).tocsr()
-    vol = g.cell_volumes
+def _restated(prob, mats):
+    """A and b of the three equations of ``prob`` from its inputs and the 14 TPSA matrices with scipy, in the
+    cell-interleaved order."""
+    div, dn, dr = _divergences(prob)
+    vol = prob.sd.cell_volumes
+    C = prob.data[pb.PARAMETERS][prob.keyword]["fourth_order_tensor"]
     M = {k: sps.csr_matrix(v) for k, v in mats.items()}
     A = sps.bmat([[-dn @ M["stress"], -dn @ M["stress_rotation"], -dn @ M["stress_total_pressure"]],
-                  [dr @ M["rotation_displacement"], dr @ M["rotation_rotation"] - sps.diags(np.repeat(vol / mu, nr)),
-                   None],
+                  [dr @ M["rotation_displacement"],
+                   dr @ M["rotation_rotation"] - sps.diags(np.repeat(vol / C.mu, prob.nr)), None],
                   [div @ M["solid_mass_displacement"], None,
-                   div @ M["solid_mass_total_pressure"] - sps.diags(vol / lam)]]).tocsr()
-    b = np.concatenate([dn @ (M["bound_stress"] @ bcv) + f, -(dr @ (M["bound_rotation_displacement"] @ bcv)) + sr,
-                        -(div @ (M["bound_mass_displacement"] @ bcv)) + sp])
-    perm = _field_order(nd, nc)
-    return A[perm][:, perm].tocsr(), b[perm]
+                   div @ M["solid_mass_total_pressure"] - sps.diags(vol / C.lmbda)]]).tocsr()
+    perm = field_order(prob)
+    return A[perm][:, perm].tocsr(), _restated_rhs(prob, mats)
 
 
 def _seeded_inputs(g, seed):
     nd, nc, nf = g.dim, g.num_cells, g.num_faces
     rng = np.random.default_rng(seed)
     lam = np.exp(rng.standard_normal(nc))
-    return (lam, rng.standard_normal(nd * nf), rng.standard_normal(nd * nc), rng.standard_normal(_nr(nd) * nc),
+    return (lam, rng.standard_normal(nd * nf), rng.standard_normal(nd * nc), rng.standard_normal((3 if nd == 3 else 1) * nc),
             rng.standard_normal(nc))
 
 
@@ -81,10 +85,6 @@ def _problem(c, lam=None, bcv=None, f=None, sr=None, sp=None):
     return TpsaElasticity(c.g, data, "mech", bcv, f, sr, sp)
 
 
-def _host(x):
-    return x.cpu().numpy() if hasattr(x, "cpu") else np.asarray(x)
-
-
 def _scipy(A):
     return A.to_scipy() if hasattr(A, "to_scipy") else sps.csr_matrix(A)
 
@@ -96,11 +96,11 @@ def _check_restatement(name, tol):
     lam, bcv, f, sr, sp = _seeded_inputs(c.g, 11)
     prob = _problem(c, lam, bcv, f, sr, sp)
     A, b = prob.assemble()
-    A, b = _scipy(A), _host(b)
+    A, b = _scipy(A), host(b)
     C = pb.FourthOrderTensor(c.raw["mu"], lam)
     data = pb.initialize_data({}, "mech", {"fourth_order_tensor": C, "bc": c.bc})
     pb.Tpsa("mech").discretize(c.g, data)
-    Ar, br = _restated(c.g, data[pb.DISCRETIZATION_MATRICES]["mech"], c.raw["mu"], lam, bcv, f, sr, sp)
+    Ar, br = _restated(prob, data[pb.DISCRETIZATION_MATRICES]["mech"])
     assert A.shape == Ar.shape
     nd = c.g.dim
     assert A.nnz == (37 if nd == 3 else 12) * (c.g.num_cells + 2 * int((np.diff(sps.csr_matrix(c.g.cell_faces).indptr)
@@ -115,8 +115,8 @@ def _check_model(name, tol):
     prob = _problem(c)
     prob.column_map, prob.row_map = d["column_map"], d["row_map"]
     A, b = prob.assemble()
-    Am, bm = prob.to_model_order(_scipy(A), _host(b))
-    J = sps.csr_matrix((d["J__data"], d["J__indices"], d["J__indptr"]), shape=tuple(d["J__shape"]))
+    Am, bm = prob.to_model_order(_scipy(A), host(b))
+    J = csr(d, "J")
     assert abs(Am - J).max() <= tol * abs(J).max(), name
     assert np.abs(bm - d["rhs"]).max() <= tol * np.abs(d["rhs"]).max(), name
 
@@ -149,18 +149,8 @@ def test_refusals_host():
     with pytest.raises(ValueError, match="no dof maps"):
         TpsaElasticity(g, {}, "mech", np.zeros(2 * g.num_faces)).to_model_order(sps.eye(4 * g.num_cells))
     from porepy_b200 import model_bridge
-    sd = SimpleNamespace(dim=2)
-    fake = SimpleNamespace(nd=2, mdg=SimpleNamespace(subdomains=lambda: [sd, sd], interfaces=lambda: []),
-                           equation_system=SimpleNamespace(equations={}))
-    with pytest.raises(NotImplementedError, match="one subdomain"):
-        model_bridge.tpsa_momentum_from_model(fake)
-    fake.mdg = SimpleNamespace(subdomains=lambda: [sd, SimpleNamespace(dim=1)], interfaces=lambda: [])
-    with pytest.raises(NotImplementedError, match="fractures"):
-        model_bridge.tpsa_momentum_from_model(fake)
-    fake.mdg = SimpleNamespace(subdomains=lambda: [sd], interfaces=lambda: [])
-    fake.equation_system = SimpleNamespace(equations={"mass_balance_equation": None})
-    with pytest.raises(NotImplementedError, match="poromechanics"):
-        model_bridge.tpsa_momentum_from_model(fake)
+    check_single_grid_refusals(model_bridge.tpsa_momentum_from_model, model_bridge.tpsa_momentum_from_model,
+                               ["mass_balance_equation"], "poromechanics")
 
 
 # ---- the stock model through the plugin's bridge -----------------------------------------------------------------
@@ -209,19 +199,22 @@ def _stock_model(pp, nd):
     return m
 
 
-@pytest.mark.skipif(not reference_available(), reason="reference tree not present")
-@pytest.mark.parametrize("nd", [2, 3])
-def test_bridge_host_build(nd, host_build):
+def _check_bridge(nd):
+    """The stock model through ``tpsa_momentum_from_model``: A and b equal the model's own Jacobian and right-hand
+    side.  Returns the problem, the model's Jacobian and right-hand side."""
     from porepy_b200.porepy_plugin import plugin
     pp = load_porepy()
     m = _stock_model(pp, nd)
     prob, cols, rows = plugin(pp).tpsa_momentum_from_model(m)
     J, rhs = m.equation_system.assemble()
-    A, b = prob.assemble()
-    Am, bm = prob.to_model_order(A, b)
-    assert abs(Am - J).max() <= 1e-12 * abs(J).max()
-    assert np.abs(bm - rhs).max() <= 1e-12 * np.abs(rhs).max()
-    assert np.array_equal(np.sort(cols), np.arange(J.shape[1])) and np.array_equal(np.sort(rows), np.arange(J.shape[0]))
+    check_model_order(prob, *prob.assemble(), J, rhs, cols, rows)
+    return prob, J, rhs
+
+
+@pytest.mark.skipif(not reference_available(), reason="reference tree not present")
+@pytest.mark.parametrize("nd", [2, 3])
+def test_bridge_host_build(nd, host_build):
+    _check_bridge(nd)
 
 
 @pytest.mark.skipif(not reference_available(), reason="reference tree not present")
@@ -238,7 +231,7 @@ def test_bridge_refuses_tpsa_poromechanics():
         model_bridge.tpsa_momentum_from_model(m)
 
 
-# ---- register use of every TPSA kernel of face.cu (compile only) --------------------------------------------------
+# ---- register use (compile only) ----------------------------------------------------------------------------------
 
 _ND = ["<2>", "<3>"]
 _ND_NS = [f"<{nd}, {ns}>" for nd in (2, 3) for ns in (1, 2)]
@@ -252,29 +245,15 @@ TPSA_KERNELS = {
 }
 # the kernels that enumerate the face neighbours of a cell hold them in a kTpsaMaxNb = 32 int32 array on the stack
 NB_STACK = {"tpsa_nb_count_kernel": 128, "tpsa_nb_list_kernel": 128}
-
-
-def _kernel_name(mangled):
-    """'stem<a, b>' of an Itanium-mangled kernel whose template arguments are ints ('_Z<len><stem>ILi2ELi1EE...')."""
-    m = re.match(r"_Z(\d+)", mangled)
-    n = int(m.group(1))
-    stem, rest = mangled[m.end():m.end() + n], mangled[m.end() + n:]
-    args = re.match(r"I((?:Li-?\d+E)+)E", rest)
-    return stem + (f"<{', '.join(re.findall(r'Li(-?\d+)E', args.group(1)))}>" if args else "")
+# the block sizes of the thermo-poromechanics systems (6 in 2-D, 9 in 3-D)
+KRYLOV_KERNELS = re.compile(r"(block_diag_inv_inplace|kry_[ps])_kernel<[69]>")
 
 
 def test_tpsa_kernels_do_not_spill(tmp_path):
-    nvcc = os.environ.get("NVCC") or shutil.which("nvcc") or "/usr/local/cuda/bin/nvcc"
-    if not os.path.exists(nvcc):
-        pytest.skip("nvcc not available")
-    out = subprocess.run([nvcc, "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-std=c++17", "-Xptxas", "-v",
-                          "-I", os.path.join(ROOT, "include"), "-c", os.path.join(ROOT, "porepy_b200", "csrc", "face.cu"),
-                          "-o", str(tmp_path / "face.o")], capture_output=True, text=True, check=True)
     seen = set()
-    for fn, props in re.findall(r"Function properties for (\S+)\n\s*(.*)", out.stderr):
-        if "tpsa" not in fn:
+    for name, props in ptxas_properties("face.cu", tmp_path).items():
+        if "tpsa" not in name:
             continue
-        name = _kernel_name(fn)
         seen.add(name)
         stack = NB_STACK.get(name, 0)
         assert props.startswith(f"{stack} bytes stack frame, 0 bytes spill stores, 0 bytes spill loads"), (name, props)
@@ -282,24 +261,27 @@ def test_tpsa_kernels_do_not_spill(tmp_path):
     assert want <= seen, sorted(want - seen)
 
 
+def test_krylov_kernels_do_not_spill(tmp_path):
+    seen = []
+    for name, props in ptxas_properties("krylov.cu", tmp_path).items():
+        if KRYLOV_KERNELS.fullmatch(name):
+            seen.append(name)
+            assert props.startswith("0 bytes stack frame, 0 bytes spill stores, 0 bytes spill loads"), (name, props)
+    assert len(seen) == 6, seen
+
+
 # ---- GPU ----------------------------------------------------------------------------------------------------------
 
 
 @pytest.mark.gpu
 @pytest.mark.parametrize("name", CASES)
-def test_gpu_matches_restatement_and_host_build(name, monkeypatch):
-    from emu_tpsa import EmuTpsaFaceGrid
+def test_gpu_matches_restatement_and_host_build(name):
     _check_restatement(name, 1e-13)
     c = load_case(name)
-    lam, bcv, f, sr, sp = _seeded_inputs(c.g, 11)
-    A, b = _problem(c, lam, bcv, f, sr, sp).assemble()
-    A, b = A.to_scipy(), b.cpu().numpy()
-    with monkeypatch.context() as mp:
-        mp.setattr(fv, "FaceGrid", EmuTpsaFaceGrid)
-        Ah, bh = _problem(load_case(name), lam, bcv, f, sr, sp).assemble()
-    assert np.array_equal(A.indptr, Ah.indptr) and np.array_equal(A.indices, Ah.indices)
-    assert np.abs(A.data - Ah.data).max() <= 1e-13 * np.abs(Ah.data).max()
-    assert np.abs(b - bh).max() <= 1e-13 * np.abs(bh).max()
+    inputs = _seeded_inputs(c.g, 11)
+    A, b = _problem(c, *inputs).assemble()
+    compare_with_host_build(lambda: [_problem(load_case(name), *inputs).assemble()], [(A.to_scipy(), host(b))],
+                            same_pattern=True, plan=False, sparse=False)
 
 
 @pytest.mark.gpu
@@ -318,11 +300,9 @@ def test_gpu_solve_matches_reference_solution(name):
     x, info = prob.solve(tol=1e-12, maxiter=5000)
     assert info["converged"] and info.get("fused"), info
     A, b = prob.assemble()
-    A, b, x = A.to_scipy(), b.cpu().numpy(), x.cpu().numpy()
-    assert np.linalg.norm(b - A @ x) <= 1e-11 * np.linalg.norm(b)
-    xm = np.empty_like(x)
-    xm[prob.column_map] = x
-    assert np.linalg.norm(xm - d["solution"]) <= 1e-8 * np.linalg.norm(d["solution"])
+    A, b = A.to_scipy(), b.cpu().numpy()
+    assert np.linalg.norm(b - A @ host(x)) <= 1e-11 * np.linalg.norm(b)
+    assert np.linalg.norm(to_model(prob, x) - d["solution"]) <= 1e-8 * np.linalg.norm(d["solution"])
 
 
 @pytest.mark.gpu
@@ -369,18 +349,22 @@ def _blocks_csr(blocks, noise, rng):
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize("bs", [4, 7])
-def test_gpu_block_inverse_4_and_7(bs):
+@pytest.mark.parametrize("bs", [4, 5, 6, 7, 8, 9])
+def test_gpu_block_inverse(bs):
+    """The block-diagonal inverse of every TPSA block size (elasticity 4 / 7, poromechanics 5 / 8, thermo-poromechanics
+    6 / 9) against numpy, with blocks that need a pivot swap at some or every step and a singular block."""
     rng = np.random.default_rng(bs)
-    nb = 200
+    nb = 300
     blocks = rng.standard_normal((nb, bs, bs)) + 3 * bs * np.eye(bs)
-    blocks[5, 0, 0] = 0.0                                   # pivoting needed, still regular
+    blocks[5, 0, 0] = 0.0                                    # pivoting needed, still regular
+    blocks[6] = blocks[6][rng.permutation(bs)]                # every row swapped
+    blocks[8] = blocks[8][::-1]                               # anti-diagonal dominant: a swap at every step
     A = pb.DeviceCsr(_blocks_csr(blocks, 0.7, rng))
     got = A.block_diagonal_inverse(bs).cpu().numpy().reshape(nb, bs, bs)
     want = np.linalg.inv(blocks)
     assert np.abs(got - want).max() <= 1e-12 * np.abs(want).max()
     sing = blocks.copy()
-    sing[7, 1, :] = 0.0                                     # singular block: inverse of its diagonal, 1 where it is 0
+    sing[7, 1, :] = 0.0                                      # singular block: inverse of its diagonal, 1 where it is 0
     sing[7, 2, :] = sing[7, 3, :]
     got = pb.DeviceCsr(_blocks_csr(sing, 0.7, rng)).block_diagonal_inverse(bs).cpu().numpy().reshape(nb, bs, bs)
     dg = np.diagonal(sing[7])
@@ -390,20 +374,13 @@ def test_gpu_block_inverse_4_and_7(bs):
 
 @pytest.mark.gpu
 def test_gpu_full_size_matches_device_ad_assembly():
-    """998,250 tetrahedra with Dirichlet, roller, Robin and Neumann faces and a seeded lambda field: A and b of the new
-    kernels against the porepy_b200.ad assembly (device SpGEMM / bmat) of the same pb.Tpsa face matrices, and two
-    assemblies bit-identical."""
+    """998,250 tetrahedra with Dirichlet, roller, Robin and Neumann faces and a seeded lambda field: A of the new kernels
+    against the field-ordered porepy_b200.ad bmat assembly (device SpGEMM) of the same pb.Tpsa face matrices, b against
+    their scipy restatement, and two assemblies bit-identical."""
     import torch
-    from porepy_b200 import ad
-    from porepy_b200.sparse import DeviceCsr
-    from test_tpsa import _full_size_problem
-    g, bc, mu = _full_size_problem()
+    prob, _ = full_size_problem("elasticity", 23)
+    g = prob.sd
     assert g.num_cells == 998_250
-    nd, nc, nf, nr = 3, g.num_cells, g.num_faces, 3
-    B, n = 7, 7 * g.num_cells
-    lam, bcv, f, sr, sp = _seeded_inputs(g, 23)
-    data = pb.initialize_data({}, "mech", {"fourth_order_tensor": pb.FourthOrderTensor(mu, lam), "bc": bc})
-    prob = TpsaElasticity(g, data, "mech", bcv, f, sr, sp)
     A1, b1 = prob.assemble()
     a1 = A1.to_scipy()
     del A1
@@ -413,37 +390,13 @@ def test_gpu_full_size_matches_device_ad_assembly():
     assert np.array_equal(a1.indptr, a2.indptr) and np.array_equal(a1.indices, a2.indices)
     assert np.array_equal(a1.data, a2.data) and torch.equal(b1, b2)
     del a2, A2
-    # the same equations on the device AD chain, unknowns numbered cell by cell through the variables' Jacobians
-    pb.Tpsa("mech").discretize(g, data)
-    M = {k: ad.as_device_csr(v) for k, v in data[pb.DISCRETIZATION_MATRICES]["mech"].items()}
-    pos = np.empty(n, np.int64)
-    pos[_field_order(nd, nc)] = np.arange(n)             # field-wise dof -> cell-interleaved column
-    sizes = [nd * nc, nr * nc, nc]
-    starts = np.cumsum([0] + sizes)
-    u, r, p = (ad.DeviceAdArray(np.zeros(m), DeviceCsr(sps.csr_matrix(
-        (np.ones(m), (np.arange(m), pos[s:s + m])), shape=(m, n)))) for m, s in zip(sizes, starts))
-    div = sps.csr_matrix(g.cell_faces).T.tocsr()
-    dn, dr, d1 = (DeviceCsr(sps.kron(div, sps.eye(k)).tocsr()) for k in (nd, nr, 1))
-    vol = g.cell_volumes
-    mom = -(dn @ (M["stress"] @ u + M["stress_rotation"] @ r + M["stress_total_pressure"] @ p
-                  + torch.as_tensor(M["bound_stress"] @ bcv, device="cuda"))) - f
-    ang = (dr @ (M["rotation_displacement"] @ u + M["rotation_rotation"] @ r
-                 + torch.as_tensor(M["bound_rotation_displacement"] @ bcv, device="cuda"))
-           + r * (-np.repeat(vol / mu, nr)) - sr)
-    mass = (d1 @ (M["solid_mass_displacement"] @ u + M["solid_mass_total_pressure"] @ p
-                  + torch.as_tensor(M["bound_mass_displacement"] @ bcv, device="cuda"))
-            + p * (-vol / lam) - sp)
-    jac, rhs = ad.assemble([mom, ang, mass])
-    order = _field_order(nd, nc)
-    P = DeviceCsr(sps.csr_matrix((np.ones(n), (np.arange(n), order)), shape=(n, n)))
-    ref = P @ jac
-    del jac, mom, ang, mass
-    diff = ref.axpby(1.0, prob.A, -1.0).to_scipy()
-    scale = np.abs(a1.data).max()
-    assert np.abs(diff.data).max() <= 1e-13 * scale
-    assert a1.nnz == 37 * (nc + 2 * int((np.diff(sps.csr_matrix(g.cell_faces).indptr) == 2).sum()))
-    bref = rhs[torch.as_tensor(order, device=rhs.device)]
-    assert float((b1 - bref).abs().max()) <= 1e-13 * float(bref.abs().max())
+    pb.Tpsa("mech").discretize(g, prob.data)
+    mats = prob.data[pb.DISCRETIZATION_MATRICES]["mech"]
+    diff = field_ordered_reference(prob, mats, []).axpby(1.0, prob.A, -1.0).to_scipy()
+    assert np.abs(diff.data).max() <= 1e-13 * np.abs(a1.data).max()
+    assert a1.nnz == 37 * (g.num_cells + 2 * int((np.diff(sps.csr_matrix(g.cell_faces).indptr) == 2).sum()))
+    bref = _restated_rhs(prob, mats)
+    assert np.abs(host(b1) - bref).max() <= 1e-13 * np.abs(bref).max()
 
 
 @pytest.mark.gpu
@@ -452,19 +405,9 @@ def test_gpu_full_size_matches_device_ad_assembly():
 def test_gpu_bridge_solves_stock_model(nd):
     """The stock TPSA model through ``tpsa_momentum_from_model``: A, b equal the model's own Jacobian and right-hand
     side, and the device solve gives the model's solution."""
-    from porepy_b200.porepy_plugin import plugin
-    pp = load_porepy()
-    m = _stock_model(pp, nd)
-    prob, cols, rows = plugin(pp).tpsa_momentum_from_model(m)
-    J, rhs = m.equation_system.assemble()
-    A, b = prob.assemble()
-    Am, bm = prob.to_model_order(A.to_scipy(), b.cpu().numpy())
-    assert abs(Am - J).max() <= 1e-12 * abs(J).max()
-    assert np.abs(bm - rhs).max() <= 1e-12 * np.abs(rhs).max()
+    import scipy.sparse.linalg as spla
+    prob, J, rhs = _check_bridge(nd)
     x, info = prob.solve(tol=1e-12, maxiter=5000)
     assert info["converged"], info
-    xm = np.empty(x.numel())
-    xm[cols] = x.cpu().numpy()
-    import scipy.sparse.linalg as spla
     ref = spla.spsolve(sps.csc_matrix(J), rhs)
-    assert np.linalg.norm(xm - ref) <= 1e-8 * np.linalg.norm(ref)
+    assert np.linalg.norm(to_model(prob, x) - ref) <= 1e-8 * np.linalg.norm(ref)

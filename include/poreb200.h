@@ -290,6 +290,35 @@ int pb_dual_download(pb_dual *d, double *mass, double *proj);
 int pb_dual_system(pb_dual *d, const uint8_t *codes, const double *robin_weight, const double *face_areas,
                    const double *bc_values, const double *vector_source, pb_csr **out, double *rhs, double *norm);
 
+/* Hybridization (csrc/dual_hybrid.cuh): every cell's local saddle system is condensed exactly onto one pressure
+ * lambda per face (reference numerics/vem/hybrid.py), one warp per cell; cells of at most 32 faces (PB_ENOTIMPL).
+ * pb_dual_hybrid_system returns the nf x nf face matrix in the mass pattern (*out) and its right-hand side (rhs, nf,
+ * host); pb_dual_hybrid_recover takes lambda (nf, host) and writes [u; p] (nf + nc, host), each u_f by the face's
+ * first cell.  *kernel_ms: the per-cell kernel.  Two modes:
+ *   PB_DUAL_HYBRID_VEM: HybridDualVEM.matrix_rhs / compute_up.  Geometry as pb_dual_discretize, with perm as given
+ *     (not rotated, as hybrid.py reads it) and aperture (nc) scaling cell volumes and normals; values = [bc_values (nf);
+ *     source (nc)]; codes PB_BC_DIR / PB_BC_NEU.  Dirichlet rows are cleared with |H|_inf (before the boundary
+ *     conditions) on the diagonal and norm bc_values in rhs, Neumann faces add s bc_values area (s: the sign of the
+ *     face's first cell).  *bad_cell: as pb_dual_discretize.
+ *   PB_DUAL_HYBRID_SADDLE: the face system of the saddle point of pb_dual_system, from the values and geometry of the
+ *     last pb_dual_discretize (geometry pointers and aperture NULL); values = any right-hand side b (nf + nc) of that
+ *     system; codes and robin_weight / face_areas as pb_dual_system.  Faces with a given pressure (Dirichlet, and
+ *     boundary faces without a condition) get identity rows and zeroed columns, Robin faces add -robin_weight area on
+ *     the diagonal, Neumann faces the flux s b_f / |mass|_inf; the face right-hand side b_f enters the local system
+ *     of the face's first cell.  [u; p] then solves the saddle-point system with right-hand side b.
+ * PB_ESINGULAR: a singular local matrix (named by cell). */
+#define PB_DUAL_HYBRID_VEM 0
+#define PB_DUAL_HYBRID_SADDLE 1
+int pb_dual_hybrid_system(pb_dual *d, int mode, const double *nodes, const double *face_normals,
+                          const double *face_centers, const double *cell_centers, const double *cell_volumes,
+                          const double *perm, const double *rot, const double *aperture, const uint8_t *codes,
+                          const double *robin_weight, const double *face_areas, const double *values, pb_csr **out,
+                          double *rhs, int64_t *bad_cell, float *kernel_ms);
+int pb_dual_hybrid_recover(pb_dual *d, int mode, const double *nodes, const double *face_normals,
+                           const double *face_centers, const double *cell_centers, const double *cell_volumes,
+                           const double *perm, const double *rot, const double *aperture, const uint8_t *codes,
+                           const double *values, const double *lambda, double *up, float *kernel_ms);
+
 /* ---- two-point stress approximation (csrc/tpsa_face.cuh; reference numerics/fv/tpsa.py:376-1430) ------------------
  * One thread per face writes every value of the 14 TPSA matrices in that face's rows.  nr = nd in 3-D (the rotation
  * is a 3-vector) and nr = 1 in 2-D (a scalar).  Shapes (rows x columns) and the block of one (face, cell) entry or of

@@ -7,7 +7,7 @@ first use; there is no CPU fallback.
 from .contact import FractureContact, FracturedMomentumBalance  # noqa: F401
 from .fractured_poromech import FractureCoupling, FracturedPoromechanics  # noqa: F401
 from .fractured_thm import FracturedThermoporomechanics  # noqa: F401
-from .fv import (MVEM, RT0, Biot, DevicePlan, DualGrid, FaceGrid, Mpfa, Mpsa, Tpfa, Tpsa, Upwind, UpwindCoupling,  # noqa: F401
+from .fv import (MVEM, RT0, Biot, DevicePlan, DualGrid, FaceGrid, HybridDualVEM, Mpfa, Mpsa, Tpfa, Tpsa, Upwind, UpwindCoupling,  # noqa: F401
                  determine_eta)
 from .geometry import compute_geometry  # noqa: F401
 from .grid import Grid, cart_grid_2d, cart_grid_3d, structured_tet_grid, tet_grid_from_cells  # noqa: F401
@@ -26,7 +26,7 @@ from .tpsa_thermoporomech import TpsaThermoporomechanics  # noqa: F401
 from .tpsa_contact import TpsaFracturedMomentumBalance  # noqa: F401
 from .tpfa_ad import DifferentiableTpfa  # noqa: F401
 
-__all__ = ["Mpfa", "Mpsa", "Biot", "Tpfa", "Tpsa", "MVEM", "RT0", "DualGrid", "Upwind", "UpwindCoupling", "DevicePlan", "FaceGrid", "DeviceCsr", "Grid", "cart_grid_2d", "cart_grid_3d",
+__all__ = ["Mpfa", "Mpsa", "Biot", "Tpfa", "Tpsa", "MVEM", "RT0", "HybridDualVEM", "DualGrid", "Upwind", "UpwindCoupling", "DevicePlan", "FaceGrid", "DeviceCsr", "Grid", "cart_grid_2d", "cart_grid_3d",
            "structured_tet_grid", "tet_grid_from_cells", "SecondOrderTensor", "FourthOrderTensor",
            "BoundaryCondition", "BoundaryConditionVectorial", "initialize_data", "PARAMETERS",
            "DISCRETIZATION_MATRICES", "determine_eta", "compute_geometry", "DifferentiableTpfa",

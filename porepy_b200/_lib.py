@@ -13,6 +13,7 @@ LIB_PATH = os.path.join(HERE, "libporeb200.so")
 PB_OK, PB_EINVAL, PB_ESINGULAR, PB_ECELLTYPE, PB_ECUDA, PB_ENOTIMPL = range(6)
 BC_INTERIOR, BC_DIR, BC_NEU, BC_ROB = 0, 1, 2, 3
 DUAL_MVEM, DUAL_RT0 = 0, 1   # PB_DUAL_*
+DUAL_HYBRID_VEM, DUAL_HYBRID_SADDLE = 0, 1   # PB_DUAL_HYBRID_*
 PAT_FACE_CELL, PAT_FACE_BFACE, PAT_CELL_CELL, PAT_CELL_BFACE = 0, 1, 2, 3
 
 _i32p = C.POINTER(C.c_int32)
@@ -98,6 +99,9 @@ _SIGNATURES = {
     "pb_dual_download": (C.c_int, [C.c_void_p, _f64p, _f64p]),
     "pb_dual_system": (C.c_int, [C.c_void_p, _u8p, _f64p, _f64p, _f64p, _f64p, C.POINTER(C.c_void_p), _f64p,
                                  _f64p]),
+    "pb_dual_hybrid_system": (C.c_int, [C.c_void_p, C.c_int] + [_f64p] * 8 + [_u8p, _f64p, _f64p, _f64p,
+                                        C.POINTER(C.c_void_p), _f64p, _i64p, _f32p]),
+    "pb_dual_hybrid_recover": (C.c_int, [C.c_void_p, C.c_int] + [_f64p] * 8 + [_u8p, _f64p, _f64p, _f64p, _f32p]),
     "pb_compute_geometry_3d": (C.c_int, [C.c_int64, C.c_int64, C.c_int64, _i32p, _i32p, _i8p, _i32p, _i32p] + [_f64p] * 6
                                + [_f32p]),
     "pb_shard_create": (C.c_int, [C.c_int64, C.c_int64, C.c_int64, _i32p, _i32p, _f64p, _i32p, _i32p, _i64p, C.c_int64,

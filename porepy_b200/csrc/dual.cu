@@ -1,10 +1,10 @@
 // dual.cu -- the mixed (dual) discretizations of Darcy flow, MVEM and RT0 (dual_cell.cuh), on a handle that keeps a
-// grid's topology and the FACE x FACE mass pattern on the device.
+// grid's topology and the FACE x FACE mass pattern on the device, and their hybridization (dual_hybrid.cuh).
 #include <climits>
 #include <cstring>
 
 #include "csr_build.cuh"
-#include "dual_cell.cuh"
+#include "dual_hybrid.cuh"
 
 struct pb_csr;
 int pb_csr_from_device_pattern_(int64_t nrows, int64_t ncols, int64_t nnz, const int32_t *indptr_dev,
@@ -20,7 +20,10 @@ struct pb_dual {
     std::vector<int32_t> cf_ip_h;
     // values of the last pb_dual_discretize, kept for pb_dual_download and pb_dual_system
     bool have_values = false;
+    int method = -1;
     DevBuf mass_val, proj_val;
+    // geometry of the last pb_dual_discretize, for the hybridized solve of its saddle point
+    DevBuf geo_nodes, geo_fn, geo_fc, geo_cc, geo_vol, geo_perm, geo_rot;
     // saddle-point pattern (pb_dual_system), built at its first call
     int64_t sys_nnz = -1;
     DevBuf sys_ip, sys_ix;
@@ -169,7 +172,9 @@ extern "C" int pb_dual_discretize(pb_dual *d, int method, const double *nodes, c
         if (rc) return rc;
     }
     cudaStream_t st = d->stream;
-    DevBuf dn, dfn, dfc, dcc, dvol, dperm, drot, dbad;
+    DevBuf &dn = d->geo_nodes, &dfn = d->geo_fn, &dfc = d->geo_fc, &dcc = d->geo_cc, &dvol = d->geo_vol,
+           &dperm = d->geo_perm, &drot = d->geo_rot;
+    DevBuf dbad;
     DevBuf &dmass = d->mass_val, &dproj = d->proj_val;
     d->have_values = false;
     CUDA_TRY(dn.upload(nodes, (size_t)3 * nn, st));
@@ -217,6 +222,7 @@ extern "C" int pb_dual_discretize(pb_dual *d, int method, const double *nodes, c
     if (kernel_ms) *kernel_ms = ms;
     *bad_cell = hbad == none ? -1 : (int64_t)hbad;
     d->have_values = hbad == none;
+    d->method = method;
     return PB_OK;
 }
 
@@ -393,5 +399,261 @@ extern "C" int pb_dual_system(pb_dual *d, const uint8_t *codes, const double *ro
 #undef DS_TRY
     std::memcpy(norm, &nb, sizeof(double));
     *out = a;
+    return PB_OK;
+}
+
+// ---- hybridization (dual_hybrid.cuh): one warp per cell, lane i on local face i ----
+constexpr int kHybridWarps = 4;
+
+// The cell's local matrix, inverted in place by the Gauss-Jordan steps of group_inv_kernel (gmres.cu), then z, r and
+// lambda.  Returns false when a pivot is zero or not finite (every lane agrees).
+template <int ND, int METHOD>
+__device__ bool hybrid_cell(int64_t c, int lane, const pb::DualTopo &T, const pb::DualGeo &G, const pb::HybridIn &H,
+                            const double *lam, double *A, double *E, double *z, double *r, double *lv, int32_t *bad) {
+    const int n = T.cf_ip[c + 1] - T.cf_ip[c];
+    if (lane < n) {
+        pb::hybrid_local_row<ND>(METHOD, c, lane, T, G, H, A, bad);
+        pb::group_identity_row(E, n, lane);
+    }
+    __syncwarp();
+    for (int k = 0; k < n; ++k) {
+        const int p = pb::group_pivot(A, n, k);   // every lane finds the same pivot
+        if (p < 0) return false;
+        __syncwarp();
+        if (lane < n) pb::group_swap_col(A, E, n, k, p, lane);
+        __syncwarp();
+        if (lane < n && lane != k) pb::group_eliminate_row(A, E, n, k, lane);
+        __syncwarp();
+        if (lane == k) pb::group_scale_row(A, E, n, k);
+        __syncwarp();
+    }
+    if (lane < n) pb::hybrid_vectors(c, lane, T, H, E, lam, z, r, lv);
+    __syncwarp();
+    return true;
+}
+
+// lam == NULL: condensation into hval / rhs; else recovery of u / p.  singular: smallest cell with a singular A.
+template <int ND, int METHOD>
+__global__ void hybrid_cell_kernel(int64_t nc, pb::DualTopo T, pb::DualGeo G, pb::HybridIn H, int nmax,
+                                   const double *__restrict__ lam, double *__restrict__ hval, double *__restrict__ rhs,
+                                   double *__restrict__ u, double *__restrict__ p, int32_t *bad, int32_t *singular) {
+    extern __shared__ double sm[];
+    const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
+    double *A = sm + (size_t)wid * pb::hybrid_cell_doubles(nmax);
+    double *E = A + nmax * nmax, *z = E + nmax * nmax, *r = z + nmax, *lv = r + nmax;
+    for (int64_t c = (int64_t)blockIdx.x * kHybridWarps + wid; c < nc; c += (int64_t)gridDim.x * kHybridWarps) {
+        const int n = T.cf_ip[c + 1] - T.cf_ip[c];
+        if (!hybrid_cell<ND, METHOD>(c, lane, T, G, H, lam, A, E, z, r, lv, bad)) {
+            if (lane == 0) atomicMin(singular, (int32_t)c);
+        } else if (lane < n) {
+            if (lam) pb::hybrid_recover_row(c, lane, T, H, E, z, r, lv, u, p);
+            else pb::hybrid_condense_row(c, lane, T, H, E, z, r, hval, rhs);
+        }
+        __syncwarp();
+    }
+}
+
+__global__ void hybrid_bc_kernel(int64_t nf, pb::DualTopo T, pb::HybridIn H, const double *__restrict__ robin_weight,
+                                 const double *__restrict__ face_areas, const unsigned long long *__restrict__ norm_bits,
+                                 double *__restrict__ hval, double *__restrict__ rhs) {
+    const double norm = __longlong_as_double((long long)*norm_bits);
+    for (int64_t f = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; f < nf; f += (int64_t)gridDim.x * blockDim.x)
+        pb::hybrid_bc_row((int32_t)f, T, H, robin_weight, face_areas, norm, hval, rhs);
+}
+
+template <int ND>
+static void hybrid_launch(int method, int grid, size_t smem, cudaStream_t st, int64_t nc, const pb::DualTopo &T,
+                          const pb::DualGeo &G, const pb::HybridIn &H, int nmax, const double *lam, double *hval,
+                          double *rhs, double *u, double *p, int32_t *bad, int32_t *singular) {
+    if (method == PB_DUAL_MVEM)
+        hybrid_cell_kernel<ND, pb::kDualMvem><<<grid, 32 * kHybridWarps, smem, st>>>(nc, T, G, H, nmax, lam, hval, rhs,
+                                                                                     u, p, bad, singular);
+    else
+        hybrid_cell_kernel<ND, pb::kDualRt0><<<grid, 32 * kHybridWarps, smem, st>>>(nc, T, G, H, nmax, lam, hval, rhs,
+                                                                                    u, p, bad, singular);
+}
+
+// Everything both entry points share: the checks, the geometry (uploaded, or that of the last pb_dual_discretize), the
+// values and codes, and one timed launch of hybrid_cell_kernel.
+struct HybridRun {
+    DevBuf geo[7], aper, vals, codes, lam, flags;
+    pb::DualGeo G{};
+    pb::HybridIn H{};
+    int method = 0, nmax = 0;
+};
+
+static int hybrid_prepare(pb_dual *d, int mode, const double *const geo[7], const double *aperture,
+                          const uint8_t *codes, const double *values, HybridRun &R) {
+    if (mode != PB_DUAL_HYBRID_VEM && mode != PB_DUAL_HYBRID_SADDLE) return pb_fail_(PB_EINVAL, "unknown hybrid mode");
+    const int64_t nc = d->nc, nf = d->nf, nn = d->nn;
+    for (int64_t c = 0; c < nc; ++c)
+        R.nmax = std::max<int>(R.nmax, d->cf_ip_h[c + 1] - d->cf_ip_h[c]);
+    if (R.nmax > pb::kHybridMaxFaces)
+        return pb_fail_(PB_ENOTIMPL, "hybridization: a cell has " + std::to_string(R.nmax) +
+                                         " faces; one warp condenses one cell of at most 32 faces");
+    for (int64_t f = 0; f < nf; ++f)
+        if (codes[f] > PB_BC_ROB) return pb_fail_(PB_EINVAL, "boundary code out of range");
+    if (d->mass_nnz < 0) {
+        const int rc = dual_build_pattern(d);
+        if (rc) return rc;
+    }
+    cudaStream_t st = d->stream;
+    const double *const *g = geo;
+    const DevBuf *src[7];
+    if (mode == PB_DUAL_HYBRID_VEM) {
+        for (int k = 0; k < 7; ++k)
+            if (!geo[k]) return pb_fail_(PB_EINVAL, "null pointer");
+        if (!aperture) return pb_fail_(PB_EINVAL, "null pointer");
+        const size_t sizes[7] = {(size_t)3 * nn, (size_t)3 * nf, (size_t)3 * nf, (size_t)3 * nc, (size_t)nc,
+                                 (size_t)9 * nc, 9};
+        for (int k = 0; k < 7; ++k) {
+            CUDA_TRY(R.geo[k].upload(g[k], sizes[k], st));
+            src[k] = &R.geo[k];
+        }
+        CUDA_TRY(R.aper.upload(aperture, (size_t)nc, st));
+        R.method = PB_DUAL_MVEM;
+    } else {
+        if (!d->have_values)
+            return pb_fail_(PB_EINVAL, "hybridization of the saddle point: no discretization on the handle");
+        const DevBuf *kept[7] = {&d->geo_nodes, &d->geo_fn, &d->geo_fc, &d->geo_cc, &d->geo_vol, &d->geo_perm,
+                                 &d->geo_rot};
+        for (int k = 0; k < 7; ++k) src[k] = kept[k];
+        R.method = d->method;
+    }
+    CUDA_TRY(R.vals.upload(values, (size_t)(nf + nc), st));
+    CUDA_TRY(R.codes.upload(codes, (size_t)nf, st));
+    R.G = pb::DualGeo{nn, nf, nc, src[0]->as<double>(), src[1]->as<double>(), src[2]->as<double>(),
+                      src[3]->as<double>(), src[4]->as<double>(), src[5]->as<double>(), src[6]->as<double>()};
+    R.H = pb::HybridIn{mode, nf, d->fc_ip.as<int32_t>(), d->fc_cell.as<int32_t>(),
+                       mode == PB_DUAL_HYBRID_VEM ? R.aper.as<double>() : nullptr, R.vals.as<double>(),
+                       R.codes.as<uint8_t>()};
+    CUDA_TRY(R.flags.ensure(2 * sizeof(int32_t)));
+    CUDA_TRY(cudaMemsetAsync(R.flags.p, 0x7f, 2 * sizeof(int32_t), st));
+    return PB_OK;
+}
+
+static pb::DualTopo dual_topo(pb_dual *d) {
+    return pb::DualTopo{d->cf_ip.as<int32_t>(), d->cf_ix.as<int32_t>(), d->cf_cell.as<int32_t>(),
+                        d->cf_sg.as<int8_t>(), d->fn_ip.as<int32_t>(), d->fn_ix.as<int32_t>(),
+                        d->mass_ip.as<int32_t>(), d->mass_ix.as<int32_t>()};
+}
+
+// One timed launch of hybrid_cell_kernel; then the two flags: MVEM consistency (AssertionError in Python) and a
+// singular local matrix.
+static int hybrid_run(pb_dual *d, HybridRun &R, const double *lam, double *hval, double *rhs, double *u, double *p,
+                      int64_t *bad_cell, float *kernel_ms) {
+    cudaStream_t st = d->stream;
+    const pb::DualTopo T = dual_topo(d);
+    const size_t smem = (size_t)kHybridWarps * pb::hybrid_cell_doubles(R.nmax) * sizeof(double);
+    int32_t *flags = R.flags.as<int32_t>();
+    cudaEvent_t e0 = nullptr, e1 = nullptr;
+    struct Guard {
+        cudaEvent_t &a, &b;
+        ~Guard() { if (a) cudaEventDestroy(a); if (b) cudaEventDestroy(b); }
+    } guard{e0, e1};
+    CUDA_TRY(cudaEventCreate(&e0));
+    CUDA_TRY(cudaEventCreate(&e1));
+    const int grid = (int)std::max<int64_t>(1, std::min<int64_t>((d->nc + kHybridWarps - 1) / kHybridWarps,
+                                                                 (int64_t)pb_sm_count() * 32));
+    CUDA_TRY(cudaEventRecord(e0, st));
+    if (d->nd == 1) {
+        CUDA_TRY(cudaFuncSetAttribute(hybrid_cell_kernel<1, pb::kDualMvem>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        CUDA_TRY(cudaFuncSetAttribute(hybrid_cell_kernel<1, pb::kDualRt0>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        hybrid_launch<1>(R.method, grid, smem, st, d->nc, T, R.G, R.H, R.nmax, lam, hval, rhs, u, p, flags, flags + 1);
+    } else if (d->nd == 2) {
+        CUDA_TRY(cudaFuncSetAttribute(hybrid_cell_kernel<2, pb::kDualMvem>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        CUDA_TRY(cudaFuncSetAttribute(hybrid_cell_kernel<2, pb::kDualRt0>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        hybrid_launch<2>(R.method, grid, smem, st, d->nc, T, R.G, R.H, R.nmax, lam, hval, rhs, u, p, flags, flags + 1);
+    } else {
+        CUDA_TRY(cudaFuncSetAttribute(hybrid_cell_kernel<3, pb::kDualMvem>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        CUDA_TRY(cudaFuncSetAttribute(hybrid_cell_kernel<3, pb::kDualRt0>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        hybrid_launch<3>(R.method, grid, smem, st, d->nc, T, R.G, R.H, R.nmax, lam, hval, rhs, u, p, flags, flags + 1);
+    }
+    pb_count_launch_();
+    CUDA_TRY(cudaGetLastError());
+    CUDA_TRY(cudaEventRecord(e1, st));
+    int32_t hf[2];
+    CUDA_TRY(cudaMemcpyAsync(hf, flags, sizeof(hf), cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(cudaStreamSynchronize(st));
+    float ms = 0.0f;
+    CUDA_TRY(cudaEventElapsedTime(&ms, e0, e1));
+    if (kernel_ms) *kernel_ms = ms;
+    if (hf[1] != 0x7f7f7f7f)
+        return pb_fail_(PB_ESINGULAR, "hybridization: the local matrix of cell " + std::to_string(hf[1]) +
+                                          " is singular");
+    if (bad_cell) *bad_cell = hf[0] == 0x7f7f7f7f ? -1 : (int64_t)hf[0];
+    return PB_OK;
+}
+
+extern "C" int pb_dual_hybrid_system(pb_dual *d, int mode, const double *nodes, const double *face_normals,
+                                     const double *face_centers, const double *cell_centers,
+                                     const double *cell_volumes, const double *perm, const double *rot,
+                                     const double *aperture, const uint8_t *codes, const double *robin_weight,
+                                     const double *face_areas, const double *values, pb_csr **out, double *rhs,
+                                     int64_t *bad_cell, float *kernel_ms) {
+    if (!d || !codes || !robin_weight || !face_areas || !values || !out || !rhs || !bad_cell)
+        return pb_fail_(PB_EINVAL, "null pointer");
+    const double *const geo[7] = {nodes, face_normals, face_centers, cell_centers, cell_volumes, perm, rot};
+    HybridRun R;
+    int rc = hybrid_prepare(d, mode, geo, aperture, codes, values, R);
+    if (rc) return rc;
+    const int64_t nf = d->nf;
+    cudaStream_t st = d->stream;
+    pb_csr *a = nullptr;
+    rc = pb_csr_from_device_pattern_(nf, nf, d->mass_nnz, d->mass_ip.as<int32_t>(), d->mass_ix.as<int32_t>(), &a);
+    if (rc) return rc;
+    auto fail_cuda = [&](cudaError_t e, const char *what) {
+        pb_csr_destroy(a);
+        return pb_fail_(PB_ECUDA, std::string(what) + ": " + cudaGetErrorString(e));
+    };
+#define HY_TRY(x) do { cudaError_t e_ = (x); if (e_ != cudaSuccess) return fail_cuda(e_, #x); } while (0)
+    double *hval = pb_csr_data_(a);
+    DevBuf drhs, drw, darea, dnorm;
+    HY_TRY(drhs.ensure((size_t)nf * sizeof(double)));
+    HY_TRY(drw.upload(robin_weight, (size_t)nf, st));
+    HY_TRY(darea.upload(face_areas, (size_t)nf, st));
+    HY_TRY(dnorm.ensure(sizeof(unsigned long long)));
+    HY_TRY(cudaMemsetAsync(hval, 0, (size_t)d->mass_nnz * sizeof(double), st));
+    HY_TRY(cudaMemsetAsync(drhs.p, 0, (size_t)nf * sizeof(double), st));
+    HY_TRY(cudaMemsetAsync(dnorm.p, 0, sizeof(unsigned long long), st));
+    rc = hybrid_run(d, R, nullptr, hval, drhs.as<double>(), nullptr, nullptr, bad_cell, kernel_ms);
+    if (rc) { pb_csr_destroy(a); return rc; }
+    // |H|_inf before the boundary conditions (hybrid.py), or |mass|_inf of the saddle-point system
+    const int grid = (int)std::max<int64_t>(1, std::min<int64_t>((nf + 255) / 256, (int64_t)pb_sm_count() * 16));
+    dual_norm_kernel<<<grid, 256, 0, st>>>(nf, d->mass_ip.as<int32_t>(),
+                                           mode == PB_DUAL_HYBRID_VEM ? hval : d->mass_val.as<double>(),
+                                           dnorm.as<unsigned long long>());
+    hybrid_bc_kernel<<<grid, 256, 0, st>>>(nf, dual_topo(d), R.H, drw.as<double>(), darea.as<double>(),
+                                           dnorm.as<unsigned long long>(), hval, drhs.as<double>());
+    pb_count_launch_(); pb_count_launch_();
+    HY_TRY(cudaGetLastError());
+    HY_TRY(cudaMemcpyAsync(rhs, drhs.p, (size_t)nf * sizeof(double), cudaMemcpyDeviceToHost, st));
+    HY_TRY(cudaStreamSynchronize(st));
+#undef HY_TRY
+    *out = a;
+    return PB_OK;
+}
+
+extern "C" int pb_dual_hybrid_recover(pb_dual *d, int mode, const double *nodes, const double *face_normals,
+                                      const double *face_centers, const double *cell_centers,
+                                      const double *cell_volumes, const double *perm, const double *rot,
+                                      const double *aperture, const uint8_t *codes, const double *values,
+                                      const double *lambda, double *up, float *kernel_ms) {
+    if (!d || !codes || !values || !lambda || !up) return pb_fail_(PB_EINVAL, "null pointer");
+    const double *const geo[7] = {nodes, face_normals, face_centers, cell_centers, cell_volumes, perm, rot};
+    HybridRun R;
+    int rc = hybrid_prepare(d, mode, geo, aperture, codes, values, R);
+    if (rc) return rc;
+    const int64_t nf = d->nf, nc = d->nc;
+    cudaStream_t st = d->stream;
+    DevBuf dup;
+    CUDA_TRY(R.lam.upload(lambda, (size_t)nf, st));
+    CUDA_TRY(dup.ensure((size_t)(nf + nc) * sizeof(double)));
+    CUDA_TRY(cudaMemsetAsync(dup.p, 0, (size_t)(nf + nc) * sizeof(double), st));
+    double *u = dup.as<double>();
+    rc = hybrid_run(d, R, R.lam.as<double>(), nullptr, nullptr, u, u + nf, nullptr, kernel_ms);
+    if (rc) return rc;
+    CUDA_TRY(cudaMemcpyAsync(up, dup.p, (size_t)(nf + nc) * sizeof(double), cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(cudaStreamSynchronize(st));
     return PB_OK;
 }

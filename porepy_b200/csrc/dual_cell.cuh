@@ -1,10 +1,11 @@
 // dual_cell.cuh -- per-(cell, local face) routines of the two mixed (dual) discretizations of Darcy flow: the lowest
 // order mixed virtual element method (reference numerics/vem/mvem.py, MVEM.massHdiv and cell_diameters of
 // grids/grid.py) and the lowest order Raviart-Thomas element (numerics/fem/rt0.py, RT0.massHdiv, faces_to_cell and
-// _compute_cell_face_to_opposite_node).  One call writes row i of the local mass matrix of cell c into the global
-// FACE x FACE values and column i of the cell's (3 x n_faces) flux reconstruction; nothing is staged per cell, so
-// polyhedra with any number of faces need no local arrays.  The CUDA kernel (dual.cu) runs one thread per entry of
-// cell_faces; the test-only host build loops over them.
+// _compute_cell_face_to_opposite_node).  One call computes row i of the local mass matrix of cell c and hands it to a
+// row sink: DualScatter adds it into the global FACE x FACE values and writes column i of the cell's (3 x n_faces)
+// flux reconstruction, with nothing staged per cell, so polyhedra with any number of faces need no local arrays;
+// DualLocalRow writes it into row i of a per-cell buffer for the hybridization (dual_hybrid.cuh).  The CUDA kernel
+// dual_kernel (dual.cu) runs one thread per entry of cell_faces with DualScatter; the test-only host build loops.
 #pragma once
 #include <cmath>
 #include <cstdint>
@@ -106,6 +107,37 @@ PB_HD int32_t dual_pos(const DualTopo &T, int32_t f, int32_t j) {
     return lo;
 }
 
+// Row sink of dual_kernel: mass entry (row fi, column face of entry qj) added into the global values, flux
+// reconstruction column written to proj.
+struct DualScatter {
+    double *mass, *proj;
+    PB_HD void entry(const DualTopo &T, int32_t fi, int qj, double v) const {
+        dual_add(mass + dual_pos(T, fi, T.cf_ix[qj]), v);
+    }
+    // MVEM entry: consistency part and weighted stabilization, F_i^T G^-1 F_j + w stab
+    PB_HD void mvem_entry(const DualTopo &T, int32_t fi, int qj, double cons, double w, double stab) const {
+        dual_add(mass + dual_pos(T, fi, T.cf_ix[qj]), cons + w * stab);
+    }
+    template <int ND>
+    PB_HD void column(const DualTopo &T, const DualGeo &G, int64_t c, int i, const double p[ND]) const;
+};
+
+// Row sink of the hybridization: row i of the cell's local matrix in outward-flux variables, s_i s_j A_ij (hybrid.py
+// passes outward normals and unit signs to massHdiv), at row[j] for the j-th face of the cell.  inv_a = 1 / aperture:
+// hybrid.py scales the cell volume and the normals by the aperture, which divides the consistency part by it and
+// leaves the stabilization unchanged.  No flux reconstruction.
+struct DualLocalRow {
+    double *row;
+    double si, inv_a;
+    int b;   // cf_ip[c]
+    PB_HD void entry(const DualTopo &T, int32_t, int qj, double v) const { row[qj - b] = si * (double)T.cf_sg[qj] * v; }
+    PB_HD void mvem_entry(const DualTopo &T, int32_t, int qj, double cons, double w, double stab) const {
+        row[qj - b] = si * (double)T.cf_sg[qj] * (cons * inv_a + w * stab);
+    }
+    template <int ND>
+    PB_HD void column(const DualTopo &, const DualGeo &, int64_t, int, const double *) const {}
+};
+
 // Flux reconstruction column: proj row 3c + a holds the faces of c in cell_faces order, at 3 cf_ip[c] + a n + i.
 template <int ND>
 PB_HD void dual_proj_column(const DualTopo &T, const DualGeo &G, int64_t c, int i, const double p[ND], double *proj) {
@@ -117,13 +149,18 @@ PB_HD void dual_proj_column(const DualTopo &T, const DualGeo &G, int64_t c, int 
     }
 }
 
+template <int ND>
+PB_HD void DualScatter::column(const DualTopo &T, const DualGeo &G, int64_t c, int i, const double p[ND]) const {
+    dual_proj_column<ND>(T, G, c, i, p, proj);
+}
+
 // MVEM row, with diam the cell diameter, s_j the sign and x_j, n_j the centre and normal of face j:
 //   D_j = K^T n_j / diam, F_j = s_j (x_j - x_c) / diam, G = K vol / diam^2, Pi_j = G^-1 F_j,
 //   A_ij = F_i^T G^-1 F_j + w sum_k (delta_ki - D_k.Pi_i)(delta_kj - D_k.Pi_j),  w = diam^(2 - dim) |K^-1|_inf,
 // which is Pi^T G Pi + w (I - D Pi)^T (I - D Pi) of MVEM.massHdiv entry by entry.  The entry q of cell_faces with
 // i == 0 also tests the reference's assertion allclose(G, F D) and records the smallest failing cell in *bad.
-template <int ND>
-PB_HD void mvem_row(int64_t q, const DualTopo &T, const DualGeo &G, double *mass, double *proj, int32_t *bad) {
+template <int ND, class Out>
+PB_HD void mvem_row(int64_t q, const DualTopo &T, const DualGeo &G, const Out &out, int32_t *bad) {
     const int64_t c = T.cf_cell[q];
     const int b = T.cf_ip[c], e = T.cf_ip[c + 1], i = (int)(q - b);
     double K[ND][ND], Ki[ND][ND], xc[ND];
@@ -200,12 +237,12 @@ PB_HD void mvem_row(int64_t q, const DualTopo &T, const DualGeo &G, double *mass
             }
             stab += ui * uj;
         }
-        dual_add(mass + dual_pos(T, fi, T.cf_ix[qj]), cons + w * stab);
+        out.mvem_entry(T, fi, qj, cons, w, stab);
     }
     // vector_proj: R^T Pi(K = I) / diam = R^T s_i (x_i - x_c) / vol
     double p[ND];
     for (int k = 0; k < ND; ++k) p[k] = Fi[k] * diam / vol;
-    dual_proj_column<ND>(T, G, c, i, p, proj);
+    out.template column<ND>(T, G, c, i, p);
 }
 
 // Node of the simplex c opposite its face at entry qi: a node of another face of c that face qi lacks.
@@ -228,8 +265,8 @@ PB_HD int32_t rt0_opposite(const DualTopo &T, int64_t c, int qi) {
 // h = dim^2 (dim + 1)(dim + 2): C^T N^T HB (I (x) K^-1) / vol N C of RT0.massHdiv, since HB holds (1 + delta_ab) / h
 // on the diagonal of every dim x dim block (a, b).  Flux reconstruction (faces_to_cell): R^T (x_c - o_i) /
 // ((x_i - o_i) . n_i), x_i and n_i the centre and normal of face i.
-template <int ND>
-PB_HD void rt0_row(int64_t q, const DualTopo &T, const DualGeo &G, double *mass, double *proj) {
+template <int ND, class Out>
+PB_HD void rt0_row(int64_t q, const DualTopo &T, const DualGeo &G, const Out &out) {
     const int64_t c = T.cf_cell[q];
     const int b = T.cf_ip[c], e = T.cf_ip[c + 1], i = (int)(q - b);
     double K[ND][ND], Ki[ND][ND];
@@ -273,19 +310,20 @@ PB_HD void rt0_row(int64_t q, const DualTopo &T, const DualGeo &G, double *mass,
         }
         for (int k = 0; k < ND; ++k) acc += si[k] * KiSj[k];
         const double a = sgi * (double)T.cf_sg[qj] * acc / (G.vol[c] * h);
-        dual_add(mass + dual_pos(T, fi, T.cf_ix[qj]), a);
+        out.entry(T, fi, qj, a);
     }
     double den = 0.0, p[ND];
     for (int k = 0; k < ND; ++k) den += (G.fcent[k * G.nf + fi] - oi[k]) * G.fnorm[k * G.nf + fi];
     for (int k = 0; k < ND; ++k) p[k] = (G.ccent[k * G.nc + c] - oi[k]) / den;
-    dual_proj_column<ND>(T, G, c, i, p, proj);
+    out.template column<ND>(T, G, c, i, p);
 }
 
 template <int ND>
 PB_HD void dual_row(int method, int64_t q, const DualTopo &T, const DualGeo &G, double *mass, double *proj,
                     int32_t *bad) {
-    if (method == kDualMvem) mvem_row<ND>(q, T, G, mass, proj, bad);
-    else rt0_row<ND>(q, T, G, mass, proj);
+    const DualScatter out{mass, proj};
+    if (method == kDualMvem) mvem_row<ND>(q, T, G, out, bad);
+    else rt0_row<ND>(q, T, G, out);
 }
 
 }  // namespace pb

@@ -1584,6 +1584,56 @@ class DualGrid:
                                            C.byref(norm)))
         return DeviceCsr.from_handle(h), rhs, float(norm.value)
 
+    @staticmethod
+    def _geo_ptrs(geo):
+        """Geometry pointers of the hybrid entry points: nodes, face normals, face centres, cell centres, cell volumes,
+        perm, rot and aperture, or eight NULLs (the geometry of the last ``discretize``)."""
+        if geo is None:
+            return [None] * 8, []
+        arrs = [_lib.f64(a) for a in geo]
+        return [_lib.ptr(a, _lib._f64p) for a in arrs], arrs
+
+    def hybrid_system(self, mode: int, geo, codes, robin_weight, face_areas, values):
+        """The hybridized face system (``pb_dual_hybrid_system``): a ``DeviceCsr`` in the mass pattern, its right-hand
+        side, the first cell failing the MVEM consistency test (-1: none) and the kernel time in ms."""
+        from .sparse import DeviceCsr
+        ptrs, keep = self._geo_ptrs(geo)
+        arrs = [_lib.f64(a) for a in (robin_weight, face_areas, values)]
+        cod = np.ascontiguousarray(codes, dtype=np.uint8)
+        rhs, h, bad, ms = np.empty(self.nf), C.c_void_p(), C.c_int64(-1), C.c_float(0.0)
+        _lib.check(self.lib.pb_dual_hybrid_system(self.h, int(mode), *ptrs, _lib.ptr(cod, _lib._u8p),
+                                                  *[_lib.ptr(a, _lib._f64p) for a in arrs], C.byref(h),
+                                                  _lib.ptr(rhs, _lib._f64p), C.byref(bad), C.byref(ms)))
+        return DeviceCsr.from_handle(h), rhs, int(bad.value), float(ms.value)
+
+    def hybrid_recover(self, mode: int, geo, codes, values, lam):
+        """[u; p] from the face pressures ``lam`` (``pb_dual_hybrid_recover``) and the kernel time in ms."""
+        ptrs, keep = self._geo_ptrs(geo)
+        cod = np.ascontiguousarray(codes, dtype=np.uint8)
+        vals, lam = _lib.f64(values), _lib.f64(lam)
+        up, ms = np.empty(self.nf + self.nc), C.c_float(0.0)
+        _lib.check(self.lib.pb_dual_hybrid_recover(self.h, int(mode), *ptrs, _lib.ptr(cod, _lib._u8p),
+                                                   _lib.ptr(vals, _lib._f64p), _lib.ptr(lam, _lib._f64p),
+                                                   _lib.ptr(up, _lib._f64p), C.byref(ms)))
+        return up, float(ms.value)
+
+
+def dual_bc_codes(sd, bc) -> np.ndarray:
+    """PB_BC_* per face for the mixed schemes: Dirichlet, Neumann and Robin faces that are not internal."""
+    internal = np.asarray(bc.is_internal, bool)
+    codes = np.zeros(sd.num_faces, np.uint8)
+    codes[np.asarray(bc.is_dir, bool) & ~internal] = _lib.BC_DIR
+    codes[np.asarray(bc.is_rob, bool) & ~internal] = _lib.BC_ROB
+    codes[np.asarray(bc.is_neu, bool) & ~internal] = _lib.BC_NEU
+    return codes
+
+
+def _to_host(x) -> np.ndarray:
+    """A solver's solution (torch tensor on any device, or array) as a float64 NumPy array."""
+    if hasattr(x, "detach"):
+        x = x.detach().cpu().numpy()
+    return np.asarray(x, dtype=np.float64)
+
 
 class _DualElliptic(_Base):
     """Mixed (dual) discretizations of Darcy flow (numerics/vem/dual_elliptic.py ``DualElliptic``): the same
@@ -1722,28 +1772,80 @@ class _DualElliptic(_Base):
         the device-resident ones of the last ``discretize`` (``LazyCsr`` not yet touched), the system is assembled on
         the GPU from exactly those values (``pb_dual_system``) and ``A`` comes back as a ``LazyCsr`` backed by the
         device system (``A.device_csr``); otherwise the host formulas of the reference."""
-        mats = data[DISCRETIZATION_MATRICES][self.keyword]
         params = data[PARAMETERS][self.keyword]
-        dg = getattr(sd, "_b200_dual", None)
-        cur = None if dg is None else dg.current
-        if (sd.dim > 0 and cur is not None and getattr(dg, "h", None) is not None and params.get("bc") is not None
-                and cur[0] is mats[self.mass_matrix_key] and cur[1] is mats[self.vector_proj_key]
-                and cur[2] is mats[self.div_matrix_key] and not cur[0].on_host and not cur[1].on_host):
+        dg = self._resident(sd, data)
+        if dg is not None and getattr(dg, "h", None) is not None and params.get("bc") is not None:
             bc = params["bc"]
             if getattr(sd, "periodic_face_map", None) is not None:
                 raise NotImplementedError("Periodic boundary conditions are not implemented for DualElliptic")
-            internal = np.asarray(bc.is_internal, bool)
-            codes = np.zeros(sd.num_faces, np.uint8)
-            codes[np.asarray(bc.is_dir, bool) & ~internal] = _lib.BC_DIR
-            codes[np.asarray(bc.is_rob, bool) & ~internal] = _lib.BC_ROB
-            codes[np.asarray(bc.is_neu, bool) & ~internal] = _lib.BC_NEU
             vs = params.get("vector_source")
-            a, rhs, _ = dg.system(codes, np.broadcast_to(np.asarray(bc.robin_weight, float), (sd.num_faces,)),
+            a, rhs, _ = dg.system(dual_bc_codes(sd, bc),
+                                  np.broadcast_to(np.asarray(bc.robin_weight, float), (sd.num_faces,)),
                                   sd.face_areas, params["bc_values"], vs)
             return _lazy_system(a), rhs
         M = self.assemble_matrix(sd, data)
         M, norm = self.assemble_neumann_robin(sd, data, M, bc_weight=True)
         return M, self.assemble_rhs(sd, data, norm)
+
+    def _resident(self, sd, data: dict):
+        """The ``DualGrid`` whose device values are this keyword's stored matrices (the ``LazyCsr`` of the last
+        ``discretize``, untouched by the host), or None."""
+        mats = data.get(DISCRETIZATION_MATRICES, {}).get(self.keyword, {})
+        dg = getattr(sd, "_b200_dual", None)
+        cur = None if dg is None else dg.current
+        if (sd.dim > 0 and cur is not None and cur[0] is mats.get(self.mass_matrix_key)
+                and cur[1] is mats.get(self.vector_proj_key) and cur[2] is mats.get(self.div_matrix_key)
+                and not cur[0].on_host and not cur[1].on_host):
+            return dg
+        return None
+
+    def solve(self, sd, data: dict, b, tol: float = 1e-10, maxiter: int = 5000, linear_solver=None) -> np.ndarray:
+        """[u; p] solving the saddle-point system ``A x = b`` of ``assemble_matrix_rhs`` for any right-hand side ``b``
+        (e.g. the returned one with a source added to the cell rows), by hybridization on the device: every cell's
+        local system is condensed onto one pressure per face (csrc/dual_hybrid.cuh), the symmetric face system is
+        solved by ``linear_solver(H, rhs)`` (default: ``krylov.bicgstab_solver(tol, maxiter)``, Jacobi-preconditioned
+        BiCGStab on the ``DeviceCsr`` H), and u and p are recovered cell by cell.  No matrix leaves the device.
+
+        Faces with a given pressure (Dirichlet, and boundary faces without a condition) are fixed in the face system;
+        Neumann faces prescribe the flux b_f / |mass|_inf of their saddle-point row; Robin faces keep their
+        1 / (robin_weight area) as a local term.  Needs the device-resident discretization (the condition under which
+        ``assemble_matrix_rhs`` assembles on the device) and at least one Dirichlet or Robin face, else ``ValueError``.
+        ``last_solve``: iterations, relative residual of the face system, kernel times (ms) and wall time (s)."""
+        t0 = time.perf_counter()
+        params = data[PARAMETERS][self.keyword]
+        dg = self._resident(sd, data)
+        if dg is None:
+            raise ValueError(f"{self.name}.solve needs the device-resident discretization of the last discretize(); "
+                             "the stored mass / vector_proj / div matrices were downloaded or replaced")
+        bc = params.get("bc")
+        if bc is None:
+            raise ValueError(f"{self.name}.solve needs boundary conditions (params['bc'])")
+        if getattr(sd, "periodic_face_map", None) is not None:
+            raise NotImplementedError("Periodic boundary conditions are not implemented for DualElliptic")
+        codes = dual_bc_codes(sd, bc)
+        one_cell = np.diff(sps.csr_matrix(sd.cell_faces).indptr) == 1
+        fixed = (codes == _lib.BC_DIR) | ((codes == _lib.BC_INTERIOR) & one_cell)
+        if not fixed.any() and not (codes == _lib.BC_ROB).any():
+            raise ValueError(f"{self.name}.solve: no Dirichlet and no Robin face, the pressure is determined only up "
+                             "to a constant and the face system is singular")
+        b = _lib.f64(b)
+        if b.shape != (self.ndof(sd),):
+            raise ValueError(f"b must have {self.ndof(sd)} entries")
+        rw = np.broadcast_to(np.asarray(bc.robin_weight, float), (sd.num_faces,))
+        H, rhs, _, ms_c = dg.hybrid_system(_lib.DUAL_HYBRID_SADDLE, None, codes, rw, sd.face_areas, b)
+        if linear_solver is None:
+            from .krylov import bicgstab_solver
+            linear_solver = bicgstab_solver(tol, maxiter)
+        t1 = time.perf_counter()
+        lam = _to_host(linear_solver(H, rhs))
+        t2 = time.perf_counter()
+        up, ms_r = dg.hybrid_recover(_lib.DUAL_HYBRID_SADDLE, None, codes, b, lam)
+        info = getattr(linear_solver, "last_info", None) or {}
+        res = np.linalg.norm(rhs - _to_host(H @ lam)) / max(np.linalg.norm(rhs), 1e-300)
+        self.last_solve = dict(iterations=info.get("iterations"), converged=info.get("converged"),
+                               face_residual=float(res), condense_ms=ms_c, recover_ms=ms_r, solve_s=t2 - t1,
+                               wall_s=time.perf_counter() - t0, face_unknowns=sd.num_faces, face_nnz=int(H.nnz))
+        return up
 
     def project_flux(self, sd, u: np.ndarray, data: dict) -> np.ndarray:
         """dual_elliptic.py ``project_flux``: one 3-vector per cell, (3, nc)."""
@@ -1775,6 +1877,72 @@ class RT0(_DualElliptic):
 
     def __init__(self, keyword: str) -> None:
         super().__init__(keyword, "RT0")
+
+
+class HybridDualVEM:
+    """Hybridized mixed virtual element method (numerics/vem/hybrid.py ``HybridDualVEM``): the same constructor,
+    ``ndof`` (one pressure per face) and ``matrix_rhs``.  Every cell's MVEM saddle system is condensed onto its face
+    pressures on the GPU, one warp per cell (csrc/dual_hybrid.cuh); H comes back as scipy CSR.  The local matrix is
+    built as hybrid.py builds it: ``second_order_tensor`` as given (not rotated), the geometry in the frame of
+    ``map_geometry.map_grid``, outward normals and unit signs, cell volume and normals scaled by ``aperture``.
+
+    ``compute_up`` restates the reference's formulas on the device, p = S (f - B^T A^-1 C lambda) and
+    u = -sgn A^-1 (B p + C lambda), with the parameters ``matrix_rhs`` reads (``second_order_tensor``, ``source``,
+    ``aperture`` under ``data["parameters"][keyword]``).  The reference's own ``compute_up`` reads ``data["param"]``
+    and calls ``pp.DualVEM``, neither of which exists any more.  Each u_f is taken from the face's first cell (the
+    reference keeps the last one; the two agree to the accuracy of lambda).
+
+    Mapping to the saddle-point system of ``MVEM.assemble_matrix_rhs`` (aperture 1, a tensor that needs no rotation):
+    Dirichlet faces carry the same pressures bc_values in both; a Neumann value here is the flux per unit area along
+    the face normal, u_f = bc_values area, where MVEM prescribes u_f = s bc_values (s: the sign of the face in its
+    first cell); and the source f here, the net outflow of a cell, enters MVEM's right-hand side as -f in the cell
+    rows (the source convention of the MVEM tutorial)."""
+
+    def __init__(self, keyword: str = "flow") -> None:
+        self.keyword = keyword
+
+    def ndof(self, g) -> int:
+        return g.num_faces
+
+    def _inputs(self, g, data: dict):
+        params = data[PARAMETERS][self.keyword]
+        rot = dual_frame(g, data.get("deviation_from_plane_tol", 1e-5))
+        geo = [rot @ np.asarray(a, dtype=np.float64) for a in (g.nodes, g.face_normals, g.face_centers,
+                                                                g.cell_centers)]
+        geo += [g.cell_volumes, np.asarray(params["second_order_tensor"].values, dtype=np.float64), rot,
+                np.broadcast_to(np.asarray(params["aperture"], dtype=np.float64), (g.num_cells,))]
+        bc = params["bc"]
+        codes = np.zeros(g.num_faces, np.uint8)
+        if bc is not None:
+            codes[np.asarray(bc.is_dir, bool)] = _lib.BC_DIR
+            codes[np.asarray(bc.is_neu, bool)] = _lib.BC_NEU
+        bc_val = params.get("bc_values")
+        bc_val = np.zeros(g.num_faces) if bc_val is None else np.asarray(bc_val, dtype=np.float64)
+        f = np.broadcast_to(np.asarray(params["source"], dtype=np.float64), (g.num_cells,))
+        return geo, codes, np.concatenate((bc_val, f))
+
+    def matrix_rhs(self, g, data: dict):
+        """hybrid.py ``matrix_rhs``: the face matrix H (Dirichlet rows cleared, |H|_inf before the boundary
+        conditions on their diagonal) and its right-hand side."""
+        if g.dim == 0:
+            return sps.identity(self.ndof(g), format="csr"), np.zeros(1)
+        t0 = time.perf_counter()
+        geo, codes, values = self._inputs(g, data)
+        dg = DualGrid.for_grid(g)
+        H, rhs, bad, ms = dg.hybrid_system(_lib.DUAL_HYBRID_VEM, geo, codes, np.zeros(g.num_faces), g.face_areas,
+                                           values)
+        if bad >= 0:   # mvem.py massHdiv: assert np.allclose(G, F @ D)
+            raise AssertionError(f"HybridDualVEM: the consistency test G == F D fails in cell {bad}")
+        self.last_timing = dict(kernel_ms=ms, total_s=time.perf_counter() - t0)
+        return H.to_scipy(), rhs
+
+    def compute_up(self, g, solution, data: dict):
+        """u (per face) and p (per cell) from the face pressures ``solution`` (see the class docstring)."""
+        if g.dim == 0:
+            return 0, solution[0]
+        geo, codes, values = self._inputs(g, data)
+        up, _ = DualGrid.for_grid(g).hybrid_recover(_lib.DUAL_HYBRID_VEM, geo, codes, values, solution)
+        return up[:g.num_faces], up[g.num_faces:]
 
 
 class Upwind(_Base):

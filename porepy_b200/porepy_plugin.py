@@ -57,6 +57,9 @@ def plugin(pp, allow_reference_fallback: bool = False) -> SimpleNamespace:
     RefTpsa, RefTpsaAd = pp.Tpsa, pp.ad.TpsaAd
     RefUpwindCoupling = pp.UpwindCoupling
     RefMVEM, RefRT0 = pp.MVEM, pp.RT0
+    import importlib
+    hybrid_module = importlib.import_module(pp.__name__ + ".numerics.vem.hybrid")
+    RefHybridDualVEM = hybrid_module.HybridDualVEM
     RefMpfaAd, RefMpsaAd, RefBiotAd = pp.ad.MpfaAd, pp.ad.MpsaAd, pp.ad.BiotAd
 
     def _core(name, gpu_cls, ref_cls, flow):
@@ -131,6 +134,22 @@ def plugin(pp, allow_reference_fallback: bool = False) -> SimpleNamespace:
 
         def assemble_matrix_rhs(self, sd, data):
             return RefUpwind.assemble_matrix_rhs(self, sd, data)
+
+    class HybridDualVEM(fv.HybridDualVEM, RefHybridDualVEM):
+        """porepy.numerics.vem.hybrid.HybridDualVEM with the condensation and recovery on the GPU
+        (porepy_b200.fv.HybridDualVEM)."""
+
+        def __init__(self, keyword: str = "flow") -> None:
+            RefHybridDualVEM.__init__(self, keyword)
+            fv.HybridDualVEM.__init__(self, keyword)
+
+        def matrix_rhs(self, g, data):
+            out = fv.HybridDualVEM.matrix_rhs(self, g, data)
+            _count(gpu_calls, "HybridDualVEM")
+            return out
+
+        def compute_up(self, g, solution, data):
+            return fv.HybridDualVEM.compute_up(self, g, solution, data)
 
     class UpwindCoupling(fv.UpwindCoupling, RefUpwindCoupling):
         """pp.UpwindCoupling with the interface masks computed by the per-entry GPU kernel."""
@@ -215,6 +234,7 @@ def plugin(pp, allow_reference_fallback: bool = False) -> SimpleNamespace:
         pp.UpwindCoupling = UpwindCoupling
         pp.Tpsa = Tpsa
         pp.MVEM, pp.RT0 = MVEM, RT0
+        hybrid_module.HybridDualVEM = HybridDualVEM
 
     def uninstall() -> None:
         pp.Mpfa, pp.Mpsa, pp.Biot = RefMpfa, RefMpsa, RefBiot
@@ -222,6 +242,7 @@ def plugin(pp, allow_reference_fallback: bool = False) -> SimpleNamespace:
         pp.UpwindCoupling = RefUpwindCoupling
         pp.Tpsa = RefTpsa
         pp.MVEM, pp.RT0 = RefMVEM, RefRT0
+        hybrid_module.HybridDualVEM = RefHybridDualVEM
 
     def md_flow_from_model(model, keyword=None):
         """The mixed-dimensional Darcy problem of a prepared single-phase flow model (``pp.SinglePhaseFlow`` after
@@ -254,7 +275,7 @@ def plugin(pp, allow_reference_fallback: bool = False) -> SimpleNamespace:
             specific_volume=lambda it: evaluated(model.specific_volume([it]), it.num_cells))
 
     from . import model_bridge as bridge
-    return SimpleNamespace(Mpfa=Mpfa, Mpsa=Mpsa, Biot=Biot, Tpfa=Tpfa, Tpsa=Tpsa, MVEM=MVEM, RT0=RT0, Upwind=Upwind, UpwindCoupling=UpwindCoupling,
+    return SimpleNamespace(Mpfa=Mpfa, Mpsa=Mpsa, Biot=Biot, Tpfa=Tpfa, Tpsa=Tpsa, MVEM=MVEM, RT0=RT0, HybridDualVEM=HybridDualVEM, Upwind=Upwind, UpwindCoupling=UpwindCoupling,
                            MpfaAd=MpfaAd, MpsaAd=MpsaAd, BiotAd=BiotAd, TpsaAd=TpsaAd,
                            ModelMixin=ModelMixin, install=install, uninstall=uninstall, md_flow_from_model=md_flow_from_model,
                            # nonlinear model problems on the device AD chain (porepy_b200/model_bridge.py)

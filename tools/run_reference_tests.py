@@ -1,8 +1,9 @@
 """Run the REFERENCE's own finite-volume unit tests (tests/numerics/fv/test_{mpfa,mpsa,biot,tpsa}.py of the
-read-only tree) with pp.Mpfa / pp.Mpsa / pp.Biot / pp.Tpsa (and pp.Tpfa / pp.Upwind / pp.MVEM / pp.RT0) rebound to the
+read-only tree) with pp.Mpfa / pp.Mpsa / pp.Biot / pp.Tpsa (and pp.Tpfa / pp.Upwind / pp.MVEM / pp.RT0 / HybridDualVEM) rebound to the
 porepy_b200 plugin classes.  The mixed schemes' tests are named on the command line:
 
     python tools/run_reference_tests.py numerics/vem/test_dual_vem.py numerics/vem/test_rt0.py
+    python tools/run_reference_tests.py numerics/vem/test_hybrid_vem.py   # HybridDualVEM.matrix_rhs counted as well
 
     python tools/run_reference_tests.py            # build container or any box with /root/reference
     python tools/run_reference_tests.py functional/test_terzaghi.py [--stock] [pytest options]
@@ -39,10 +40,10 @@ class Rebind:
         if not gpu:
             from emu_binding import EmuBackedPlan
             from emu_tpsa import EmuTpsaFaceGrid   # the host build of the per-face routines, TPSA included
-            from emu_dual import EmuDualGrid   # the host build of the MVEM / RT0 routines
+            from emu_dual_hybrid import EmuHybridDualGrid   # the host build of MVEM / RT0 and their hybridization
             fv.DevicePlan = EmuBackedPlan
             fv.FaceGrid = EmuTpsaFaceGrid
-            fv.DualGrid = EmuDualGrid
+            fv.DualGrid = EmuHybridDualGrid
             import emu_binding
             fv.interface_upwind_masks = emu_binding.emu_interface_upwind_masks
         COUNTS["backend: " + ("cuda" if gpu else "host build of the node routines")] = 1
@@ -55,6 +56,16 @@ class Rebind:
                     COUNTS[f"{_name}.discretize on the {_tag} path"] += 1
                     return out
                 owner.discretize = counted
+        import importlib
+        hybrid = importlib.import_module(pp.__name__ + ".numerics.vem.hybrid")
+        for owner, tag in ((fv.HybridDualVEM, "porepy_b200"), (hybrid.HybridDualVEM, "reference")):
+            stock = owner.matrix_rhs
+
+            def counted_matrix_rhs(self, g, data, _stock=stock, _tag=tag):
+                out = _stock(self, g, data)
+                COUNTS[f"HybridDualVEM.matrix_rhs on the {_tag} path"] += 1
+                return out
+            owner.matrix_rhs = counted_matrix_rhs
         if "--stock" in sys.argv:  # control run: the unmodified reference in the same environment
             COUNTS["classes: stock reference (control run)"] = 1
             return

@@ -13,6 +13,7 @@ import scipy.sparse.linalg as spla
 
 import porepy_b200 as pb
 from porepy_b200 import fv
+import dual_mp
 from emu_dual_hybrid import EmuHybridDualGrid
 from golden_io import case_names, load_case, rel_err
 
@@ -72,7 +73,7 @@ def _check_hybrid(c, H, rhs, tol):
 
 def test_fixtures_cover_the_cases():
     assert {f"hybrid_{k}" for k in ("line", "line_tilted", "cart2d", "tri2d_sheared", "plane_tilted", "cart3d_pert",
-                                    "tet3d_delaunay")} <= set(HYBRID)
+                                    "tet3d_delaunay", "poly2d", "poly3d")} <= set(HYBRID)
     apertures = 0
     for name in HYBRID:
         c = load_case(name)
@@ -177,7 +178,8 @@ def check_linear_pressure(g, method, linear_solver, accuracy, **kw):
 
 
 @pytest.mark.parametrize("name", ["dual_mvem_cart3d_pert", "dual_mvem_tri2d_sheared", "dual_rt0_tet3d_delaunay",
-                                  "dual_rt0_tri2d_sheared", "dual_mvem_line_tilted", "dual_mvem_plane_tilted"])
+                                  "dual_rt0_tri2d_sheared", "dual_mvem_line_tilted", "dual_mvem_plane_tilted",
+                                  "dual_mvem_poly2d", "dual_mvem_poly3d", "dual_mvem_poly_plane_tilted"])
 def test_linear_pressure_is_exact_on_the_host_build(name, host_build):
     c = load_case(name)
     check_linear_pressure(c.g, c.kind, direct, 1e-10)
@@ -213,7 +215,7 @@ def _up_pair(c, linear_solver):
 
 
 @pytest.mark.parametrize("name", ["hybrid_cart2d", "hybrid_tri2d_sheared", "hybrid_cart3d_pert",
-                                  "hybrid_tet3d_delaunay", "hybrid_line"])
+                                  "hybrid_tet3d_delaunay", "hybrid_line", "hybrid_poly2d", "hybrid_poly3d"])
 def test_compute_up_matches_the_mvem_saddle_point_on_the_host_build(name, host_build):
     u_h, p_h, u, p = _up_pair(load_case(name), direct)
     assert np.abs(p_h - p).max() <= 1e-10 * np.abs(p).max()
@@ -315,15 +317,16 @@ def test_hybrid_goldens_on_the_gpu(name):
     geo, codes, values = d._inputs(c.g, _hybrid_data(c))
     He, rhse, _, _ = emu.hybrid_system(0, geo, codes, np.zeros(c.g.num_faces), c.g.face_areas, values)
     He = He.to_scipy()
-    assert np.abs((H - He)).max() <= 1e-13 * abs(He).max()
-    assert np.abs(rhs - rhse).max() <= 1e-13 * np.abs(rhse).max()
+    # entry by entry, each at the scale of its own cells (tests/dual_mp.py): kappa(A_c) max |E_c| for H, and for the
+    # right-hand side and the recovery what the errors of E, z and S bring in
+    R = dual_mp.HybridReference(c.g, geo, codes, values)
+    assert dual_mp.worst(H.toarray(), He.toarray(), R.Hs)[0] <= dual_mp.HYBRID_TOL
+    assert dual_mp.worst(rhs, rhse, R.rs)[0] <= dual_mp.HYBRID_TOL
     lam = spla.spsolve(sps.csc_matrix(H), rhs)
     u, p = d.compute_up(c.g, lam, _hybrid_data(c))
     upe, _ = emu.hybrid_recover(0, geo, codes, values, lam)
-    # the recovery v = A^-1 (r - B p - lambda) cancels large terms on the ill-conditioned Delaunay cells, which
-    # amplifies the last-bit differences of the two inverses (fused multiply-adds on the device)
-    ref = np.concatenate((u, p))
-    assert np.abs(ref - upe).max() <= 1e-11 * np.abs(upe).max()
+    _, ups = R.recover(lam)
+    assert dual_mp.worst(np.concatenate((u, p)), upe, ups)[0] <= dual_mp.HYBRID_TOL
 
 
 # Jacobi BiCGStab does not converge on the face system of dual_rt0_tet3d (a 2 x 2 x 2 tetrahedral grid with a 10^6

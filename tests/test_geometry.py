@@ -1,7 +1,8 @@
 """Grid.compute_geometry on the device (csrc/geometry_kernels.cuh + geometry.cu; reference grids/grid.py:572-778).
 The ``geom_*`` fixtures hold what the UNMODIFIED reference computed (tools/make_golden.py ``case_geometry``:
 ``compute_geometry`` of pp.CartGrid with all nodes displaced -- warped faces --, of a perturbed
-StructuredTetrahedralGrid and of a Delaunay TetrahedralGrid), with the face-node loops in the reference's order:
+StructuredTetrahedralGrid, of a Delaunay TetrahedralGrid and of agglomerated polyhedra with up to 32 faces of up to 10
+nodes), with the face-node loops in the reference's order:
 same topology + nodes in, the reference's face normals / centres / areas and cell centres / volumes out.
 CPU: host build of the per-face / per-cell routines; GPU: ``pb.compute_geometry`` through the C ABI."""
 import os
@@ -12,7 +13,7 @@ import pytest
 import porepy_b200 as pb
 
 GOLD = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
-CASES_3D = ["geom_cart3d_warped", "geom_tet3d_perturbed", "geom_tet3d_delaunay"]
+CASES_3D = ["geom_cart3d_warped", "geom_tet3d_perturbed", "geom_tet3d_delaunay", "geom_poly3d"]
 
 
 def _grid(case):

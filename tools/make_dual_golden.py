@@ -1,6 +1,7 @@
 """Generate tests/golden/dual_{mvem,rt0}_*.npz from the unmodified reference: ``pp.MVEM`` / ``pp.RT0`` discretize and
 ``assemble_matrix_rhs`` on 1-D, 2-D and 3-D grids (Cartesian, sheared triangles, perturbed Cartesian, structured and
-Delaunay tetrahedra, a tilted line and a tilted plane in 3-D), with a heterogeneous full anisotropic permeability of
+Delaunay tetrahedra, a tilted line and a tilted plane in 3-D, and agglomerated polygons and polyhedra of up to 32
+faces: ``poly2d``, ``poly3d`` and ``poly_plane_tilted``), with a heterogeneous full anisotropic permeability of
 10^6 contrast, Dirichlet, Neumann and Robin faces together, and a vector source.  Each fixture holds the grid arrays
 (``make_golden.grid_arrays``), the tensor (``K``), the boundary condition in the ``golden_io`` layout, ``bc_values``,
 ``vector_source`` and the reference's ``mass``, ``div``, ``vector_proj``, ``A`` and ``b``.  The prefix ``dual_`` keeps
@@ -12,9 +13,11 @@ import os
 import sys
 
 import numpy as np
+import scipy.sparse as sps
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, HERE)
+from agglomerate import agglomerate, interleave  # noqa: E402
 from make_golden import OUT, grid_arrays, pp, put_matrix  # noqa: E402
 
 
@@ -24,6 +27,58 @@ def rotation(a, b, c):
     ry = np.array([[cb, 0, sb], [0, 1, 0], [-sb, 0, cb]])
     rx = np.array([[1, 0, 0], [0, cc, -sc], [0, sc, cc]])
     return rz @ ry @ rx
+
+
+# poly2d: the labels of a 12 x 10 CartGrid, top row first.  A: an 8 x 8 block (32 edges); U: a U-shaped cell whose
+# centroid lies in its notch N (16 edges); the rest are 1 x 1 to 5 x 1 and 3 x 2 rectangles (4, 6, 8, 10, 12 edges).
+POLY2D = ["aabbbcccddee",
+          "fffffcccggee",
+          "AAAAAAAAgghi",
+          "AAAAAAAAjjji",
+          "AAAAAAAAkkkk",
+          "AAAAAAAAlllm",
+          "AAAAAAAAlllm",
+          "AAAAAAAAUNUm",
+          "AAAAAAAAUNUm",
+          "AAAAAAAAUUUm"]
+
+
+def polytopes(g, label, merge=()):
+    """``agglomerate`` with the coarse cells numbered round-robin by face count (the four warps of one block of the
+    hybridization kernel then hold cells of different sizes)."""
+    counts = np.diff(sps.csc_matrix(agglomerate(g, label, merge).cell_faces).indptr)
+    return agglomerate(g, interleave(counts)[label], merge)
+
+
+def poly2d():
+    g = pp.CartGrid([12, 10], [1.2, 1.0])
+    g.nodes = np.array([[1.0, 0.35, 0.0], [0.1, 1.0, 0.0], [0.0, 0.0, 1.0]]) @ g.nodes   # edges off the axes
+    _, label = np.unique(np.array([list(r) for r in POLY2D[::-1]]).ravel(), return_inverse=True)
+    return polytopes(g, label)
+
+
+def poly3d(rng):
+    """A 5 x 4 x 4 TensorGrid of uneven spacing under a global shear (planar faces), agglomerated into 3 x 2 x 2 (32
+    faces), 2 x 2 x 2 (24), 2 x 1 x 1 (10) and single cells; on the 3 x 2 x 2 cell at the origin the boundary sub-faces
+    of the planes x = 0 and y = 0 are merged into one face of 8 and one of 10 nodes (that cell keeps 24 faces)."""
+    g = pp.TensorGrid(*[np.concatenate(([0.0], np.cumsum(0.5 + rng.random(n)))) for n in (5, 4, 4)])
+    lab = -np.ones((5, 4, 4), int)
+    blocks = [(slice(0, 3), slice(0, 2), slice(0, 2)), (slice(0, 3), slice(2, 4), slice(0, 2)),
+              (slice(3, 5), slice(0, 2), slice(0, 2)), (slice(0, 3), slice(0, 2), slice(2, 4)),
+              (slice(3, 5), slice(0, 2), slice(2, 4))]
+    blocks += [(slice(3, 5), j, k) for j in (2, 3) for k in (0, 1, 2, 3)]
+    blocks += [(i, j, k) for i in range(3) for j in (2, 3) for k in (2, 3)]
+    for n, b in enumerate(blocks):
+        lab[b] = n
+    label = lab.ravel(order="F")    # cell i + nx (j + ny k)
+    g.compute_geometry()
+    cf = sps.csr_matrix(g.cell_faces)
+    first = np.flatnonzero(label == 0)
+    faces = np.unique(sps.csc_matrix(g.cell_faces)[:, first].indices)
+    bnd = faces[np.diff(cf.indptr)[faces] == 1]
+    merge = [bnd[np.abs(g.face_centers[0, bnd]) < 1e-12], bnd[np.abs(g.face_centers[1, bnd]) < 1e-12]]
+    g.nodes = np.array([[1.0, 0.3, -0.2], [0.1, 1.0, 0.25], [-0.15, 0.2, 1.0]]) @ g.nodes
+    return polytopes(g, label, merge)
 
 
 def make_grid(kind, rng):
@@ -61,6 +116,13 @@ def make_grid(kind, rng):
         g.nodes = rotation(0.4, -0.7, 0.2) @ g.nodes + np.array([[0.3], [-0.1], [0.5]])
     elif kind == "plane_tilted":
         g = pp.CartGrid([4, 3], [1.0, 0.8])
+        g.nodes = rotation(0.3, 0.9, -0.5) @ g.nodes + np.array([[0.2], [0.1], [-0.3]])
+    elif kind == "poly2d":
+        g = poly2d()
+    elif kind == "poly3d":
+        g = poly3d(rng)
+    elif kind == "poly_plane_tilted":
+        g = poly2d()
         g.nodes = rotation(0.3, 0.9, -0.5) @ g.nodes + np.array([[0.2], [0.1], [-0.3]])
     elif kind == "tri_plane_tilted":
         g = pp.StructuredTriangleGrid([3, 3], [1.0, 1.0])
@@ -128,7 +190,7 @@ def case(method, kind, seed):
 CASES = [("mvem", "cart2d"), ("mvem", "tri2d_sheared"), ("mvem", "cart3d"), ("mvem", "cart3d_pert"),
          ("mvem", "tet3d"), ("mvem", "tet3d_delaunay"), ("mvem", "line_tilted"), ("mvem", "plane_tilted"),
          ("rt0", "tri2d_sheared"), ("rt0", "tet3d"), ("rt0", "tet3d_delaunay"), ("rt0", "line_tilted"),
-         ("rt0", "tri_plane_tilted")]
+         ("rt0", "tri_plane_tilted"), ("mvem", "poly2d"), ("mvem", "poly3d"), ("mvem", "poly_plane_tilted")]
 
 if __name__ == "__main__":
     for i, (m, k) in enumerate(CASES):

@@ -312,9 +312,13 @@ def case_line(name, seed):
 def case_geometry(name, kind, seed, amp=0.3):
     """``Grid.compute_geometry`` (grids/grid.py:362-778) of a 3-D grid whose nodes -- ALL of them, so the
     faces of the hexahedra are warped -- were displaced: topology with the face-node loops in the
-    reference's own order, nodes, and the five geometry arrays the reference computes."""
+    reference's own order, nodes, and the five geometry arrays the reference computes.  ``poly3d``: the agglomerated
+    polyhedra of ``make_dual_golden`` (up to 32 faces, faces of 4, 8 and 10 nodes), displaced like the rest."""
     rng = np.random.default_rng(seed)
-    if kind == "cart3d":
+    if kind == "poly3d":
+        from make_dual_golden import poly3d
+        g = poly3d(rng)
+    elif kind == "cart3d":
         g = pp.CartGrid([5, 4, 3], [1.0, 0.8, 0.6])
     elif kind == "tet3d":
         g = pp.StructuredTetrahedralGrid([3, 2, 2], [1.0, 1.0, 1.0])
@@ -526,6 +530,8 @@ def main():
         (case_geometry, ("geom_cart3d_warped", "cart3d", 71), {}),
         (case_geometry, ("geom_tet3d_perturbed", "tet3d", 72), {}),
         (case_geometry, ("geom_tet3d_delaunay", "delaunay", 73), {}),
+        # displaced by 0.1 h: at 0.3 h the reference finds negative sub-tetrahedra in these cells
+        (case_geometry, ("geom_poly3d", "poly3d", 74), {"amp": 0.1}),
         # a 1-D intersection line (prefix "line")
         (case_line, ("line1d_tilted", 44), {}),
         # the reference's in-place partial update (prefix "partial")

@@ -1,10 +1,11 @@
 """Generate tests/golden/hybrid_*.npz from the unmodified reference: ``HybridDualVEM.matrix_rhs``
 (numerics/vem/hybrid.py) on a Cartesian line, a tilted line, an anisotropic 2-D Cartesian grid, sheared triangles, a
-tilted plane, perturbed hexahedra and Delaunay tetrahedra.  Every fixture has Dirichlet faces (the low end of the
-grid's longest extent) and Neumann faces (the rest of the boundary), nonzero boundary values and a nonzero source; the
-line, the tilted plane and the hexahedra have a heterogeneous aperture.  Each fixture holds the grid arrays
-(``make_golden.grid_arrays``), the tensor (``K``), the boundary condition in the ``golden_io`` layout, ``bc_values``,
-``source``, ``aperture`` and the reference's ``H`` and ``rhs``.
+tilted plane, perturbed hexahedra, Delaunay tetrahedra and the agglomerated polygons and polyhedra of
+``make_dual_golden`` (up to 32 faces per cell, the most one warp condenses).  Every fixture has Dirichlet faces (the
+low end of the grid's longest extent) and Neumann faces (the rest of the boundary), nonzero boundary values and a
+nonzero source; the line, the tilted plane, the hexahedra and the polyhedra have a heterogeneous aperture.  Each
+fixture holds the grid arrays (``make_golden.grid_arrays``), the tensor (``K``), the boundary condition in the
+``golden_io`` layout, ``bc_values``, ``source``, ``aperture`` and the reference's ``H`` and ``rhs``.
    python tools/make_hybrid_golden.py"""
 from __future__ import annotations
 
@@ -81,7 +82,7 @@ def case(kind, seed, aperture):
 
 
 CASES = [("line", True), ("line_tilted", False), ("cart2d", False), ("tri2d_sheared", False),
-         ("plane_tilted", True), ("cart3d_pert", True), ("tet3d_delaunay", False)]
+         ("plane_tilted", True), ("cart3d_pert", True), ("tet3d_delaunay", False), ("poly2d", False), ("poly3d", True)]
 
 if __name__ == "__main__":
     for i, (kind, aperture) in enumerate(CASES):

@@ -32,11 +32,10 @@ static thread_local std::string g_err;
 static thread_local int64_t g_err_node = -1;
 static std::atomic<int64_t> g_launches{0};
 
-static int fail(int code, const std::string &msg) {
+int pb_fail_(int code, const std::string &msg) {
     g_err = msg;
     return code;
 }
-int pb_fail_(int code, const std::string &msg) { return fail(code, msg); }  // for spmv.cu
 void pb_count_launch_() { g_launches++; }
 
 DevPool &pb_dev_pool_() {
@@ -73,7 +72,7 @@ extern "C" int pb_set_device(int device) {
 }
 
 extern "C" int pb_host_alloc(uint64_t bytes, void **out) {
-    if (!out) return fail(PB_EINVAL, "null pointer");
+    if (!out) return pb_fail_(PB_EINVAL, "null pointer");
     CUDA_TRY(cudaHostAlloc(out, bytes ? bytes : 8, cudaHostAllocDefault));
     return PB_OK;
 }
@@ -132,7 +131,7 @@ static int build_classes(pb_plan *p, std::vector<NodeClass> &out, bool rows_to_s
         const int tpb = kCfg[cfg].team == 32 ? 4 : 1;
         bool glob = (size_t)(a + r + scr) * 8 * tpb > kMaxSmem;
         if (glob && (size_t)(r + scr) * 8 * tpb > kMaxSmem)
-            return fail(PB_ENOTIMPL, "interaction region at node " + std::to_string(s) +
+            return pb_fail_(PB_ENOTIMPL, "interaction region at node " + std::to_string(s) +
                                          " is too large for this build (" + std::to_string(nsf) +
                                          " sub-faces)");
         int key = cfg * 2 + (glob ? 1 : 0);
@@ -166,7 +165,7 @@ static int build_classes(pb_plan *p, std::vector<NodeClass> &out, bool rows_to_s
             const std::vector<uint32_t> &nk = p->node_key;
             std::stable_sort(lists[key].begin(), lists[key].end(), [&](int32_t x, int32_t y) { return nk[x] < nk[y]; });
         }
-        if (c.nodes.upload(lists[key], p->stream) != cudaSuccess) return fail(PB_ECUDA, "upload of node list failed");
+        if (c.nodes.upload(lists[key], p->stream) != cudaSuccess) return pb_fail_(PB_ECUDA, "upload of node list failed");
     }
     return PB_OK;
 }
@@ -213,11 +212,10 @@ extern "C" int pb_plan_create(int nd, int64_t nc, int64_t nf, int64_t nn, const 
                               const int32_t *fn_indptr, const int32_t *fn_indices, pb_plan **out) {
     NvtxRange nvtx_("pb_plan_create");
     if (!out || !cf_indptr || !cf_indices || !cf_data || !fn_indptr || !fn_indices)
-        return fail(PB_EINVAL, "null pointer");
-    int ndev = 0;
-    if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev < 1)
-        return fail(PB_ECUDA, "no CUDA device: libporeb200 has no CPU path");
-    pb_plan *p = new pb_plan;
+        return pb_fail_(PB_EINVAL, "null pointer");
+    if (int rc = pb_require_device()) return rc;
+    DevBuf fn_idx_dev;                        // declared first: released after the plan has synchronized its stream
+    std::unique_ptr<pb_plan> p(new pb_plan);
     {
         // torchrun exports OMP_NUM_THREADS=1; the plan builder is the one OpenMP user here, so give
         // it this rank's share of the cores (POREB200_PLAN_THREADS overrides) -- through a num_threads clause on
@@ -230,24 +228,16 @@ extern "C" int pb_plan_create(int nd, int64_t nc, int64_t nf, int64_t nn, const 
         pb::g_plan_threads = std::max(1, nt);
     }
     auto tp0 = std::chrono::steady_clock::now();
-    auto bail = [&](const char *what, cudaError_t e) {
-        std::string m = std::string(what) + ": " + cudaGetErrorString(e);
-        delete p;
-        return fail(PB_ECUDA, m);
-    };
-    cudaError_t e;
-    if ((e = cudaStreamCreateWithFlags(&p->stream, cudaStreamNonBlocking)) != cudaSuccess) return bail("stream", e);
-    if ((e = cudaEventCreate(&p->e0)) != cudaSuccess) return bail("event", e);
-    if ((e = cudaEventCreate(&p->e1)) != cudaSuccess) return bail("event", e);
+    CUDA_TRY(p->stream.create());
+    CUDA_TRY(p->timer.create());
     HostPlan &H = p->H;
     cudaStream_t st = p->stream;
-    DevBuf fn_idx_dev;
     // ---- sub-cell topology: on the device (plan_device.cu); the host construction (plan_host.hpp) is the fallback
     // for interaction regions beyond the shared-memory sort capacity, and can be forced with POREB200_HOST_PLAN=1
     int rc = getenv("POREB200_HOST_PLAN") ? -1
-             : pb_build_device_topology_(p, nd, nc, nf, nn, cf_indptr, cf_indices, cf_data, fn_indptr, fn_indices,
-                                         fn_idx_dev);
-    if (rc > 0) { delete p; return rc; }
+             : pb_build_device_topology_(p.get(), nd, nc, nf, nn, cf_indptr, cf_indices, cf_data, fn_indptr,
+                                         fn_indices, fn_idx_dev);
+    if (rc > 0) return rc;
     const bool device_topology = rc == 0;
     if (getenv("POREB200_PLAN_TIMING")) {
         cudaStreamSynchronize(st);
@@ -259,23 +249,30 @@ extern "C" int pb_plan_create(int nd, int64_t nc, int64_t nf, int64_t nn, const 
         std::string err;
         rc = build_host_plan(nd, nc, nf, nn, cf_indptr, cf_indices, cf_data, fn_indptr, fn_indices,
                              p->H, err, /*build_pos_maps=*/false, /*build_patterns=*/false);
-        if (rc) {
-            delete p;
-            return fail(rc, err);
-        }
-#define UP(field, vec)                                                      \
-    if ((e = p->field.upload(vec, st)) != cudaSuccess) return bail(#field, e);
-        UP(fn_indptr, H.fn_indptr) UP(node_sc_ptr, H.node_sc_ptr) UP(sc_cell, H.sc_cell)
-        UP(node_sf_ptr, H.node_sf_ptr) UP(sf_face, H.sf_face) UP(sf_sides, H.sf_sides)
-        UP(sf_bloc, H.sf_bloc) UP(slot_sf, H.slot_sf) UP(node_nb, H.node_nb) UP(sc_ncn, H.sc_ncn)
-        UP(posfc_ptr, H.posfc_ptr) UP(posfb_ptr, H.posfb_ptr) UP(poscc_ptr, H.poscc_ptr)
-        UP(poscb_ptr, H.poscb_ptr) UP(nbf_ptr, H.nbf_ptr) UP(nbf_idx, H.nbf_idx) UP(cn_ptr, H.cn_ptr)
-        UP(cn_idx, H.cn_idx) UP(face_cells, H.face_cells)
-#undef UP
-        if ((e = fn_idx_dev.upload(fn_indices, (size_t)fn_indptr[nf], st)) != cudaSuccess) return bail("fn_indices", e);
-        if ((e = p->cf_ip.upload(cf_indptr, (size_t)nc + 1, st)) != cudaSuccess) return bail("cf_indptr", e);
-        if ((e = p->cf_ix.upload(cf_indices, (size_t)cf_indptr[nc], st)) != cudaSuccess) return bail("cf_indices", e);
-        if ((e = p->cf_sg.upload(cf_data, (size_t)cf_indptr[nc], st)) != cudaSuccess) return bail("cf_data", e);
+        if (rc) return pb_fail_(rc, err);
+        CUDA_TRY(p->fn_indptr.upload(H.fn_indptr, st));
+        CUDA_TRY(p->node_sc_ptr.upload(H.node_sc_ptr, st));
+        CUDA_TRY(p->sc_cell.upload(H.sc_cell, st));
+        CUDA_TRY(p->node_sf_ptr.upload(H.node_sf_ptr, st));
+        CUDA_TRY(p->sf_face.upload(H.sf_face, st));
+        CUDA_TRY(p->sf_sides.upload(H.sf_sides, st));
+        CUDA_TRY(p->sf_bloc.upload(H.sf_bloc, st));
+        CUDA_TRY(p->slot_sf.upload(H.slot_sf, st));
+        CUDA_TRY(p->node_nb.upload(H.node_nb, st));
+        CUDA_TRY(p->sc_ncn.upload(H.sc_ncn, st));
+        CUDA_TRY(p->posfc_ptr.upload(H.posfc_ptr, st));
+        CUDA_TRY(p->posfb_ptr.upload(H.posfb_ptr, st));
+        CUDA_TRY(p->poscc_ptr.upload(H.poscc_ptr, st));
+        CUDA_TRY(p->poscb_ptr.upload(H.poscb_ptr, st));
+        CUDA_TRY(p->nbf_ptr.upload(H.nbf_ptr, st));
+        CUDA_TRY(p->nbf_idx.upload(H.nbf_idx, st));
+        CUDA_TRY(p->cn_ptr.upload(H.cn_ptr, st));
+        CUDA_TRY(p->cn_idx.upload(H.cn_idx, st));
+        CUDA_TRY(p->face_cells.upload(H.face_cells, st));
+        CUDA_TRY(fn_idx_dev.upload(fn_indices, (size_t)fn_indptr[nf], st));
+        CUDA_TRY(p->cf_ip.upload(cf_indptr, (size_t)nc + 1, st));
+        CUDA_TRY(p->cf_ix.upload(cf_indices, (size_t)cf_indptr[nc], st));
+        CUDA_TRY(p->cf_sg.upload(cf_data, (size_t)cf_indptr[nc], st));
     }
     {
         // ---- structural patterns on the device (host fallback when a row has > 256 candidates)
@@ -285,31 +282,31 @@ extern "C" int pb_plan_create(int nd, int64_t nc, int64_t nf, int64_t nn, const 
                       {2, nc, nc, &p->cn_ptr, &p->cn_idx, &p->node_sc_ptr, &p->sc_cell},
                       {3, nc, nf, &p->cn_ptr, &p->cn_idx, &p->nbf_ptr, &p->nbf_idx}};
         DevBuf counts, flag;
-        if ((e = flag.ensure(sizeof(int))) != cudaSuccess) return bail("flag", e);
-        if ((e = cudaMemsetAsync(flag.p, 0, sizeof(int), st)) != cudaSuccess) return bail("memset", e);
+        CUDA_TRY(flag.ensure(sizeof(int)));
+        CUDA_TRY(cudaMemsetAsync(flag.p, 0, sizeof(int), st));
         bool host_fallback = false;
         for (auto &j : pj) {
             DevBuf &ip = p->pat_ip[j.which];
-            if ((e = counts.ensure((size_t)j.nrows * sizeof(int32_t))) != cudaSuccess) return bail("counts", e);
-            if ((e = ip.ensure((size_t)(j.nrows + 1) * sizeof(int32_t))) != cudaSuccess) return bail("indptr", e);
+            CUDA_TRY(counts.ensure((size_t)j.nrows * sizeof(int32_t)));
+            CUDA_TRY(ip.ensure((size_t)(j.nrows + 1) * sizeof(int32_t)));
             const int block = 256;
-            int grid = (int)std::max<int64_t>(1, std::min<int64_t>((j.nrows + 7) / 8, (int64_t)pb_sm_count() * 8));
+            const int grid = grid_stride_blocks(j.nrows, 8, 8);
             pattern_kernel<256><<<grid, block, 0, st>>>(j.nrows, j.rnp->as<int32_t>(), j.rn->as<int32_t>(),
                                                         j.cp->as<int32_t>(), j.ci->as<int32_t>(),
                                                         counts.as<int32_t>(), nullptr, nullptr, 0, flag.as<int>());
-            g_launches++;
+            pb_count_launch_();
             int ov = 0;
-            if ((e = cudaMemcpyAsync(&ov, flag.p, sizeof(ov), cudaMemcpyDeviceToHost, st)) != cudaSuccess) return bail("copy", e);
+            CUDA_TRY(cudaMemcpyAsync(&ov, flag.p, sizeof(ov), cudaMemcpyDeviceToHost, st));
             int64_t tot = 0;
-            if ((rc = pb_scan_offsets_(counts.as<int32_t>(), ip.as<int32_t>(), j.nrows, st, &tot))) { delete p; return rc; }
+            if ((rc = pb_scan_offsets_(counts.as<int32_t>(), ip.as<int32_t>(), j.nrows, st, &tot))) return rc;
             if (ov) { host_fallback = true; break; }
-            if (tot > 0x7FFFFFFFll) { delete p; return fail(PB_EINVAL, "pattern exceeds 2^31 entries; split the grid"); }
-            if ((e = p->pat_idx[j.which].ensure((size_t)std::max<int64_t>(1, tot) * sizeof(int32_t))) != cudaSuccess) return bail("indices", e);
+            if (tot > 0x7FFFFFFFll) return pb_fail_(PB_EINVAL, "pattern exceeds 2^31 entries; split the grid");
+            CUDA_TRY(p->pat_idx[j.which].ensure((size_t)std::max<int64_t>(1, tot) * sizeof(int32_t)));
             pattern_kernel<256><<<grid, block, 0, st>>>(j.nrows, j.rnp->as<int32_t>(), j.rn->as<int32_t>(),
                                                         j.cp->as<int32_t>(), j.ci->as<int32_t>(), nullptr,
                                                         ip.as<int32_t>(), p->pat_idx[j.which].as<int32_t>(), 1,
                                                         flag.as<int>());
-            g_launches++;
+            pb_count_launch_();
             p->pat_rows[j.which] = j.nrows; p->pat_cols[j.which] = j.ncols; p->pat_nnz[j.which] = tot;
         }
         if (host_fallback) {
@@ -318,13 +315,13 @@ extern "C" int pb_plan_create(int nd, int64_t nc, int64_t nf, int64_t nn, const 
             HostPlan H2;
             int rc2 = build_host_plan(nd, nc, nf, nn, cf_indptr, cf_indices, cf_data, fn_indptr, fn_indices,
                                       H2, err2, false, true);
-            if (rc2) { delete p; return fail(rc2, err2); }
+            if (rc2) return pb_fail_(rc2, err2);
             for (int w = 0; w < 4; ++w) {
-                if ((e = p->pat_ip[w].upload(H2.pat[w].indptr, st)) != cudaSuccess) return bail("indptr", e);
-                if ((e = p->pat_idx[w].upload(H2.pat[w].indices, st)) != cudaSuccess) return bail("indices", e);
+                CUDA_TRY(p->pat_ip[w].upload(H2.pat[w].indptr, st));
+                CUDA_TRY(p->pat_idx[w].upload(H2.pat[w].indices, st));
                 p->pat_rows[w] = H2.pat[w].nrows; p->pat_cols[w] = H2.pat[w].ncols; p->pat_nnz[w] = H2.pat[w].nnz();
             }
-            if ((e = cudaStreamSynchronize(st)) != cudaSuccess) return bail("sync", e);
+            CUDA_TRY(cudaStreamSynchronize(st));
         }
         if (getenv("POREB200_PLAN_TIMING")) {
             cudaStreamSynchronize(st);
@@ -342,20 +339,17 @@ extern "C" int pb_plan_create(int nd, int64_t nc, int64_t nf, int64_t nn, const 
             {&p->pos_cb, &H.poscb_ptr, &p->poscb_ptr, 3, &p->node_sc_ptr, &p->sc_cell, &p->nbf_ptr, &p->nbf_idx},
         };
         for (auto &j : jobs) {
-            if ((e = j.pos->ensure((size_t)std::max<int64_t>(1, j.ptr->back()) * sizeof(int32_t))) != cudaSuccess)
-                return bail("pos map", e);
+            CUDA_TRY(j.pos->ensure((size_t)std::max<int64_t>(1, j.ptr->back()) * sizeof(int32_t)));
             const int block = 256;
-            int64_t need = (nn * 32 + block - 1) / block;
-            int grid = (int)std::max<int64_t>(1, std::min<int64_t>(need, (int64_t)pb_sm_count() * 16));
-            posmap_kernel<<<grid, block, 0, st>>>(nn, j.rp->as<int32_t>(), j.re->as<int32_t>(),
-                                                  j.cp->as<int32_t>(), j.ce->as<int32_t>(),
-                                                  p->pat_ip[j.pat].as<int32_t>(), p->pat_idx[j.pat].as<int32_t>(),
-                                                  j.pptr->as<int64_t>(), j.pos->as<int32_t>());
-            g_launches++;
-            if ((e = cudaGetLastError()) != cudaSuccess) return bail("posmap_kernel", e);
+            posmap_kernel<<<grid_stride_blocks(nn * 32, block, 16), block, 0, st>>>(
+                nn, j.rp->as<int32_t>(), j.re->as<int32_t>(), j.cp->as<int32_t>(), j.ce->as<int32_t>(),
+                p->pat_ip[j.pat].as<int32_t>(), p->pat_idx[j.pat].as<int32_t>(), j.pptr->as<int64_t>(),
+                j.pos->as<int32_t>());
+            pb_count_launch_();
+            CUDA_TRY(cudaGetLastError());
         }
     }
-    if ((e = p->err.ensure(sizeof(int))) != cudaSuccess) return bail("err", e);
+    CUDA_TRY(p->err.ensure(sizeof(int)));
     PlanView &v = p->view;
     v.nd = nd; v.nc = nc; v.nf = nf; v.nn = nn;
     v.fn_indptr = p->fn_indptr.as<int32_t>();
@@ -370,9 +364,9 @@ extern "C" int pb_plan_create(int nd, int64_t nc, int64_t nf, int64_t nn, const 
     v.pos_cc = p->pos_cc.as<int32_t>(); v.pos_cb = p->pos_cb.as<int32_t>();
     v.fc_indptr = p->pat_ip[0].as<int32_t>(); v.fb_indptr = p->pat_ip[1].as<int32_t>();
     v.cc_indptr = p->pat_ip[2].as<int32_t>(); v.cb_indptr = p->pat_ip[3].as<int32_t>();
-    rc = build_mpfa_classes(p);
-    if (rc) { delete p; return rc; }
-    if ((e = cudaStreamSynchronize(st)) != cudaSuccess) return bail("sync", e);
+    rc = build_mpfa_classes(p.get());
+    if (rc) return rc;
+    CUDA_TRY(cudaStreamSynchronize(st));
     // the host copies of the node-major lists are only needed for the uploads above
     {
         auto drop = [](auto &v) { v.clear(); v.shrink_to_fit(); };
@@ -383,22 +377,15 @@ extern "C" int pb_plan_create(int nd, int64_t nc, int64_t nf, int64_t nn, const 
     if (getenv("POREB200_PLAN_TIMING"))
         fprintf(stderr, "[plan] total incl. upload          %8.1f ms\n",
                 std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - tp0).count());
-    *out = p;
+    *out = p.release();
     return PB_OK;
 }
 
-extern "C" void pb_plan_destroy(pb_plan *p) {
-    if (!p) return;
-    if (p->stream) cudaStreamSynchronize(p->stream);
-    if (p->e0) cudaEventDestroy(p->e0);
-    if (p->e1) cudaEventDestroy(p->e1);
-    if (p->stream) cudaStreamDestroy(p->stream);
-    delete p;
-}
+extern "C" void pb_plan_destroy(pb_plan *p) { delete p; }
 
 extern "C" int pb_plan_sizes(const pb_plan *p, int64_t *num_subcells, int64_t *num_subfaces,
                              int64_t *num_subhalffaces, int32_t *max_sf, int32_t *max_sc) {
-    if (!p) return fail(PB_EINVAL, "null plan");
+    if (!p) return pb_fail_(PB_EINVAL, "null plan");
     if (num_subcells) *num_subcells = p->H.S;
     if (num_subfaces) *num_subfaces = p->H.U;
     if (num_subhalffaces) *num_subhalffaces = p->H.H;
@@ -408,8 +395,8 @@ extern "C" int pb_plan_sizes(const pb_plan *p, int64_t *num_subcells, int64_t *n
 }
 
 extern "C" int pb_plan_class_counts(const pb_plan *p, int kind, int64_t *counts) {
-    if (!p || !counts) return fail(PB_EINVAL, "null pointer");
-    if (kind != 0 && kind != 1) return fail(PB_EINVAL, "kind must be 0 (MPFA) or 1 (MPSA)");
+    if (!p || !counts) return pb_fail_(PB_EINVAL, "null pointer");
+    if (kind != 0 && kind != 1) return pb_fail_(PB_EINVAL, "kind must be 0 (MPFA) or 1 (MPSA)");
     for (int k = 0; k < 2 * kNumCfg; ++k) counts[k] = 0;
     for (const NodeClass &c : kind == 0 ? p->mpfa_cls : p->mpsa_cls) counts[2 * c.cfg + (c.a_global ? 1 : 0)] += c.n;
     return PB_OK;
@@ -426,14 +413,14 @@ extern "C" int pb_plan_set_active_nodes(pb_plan *p, const uint8_t *mask) {
 }
 
 extern "C" int pb_plan_pattern_size(const pb_plan *p, int which, int64_t *nrows, int64_t *nnz) {
-    if (!p || which < 0 || which > 3) return fail(PB_EINVAL, "bad pattern id");
+    if (!p || which < 0 || which > 3) return pb_fail_(PB_EINVAL, "bad pattern id");
     *nrows = p->pat_rows[which];
     *nnz = p->pat_nnz[which];
     return PB_OK;
 }
 
 extern "C" int pb_plan_pattern_get(const pb_plan *p, int which, int32_t *indptr, int32_t *indices) {
-    if (!p || which < 0 || which > 3) return fail(PB_EINVAL, "bad pattern id");
+    if (!p || which < 0 || which > 3) return pb_fail_(PB_EINVAL, "bad pattern id");
     CUDA_TRY(cudaMemcpyAsync(indptr, p->pat_ip[which].p, (p->pat_rows[which] + 1) * sizeof(int32_t), cudaMemcpyDeviceToHost, p->stream));
     if (p->pat_nnz[which])
         CUDA_TRY(cudaMemcpyAsync(indices, p->pat_idx[which].p, p->pat_nnz[which] * sizeof(int32_t),
@@ -467,11 +454,9 @@ __global__ void expand_pattern_kernel(int64_t nrows, const int32_t *__restrict__
 // pattern `which` expanded into br x bc blocks (layout as documented at pb_plan_pattern_expanded), on the plan's stream
 static int expand_pattern(pb_plan *p, int which, int br, int bc, int32_t *nip, int32_t *nix) {
     const int64_t nrows = p->pat_rows[which];
-    const int block = 256;
-    int grid = (int)std::max<int64_t>(1, std::min<int64_t>((nrows * 32 + block - 1) / block, (int64_t)pb_sm_count() * 16));
-    expand_pattern_kernel<<<grid, block, 0, p->stream>>>(nrows, p->pat_ip[which].as<int32_t>(),
-                                                         p->pat_idx[which].as<int32_t>(), br, bc, nip, nix);
-    g_launches++;
+    expand_pattern_kernel<<<grid_stride_blocks(nrows * 32, 256, 16), 256, 0, p->stream>>>(
+        nrows, p->pat_ip[which].as<int32_t>(), p->pat_idx[which].as<int32_t>(), br, bc, nip, nix);
+    pb_count_launch_();
     CUDA_TRY(cudaGetLastError());
     return PB_OK;
 }
@@ -479,11 +464,11 @@ static int expand_pattern(pb_plan *p, int which, int br, int bc, int32_t *nip, i
 extern "C" int pb_plan_pattern_expanded(pb_plan *p, int which, int br, int bc, int32_t *indptr,
                                         int32_t *indices) {
     if (!p || which < 0 || which > 3 || br < 1 || bc < 1 || !indptr || !indices)
-        return fail(PB_EINVAL, "bad arguments");
+        return pb_fail_(PB_EINVAL, "bad arguments");
     struct { int64_t nrows, ncols; } c{p->pat_rows[which], p->pat_cols[which]};
     const int64_t nnz = p->pat_nnz[which] * br * bc;
     if (nnz >= 0x7FFFFFFFll || c.ncols * bc >= 0x7FFFFFFFll)
-        return fail(PB_ENOTIMPL, "expanded pattern does not fit int32 indices");
+        return pb_fail_(PB_ENOTIMPL, "expanded pattern does not fit int32 indices");
     DevBuf nip, nix;
     cudaStream_t st = p->stream;
     CUDA_TRY(nip.ensure((c.nrows * br + 1) * sizeof(int32_t)));
@@ -510,10 +495,9 @@ __global__ void repack_kernel(const double *__restrict__ in, double *__restrict_
 int pb_upload_repacked_(cudaStream_t st, DevBuf &tmp, DevBuf &dst, const double *host, int ncomp, int64_t n) {
     CUDA_TRY(tmp.upload(host, (size_t)ncomp * n, st));
     CUDA_TRY(dst.ensure((size_t)ncomp * n * sizeof(double)));
-    const int64_t total = (int64_t)ncomp * n;
-    int grid = (int)std::max<int64_t>(1, std::min<int64_t>((total + 255) / 256, (int64_t)pb_sm_count() * 32));
-    repack_kernel<<<grid, 256, 0, st>>>(tmp.as<double>(), dst.as<double>(), ncomp, n);
-    g_launches++;
+    repack_kernel<<<grid_stride_blocks((int64_t)ncomp * n, 256, 32), 256, 0, st>>>(tmp.as<double>(), dst.as<double>(),
+                                                                                   ncomp, n);
+    pb_count_launch_();
     CUDA_TRY(cudaGetLastError());
     return PB_OK;
 }
@@ -542,21 +526,19 @@ static int upload_cell_tensor(pb_plan *p, DevBuf &dst, const double *host, int n
     cudaStream_t st = p->stream;
     CUDA_TRY(p->repack_tmp.upload(host, (size_t)ncomp * p->cell_map_src, st));
     CUDA_TRY(dst.ensure((size_t)ncomp * n * sizeof(double)));
-    const int64_t total = (int64_t)ncomp * n;
-    int grid = (int)std::max<int64_t>(1, std::min<int64_t>((total + 255) / 256, (int64_t)pb_sm_count() * 32));
-    repack_gather_kernel<<<grid, 256, 0, st>>>(p->repack_tmp.as<double>(), dst.as<double>(), ncomp, n, p->cell_map_src,
-                                               p->cell_map.as<int64_t>());
-    g_launches++;
+    repack_gather_kernel<<<grid_stride_blocks((int64_t)ncomp * n, 256, 32), 256, 0, st>>>(
+        p->repack_tmp.as<double>(), dst.as<double>(), ncomp, n, p->cell_map_src, p->cell_map.as<int64_t>());
+    pb_count_launch_();
     CUDA_TRY(cudaGetLastError());
     return PB_OK;
 }
 
 extern "C" int pb_plan_set_cell_map(pb_plan *p, const int64_t *cells, int64_t n_source_cells) {
-    if (!p) return fail(PB_EINVAL, "null plan");
+    if (!p) return pb_fail_(PB_EINVAL, "null plan");
     if (!cells) { p->cell_map.release(); p->cell_map_src = 0; return PB_OK; }
-    if (n_source_cells < 1) return fail(PB_EINVAL, "bad source size");
+    if (n_source_cells < 1) return pb_fail_(PB_EINVAL, "bad source size");
     for (int64_t e = 0; e < p->H.nc; ++e)
-        if (cells[e] < 0 || cells[e] >= n_source_cells) return fail(PB_EINVAL, "cell map entry out of range");
+        if (cells[e] < 0 || cells[e] >= n_source_cells) return pb_fail_(PB_EINVAL, "cell map entry out of range");
     CUDA_TRY(p->cell_map.upload(cells, (size_t)p->H.nc, p->stream));
     CUDA_TRY(cudaStreamSynchronize(p->stream));
     p->cell_map_src = n_source_cells;
@@ -568,7 +550,7 @@ extern "C" int pb_plan_set_geometry(pb_plan *p, const double *nodes, const doubl
                                     const double *cell_centers, const double *cell_volumes) {
     NvtxRange nvtx_("pb_plan_set_geometry");
     if (!p || !nodes || !face_normals || !face_centers || !face_areas || !cell_centers || !cell_volumes)
-        return fail(PB_EINVAL, "null pointer");
+        return pb_fail_(PB_EINVAL, "null pointer");
     const HostPlan &H = p->H;
     cudaStream_t st = p->stream;
     int rc;
@@ -625,7 +607,7 @@ static int check_singular(pb_plan *p) {
     CUDA_TRY(cudaStreamSynchronize(p->stream));
     if (h != INT_MAX) {
         g_err_node = h;
-        return fail(PB_ESINGULAR, "singular local system at node " + std::to_string(h));
+        return pb_fail_(PB_ESINGULAR, "singular local system at node " + std::to_string(h));
     }
     return PB_OK;
 }
@@ -636,8 +618,8 @@ static int check_singular(pb_plan *p) {
 extern "C" int pb_mpfa_upload(pb_plan *p, const double *perm, const uint8_t *bc,
                               const double *robin_weight, double eta) {
     NvtxRange nvtx_("pb_mpfa_upload");
-    if (!p || !perm || !bc) return fail(PB_EINVAL, "null pointer");
-    if (!p->have_geo) return fail(PB_EINVAL, "pb_plan_set_geometry has not been called");
+    if (!p || !perm || !bc) return pb_fail_(PB_EINVAL, "null pointer");
+    if (!p->have_geo) return pb_fail_(PB_EINVAL, "pb_plan_set_geometry has not been called");
     const HostPlan &H = p->H;
     cudaStream_t st = p->stream;
     { int rcp = upload_cell_tensor(p, p->perm, perm, 9); if (rcp) return rcp; }
@@ -652,8 +634,8 @@ extern "C" int pb_mpfa_upload(pb_plan *p, const double *perm, const uint8_t *bc,
 
 extern "C" int pb_mpfa_assemble(pb_plan *p, int want_flux, int want_trace, int want_vs, float *ms) {
     NvtxRange nvtx_("pb_mpfa_assemble");
-    if (!p) return fail(PB_EINVAL, "null plan");
-    if (!p->mpfa_ready) return fail(PB_EINVAL, "pb_mpfa_upload has not been called");
+    if (!p) return pb_fail_(PB_EINVAL, "null plan");
+    if (!p->mpfa_ready) return pb_fail_(PB_EINVAL, "pb_mpfa_upload has not been called");
     const HostPlan &H = p->H;
     const int nd = H.nd;
     cudaStream_t st = p->stream;
@@ -668,7 +650,7 @@ extern "C" int pb_mpfa_assemble(pb_plan *p, int want_flux, int want_trace, int w
                    {&p->o_bpvs, &o.bpvs, nfc * nd, want_vs != 0 && want_trace != 0}};
     for (auto &r : reqs)
         if (r.want) CUDA_TRY(r.b->ensure(r.n * sizeof(double)));
-    CUDA_TRY(cudaEventRecord(p->e0, st));
+    CUDA_TRY(p->timer.mark(0, st));
     for (auto &r : reqs) {
         if (!r.want) { *r.slot = nullptr; continue; }
         CUDA_TRY(cudaMemsetAsync(r.b->p, 0, r.n * sizeof(double), st));
@@ -679,22 +661,22 @@ extern "C" int pb_mpfa_assemble(pb_plan *p, int want_flux, int want_trace, int w
     MpfaParams prm{p->perm.as<double>(), p->bc.as<uint8_t>(),
                    p->have_robw ? p->robw.as<double>() : nullptr, p->eta, 1, 9};
     { int rc = pb_launch_mpfa_(p, prm, o); if (rc) return rc; }
-    CUDA_TRY(cudaEventRecord(p->e1, st));
-    CUDA_TRY(cudaEventSynchronize(p->e1));
-    if (ms) CUDA_TRY(cudaEventElapsedTime(ms, p->e0, p->e1));
+    CUDA_TRY(p->timer.mark(1, st));
+    CUDA_TRY(cudaEventSynchronize(p->timer.ev[1]));
+    if (ms) CUDA_TRY(p->timer.ms(ms));
     return check_singular(p);
 }
 
 static int dl(pb_plan *p, DevBuf &b, double *h, size_t n) {
     if (!h) return PB_OK;
-    if (!b.p || b.bytes < n * sizeof(double)) return fail(PB_EINVAL, "output was not assembled");
+    if (!b.p || b.bytes < n * sizeof(double)) return pb_fail_(PB_EINVAL, "output was not assembled");
     CUDA_TRY(cudaMemcpyAsync(h, b.p, n * sizeof(double), cudaMemcpyDeviceToHost, p->stream));
     return PB_OK;
 }
 
 extern "C" int pb_mpfa_download(pb_plan *p, double *flux, double *bound_flux, double *bpc,
                                 double *bpf, double *vs, double *bpvs) {
-    if (!p) return fail(PB_EINVAL, "null plan");
+    if (!p) return pb_fail_(PB_EINVAL, "null plan");
     const HostPlan &H = p->H;
     const size_t nfc = (size_t)p->pat_nnz[0], nfb = (size_t)p->pat_nnz[1];
     int rc;
@@ -748,11 +730,11 @@ static DevBuf *output_slot(pb_plan *p, int key, int64_t *n) {
 }
 
 extern "C" int pb_plan_take_output(pb_plan *p, int key, pb_values **out) {
-    if (!p || !out) return fail(PB_EINVAL, "null pointer");
+    if (!p || !out) return pb_fail_(PB_EINVAL, "null pointer");
     int64_t n = 0;
     DevBuf *slot = output_slot(p, key, &n);
-    if (!slot) return fail(PB_EINVAL, "unknown output key");
-    if (!slot->p || slot->bytes < (size_t)n * sizeof(double)) return fail(PB_EINVAL, "output was not assembled");
+    if (!slot) return pb_fail_(PB_EINVAL, "unknown output key");
+    if (!slot->p || slot->bytes < (size_t)n * sizeof(double)) return pb_fail_(PB_EINVAL, "output was not assembled");
     pb_values *v = new pb_values;
     v->buf = std::move(*slot);   // the plan allocates a fresh array at its next assemble
     v->n = n;
@@ -763,7 +745,7 @@ extern "C" int pb_plan_take_output(pb_plan *p, int key, pb_values **out) {
 extern "C" int64_t pb_values_size(const pb_values *v) { return v ? v->n : -1; }
 extern "C" void pb_values_destroy(pb_values *v) { delete v; }
 extern "C" int pb_values_download(pb_values *v, double *host) {
-    if (!v || !host) return fail(PB_EINVAL, "null pointer");
+    if (!v || !host) return pb_fail_(PB_EINVAL, "null pointer");
     if (v->n) CUDA_TRY(cudaMemcpy(host, v->buf.p, (size_t)v->n * sizeof(double), cudaMemcpyDeviceToHost));
     return PB_OK;
 }
@@ -781,9 +763,8 @@ int pb_checksum_dev_(const double *v, int64_t n, double *sum, double *sumsq) {
     DevBuf o;
     CUDA_TRY(o.ensure(16));
     CUDA_TRY(cudaMemset(o.p, 0, 16));
-    const int grid = (int)std::max<int64_t>(1, std::min<int64_t>((n + 255) / 256, (int64_t)pb_sm_count() * 8));
-    values_checksum_kernel<<<grid, 256>>>(n, v, o.as<double>());
-    g_launches++;
+    values_checksum_kernel<<<grid_stride_blocks(n, 256, 8), 256>>>(n, v, o.as<double>());
+    pb_count_launch_();
     double h[2];
     CUDA_TRY(cudaMemcpy(h, o.p, 16, cudaMemcpyDeviceToHost));
     if (sum) *sum = h[0];
@@ -791,7 +772,7 @@ int pb_checksum_dev_(const double *v, int64_t n, double *sum, double *sumsq) {
     return PB_OK;
 }
 extern "C" int pb_values_checksum(pb_values *v, double *sum, double *sumsq) {
-    if (!v) return fail(PB_EINVAL, "null pointer");
+    if (!v) return pb_fail_(PB_EINVAL, "null pointer");
     CUDA_TRY(cudaStreamSynchronize(v->stream));
     return pb_checksum_dev_(v->buf.as<double>(), v->n, sum, sumsq);
 }
@@ -799,11 +780,6 @@ extern "C" int pb_values_checksum(pb_values *v, double *sum, double *sumsq) {
 // ------------------------------------------------------------------------------------
 // device-side flow system  A = div @ flux,  b = -div @ (bound_flux @ bc [+ vector_source @ v])
 // ------------------------------------------------------------------------------------
-struct pb_csr;
-int pb_csr_from_device_pattern_(int64_t nrows, int64_t ncols, int64_t nnz, const int32_t *indptr_dev,
-                                const int32_t *indices_dev, pb_csr **out);  // spmv.cu
-double *pb_csr_data_(pb_csr *a);
-
 // one warp per face: every entry (f, k) of the flux row goes to row c of A for the one or two
 // cells c of the face, with the sign of cell_faces[f, c] (= div[c, f]); position by binary search
 // in the CELL_CELL row (the flux row's columns are a subset of it)
@@ -866,69 +842,63 @@ __global__ void neg_div_kernel(int64_t nf, const int32_t *__restrict__ face_cell
 
 static int ensure_face_cells(pb_plan *p) {
     if (p->face_cells.p) return PB_OK;  // uploaded by pb_plan_create
-    return fail(PB_EINVAL, "plan has no face->cell table");
+    return pb_fail_(PB_EINVAL, "plan has no face->cell table");
 }
-
-int pb_csr_alloc_(int64_t nrows, int64_t ncols, int64_t nnz, pb_csr **out);  // spmv.cu
-int32_t *pb_csr_indptr_(pb_csr *a);
-int32_t *pb_csr_indices_(pb_csr *a);
 
 // One output matrix as a device CSR (the block-expanded pattern + a copy of the values): the operand form of the
 // device-side AD chain (sparse_ops.cu).  which / br / bc as in pb_plan_pattern_expanded.
 extern "C" int pb_plan_output_csr(pb_plan *p, const pb_values *v, int which, int br, int bc, pb_csr **out) {
-    if (!p || !v || !out || which < 0 || which > 3 || br < 1 || bc < 1) return fail(PB_EINVAL, "bad arguments");
+    if (!p || !v || !out || which < 0 || which > 3 || br < 1 || bc < 1) return pb_fail_(PB_EINVAL, "bad arguments");
     const int64_t nrows = p->pat_rows[which], nnz = p->pat_nnz[which] * br * bc;
-    if (v->n != nnz) return fail(PB_EINVAL, "values do not match this pattern / block size");
-    if (nnz >= 0x7FFFFFFFll || p->pat_cols[which] * bc >= 0x7FFFFFFFll) return fail(PB_ENOTIMPL, "matrix does not fit int32 indices");
-    pb_csr *a = nullptr;
-    int rc = pb_csr_alloc_(nrows * br, p->pat_cols[which] * bc, nnz, &a);
+    if (v->n != nnz) return pb_fail_(PB_EINVAL, "values do not match this pattern / block size");
+    if (nnz >= 0x7FFFFFFFll || p->pat_cols[which] * bc >= 0x7FFFFFFFll) return pb_fail_(PB_ENOTIMPL, "matrix does not fit int32 indices");
+    CsrPtr a;
+    int rc = pb_csr_alloc_(nrows * br, p->pat_cols[which] * bc, nnz, a);
     if (rc) return rc;
-    rc = expand_pattern(p, which, br, bc, pb_csr_indptr_(a), pb_csr_indices_(a));
+    const CsrView A = pb_csr_view_(a.get());
+    rc = expand_pattern(p, which, br, bc, A.indptr, A.indices);
     if (rc) return rc;
-    if (nnz) CUDA_TRY(cudaMemcpyAsync(pb_csr_data_(a), v->buf.p, (size_t)nnz * sizeof(double), cudaMemcpyDeviceToDevice, p->stream));
+    if (nnz) CUDA_TRY(cudaMemcpyAsync(A.data, v->buf.p, (size_t)nnz * sizeof(double), cudaMemcpyDeviceToDevice, p->stream));
     CUDA_TRY(cudaStreamSynchronize(p->stream));
-    *out = a;
+    *out = a.release();
     return PB_OK;
 }
 
 extern "C" int pb_mpfa_system(pb_plan *p, const pb_values *flux, pb_csr **out) {
     NvtxRange nvtx_("pb_mpfa_system");
-    if (!p || !out) return fail(PB_EINVAL, "null pointer");
+    if (!p || !out) return pb_fail_(PB_EINVAL, "null pointer");
     const double *flux_dev = flux ? flux->buf.as<double>() : p->o_flux.as<double>();
-    if (flux && flux->n != p->pat_nnz[0]) return fail(PB_EINVAL, "flux values do not belong to this plan");
-    if (!flux_dev) return fail(PB_EINVAL, "pb_mpfa_assemble (flux terms) has not been called");
+    if (flux && flux->n != p->pat_nnz[0]) return pb_fail_(PB_EINVAL, "flux values do not belong to this plan");
+    if (!flux_dev) return pb_fail_(PB_EINVAL, "pb_mpfa_assemble (flux terms) has not been called");
     const HostPlan &H = p->H;
     int rc = ensure_face_cells(p);
     if (rc) return rc;
     CUDA_TRY(cudaStreamSynchronize(p->stream));
-    pb_csr *a = nullptr;
+    CsrPtr a;
     rc = pb_csr_from_device_pattern_(H.nc, H.nc, p->pat_nnz[2], p->pat_ip[2].as<int32_t>(),
-                                     p->pat_idx[2].as<int32_t>(), &a);
+                                     p->pat_idx[2].as<int32_t>(), a);
     if (rc) return rc;
-    const int block = 256;
-    int grid = (int)std::max<int64_t>(1, std::min<int64_t>((H.nf * 32 + block - 1) / block, (int64_t)pb_sm_count() * 16));
-    div_flux_kernel<<<grid, block, 0, p->stream>>>(H.nf, p->pat_ip[0].as<int32_t>(), p->pat_idx[0].as<int32_t>(),
-                                                   flux_dev, p->face_cells.as<int32_t>(),
-                                                   p->pat_ip[2].as<int32_t>(), p->pat_idx[2].as<int32_t>(),
-                                                   pb_csr_data_(a));
-    g_launches++;
+    div_flux_kernel<<<grid_stride_blocks(H.nf * 32, 256, 16), 256, 0, p->stream>>>(
+        H.nf, p->pat_ip[0].as<int32_t>(), p->pat_idx[0].as<int32_t>(), flux_dev, p->face_cells.as<int32_t>(),
+        p->pat_ip[2].as<int32_t>(), p->pat_idx[2].as<int32_t>(), pb_csr_view_(a.get()).data);
+    pb_count_launch_();
     CUDA_TRY(cudaGetLastError());
     CUDA_TRY(cudaStreamSynchronize(p->stream));
-    *out = a;
+    *out = a.release();
     return PB_OK;
 }
 
 extern "C" int pb_mpfa_rhs(pb_plan *p, const pb_values *bound_flux, const pb_values *vector_source_discr,
                            const double *bc_values, const double *vector_source, double *rhs) {
     NvtxRange nvtx_("pb_mpfa_rhs");
-    if (!p || !bc_values || !rhs) return fail(PB_EINVAL, "null pointer");
+    if (!p || !bc_values || !rhs) return pb_fail_(PB_EINVAL, "null pointer");
     const double *bflux_dev = bound_flux ? bound_flux->buf.as<double>() : p->o_bflux.as<double>();
     const double *vs_dev = vector_source_discr ? vector_source_discr->buf.as<double>() : p->o_vs.as<double>();
-    if (bound_flux && bound_flux->n != p->pat_nnz[1]) return fail(PB_EINVAL, "bound_flux values do not belong to this plan");
+    if (bound_flux && bound_flux->n != p->pat_nnz[1]) return pb_fail_(PB_EINVAL, "bound_flux values do not belong to this plan");
     if (vector_source_discr && vector_source_discr->n != p->pat_nnz[0] * p->H.nd)
-        return fail(PB_EINVAL, "vector_source values do not belong to this plan");
-    if (!bflux_dev) return fail(PB_EINVAL, "pb_mpfa_assemble (flux terms) has not been called");
-    if (vector_source && !vs_dev) return fail(PB_EINVAL, "vector source terms were not assembled");
+        return pb_fail_(PB_EINVAL, "vector_source values do not belong to this plan");
+    if (!bflux_dev) return pb_fail_(PB_EINVAL, "pb_mpfa_assemble (flux terms) has not been called");
+    if (vector_source && !vs_dev) return pb_fail_(PB_EINVAL, "vector source terms were not assembled");
     const HostPlan &H = p->H;
     cudaStream_t st = p->stream;
     int rc = ensure_face_cells(p);
@@ -939,20 +909,19 @@ extern "C" int pb_mpfa_rhs(pb_plan *p, const pb_values *bound_flux, const pb_val
     CUDA_TRY(r.ensure((size_t)H.nc * sizeof(double)));
     CUDA_TRY(cudaMemsetAsync(w.p, 0, (size_t)H.nf * sizeof(double), st));
     CUDA_TRY(cudaMemsetAsync(r.p, 0, (size_t)H.nc * sizeof(double), st));
-    const int block = 256;
-    int grid = (int)std::max<int64_t>(1, std::min<int64_t>((H.nf * 32 + block - 1) / block, (int64_t)pb_sm_count() * 16));
+    const int block = 256, grid = grid_stride_blocks(H.nf * 32, block, 16);
     face_row_dot_kernel<<<grid, block, 0, st>>>(H.nf, p->pat_ip[1].as<int32_t>(), p->pat_idx[1].as<int32_t>(),
                                                 bflux_dev, 1, bc.as<double>(), w.as<double>());
-    g_launches++;
+    pb_count_launch_();
     if (vector_source) {
         CUDA_TRY(vs.upload(vector_source, (size_t)H.nc * H.nd, st));
         face_row_dot_kernel<<<grid, block, 0, st>>>(H.nf, p->pat_ip[0].as<int32_t>(), p->pat_idx[0].as<int32_t>(),
                                                     vs_dev, H.nd, vs.as<double>(), w.as<double>());
-        g_launches++;
+        pb_count_launch_();
     }
-    int grid2 = (int)std::max<int64_t>(1, std::min<int64_t>((H.nf + block - 1) / block, (int64_t)pb_sm_count() * 16));
-    neg_div_kernel<<<grid2, block, 0, st>>>(H.nf, p->face_cells.as<int32_t>(), w.as<double>(), r.as<double>());
-    g_launches++;
+    neg_div_kernel<<<grid_stride_blocks(H.nf, block, 16), block, 0, st>>>(H.nf, p->face_cells.as<int32_t>(),
+                                                                          w.as<double>(), r.as<double>());
+    pb_count_launch_();
     CUDA_TRY(cudaGetLastError());
     CUDA_TRY(cudaMemcpyAsync(rhs, r.p, (size_t)H.nc * sizeof(double), cudaMemcpyDeviceToHost, st));
     CUDA_TRY(cudaStreamSynchronize(st));
@@ -1046,13 +1015,13 @@ __global__ void neg_div_nd_kernel(int64_t nf, int nd, const int32_t *__restrict_
 
 extern "C" int pb_mpsa_system(pb_plan *p, const pb_values *stress, pb_csr **out) {
     NvtxRange nvtx_("pb_mpsa_system");
-    if (!p || !out) return fail(PB_EINVAL, "null pointer");
+    if (!p || !out) return pb_fail_(PB_EINVAL, "null pointer");
     const double *stress_dev = stress ? stress->buf.as<double>() : p->o_stress.as<double>();
-    if (stress && stress->n != p->pat_nnz[0] * p->H.nd * p->H.nd) return fail(PB_EINVAL, "stress values do not belong to this plan");
-    if (!stress_dev) return fail(PB_EINVAL, "pb_mpsa_assemble has not been called");
+    if (stress && stress->n != p->pat_nnz[0] * p->H.nd * p->H.nd) return pb_fail_(PB_EINVAL, "stress values do not belong to this plan");
+    if (!stress_dev) return pb_fail_(PB_EINVAL, "pb_mpsa_assemble has not been called");
     const HostPlan &H = p->H;
     const int nd = H.nd, nd2 = nd * nd;
-    if ((int64_t)p->pat_nnz[2] * nd2 >= 0x7FFFFFFFll) return fail(PB_ENOTIMPL, "system matrix does not fit int32 indices");
+    if ((int64_t)p->pat_nnz[2] * nd2 >= 0x7FFFFFFFll) return pb_fail_(PB_ENOTIMPL, "system matrix does not fit int32 indices");
     cudaStream_t st = p->stream;
     // block-expanded CELL_CELL pattern on the device
     DevBuf nip, nix;
@@ -1061,30 +1030,30 @@ extern "C" int pb_mpsa_system(pb_plan *p, const pb_values *stress, pb_csr **out)
     int rc = expand_pattern(p, 2, nd, nd, nip.as<int32_t>(), nix.as<int32_t>());
     if (rc) return rc;
     CUDA_TRY(cudaStreamSynchronize(st));
-    pb_csr *a = nullptr;
-    rc = pb_csr_from_device_pattern_(H.nc * nd, H.nc * nd, p->pat_nnz[2] * nd2, nip.as<int32_t>(), nix.as<int32_t>(), &a);
+    CsrPtr a;
+    rc = pb_csr_from_device_pattern_(H.nc * nd, H.nc * nd, p->pat_nnz[2] * nd2, nip.as<int32_t>(), nix.as<int32_t>(), a);
     if (rc) return rc;
     constexpr int kWarps = 4, kCap = 128;           // 4 x 128 x 9 doubles = 36 KB of shared memory per block
-    int gridg = (int)std::max<int64_t>(1, std::min<int64_t>((H.nc + kWarps - 1) / kWarps, (int64_t)pb_sm_count() * 24));
+    const int gridg = grid_stride_blocks(H.nc, kWarps, 24);
     div_stress_gather_kernel<kWarps><<<gridg, kWarps * 32, (size_t)kWarps * kCap * nd2 * sizeof(double), st>>>(
         H.nc, nd, p->cf_ip.as<int32_t>(), p->cf_ix.as<int32_t>(), p->cf_sg.as<int8_t>(), p->pat_ip[0].as<int32_t>(),
         p->pat_idx[0].as<int32_t>(), stress_dev, p->pat_ip[2].as<int32_t>(), p->pat_idx[2].as<int32_t>(),
-        pb_csr_data_(a), kCap);
-    g_launches++;
+        pb_csr_view_(a.get()).data, kCap);
+    pb_count_launch_();
     CUDA_TRY(cudaGetLastError());
     CUDA_TRY(cudaStreamSynchronize(st));
-    *out = a;
+    *out = a.release();
     return PB_OK;
 }
 
 extern "C" int pb_mpsa_rhs(pb_plan *p, const pb_values *bound_stress, const double *bc_values, const double *source,
                            double *rhs) {
     NvtxRange nvtx_("pb_mpsa_rhs");
-    if (!p || !bc_values || !rhs) return fail(PB_EINVAL, "null pointer");
+    if (!p || !bc_values || !rhs) return pb_fail_(PB_EINVAL, "null pointer");
     const double *bstress_dev = bound_stress ? bound_stress->buf.as<double>() : p->o_bstress.as<double>();
     if (bound_stress && bound_stress->n != p->pat_nnz[1] * p->H.nd * p->H.nd)
-        return fail(PB_EINVAL, "bound_stress values do not belong to this plan");
-    if (!bstress_dev) return fail(PB_EINVAL, "pb_mpsa_assemble has not been called");
+        return pb_fail_(PB_EINVAL, "bound_stress values do not belong to this plan");
+    if (!bstress_dev) return pb_fail_(PB_EINVAL, "pb_mpsa_assemble has not been called");
     const HostPlan &H = p->H;
     const int nd = H.nd;
     cudaStream_t st = p->stream;
@@ -1097,12 +1066,13 @@ extern "C" int pb_mpsa_rhs(pb_plan *p, const pb_values *bound_stress, const doub
     if (source) CUDA_TRY(cudaMemcpyAsync(r.p, source, (size_t)H.nc * nd * sizeof(double), cudaMemcpyHostToDevice, st));
     else CUDA_TRY(cudaMemsetAsync(r.p, 0, (size_t)H.nc * nd * sizeof(double), st));
     const int block = 256;
-    int grid = (int)std::max<int64_t>(1, std::min<int64_t>((H.nf * nd * 32 + block - 1) / block, (int64_t)pb_sm_count() * 16));
-    bound_stress_dot_kernel<<<grid, block, 0, st>>>(H.nf, nd, p->pat_ip[1].as<int32_t>(), p->pat_idx[1].as<int32_t>(),
-                                                    bstress_dev, bc.as<double>(), w.as<double>());
-    int grid2 = (int)std::max<int64_t>(1, std::min<int64_t>((H.nf * nd + block - 1) / block, (int64_t)pb_sm_count() * 16));
-    neg_div_nd_kernel<<<grid2, block, 0, st>>>(H.nf, nd, p->face_cells.as<int32_t>(), w.as<double>(), r.as<double>());
-    g_launches += 2;
+    bound_stress_dot_kernel<<<grid_stride_blocks(H.nf * nd * 32, block, 16), block, 0, st>>>(
+        H.nf, nd, p->pat_ip[1].as<int32_t>(), p->pat_idx[1].as<int32_t>(), bstress_dev, bc.as<double>(),
+        w.as<double>());
+    neg_div_nd_kernel<<<grid_stride_blocks(H.nf * nd, block, 16), block, 0, st>>>(H.nf, nd, p->face_cells.as<int32_t>(),
+                                                                                  w.as<double>(), r.as<double>());
+    pb_count_launch_();
+    pb_count_launch_();
     CUDA_TRY(cudaGetLastError());
     CUDA_TRY(cudaMemcpyAsync(rhs, r.p, (size_t)H.nc * nd * sizeof(double), cudaMemcpyDeviceToHost, st));
     CUDA_TRY(cudaStreamSynchronize(st));
@@ -1116,10 +1086,10 @@ extern "C" int pb_mpsa_upload(pb_plan *p, const double *stiffness, const uint8_t
                               const double *robin_weight, double eta, int n_alpha,
                               const double *alpha) {
     NvtxRange nvtx_("pb_mpsa_upload");
-    if (!p || !stiffness || !bc) return fail(PB_EINVAL, "null pointer");
-    if (!p->have_geo) return fail(PB_EINVAL, "pb_plan_set_geometry has not been called");
-    if (n_alpha < 0 || n_alpha > PB_MAX_ALPHA) return fail(PB_EINVAL, "0 <= n_alpha <= 4");
-    if (n_alpha > 0 && !alpha) return fail(PB_EINVAL, "null alpha");
+    if (!p || !stiffness || !bc) return pb_fail_(PB_EINVAL, "null pointer");
+    if (!p->have_geo) return pb_fail_(PB_EINVAL, "pb_plan_set_geometry has not been called");
+    if (n_alpha < 0 || n_alpha > PB_MAX_ALPHA) return pb_fail_(PB_EINVAL, "0 <= n_alpha <= 4");
+    if (n_alpha > 0 && !alpha) return pb_fail_(PB_EINVAL, "null alpha");
     const HostPlan &H = p->H;
     const int nd = H.nd;
     cudaStream_t st = p->stream;
@@ -1158,8 +1128,8 @@ extern "C" int pb_mpsa_upload(pb_plan *p, const double *stiffness, const uint8_t
 }
 
 extern "C" int pb_mpsa_set_basis(pb_plan *p, const double *basis) {
-    if (!p) return fail(PB_EINVAL, "null plan");
-    if (!p->mpsa_ready) return fail(PB_EINVAL, "pb_mpsa_upload has not been called");
+    if (!p) return pb_fail_(PB_EINVAL, "null plan");
+    if (!p->mpsa_ready) return pb_fail_(PB_EINVAL, "pb_mpsa_upload has not been called");
     p->have_vbasis = basis != nullptr;
     if (basis) {
         const HostPlan &H = p->H;
@@ -1171,8 +1141,8 @@ extern "C" int pb_mpsa_set_basis(pb_plan *p, const double *basis) {
 
 extern "C" int pb_mpsa_assemble(pb_plan *p, float *ms) {
     NvtxRange nvtx_("pb_mpsa_assemble");
-    if (!p) return fail(PB_EINVAL, "null plan");
-    if (!p->mpsa_ready) return fail(PB_EINVAL, "pb_mpsa_upload has not been called");
+    if (!p) return pb_fail_(PB_EINVAL, "null plan");
+    if (!p->mpsa_ready) return pb_fail_(PB_EINVAL, "pb_mpsa_upload has not been called");
     const HostPlan &H = p->H;
     const int nd = H.nd;
     cudaStream_t st = p->stream;
@@ -1191,7 +1161,7 @@ extern "C" int pb_mpsa_assemble(pb_plan *p, float *ms) {
         reqs.push_back({&p->o_bdp[a], &o.bdp[a], nfc * nd});
     }
     for (auto &r : reqs) CUDA_TRY(r.b->ensure(r.n * sizeof(double)));
-    CUDA_TRY(cudaEventRecord(p->e0, st));
+    CUDA_TRY(p->timer.mark(0, st));
     for (auto &r : reqs) {
         CUDA_TRY(cudaMemsetAsync(r.b->p, 0, r.n * sizeof(double), st));
         *r.slot = r.b->as<double>();
@@ -1203,15 +1173,15 @@ extern "C" int pb_mpsa_assemble(pb_plan *p, float *ms) {
                    p->have_vbasis ? p->vbasis.as<double>() : nullptr, p->veta, p->n_alpha,
                    p->n_alpha ? p->alpha.as<double>() : nullptr, 1, 81, 1, 9, 9 * H.nc};
     { int rc = nd == 3 ? pb_launch_mpsa3_(p, prm, o) : pb_launch_mpsa2_(p, prm, o); if (rc) return rc; }
-    CUDA_TRY(cudaEventRecord(p->e1, st));
-    CUDA_TRY(cudaEventSynchronize(p->e1));
-    if (ms) CUDA_TRY(cudaEventElapsedTime(ms, p->e0, p->e1));
+    CUDA_TRY(p->timer.mark(1, st));
+    CUDA_TRY(cudaEventSynchronize(p->timer.ev[1]));
+    if (ms) CUDA_TRY(p->timer.ms(ms));
     return check_singular(p);
 }
 
 extern "C" int pb_mpsa_download(pb_plan *p, double *stress, double *bound_stress, double *bdc,
                                 double *bdf) {
-    if (!p) return fail(PB_EINVAL, "null plan");
+    if (!p) return pb_fail_(PB_EINVAL, "null plan");
     const HostPlan &H = p->H;
     const size_t nd2 = (size_t)H.nd * H.nd;
     int rc;
@@ -1225,8 +1195,8 @@ extern "C" int pb_mpsa_download(pb_plan *p, double *stress, double *bound_stress
 
 extern "C" int pb_biot_download(pb_plan *p, int a, double *dd, double *bdd, double *sg, double *cons,
                                 double *bdp) {
-    if (!p) return fail(PB_EINVAL, "null plan");
-    if (a < 0 || a >= p->n_alpha) return fail(PB_EINVAL, "coupling tensor index out of range");
+    if (!p) return pb_fail_(PB_EINVAL, "null plan");
+    if (a < 0 || a >= p->n_alpha) return pb_fail_(PB_EINVAL, "coupling tensor index out of range");
     const HostPlan &H = p->H;
     const size_t nd = H.nd;
     int rc;

@@ -6,16 +6,10 @@
 #include "csr_build.cuh"
 #include "dual_hybrid.cuh"
 
-struct pb_csr;
-int pb_csr_from_device_pattern_(int64_t nrows, int64_t ncols, int64_t nnz, const int32_t *indptr_dev,
-                                const int32_t *indices_dev, pb_csr **out);   // spmv.cu
-double *pb_csr_data_(pb_csr *a);                                              // spmv.cu
-extern "C" void pb_csr_destroy(pb_csr *a);
-
 struct pb_dual {
     int nd = 0;
     int64_t nc = 0, nf = 0, nn = 0, ncf = 0, mass_nnz = -1;   // mass_nnz < 0: pattern not built yet
-    cudaStream_t stream = nullptr;
+    Stream stream;
     DevBuf cf_ip, cf_ix, cf_sg, cf_cell, fc_ip, fc_cell, fn_ip, fn_ix, mass_ip, mass_ix;
     std::vector<int32_t> cf_ip_h;
     // values of the last pb_dual_discretize, kept for pb_dual_download and pb_dual_system
@@ -27,13 +21,11 @@ struct pb_dual {
     // saddle-point pattern (pb_dual_system), built at its first call
     int64_t sys_nnz = -1;
     DevBuf sys_ip, sys_ix;
+    // the stream's copies and kernels may still use the buffers, which go back to the pool right after
+    ~pb_dual() { if (stream) cudaStreamSynchronize(stream); }
 };
 
-extern "C" void pb_dual_destroy(pb_dual *d) {
-    if (!d) return;
-    if (d->stream) { cudaStreamSynchronize(d->stream); cudaStreamDestroy(d->stream); }
-    delete d;
-}
+extern "C" void pb_dual_destroy(pb_dual *d) { delete d; }
 
 extern "C" int pb_dual_create(int nd, int64_t nc, int64_t nf, int64_t nn, const int32_t *cf_indptr,
                               const int32_t *cf_indices, const int8_t *cf_data, const int32_t *fn_indptr,
@@ -42,9 +34,7 @@ extern "C" int pb_dual_create(int nd, int64_t nc, int64_t nf, int64_t nn, const 
         return pb_fail_(PB_EINVAL, "null pointer");
     if (nd < 1 || nd > 3) return pb_fail_(PB_EINVAL, "MVEM / RT0 discretize grids of dimension 1, 2 or 3");
     if (nc <= 0 || nf <= 0 || nn <= 0 || nc >= INT_MAX || nf >= INT_MAX) return pb_fail_(PB_EINVAL, "grid size");
-    int ndev = 0;
-    if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev < 1)
-        return pb_fail_(PB_ECUDA, "no CUDA device: libporeb200 has no CPU path");
+    if (int rc = pb_require_device()) return rc;
     const int64_t ncf = cf_indptr[nc];
     std::vector<int32_t> cf_cell((size_t)ncf), fc_ip((size_t)nf + 1, 0), fc_cell((size_t)ncf);
     for (int64_t c = 0; c < nc; ++c)
@@ -66,27 +56,21 @@ extern "C" int pb_dual_create(int nd, int64_t nc, int64_t nf, int64_t nn, const 
         std::vector<int32_t> next(fc_ip.begin(), fc_ip.end() - 1);
         for (int64_t q = 0; q < ncf; ++q) fc_cell[next[cf_indices[q]]++] = cf_cell[q];
     }
-    pb_dual *d = new pb_dual;
+    std::unique_ptr<pb_dual> d(new pb_dual);
     d->nd = nd; d->nc = nc; d->nf = nf; d->nn = nn; d->ncf = ncf;
     d->cf_ip_h.assign(cf_indptr, cf_indptr + nc + 1);
-    auto bail = [&](cudaError_t e, const char *what) {
-        pb_dual_destroy(d);
-        return pb_fail_(PB_ECUDA, std::string(what) + ": " + cudaGetErrorString(e));
-    };
-#define DU_TRY(x) do { cudaError_t e_ = (x); if (e_ != cudaSuccess) return bail(e_, #x); } while (0)
-    DU_TRY(cudaStreamCreateWithFlags(&d->stream, cudaStreamNonBlocking));
+    CUDA_TRY(d->stream.create());
     cudaStream_t st = d->stream;
-    DU_TRY(d->cf_ip.upload(cf_indptr, (size_t)nc + 1, st));
-    DU_TRY(d->cf_ix.upload(cf_indices, (size_t)ncf, st));
-    DU_TRY(d->cf_sg.upload(cf_data, (size_t)ncf, st));
-    DU_TRY(d->cf_cell.upload(cf_cell, st));
-    DU_TRY(d->fc_ip.upload(fc_ip, st));
-    DU_TRY(d->fc_cell.upload(fc_cell, st));
-    DU_TRY(d->fn_ip.upload(fn_indptr, (size_t)nf + 1, st));
-    DU_TRY(d->fn_ix.upload(fn_indices, (size_t)fn_indptr[nf], st));
-    DU_TRY(cudaStreamSynchronize(st));
-#undef DU_TRY
-    *out = d;
+    CUDA_TRY(d->cf_ip.upload(cf_indptr, (size_t)nc + 1, st));
+    CUDA_TRY(d->cf_ix.upload(cf_indices, (size_t)ncf, st));
+    CUDA_TRY(d->cf_sg.upload(cf_data, (size_t)ncf, st));
+    CUDA_TRY(d->cf_cell.upload(cf_cell, st));
+    CUDA_TRY(d->fc_ip.upload(fc_ip, st));
+    CUDA_TRY(d->fc_cell.upload(fc_cell, st));
+    CUDA_TRY(d->fn_ip.upload(fn_indptr, (size_t)nf + 1, st));
+    CUDA_TRY(d->fn_ix.upload(fn_indices, (size_t)fn_indptr[nf], st));
+    CUDA_TRY(cudaStreamSynchronize(st));
+    *out = d.release();
     return PB_OK;
 }
 
@@ -99,7 +83,7 @@ static int dual_build_pattern(pb_dual *d) {
     CUDA_TRY(flag.ensure(sizeof(int)));
     CUDA_TRY(cudaMemsetAsync(flag.p, 0, sizeof(int), st));
     CUDA_TRY(d->mass_ip.ensure((size_t)(nf + 1) * sizeof(int32_t)));
-    const int grid = (int)std::max<int64_t>(1, std::min<int64_t>((nf + 7) / 8, (int64_t)pb_sm_count() * 8));
+    const int grid = grid_stride_blocks(nf, 8, 8);
     pattern_kernel<256><<<grid, 256, 0, st>>>(nf, d->fc_ip.as<int32_t>(), d->fc_cell.as<int32_t>(),
                                               d->cf_ip.as<int32_t>(), d->cf_ix.as<int32_t>(), counts.as<int32_t>(),
                                               nullptr, nullptr, 0, flag.as<int>());
@@ -139,18 +123,17 @@ extern "C" int pb_dual_mass_pattern(pb_dual *d, int64_t *nnz, int32_t *indptr, i
     return PB_OK;
 }
 
+static pb::DualTopo dual_topo(pb_dual *d) {
+    return pb::DualTopo{d->cf_ip.as<int32_t>(), d->cf_ix.as<int32_t>(), d->cf_cell.as<int32_t>(),
+                        d->cf_sg.as<int8_t>(), d->fn_ip.as<int32_t>(), d->fn_ix.as<int32_t>(),
+                        d->mass_ip.as<int32_t>(), d->mass_ix.as<int32_t>()};
+}
+
 template <int ND, int METHOD>
 __global__ void dual_kernel(int64_t ncf, pb::DualTopo T, pb::DualGeo G, double *__restrict__ mass,
                             double *__restrict__ proj, int32_t *bad) {
     for (int64_t q = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; q < ncf; q += (int64_t)gridDim.x * blockDim.x)
         pb::dual_row<ND>(METHOD, q, T, G, mass, proj, bad);
-}
-
-template <int ND>
-static void dual_launch(int method, int grid, cudaStream_t st, int64_t ncf, const pb::DualTopo &T,
-                        const pb::DualGeo &G, double *mass, double *proj, int32_t *bad) {
-    if (method == PB_DUAL_MVEM) dual_kernel<ND, pb::kDualMvem><<<grid, 256, 0, st>>>(ncf, T, G, mass, proj, bad);
-    else dual_kernel<ND, pb::kDualRt0><<<grid, 256, 0, st>>>(ncf, T, G, mass, proj, bad);
 }
 
 extern "C" int pb_dual_discretize(pb_dual *d, int method, const double *nodes, const double *face_normals,
@@ -190,35 +173,27 @@ extern "C" int pb_dual_discretize(pb_dual *d, int method, const double *nodes, c
     CUDA_TRY(cudaMemsetAsync(dmass.p, 0, (size_t)d->mass_nnz * sizeof(double), st));
     const int32_t none = INT_MAX;
     CUDA_TRY(cudaMemcpyAsync(dbad.p, &none, sizeof(int32_t), cudaMemcpyHostToDevice, st));
-    const pb::DualTopo T{d->cf_ip.as<int32_t>(), d->cf_ix.as<int32_t>(), d->cf_cell.as<int32_t>(),
-                         d->cf_sg.as<int8_t>(), d->fn_ip.as<int32_t>(), d->fn_ix.as<int32_t>(),
-                         d->mass_ip.as<int32_t>(), d->mass_ix.as<int32_t>()};
+    const pb::DualTopo T = dual_topo(d);
     const pb::DualGeo G{nn, nf, nc, dn.as<double>(), dfn.as<double>(), dfc.as<double>(), dcc.as<double>(),
                         dvol.as<double>(), dperm.as<double>(), drot.as<double>()};
-    cudaEvent_t e0 = nullptr, e1 = nullptr;
-    struct Guard {
-        cudaEvent_t &a, &b;
-        ~Guard() { if (a) cudaEventDestroy(a); if (b) cudaEventDestroy(b); }
-    } guard{e0, e1};
-    CUDA_TRY(cudaEventCreate(&e0));
-    CUDA_TRY(cudaEventCreate(&e1));
-    CUDA_TRY(cudaEventRecord(e0, st));
-    const int grid = (int)std::max<int64_t>(1, std::min<int64_t>((ncf + 255) / 256, (int64_t)pb_sm_count() * 16));
-    double *m = dmass.as<double>(), *p = dproj.as<double>();
-    int32_t *b = dbad.as<int32_t>();
-    if (nd == 1) dual_launch<1>(method, grid, st, ncf, T, G, m, p, b);
-    else if (nd == 2) dual_launch<2>(method, grid, st, ncf, T, G, m, p, b);
-    else dual_launch<3>(method, grid, st, ncf, T, G, m, p, b);
+    KernelTimer timer;
+    CUDA_TRY(timer.create());
+    CUDA_TRY(timer.mark(0, st));
+    dispatch_nd<1, 2, 3>(nd, [&](auto ND) {
+        auto kernel = method == PB_DUAL_MVEM ? dual_kernel<ND, pb::kDualMvem> : dual_kernel<ND, pb::kDualRt0>;
+        kernel<<<grid_stride_blocks(ncf, 256, 16), 256, 0, st>>>(ncf, T, G, dmass.as<double>(), dproj.as<double>(),
+                                                                 dbad.as<int32_t>());
+    });
     pb_count_launch_();
     CUDA_TRY(cudaGetLastError());
-    CUDA_TRY(cudaEventRecord(e1, st));
+    CUDA_TRY(timer.mark(1, st));
     int32_t hbad = none;
     if (mass) CUDA_TRY(cudaMemcpyAsync(mass, dmass.p, (size_t)d->mass_nnz * sizeof(double), cudaMemcpyDeviceToHost, st));
     if (proj) CUDA_TRY(cudaMemcpyAsync(proj, dproj.p, (size_t)3 * ncf * sizeof(double), cudaMemcpyDeviceToHost, st));
     CUDA_TRY(cudaMemcpyAsync(&hbad, dbad.p, sizeof(int32_t), cudaMemcpyDeviceToHost, st));
     CUDA_TRY(cudaStreamSynchronize(st));
     float ms = 0.0f;
-    CUDA_TRY(cudaEventElapsedTime(&ms, e0, e1));
+    CUDA_TRY(timer.ms(&ms));
     if (kernel_ms) *kernel_ms = ms;
     *bad_cell = hbad == none ? -1 : (int64_t)hbad;
     d->have_values = hbad == none;
@@ -341,7 +316,7 @@ extern "C" int pb_dual_system(pb_dual *d, const uint8_t *codes, const double *ro
     for (int64_t f = 0; f < nf; ++f)
         if (codes[f] > PB_BC_ROB) return pb_fail_(PB_EINVAL, "boundary code out of range");
     cudaStream_t st = d->stream;
-    const int grid = (int)std::max<int64_t>(1, std::min<int64_t>((nf + nc + 255) / 256, (int64_t)pb_sm_count() * 16));
+    const int grid = grid_stride_blocks(nf + nc, 256, 16);
     if (d->sys_nnz < 0) {
         DevBuf count;
         CUDA_TRY(count.ensure((size_t)(nf + nc) * sizeof(int32_t)));
@@ -364,24 +339,19 @@ extern "C" int pb_dual_system(pb_dual *d, const uint8_t *codes, const double *ro
         CUDA_TRY(cudaStreamSynchronize(st));
         d->sys_nnz = total;
     }
-    pb_csr *a = nullptr;
+    CsrPtr a;
     int rc = pb_csr_from_device_pattern_(nf + nc, nf + nc, d->sys_nnz, d->sys_ip.as<int32_t>(), d->sys_ix.as<int32_t>(),
-                                         &a);
+                                         a);
     if (rc) return rc;
-    auto fail_cuda = [&](cudaError_t e, const char *what) {
-        pb_csr_destroy(a);
-        return pb_fail_(PB_ECUDA, std::string(what) + ": " + cudaGetErrorString(e));
-    };
-#define DS_TRY(x) do { cudaError_t e_ = (x); if (e_ != cudaSuccess) return fail_cuda(e_, #x); } while (0)
     DevBuf dcodes, drw, darea, dbc, dvs, dnorm, drhs;
-    DS_TRY(dcodes.upload(codes, (size_t)nf, st));
-    DS_TRY(drw.upload(robin_weight, (size_t)nf, st));
-    DS_TRY(darea.upload(face_areas, (size_t)nf, st));
-    DS_TRY(dbc.upload(bc_values, (size_t)nf, st));
-    if (vector_source) DS_TRY(dvs.upload(vector_source, (size_t)3 * nc, st));
-    DS_TRY(dnorm.ensure(sizeof(unsigned long long)));
-    DS_TRY(drhs.ensure((size_t)(nf + nc) * sizeof(double)));
-    DS_TRY(cudaMemsetAsync(dnorm.p, 0, sizeof(unsigned long long), st));
+    CUDA_TRY(dcodes.upload(codes, (size_t)nf, st));
+    CUDA_TRY(drw.upload(robin_weight, (size_t)nf, st));
+    CUDA_TRY(darea.upload(face_areas, (size_t)nf, st));
+    CUDA_TRY(dbc.upload(bc_values, (size_t)nf, st));
+    if (vector_source) CUDA_TRY(dvs.upload(vector_source, (size_t)3 * nc, st));
+    CUDA_TRY(dnorm.ensure(sizeof(unsigned long long)));
+    CUDA_TRY(drhs.ensure((size_t)(nf + nc) * sizeof(double)));
+    CUDA_TRY(cudaMemsetAsync(dnorm.p, 0, sizeof(unsigned long long), st));
     dual_norm_kernel<<<grid, 256, 0, st>>>(nf, d->mass_ip.as<int32_t>(), d->mass_val.as<double>(),
                                            dnorm.as<unsigned long long>());
     dual_sys_values_kernel<<<grid, 256, 0, st>>>(
@@ -389,16 +359,15 @@ extern "C" int pb_dual_system(pb_dual *d, const uint8_t *codes, const double *ro
         d->fc_cell.as<int32_t>(), d->cf_ip.as<int32_t>(), d->cf_ix.as<int32_t>(), d->cf_sg.as<int8_t>(),
         d->proj_val.as<double>(), dcodes.as<uint8_t>(), drw.as<double>(), darea.as<double>(), dbc.as<double>(),
         vector_source ? dvs.as<double>() : nullptr, dnorm.as<unsigned long long>(), d->sys_ip.as<int32_t>(),
-        pb_csr_data_(a), drhs.as<double>());
+        pb_csr_view_(a.get()).data, drhs.as<double>());
     pb_count_launch_(); pb_count_launch_();
-    DS_TRY(cudaGetLastError());
+    CUDA_TRY(cudaGetLastError());
     unsigned long long nb = 0;
-    DS_TRY(cudaMemcpyAsync(rhs, drhs.p, (size_t)(nf + nc) * sizeof(double), cudaMemcpyDeviceToHost, st));
-    DS_TRY(cudaMemcpyAsync(&nb, dnorm.p, sizeof(nb), cudaMemcpyDeviceToHost, st));
-    DS_TRY(cudaStreamSynchronize(st));
-#undef DS_TRY
+    CUDA_TRY(cudaMemcpyAsync(rhs, drhs.p, (size_t)(nf + nc) * sizeof(double), cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(cudaMemcpyAsync(&nb, dnorm.p, sizeof(nb), cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(cudaStreamSynchronize(st));
     std::memcpy(norm, &nb, sizeof(double));
-    *out = a;
+    *out = a.release();
     return PB_OK;
 }
 
@@ -461,18 +430,6 @@ __global__ void hybrid_bc_kernel(int64_t nf, pb::DualTopo T, pb::HybridIn H, con
         pb::hybrid_bc_row((int32_t)f, T, H, robin_weight, face_areas, norm, hval, rhs);
 }
 
-template <int ND>
-static void hybrid_launch(int method, int grid, size_t smem, cudaStream_t st, int64_t nc, const pb::DualTopo &T,
-                          const pb::DualGeo &G, const pb::HybridIn &H, int nmax, const double *lam, double *hval,
-                          double *rhs, double *u, double *p, int32_t *bad, int32_t *singular) {
-    if (method == PB_DUAL_MVEM)
-        hybrid_cell_kernel<ND, pb::kDualMvem><<<grid, 32 * kHybridWarps, smem, st>>>(nc, T, G, H, nmax, lam, hval, rhs,
-                                                                                     u, p, bad, singular);
-    else
-        hybrid_cell_kernel<ND, pb::kDualRt0><<<grid, 32 * kHybridWarps, smem, st>>>(nc, T, G, H, nmax, lam, hval, rhs,
-                                                                                    u, p, bad, singular);
-}
-
 // Everything both entry points share: the checks, the geometry (uploaded, or that of the last pb_dual_discretize), the
 // values and codes, and one timed launch of hybrid_cell_kernel.
 struct HybridRun {
@@ -532,12 +489,6 @@ static int hybrid_prepare(pb_dual *d, int mode, const double *const geo[7], cons
     return PB_OK;
 }
 
-static pb::DualTopo dual_topo(pb_dual *d) {
-    return pb::DualTopo{d->cf_ip.as<int32_t>(), d->cf_ix.as<int32_t>(), d->cf_cell.as<int32_t>(),
-                        d->cf_sg.as<int8_t>(), d->fn_ip.as<int32_t>(), d->fn_ix.as<int32_t>(),
-                        d->mass_ip.as<int32_t>(), d->mass_ix.as<int32_t>()};
-}
-
 // One timed launch of hybrid_cell_kernel; then the two flags: MVEM consistency (AssertionError in Python) and a
 // singular local matrix.
 static int hybrid_run(pb_dual *d, HybridRun &R, const double *lam, double *hval, double *rhs, double *u, double *p,
@@ -546,37 +497,26 @@ static int hybrid_run(pb_dual *d, HybridRun &R, const double *lam, double *hval,
     const pb::DualTopo T = dual_topo(d);
     const size_t smem = (size_t)kHybridWarps * pb::hybrid_cell_doubles(R.nmax) * sizeof(double);
     int32_t *flags = R.flags.as<int32_t>();
-    cudaEvent_t e0 = nullptr, e1 = nullptr;
-    struct Guard {
-        cudaEvent_t &a, &b;
-        ~Guard() { if (a) cudaEventDestroy(a); if (b) cudaEventDestroy(b); }
-    } guard{e0, e1};
-    CUDA_TRY(cudaEventCreate(&e0));
-    CUDA_TRY(cudaEventCreate(&e1));
-    const int grid = (int)std::max<int64_t>(1, std::min<int64_t>((d->nc + kHybridWarps - 1) / kHybridWarps,
-                                                                 (int64_t)pb_sm_count() * 32));
-    CUDA_TRY(cudaEventRecord(e0, st));
-    if (d->nd == 1) {
-        CUDA_TRY(cudaFuncSetAttribute(hybrid_cell_kernel<1, pb::kDualMvem>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        CUDA_TRY(cudaFuncSetAttribute(hybrid_cell_kernel<1, pb::kDualRt0>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        hybrid_launch<1>(R.method, grid, smem, st, d->nc, T, R.G, R.H, R.nmax, lam, hval, rhs, u, p, flags, flags + 1);
-    } else if (d->nd == 2) {
-        CUDA_TRY(cudaFuncSetAttribute(hybrid_cell_kernel<2, pb::kDualMvem>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        CUDA_TRY(cudaFuncSetAttribute(hybrid_cell_kernel<2, pb::kDualRt0>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        hybrid_launch<2>(R.method, grid, smem, st, d->nc, T, R.G, R.H, R.nmax, lam, hval, rhs, u, p, flags, flags + 1);
-    } else {
-        CUDA_TRY(cudaFuncSetAttribute(hybrid_cell_kernel<3, pb::kDualMvem>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        CUDA_TRY(cudaFuncSetAttribute(hybrid_cell_kernel<3, pb::kDualRt0>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        hybrid_launch<3>(R.method, grid, smem, st, d->nc, T, R.G, R.H, R.nmax, lam, hval, rhs, u, p, flags, flags + 1);
-    }
+    KernelTimer timer;
+    CUDA_TRY(timer.create());
+    CUDA_TRY(timer.mark(0, st));
+    const int rc = dispatch_nd<1, 2, 3>(d->nd, [&](auto ND) {
+        auto kernel = R.method == PB_DUAL_MVEM ? hybrid_cell_kernel<ND, pb::kDualMvem>
+                                               : hybrid_cell_kernel<ND, pb::kDualRt0>;
+        CUDA_TRY(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        kernel<<<grid_stride_blocks(d->nc, kHybridWarps, 32), 32 * kHybridWarps, smem, st>>>(
+            d->nc, T, R.G, R.H, R.nmax, lam, hval, rhs, u, p, flags, flags + 1);
+        return PB_OK;
+    });
+    if (rc) return rc;
     pb_count_launch_();
     CUDA_TRY(cudaGetLastError());
-    CUDA_TRY(cudaEventRecord(e1, st));
+    CUDA_TRY(timer.mark(1, st));
     int32_t hf[2];
     CUDA_TRY(cudaMemcpyAsync(hf, flags, sizeof(hf), cudaMemcpyDeviceToHost, st));
     CUDA_TRY(cudaStreamSynchronize(st));
     float ms = 0.0f;
-    CUDA_TRY(cudaEventElapsedTime(&ms, e0, e1));
+    CUDA_TRY(timer.ms(&ms));
     if (kernel_ms) *kernel_ms = ms;
     if (hf[1] != 0x7f7f7f7f)
         return pb_fail_(PB_ESINGULAR, "hybridization: the local matrix of cell " + std::to_string(hf[1]) +
@@ -599,38 +539,32 @@ extern "C" int pb_dual_hybrid_system(pb_dual *d, int mode, const double *nodes, 
     if (rc) return rc;
     const int64_t nf = d->nf;
     cudaStream_t st = d->stream;
-    pb_csr *a = nullptr;
-    rc = pb_csr_from_device_pattern_(nf, nf, d->mass_nnz, d->mass_ip.as<int32_t>(), d->mass_ix.as<int32_t>(), &a);
+    CsrPtr a;
+    rc = pb_csr_from_device_pattern_(nf, nf, d->mass_nnz, d->mass_ip.as<int32_t>(), d->mass_ix.as<int32_t>(), a);
     if (rc) return rc;
-    auto fail_cuda = [&](cudaError_t e, const char *what) {
-        pb_csr_destroy(a);
-        return pb_fail_(PB_ECUDA, std::string(what) + ": " + cudaGetErrorString(e));
-    };
-#define HY_TRY(x) do { cudaError_t e_ = (x); if (e_ != cudaSuccess) return fail_cuda(e_, #x); } while (0)
-    double *hval = pb_csr_data_(a);
+    double *hval = pb_csr_view_(a.get()).data;
     DevBuf drhs, drw, darea, dnorm;
-    HY_TRY(drhs.ensure((size_t)nf * sizeof(double)));
-    HY_TRY(drw.upload(robin_weight, (size_t)nf, st));
-    HY_TRY(darea.upload(face_areas, (size_t)nf, st));
-    HY_TRY(dnorm.ensure(sizeof(unsigned long long)));
-    HY_TRY(cudaMemsetAsync(hval, 0, (size_t)d->mass_nnz * sizeof(double), st));
-    HY_TRY(cudaMemsetAsync(drhs.p, 0, (size_t)nf * sizeof(double), st));
-    HY_TRY(cudaMemsetAsync(dnorm.p, 0, sizeof(unsigned long long), st));
+    CUDA_TRY(drhs.ensure((size_t)nf * sizeof(double)));
+    CUDA_TRY(drw.upload(robin_weight, (size_t)nf, st));
+    CUDA_TRY(darea.upload(face_areas, (size_t)nf, st));
+    CUDA_TRY(dnorm.ensure(sizeof(unsigned long long)));
+    CUDA_TRY(cudaMemsetAsync(hval, 0, (size_t)d->mass_nnz * sizeof(double), st));
+    CUDA_TRY(cudaMemsetAsync(drhs.p, 0, (size_t)nf * sizeof(double), st));
+    CUDA_TRY(cudaMemsetAsync(dnorm.p, 0, sizeof(unsigned long long), st));
     rc = hybrid_run(d, R, nullptr, hval, drhs.as<double>(), nullptr, nullptr, bad_cell, kernel_ms);
-    if (rc) { pb_csr_destroy(a); return rc; }
+    if (rc) return rc;
     // |H|_inf before the boundary conditions (hybrid.py), or |mass|_inf of the saddle-point system
-    const int grid = (int)std::max<int64_t>(1, std::min<int64_t>((nf + 255) / 256, (int64_t)pb_sm_count() * 16));
+    const int grid = grid_stride_blocks(nf, 256, 16);
     dual_norm_kernel<<<grid, 256, 0, st>>>(nf, d->mass_ip.as<int32_t>(),
                                            mode == PB_DUAL_HYBRID_VEM ? hval : d->mass_val.as<double>(),
                                            dnorm.as<unsigned long long>());
     hybrid_bc_kernel<<<grid, 256, 0, st>>>(nf, dual_topo(d), R.H, drw.as<double>(), darea.as<double>(),
                                            dnorm.as<unsigned long long>(), hval, drhs.as<double>());
     pb_count_launch_(); pb_count_launch_();
-    HY_TRY(cudaGetLastError());
-    HY_TRY(cudaMemcpyAsync(rhs, drhs.p, (size_t)nf * sizeof(double), cudaMemcpyDeviceToHost, st));
-    HY_TRY(cudaStreamSynchronize(st));
-#undef HY_TRY
-    *out = a;
+    CUDA_TRY(cudaGetLastError());
+    CUDA_TRY(cudaMemcpyAsync(rhs, drhs.p, (size_t)nf * sizeof(double), cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(cudaStreamSynchronize(st));
+    *out = a.release();
     return PB_OK;
 }
 

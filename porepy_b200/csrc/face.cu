@@ -22,7 +22,7 @@ struct TpsaPattern {
 
 struct pb_facegrid {
     int64_t nc = 0, nf = 0;
-    cudaStream_t stream = nullptr;
+    Stream stream;
     DevBuf face_cells, fnorm, fcent, ccent, farea, tmp;   // farea: set by pb_facegrid_set_face_areas
     DevBuf cf_ip, cf_ix;                                  // cell -> face lists (cell_faces, CSC)
     std::vector<uint8_t> face_ncell;                      // host: cells per face
@@ -38,6 +38,8 @@ struct pb_facegrid {
     double ctc_ct = 0.0;
     std::vector<int32_t> ctc_face_h, ctc_cell_h;
     DevBuf ctc_fm, ctc_face, ctc_cell, ctc_pair, ctc_w, ctc_frame;
+    // the stream's copies and kernels may still use the buffers, which go back to the pool right after
+    ~pb_facegrid() { if (stream) cudaStreamSynchronize(stream); }
 };
 
 // one thread per cell: claim the first free slot of each of its faces
@@ -65,57 +67,44 @@ extern "C" int pb_facegrid_create(int64_t nc, int64_t nf, const int32_t *cf_indp
     if (!out || !cf_indptr || !cf_indices || !cf_data || !face_normals || !face_centers || !cell_centers)
         return pb_fail_(PB_EINVAL, "null pointer");
     if (nc <= 0 || nf <= 0) return pb_fail_(PB_EINVAL, "empty grid");
-    int ndev = 0;
-    if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev < 1)
-        return pb_fail_(PB_ECUDA, "no CUDA device: libporeb200 has no CPU path");
+    if (int rc = pb_require_device()) return rc;
     std::vector<uint8_t> ncell((size_t)nf, 0);
     for (int64_t q = 0; q < cf_indptr[nc]; ++q) {
         if (cf_indices[q] < 0 || cf_indices[q] >= nf) return pb_fail_(PB_EINVAL, "cell_faces index out of range");
         if (ncell[cf_indices[q]] < 255) ++ncell[cf_indices[q]];
     }
-    pb_facegrid *g = new pb_facegrid;
+    std::unique_ptr<pb_facegrid> g(new pb_facegrid);
     g->nc = nc; g->nf = nf;
     g->face_ncell.swap(ncell);
-    auto bail = [&](int rc) { pb_facegrid_destroy(g); return rc; };
-#define FG_TRY(x) do { cudaError_t e_ = (x); if (e_ != cudaSuccess) return bail(pb_fail_(PB_ECUDA, std::string(#x) + ": " + cudaGetErrorString(e_))); } while (0)
-    FG_TRY(cudaStreamCreateWithFlags(&g->stream, cudaStreamNonBlocking));
+    CUDA_TRY(g->stream.create());
     cudaStream_t st = g->stream;
     DevBuf &ip = g->cf_ip, &ix = g->cf_ix, da, bad;
-    FG_TRY(ip.upload(cf_indptr, (size_t)nc + 1, st));
-    FG_TRY(ix.upload(cf_indices, (size_t)cf_indptr[nc], st));
-    FG_TRY(da.upload(cf_data, (size_t)cf_indptr[nc], st));
-    FG_TRY(bad.ensure(sizeof(int)));
-    FG_TRY(cudaMemsetAsync(bad.p, 0, sizeof(int), st));
-    FG_TRY(g->face_cells.ensure((size_t)2 * nf * sizeof(int32_t)));
-    FG_TRY(cudaMemsetAsync(g->face_cells.p, 0xFF, (size_t)2 * nf * sizeof(int32_t), st));
-    const int block = 256;
-    int grid = (int)std::max<int64_t>(1, std::min<int64_t>((nc + block - 1) / block, (int64_t)pb_sm_count() * 16));
-    face_cells_kernel<<<grid, block, 0, st>>>(nc, ip.as<int32_t>(), ix.as<int32_t>(), da.as<int8_t>(),
-                                              g->face_cells.as<int32_t>(), bad.as<int>());
-    grid = (int)std::max<int64_t>(1, std::min<int64_t>((nf + block - 1) / block, (int64_t)pb_sm_count() * 16));
-    face_cells_order_kernel<<<grid, block, 0, st>>>(nf, g->face_cells.as<int32_t>());
+    CUDA_TRY(ip.upload(cf_indptr, (size_t)nc + 1, st));
+    CUDA_TRY(ix.upload(cf_indices, (size_t)cf_indptr[nc], st));
+    CUDA_TRY(da.upload(cf_data, (size_t)cf_indptr[nc], st));
+    CUDA_TRY(bad.ensure(sizeof(int)));
+    CUDA_TRY(cudaMemsetAsync(bad.p, 0, sizeof(int), st));
+    CUDA_TRY(g->face_cells.ensure((size_t)2 * nf * sizeof(int32_t)));
+    CUDA_TRY(cudaMemsetAsync(g->face_cells.p, 0xFF, (size_t)2 * nf * sizeof(int32_t), st));
+    face_cells_kernel<<<grid_stride_blocks(nc, 256, 16), 256, 0, st>>>(
+        nc, ip.as<int32_t>(), ix.as<int32_t>(), da.as<int8_t>(), g->face_cells.as<int32_t>(), bad.as<int>());
+    face_cells_order_kernel<<<grid_stride_blocks(nf, 256, 16), 256, 0, st>>>(nf, g->face_cells.as<int32_t>());
     pb_count_launch_(); pb_count_launch_();
-    FG_TRY(cudaGetLastError());
-    int rc;
-    if ((rc = pb_upload_repacked_(st, g->tmp, g->fnorm, face_normals, 3, nf))) return bail(rc);
-    if ((rc = pb_upload_repacked_(st, g->tmp, g->fcent, face_centers, 3, nf))) return bail(rc);
-    if ((rc = pb_upload_repacked_(st, g->tmp, g->ccent, cell_centers, 3, nc))) return bail(rc);
+    CUDA_TRY(cudaGetLastError());
+    if (int rc = pb_upload_repacked_(st, g->tmp, g->fnorm, face_normals, 3, nf)) return rc;
+    if (int rc = pb_upload_repacked_(st, g->tmp, g->fcent, face_centers, 3, nf)) return rc;
+    if (int rc = pb_upload_repacked_(st, g->tmp, g->ccent, cell_centers, 3, nc)) return rc;
     int hbad = 0;
-    FG_TRY(cudaMemcpyAsync(&hbad, bad.p, sizeof(int), cudaMemcpyDeviceToHost, st));
-    FG_TRY(cudaStreamSynchronize(st));
-#undef FG_TRY
-    if (hbad) return bail(pb_fail_(PB_EINVAL, "face with more than two neighbouring cells"));
+    CUDA_TRY(cudaMemcpyAsync(&hbad, bad.p, sizeof(int), cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(cudaStreamSynchronize(st));
+    if (hbad) return pb_fail_(PB_EINVAL, "face with more than two neighbouring cells");
     g->geo = GeoView{nullptr, g->fnorm.as<double>(), g->fcent.as<double>(), nullptr, g->ccent.as<double>(), nullptr,
                      1, 3, 1, 3, 1, 3};
-    *out = g;
+    *out = g.release();
     return PB_OK;
 }
 
-extern "C" void pb_facegrid_destroy(pb_facegrid *g) {
-    if (!g) return;
-    if (g->stream) { cudaStreamSynchronize(g->stream); cudaStreamDestroy(g->stream); }
-    delete g;
-}
+extern "C" void pb_facegrid_destroy(pb_facegrid *g) { delete g; }
 
 __global__ void tpfa_kernel(int64_t nf, GeoView G, const double *__restrict__ perm, int64_t perm_cs,
                             int64_t perm_es, const uint8_t *__restrict__ bc,
@@ -161,10 +150,8 @@ extern "C" int pb_tpfa(pb_facegrid *g, const double *permeability, const uint8_t
     CUDA_TRY(o_bpf.ensure((size_t)nf * sizeof(double)));
     TpfaOut o{o_flux.as<double>(), o_bpc.as<double>(), o_vs.as<double>(), o_bpvs.as<double>(),
               o_bf.as<double>(), o_bpf.as<double>()};
-    const int block = 256;
-    const int grid = (int)std::max<int64_t>(1, std::min<int64_t>((nf + block - 1) / block, (int64_t)pb_sm_count() * 16));
-    tpfa_kernel<<<grid, block, 0, st>>>(nf, g->geo, perm.as<double>(), 1, 9, bc.as<uint8_t>(),
-                                        g->face_cells.as<int32_t>(), ip.as<int32_t>(), vdim, o);
+    tpfa_kernel<<<grid_stride_blocks(nf, 256, 16), 256, 0, st>>>(
+        nf, g->geo, perm.as<double>(), 1, 9, bc.as<uint8_t>(), g->face_cells.as<int32_t>(), ip.as<int32_t>(), vdim, o);
     pb_count_launch_();
     CUDA_TRY(cudaGetLastError());
     auto down = [&](double *h, DevBuf &d, size_t n) -> cudaError_t {
@@ -201,10 +188,9 @@ extern "C" int pb_tpfa_diff(pb_facegrid *g, const double *k, const int32_t *fc_i
     CUDA_TRY(o_t.ensure(nhf * sizeof(double)));
     CUDA_TRY(o_T.ensure((size_t)nf * sizeof(double)));
     CUDA_TRY(o_d.ensure(nhf * 9 * sizeof(double)));
-    const int block = 256;
-    const int grid = (int)std::max<int64_t>(1, std::min<int64_t>((nf + block - 1) / block, (int64_t)pb_sm_count() * 16));
-    tpfa_diff_kernel<<<grid, block, 0, st>>>(nf, g->geo, dk.as<double>(), g->face_cells.as<int32_t>(), ip.as<int32_t>(),
-                                             o_t.as<double>(), o_T.as<double>(), o_d.as<double>());
+    tpfa_diff_kernel<<<grid_stride_blocks(nf, 256, 16), 256, 0, st>>>(
+        nf, g->geo, dk.as<double>(), g->face_cells.as<int32_t>(), ip.as<int32_t>(), o_t.as<double>(), o_T.as<double>(),
+        o_d.as<double>());
     pb_count_launch_();
     CUDA_TRY(cudaGetLastError());
     CUDA_TRY(cudaMemcpyAsync(t_hf, o_t.p, nhf * sizeof(double), cudaMemcpyDeviceToHost, st));
@@ -226,10 +212,9 @@ extern "C" int pb_upwind(pb_facegrid *g, const double *darcy_flux, const uint8_t
     CUDA_TRY(up.ensure((size_t)nf * sizeof(int32_t)));
     CUDA_TRY(neu.ensure((size_t)nf * sizeof(double)));
     CUDA_TRY(dir.ensure((size_t)nf * sizeof(double)));
-    const int block = 256;
-    const int grid = (int)std::max<int64_t>(1, std::min<int64_t>((nf + block - 1) / block, (int64_t)pb_sm_count() * 16));
-    upwind_kernel<<<grid, block, 0, st>>>(nf, q.as<double>(), bc.as<uint8_t>(), g->face_cells.as<int32_t>(),
-                                          up.as<int32_t>(), neu.as<double>(), dir.as<double>());
+    upwind_kernel<<<grid_stride_blocks(nf, 256, 16), 256, 0, st>>>(nf, q.as<double>(), bc.as<uint8_t>(),
+                                                                   g->face_cells.as<int32_t>(), up.as<int32_t>(),
+                                                                   neu.as<double>(), dir.as<double>());
     pb_count_launch_();
     CUDA_TRY(cudaGetLastError());
     CUDA_TRY(cudaMemcpyAsync(upstream_cell, up.p, (size_t)nf * sizeof(int32_t), cudaMemcpyDeviceToHost, st));
@@ -257,15 +242,12 @@ extern "C" int pb_upwind_coupling(int64_t n, const double *interface_flux, doubl
     if (n < 0 || (n > 0 && (!interface_flux || !sign || !from_primary || !from_secondary)))
         return pb_fail_(PB_EINVAL, "bad arguments");
     if (n == 0) return PB_OK;
-    int ndev = 0;
-    if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev < 1)
-        return pb_fail_(PB_ECUDA, "no CUDA device: libporeb200 has no CPU path");
+    if (int rc = pb_require_device()) return rc;
     DevBuf in, o0, o1, o2;
     CUDA_TRY(in.upload(interface_flux, (size_t)n, 0));
     CUDA_TRY(o0.ensure((size_t)n * 8)); CUDA_TRY(o1.ensure((size_t)n * 8)); CUDA_TRY(o2.ensure((size_t)n * 8));
-    const int block = 256;
-    const int grid = (int)std::max<int64_t>(1, std::min<int64_t>((n + block - 1) / block, (int64_t)pb_sm_count() * 16));
-    upwind_coupling_kernel<<<grid, block>>>(n, in.as<double>(), o0.as<double>(), o1.as<double>(), o2.as<double>());
+    upwind_coupling_kernel<<<grid_stride_blocks(n, 256, 16), 256>>>(n, in.as<double>(), o0.as<double>(),
+                                                                    o1.as<double>(), o2.as<double>());
     pb_count_launch_();
     CUDA_TRY(cudaGetLastError());
     CUDA_TRY(cudaMemcpy(sign, o0.p, (size_t)n * 8, cudaMemcpyDeviceToHost));
@@ -283,29 +265,6 @@ extern "C" int pb_facegrid_set_face_areas(pb_facegrid *g, const double *face_are
 }
 
 // ---- TPSA: the per-face terms (tpsa_face.cuh) and the assembled systems (tpsa_system.cuh) -------------------------
-struct pb_csr;
-int pb_csr_from_device_pattern_(int64_t nrows, int64_t ncols, int64_t nnz, const int32_t *indptr_dev,
-                                const int32_t *indices_dev, pb_csr **out);   // spmv.cu
-double *pb_csr_data_(pb_csr *a);                                              // spmv.cu
-struct CsrView { int64_t nrows, ncols, nnz; int32_t *indptr, *indices; double *data; };
-CsrView pb_csr_view_(const pb_csr *a);                                        // spmv.cu
-
-static int fg_grid(int64_t n) {
-    return (int)std::max<int64_t>(1, std::min<int64_t>((n + 255) / 256, (int64_t)pb_sm_count() * 16));
-}
-
-// Calls f with std::integral_constant<int, nd> (nd = 2 or 3): a launch site names its kernel<ND> once.
-template <class F>
-static void tpsa_nd(int nd, F &&f) {
-    if (nd == 3) f(std::integral_constant<int, 3>{});
-    else f(std::integral_constant<int, 2>{});
-}
-
-struct FgEvents {
-    cudaEvent_t e[3] = {nullptr, nullptr, nullptr};
-    ~FgEvents() { for (auto x : e) if (x) cudaEventDestroy(x); }
-};
-
 // Inputs of the TPSA calls on the device.
 struct TpsaInputs {
     DevBuf mu, lam, vol, codes, rob, flags;
@@ -355,10 +314,10 @@ static int tpsa_prepare(pb_facegrid *g, int nd, const double *mu, const double *
 static int tpsa_face_launch(pb_facegrid *g, int nd, const TpsaInputs &in, const int32_t *fc_ptr, const TpsaOut &o) {
     const int64_t nf = g->nf;
     const double *rw = in.any_rob ? in.rob.as<double>() : nullptr;
-    tpsa_nd(nd, [&](auto ND) {
-        tpsa_kernel<ND><<<fg_grid(nf), 256, 0, g->stream>>>(nf, g->geo, in.mu.as<double>(), in.codes.as<uint8_t>(), rw,
-                                                             in.flags.as<uint8_t>(), g->face_cells.as<int32_t>(), fc_ptr,
-                                                             o);
+    dispatch_nd<2, 3>(nd, [&](auto ND) {
+        tpsa_kernel<ND><<<grid_stride_blocks(nf, 256, 16), 256, 0, g->stream>>>(
+            nf, g->geo, in.mu.as<double>(), in.codes.as<uint8_t>(), rw, in.flags.as<uint8_t>(),
+            g->face_cells.as<int32_t>(), fc_ptr, o);
     });
     pb_count_launch_();
     CUDA_TRY(cudaGetLastError());
@@ -384,18 +343,17 @@ extern "C" int pb_tpsa(pb_facegrid *g, int nd, const double *mu, const uint8_t *
         CUDA_TRY(o_buf[k].ensure(count[k] * sizeof(double)));
         o.t[k] = o_buf[k].as<double>();
     }
-    FgEvents ev;
+    KernelTimer timer;
     if (kernel_ms) {
-        CUDA_TRY(cudaEventCreate(&ev.e[0]));
-        CUDA_TRY(cudaEventCreate(&ev.e[1]));
-        CUDA_TRY(cudaEventRecord(ev.e[0], st));
+        CUDA_TRY(timer.create());
+        CUDA_TRY(timer.mark(0, st));
     }
     if ((rc = tpsa_face_launch(g, nd, in, dip.as<int32_t>(), o))) return rc;
-    if (kernel_ms) CUDA_TRY(cudaEventRecord(ev.e[1], st));
+    if (kernel_ms) CUDA_TRY(timer.mark(1, st));
     for (int k = 0; k < PB_TPSA_NTERMS; ++k)
         if (out[k]) CUDA_TRY(cudaMemcpyAsync(out[k], o_buf[k].p, count[k] * sizeof(double), cudaMemcpyDeviceToHost, st));
     CUDA_TRY(cudaStreamSynchronize(st));
-    if (kernel_ms) CUDA_TRY(cudaEventElapsedTime(kernel_ms, ev.e[0], ev.e[1]));
+    if (kernel_ms) CUDA_TRY(timer.ms(kernel_ms));
     return PB_OK;
 }
 
@@ -459,7 +417,7 @@ static int tpsa_neighbours(pb_facegrid *g) {
     CUDA_TRY(count.ensure((size_t)nc * sizeof(int32_t)));
     CUDA_TRY(bad.ensure(sizeof(int)));
     CUDA_TRY(cudaMemsetAsync(bad.p, 0, sizeof(int), st));
-    tpsa_nb_count_kernel<<<fg_grid(nc), 256, 0, st>>>(t, count.as<int32_t>(), bad.as<int>());
+    tpsa_nb_count_kernel<<<grid_stride_blocks(nc, 256, 16), 256, 0, st>>>(t, count.as<int32_t>(), bad.as<int>());
     pb_count_launch_();
     CUDA_TRY(cudaGetLastError());
     CUDA_TRY(g->cc_ptr.ensure((size_t)(nc + 1) * sizeof(int32_t)));
@@ -471,8 +429,8 @@ static int tpsa_neighbours(pb_facegrid *g) {
     if (hbad) return pb_fail_(PB_ENOTIMPL, "Tpsa system: a cell has more than 31 face neighbours");
     CUDA_TRY(g->cc_ix.ensure((size_t)std::max<int64_t>(1, total) * sizeof(int32_t)));
     CUDA_TRY(g->cc_cell.ensure((size_t)std::max<int64_t>(1, total) * sizeof(int32_t)));
-    tpsa_nb_list_kernel<<<fg_grid(nc), 256, 0, st>>>(t, g->cc_ptr.as<int32_t>(), g->cc_ix.as<int32_t>(),
-                                                      g->cc_cell.as<int32_t>());
+    tpsa_nb_list_kernel<<<grid_stride_blocks(nc, 256, 16), 256, 0, st>>>(
+        t, g->cc_ptr.as<int32_t>(), g->cc_ix.as<int32_t>(), g->cc_cell.as<int32_t>());
     pb_count_launch_();
     CUDA_TRY(cudaGetLastError());
     g->npairs = total;
@@ -510,7 +468,7 @@ static int tpsa_pattern(pb_facegrid *g, TpsaPattern &P, const TpsaKey &key, Buil
     if (P.key == key) return PB_OK;
     P.key = {};
     int rc = tpsa_neighbours(g);
-    if (!rc) tpsa_nd((int)key[0], [&](auto ND) { rc = build(ND); });
+    if (!rc) dispatch_nd<2, 3>((int)key[0], [&](auto ND) { rc = build(ND); });
     if (rc) return rc;
     pb_count_launch_();
     CUDA_TRY(cudaGetLastError());
@@ -533,8 +491,8 @@ static int tpsa_sys_pattern(pb_facegrid *g) {
     TpsaPattern &P = g->sys;
     const int rc = tpsa_pattern_alloc(g, P, nc * TpsaDims<ND>::B, (int64_t)TpsaDims<ND>::NZ * g->npairs);
     if (rc) return rc;
-    tpsa_pattern_kernel<ND><<<fg_grid(nc), 256, 0, g->stream>>>(nc, g->cc_ptr.as<int32_t>(), g->cc_ix.as<int32_t>(),
-                                                                 P.ip.as<int32_t>(), P.ix.as<int32_t>());
+    tpsa_pattern_kernel<ND><<<grid_stride_blocks(nc, 256, 16), 256, 0, g->stream>>>(
+        nc, g->cc_ptr.as<int32_t>(), g->cc_ix.as<int32_t>(), P.ip.as<int32_t>(), P.ix.as<int32_t>());
     return PB_OK;
 }
 
@@ -563,12 +521,13 @@ static int tpsa_poro_pattern(pb_facegrid *g, const CsrView &fp) {
     TpsaPattern &P = g->poro;
     int64_t nnz = 0;
     int rc = tpsa_block_offsets(g, P, &nnz, [&](int32_t *count) {
-        tpsa_poro_count_kernel<ND, NS><<<fg_grid(nc), 256, 0, g->stream>>>(nc, cc_ptr, fp.indptr, fp.indices, count);
+        tpsa_poro_count_kernel<ND, NS><<<grid_stride_blocks(nc, 256, 16), 256, 0, g->stream>>>(nc, cc_ptr, fp.indptr,
+                                                                                               fp.indices, count);
     });
     if (rc || (rc = tpsa_pattern_alloc(g, P, nc * TpsaPoroDims<ND, NS>::B, nnz))) return rc;
-    tpsa_poro_pattern_kernel<ND, NS><<<fg_grid(nc), 256, 0, g->stream>>>(nc, cc_ptr, g->cc_ix.as<int32_t>(),
-                                                                          P.blk.as<int64_t>(), fp.indptr, fp.indices,
-                                                                          P.ip.as<int32_t>(), P.ix.as<int32_t>());
+    tpsa_poro_pattern_kernel<ND, NS><<<grid_stride_blocks(nc, 256, 16), 256, 0, g->stream>>>(
+        nc, cc_ptr, g->cc_ix.as<int32_t>(), P.blk.as<int64_t>(), fp.indptr, fp.indices, P.ip.as<int32_t>(),
+        P.ix.as<int32_t>());
     return PB_OK;
 }
 
@@ -609,56 +568,47 @@ static int tpsa_contact_pattern(pb_facegrid *g) {
     TpsaPattern &P = g->ctc;
     int64_t ncell = 0;
     int rc = tpsa_block_offsets(g, P, &ncell, [&](int32_t *count) {
-        tpsa_contact_count_kernel<ND><<<fg_grid(nc), 256, 0, g->stream>>>(t, cc_ptr, I.face_mortar, count);
+        tpsa_contact_count_kernel<ND><<<grid_stride_blocks(nc, 256, 16), 256, 0, g->stream>>>(t, cc_ptr, I.face_mortar,
+                                                                                              count);
     });
     const int64_t nnz = ncell + (int64_t)ND * I.nm * D::LF + (int64_t)ND * I.nk * D::LC;
     if (rc || (rc = tpsa_pattern_alloc(g, P, nc * D::B + ni, nnz))) return rc;
-    tpsa_contact_pattern_kernel<ND><<<fg_grid(nc), 256, 0, g->stream>>>(t, cc_ptr, g->cc_ix.as<int32_t>(),
-                                                                         P.blk.as<int64_t>(), I, P.ip.as<int32_t>(),
-                                                                         P.ix.as<int32_t>());
-    if (ni) tpsa_contact_iface_pattern_kernel<ND><<<fg_grid(ni), 256, 0, g->stream>>>(t, P.blk.as<int64_t>(), I,
-                                                                                      P.ip.as<int32_t>(), P.ix.as<int32_t>());
+    tpsa_contact_pattern_kernel<ND><<<grid_stride_blocks(nc, 256, 16), 256, 0, g->stream>>>(
+        t, cc_ptr, g->cc_ix.as<int32_t>(), P.blk.as<int64_t>(), I, P.ip.as<int32_t>(), P.ix.as<int32_t>());
+    if (ni) tpsa_contact_iface_pattern_kernel<ND><<<grid_stride_blocks(ni, 256, 16), 256, 0, g->stream>>>(
+        t, P.blk.as<int64_t>(), I, P.ip.as<int32_t>(), P.ix.as<int32_t>());
     return PB_OK;
 }
 
 // ---- assembly ------------------------------------------------------------------------------------------------------
 // A TPSA system on the pattern P (nrows x nrows), in two stages: the face terms (tpsa_face_terms), then
 // launch(ND, T, values of A), which gathers the blocks of A from them.  stage_ms (optional): the two stage times in ms.
-// A is destroyed on every error.
 template <class Launch>
 static int tpsa_assemble(pb_facegrid *g, int nd, const TpsaInputs &in, const TpsaPattern &P, int64_t nrows,
                          pb_csr **out, float *stage_ms, Launch &&launch) {
-    pb_csr *a = nullptr;
-    int rc = pb_csr_from_device_pattern_(nrows, nrows, P.nnz, P.ip.as<int32_t>(), P.ix.as<int32_t>(), &a);
+    CsrPtr a;
+    int rc = pb_csr_from_device_pattern_(nrows, nrows, P.nnz, P.ip.as<int32_t>(), P.ix.as<int32_t>(), a);
     if (rc) return rc;
     cudaStream_t st = g->stream;
-    FgEvents ev;
-    auto stages = [&]() -> int {
-        if (stage_ms) {
-            for (auto &x : ev.e) CUDA_TRY(cudaEventCreate(&x));
-            CUDA_TRY(cudaEventRecord(ev.e[0], st));
-        }
-        TpsaTerms T{};
-        const int rt = tpsa_face_terms(g, nd, in, T);
-        if (rt) return rt;
-        if (stage_ms) CUDA_TRY(cudaEventRecord(ev.e[1], st));
-        tpsa_nd(nd, [&](auto ND) { launch(ND, T, pb_csr_data_(a)); });
-        pb_count_launch_();
-        CUDA_TRY(cudaGetLastError());
-        if (stage_ms) CUDA_TRY(cudaEventRecord(ev.e[2], st));
-        CUDA_TRY(cudaStreamSynchronize(st));
-        if (stage_ms) {
-            CUDA_TRY(cudaEventElapsedTime(stage_ms, ev.e[0], ev.e[1]));
-            CUDA_TRY(cudaEventElapsedTime(stage_ms + 1, ev.e[1], ev.e[2]));
-        }
-        return PB_OK;
-    };
-    if ((rc = stages())) {
-        pb_csr_destroy(a);
-        return rc;
+    KernelTimer timer;
+    if (stage_ms) {
+        CUDA_TRY(timer.create(3));
+        CUDA_TRY(timer.mark(0, st));
+    }
+    TpsaTerms T{};
+    if ((rc = tpsa_face_terms(g, nd, in, T))) return rc;
+    if (stage_ms) CUDA_TRY(timer.mark(1, st));
+    dispatch_nd<2, 3>(nd, [&](auto ND) { launch(ND, T, pb_csr_view_(a.get()).data); });
+    pb_count_launch_();
+    CUDA_TRY(cudaGetLastError());
+    if (stage_ms) CUDA_TRY(timer.mark(2, st));
+    CUDA_TRY(cudaStreamSynchronize(st));
+    if (stage_ms) {
+        CUDA_TRY(timer.ms(stage_ms, 0));
+        CUDA_TRY(timer.ms(stage_ms + 1, 1));
     }
     g->terms_nd = nd;
-    *out = a;
+    *out = a.release();
     return PB_OK;
 }
 
@@ -701,8 +651,9 @@ static int tpsa_rhs(pb_facegrid *g, int nd, bool contact, const double *bc_value
     const int64_t rows = nc * (nd + nr + 1 + NS) + (int64_t)nd * (I.nm + I.nk);
     const double *pf = body_force ? df.as<double>() : nullptr, *psr = angular_source ? dsr.as<double>() : nullptr,
                  *psp = mass_source ? dsp.as<double>() : nullptr;
-    tpsa_nd(nd, [&](auto ND) {
-        tpsa_rhs_kernel<ND, NS><<<fg_grid(rows), 256, 0, st>>>(t, I, T, dg.as<double>(), pf, psr, psp, rhs_dev);
+    dispatch_nd<2, 3>(nd, [&](auto ND) {
+        tpsa_rhs_kernel<ND, NS><<<grid_stride_blocks(rows, 256, 16), 256, 0, st>>>(t, I, T, dg.as<double>(), pf, psr,
+                                                                                   psp, rhs_dev);
     });
     pb_count_launch_();
     CUDA_TRY(cudaGetLastError());
@@ -738,9 +689,9 @@ extern "C" int pb_tpsa_system(pb_facegrid *g, int nd, const double *mu, const do
     const int64_t np = g->npairs;
     return tpsa_assemble(g, nd, in, g->sys, g->nc * (nd == 3 ? 7 : 4), out, stage_ms,
                          [&](auto ND, const TpsaTerms &T, double *a) {
-        tpsa_system_kernel<ND><<<fg_grid(np), 256, 0, g->stream>>>(np, t, g->cc_ptr.as<int32_t>(), g->cc_ix.as<int32_t>(),
-                                                                    g->cc_cell.as<int32_t>(), T, in.mu.as<double>(),
-                                                                    in.lam.as<double>(), in.vol.as<double>(), a);
+        tpsa_system_kernel<ND><<<grid_stride_blocks(np, 256, 16), 256, 0, g->stream>>>(
+            np, t, g->cc_ptr.as<int32_t>(), g->cc_ix.as<int32_t>(), g->cc_cell.as<int32_t>(), T, in.mu.as<double>(),
+            in.lam.as<double>(), in.vol.as<double>(), a);
     });
 }
 
@@ -816,9 +767,9 @@ static int tpsa_poro_system(pb_facegrid *g, int nd, const double *mu, const doub
     const int64_t np = g->npairs;
     return tpsa_assemble(g, nd, in, g->poro, nc * ((nd == 3 ? 7 : 4) + NS), out, stage_ms,
                          [&](auto ND, const TpsaTerms &T, double *a) {
-        tpsa_poro_system_kernel<ND, NS><<<fg_grid(np), 256, 0, g->stream>>>(
-            np, t, g->cc_ptr.as<int32_t>(), g->cc_ix.as<int32_t>(), g->cc_cell.as<int32_t>(), g->poro.blk.as<int64_t>(), T,
-            in.mu.as<double>(), in.lam.as<double>(), dal.as<double>(), in.vol.as<double>(), a);
+        tpsa_poro_system_kernel<ND, NS><<<grid_stride_blocks(np, 256, 16), 256, 0, g->stream>>>(
+            np, t, g->cc_ptr.as<int32_t>(), g->cc_ix.as<int32_t>(), g->cc_cell.as<int32_t>(), g->poro.blk.as<int64_t>(),
+            T, in.mu.as<double>(), in.lam.as<double>(), dal.as<double>(), in.vol.as<double>(), a);
     });
 }
 
@@ -846,8 +797,8 @@ static int tpsa_poro_fluid_rows(pb_facegrid *g, pb_csr *a, const pb_csr *jf, con
         return pb_fail_(PB_EINVAL, std::string("the matrix is not the ") + TpsaPoroNames<NS>::model +
                                        " system of this grid");
     if (vj.nrows != NS * nc || vj.ncols != (1 + NS) * nc) return pb_fail_(PB_EINVAL, TpsaPoroNames<NS>::jac);
-    tpsa_nd(nd, [&](auto ND) {
-        tpsa_poro_fluid_kernel<ND, NS><<<fg_grid(nc), 256, 0, (cudaStream_t)stream>>>(
+    dispatch_nd<2, 3>(nd, [&](auto ND) {
+        tpsa_poro_fluid_kernel<ND, NS><<<grid_stride_blocks(nc, 256, 16), 256, 0, (cudaStream_t)stream>>>(
             nc, g->cc_ptr.as<int32_t>(), g->poro.blk.as<int64_t>(), va.indices, vj.indptr, vj.indices, vj.data,
             neg_res_dev, va.data, rhs_dev, missing_dev);
     });
@@ -1003,10 +954,11 @@ extern "C" int pb_tpsa_contact_system(pb_facegrid *g, int nd, const double *mu, 
     const int64_t np = g->npairs, ni = (int64_t)nd * (g->ctc_nm + g->ctc_nk);
     return tpsa_assemble(g, nd, in, g->ctc, g->nc * (nd == 3 ? 7 : 4) + ni, out, stage_ms,
                          [&](auto ND, const TpsaTerms &T, double *a) {
-        tpsa_contact_block_kernel<ND><<<fg_grid(np), 256, 0, g->stream>>>(
-            np, t, g->cc_ptr.as<int32_t>(), g->cc_ix.as<int32_t>(), g->cc_cell.as<int32_t>(), g->ctc.blk.as<int64_t>(), I,
-            T, in.mu.as<double>(), in.lam.as<double>(), in.vol.as<double>(), a);
-        if (ni) tpsa_contact_iface_kernel<ND><<<fg_grid(ni), 256, 0, g->stream>>>(t, g->ctc.blk.as<int64_t>(), I, T, a);
+        tpsa_contact_block_kernel<ND><<<grid_stride_blocks(np, 256, 16), 256, 0, g->stream>>>(
+            np, t, g->cc_ptr.as<int32_t>(), g->cc_ix.as<int32_t>(), g->cc_cell.as<int32_t>(), g->ctc.blk.as<int64_t>(),
+            I, T, in.mu.as<double>(), in.lam.as<double>(), in.vol.as<double>(), a);
+        if (ni) tpsa_contact_iface_kernel<ND><<<grid_stride_blocks(ni, 256, 16), 256, 0, g->stream>>>(
+            t, g->ctc.blk.as<int64_t>(), I, T, a);
     });
 }
 
@@ -1034,8 +986,8 @@ extern "C" int pb_tpsa_contact_rows(pb_facegrid *g, pb_csr *a, const pb_csr *jc,
     if (!nk) return PB_OK;
     // the contact rows are the last nd nk rows, of 3 nd entries each
     const int64_t n = (int64_t)nd * nk, e0 = g->ctc.nnz - n * 3 * nd;
-    tpsa_nd(nd, [&](auto ND) {
-        tpsa_contact_law_kernel<ND><<<fg_grid(n), 256, 0, (cudaStream_t)stream>>>(
+    dispatch_nd<2, 3>(nd, [&](auto ND) {
+        tpsa_contact_law_kernel<ND><<<grid_stride_blocks(n, 256, 16), 256, 0, (cudaStream_t)stream>>>(
             n, c0, c0 + (int64_t)nd * nm, e0, va.indices, vj.indptr, vj.indices, vj.data, neg_res_dev, va.data, rhs_dev,
             missing_dev);
     });

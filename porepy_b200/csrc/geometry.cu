@@ -35,66 +35,50 @@ extern "C" int pb_compute_geometry_3d(int64_t nc, int64_t nf, int64_t nn, const 
     if (!cf_indptr || !cf_indices || !cf_data || !fn_indptr || !fn_indices || !nodes || !face_normals || !face_centers ||
         !face_areas || !cell_centers || !cell_volumes || nc < 0 || nf < 0 || nn < 0)
         return pb_fail_(PB_EINVAL, "pb_compute_geometry_3d: null pointer or negative size");
-    int ndev = 0;
-    if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev < 1)
-        return pb_fail_(PB_ECUDA, "no CUDA device: libporeb200 has no CPU path");
-    cudaStream_t st = nullptr;
-    CUDA_TRY(cudaStreamCreateWithFlags(&st, cudaStreamNonBlocking));
-    cudaEvent_t e0 = nullptr, e1 = nullptr;
+    if (int rc = pb_require_device()) return rc;
+    Stream st;
+    KernelTimer timer;
+    CUDA_TRY(st.create());
+    CUDA_TRY(timer.create());
     DevBuf d_cf_ip, d_cf_ix, d_cf_sg, d_fn_ip, d_fn_ix, d_nodes, tmp, d_fn, d_fc, d_fa, d_cc, d_cv, d_bad;
-    int rc = PB_OK;
-    auto done = [&](int code) {
-        if (e0) cudaEventDestroy(e0);
-        if (e1) cudaEventDestroy(e1);
-        cudaStreamDestroy(st);
-        return code;
-    };
-#define G_TRY(x)                                                                                     \
-    do {                                                                                             \
-        cudaError_t e_ = (x);                                                                        \
-        if (e_ != cudaSuccess) return done(pb_fail_(PB_ECUDA, std::string(#x) + ": " + cudaGetErrorString(e_))); \
-    } while (0)
-    G_TRY(cudaEventCreate(&e0));
-    G_TRY(cudaEventCreate(&e1));
-    G_TRY(d_cf_ip.upload(cf_indptr, (size_t)nc + 1, st));
-    G_TRY(d_cf_ix.upload(cf_indices, (size_t)cf_indptr[nc], st));
-    G_TRY(d_cf_sg.upload(cf_data, (size_t)cf_indptr[nc], st));
-    G_TRY(d_fn_ip.upload(fn_indptr, (size_t)nf + 1, st));
-    G_TRY(d_fn_ix.upload(fn_indices, (size_t)fn_indptr[nf], st));
-    if ((rc = pb_upload_repacked_(st, tmp, d_nodes, nodes, 3, nn))) return done(rc);
-    G_TRY(d_fn.ensure((size_t)3 * nf * sizeof(double)));
-    G_TRY(d_fc.ensure((size_t)3 * nf * sizeof(double)));
-    G_TRY(d_fa.ensure((size_t)nf * sizeof(double)));
-    G_TRY(d_cc.ensure((size_t)3 * nc * sizeof(double)));
-    G_TRY(d_cv.ensure((size_t)nc * sizeof(double)));
-    G_TRY(d_bad.ensure(sizeof(int)));
+    CUDA_TRY(d_cf_ip.upload(cf_indptr, (size_t)nc + 1, st));
+    CUDA_TRY(d_cf_ix.upload(cf_indices, (size_t)cf_indptr[nc], st));
+    CUDA_TRY(d_cf_sg.upload(cf_data, (size_t)cf_indptr[nc], st));
+    CUDA_TRY(d_fn_ip.upload(fn_indptr, (size_t)nf + 1, st));
+    CUDA_TRY(d_fn_ix.upload(fn_indices, (size_t)fn_indptr[nf], st));
+    if (int rc = pb_upload_repacked_(st, tmp, d_nodes, nodes, 3, nn)) return rc;
+    CUDA_TRY(d_fn.ensure((size_t)3 * nf * sizeof(double)));
+    CUDA_TRY(d_fc.ensure((size_t)3 * nf * sizeof(double)));
+    CUDA_TRY(d_fa.ensure((size_t)nf * sizeof(double)));
+    CUDA_TRY(d_cc.ensure((size_t)3 * nc * sizeof(double)));
+    CUDA_TRY(d_cv.ensure((size_t)nc * sizeof(double)));
+    CUDA_TRY(d_bad.ensure(sizeof(int)));
     int init = INT_MAX;
-    G_TRY(cudaMemcpyAsync(d_bad.p, &init, sizeof(int), cudaMemcpyHostToDevice, st));
+    CUDA_TRY(cudaMemcpyAsync(d_bad.p, &init, sizeof(int), cudaMemcpyHostToDevice, st));
     // outputs straight in the reference's (3, n) row-major layout: component stride n, entity stride 1
     GeomOut o{d_fn.as<double>(), d_fc.as<double>(), d_fa.as<double>(), d_cc.as<double>(), d_cv.as<double>(), nf, 1, nc, 1};
-    auto grid = [](int64_t n) { return (int)std::max<int64_t>(1, std::min<int64_t>((n + 127) / 128, (int64_t)pb_sm_count() * 16)); };
-    G_TRY(cudaEventRecord(e0, st));
-    geom_face_kernel<<<grid(nf), 128, 0, st>>>(nf, d_fn_ip.as<int32_t>(), d_fn_ix.as<int32_t>(), d_nodes.as<double>(), o);
+    CUDA_TRY(timer.mark(0, st));
+    geom_face_kernel<<<grid_stride_blocks(nf, 128, 16), 128, 0, st>>>(nf, d_fn_ip.as<int32_t>(), d_fn_ix.as<int32_t>(),
+                                                                      d_nodes.as<double>(), o);
     pb_count_launch_();
-    geom_cell_kernel<<<grid(nc), 128, 0, st>>>(nc, d_cf_ip.as<int32_t>(), d_cf_ix.as<int32_t>(), d_cf_sg.as<int8_t>(),
-                                               d_fn_ip.as<int32_t>(), d_fn_ix.as<int32_t>(), d_nodes.as<double>(), o,
-                                               d_bad.as<int>());
+    geom_cell_kernel<<<grid_stride_blocks(nc, 128, 16), 128, 0, st>>>(
+        nc, d_cf_ip.as<int32_t>(), d_cf_ix.as<int32_t>(), d_cf_sg.as<int8_t>(), d_fn_ip.as<int32_t>(),
+        d_fn_ix.as<int32_t>(), d_nodes.as<double>(), o, d_bad.as<int>());
     pb_count_launch_();
-    G_TRY(cudaGetLastError());
-    G_TRY(cudaEventRecord(e1, st));
+    CUDA_TRY(cudaGetLastError());
+    CUDA_TRY(timer.mark(1, st));
     int bad = INT_MAX;
-    G_TRY(cudaMemcpyAsync(face_normals, d_fn.p, (size_t)3 * nf * sizeof(double), cudaMemcpyDeviceToHost, st));
-    G_TRY(cudaMemcpyAsync(face_centers, d_fc.p, (size_t)3 * nf * sizeof(double), cudaMemcpyDeviceToHost, st));
-    G_TRY(cudaMemcpyAsync(face_areas, d_fa.p, (size_t)nf * sizeof(double), cudaMemcpyDeviceToHost, st));
-    G_TRY(cudaMemcpyAsync(cell_centers, d_cc.p, (size_t)3 * nc * sizeof(double), cudaMemcpyDeviceToHost, st));
-    G_TRY(cudaMemcpyAsync(cell_volumes, d_cv.p, (size_t)nc * sizeof(double), cudaMemcpyDeviceToHost, st));
-    G_TRY(cudaMemcpyAsync(&bad, d_bad.p, sizeof(int), cudaMemcpyDeviceToHost, st));
-    G_TRY(cudaStreamSynchronize(st));
-    if (kernel_ms) G_TRY(cudaEventElapsedTime(kernel_ms, e0, e1));
-#undef G_TRY
+    CUDA_TRY(cudaMemcpyAsync(face_normals, d_fn.p, (size_t)3 * nf * sizeof(double), cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(cudaMemcpyAsync(face_centers, d_fc.p, (size_t)3 * nf * sizeof(double), cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(cudaMemcpyAsync(face_areas, d_fa.p, (size_t)nf * sizeof(double), cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(cudaMemcpyAsync(cell_centers, d_cc.p, (size_t)3 * nc * sizeof(double), cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(cudaMemcpyAsync(cell_volumes, d_cv.p, (size_t)nc * sizeof(double), cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(cudaMemcpyAsync(&bad, d_bad.p, sizeof(int), cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(cudaStreamSynchronize(st));
+    if (kernel_ms) CUDA_TRY(timer.ms(kernel_ms));
     if (bad != INT_MAX) {
         pb_set_error_node_(bad);
-        return done(pb_fail_(PB_EINVAL, "Some tetrahedra have negative volume (cell " + std::to_string(bad) + ")"));
+        return pb_fail_(PB_EINVAL, "Some tetrahedra have negative volume (cell " + std::to_string(bad) + ")");
     }
-    return done(PB_OK);
+    return PB_OK;
 }

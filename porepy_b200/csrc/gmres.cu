@@ -325,27 +325,20 @@ __global__ void gm_restart_kernel(int nblk, const double *__restrict__ partial, 
     for (int i = 1; i <= m; ++i) g[i] = 0.0;
 }
 
-int nthreads_grid(int64_t n) {
-    return (int)std::max<int64_t>(1, std::min<int64_t>((n + GM_THREADS - 1) / GM_THREADS, (int64_t)pb_sm_count() * 8));
-}
-
 bool gm_args_ok(int64_t n, int m, int nblk) { return n > 0 && m >= 1 && m <= GM_MAX_RESTART && nblk >= 1 && nblk <= 4096; }
 
 // z = M^-1 y (acc: z +=) with the group arrays; no preconditioner: z = y, or z += y
 int apply_prec(int64_t n, const int32_t *grp_of, const int64_t *gptr, const int32_t *grows, const int32_t *gcols,
                const int64_t *inv_off, const double *inv, const double *y, double *z, int acc, const double *scal,
                cudaStream_t st) {
-    group_apply_kernel<<<nthreads_grid(n), GM_THREADS, 0, st>>>(n, grp_of, gptr, grows, gcols, inv_off, inv, y, z, acc,
-                                                                 scal);
+    group_apply_kernel<<<grid_stride_blocks(n, GM_THREADS, 8), GM_THREADS, 0, st>>>(n, grp_of, gptr, grows, gcols,
+                                                                                    inv_off, inv, y, z, acc, scal);
     pb_count_launch_();
     CUDA_TRY(cudaGetLastError());
     return PB_OK;
 }
 
 }  // namespace
-
-struct CsrView { int64_t nrows, ncols, nnz; int32_t *indptr, *indices; double *data; };
-CsrView pb_csr_view_(const pb_csr *a);   // spmv.cu
 
 extern "C" int pb_group_inv_dev(const pb_csr *a, int64_t ngroups, const int64_t *gptr, const int32_t *grows,
                                 const int32_t *gcols, const int64_t *inv_off, int smax, double *inv_out,
@@ -360,9 +353,8 @@ extern "C" int pb_group_inv_dev(const pb_csr *a, int64_t ngroups, const int64_t 
     const size_t smem = (size_t)kInvWarps * 2 * smax * smax * sizeof(double);
     CUDA_TRY(cudaFuncSetAttribute(group_inv_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     CUDA_TRY(cudaMemsetAsync(status_dev, 0x7f, sizeof(int32_t), st));
-    const int64_t blocks = std::min<int64_t>((ngroups + kInvWarps - 1) / kInvWarps, (int64_t)pb_sm_count() * 16);
-    group_inv_kernel<<<(int)blocks, 32 * kInvWarps, smem, st>>>(ngroups, v.indptr, v.indices, v.data, gptr, grows, gcols,
-                                                                inv_off, smax, inv_out, status_dev);
+    group_inv_kernel<<<grid_stride_blocks(ngroups, kInvWarps, 16), 32 * kInvWarps, smem, st>>>(
+        ngroups, v.indptr, v.indices, v.data, gptr, grows, gcols, inv_off, smax, inv_out, status_dev);
     pb_count_launch_();
     CUDA_TRY(cudaGetLastError());
     int32_t bad = INT_MAX;

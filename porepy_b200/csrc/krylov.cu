@@ -159,8 +159,6 @@ __global__ void kry_xr_kernel(int64_t n, double *__restrict__ x, const double *_
     block_add(rho, gn + KS_RHO);
 }
 
-static int kgrid(int64_t n) { return (int)std::max<int64_t>(1, std::min<int64_t>((n + 255) / 256, (int64_t)pb_sm_count() * 8)); }
-
 extern "C" int pb_kry_init(int64_t n, const double *b, double *x, double *r, double *rhat, double *p, double *v,
                            double *scal, double tol, uint64_t stream) {
     if (!b || !x || !r || !rhat || !p || !v || !scal) return pb_fail_(PB_EINVAL, "null pointer");
@@ -169,7 +167,7 @@ extern "C" int pb_kry_init(int64_t n, const double *b, double *x, double *r, dou
                     1.0, 1.0, 1.0, 0.0, 1.0,  /* group 1 = "previous" of iteration 0: alpha = omega = rho = 1 */
                     0.0, 0.0, 0.0, tol * tol};
     CUDA_TRY(cudaMemcpyAsync(scal, h, sizeof(h), cudaMemcpyHostToDevice, st));
-    kry_init_kernel<<<kgrid(n), 256, 0, st>>>(n, b, x, r, rhat, p, v, scal);
+    kry_init_kernel<<<grid_stride_blocks(n, 256, 8), 256, 0, st>>>(n, b, x, r, rhat, p, v, scal);
     pb_count_launch_();
     CUDA_TRY(cudaGetLastError());
     return PB_OK;
@@ -191,15 +189,16 @@ extern "C" int pb_kry_p(int64_t n, const double *r, double *p, const double *v, 
     if (!kry_block_size_ok(bs) || n % bs)
         return pb_fail_(PB_EINVAL, "pb_kry_p: block size must be 1, 2, 3, 4, 5, 7 or 8 and divide n");
     cudaStream_t st = (cudaStream_t)stream;
-    if (bs == 1) kry_p_kernel<1><<<kgrid(n), 256, 0, st>>>(n, r, p, v, minv, ph, scal, cur & 1);
-    else if (bs == 2) kry_p_kernel<2><<<kgrid(n / 2), 256, 0, st>>>(n, r, p, v, minv, ph, scal, cur & 1);
-    else if (bs == 3) kry_p_kernel<3><<<kgrid(n / 3), 256, 0, st>>>(n, r, p, v, minv, ph, scal, cur & 1);
-    else if (bs == 4) kry_p_kernel<4><<<kgrid(n / 4), 256, 0, st>>>(n, r, p, v, minv, ph, scal, cur & 1);
-    else if (bs == 5) kry_p_kernel<5><<<kgrid(n / 5), 256, 0, st>>>(n, r, p, v, minv, ph, scal, cur & 1);
-    else if (bs == 6) kry_p_kernel<6><<<kgrid(n / 6), 256, 0, st>>>(n, r, p, v, minv, ph, scal, cur & 1);
-    else if (bs == 7) kry_p_kernel<7><<<kgrid(n / 7), 256, 0, st>>>(n, r, p, v, minv, ph, scal, cur & 1);
-    else if (bs == 8) kry_p_kernel<8><<<kgrid(n / 8), 256, 0, st>>>(n, r, p, v, minv, ph, scal, cur & 1);
-    else kry_p_kernel<9><<<kgrid(n / 9), 256, 0, st>>>(n, r, p, v, minv, ph, scal, cur & 1);
+    const int grid = grid_stride_blocks(n / bs, 256, 8);
+    if (bs == 1) kry_p_kernel<1><<<grid, 256, 0, st>>>(n, r, p, v, minv, ph, scal, cur & 1);
+    else if (bs == 2) kry_p_kernel<2><<<grid, 256, 0, st>>>(n, r, p, v, minv, ph, scal, cur & 1);
+    else if (bs == 3) kry_p_kernel<3><<<grid, 256, 0, st>>>(n, r, p, v, minv, ph, scal, cur & 1);
+    else if (bs == 4) kry_p_kernel<4><<<grid, 256, 0, st>>>(n, r, p, v, minv, ph, scal, cur & 1);
+    else if (bs == 5) kry_p_kernel<5><<<grid, 256, 0, st>>>(n, r, p, v, minv, ph, scal, cur & 1);
+    else if (bs == 6) kry_p_kernel<6><<<grid, 256, 0, st>>>(n, r, p, v, minv, ph, scal, cur & 1);
+    else if (bs == 7) kry_p_kernel<7><<<grid, 256, 0, st>>>(n, r, p, v, minv, ph, scal, cur & 1);
+    else if (bs == 8) kry_p_kernel<8><<<grid, 256, 0, st>>>(n, r, p, v, minv, ph, scal, cur & 1);
+    else kry_p_kernel<9><<<grid, 256, 0, st>>>(n, r, p, v, minv, ph, scal, cur & 1);
     pb_count_launch_();
     CUDA_TRY(cudaGetLastError());
     return PB_OK;
@@ -209,15 +208,16 @@ extern "C" int pb_kry_s(int64_t n, const double *r, const double *v, const doubl
     if (!kry_block_size_ok(bs) || n % bs)
         return pb_fail_(PB_EINVAL, "pb_kry_s: block size must be 1, 2, 3, 4, 5, 7 or 8 and divide n");
     cudaStream_t st = (cudaStream_t)stream;
-    if (bs == 1) kry_s_kernel<1><<<kgrid(n), 256, 0, st>>>(n, r, v, minv, s, sh, scal, cur & 1);
-    else if (bs == 2) kry_s_kernel<2><<<kgrid(n / 2), 256, 0, st>>>(n, r, v, minv, s, sh, scal, cur & 1);
-    else if (bs == 3) kry_s_kernel<3><<<kgrid(n / 3), 256, 0, st>>>(n, r, v, minv, s, sh, scal, cur & 1);
-    else if (bs == 4) kry_s_kernel<4><<<kgrid(n / 4), 256, 0, st>>>(n, r, v, minv, s, sh, scal, cur & 1);
-    else if (bs == 5) kry_s_kernel<5><<<kgrid(n / 5), 256, 0, st>>>(n, r, v, minv, s, sh, scal, cur & 1);
-    else if (bs == 6) kry_s_kernel<6><<<kgrid(n / 6), 256, 0, st>>>(n, r, v, minv, s, sh, scal, cur & 1);
-    else if (bs == 7) kry_s_kernel<7><<<kgrid(n / 7), 256, 0, st>>>(n, r, v, minv, s, sh, scal, cur & 1);
-    else if (bs == 8) kry_s_kernel<8><<<kgrid(n / 8), 256, 0, st>>>(n, r, v, minv, s, sh, scal, cur & 1);
-    else kry_s_kernel<9><<<kgrid(n / 9), 256, 0, st>>>(n, r, v, minv, s, sh, scal, cur & 1);
+    const int grid = grid_stride_blocks(n / bs, 256, 8);
+    if (bs == 1) kry_s_kernel<1><<<grid, 256, 0, st>>>(n, r, v, minv, s, sh, scal, cur & 1);
+    else if (bs == 2) kry_s_kernel<2><<<grid, 256, 0, st>>>(n, r, v, minv, s, sh, scal, cur & 1);
+    else if (bs == 3) kry_s_kernel<3><<<grid, 256, 0, st>>>(n, r, v, minv, s, sh, scal, cur & 1);
+    else if (bs == 4) kry_s_kernel<4><<<grid, 256, 0, st>>>(n, r, v, minv, s, sh, scal, cur & 1);
+    else if (bs == 5) kry_s_kernel<5><<<grid, 256, 0, st>>>(n, r, v, minv, s, sh, scal, cur & 1);
+    else if (bs == 6) kry_s_kernel<6><<<grid, 256, 0, st>>>(n, r, v, minv, s, sh, scal, cur & 1);
+    else if (bs == 7) kry_s_kernel<7><<<grid, 256, 0, st>>>(n, r, v, minv, s, sh, scal, cur & 1);
+    else if (bs == 8) kry_s_kernel<8><<<grid, 256, 0, st>>>(n, r, v, minv, s, sh, scal, cur & 1);
+    else kry_s_kernel<9><<<grid, 256, 0, st>>>(n, r, v, minv, s, sh, scal, cur & 1);
     pb_count_launch_();
     CUDA_TRY(cudaGetLastError());
     return PB_OK;
@@ -355,15 +355,13 @@ __global__ void block_diag_inv_inplace_kernel(int64_t nb, const int32_t *__restr
     }
 }
 
-struct CsrView { int64_t nrows, ncols, nnz; int32_t *indptr, *indices; double *data; };
-CsrView pb_csr_view_(const pb_csr *a);   // spmv.cu
 extern "C" int pb_csr_block_diag_inv_dev(const pb_csr *a, int bs, int64_t nblocks, double *out_dev, uint64_t stream) {
     if (!a || !out_dev) return pb_fail_(PB_EINVAL, "null pointer");
     const CsrView v = pb_csr_view_(a);
     if (!kry_block_size_ok(bs) || nblocks < 0 || nblocks * bs > v.nrows)
         return pb_fail_(PB_EINVAL, "pb_csr_block_diag_inv_dev: bad block size / count");
     cudaStream_t st = (cudaStream_t)stream;
-    const int grid = kgrid(nblocks);
+    const int grid = grid_stride_blocks(nblocks, 256, 8);
     if (bs == 1) block_diag_inv_kernel<1><<<grid, 256, 0, st>>>(nblocks, v.indptr, v.indices, v.data, out_dev);
     else if (bs == 2) block_diag_inv_kernel<2><<<grid, 256, 0, st>>>(nblocks, v.indptr, v.indices, v.data, out_dev);
     else if (bs == 3) block_diag_inv_kernel<3><<<grid, 256, 0, st>>>(nblocks, v.indptr, v.indices, v.data, out_dev);
@@ -379,7 +377,8 @@ extern "C" int pb_csr_block_diag_inv_dev(const pb_csr *a, int bs, int64_t nblock
 }
 extern "C" int pb_kry_xr(int64_t n, double *x, const double *ph, const double *sh, const double *s, const double *t,
                          double *r, const double *rhat, double *scal, int cur, int carry, uint64_t stream) {
-    kry_xr_kernel<<<kgrid(n), 256, 0, (cudaStream_t)stream>>>(n, x, ph, sh, s, t, r, rhat, scal, cur & 1, carry);
+    kry_xr_kernel<<<grid_stride_blocks(n, 256, 8), 256, 0, (cudaStream_t)stream>>>(n, x, ph, sh, s, t, r, rhat, scal,
+                                                                                   cur & 1, carry);
     pb_count_launch_();
     CUDA_TRY(cudaGetLastError());
     return PB_OK;

@@ -74,31 +74,28 @@ extern "C" int pb_fp64_peak(int kind, double *tflops) {
     if (!tflops || kind < 0 || kind > 4) return pb_fail_(PB_EINVAL, "bad arguments");
     DevBuf sink;
     CUDA_TRY(sink.ensure(8));
-    cudaEvent_t e0, e1;
-    CUDA_TRY(cudaEventCreate(&e0));
-    CUDA_TRY(cudaEventCreate(&e1));
+    KernelTimer timer;
+    CUDA_TRY(timer.create());
     const int iters = 1 << 15, block = 256, grid = pb_sm_count() * 8;
     double best = 0.0;
     for (int rep = 0; rep < 6; ++rep) {
-        CUDA_TRY(cudaEventRecord(e0, 0));
+        CUDA_TRY(timer.mark(0, 0));
         if (kind == 0) dmma_peak_kernel<<<grid, block>>>(iters, sink.as<double>());
         else if (kind == 1) dfma_peak_kernel<<<grid, block>>>(iters, sink.as<double>());
         else if (kind == 2) dmma16_peak_kernel<4><<<grid, block>>>(iters, sink.as<double>());
         else if (kind == 3) dmma16_peak_kernel<8><<<grid, block>>>(iters, sink.as<double>());
         else dmma16_peak_kernel<16><<<grid, block>>>(iters, sink.as<double>());
-        CUDA_TRY(cudaEventRecord(e1, 0));
-        CUDA_TRY(cudaEventSynchronize(e1));
+        CUDA_TRY(timer.mark(1, 0));
+        CUDA_TRY(cudaEventSynchronize(timer.ev[1]));
         pb_count_launch_();
         float ms = 0.f;
-        CUDA_TRY(cudaEventElapsedTime(&ms, e0, e1));
+        CUDA_TRY(timer.ms(&ms));
         const double per_thread_instr = (double)iters * 8;
         const double per_warp_instr[5] = {512.0, 0.0, 1024.0, 2048.0, 4096.0};
         const double flops = kind == 1 ? per_thread_instr * (grid * (double)block) * 2.0
                                        : per_thread_instr * (grid * (double)block / 32) * per_warp_instr[kind];
         if (rep > 0) best = std::max(best, flops / (ms * 1e-3) / 1e12);
     }
-    cudaEventDestroy(e0);
-    cudaEventDestroy(e1);
     *tflops = best;
     return PB_OK;
 }

@@ -1,20 +1,16 @@
-// plan.hpp -- state shared by the translation units of libporeb200.so: device buffers, the solver
-// configurations, the plan handle and the per-class kernel launcher.  api.cu owns the C ABI; the
-// kernel templates are instantiated in mpfa_launch.cu / mpsa2d.cu / mpsa3d.cu (one TU each so that
-// they compile in parallel).
+// plan.hpp -- the solver configurations, the plan handle and the per-class kernel launcher.  api.cu owns the C ABI;
+// the kernel templates are instantiated in mpfa_launch.cu / mpsa2d.cu / mpsa3d.cu (one TU each so that they compile in
+// parallel).
 #pragma once
 #include <cuda_runtime.h>
 
 #include <algorithm>
 #include <atomic>
-#include <chrono>
 #include <climits>
 #include <cstdint>
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
-#include <map>
-#include <mutex>
 #include <string>
 #include <vector>
 
@@ -22,114 +18,10 @@
 #include "mpsa_node.cuh"
 #include "face_kernels.cuh"
 #include "node_kernels.cuh"
+#include "host.hpp"
 #include "plan_host.hpp"
 
-int pb_fail_(int code, const std::string &msg);  // api.cu: sets pb_last_error()
-void pb_count_launch_();                         // api.cu: pb_launch_count()
-void pb_set_error_node_(int64_t node);           // api.cu: pb_last_error_node()
-#define CUDA_TRY(x)                                                                        \
-    do {                                                                                   \
-        cudaError_t e_ = (x);                                                              \
-        if (e_ != cudaSuccess)                                                             \
-            return pb_fail_(PB_ECUDA, std::string(#x) + ": " + cudaGetErrorString(e_));    \
-    } while (0)
-
 using namespace pb;
-
-// ------------------------------------------------------------------------------------
-// device buffers
-// ------------------------------------------------------------------------------------
-// Freed device arrays are kept in a size-keyed pool (like the page-locked host pool of the Python layer): every
-// discretize() of a model allocates and releases the same ~25 GB of value arrays, and cudaMalloc / cudaFree of such
-// blocks cost tens of milliseconds each and synchronise the device.  POREB200_DEVICE_POOL_BYTES caps the pool
-// (default 64 GiB; 0 disables it).
-struct DevPool {
-    std::mutex mu;
-    std::multimap<size_t, void *> free_blocks;
-    size_t held = 0, cap = 64ull << 30;
-    DevPool() {
-        if (const char *e = getenv("POREB200_DEVICE_POOL_BYTES")) cap = strtoull(e, nullptr, 10);
-    }
-    void *take(size_t n, size_t &got) {
-        std::lock_guard<std::mutex> g(mu);
-        // exact size only: a near fit takes a block that the next request of ITS size then misses (measured: two
-        // slow re-discretizations, pb_plan_create 0.19-0.27 s instead of 0.045 s, until the pool had spares of every size)
-        auto it = free_blocks.find(n);
-        if (it == free_blocks.end()) return nullptr;
-        void *q = it->second;
-        got = it->first;
-        free_blocks.erase(it);
-        held -= got;
-        return q;
-    }
-    bool give(void *q, size_t n) {
-        std::lock_guard<std::mutex> g(mu);
-        if (held + n > cap) return false;   // small blocks are pooled as well: their cudaMalloc / cudaFree pairs were
-                                            // measured to stall sporadically (26 calls: 0.6 ms, or 230 ms once in four)
-        free_blocks.emplace(n, q);
-        held += n;
-        return true;
-    }
-    void trim() {
-        std::lock_guard<std::mutex> g(mu);
-        for (auto &kv : free_blocks) cudaFree(kv.second);
-        free_blocks.clear();
-        held = 0;
-    }
-};
-DevPool &pb_dev_pool_();  // api.cu
-void pb_alloc_stat_(int kind, double seconds);   // api.cu: cudaMalloc (0) / cudaFree (1) calls that missed the pool
-
-struct DevBuf {
-    void *p = nullptr;
-    size_t bytes = 0;
-    DevBuf() = default;
-    DevBuf(const DevBuf &) = delete;
-    DevBuf &operator=(const DevBuf &) = delete;
-    DevBuf(DevBuf &&o) noexcept : p(o.p), bytes(o.bytes) { o.p = nullptr; o.bytes = 0; }
-    DevBuf &operator=(DevBuf &&o) noexcept {
-        if (this != &o) { release(); p = o.p; bytes = o.bytes; o.p = nullptr; o.bytes = 0; }
-        return *this;
-    }
-    ~DevBuf() { release(); }
-    void release() {
-        if (p && !pb_dev_pool_().give(p, bytes)) {
-            const auto t0_ = std::chrono::steady_clock::now();
-            cudaFree(p);
-            pb_alloc_stat_(1, std::chrono::duration<double>(std::chrono::steady_clock::now() - t0_).count());
-        }
-        p = nullptr;
-        bytes = 0;
-    }
-    cudaError_t ensure(size_t n) {
-        if (n <= bytes && p) return cudaSuccess;
-        release();
-        if (n == 0) n = 8;
-        size_t got = 0;
-        if ((p = pb_dev_pool_().take(n, got)) != nullptr) { bytes = got; return cudaSuccess; }
-        const auto t0_ = std::chrono::steady_clock::now();
-        cudaError_t e = cudaMalloc(&p, n);
-        pb_alloc_stat_(0, std::chrono::duration<double>(std::chrono::steady_clock::now() - t0_).count());
-        if (e == cudaErrorMemoryAllocation) {   // give the pooled blocks back to the driver and retry once
-            (void)cudaGetLastError();
-            pb_dev_pool_().trim();
-            e = cudaMalloc(&p, n);
-        }
-        if (e == cudaSuccess) bytes = n; else p = nullptr;
-        return e;
-    }
-    template <class T>
-    cudaError_t upload(const T *h, size_t count, cudaStream_t st) {
-        cudaError_t e = ensure(count * sizeof(T));
-        if (e != cudaSuccess) return e;
-        if (count == 0) return cudaSuccess;
-        return cudaMemcpyAsync(p, h, count * sizeof(T), cudaMemcpyHostToDevice, st);
-    }
-    template <class T>
-    cudaError_t upload(const std::vector<T> &v, cudaStream_t st) { return upload(v.data(), v.size(), st); }
-    template <class T>
-    T *as() const { return (T *)p; }
-};
 
 // Solver configurations (node_kernels.cuh).  A node goes to the first one that fits.
 using Cfg0 = TileGJ<1, 2, 6, 4>;   // team 32  : MPFA hexahedral nodes (12 x 45), DMMA, one warp per node
@@ -163,8 +55,8 @@ struct NodeClass {
 
 struct pb_plan {
     HostPlan H;
-    cudaStream_t stream = nullptr;
-    cudaEvent_t e0 = nullptr, e1 = nullptr;
+    Stream stream;
+    KernelTimer timer;             // pb_mpfa_assemble / pb_mpsa_assemble
     // plan arrays
     DevBuf fn_indptr, node_sc_ptr, sc_cell, node_sf_ptr, sf_face, sf_sides, sf_bloc, slot_sf, node_nb,
         sc_ncn, posfc_ptr, posfb_ptr, poscc_ptr, poscb_ptr, pos_fc, pos_fb, pos_cc, pos_cb, nbf_ptr, nbf_idx,
@@ -201,23 +93,11 @@ struct pb_plan {
     DevBuf o_stress, o_bstress, o_bdc, o_bdf;
     DevBuf o_dd[PB_MAX_ALPHA], o_bdd[PB_MAX_ALPHA], o_sg[PB_MAX_ALPHA], o_cons[PB_MAX_ALPHA],
         o_bdp[PB_MAX_ALPHA];
+    // the stream's copies and kernels may still use the buffers, which go back to the pool right after
+    ~pb_plan() { if (stream) cudaStreamSynchronize(stream); }
 };
 
-
 static const size_t kMaxSmem = 227 * 1024;
-// SMs of the current device: the cap of every grid-stride launch (H100 SXM 132, H100 PCIe 114)
-inline int pb_sm_count() {
-    static int cache[64] = {0};
-    int dev = 0;
-    if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) dev = 0;
-    if (!cache[dev]) {
-        int n = 0;
-        if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n < 1) n = 1;
-        cache[dev] = n;
-    }
-    return cache[dev];
-}
-
 
 // launch one class with kernel template KERNEL<ND, Solver>
 #define PB_LAUNCH_CFG(KERNEL, ND, ...)                                              \
@@ -257,8 +137,7 @@ static int launch_one(K kernel, const NodeClass &c, pb_plan *p, const Prm &prm, 
             if ((size_t)kb * 1024 >= need) { pct = kb * 100 / 228; break; }
         CUDA_TRY(cudaFuncSetAttribute(kernel, cudaFuncAttributePreferredSharedMemoryCarveout, pct));
     }
-    int64_t need = ((int64_t)c.n + tpb - 1) / tpb;
-    int grid = (int)std::max<int64_t>(1, std::min<int64_t>(need, (int64_t)pb_sm_count() * per_sm));
+    const int grid = grid_stride_blocks(c.n, tpb, per_sm);
     double *ws = nullptr;
     if (c.a_global) {
         CUDA_TRY(p->a_ws.ensure((size_t)grid * tpb * c.a_doubles * sizeof(double)));
@@ -271,7 +150,6 @@ static int launch_one(K kernel, const NodeClass &c, pb_plan *p, const Prm &prm, 
     CUDA_TRY(cudaGetLastError());
     return PB_OK;
 }
-
 
 // kernel launches of all node classes of a plan (mpfa_launch.cu, mpsa2d.cu, mpsa3d.cu)
 int pb_launch_mpfa_(pb_plan *p, const MpfaParams &prm, const MpfaOut &o);

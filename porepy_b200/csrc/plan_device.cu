@@ -222,13 +222,14 @@ int pb_build_device_topology_(pb_plan *p, int nd, int64_t nc, int64_t nf, int64_
     CUDA_TRY(cudaMemsetAsync(sfcount.p, 0, (size_t)(nn + 1) * 4, st));
     CUDA_TRY(cudaMemsetAsync(fill.p, 0, (size_t)(nn + 1) * 4, st));
     CUDA_TRY(cudaMemsetAsync(flags.p, 0, 8 * sizeof(int), st));
-    const int block = 256;
-    auto grid_for = [&](int64_t n) { return (int)std::max<int64_t>(1, std::min<int64_t>((n + block - 1) / block, (int64_t)pb_sm_count() * 16)); };
-    pd_count_kernel<<<grid_for(nc), block, 0, st>>>(nc, cf_ip.as<int32_t>(), cf_ix.as<int32_t>(), p->fn_indptr.as<int32_t>(),
-                                                    fn_idx_dev.as<int32_t>(), hcount.as<int32_t>(), ncnx.as<int32_t>());
-    pd_count_sf_kernel<<<grid_for(U), block, 0, st>>>(U, fn_idx_dev.as<int32_t>(), sfcount.as<int32_t>());
+    const int block = 256;   // one thread per cell (gc), node (gn), face (gf) or sub-face (gu)
+    const int gc = grid_stride_blocks(nc, block, 16), gn = grid_stride_blocks(nn, block, 16),
+              gf = grid_stride_blocks(nf, block, 16), gu = grid_stride_blocks(U, block, 16);
+    pd_count_kernel<<<gc, block, 0, st>>>(nc, cf_ip.as<int32_t>(), cf_ix.as<int32_t>(), p->fn_indptr.as<int32_t>(),
+                                          fn_idx_dev.as<int32_t>(), hcount.as<int32_t>(), ncnx.as<int32_t>());
+    pd_count_sf_kernel<<<gu, block, 0, st>>>(U, fn_idx_dev.as<int32_t>(), sfcount.as<int32_t>());
     // sub-cells per node = half-faces per node / nd
-    pd_div_kernel<<<grid_for(nn), block, 0, st>>>(nn, nd, hcount.as<int32_t>(), hcount.as<int32_t>(), flags.as<int>());
+    pd_div_kernel<<<gn, block, 0, st>>>(nn, nd, hcount.as<int32_t>(), hcount.as<int32_t>(), flags.as<int>());
     CUDA_TRY(p->node_sc_ptr.ensure((size_t)(nn + 1) * 4));
     CUDA_TRY(p->node_sf_ptr.ensure((size_t)(nn + 1) * 4));
     int64_t S = 0, sf_total = 0;
@@ -250,9 +251,9 @@ int pb_build_device_topology_(pb_plan *p, int nd, int64_t nc, int64_t nf, int64_
     H.S = S; H.H = Hh;
     if (sf_total != U) return pb_fail_(PB_EINVAL, "internal: sub-face count");
     CUDA_TRY(hfbuf.ensure((size_t)std::max<int64_t>(1, Hh) * sizeof(HalfFace)));
-    pd_scatter_kernel<<<grid_for(nc), block, 0, st>>>(nc, cf_ip.as<int32_t>(), cf_ix.as<int32_t>(), cf_da.as<int8_t>(),
-                                                      p->fn_indptr.as<int32_t>(), fn_idx_dev.as<int32_t>(),
-                                                      p->node_sc_ptr.as<int32_t>(), nd, fill.as<int32_t>(), hfbuf.as<HalfFace>());
+    pd_scatter_kernel<<<gc, block, 0, st>>>(nc, cf_ip.as<int32_t>(), cf_ix.as<int32_t>(), cf_da.as<int8_t>(),
+                                            p->fn_indptr.as<int32_t>(), fn_idx_dev.as<int32_t>(),
+                                            p->node_sc_ptr.as<int32_t>(), nd, fill.as<int32_t>(), hfbuf.as<HalfFace>());
     CUDA_TRY(p->sc_cell.ensure((size_t)std::max<int64_t>(1, S) * 4));
     CUDA_TRY(p->slot_sf.ensure((size_t)std::max<int64_t>(1, Hh) * 2));
     CUDA_TRY(p->sf_face.ensure((size_t)std::max<int64_t>(1, U) * 4));
@@ -262,7 +263,7 @@ int pb_build_device_topology_(pb_plan *p, int nd, int64_t nc, int64_t nf, int64_
     constexpr int CAP = 1024, WPB = 4;
     const size_t smem = (size_t)WPB * CAP * (8 + 5 * 4);
     CUDA_TRY(cudaFuncSetAttribute(pd_node_kernel<CAP>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    const int gridn = (int)std::max<int64_t>(1, std::min<int64_t>((nn + WPB - 1) / WPB, (int64_t)pb_sm_count() * 2));
+    const int gridn = grid_stride_blocks(nn, WPB, 2);
     pd_node_kernel<CAP><<<gridn, WPB * 32, smem, st>>>(nn, nd, nf, hfbuf.as<HalfFace>(), p->node_sc_ptr.as<int32_t>(),
                                                        p->node_sf_ptr.as<int32_t>(), p->fn_indptr.as<int32_t>(),
                                                        p->sc_cell.as<int32_t>(), p->slot_sf.as<uint16_t>(),
@@ -271,7 +272,7 @@ int pb_build_device_topology_(pb_plan *p, int nd, int64_t nc, int64_t nf, int64_
                                                        flags.as<int>() + 1, flags.as<int>() + 4);
     // nodes per cell, cell -> nodes, boundary faces per node, face -> cells
     CUDA_TRY(p->sc_ncn.ensure((size_t)nc * 4));
-    pd_div_kernel<<<grid_for(nc), block, 0, st>>>(nc, nd, ncnx.as<int32_t>(), p->sc_ncn.as<int32_t>(), nullptr);
+    pd_div_kernel<<<gc, block, 0, st>>>(nc, nd, ncnx.as<int32_t>(), p->sc_ncn.as<int32_t>(), nullptr);
     CUDA_TRY(p->cn_ptr.ensure((size_t)(nc + 1) * 4));
     CUDA_TRY(p->nbf_ptr.ensure((size_t)(nn + 1) * 4));
     int64_t cn_total = 0, nbf_total = 0;
@@ -294,16 +295,16 @@ int pb_build_device_topology_(pb_plan *p, int nd, int64_t nc, int64_t nf, int64_
     CUDA_TRY(cudaMemsetAsync(cfill.p, 0, (size_t)nc * 4, st));
     CUDA_TRY(p->cn_idx.ensure((size_t)std::max<int64_t>(1, S) * 4));
     CUDA_TRY(p->nbf_idx.ensure((size_t)std::max<int64_t>(1, nbf_total) * 4));
-    pd_adjacency_kernel<<<grid_for(nn), block, 0, st>>>(nn, p->node_sc_ptr.as<int32_t>(), p->sc_cell.as<int32_t>(),
-                                                        p->cn_ptr.as<int32_t>(), cfill.as<int32_t>(), p->cn_idx.as<int32_t>(),
-                                                        p->node_sf_ptr.as<int32_t>(), p->sf_face.as<int32_t>(),
-                                                        p->sf_bloc.as<uint16_t>(), p->nbf_ptr.as<int32_t>(),
-                                                        p->nbf_idx.as<int32_t>());
+    pd_adjacency_kernel<<<gn, block, 0, st>>>(nn, p->node_sc_ptr.as<int32_t>(), p->sc_cell.as<int32_t>(),
+                                              p->cn_ptr.as<int32_t>(), cfill.as<int32_t>(), p->cn_idx.as<int32_t>(),
+                                              p->node_sf_ptr.as<int32_t>(), p->sf_face.as<int32_t>(),
+                                              p->sf_bloc.as<uint16_t>(), p->nbf_ptr.as<int32_t>(),
+                                              p->nbf_idx.as<int32_t>());
     CUDA_TRY(p->face_cells.ensure((size_t)2 * nf * 4));
     CUDA_TRY(cudaMemsetAsync(p->face_cells.p, 0xFF, (size_t)2 * nf * 4, st));
-    pd_face_cells_kernel<<<grid_for(nc), block, 0, st>>>(nc, cf_ip.as<int32_t>(), cf_ix.as<int32_t>(), cf_da.as<int8_t>(),
-                                                         p->face_cells.as<int32_t>(), flags.as<int>() + 2);
-    pd_face_cells_order_kernel<<<grid_for(nf), block, 0, st>>>(nf, p->face_cells.as<int32_t>());
+    pd_face_cells_kernel<<<gc, block, 0, st>>>(nc, cf_ip.as<int32_t>(), cf_ix.as<int32_t>(), cf_da.as<int8_t>(),
+                                               p->face_cells.as<int32_t>(), flags.as<int>() + 2);
+    pd_face_cells_order_kernel<<<gf, block, 0, st>>>(nf, p->face_cells.as<int32_t>());
     for (int i = 0; i < 9; ++i) pb_count_launch_();
     CUDA_TRY(cudaGetLastError());
     // position-map offsets on the host from the three per-node arrays

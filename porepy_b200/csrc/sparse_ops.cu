@@ -8,12 +8,6 @@
 // on pb_csr matrices that never leave HBM.  FP64 values, int32 indices, sorted rows (canonical CSR, like scipy's).
 #include "csr_build.cuh"
 
-struct pb_csr;
-int pb_csr_alloc_(int64_t nrows, int64_t ncols, int64_t nnz, pb_csr **out);  // spmv.cu
-struct CsrView { int64_t nrows, ncols, nnz; int32_t *indptr, *indices; double *data; };
-CsrView pb_csr_view_(const pb_csr *a);                                        // spmv.cu
-void pb_csr_set_nnz_(pb_csr *a, int64_t nnz);                                 // spmv.cu (shrink only)
-
 // The two passes of every operation here, on the legacy default stream: count(counts) launches the pass that writes
 // the length of each of the nrows rows of C (and may refuse), the lengths are scanned into C's row offsets, and
 // fill(C) launches the pass that writes C's entries.  `what` names the result in the overflow message.
@@ -29,16 +23,16 @@ static int csr_two_pass(int64_t nrows, int64_t ncols, const char *what, Count co
     rc = pb_scan_offsets_(counts.as<int32_t>(), ip.as<int32_t>(), nrows, 0, &nnz);
     if (rc) return rc;
     if (nnz >= 0x7fffffffll) return pb_fail_(PB_ENOTIMPL, std::string(what) + " exceeds int32 indices");
-    pb_csr *c = nullptr;
-    rc = pb_csr_alloc_(nrows, ncols, nnz, &c);
+    CsrPtr c;
+    rc = pb_csr_alloc_(nrows, ncols, nnz, c);
     if (rc) return rc;
-    const CsrView C = pb_csr_view_(c);
+    const CsrView C = pb_csr_view_(c.get());
     CUDA_TRY(cudaMemcpy(C.indptr, ip.p, (size_t)(nrows + 1) * sizeof(int32_t), cudaMemcpyDeviceToDevice));
     fill(C);
     pb_count_launch_();
     CUDA_TRY(cudaGetLastError());
     CUDA_TRY(cudaDeviceSynchronize());
-    *out = c;
+    *out = c.release();
     return PB_OK;
 }
 
@@ -127,8 +121,8 @@ extern "C" int pb_csr_spgemm(const pb_csr *a_, const pb_csr *b_, pb_csr **out) {
     DevBuf flag;
     CUDA_TRY(flag.ensure(2 * sizeof(int)));
     CUDA_TRY(cudaMemset(flag.p, 0, 2 * sizeof(int)));
-    const int g1 = (int)std::max<int64_t>(1, std::min<int64_t>((A.nrows + 255) / 256, (int64_t)pb_sm_count() * 8));
-    spgemm_bound_kernel<<<g1, 256>>>(A.nrows, A.indptr, A.indices, B.indptr, flag.as<int>() + 1);
+    spgemm_bound_kernel<<<grid_stride_blocks(A.nrows, 256, 8), 256>>>(A.nrows, A.indptr, A.indices, B.indptr,
+                                                                      flag.as<int>() + 1);
     pb_count_launch_();
     int hb[2] = {0, 0};
     CUDA_TRY(cudaMemcpy(hb, flag.p, sizeof(hb), cudaMemcpyDeviceToHost));
@@ -141,7 +135,7 @@ extern "C" int pb_csr_spgemm(const pb_csr *a_, const pb_csr *b_, pb_csr **out) {
     const size_t smem = (size_t)wpb * tsize * (sizeof(int32_t) + sizeof(double));
     CUDA_TRY(cudaFuncSetAttribute(spgemm_kernel<0>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     CUDA_TRY(cudaFuncSetAttribute(spgemm_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    const int grid = (int)std::max<int64_t>(1, std::min<int64_t>((A.nrows + wpb - 1) / wpb, (int64_t)pb_sm_count() * 4));
+    const int grid = grid_stride_blocks(A.nrows, wpb, 4);
     return csr_two_pass(
         A.nrows, B.ncols, "sparse product",
         [&](int32_t *counts) {
@@ -188,7 +182,7 @@ extern "C" int pb_csr_axpby(double alpha, const pb_csr *a_, double beta, const p
     if (!a_ || !b_ || !out) return pb_fail_(PB_EINVAL, "null pointer");
     const CsrView A = pb_csr_view_(a_), B = pb_csr_view_(b_);
     if (A.nrows != B.nrows || A.ncols != B.ncols) return pb_fail_(PB_EINVAL, "dimension mismatch in sparse sum");
-    const int grid = (int)std::max<int64_t>(1, std::min<int64_t>((A.nrows + 127) / 128, (int64_t)pb_sm_count() * 16));
+    const int grid = grid_stride_blocks(A.nrows, 128, 16);
     return csr_two_pass(
         A.nrows, A.ncols, "sparse sum",
         [&](int32_t *counts) {
@@ -222,18 +216,18 @@ extern "C" int pb_csr_scale_dev(const pb_csr *a_, const double *d_dev, int by_co
     long long nnz = 0;
     CUDA_TRY(cudaMemcpy(&nnz, A.indptr + A.nrows, sizeof(int32_t), cudaMemcpyDeviceToHost));
     nnz &= 0xffffffffll;
-    pb_csr *c = nullptr;
-    int rc = pb_csr_alloc_(A.nrows, A.ncols, nnz, &c);
+    CsrPtr c;
+    int rc = pb_csr_alloc_(A.nrows, A.ncols, nnz, c);
     if (rc) return rc;
-    const CsrView C = pb_csr_view_(c);
+    const CsrView C = pb_csr_view_(c.get());
     CUDA_TRY(cudaMemcpy(C.indptr, A.indptr, (size_t)(A.nrows + 1) * sizeof(int32_t), cudaMemcpyDeviceToDevice));
     if (nnz) CUDA_TRY(cudaMemcpy(C.indices, A.indices, (size_t)nnz * sizeof(int32_t), cudaMemcpyDeviceToDevice));
-    const int grid = (int)std::max<int64_t>(1, std::min<int64_t>((A.nrows * 32 + 255) / 256, (int64_t)pb_sm_count() * 16));
-    scale_kernel<<<grid, 256>>>(A.nrows, A.indptr, A.indices, A.data, d_dev, by_cols, C.data);
+    scale_kernel<<<grid_stride_blocks(A.nrows * 32, 256, 16), 256>>>(A.nrows, A.indptr, A.indices, A.data, d_dev,
+                                                                     by_cols, C.data);
     pb_count_launch_();
     CUDA_TRY(cudaGetLastError());
     CUDA_TRY(cudaDeviceSynchronize());
-    *out = c;
+    *out = c.release();
     return PB_OK;
 }
 
@@ -284,7 +278,7 @@ extern "C" int pb_csr_bmat(int nbr, int nbc, const pb_csr *const *blocks, const 
     CUDA_TRY(dblocks.upload(hb, 0));
     CUDA_TRY(drow.upload(ro, 0));
     CUDA_TRY(dcol.upload(co, 0));
-    const int grid = (int)std::max<int64_t>(1, std::min<int64_t>((nrows + 127) / 128, (int64_t)pb_sm_count() * 16));
+    const int grid = grid_stride_blocks(nrows, 128, 16);
     return csr_two_pass(
         nrows, co[nbc], "block matrix",
         [&](int32_t *counts) {

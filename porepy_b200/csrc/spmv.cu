@@ -21,26 +21,36 @@
 #include <tuple>
 
 
+// Destroying a matrix does not synchronize: its stream and events go first, then its arrays return to the pool.
 struct pb_csr {
     int64_t nrows = 0, ncols = 0, nnz = 0;
     int32_t *indptr = nullptr, *indices = nullptr;
     double *data = nullptr, *x = nullptr, *y = nullptr;
     DevBuf b_indptr, b_indices, b_data, b_x, b_y;   // owners of the arrays above (pooled device blocks)
-    cudaError_t alloc() {
-        cudaError_t e;
-        if ((e = b_indptr.ensure((size_t)(nrows + 1) * sizeof(int32_t))) != cudaSuccess) return e;
-        if ((e = b_indices.ensure((size_t)(nnz ? nnz : 1) * sizeof(int32_t))) != cudaSuccess) return e;
-        if ((e = b_data.ensure((size_t)(nnz ? nnz : 1) * sizeof(double))) != cudaSuccess) return e;
-        if ((e = b_x.ensure((size_t)(ncols ? ncols : 1) * sizeof(double))) != cudaSuccess) return e;
-        if ((e = b_y.ensure((size_t)(nrows ? nrows : 1) * sizeof(double))) != cudaSuccess) return e;
-        indptr = b_indptr.as<int32_t>(); indices = b_indices.as<int32_t>();
-        data = b_data.as<double>(); x = b_x.as<double>(); y = b_y.as<double>();
-        return cudaSuccess;
-    }
     int tpr = 8;
-    cudaStream_t stream = nullptr;
-    cudaEvent_t e0 = nullptr, e1 = nullptr;
+    Stream stream;
+    KernelTimer timer;                               // the lane-count tuning and pb_csr_spmv_bench
 };
+
+// The body of every constructor: the sizes, the stream, the timer, the arrays and the default lanes per row.
+static int csr_new(int64_t nrows, int64_t ncols, int64_t nnz, CsrPtr &out) {
+    CsrPtr a(new pb_csr);
+    a->nrows = nrows; a->ncols = ncols; a->nnz = nnz;
+    CUDA_TRY(a->stream.create());
+    CUDA_TRY(a->timer.create());
+    CUDA_TRY(a->b_indptr.ensure((size_t)(nrows + 1) * sizeof(int32_t)));
+    CUDA_TRY(a->b_indices.ensure((size_t)(nnz ? nnz : 1) * sizeof(int32_t)));
+    CUDA_TRY(a->b_data.ensure((size_t)(nnz ? nnz : 1) * sizeof(double)));
+    CUDA_TRY(a->b_x.ensure((size_t)(ncols ? ncols : 1) * sizeof(double)));
+    CUDA_TRY(a->b_y.ensure((size_t)(nrows ? nrows : 1) * sizeof(double)));
+    a->indptr = a->b_indptr.as<int32_t>(); a->indices = a->b_indices.as<int32_t>();
+    a->data = a->b_data.as<double>(); a->x = a->b_x.as<double>(); a->y = a->b_y.as<double>();
+    const double mean = nrows ? (double)nnz / (double)nrows : 0.0;
+    a->tpr = mean <= 3 ? 2 : mean <= 6 ? 4 : mean <= 24 ? 8 : mean <= 48 ? 16 : 32;
+    out = std::move(a);
+    return PB_OK;
+}
+void CsrDeleter::operator()(pb_csr *a) const { delete a; }
 
 template <int TPR>
 __global__ void __launch_bounds__(256)
@@ -119,10 +129,7 @@ __global__ void __launch_bounds__(256)
 static int launch_spmv_dots(pb_csr *a, const double *x, double *y, const double *w1, double *d1, const double *w2,
                             int w2_is_y, double *d2, cudaStream_t st) {
     const int block = 256;
-    const int64_t groups_per_block = block / a->tpr;
-    int64_t need = (a->nrows + groups_per_block - 1) / groups_per_block;
-    int64_t cap = (int64_t)pb_sm_count() * 8 * 4;
-    int grid = (int)(need < cap ? (need < 1 ? 1 : need) : cap);
+    const int grid = grid_stride_blocks(a->nrows, block / a->tpr, 8 * 4);
 #define PB_SPMV_DOTS(T) csr_spmv_dots_kernel<T><<<grid, block, 0, st>>>(a->nrows, a->indptr, a->indices, a->data, x, y, w1, d1, w2, w2_is_y, d2)
     switch (a->tpr) {
         case 2: PB_SPMV_DOTS(2); break;
@@ -139,10 +146,8 @@ static int launch_spmv_dots(pb_csr *a, const double *x, double *y, const double 
 
 static int launch_spmv(pb_csr *a, const double *x, double *y, cudaStream_t st) {
     const int block = 256;
-    const int64_t groups_per_block = block / a->tpr;
-    int64_t need = (a->nrows + groups_per_block - 1) / groups_per_block;
-    int64_t cap = (int64_t)pb_sm_count() * 8 * 4;  // 8 resident CTAs of 256 threads per SM, 4 waves
-    int grid = (int)(need < cap ? (need < 1 ? 1 : need) : cap);
+    // 8 resident CTAs of 256 threads per SM, 4 waves
+    const int grid = grid_stride_blocks(a->nrows, block / a->tpr, 8 * 4);
     switch (a->tpr) {
         case 2: csr_spmv_kernel<2><<<grid, block, 0, st>>>(a->nrows, a->indptr, a->indices, a->data, x, y); break;
         case 4: csr_spmv_kernel<4><<<grid, block, 0, st>>>(a->nrows, a->indptr, a->indices, a->data, x, y); break;
@@ -180,10 +185,10 @@ static void autotune_tpr(pb_csr *a) {
         a->tpr = cands[ci];
         float ms = 1e30f;
         if (launch_spmv(a, a->x, a->y, a->stream) != PB_OK) break;
-        cudaEventRecord(a->e0, a->stream);
+        a->timer.mark(0, a->stream);
         for (int i = 0; i < 10; ++i) launch_spmv(a, a->x, a->y, a->stream);
-        cudaEventRecord(a->e1, a->stream);
-        if (cudaEventSynchronize(a->e1) == cudaSuccess) cudaEventElapsedTime(&ms, a->e0, a->e1);
+        a->timer.mark(1, a->stream);
+        if (cudaEventSynchronize(a->timer.ev[1]) == cudaSuccess) a->timer.ms(&ms);
         if (ms < best) { best = ms; best_tpr = cands[ci]; }
     }
     a->tpr = best_tpr;
@@ -191,42 +196,22 @@ static void autotune_tpr(pb_csr *a) {
     tuned[key] = best_tpr;
 }
 
-extern "C" void pb_csr_destroy(pb_csr *a) {
-    if (!a) return;
-    if (a->e0) cudaEventDestroy(a->e0);
-    if (a->e1) cudaEventDestroy(a->e1);
-    if (a->stream) cudaStreamDestroy(a->stream);
-    delete a;
-}
+extern "C" void pb_csr_destroy(pb_csr *a) { delete a; }
 
 extern "C" int pb_csr_create(int64_t nrows, int64_t ncols, int64_t nnz, const int32_t *indptr,
                              const int32_t *indices, const double *data, pb_csr **out) {
     if (!out || !indptr || (nnz > 0 && (!indices || !data)) || nrows < 0 || ncols < 0)
         return pb_fail_(PB_EINVAL, "bad CSR arguments");
-    int ndev = 0;
-    if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev < 1)
-        return pb_fail_(PB_ECUDA, "no CUDA device: libporeb200 has no CPU path");
-    pb_csr *a = new pb_csr;
-    a->nrows = nrows; a->ncols = ncols; a->nnz = nnz;
-    auto bail = [&](cudaError_t e) {
-        std::string m = cudaGetErrorString(e);
-        pb_csr_destroy(a);
-        return pb_fail_(PB_ECUDA, m);
-    };
-    cudaError_t e;
-    if ((e = cudaStreamCreateWithFlags(&a->stream, cudaStreamNonBlocking)) != cudaSuccess) return bail(e);
-    if ((e = cudaEventCreate(&a->e0)) != cudaSuccess) return bail(e);
-    if ((e = cudaEventCreate(&a->e1)) != cudaSuccess) return bail(e);
-    if ((e = a->alloc()) != cudaSuccess) return bail(e);
-    if ((e = cudaMemcpy(a->indptr, indptr, (nrows + 1) * sizeof(int32_t), cudaMemcpyHostToDevice)) != cudaSuccess) return bail(e);
+    if (int rc = pb_require_device()) return rc;
+    CsrPtr a;
+    if (int rc = csr_new(nrows, ncols, nnz, a)) return rc;
+    CUDA_TRY(cudaMemcpy(a->indptr, indptr, (nrows + 1) * sizeof(int32_t), cudaMemcpyHostToDevice));
     if (nnz) {
-        if ((e = cudaMemcpy(a->indices, indices, nnz * sizeof(int32_t), cudaMemcpyHostToDevice)) != cudaSuccess) return bail(e);
-        if ((e = cudaMemcpy(a->data, data, nnz * sizeof(double), cudaMemcpyHostToDevice)) != cudaSuccess) return bail(e);
+        CUDA_TRY(cudaMemcpy(a->indices, indices, nnz * sizeof(int32_t), cudaMemcpyHostToDevice));
+        CUDA_TRY(cudaMemcpy(a->data, data, nnz * sizeof(double), cudaMemcpyHostToDevice));
     }
-    double mean = nrows ? (double)nnz / (double)nrows : 0.0;
-    a->tpr = mean <= 3 ? 2 : mean <= 6 ? 4 : mean <= 24 ? 8 : mean <= 48 ? 16 : 32;
-    autotune_tpr(a);
-    *out = a;
+    autotune_tpr(a.get());
+    *out = a.release();
     return PB_OK;
 }
 
@@ -265,12 +250,10 @@ extern "C" int pb_csr_diagonal(pb_csr *a, double *diag) {
     DevBuf tmp;                       // pooled: no cudaMalloc / cudaFree pair (a device sync each) per call
     CUDA_TRY(tmp.ensure((size_t)(n ? n : 1) * sizeof(double)));
     double *d = tmp.as<double>();
-    const int grid = (int)(n / 256 + 1 < pb_sm_count() * 16 ? n / 256 + 1 : pb_sm_count() * 16);
-    csr_diagonal_kernel<<<grid, 256, 0, a->stream>>>(n, a->indptr, a->indices, a->data, d);
+    csr_diagonal_kernel<<<grid_stride_blocks(n, 256, 16), 256, 0, a->stream>>>(n, a->indptr, a->indices, a->data, d);
     pb_count_launch_();
-    cudaError_t e = cudaMemcpyAsync(diag, d, n * sizeof(double), cudaMemcpyDeviceToHost, a->stream);
-    if (e == cudaSuccess) e = cudaStreamSynchronize(a->stream);
-    if (e != cudaSuccess) return pb_fail_(PB_ECUDA, cudaGetErrorString(e));
+    CUDA_TRY(cudaMemcpyAsync(diag, d, n * sizeof(double), cudaMemcpyDeviceToHost, a->stream));
+    CUDA_TRY(cudaStreamSynchronize(a->stream));
     return PB_OK;
 }
 
@@ -290,55 +273,23 @@ extern "C" int pb_csr_download(pb_csr *a, int32_t *indptr, int32_t *indices, dou
     return PB_OK;
 }
 
-// matrix whose pattern is copied from device arrays and whose values the caller fills (api.cu)
 int pb_csr_from_device_pattern_(int64_t nrows, int64_t ncols, int64_t nnz, const int32_t *indptr_dev,
-                                const int32_t *indices_dev, pb_csr **out) {
-    pb_csr *a = new pb_csr;
-    a->nrows = nrows; a->ncols = ncols; a->nnz = nnz;
-    auto bail = [&](cudaError_t e) {
-        std::string m = cudaGetErrorString(e);
-        pb_csr_destroy(a);
-        return pb_fail_(PB_ECUDA, m);
-    };
-    cudaError_t e;
-    if ((e = cudaStreamCreateWithFlags(&a->stream, cudaStreamNonBlocking)) != cudaSuccess) return bail(e);
-    if ((e = cudaEventCreate(&a->e0)) != cudaSuccess) return bail(e);
-    if ((e = cudaEventCreate(&a->e1)) != cudaSuccess) return bail(e);
-    if ((e = a->alloc()) != cudaSuccess) return bail(e);
-    if ((e = cudaMemcpy(a->indptr, indptr_dev, (nrows + 1) * sizeof(int32_t), cudaMemcpyDeviceToDevice)) != cudaSuccess) return bail(e);
-    if (nnz && (e = cudaMemcpy(a->indices, indices_dev, nnz * sizeof(int32_t), cudaMemcpyDeviceToDevice)) != cudaSuccess) return bail(e);
-    if ((e = cudaMemset(a->data, 0, (nnz ? nnz : 1) * sizeof(double))) != cudaSuccess) return bail(e);
+                                const int32_t *indices_dev, CsrPtr &out) {
+    CsrPtr a;
+    if (int rc = csr_new(nrows, ncols, nnz, a)) return rc;
+    CUDA_TRY(cudaMemcpy(a->indptr, indptr_dev, (nrows + 1) * sizeof(int32_t), cudaMemcpyDeviceToDevice));
+    if (nnz) CUDA_TRY(cudaMemcpy(a->indices, indices_dev, nnz * sizeof(int32_t), cudaMemcpyDeviceToDevice));
+    CUDA_TRY(cudaMemset(a->data, 0, (nnz ? nnz : 1) * sizeof(double)));
     // the copies and the memset above ran on the legacy default stream, which does NOT order against the callers'
     // non-blocking streams (the assembly kernels accumulate into `data` right after this returns)
-    if ((e = cudaStreamSynchronize(0)) != cudaSuccess) return bail(e);
-    autotune_tpr(a);
-    *out = a;
+    CUDA_TRY(cudaStreamSynchronize(0));
+    autotune_tpr(a.get());
+    out = std::move(a);
     return PB_OK;
 }
-double *pb_csr_data_(pb_csr *a) { return a->data; }
 
-// an empty matrix of the given sizes (sparse_ops.cu fills indptr / indices / data)
-int pb_csr_alloc_(int64_t nrows, int64_t ncols, int64_t nnz, pb_csr **out) {
-    pb_csr *a = new pb_csr;
-    a->nrows = nrows; a->ncols = ncols; a->nnz = nnz;
-    auto bail = [&](cudaError_t e) {
-        std::string m = cudaGetErrorString(e);
-        pb_csr_destroy(a);
-        return pb_fail_(PB_ECUDA, m);
-    };
-    cudaError_t e;
-    if ((e = cudaStreamCreateWithFlags(&a->stream, cudaStreamNonBlocking)) != cudaSuccess) return bail(e);
-    if ((e = cudaEventCreate(&a->e0)) != cudaSuccess) return bail(e);
-    if ((e = cudaEventCreate(&a->e1)) != cudaSuccess) return bail(e);
-    if ((e = a->alloc()) != cudaSuccess) return bail(e);
-    const double mean = nrows ? (double)nnz / (double)nrows : 0.0;
-    a->tpr = mean <= 3 ? 2 : mean <= 6 ? 4 : mean <= 24 ? 8 : mean <= 48 ? 16 : 32;
-    *out = a;
-    return PB_OK;
-}
-int32_t *pb_csr_indptr_(pb_csr *a) { return a->indptr; }
-int32_t *pb_csr_indices_(pb_csr *a) { return a->indices; }
-struct CsrView { int64_t nrows, ncols, nnz; int32_t *indptr, *indices; double *data; };
+int pb_csr_alloc_(int64_t nrows, int64_t ncols, int64_t nnz, CsrPtr &out) { return csr_new(nrows, ncols, nnz, out); }
+
 CsrView pb_csr_view_(const pb_csr *a) { return CsrView{a->nrows, a->ncols, a->nnz, a->indptr, a->indices, a->data}; }
 
 extern "C" int pb_csr_spmv(pb_csr *a, const double *x, double *y) {
@@ -372,15 +323,15 @@ extern "C" int pb_csr_spmv_bench(pb_csr *a, int reps, float *mean_ms) {
         int rc = launch_spmv(a, a->x, a->y, a->stream);
         if (rc) return rc;
     }
-    CUDA_TRY(cudaEventRecord(a->e0, a->stream));
+    CUDA_TRY(a->timer.mark(0, a->stream));
     for (int i = 0; i < reps; ++i) {
         int rc = launch_spmv(a, a->x, a->y, a->stream);
         if (rc) return rc;
     }
-    CUDA_TRY(cudaEventRecord(a->e1, a->stream));
-    CUDA_TRY(cudaEventSynchronize(a->e1));
+    CUDA_TRY(a->timer.mark(1, a->stream));
+    CUDA_TRY(cudaEventSynchronize(a->timer.ev[1]));
     float ms = 0.f;
-    CUDA_TRY(cudaEventElapsedTime(&ms, a->e0, a->e1));
+    CUDA_TRY(a->timer.ms(&ms));
     *mean_ms = ms / reps;
     return PB_OK;
 }
